@@ -1,4 +1,4 @@
-/* vorbis_b200.h — C ABI of the B200-native per-block DSP path of libvorbis.
+/* vorbis_b200.h — C ABI of the CUDA per-block DSP path of libvorbis.
  *
  * This is the drop-in boundary: plain pointers and sizes, no torch / C++ types.
  * Every entry point names the reference interface it replaces (paths relative

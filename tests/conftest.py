@@ -20,7 +20,7 @@ REF_ARGS = {  # the vorbis_encode_init_vbr arguments each fixture was generated 
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device (an H100)")
 
 
 def bits(a):

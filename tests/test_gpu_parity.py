@@ -63,7 +63,7 @@ def test_transforms_vs_oracle_random(cfg, W):
     assert_bits_equal(ctx.apply_window(W, x, lW, nW), o.apply_window(W, x, lW, nW), "window")
     # empty batch is a no-op
     assert ctx.mdct_forward(W, np.zeros((0, N), np.float32)).shape == (0, N // 2)
-    # more vectors than resident CTAs (148 SMs x 8): every CTA walks several vectors, the next one staged by
+    # more vectors than resident CTAs (132 SMs x 8): every CTA walks several vectors, the next one staged by
     # cp.async while the current one is transformed
     big = rng.uniform(-1, 1, (4000, N)).astype(np.float32)
     assert_bits_equal(ctx.mdct_forward(W, big), o.mdct_forward(W, big), "mdct_forward, 4000 vectors")
@@ -918,24 +918,30 @@ def test_encode_dsp_dev_split_half_batches(cfg, monkeypatch):
 
 
 # ---- whole streams through the batch path (SURVEY §8 a12, a15) -----------------------------------------------
+def streams_signals(ch, rate, q):
+    from test_plan_vs_ref import burst_signal
+    return [probe_signal(ch, rate, 1.2, 11), burst_signal(ch, rate, 0.9, 5), burst_signal(ch, rate, 1.4, 9)]
+
+
 @pytest.mark.parametrize("fmt", ["f32", "s16"])
 def test_encode_streams_mixed_block_sizes(cfg, fmt):
     """vb200_encode_streams: envelope search, block planning (lib/block.c:556-615), both block sizes and the
     ampmax chain across sizes in ONE call.  f32: every block's W/lW/nW/blocktype/position, posts, nonzero and
     quantised residue must equal what the UNMODIFIED reference produced for the same streams through its public
-    API (the timeline is the reference's own v->pcm: pre-extrapolated preamble, input, EOF tail).  s16: the same
-    call on int16 timelines against the oracle's composition."""
-    from oracle import pyref
-    from test_plan_vs_ref import burst_signal
+    API (the timeline is the reference's own v->pcm: pre-extrapolated preamble, input, EOF tail; stored under
+    tests/golden/ref by tests/golden/make_golden_ref.py).  s16: the same call on int16 timelines against the
+    oracle's composition."""
+    import refgold
     name, setup, ctx, o, _, _ = cfg
-    ch, rate, q = REF_ARGS[name]
-    if not pyref.available():
-        pytest.skip("oracle/_ref not built")
-    sigs = [probe_signal(ch, rate, 1.2, 11), burst_signal(ch, rate, 0.9, 5), burst_signal(ch, rate, 1.4, 9)]
+    rec = refgold.load("streams_" + name)
     caps = []
-    for s in sigs:
-        r = pyref.Ref(ch, rate, q)
-        caps.append(r.encode_capture(s, fields=("pcm", "iwork_out"), timeline=True))
+    for i, s in enumerate(streams_signals(*REF_ARGS[name])):
+        p = "s%d_" % i
+        c = {k: rec[p + k] for k in ("W", "lW", "nW", "blocktype", "nonzero_out", "enc_posts", "ampmax_out",
+                                     "d_blocks", "d_iwork_blocks")}
+        c["nblocks"], c["eof"], c["timeline"] = int(rec[p + "nblocks"]), int(rec[p + "eof"]), refgold.timeline(rec, s, p)
+        caps.append(c)
+    ch = setup.channels
     stride = (max(c["timeline"].shape[1] for c in caps) + 3) & ~3
     tl = np.zeros((len(caps), ch, stride), np.float32)
     for i, c in enumerate(caps):
@@ -961,20 +967,21 @@ def test_encode_streams_mixed_block_sizes(cfg, fmt):
         plan = got["plan"][i, :k]
         for nm in ("W", "lW", "nW", "blocktype"):
             assert np.array_equal(plan[nm], want_plan[nm]), "stream %d %s" % (i, nm)
+        if fmt == "f32":
+            blocks = [tl[i][:, p:p + setup.blocksize(int(w))].ravel() for p, w in zip(plan["pos"], plan["W"])]
+            refgold.assert_digest(np.concatenate(blocks), c["d_blocks"], "stream %d block positions" % i)
         for b in range(k):
             W, slot = int(plan[b]["W"]), int(plan[b]["slot"])
             n = setup.blocksize(W) // 2
             nshort += W == 0
             g = got[W]
             if fmt == "f32":
-                P = setup.floor_posts(W, 0)
-                assert np.array_equal(tl[i][:, plan[b]["pos"]:plan[b]["pos"] + 2 * n], c["pcm"][b][:, :2 * n]), "block position"
                 assert np.array_equal(g["nonzero"][slot], c["nonzero_out"][b]), "stream %d block %d nonzero" % (i, b)
                 for cc in range(ch):
                     if c["enc_posts"][b][cc][0] >= 0:
                         Pc = setup.floor_posts(W, setup.floor_of(W, cc))
                         assert np.array_equal(g["posts"][slot][cc][:Pc], c["enc_posts"][b][cc][:Pc]), "stream %d block %d posts" % (i, b)
-                assert np.array_equal(g["iwork"][slot], c["iwork_out"][b][:, :n]), "stream %d block %d residue" % (i, b)
+                refgold.assert_digest(g["iwork"][slot], c["d_iwork_blocks"][b], "stream %d block %d residue" % (i, b))
                 assert g["ampmax_out"][slot] == c["ampmax_out"][b]
             else:
                 w = wouts[b]

@@ -5,7 +5,7 @@ and residue backend write the bits on ONE host thread) against the stock referen
 same streams, same box.  Prints one JSON object; packets are cross-checked by hash.
 
 usage: python tools/dropin_throughput.py [--streams 1000] [--seconds 2.0]
-Needs oracle/_ref/*.so (built where /root/reference exists; the .so files travel to the GPU box)."""
+Needs oracle/_ref/*.so (built by __graft_entry__.build() where the reference sources exist)."""
 import argparse
 import ctypes as C
 import json

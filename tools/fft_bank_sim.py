@@ -5,7 +5,7 @@ vorbis_b200/csrc/vb200_kernels.cuh), to choose a padding of the ping-pong buffer
 Counts wavefronts per (block,channel) row the way the hardware serves a warp request: 32 banks x 4 B; a 32-bit
 request costs max over banks of the number of distinct words; a 64-bit request is served per half-warp, a
 128-bit one per quarter-warp.  Lanes of a warp that take different branches issue separate instructions.
-Compare with profiles/r1_transform_smem_conflicts_by_line.txt (measured: the FFT stores dominate).
+Compare with the shared-memory bank conflicts by source line of a profile of k_phaseA_transform.
 
 usage: tools/fft_bank_sim.py [N] [threads]
 """

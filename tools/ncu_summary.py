@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""profiles/summary.json from one `ncu --set full` report of the chain kernels (one launch each).
+"""A JSON summary (stdout) of one `ncu --set full` report of the chain kernels (one launch each).
 
 usage: tools/ncu_summary.py <report.ncu-rep> <blocks in the captured step> [note]
 Per kernel: DRAM bytes read/written (dram__bytes_{read,write}.sum), rows, duration, executed warp
 instructions per (block,channel) row, IPC, registers, and the algorithmic bytes per row of DESIGN.md §4.
-bench.py scales dram_bytes_per_row into roofline.traffic and warp_instructions_per_row into roofline.issue."""
+"""
 import csv
 import json
 import subprocess
@@ -18,7 +18,7 @@ rows = list(csv.reader(raw.splitlines()))
 hdr, units = rows[0], rows[1]
 ALG = {"k_phaseA_transform": 8 * N, "k_phaseA_psy": 10 * N, "k_floor1_fit": 4 * N, "k_floor1_render": 2 * N, "k_cqn": 6 * N}
 out = {"note": note or ("ncu --set full --clock-control none --import-source on, one un-split step of %d long stereo blocks "
-                        "(%d (block,channel) rows per launch): the step's intermediates (%.1f GB) exceed the 126 MB L2"
+                        "(%d (block,channel) rows per launch): the step's intermediates (%.1f GB) exceed the 50 MB L2"
                         % (blocks, blocks * ch, 30 * N * ch * blocks / 1e9)),
        "blocks": blocks, "kernels": {}}
 

@@ -20,5 +20,6 @@ cyc = ctx.debug_phase_cycles(True)
 rows = nb*ch*R
 names=["load","runs","scatter","chase","grp_min","terms1","scan1","regress1","terms2","scan2","regress2+mix","  chase:records","  chase:simulate","  chase:fill"]
 tot=sum(cyc[:11])
-for n,c in zip(names,cyc): print("%-14s %8.0f cycles/row  %5.1f%%  (%.2f us @1.965GHz)"%(n,c/rows,100*c/tot,c/rows/1965))
-print("total %.0f cycles/row = %.1f us"%(tot/rows, tot/rows/1965))
+ghz=torch.cuda.get_device_properties(0).clock_rate/1e6  # the device's maximum SM clock: times are lower bounds
+for n,c in zip(names,cyc): print("%-14s %8.0f cycles/row  %5.1f%%  (%.2f us @%.3fGHz)"%(n,c/rows,100*c/tot,c/rows/ghz/1e3,ghz))
+print("total %.0f cycles/row = %.1f us"%(tot/rows, tot/rows/ghz/1e3))

@@ -1,6 +1,6 @@
 // vb200.cu — kernels (__global__) and the C ABI of include/vorbis_b200.h.
 //
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -O3 -lineinfo -fmad=false
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -O3 -lineinfo -fmad=false
 //        -Xcompiler -fPIC -shared   (see __graft_entry__.build()).
 // No torch, no oracle/ dependency: this is the product library.
 #include <cuda_runtime.h>
@@ -54,7 +54,7 @@ struct DevBuf {
 
 struct vb200_ctx {
   int device = 0;
-  int sm_count = 148;
+  int sm_count = 132;
   vb200_setup setup;                 // scalar copy (pointers not used after create)
   HostXform hx[2];
   XformDev dx[2];
@@ -1261,7 +1261,7 @@ static int phaseA_psy_launch(vb200_ctx *c, int W, int nblocks, const vb200_phase
       const int total = P0.total > P1.total ? P0.total : P1.total;
       const int nruns = P0.nruns > P1.nruns ? P0.nruns : P1.nruns;
       const int ngrp = P0.ngrp > P1.ngrp ? P0.ngrp : P1.ngrp;
-      int R = 1;                                     // rows per CTA sharing one scan warp (2: fewer instructions, same time)
+      int R = 1;                                     // rows per CTA sharing one scan warp (2: fewer instructions; DESIGN.md §4)
       { const char *e = getenv("VB200_PSY_ROWS"); if (e) R = atoi(e) == 1 ? 1 : 2; }
       const size_t row_bytes = sizeof(float) * ((psy3_floats(n, total, nruns, ngrp) + 3) & ~(size_t)3);
       const size_t smem3 = row_bytes * R;
@@ -1281,7 +1281,7 @@ static int phaseA_psy_launch(vb200_ctx *c, int W, int nblocks, const vb200_phase
         if ((rc = set_smem(k_phaseA_psy4<KK>, row_bytes))) return rc;                              \
         k_phaseA_psy4<KK><<<grid_for(c, rows, PSY3_MINB), PSY3_THREADS, row_bytes, st>>>(P0, P1, ch, rows, A); \
       } while (0)
-      // k_phaseA_psy4 (regressions run behind the scans) is an experiment that measured slower than psy3 (DESIGN.md §4): opt-in
+      // k_phaseA_psy4 (regressions run behind the scans) is an experiment, slower than psy3 (polling, operands from L2; DESIGN.md §4): opt-in
       static const bool psy_v4 = []() { const char *e = getenv("VB200_PSY_V4"); return e && atoi(e); }();
 #define LAUNCH_PSY3(KK) do { if (psy_v4) LAUNCH_PSY4(KK); else if (R == 1) LAUNCH_PSY3R(KK, 1); else LAUNCH_PSY3R(KK, 2); } while (0)
       switch (n / 128) {
@@ -1845,7 +1845,7 @@ extern "C" int vb200_encode_dsp_dev(vb200_ctx *c, int W, int nstreams, int bps, 
   // Two half-batches (whole streams each) on two internal streams, every kernel launched with half its
   // grid: the halves drift apart, so CTAs of different kernels (shared-memory bound transform, issue bound
   // psy, latency bound floor fit) share the SMs instead of one kernel type owning the machine at a time.
-  int split = 2;                      // measured: 19.24 -> 18.88 ms per 100 000 blocks; 4 staggered pieces: no gain
+  int split = 2;                      // H100 80GB HBM3 at a 400 W limit: 1 and 2 within noise (5.45 / 5.47 M blocks/s)
   { const char *e = getenv("VB200_SPLIT"); if (e) split = atoi(e); }
   size_t split_min = 2048;
   { const char *e = getenv("VB200_SPLIT_MIN"); if (e && atoi(e) > 0) split_min = (size_t)atoi(e); }
@@ -2009,7 +2009,7 @@ extern "C" int vb200_encode_dsp(vb200_ctx *c, int W, int nstreams, int bps, int 
   if ((rc = enc_check(c, W, nstreams, bps, blobno, h))) return rc;
   std::lock_guard<std::mutex> lk(c->mu);
   const int ch = c->setup.channels, N = c->dx[W].N, n = N / 2;
-  int chunk_blocks = 8192;                           // measured on B200 (ramped schedule): 2048 -> 5.56, 4096 -> 6.11, 8192 -> 6.16 M blocks/s end to end
+  int chunk_blocks = 8192;                           // H100 80GB HBM3 at a 400 W limit (ramped schedule): 4096 -> 5.34, 8192 -> 5.36, 16384 -> 5.21 M blocks/s end to end
   { const char *e = getenv("VB200_CHUNK_BLOCKS"); if (e && atoi(e) > 0) chunk_blocks = atoi(e); }
   int cs = chunk_blocks / bps;                       // whole streams per chunk
   if (cs < 1) cs = 1;

@@ -1,4 +1,4 @@
-// vb200_kernels.cuh — hand-written sm_100a kernels for the libvorbis per-block
+// vb200_kernels.cuh — hand-written sm_90a kernels for the libvorbis per-block
 // DSP path (window, MDCT, real FFT, log spectra, noise/tone masks, mix).
 //
 // Numerics contract: every output value is produced by the same sequence of

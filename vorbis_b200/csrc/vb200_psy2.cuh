@@ -1,6 +1,6 @@
 // vb200_psy2.cuh — k_phaseA_psy2: the fused noise/tone/mix kernel, occupancy-first layout.
 //
-// Measured on B200 the psy stage is latency bound and its throughput scales with resident
+// The psy stage is latency bound and its throughput scales with resident
 // CTAs, so this version minimises shared memory per (block,channel) row:
 //   * every per-bin value a thread needs twice (logmdct, first-pass noise) stays in
 //     registers: thread t owns bins t, t+128, ... in every per-bin phase;
