@@ -1261,8 +1261,7 @@ static int phaseA_psy_launch(vb200_ctx *c, int W, int nblocks, const vb200_phase
       const int total = P0.total > P1.total ? P0.total : P1.total;
       const int nruns = P0.nruns > P1.nruns ? P0.nruns : P1.nruns;
       const int ngrp = P0.ngrp > P1.ngrp ? P0.ngrp : P1.ngrp;
-      int R = 1;                                     // rows per CTA sharing one scan warp (2: fewer instructions; DESIGN.md §4)
-      { const char *e = getenv("VB200_PSY_ROWS"); if (e) R = atoi(e) == 1 ? 1 : 2; }
+      constexpr int R = 2;                           // rows per CTA sharing one scan warp (DESIGN.md §4)
       const size_t row_bytes = sizeof(float) * ((psy3_floats(n, total, nruns, ngrp) + 3) & ~(size_t)3);
       const size_t smem3 = row_bytes * R;
       int ctas = (int)((227 * 1024) / (smem3 + 1024));
@@ -1270,20 +1269,12 @@ static int phaseA_psy_launch(vb200_ctx *c, int W, int nblocks, const vb200_phase
       if (ctas < 1) ctas = 1;
       { const char *e = getenv("VB200_PSY_CTAS"); if (e) ctas = atoi(e); }
       const bool dbg3 = A.dbg_cycles || A.tap_noise || A.tap_tone;   // clock marks / taps: the debug instance
-#define LAUNCH_PSY3D(KK, RR, DD)                                                                   \
+#define LAUNCH_PSY3D(KK, DD)                                                                       \
       do {                                                                                         \
-        if ((rc = set_smem(k_phaseA_psy3<KK, RR, DD>, smem3))) return rc;                          \
-        k_phaseA_psy3<KK, RR, DD><<<grid_for(c, (rows + RR - 1) / RR, ctas), PSY3_THREADS * RR, smem3, st>>>(P0, P1, ch, rows, A); \
+        if ((rc = set_smem(k_phaseA_psy3<KK, R, DD>, smem3))) return rc;                           \
+        k_phaseA_psy3<KK, R, DD><<<grid_for(c, (rows + R - 1) / R, ctas), PSY3_THREADS * R, smem3, st>>>(P0, P1, ch, rows, A); \
       } while (0)
-#define LAUNCH_PSY3R(KK, RR) do { if (dbg3) LAUNCH_PSY3D(KK, RR, true); else LAUNCH_PSY3D(KK, RR, false); } while (0)
-#define LAUNCH_PSY4(KK)                                                                            \
-      do {                                                                                         \
-        if ((rc = set_smem(k_phaseA_psy4<KK>, row_bytes))) return rc;                              \
-        k_phaseA_psy4<KK><<<grid_for(c, rows, PSY3_MINB), PSY3_THREADS, row_bytes, st>>>(P0, P1, ch, rows, A); \
-      } while (0)
-      // k_phaseA_psy4 (regressions run behind the scans) is an experiment, slower than psy3 (polling, operands from L2; DESIGN.md §4): opt-in
-      static const bool psy_v4 = []() { const char *e = getenv("VB200_PSY_V4"); return e && atoi(e); }();
-#define LAUNCH_PSY3(KK) do { if (psy_v4) LAUNCH_PSY4(KK); else if (R == 1) LAUNCH_PSY3R(KK, 1); else LAUNCH_PSY3R(KK, 2); } while (0)
+#define LAUNCH_PSY3(KK) do { if (dbg3) LAUNCH_PSY3D(KK, true); else LAUNCH_PSY3D(KK, false); } while (0)
       switch (n / 128) {
         case 1: LAUNCH_PSY3(1); break;
         case 2: LAUNCH_PSY3(2); break;
@@ -1291,9 +1282,7 @@ static int phaseA_psy_launch(vb200_ctx *c, int W, int nblocks, const vb200_phase
         case 8: LAUNCH_PSY3(8); break;
         default: LAUNCH_PSY3(16); break;
       }
-#undef LAUNCH_PSY3R
 #undef LAUNCH_PSY3D
-#undef LAUNCH_PSY4
 #undef LAUNCH_PSY3
     } else if (v2ok) {
       const int total = P0.total > P1.total ? P0.total : P1.total;

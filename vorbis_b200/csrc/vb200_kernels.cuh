@@ -121,23 +121,8 @@ __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wai
 // acquire orders the consumer's later loads after the flag read
 __device__ __forceinline__ void sts_release(unsigned a, int v) { asm volatile("st.release.cta.shared.s32 [%0], %1;" :: "r"(a), "r"(v) : "memory"); }
 __device__ __forceinline__ int lds_acquire(unsigned a) { int v; asm volatile("ld.acquire.cta.shared.s32 %0, [%1];" : "=r"(v) : "r"(a) : "memory"); return v; }
-__device__ __forceinline__ int lds_volatile(unsigned a) { int v; asm volatile("ld.volatile.shared.s32 %0, [%1];" : "=r"(v) : "r"(a) : "memory"); return v; }
-__device__ __forceinline__ void fence_cta() { asm volatile("fence.acq_rel.cta;" ::: "memory"); }
 __device__ __forceinline__ void spin_pause(unsigned ns) { __nanosleep(ns); }
 __device__ __forceinline__ void prefetch_l2(const void *p) { asm volatile("prefetch.global.L2 [%0];" :: "l"(p)); }
-// mbarrier with an arrival count of one: every arrive of the producer completes a phase; a consumer that finds the
-// data it needs not yet published parks on the current phase (try_wait suspends the warp in hardware instead of
-// spending issue slots on a poll loop; it is time limited, so the caller re-checks its condition in a loop)
-__device__ __forceinline__ void mbar_init1(unsigned a) { asm volatile("mbarrier.init.shared::cta.b64 [%0], 1;" :: "r"(a) : "memory"); }
-__device__ __forceinline__ void mbar_arrive_release(unsigned a) {
-  // relaxed: a release here is a full memory barrier per publish, which the scan (the critical path) cannot afford;
-  // the data were stored by earlier shared-memory instructions of this same warp, which the shared-memory pipeline
-  // performs in order, and the consumer's try_wait is an acquire
-  asm volatile("{\n\t.reg .b64 st;\n\tmbarrier.arrive.relaxed.cta.shared::cta.b64 st, [%0];\n\t}" :: "r"(a) : "memory");
-}
-__device__ __forceinline__ void mbar_park(unsigned a, unsigned parity) {
-  asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.acquire.cta.shared::cta.b64 p, [%0], %1;\n\t}" :: "r"(a), "r"(parity) : "memory");
-}
 #else   // host emulation build (tools/cuemu, development aid): "shared addresses" are offsets into the CTA's buffer
 __device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)((const unsigned char *)p - cuemu::dyn_smem()); }
 __device__ __forceinline__ float lds_f32(unsigned a) { return *reinterpret_cast<const float *>(cuemu::dyn_smem() + a); }
@@ -152,13 +137,8 @@ __device__ __forceinline__ void sts_s32(unsigned a, int v) { *reinterpret_cast<i
 __device__ __forceinline__ void named_bar_sync(int barid, int nt) { cuemu_named_barrier(barid, nt); }
 __device__ __forceinline__ void sts_release(unsigned a, int v) { __atomic_store_n(reinterpret_cast<int *>(cuemu::dyn_smem() + a), v, __ATOMIC_RELEASE); }
 __device__ __forceinline__ int lds_acquire(unsigned a) { return __atomic_load_n(reinterpret_cast<int *>(cuemu::dyn_smem() + a), __ATOMIC_ACQUIRE); }
-__device__ __forceinline__ int lds_volatile(unsigned a) { return __atomic_load_n(reinterpret_cast<int *>(cuemu::dyn_smem() + a), __ATOMIC_ACQUIRE); }
-__device__ __forceinline__ void fence_cta() { __atomic_thread_fence(__ATOMIC_ACQ_REL); }
 __device__ __forceinline__ void spin_pause(unsigned) { sched_yield(); }
 __device__ __forceinline__ void prefetch_l2(const void *) {}
-__device__ __forceinline__ void mbar_init1(unsigned) {}
-__device__ __forceinline__ void mbar_arrive_release(unsigned) { __atomic_thread_fence(__ATOMIC_RELEASE); }
-__device__ __forceinline__ void mbar_park(unsigned, unsigned) { sched_yield(); }
 __device__ __forceinline__ void cp_async16(unsigned dst, const void *src) { memcpy(cuemu::dyn_smem() + dst, src, 16); }
 __device__ __forceinline__ void cp_async_commit() {}
 __device__ __forceinline__ void cp_async_wait_all() {}

@@ -374,15 +374,17 @@ k_phaseA_psy3(PsyDev P0, PsyDev P1, int ch, int nrows, PhaseA2Args A) {
   float *grp_min = sm + area;
   int *s_misc = reinterpret_cast<int *>(grp_min + ((ngrp + 1 + 3) & ~3));
   for (int row0 = blockIdx.x * R; row0 < nrows; row0 += gridDim.x * R) {
-    // an odd tail: the spare half repeats the last row (identical values to identical addresses)
-    const int row = row0 + half < nrows ? row0 + half : nrows - 1;
+    // an odd tail: the spare half repeats the last row in lockstep but stores none of the mix (the mix re-reads the
+    // raw MDCT, which the other half may already have overwritten: mdct_out may alias mdct_in)
+    const bool spare = row0 + half >= nrows;
+    const int row = spare ? nrows - 1 : row0 + half;
     const int blk = row / ch;
     const PsyDev &P = A.desc[blk].blocktype ? P1 : P0;
     const float *gm = A.mdct_in + (size_t)row * n;
     const float *lf = A.logfft + (size_t)row * n;
     const float g = A.gmax[blk], lmax = A.lmax[row];
     const float att = tone_att(P, lmax);
-    float L[K], M[K], p1[K];
+    float L[K], p1[K];                                // the raw MDCT is read again by the mix: holding it here spilled
     long long tmark = (DBG && A.dbg_cycles) ? clock64() : 0;
     int tph = 0;
 #define PHASE_MARK()                                                              \
@@ -397,12 +399,12 @@ k_phaseA_psy3(PsyDev P0, PsyDev P1, int ch, int nrows, PhaseA2Args A) {
 #pragma unroll
     for (int k = 0; k < K; k++) {
       const int i = tid + k * nt;
-      M[k] = __ldcs(gm + i);                            // streaming: keep L1 for the lookup tables
+      L[k] = __ldcg(gm + i);                            // L2 only: keep L1 for the lookup tables
       s_fft[i] = __ldcs(lf + i);
     }
 #pragma unroll
     for (int k = 0; k < K; k++) {
-      L[k] = add345(todB_dev(M[k]));                    // lib/mapping0.c:384-385
+      L[k] = add345(todB_dev(L[k]));                    // lib/mapping0.c:384-385
       __stcs(A.logmdct + (size_t)row * n + tid + k * nt, L[k]);
     }
 #ifndef VB200_NO_PREFETCH
@@ -517,10 +519,10 @@ k_phaseA_psy3(PsyDev P0, PsyDev P1, int ch, int nrows, PhaseA2Args A) {
     const float *athp = P.ath, *compand = P.noisecompand;
     const short *bin_grp = P.bin_grp;
 #pragma unroll
-    for (int k = 0; k < K; k++) {
+    for (int k = 0; k < K && !spare; k++) {
       const int i = tid + k * nt;
       const MixOut o = final_mix_val(p2[k], L[k], p1[k], __ldg(noff + i), __ldg(athp + i),
-                                     grp_min[__ldg(bin_grp + i)], compand, MC, M[k]);
+                                     grp_min[__ldg(bin_grp + i)], compand, MC, __ldcs(gm + i));
       __stcs(A.logmask + (size_t)row * n + i, o.logmask);
       __stcs(A.mdct_out + (size_t)row * n + i, o.m);
       if (DBG && A.tap_noise) A.tap_noise[(size_t)row * n + i] = o.nz;
@@ -529,259 +531,6 @@ k_phaseA_psy3(PsyDev P0, PsyDev P1, int ch, int nrows, PhaseA2Args A) {
     if (tid == 0 && (row % ch) == 0) A.ampmax_out[blk] = g;   // lib/mapping0.c:576
     __syncthreads();
     PHASE_MARK();   // 10 regress 2 + final + mix
-#undef PHASE_MARK
-  }
-}
-
-// =====================================================================================================
-// k_phaseA_psy4: psy3 with the noise half re-scheduled so that no warp waits behind the sequential scans.
-//
-// In psy3 a row's two prefix-sum scans (5 lanes of one warp, 1024 dependent FADDs each) kept the other three
-// warps at the barrier for ~26 % of the row's time.  A bin's windowed regression only needs the prefix sums up
-// to the upper end of its window, and the scan produces them in increasing order - so here the scan warp
-// PUBLISHES its progress (a release store to shared memory after every 32 elements) and the other warps run the
-// regressions behind it: 32-bin chunks are handed out in increasing order from a shared counter, a warp waits
-// (acquire load, nanosleep) only until the scan has passed the highest index its chunk reads, and the scan warp
-// joins the chunk loop when it is done.  Chunks are dynamic, so the per-bin values a chunk needs come from
-// memory instead of registers: logmdct is re-read from the row's output (written in phase 0), the first-pass
-// mask p1 travels through the row's logmask output (overwritten with the real mask at the end), the raw MDCT
-// value is re-read from its input - all L2 hits.  The regressions are inlined in a rolled loop: no per-bin
-// calls, 24 long-lived registers fewer.  Arithmetic per value is unchanged => bit-identical.
-// =====================================================================================================
-__device__ __forceinline__ void dev_noise_scan4(int n, float *S, int ns, int lane, unsigned a_prog, unsigned a_bar) {
-  float4 *a = reinterpret_cast<float4 *>(S + (lane < 5 ? lane : 0) * ns);
-  const int q = n >> 2;
-  const bool act = lane < 5;
-  float t = 0.f;
-  float4 v0, v1, v2, v3, w0, w1, w2, w3;
-  if (act) { v0 = a[0]; v1 = a[1]; v2 = a[2]; v3 = a[3]; }
-#define SCAN4(v) do { t += v.x; v.x = t; t += v.y; v.y = t; t += v.z; v.z = t; t += v.w; v.w = t; } while (0)
-  for (int i = 0; i < q; i += 8) {
-    if (act) {
-      w0 = a[i + 4]; w1 = a[i + 5]; w2 = a[i + 6]; w3 = a[i + 7];
-      SCAN4(v0); SCAN4(v1); SCAN4(v2); SCAN4(v3);
-      a[i] = v0; a[i + 1] = v1; a[i + 2] = v2; a[i + 3] = v3;
-      if (i + 8 < q) { v0 = a[i + 8]; v1 = a[i + 9]; v2 = a[i + 10]; v3 = a[i + 11]; }
-      SCAN4(w0); SCAN4(w1); SCAN4(w2); SCAN4(w3);
-      a[i + 4] = w0; a[i + 5] = w1; a[i + 6] = w2; a[i + 7] = w3;
-    }
-    if ((i & 8) || i + 8 >= q) {                             // publish every 64 elements (and at the end)
-      __syncwarp();
-      if (lane == 0) { sts_s32(a_prog, (i + 8) * 4); mbar_arrive_release(a_bar); }   // elements [0, 4(i+8)) of all five sums are final
-    }
-  }
-#undef SCAN4
-}
-
-// wait until the scan has published `need` elements.  Publishes come every 64 elements, one mbarrier phase each;
-// `phase0` = phases the barrier had completed when this row's scan started.
-__device__ __forceinline__ void wait_progress(unsigned a_prog, unsigned a_bar, int need, int n, unsigned phase0) {
-  need = __reduce_max_sync(0xffffffffu, need);
-  if (need > n) need = n;                            // the scan ends at n
-  // bounded: the producer cannot stall (it waits for nothing), the cap only keeps a broken build from hanging the GPU
-  for (int spins = 0; spins < (1 << 16); spins++) {
-    const int p = lds_volatile(a_prog);
-    if (p >= need) break;
-    mbar_park(a_bar, (phase0 + ((unsigned)p >> 6)) & 1u);   // sleep until the publish after `p` (or the time limit)
-  }
-  fence_cta();                                       // the prefix sums read below are ordered after the flag
-}
-
-// inline form of final_mix_val (same arithmetic)
-__device__ __forceinline__ void dev_final_mix(float p2, float L, float p1, float noff, float ath, float gmin,
-                                              const float *__restrict__ compand, const MixConst &C, float m,
-                                              float &logmask, float &m_out, float &nz_out, float &tn_out) {
-  const float work = L - p1;                       // lib/psy.c:717
-  const float base = L - work;                     // lib/psy.c:722
-  int dB = (int)((double)p2 + .5);
-  if (dB >= VB200_COMPAND_LEVELS) dB = VB200_COMPAND_LEVELS - 1;
-  if (dB < 0) dB = 0;
-  const float nz = base + __ldg(compand + dB);
-  float tn = ath + C.att;                          // lib/psy.c:771, then max_seeds' flr update
-  if (tn < gmin) tn = gmin;
-  nz_out = nz; tn_out = tn;
-  float val = nz + noff;                           // lib/psy.c:789-791
-  if (val > C.noisemaxsupp) val = C.noisemaxsupp;
-  const float t = tn + C.toneatt;
-  logmask = val < t ? t : val;
-  const float coeffi = -17.2f;
-  float de;
-  val = val - L;
-  if (val > coeffi) {
-    de = (float)(1.0 - ((double)(val - coeffi) * 0.005 * (double)C.m_val));
-    if (de < 0.f) de = 0.0001f;
-  } else {
-    de = (float)(1.0 - ((double)(val - coeffi) * 0.0003 * (double)C.m_val));
-  }
-  m_out = m * de;
-}
-
-template <int K>   // K = n / 128 bins per thread in the phases that keep the static bin mapping
-__global__ void __launch_bounds__(PSY3_THREADS, PSY3_MINB)
-k_phaseA_psy4(PsyDev P0, PsyDev P1, int ch, int nrows, PhaseA2Args A) {
-  extern __shared__ __align__(16) float sm[];
-  constexpr int nt = PSY3_THREADS;
-  constexpr int NS = K * PSY3_THREADS + 4;
-  const int n = K * nt, ns = n + 4, tid = threadIdx.x, lane = tid & 31;
-  const int total = P0.total > P1.total ? P0.total : P1.total;
-  const int nruns = P0.nruns > P1.nruns ? P0.nruns : P1.nruns;
-  const int ngrp = P0.ngrp > P1.ngrp ? P0.ngrp : P1.ngrp;
-  const int tp = (total + 7) & ~7;
-  float *S = sm;
-  float *s_fft = sm;
-  float *copies = sm;
-  size_t a0 = 4 * (size_t)tp; if (a0 < (size_t)n) a0 = n;
-  int4 *run_rec = reinterpret_cast<int4 *>(sm + a0);
-  const size_t area = psy3_floats(n, total, nruns, ngrp) - (size_t)((ngrp + 1 + 3) & ~3) - 16;
-  float *grp_min = sm + area;
-  int *s_misc = reinterpret_cast<int *>(grp_min + ((ngrp + 1 + 3) & ~3));
-  // s_misc[8]: scan-1 progress, [9]: pass-1 chunk counter, [10]: scan-2 progress, [11]: pass-2 chunk counter
-  const unsigned a_prog1 = smem_u32(s_misc + 8), a_prog2 = smem_u32(s_misc + 10);
-  // s_misc[12..13], [14..15]: one mbarrier (arrival count 1) per scan; they live for the whole kernel, every row's scan
-  // adds n/64 phases, so the phase count at the start of a row's scan is (rows done) * n/64
-  const unsigned a_bar1 = smem_u32(s_misc + 12), a_bar2 = smem_u32(s_misc + 14);
-  if (tid == 0) { mbar_init1(a_bar1); mbar_init1(a_bar2); }
-  __syncthreads();
-  unsigned phase0 = 0;
-  for (int row = blockIdx.x; row < nrows; row += gridDim.x, phase0 += (unsigned)(n >> 6)) {
-    const int blk = row / ch;
-    const PsyDev &P = A.desc[blk].blocktype ? P1 : P0;
-    const float *gm = A.mdct_in + (size_t)row * n;
-    const float *lf = A.logfft + (size_t)row * n;
-    float *g_logmdct = A.logmdct + (size_t)row * n;
-    float *g_logmask = A.logmask + (size_t)row * n;     // doubles as the carrier of the first-pass mask p1
-    const float g = A.gmax[blk], lmax = A.lmax[row];
-    const float att = tone_att(P, lmax);
-    long long tmark = A.dbg_cycles ? clock64() : 0;
-    int tph = 0;
-#define PHASE_MARK()                                                              \
-    do {                                                                          \
-      if (A.dbg_cycles && tid == 0) {                                             \
-        const long long tnow = clock64();                                         \
-        atomicAdd(A.dbg_cycles + tph, (unsigned long long)(tnow - tmark));        \
-        tmark = tnow;                                                             \
-      }                                                                           \
-      tph++;                                                                      \
-    } while (0)
-    if (tid < 4) s_misc[8 + tid] = 0;
-#pragma unroll
-    for (int k = 0; k < K; k++) {
-      const int i = tid + k * nt;
-      s_fft[i] = __ldcs(lf + i);
-      __stcg(g_logmdct + i, add345(todB_dev(__ldcg(gm + i))));   // lib/mapping0.c:384-385; read back below: keep it in L2
-    }
-    __syncthreads();
-    PHASE_MARK();   // 0 load
-    dev_tone_runs3(P, s_fft, g, att, run_rec, tid);
-    __syncthreads();
-    PHASE_MARK();   // 1 runs
-    dev_tone_scatter3(P, copies, tp, run_rec, tid);
-    __syncthreads();
-    PHASE_MARK();   // 2 scatter
-    dev_chase3<true>(P, copies, tp, s_misc, tid, A.dbg_cycles);
-    PHASE_MARK();   // 3 chase
-    const float *seed = copies;
-    for (int q = tid; q <= P.ngrp; q += nt) {           // max_seeds gather, one minimum per static group (lib/psy.c:522-533)
-      float minV;
-      if (q < P.ngrp) {
-        const int4 gg = __ldg(P.grps + q);
-        if (gg.y - gg.x > 16) continue;                // long fold: done by a whole warp below
-        int pos = gg.x;
-        minV = seed[pos];
-        if (minV > P.tone_abs_limit) minV = P.tone_abs_limit;
-        while (pos < gg.y) {
-          pos++;
-          const float s = seed[pos];
-          if ((s > VB_NEGINF && s < minV) || minV == VB_NEGINF) minV = s;
-        }
-      } else {
-        minV = seed[P.total - 1];                      // tail bins (lib/psy.c:540-544)
-      }
-      grp_min[q] = minV;
-    }
-    for (int li = tid >> 5; li < P.nlong; li += nt >> 5) {   // long groups: associative fold by warp shuffles (see psy3)
-      const int q = __ldg(P.long_grp + li);
-      const int4 gg = __ldg(P.grps + q);
-      float mn = 3.0e38f;
-      int any = 0;
-      for (int pos = gg.x + lane; pos <= gg.y; pos += 32) {
-        const float s = seed[pos];
-        if (s > VB_NEGINF) {
-          any = 1;
-          if (s < mn) mn = s;
-          if (pos == gg.x && P.tone_abs_limit < mn) mn = P.tone_abs_limit;
-        }
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        mn = fminf(mn, __shfl_xor_sync(0xffffffffu, mn, o));
-        any |= __shfl_xor_sync(0xffffffffu, any, o);
-      }
-      if (lane == 0) grp_min[q] = any ? mn : VB_NEGINF;
-    }
-    __syncthreads();                                   // tone scratch is dead from here on
-    PHASE_MARK();   // 4 group minima
-    const int *bark = P.bark;
-    const int bfe = P.bark_first_extra, ffe = P.fixed_first_extra, fixedw = P.noisewindowfixed;
-    const int nchunks = n >> 5;
-    // ---- noise mask, pass 1 (offset 140, bark windows)
-#pragma unroll
-    for (int k = 0; k < K; k++) dev_noise_term1(tid + k * nt, __ldcg(g_logmdct + tid + k * nt), 140.f, S, ns);   // own writes of phase 0
-    __syncthreads();
-    PHASE_MARK();   // 5 terms 1
-    if (tid < 32) dev_noise_scan4(n, S, ns, lane, a_prog1, a_bar1);
-    for (;;) {                                         // regressions behind the scan, 32 bins per chunk
-      int c = 0;
-      if (lane == 0) c = atomicAdd(s_misc + 9, 1);
-      c = __shfl_sync(0xffffffffu, c, 0);
-      if (c >= nchunks) break;
-      const int i = c * 32 + lane;
-      int need = 0;
-      if (bfe > 0) { const int bk = __ldg(bark + (i < bfe ? i : bfe - 1)); need = (bk & 0xffff) + 1; }
-      wait_progress(a_prog1, a_bar1, need, n, phase0);
-      __stcg(g_logmask + i, dev_regress_bin<NS>(bark, bfe, ffe, S, i, 140.f, -1));
-    }
-    __syncthreads();
-    PHASE_MARK();   // 6 scan 1 || regress 1
-    PHASE_MARK();   // 7 (merged into 6)
-    // ---- pass 2 on logmdct - p1 (offset 0, bark + fixed windows)
-#pragma unroll
-    for (int k = 0; k < K; k++)
-      dev_noise_term1(tid + k * nt, __ldcg(g_logmdct + tid + k * nt) - __ldcg(g_logmask + tid + k * nt), 0.f, S, ns);
-    __syncthreads();
-    PHASE_MARK();   // 8 terms 2
-    MixConst MC;
-    MC.noisemaxsupp = P.noisemaxsupp; MC.toneatt = P.tone_masteratt[1]; MC.m_val = P.m_val;
-    MC.att = att;
-    const float *noff = P.noiseoffset + n;             // offset_select 1
-    const float *athp = P.ath, *compand = P.noisecompand;
-    const short *bin_grp = P.bin_grp;
-    if (tid < 32) dev_noise_scan4(n, S, ns, lane, a_prog2, a_bar2);
-    for (;;) {
-      int c = 0;
-      if (lane == 0) c = atomicAdd(s_misc + 11, 1);
-      c = __shfl_sync(0xffffffffu, c, 0);
-      if (c >= nchunks) break;
-      const int i = c * 32 + lane;
-      int need = 0;
-      if (bfe > 0) { const int bk = __ldg(bark + (i < bfe ? i : bfe - 1)); need = (bk & 0xffff) + 1; }
-      if (fixedw > 0 && ffe > 0) { const int h2 = (i < ffe ? i : ffe - 1) + fixedw / 2 + 1; need = h2 > need ? h2 : need; }
-      // the operands of the mix do not depend on the scan: issue their loads before waiting
-      const float Lv = __ldcg(g_logmdct + i), p1v = __ldcg(g_logmask + i), mv = __ldcg(gm + i);
-      const float nf = __ldg(noff + i), at = __ldg(athp + i), gmn = grp_min[__ldg(bin_grp + i)];
-      wait_progress(a_prog2, a_bar2, need, n, phase0);
-      const float p2 = dev_regress_bin<NS>(bark, bfe, ffe, S, i, 0.f, fixedw);
-      float lm, mo, nz, tn;
-      dev_final_mix(p2, Lv, p1v, nf, at, gmn, compand, MC, mv, lm, mo, nz, tn);
-      __stcs(g_logmask + i, lm);
-      __stcs(A.mdct_out + (size_t)row * n + i, mo);
-      if (A.tap_noise) A.tap_noise[(size_t)row * n + i] = nz;
-      if (A.tap_tone) A.tap_tone[(size_t)row * n + i] = tn;
-    }
-    if (tid == 0 && (row % ch) == 0) A.ampmax_out[blk] = g;   // lib/mapping0.c:576
-    __syncthreads();
-    PHASE_MARK();   // 9 scan 2 || regress 2 + final + mix
-    PHASE_MARK();   // 10 (merged into 9)
 #undef PHASE_MARK
   }
 }
