@@ -18,7 +18,6 @@
 #include "vb200_tables.h"
 #include "vb200_kernels.cuh"
 #include "vb200_cqn.cuh"
-#include "vb200_psy2.cuh"
 #include "vb200_psy3.cuh"
 #include "vb200_floor1.cuh"
 #include "vb200_env.cuh"
@@ -440,7 +439,7 @@ extern "C" int vb200_set_profiling(vb200_ctx *c, int on) {
   return 0;
 }
 
-// dev aid: per-phase cycle sums of k_phaseA_psy2 accumulated while VB200_PHASE_TIMING is set
+// dev aid: per-phase cycle sums of k_phaseA_psy3 (its DBG instance) accumulated while VB200_PHASE_TIMING is set
 extern "C" int vb200_debug_phase_cycles(vb200_ctx *c, unsigned long long *out16, int reset) {
   if (!c || !out16) return fail(VB200_EINVAL, "null argument");
   CU(cudaSetDevice(c->device));
@@ -757,7 +756,7 @@ __device__ __forceinline__ PsySmem psy_carve(float *sm, int n, int total, int nr
 
 #define PSY_THREADS 128
 __global__ void __launch_bounds__(PSY_THREADS)
-k_phaseA_psy(PsyDev P0, PsyDev P1, int ch, int nrows, PhaseA2Args A) {
+k_phaseA_psy(PsyDev P0, PsyDev P1, int ch, int nrows, PsyArgs A) {
   extern __shared__ __align__(16) float sm[];
   const int n = P0.n, ns = n + 4, tid = threadIdx.x, nt = PSY_THREADS;
   const int total = P0.total > P1.total ? P0.total : P1.total;
@@ -781,12 +780,12 @@ k_phaseA_psy(PsyDev P0, PsyDev P1, int ch, int nrows, PhaseA2Args A) {
     dev_tone_runs(P, S.fft, g, lmax, S.T, tid, nt);
     dev_noise_terms(n, S.logmdct, nullptr, 140.f, S.scan, ns, tid, nt);
     __syncthreads();
-    if (!(A.dbg_skip & 4)) dev_tone_slots(P, S.T, tid, nt);
+    dev_tone_slots(P, S.T, tid, nt);
     __syncthreads();
     // warp 0: the sequential seed_chase + gather; warps 1-3: the noise mask (two sequential
     // prefix-sum passes on five lanes + regressions).  The two chains are independent.
-    if (warp == 0) { if (!(A.dbg_skip & 1)) dev_tone_chase_gather(P, S.fft, lmax, S.T, lane); }
-    else if (!(A.dbg_skip & 2)) dev_noisemask(P, S.logmdct, S.noise, S.scan, ns, tid - 32, nt - 32, 1, true);
+    if (warp == 0) dev_tone_chase_gather(P, S.fft, lmax, S.T, lane);
+    else dev_noisemask(P, S.logmdct, S.noise, S.scan, ns, tid - 32, nt - 32, 1, true);
     __syncthreads();
     const float *noff = P.noiseoffset + n;               // offset_select 1
     for (int i = tid; i < n; i += nt) {
@@ -1112,7 +1111,7 @@ extern "C" int vb200_drft_forward(vb200_ctx *c, int W, int nvec, float *data) {
 
 // ======================================================================== //
 // stage-isolated psy entry points
-static size_t psy2_smem(const PsyDev &a, const PsyDev &b) {
+static size_t psy_smem_bytes(const PsyDev &a, const PsyDev &b) {
   const int total = a.total > b.total ? a.total : b.total;
   const int nruns = a.nruns > b.nruns ? a.nruns : b.nruns;
   return sizeof(float) * psy_smem_floats(a.n, total, nruns);
@@ -1130,7 +1129,7 @@ extern "C" int vb200_noisemask(vb200_ctx *c, int look, int nvec, const float *lo
   const size_t bytes = sizeof(float) * (size_t)nvec * P.n;
   if ((rc = io.h2d(logmdct, bytes, &di))) return rc;
   if ((rc = io.h2d(nullptr, bytes, &dout))) return rc;
-  const size_t smem = psy2_smem(P, P);
+  const size_t smem = psy_smem_bytes(P, P);
   if ((rc = set_smem(k_noisemask, smem))) return rc;
   k_noisemask<<<grid_for(c, nvec, 4), PSY_THREADS, smem, c->s_main>>>(P, nvec, (const float *)di, (float *)dout);
   if ((rc = post_launch(c))) return rc;
@@ -1151,7 +1150,7 @@ extern "C" int vb200_tonemask(vb200_ctx *c, int look, int nvec, const float *log
   if ((rc = io.h2d(gmax, sizeof(float) * nvec, &dg))) return rc;
   if ((rc = io.h2d(lmax, sizeof(float) * nvec, &dl))) return rc;
   if ((rc = io.h2d(nullptr, bytes, &dout))) return rc;
-  const size_t smem = psy2_smem(P, P);
+  const size_t smem = psy_smem_bytes(P, P);
   if ((rc = set_smem(k_tonemask, smem))) return rc;
   k_tonemask<<<grid_for(c, nvec, 4), PSY_THREADS, smem, c->s_main>>>(P, nvec, (const float *)di, (const float *)dg,
                                                              (const float *)dl, (float *)dout);
@@ -1218,100 +1217,68 @@ static int phaseA_transform_launch(vb200_ctx *c, int W, int nblocks, const vb200
 // stage 3: noise / tone masks + mix of `nblocks` blocks of size W, given every block's global ampmax
 static int phaseA_psy_launch(vb200_ctx *c, int W, int nblocks, const vb200_phaseA_io *io, cudaStream_t st,
                              float *d_logfft, float *d_lmax, float *d_gmax) {
-  const XformDev &X = c->dx[W];
-  const int ch = c->setup.channels, N = X.N;
+  const int ch = c->setup.channels, n = c->dx[W].N / 2;
   const int rows = nblocks * ch;
-  int rc;
+  const PsyDev &P0 = c->dpsy[2 * W], &P1 = c->dpsy[2 * W + 1];
+  const int total = P0.total > P1.total ? P0.total : P1.total;
+  const int nruns = P0.nruns > P1.nruns ? P0.nruns : P1.nruns;
+  const int ngrp = P0.ngrp > P1.ngrp ? P0.ngrp : P1.ngrp;
+  const char *ectas = getenv("VB200_PSY_CTAS");
+  const size_t smem = psy_smem_bytes(P0, P1);
+  int rc = set_smem(k_phaseA_psy, smem); if (rc) return rc;
   {
-    const PsyDev &P0 = c->dpsy[2 * W], &P1 = c->dpsy[2 * W + 1];
-    const size_t smem = psy2_smem(P0, P1);
-    int rc = set_smem(k_phaseA_psy, smem); if (rc) return rc;
-    {
-      // leave the rest of the 256 KB unified array to L1: the static psy tables (~60 KB per look)
-      // are read through it on every row
-      int &tuned = c->psy_carveout_ctas;
-      const char *e = getenv("VB200_PSY_CTAS");
-      const int ctas = e ? atoi(e) : c->psy_ctas_per_sm;
-      if (tuned != ctas) {
-        int pct = (int)((ctas * (smem + 1024) * 100 + 228 * 1024 - 1) / (228 * 1024));
-        if (pct > 100) pct = 100;
-        CU(cudaFuncSetAttribute(k_phaseA_psy, cudaFuncAttributePreferredSharedMemoryCarveout, pct));
-        tuned = ctas;
-      }
-      c->psy_ctas_per_sm = ctas;
+    // leave the rest of the 256 KB unified array to L1: the static psy tables (~60 KB per look)
+    // are read through it on every row
+    int &tuned = c->psy_carveout_ctas;
+    const int ctas = ectas ? atoi(ectas) : c->psy_ctas_per_sm;
+    if (tuned != ctas) {
+      int pct = (int)((ctas * (smem + 1024) * 100 + 228 * 1024 - 1) / (228 * 1024));
+      if (pct > 100) pct = 100;
+      CU(cudaFuncSetAttribute(k_phaseA_psy, cudaFuncAttributePreferredSharedMemoryCarveout, pct));
+      tuned = ctas;
     }
-    PhaseA2Args A;
-    A.mdct_in = io->tap_mdct_raw ? io->tap_mdct_raw : io->mdct;
-    A.logfft = d_logfft; A.lmax = d_lmax; A.gmax = d_gmax; A.desc = io->desc;
-    A.mdct_out = io->mdct; A.logmdct = io->logmdct; A.logmask = io->logmask; A.ampmax_out = io->ampmax_out;
-    A.tap_noise = io->tap_noise; A.tap_tone = io->tap_tone;
-    { const char *e = getenv("VB200_DEBUG_SKIP"); A.dbg_skip = e ? atoi(e) : 0; }
-    A.dbg_cycles = nullptr;
-    if (getenv("VB200_PHASE_TIMING")) {
-      void *p; if ((rc = ensure(c, 10, 16 * sizeof(unsigned long long), &p))) return rc;
-      A.dbg_cycles = (unsigned long long *)p;
-    }
-    const int n = N / 2;
-    const char *ev = getenv("VB200_PSY_V1");
-    const bool v2ok = !(ev && atoi(ev)) && (n == 128 || n == 256 || n == 512 || n == 1024 || n == 2048);
-    const char *ev2 = getenv("VB200_PSY_V2");
-    const bool v3ok = v2ok && !(ev2 && atoi(ev2)) && P0.linesper == P1.linesper &&
-                      psy3_supported(n, P0.total > P1.total ? P0.total : P1.total, P0.linesper);
-    if (v3ok) {
-      const int total = P0.total > P1.total ? P0.total : P1.total;
-      const int nruns = P0.nruns > P1.nruns ? P0.nruns : P1.nruns;
-      const int ngrp = P0.ngrp > P1.ngrp ? P0.ngrp : P1.ngrp;
-      constexpr int R = 2;                           // rows per CTA sharing one scan warp (DESIGN.md §4)
-      const size_t row_bytes = sizeof(float) * ((psy3_floats(n, total, nruns, ngrp) + 3) & ~(size_t)3);
-      const size_t smem3 = row_bytes * R;
-      int ctas = (int)((227 * 1024) / (smem3 + 1024));
-      if (ctas > PSY3_MINB / R) ctas = PSY3_MINB / R;
-      if (ctas < 1) ctas = 1;
-      { const char *e = getenv("VB200_PSY_CTAS"); if (e) ctas = atoi(e); }
-      const bool dbg3 = A.dbg_cycles || A.tap_noise || A.tap_tone;   // clock marks / taps: the debug instance
+    c->psy_ctas_per_sm = ctas;
+  }
+  PsyArgs A;
+  A.mdct_in = io->tap_mdct_raw ? io->tap_mdct_raw : io->mdct;
+  A.logfft = d_logfft; A.lmax = d_lmax; A.gmax = d_gmax; A.desc = io->desc;
+  A.mdct_out = io->mdct; A.logmdct = io->logmdct; A.logmask = io->logmask; A.ampmax_out = io->ampmax_out;
+  A.tap_noise = io->tap_noise; A.tap_tone = io->tap_tone;
+  A.dbg_cycles = nullptr;
+  if (getenv("VB200_PHASE_TIMING")) {
+    void *p; if ((rc = ensure(c, 10, 16 * sizeof(unsigned long long), &p))) return rc;
+    A.dbg_cycles = (unsigned long long *)p;
+  }
+  // VB200_PSY_V1=1 forces the generic kernel, so that the tests can check it on the setups the fast one takes
+  const char *ev1 = getenv("VB200_PSY_V1");
+  if (!(ev1 && atoi(ev1)) && P0.linesper == P1.linesper && psy3_supported(n, total, P0.linesper)) {
+    constexpr int R = 2;                             // rows per CTA sharing one scan warp (DESIGN.md §4)
+    const size_t row_bytes = sizeof(float) * ((psy3_floats(n, total, nruns, ngrp) + 3) & ~(size_t)3);
+    const size_t smem3 = row_bytes * R;
+    int ctas = (int)((227 * 1024) / (smem3 + 1024));
+    if (ctas > PSY3_MINB / R) ctas = PSY3_MINB / R;
+    if (ctas < 1) ctas = 1;
+    if (ectas) ctas = atoi(ectas);
+    const bool dbg3 = A.dbg_cycles || A.tap_noise || A.tap_tone;   // clock marks / taps: the debug instance
 #define LAUNCH_PSY3D(KK, DD)                                                                       \
-      do {                                                                                         \
-        if ((rc = set_smem(k_phaseA_psy3<KK, R, DD>, smem3))) return rc;                           \
-        k_phaseA_psy3<KK, R, DD><<<grid_for(c, (rows + R - 1) / R, ctas), PSY3_THREADS * R, smem3, st>>>(P0, P1, ch, rows, A); \
-      } while (0)
+    do {                                                                                           \
+      if ((rc = set_smem(k_phaseA_psy3<KK, R, DD>, smem3))) return rc;                             \
+      k_phaseA_psy3<KK, R, DD><<<grid_for(c, (rows + R - 1) / R, ctas), PSY3_THREADS * R, smem3, st>>>(P0, P1, ch, rows, A); \
+    } while (0)
 #define LAUNCH_PSY3(KK) do { if (dbg3) LAUNCH_PSY3D(KK, true); else LAUNCH_PSY3D(KK, false); } while (0)
-      switch (n / 128) {
-        case 1: LAUNCH_PSY3(1); break;
-        case 2: LAUNCH_PSY3(2); break;
-        case 4: LAUNCH_PSY3(4); break;
-        case 8: LAUNCH_PSY3(8); break;
-        default: LAUNCH_PSY3(16); break;
-      }
+    switch (n / 128) {
+      case 1: LAUNCH_PSY3(1); break;
+      case 2: LAUNCH_PSY3(2); break;
+      case 4: LAUNCH_PSY3(4); break;
+      case 8: LAUNCH_PSY3(8); break;
+      default: LAUNCH_PSY3(16); break;
+    }
 #undef LAUNCH_PSY3D
 #undef LAUNCH_PSY3
-    } else if (v2ok) {
-      const int total = P0.total > P1.total ? P0.total : P1.total;
-      const int nruns = P0.nruns > P1.nruns ? P0.nruns : P1.nruns;
-      const int ngrp = P0.ngrp > P1.ngrp ? P0.ngrp : P1.ngrp;
-      const size_t smem2 = sizeof(float) * psy2_floats(n, total, nruns, ngrp);
-      int ctas = (int)((227 * 1024) / (smem2 + 1024));
-      if (ctas > PSY2_MINB) ctas = PSY2_MINB;
-      if (ctas < 1) ctas = 1;
-      { const char *e = getenv("VB200_PSY_CTAS"); if (e) ctas = atoi(e); }
-#define LAUNCH_PSY2(KK)                                                                            \
-      do {                                                                                         \
-        if ((rc = set_smem(k_phaseA_psy2<KK>, smem2))) return rc;                                  \
-        k_phaseA_psy2<KK><<<grid_for(c, rows, ctas), PSY2_THREADS, smem2, st>>>(P0, P1, ch, rows, A); \
-      } while (0)
-      switch (n / 128) {
-        case 1: LAUNCH_PSY2(1); break;
-        case 2: LAUNCH_PSY2(2); break;
-        case 4: LAUNCH_PSY2(4); break;
-        case 8: LAUNCH_PSY2(8); break;
-        default: LAUNCH_PSY2(16); break;
-      }
-#undef LAUNCH_PSY2
-    } else {
-      k_phaseA_psy<<<grid_for(c, rows, c->psy_ctas_per_sm), PSY_THREADS, smem, st>>>(P0, P1, ch, rows, A);
-    }
-    rc = post_launch(c); if (rc) return rc;
+  } else {
+    k_phaseA_psy<<<grid_for(c, rows, c->psy_ctas_per_sm), PSY_THREADS, smem, st>>>(P0, P1, ch, rows, A);
   }
-  return 0;
+  return post_launch(c);
 }
 
 static int phaseA_launch(vb200_ctx *c, int W, int nblocks, const vb200_phaseA_io *io,
@@ -1509,8 +1476,7 @@ static int cqn_launch(vb200_ctx *c, const CqnDev &Q0, const CqnDev &Q1, const vb
   int rc;
   const int wpb = 4;
   const long tasks = (long)nblocks * (Q0.n / 32);
-  const bool v1 = getenv("VB200_CQN_V1") && atoi(getenv("VB200_CQN_V1"));
-  if (!v1 && tasks < (1L << 30) && (Q0.n & (Q0.n - 1)) == 0 && (Q0.ch == 1 || (Q0.ch == 2 && Q0.steps <= 1))) {
+  if (tasks < (1L << 30) && (Q0.n & (Q0.n - 1)) == 0 && (Q0.ch == 1 || (Q0.ch == 2 && Q0.steps <= 1))) {
     const int grid = grid_for(c, (int)((tasks + wpb - 1) / wpb), 16);
     if (Q0.ch == 1) k_cqn_fast<1><<<grid, wpb * 32, 0, st>>>(Q0, Q1, d_desc, nblocks, d_mdct, d_iwork, d_nonzero);
     else k_cqn_fast<2><<<grid, wpb * 32, 0, st>>>(Q0, Q1, d_desc, nblocks, d_mdct, d_iwork, d_nonzero);

@@ -64,6 +64,21 @@ struct PsyDev {
   int max_cls_len;           // longest class
 };
 
+// arguments of the fused psy kernels (k_phaseA_psy3 and the generic k_phaseA_psy)
+struct PsyArgs {
+  const float *mdct_in;   // [rows][n] raw mdct
+  const float *logfft;    // [rows][n]
+  const float *lmax;      // [rows]
+  const float *gmax;      // [blocks]
+  const vb200_block_desc *desc;
+  float *mdct_out;        // [rows][n] (may alias mdct_in)
+  float *logmdct;         // [rows][n]
+  float *logmask;         // [rows][n]
+  float *ampmax_out;      // [blocks]
+  float *tap_noise, *tap_tone;
+  unsigned long long *dbg_cycles;   // optional [16]: per-phase SM cycles summed over rows (thread 0 of each CTA)
+};
+
 // ------------------------------------------------------------------------
 __device__ __forceinline__ float todB_dev(float x) {           // lib/scales.h:43-51
   const unsigned int u = __float_as_uint(x) & 0x7fffffffu;
@@ -79,11 +94,9 @@ __device__ __forceinline__ float add345(float x) {             // "+ .345" is a 
 __device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)__cvta_generic_to_shared(p); }
 __device__ __forceinline__ float lds_f32(unsigned a) { float v; asm volatile("ld.shared.f32 %0, [%1];" : "=f"(v) : "r"(a)); return v; }
 __device__ __forceinline__ int lds_s32(unsigned a) { int v; asm volatile("ld.shared.s32 %0, [%1];" : "=r"(v) : "r"(a)); return v; }
-__device__ __forceinline__ int lds_s16(unsigned a) { short v; asm volatile("ld.shared.s16 %0, [%1];" : "=h"(v) : "r"(a)); return (int)v; }
 __device__ __forceinline__ int4 lds_v4(unsigned a) { int4 v; asm volatile("ld.shared.v4.s32 {%0,%1,%2,%3}, [%4];" : "=r"(v.x), "=r"(v.y), "=r"(v.z), "=r"(v.w) : "r"(a)); return v; }
 __device__ __forceinline__ float4 lds_f4(unsigned a) { float4 v; asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(v.x), "=f"(v.y), "=f"(v.z), "=f"(v.w) : "r"(a)); return v; }
 __device__ __forceinline__ void sts_f4(unsigned a, float4 v) { asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" :: "r"(a), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory"); }
-__device__ __forceinline__ void sts_s16(unsigned a, int v) { asm volatile("st.shared.s16 [%0], %1;" :: "r"(a), "h"((short)v) : "memory"); }
 __device__ __forceinline__ void sts_f32(unsigned a, float v) { asm volatile("st.shared.f32 [%0], %1;" :: "r"(a), "f"(v) : "memory"); }
 __device__ __forceinline__ void sts_s32(unsigned a, int v) { asm volatile("st.shared.s32 [%0], %1;" :: "r"(a), "r"(v) : "memory"); }
 __device__ __forceinline__ void named_bar_sync(int barid, int nt) { asm volatile("bar.sync %0, %1;" :: "r"(barid), "r"(nt) : "memory"); }
@@ -92,11 +105,6 @@ __device__ __forceinline__ void named_bar_sync(int barid, int nt) { asm volatile
 __device__ __forceinline__ float lds_f32_if(unsigned a, float old, bool p) {
   asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %2, 0;\n\t@q ld.shared.f32 %0, [%1];\n\t}" : "+f"(old) : "r"(a), "r"((int)p));
   return old;
-}
-__device__ __forceinline__ int lds_s16_if(unsigned a, int old, bool p) {
-  short v = (short)old;
-  asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %2, 0;\n\t@q ld.shared.s16 %0, [%1];\n\t}" : "+h"(v) : "r"(a), "r"((int)p));
-  return (int)v;
 }
 __device__ __forceinline__ int lds_s32_if(unsigned a, int old, bool p) {
   asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %2, 0;\n\t@q ld.shared.s32 %0, [%1];\n\t}" : "+r"(old) : "r"(a), "r"((int)p));
@@ -108,46 +116,31 @@ __device__ __forceinline__ void sts_s32_if(unsigned a, int v, bool p) {
 __device__ __forceinline__ void sts_f32_if(unsigned a, float v, bool p) {
   asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %2, 0;\n\t@q st.shared.f32 [%0], %1;\n\t}" :: "r"(a), "f"(v), "r"((int)p) : "memory");
 }
-__device__ __forceinline__ void sts_s16_if(unsigned a, int v, bool p) {
-  asm volatile("{\n\t.reg .pred q;\n\tsetp.ne.b32 q, %2, 0;\n\t@q st.shared.s16 [%0], %1;\n\t}" :: "r"(a), "h"((short)v), "r"((int)p) : "memory");
-}
 // cp.async: 16 bytes global -> shared without passing through registers (SASS: LDGSTS)
 __device__ __forceinline__ void cp_async16(unsigned dst, const void *src) {
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" :: "r"(dst), "l"(src) : "memory");
 }
 __device__ __forceinline__ void cp_async_commit() { asm volatile("cp.async.commit_group;" ::: "memory"); }
 __device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_group 0;" ::: "memory"); }
-// producer/consumer flag in shared memory: release publishes everything the warp wrote before (after a __syncwarp),
-// acquire orders the consumer's later loads after the flag read
-__device__ __forceinline__ void sts_release(unsigned a, int v) { asm volatile("st.release.cta.shared.s32 [%0], %1;" :: "r"(a), "r"(v) : "memory"); }
-__device__ __forceinline__ int lds_acquire(unsigned a) { int v; asm volatile("ld.acquire.cta.shared.s32 %0, [%1];" : "=r"(v) : "r"(a) : "memory"); return v; }
-__device__ __forceinline__ void spin_pause(unsigned ns) { __nanosleep(ns); }
 __device__ __forceinline__ void prefetch_l2(const void *p) { asm volatile("prefetch.global.L2 [%0];" :: "l"(p)); }
 #else   // host emulation build (tools/cuemu, development aid): "shared addresses" are offsets into the CTA's buffer
 __device__ __forceinline__ unsigned smem_u32(const void *p) { return (unsigned)((const unsigned char *)p - cuemu::dyn_smem()); }
 __device__ __forceinline__ float lds_f32(unsigned a) { return *reinterpret_cast<const float *>(cuemu::dyn_smem() + a); }
 __device__ __forceinline__ int lds_s32(unsigned a) { return *reinterpret_cast<const int *>(cuemu::dyn_smem() + a); }
-__device__ __forceinline__ int lds_s16(unsigned a) { return (int)*reinterpret_cast<const short *>(cuemu::dyn_smem() + a); }
 __device__ __forceinline__ int4 lds_v4(unsigned a) { return *reinterpret_cast<const int4 *>(cuemu::dyn_smem() + a); }
 __device__ __forceinline__ float4 lds_f4(unsigned a) { return *reinterpret_cast<const float4 *>(cuemu::dyn_smem() + a); }
 __device__ __forceinline__ void sts_f4(unsigned a, float4 v) { *reinterpret_cast<float4 *>(cuemu::dyn_smem() + a) = v; }
-__device__ __forceinline__ void sts_s16(unsigned a, int v) { *reinterpret_cast<short *>(cuemu::dyn_smem() + a) = (short)v; }
 __device__ __forceinline__ void sts_f32(unsigned a, float v) { *reinterpret_cast<float *>(cuemu::dyn_smem() + a) = v; }
 __device__ __forceinline__ void sts_s32(unsigned a, int v) { *reinterpret_cast<int *>(cuemu::dyn_smem() + a) = v; }
 __device__ __forceinline__ void named_bar_sync(int barid, int nt) { cuemu_named_barrier(barid, nt); }
-__device__ __forceinline__ void sts_release(unsigned a, int v) { __atomic_store_n(reinterpret_cast<int *>(cuemu::dyn_smem() + a), v, __ATOMIC_RELEASE); }
-__device__ __forceinline__ int lds_acquire(unsigned a) { return __atomic_load_n(reinterpret_cast<int *>(cuemu::dyn_smem() + a), __ATOMIC_ACQUIRE); }
-__device__ __forceinline__ void spin_pause(unsigned) { sched_yield(); }
 __device__ __forceinline__ void prefetch_l2(const void *) {}
 __device__ __forceinline__ void cp_async16(unsigned dst, const void *src) { memcpy(cuemu::dyn_smem() + dst, src, 16); }
 __device__ __forceinline__ void cp_async_commit() {}
 __device__ __forceinline__ void cp_async_wait_all() {}
 __device__ __forceinline__ float lds_f32_if(unsigned a, float old, bool p) { return p ? lds_f32(a) : old; }
-__device__ __forceinline__ int lds_s16_if(unsigned a, int old, bool p) { return p ? lds_s16(a) : old; }
 __device__ __forceinline__ void sts_f32_if(unsigned a, float v, bool p) { if (p) sts_f32(a, v); }
 __device__ __forceinline__ int lds_s32_if(unsigned a, int old, bool p) { return p ? lds_s32(a) : old; }
 __device__ __forceinline__ void sts_s32_if(unsigned a, int v, bool p) { if (p) sts_s32(a, v); }
-__device__ __forceinline__ void sts_s16_if(unsigned a, int v, bool p) { if (p) sts_s16(a, v); }
 #endif
 
 __device__ __forceinline__ float warp_max(float v) {
@@ -629,15 +622,6 @@ __device__ __forceinline__ float4 dev_window4(const WinDev &Wd, int W, int lW, i
   return x;                                         // flat middle: untouched (x*1.0f is exact)
 }
 
-__device__ __forceinline__ void dev_load_windowed(const WinDev &Wd, int W, int lW, int nW,
-                                                  const float *__restrict__ src, float *dst,
-                                                  int tid, int nt) {
-  const int N = Wd.N[W];
-  const float4 *s4 = reinterpret_cast<const float4 *>(src);
-  for (int v = tid; v < (N >> 2); v += nt)
-    *reinterpret_cast<float4 *>(dst + 4 * v) = dev_window4(Wd, W, lW, nW, 4 * v, __ldg(s4 + v));
-}
-
 // ------------------------------------------------------------------------
 // Noise mask: bark_noise_hybridmp (lib/psy.c:547-704).
 // S = 5 prefix arrays with row stride ns (ns = n+4 keeps the five sequential
@@ -759,7 +743,7 @@ __device__ __forceinline__ void dev_noise_regress(const PsyDev &P, float *noise,
   }
 }
 
-// single-bin forms used by the register-resident kernel (vb200_psy2.cuh)
+// single-bin form used by the register-resident kernel (vb200_psy3.cuh)
 __device__ __forceinline__ void dev_noise_term1(int i, float f, float offset, float *S, int ns) {
   float *aN = S, *aX = S + ns, *aXX = S + 2 * ns, *aY = S + 3 * ns, *aXY = S + 4 * ns;
   float y = f + offset;
@@ -773,34 +757,6 @@ __device__ __forceinline__ void dev_noise_term1(int i, float f, float offset, fl
     const float wx = w * x;
     aN[i] = w; aX[i] = wx; aXX[i] = wx * x; aY[i] = w * y; aXY[i] = wx * y;
   }
-}
-
-__device__ __forceinline__ float dev_noise_regress1(const PsyDev &P, int i, float offset, int fixed,
-                                                    const float *S, int ns) {
-  const int bfe = P.bark_first_extra, ffe = P.fixed_first_extra;
-  Abd cur; cur.A = 0.f; cur.B = 0.f; cur.D = 1.f;
-  if (bfe > 0) {
-    const int wb = i < bfe ? i : bfe - 1;
-    const int bk = __ldg(P.bark + wb);
-    cur = dev_window_abd(bk >> 16, bk & 0xffff, S, ns);
-  }
-  const float x = (float)i;
-  float R = (cur.A + x * cur.B) / cur.D;
-  if (R < 0.f) R = 0.f;
-  float v = R - offset;
-  if (fixed > 0) {
-    if (ffe > 0) {
-      const int wb = i < ffe ? i : ffe - 1;
-      const int hi = wb + fixed / 2, lo = hi - fixed;
-      cur = dev_window_abd(lo, hi, S, ns);
-    } else if (bfe > 0 && i < bfe) {
-      const int bk = __ldg(P.bark + (bfe - 1));
-      cur = dev_window_abd(bk >> 16, bk & 0xffff, S, ns);
-    }
-    const float R2 = (cur.A + x * cur.B) / cur.D;
-    if (R2 - offset < v) v = R2 - offset;
-  }
-  return v;
 }
 
 // _vp_noisemask (lib/psy.c:706-752): logmdct (smem) -> noise (smem).

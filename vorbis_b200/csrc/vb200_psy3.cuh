@@ -1,9 +1,8 @@
 // vb200_psy3.cuh — k_phaseA_psy3: the fused noise/tone/mix kernel, instruction-count-first layout.
 //
-// k_phaseA_psy2 measured 36.0 k warp-instructions per 1024-bin row, half of them in the tone mask
-// (profiles/r1_*; the kernel is issue bound, DRAM 4 %).  This version keeps psy2's data layout
-// (one 128-thread CTA per (block,channel) row, per-bin values in registers, tone scratch aliased
-// with the prefix-sum area) and replaces the phases whose lanes were mostly idle:
+// The kernel is issue bound, not DRAM bound.  Every 128 threads work on one (block,channel) row, with
+// the per-bin values in registers and the tone scratch aliased with the prefix-sum area, and the
+// phases are laid out so that few lanes sit idle:
 //
 //  * seed_curve scatter (lib/psy.c:390-415).  A run only has ~13 usable curve points (6..43 on
 //    the bench signal), so walking one run with 16 lanes spent ~50 instructions per 26 useful
@@ -18,10 +17,10 @@
 //  * the two sequential prefix sums run without register copies (two alternating register sets).
 //
 // Requires linesper == 8 (always, lib/modes/psych_*.h eighth_octave_lines) and
-// total_octave_lines <= 896; other setups use k_phaseA_psy2.  Exactness arguments for the
-// restart points are in vb200_kernels.cuh (dev_tone_chase_gather) and vb200_psy2.cuh.
+// total_octave_lines <= 896; other setups use the generic k_phaseA_psy.  The exactness argument for
+// the restart points is in vb200_kernels.cuh (dev_tone_chase_gather).
 #pragma once
-#include "vb200_psy2.cuh"
+#include "vb200_kernels.cuh"
 
 namespace vb200 {
 
@@ -305,7 +304,44 @@ __device__ __forceinline__ void dev_noise_scan3(int n, float *arr) {
 #undef SCAN4
 }
 
-// Two bins per call: halves the call overhead of the (deliberately not inlined, see vb200_psy2.cuh) per-bin
+// The per-bin regression and mix are called 8x (bins per thread) x 3 (windows); inlining them
+// made the kernel ~93 KB of SASS and 11 % of the stall samples were instruction-cache misses.
+// They are real functions here (scalars only in the signature, so nothing spills to local).
+template <int NS>
+__device__ __forceinline__ float dev_regress_bin(const int *__restrict__ bark, int bfe, int ffe, const float *S,
+                                                 int i, float offset, int fixed) {
+  Abd cur; cur.A = 0.f; cur.B = 0.f; cur.D = 1.f;
+  if (bfe > 0) {
+    const int wb = i < bfe ? i : bfe - 1;
+    const int bk = __ldg(bark + wb);
+    cur = dev_window_abd(bk >> 16, bk & 0xffff, S, NS);
+  }
+  const float x = (float)i;
+  float R = (cur.A + x * cur.B) / cur.D;
+  if (R < 0.f) R = 0.f;
+  float v = R - offset;
+  if (fixed > 0) {
+    if (ffe > 0) {
+      const int wb = i < ffe ? i : ffe - 1;
+      const int hi = wb + fixed / 2, lo = hi - fixed;
+      cur = dev_window_abd(lo, hi, S, NS);
+    } else if (bfe > 0 && i < bfe) {
+      const int bk = __ldg(bark + (bfe - 1));
+      cur = dev_window_abd(bk >> 16, bk & 0xffff, S, NS);
+    }
+    const float R2 = (cur.A + x * cur.B) / cur.D;
+    if (R2 - offset < v) v = R2 - offset;
+  }
+  return v;
+}
+
+template <int NS>
+__device__ __noinline__ float regress_core(const int *__restrict__ bark, int bfe, int ffe, const float *S,
+                                           int i, float offset, int fixed) {
+  return dev_regress_bin<NS>(bark, bfe, ffe, S, i, offset, fixed);
+}
+
+// Two bins per call: halves the call overhead of the (deliberately not inlined, see above) per-bin
 // regression and gives the scheduler two independent dependency chains.
 template <int NS>
 __device__ __noinline__ float2 regress_pair(const int *__restrict__ bark, int bfe, int ffe, const float *S,
@@ -317,6 +353,7 @@ __device__ __noinline__ float2 regress_pair(const int *__restrict__ bark, int bf
 }
 
 // final step of _vp_noisemask + tone lookup + _vp_offset_and_mix(select 1) for one bin, everything by value
+struct MixConst { float noisemaxsupp, toneatt, m_val, att; };
 struct MixOut { float logmask, m, nz, tn; };
 __device__ __noinline__ MixOut final_mix_val(float p2, float L, float p1, float noff, float ath, float gmin,
                                              const float *__restrict__ compand, MixConst C, float m) {
@@ -354,7 +391,7 @@ __device__ __noinline__ MixOut final_mix_val(float p2, float L, float p1, float 
 // stage-level API; the production instance carries neither (code size: instruction fetch is a first-order cost here)
 template <int K, int R, bool DBG>
 __global__ void __launch_bounds__(PSY3_THREADS * R, PSY3_MINB / R)
-k_phaseA_psy3(PsyDev P0, PsyDev P1, int ch, int nrows, PhaseA2Args A) {
+k_phaseA_psy3(PsyDev P0, PsyDev P1, int ch, int nrows, PsyArgs A) {
   extern __shared__ __align__(16) float sm_cta[];
   constexpr int nt = PSY3_THREADS;
   const int n = K * nt, ns = n + 4, tid = threadIdx.x & (nt - 1), half = threadIdx.x >> 7, lane = tid & 31;
