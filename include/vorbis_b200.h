@@ -187,7 +187,8 @@ int  vb200_debug_phase_cycles(vb200_ctx *ctx, unsigned long long *out16, int res
 /* mdct_forward, lib/mdct.c:492: in [nvec][N] -> out [nvec][N/2]            */
 int vb200_mdct_forward_dev (vb200_ctx*, int W, int nvec, const float *d_in, float *d_out, void *stream);
 int vb200_mdct_forward     (vb200_ctx*, int W, int nvec, const float *in,   float *out);
-/* mdct_backward, lib/mdct.c:396: in [nvec][N/2] -> out [nvec][N]           */
+/* mdct_backward, lib/mdct.c:396: in [nvec][N/2] -> out [nvec][N]; in half-rate mode
+ * (vb200_synthesis_halfrate) the transform of size N/2: in [nvec][N/4] -> out [nvec][N/2] */
 int vb200_mdct_backward_dev(vb200_ctx*, int W, int nvec, const float *d_in, float *d_out, void *stream);
 int vb200_mdct_backward    (vb200_ctx*, int W, int nvec, const float *in,   float *out);
 /* _vorbis_apply_window, lib/window.c:2102: in place on [nvec][N];
@@ -474,7 +475,11 @@ int vb200_encode_streams    (vb200_ctx*, int nstreams, int blobno, vb200_streams
  *       `coef`; channel c of that block is at coef_off + c*n_k
  * pcm_off  [nstreams][nblk] int64 offset (floats) into each channel's output
  *       where the samples finished by block k go (k=0 finishes nothing)
- * pcm   [nstreams][ch][pcm_stride]                                          */
+ * pcm   [nstreams][ch][pcm_stride]
+ * Half-rate mode (vb200_synthesis_halfrate): the same coef layout (channel stride n_k), of which the
+ * first n_k/2 lines of every channel are read; the IMDCT runs at N_k/2, the overlap-add uses the
+ * half windows of the halved sizes and block k finishes (N_{k-1}/4 + N_k/4)/2 samples
+ * (lib/block.c:735-842); pcm_off and pcm_stride count half-rate samples.                 */
 int vb200_synthesis_dev(vb200_ctx*, int nstreams, int nblk, const int32_t *d_Wseq,
                         const int64_t *d_coef_off, const float *d_coef,
                         const int64_t *d_pcm_off, float *d_pcm, int64_t pcm_stride, void *stream);
@@ -486,6 +491,14 @@ int vb200_synthesis_s16_dev(vb200_ctx*, int nstreams, int nblk, const int32_t *d
 int vb200_synthesis    (vb200_ctx*, int nstreams, int nblk, const int32_t *Wseq,
                         const int64_t *coef_off, const float *coef, int64_t coef_len,
                         const int64_t *pcm_off, float *pcm, int64_t pcm_stride);
+/* vorbis_synthesis_halfrate, lib/synthesis.c:166-174: flag != 0 turns half-rate decode on for the
+ * decode entry points of this context (mdct_backward, synthesis[_s16], decode_dsp; host and _dev forms).
+ * window[w] = the half-window of block size blocksizes[w]/2 (blocksizes[w]/4 floats), i.e. what
+ * _vorbis_window_get(b->window[w]-1) returns; NULL = closed form (not bit-exact, as for vb200_setup.window).
+ * The tables are built on the first call that turns the mode on; later calls do not read `window`.
+ * Returns VB200_EINVAL when flag != 0 and blocksizes[0] <= 64 (the reference returns -1 there).
+ * Takes effect for calls issued after it returns; encode entry points ignore it.                     */
+int vb200_synthesis_halfrate(vb200_ctx*, int flag, const float *const window[2]);
 
 /* ---- decode: channel de-coupling of mapping0_inverse (lib/mapping0.c:754-779).
  * res [nblocks][ch][n] residue vectors as left by the residue backend; every coupling step
@@ -507,7 +520,9 @@ int vb200_floor1_inverse2    (vb200_ctx*, int W, int floor_sel, int nrows, const
  * mdct_backward, windowed overlap-add.  Layout as vb200_synthesis; `res` holds the residue vectors as
  * the residue backend leaves them and is modified in place; posts / present are
  * [nstreams][nblk][ch][VB200_FLOOR1_STRIDE] and [nstreams][nblk][ch].  pcm_s16 != 0: the finished
- * samples leave as interleaved int16 (as vb200_synthesis_s16_dev), else planar float.                   */
+ * samples leave as interleaved int16 (as vb200_synthesis_s16_dev), else planar float.
+ * Half-rate mode: de-coupling and the floor multiply still cover all n lines, so `res` is left exactly
+ * as at full rate (lib/mapping0.c:754-790); the rest is vb200_synthesis in half-rate mode.               */
 int vb200_decode_dsp_dev(vb200_ctx*, int nstreams, int nblk, const int32_t *d_Wseq, const int64_t *d_coef_off,
                          float *d_res, const int32_t *d_posts, const int32_t *d_present,
                          const int64_t *d_pcm_off, void *d_pcm, int pcm_s16, int64_t pcm_stride, void *stream);

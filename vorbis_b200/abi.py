@@ -201,6 +201,16 @@ def _np_ptr(a, ctype):
     return a.ctypes.data_as(C.POINTER(ctype))
 
 
+def halfrate_window_ptrs(windows):
+    """the `const float *const window[2]` argument of vb200_synthesis_halfrate (and of the oracle's counterpart):
+    returns (what must stay alive during the call, pointer).  windows None: (None, NULL) = closed form."""
+    if windows is None:
+        return None, None
+    arrs = [np.ascontiguousarray(w, np.float32) for w in windows]
+    ptrs = (c_float_p * 2)(*[_np_ptr(a, C.c_float) for a in arrs])
+    return (arrs, ptrs), C.cast(ptrs, C.c_void_p)
+
+
 class SetupHolder:
     """Owns numpy copies of every table a `Setup` points to (so the ctypes struct
     stays valid), and converts to / from a flat dict of arrays (npz fixtures)."""
@@ -231,6 +241,10 @@ class SetupHolder:
             if key in a and a[key].size:
                 a[key] = np.ascontiguousarray(a[key], dtype=np.float32)
                 s.window[w] = _np_ptr(a[key], C.c_float)
+        for w in range(2):
+            key = "halfrate_window%d" % w
+            if key in a:
+                a[key] = np.ascontiguousarray(a[key], dtype=np.float32)
         if "chmux" in a:
             cm = np.asarray(a["chmux"]).astype(np.int64)
             for w in range(2):
@@ -308,6 +322,14 @@ class SetupHolder:
 
     def floor_posts(self, W, sel=0):
         return int(self.c.floor1[W][sel].posts)
+
+    def halfrate_windows(self):
+        """[w0, w1] the half windows of the block sizes blocksizes[w]/2 (blocksizes[w]/4 floats each, what
+        _vorbis_window_get(b->window[w]-1) returns) where the arrays hold them (keys halfrate_window0/1),
+        else None; the window argument of vb200_synthesis_halfrate"""
+        if "halfrate_window0" not in self.arrays:
+            return None
+        return [self.arrays["halfrate_window%d" % w] for w in range(2)]
 
     def save(self, path):
         np.savez_compressed(path, **self.arrays)

@@ -58,6 +58,12 @@ struct vb200_ctx {
   HostXform hx[2];
   XformDev dx[2];
   WinDev dwin;
+  // half-rate decode (vb200_synthesis_halfrate): transforms at blocksizes[w]/2 and the half windows of those
+  // sizes, built and uploaded the first time the mode is enabled
+  bool halfrate = false, hs_built = false;
+  HostXform hx_hs[2];
+  XformDev dx_hs[2];
+  WinDev dwin_hs;
   int n_psy = 0;
   HostPsyFlow hflow[4];
   PsyDev dpsy[4];
@@ -142,6 +148,23 @@ extern "C" int vb200_device_count(void) {
 
 static bool pow2(int v) { return v > 0 && (v & (v - 1)) == 0; }
 
+// mdct_init (and the window / FFT tables) of one block size: host tables into h, device copies into d
+static int xform_upload(vb200_ctx *c, int N, const float *window, HostXform &h, XformDev &d) {
+  build_xform(h, N, window);
+  memset(&d, 0, sizeof(d));
+  d.N = h.N; d.log2n = h.log2n; d.nst = h.log2n - 6; d.nf = h.nf; d.scale = h.scale;
+  for (int i = 0; i < h.nf && i < 8; i++) d.fac[i] = h.fac[i];
+  for (size_t i = 0; i < h.stage_off.size() && i < 8; i++) d.stage_off[i] = h.stage_off[i];
+  int rc;
+  if ((rc = upload(c, h.trig.data(), h.trig.size(), &d.trig))) return rc;
+  if ((rc = upload(c, h.bitrev.data(), h.bitrev.size(), &d.bitrev))) return rc;
+  const float *tw = nullptr;
+  if ((rc = upload(c, h.stage_tw.data(), h.stage_tw.size(), &tw))) return rc;
+  d.stage_tw = reinterpret_cast<const float2 *>(tw);
+  if ((rc = upload(c, h.win.data(), h.win.size(), &d.win))) return rc;
+  return upload(c, h.wa.data(), h.wa.size(), &d.wa);
+}
+
 extern "C" void vb200_ctx_destroy(vb200_ctx *c);
 // everything of vb200_ctx_create that can fail after the context exists; the caller destroys *c on failure
 static int ctx_build(vb200_ctx *c, const vb200_setup *s, int device) {
@@ -161,23 +184,10 @@ static int ctx_build(vb200_ctx *c, const vb200_setup *s, int device) {
   for (auto &e : c->ev_join) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
 
   for (int w = 0; w < 2; w++) {
-    HostXform &h = c->hx[w];
-    build_xform(h, s->blocksizes[w], s->window[w]);
-    XformDev &d = c->dx[w];
-    memset(&d, 0, sizeof(d));
-    d.N = h.N; d.log2n = h.log2n; d.nst = h.log2n - 6; d.nf = h.nf; d.scale = h.scale;
-    for (int i = 0; i < h.nf && i < 8; i++) d.fac[i] = h.fac[i];
-    for (size_t i = 0; i < h.stage_off.size() && i < 8; i++) d.stage_off[i] = h.stage_off[i];
     int rc;
-    if ((rc = upload(c, h.trig.data(), h.trig.size(), &d.trig))) return rc;
-    if ((rc = upload(c, h.bitrev.data(), h.bitrev.size(), &d.bitrev))) return rc;
-    const float *tw = nullptr;
-    if ((rc = upload(c, h.stage_tw.data(), h.stage_tw.size(), &tw))) return rc;
-    d.stage_tw = reinterpret_cast<const float2 *>(tw);
-    if ((rc = upload(c, h.win.data(), h.win.size(), &d.win))) return rc;
-    if ((rc = upload(c, h.wa.data(), h.wa.size(), &d.wa))) return rc;
-    c->dwin.N[w] = h.N;
-    c->dwin.win[w] = d.win;
+    if ((rc = xform_upload(c, s->blocksizes[w], s->window[w], c->hx[w], c->dx[w]))) return rc;
+    c->dwin.N[w] = c->hx[w].N;
+    c->dwin.win[w] = c->dx[w].win;
   }
   for (int w = 0; w < 2; w++) {      // residue classification parameters (lib/backends.h:103-118)
     ResDev hr[VB200_MAX_SUBMAPS];
@@ -856,6 +866,9 @@ k_offset_and_mix(PsyDev P, int nvec, int sel, const float *__restrict__ noise,
 // vorbis_synthesis_blockin (lib/block.c:767-823).  One CTA walks one (stream, channel)
 // block by block; the previous block's second half stays in shared memory, so the only
 // HBM traffic is the spectra in (2N) and the finished samples out (2N per channel-block).
+// HS: half-rate decode (lib/block.c:182,197-198,735-842).  X0/X1/Wd are then the tables of the halved block
+// sizes; the spectra keep the full-rate layout, so channel c of a block starts N_W/2 = X.N floats after
+// channel c-1 and only its first X.N/2 lines are read.
 // finished-sample sinks: planar float, or interleaved int16 as examples/decoder_example.c:250-262
 struct SinkF32 {
   float *p;
@@ -871,7 +884,7 @@ struct SinkS16 {
   }
 };
 
-template <bool S16>
+template <bool S16, bool HS>
 __global__ void __launch_bounds__(256)
 k_synthesis(XformDev X0, XformDev X1, WinDev Wd, int ch, int nstreams, int nblk,
             const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
@@ -890,7 +903,8 @@ k_synthesis(XformDev X0, XformDev X1, WinDev Wd, int ch, int nstreams, int nblk,
       const int W = Wseq[(size_t)st * nblk + k];
       const XformDev &X = W ? X1 : X0;
       const int N = X.N, n2 = N >> 1;
-      const float4 *src = reinterpret_cast<const float4 *>(coef + coef_off[(size_t)st * nblk + k] + (size_t)c * n2);
+      const size_t cstride = HS ? (size_t)N : (size_t)n2;
+      const float4 *src = reinterpret_cast<const float4 *>(coef + coef_off[(size_t)st * nblk + k] + c * cstride);
       for (int i = tid; i < (n2 >> 2); i += nt) reinterpret_cast<float4 *>(s_in)[i] = __ldg(src + i);
       __syncthreads();
       dev_mdct_backward<0>(X, s_in, s_out, tid, nt);
@@ -1013,7 +1027,7 @@ extern "C" int vb200_mdct_forward_dev(vb200_ctx *c, int W, int nvec, const float
 extern "C" int vb200_mdct_backward_dev(vb200_ctx *c, int W, int nvec, const float *d_in, float *d_out, void *stream) {
   CHECK_CTX(c); CHECK_W(W);
   if (nvec <= 0) return 0;
-  const XformDev &X = c->dx[W];
+  const XformDev &X = c->halfrate ? c->dx_hs[W] : c->dx[W];
   const size_t smem = sizeof(float) * (X.N + X.N / 2);
   const int nt = threads_for(X.N), grid = grid_for(c, nvec, 8);
   int rc;
@@ -1067,7 +1081,7 @@ extern "C" int vb200_mdct_backward(vb200_ctx *c, int W, int nvec, const float *i
   CHECK_CTX(c); CHECK_W(W);
   if (nvec <= 0) return 0;
   std::lock_guard<std::mutex> lk(c->mu);
-  const int N = c->dx[W].N;
+  const int N = (c->halfrate ? c->dx_hs[W] : c->dx[W]).N;
   HostIO io{c};
   void *di, *dout; int rc;
   if ((rc = io.h2d(in, sizeof(float) * (size_t)nvec * N / 2, &di))) return rc;
@@ -1525,18 +1539,48 @@ extern "C" int vb200_couple_quantize_normalize(vb200_ctx *c, int W, int blocktyp
 
 // ======================================================================== //
 // decode
+// vorbis_synthesis_halfrate, lib/synthesis.c:166-174
+extern "C" int vb200_synthesis_halfrate(vb200_ctx *c, int flag, const float *const window[2]) {
+  CHECK_CTX(c);
+  if (!flag) { c->halfrate = false; return 0; }
+  if (c->setup.blocksizes[0] <= 64) return fail(VB200_EINVAL, "half-rate decode needs blocksizes[0] > 64 (lib/synthesis.c:170)");
+  if (!c->hs_built) {
+    std::lock_guard<std::mutex> lk(c->mu);
+    for (int w = 0; w < 2; w++) {
+      int rc;
+      if ((rc = xform_upload(c, c->setup.blocksizes[w] / 2, window ? window[w] : nullptr, c->hx_hs[w], c->dx_hs[w])))
+        return rc;
+      c->dwin_hs.N[w] = c->hx_hs[w].N;
+      c->dwin_hs.win[w] = c->dx_hs[w].win;
+    }
+    c->hs_built = true;
+  }
+  c->halfrate = true;
+  return 0;
+}
+
+template <bool S16, bool HS>
+static int synthesis_launch(vb200_ctx *c, int nstreams, int nblk, const int32_t *d_Wseq, const int64_t *d_coef_off,
+                            const float *d_coef, const int64_t *d_pcm_off, void *d_pcm, int64_t pcm_stride,
+                            void *stream) {
+  const XformDev *X = HS ? c->dx_hs : c->dx;
+  const int ch = c->setup.channels, N1 = X[1].N;
+  const size_t smem = sizeof(float) * ((size_t)N1 / 2 + N1 + N1 / 2);
+  int rc = set_smem(k_synthesis<S16, HS>, smem); if (rc) return rc;
+  k_synthesis<S16, HS><<<grid_for(c, nstreams * ch, 8), threads_for(N1), smem, (cudaStream_t)stream>>>(
+      X[0], X[1], HS ? c->dwin_hs : c->dwin, ch, nstreams, nblk, d_Wseq, (const long long *)d_coef_off, d_coef,
+      (const long long *)d_pcm_off, d_pcm, (long long)pcm_stride);
+  return post_launch(c);
+}
+
 extern "C" int vb200_synthesis_dev(vb200_ctx *c, int nstreams, int nblk, const int32_t *d_Wseq,
                                    const int64_t *d_coef_off, const float *d_coef,
                                    const int64_t *d_pcm_off, float *d_pcm, int64_t pcm_stride, void *stream) {
   CHECK_CTX(c);
   if (nstreams <= 0 || nblk <= 0) return 0;
-  const int ch = c->setup.channels, N1 = c->dx[1].N;
-  const size_t smem = sizeof(float) * ((size_t)N1 / 2 + N1 + N1 / 2);
-  int rc = set_smem(k_synthesis<false>, smem); if (rc) return rc;
-  k_synthesis<false><<<grid_for(c, nstreams * ch, 8), threads_for(N1), smem, (cudaStream_t)stream>>>(
-      c->dx[0], c->dx[1], c->dwin, ch, nstreams, nblk, d_Wseq, (const long long *)d_coef_off, d_coef,
-      (const long long *)d_pcm_off, d_pcm, (long long)pcm_stride);
-  return post_launch(c);
+  return c->halfrate
+      ? synthesis_launch<false, true>(c, nstreams, nblk, d_Wseq, d_coef_off, d_coef, d_pcm_off, d_pcm, pcm_stride, stream)
+      : synthesis_launch<false, false>(c, nstreams, nblk, d_Wseq, d_coef_off, d_coef, d_pcm_off, d_pcm, pcm_stride, stream);
 }
 
 extern "C" int vb200_synthesis_s16_dev(vb200_ctx *c, int nstreams, int nblk, const int32_t *d_Wseq,
@@ -1544,13 +1588,9 @@ extern "C" int vb200_synthesis_s16_dev(vb200_ctx *c, int nstreams, int nblk, con
                                        const int64_t *d_pcm_off, int16_t *d_pcm16, int64_t pcm_stride, void *stream) {
   CHECK_CTX(c);
   if (nstreams <= 0 || nblk <= 0) return 0;
-  const int ch = c->setup.channels, N1 = c->dx[1].N;
-  const size_t smem = sizeof(float) * ((size_t)N1 / 2 + N1 + N1 / 2);
-  int rc = set_smem(k_synthesis<true>, smem); if (rc) return rc;
-  k_synthesis<true><<<grid_for(c, nstreams * ch, 8), threads_for(N1), smem, (cudaStream_t)stream>>>(
-      c->dx[0], c->dx[1], c->dwin, ch, nstreams, nblk, d_Wseq, (const long long *)d_coef_off, d_coef,
-      (const long long *)d_pcm_off, d_pcm16, (long long)pcm_stride);
-  return post_launch(c);
+  return c->halfrate
+      ? synthesis_launch<true, true>(c, nstreams, nblk, d_Wseq, d_coef_off, d_coef, d_pcm_off, d_pcm16, pcm_stride, stream)
+      : synthesis_launch<true, false>(c, nstreams, nblk, d_Wseq, d_coef_off, d_coef, d_pcm_off, d_pcm16, pcm_stride, stream);
 }
 
 extern "C" int vb200_synthesis(vb200_ctx *c, int nstreams, int nblk, const int32_t *Wseq,

@@ -85,11 +85,26 @@ static int32_t *bind_iscratch(size_t n){
   return g.iscratch;
 }
 
+/* vorbis_synthesis_halfrate (lib/synthesis.c:166-174) as _vds_shared_init saw it when it built vd's lookups
+ * (lib/block.c:182,197-198): the decode shims then run at the halved sizes with the windows of those sizes */
+static int bind_halfrate(vorbis_dsp_state *vd){
+  codec_setup_info *ci = (codec_setup_info*)vd->vi->codec_setup;
+  private_state *b = (private_state*)vd->backend_state;
+  const float *win[2];
+  int rc;
+  if(!ci->halfrate_flag) return vb200_synthesis_halfrate(g.ctx, 0, NULL);
+  win[0] = _vorbis_window_get(b->window[0] - 1);
+  win[1] = _vorbis_window_get(b->window[1] - 1);
+  rc = vb200_synthesis_halfrate(g.ctx, 1, win);
+  if(rc) fprintf(stderr, "vb200 shim: vb200_synthesis_halfrate failed (%d): %s\n", rc, vb200_last_error());
+  return rc;
+}
+
 /* Build the device context from the lookups _vds_shared_init made (lib/block.c:170-294). */
 int vb200shim_attach(vorbis_dsp_state *vd, int device){
   vorbis_info *vi = vd->vi;
   vb200_binding *found = vb200shim_binding(vd);
-  if(found){ found->refs++; g_cur = found; return 0; }       /* another state of the same setup: share the context */
+  if(found){ found->refs++; g_cur = found; return bind_halfrate(vd); }   /* another state of the same setup: share the context */
   {
     int slot;
     for(slot = 0; slot < VB200_MAX_BINDINGS && g_bind[slot].ctx; slot++);
@@ -203,7 +218,7 @@ int vb200shim_attach_new(vorbis_dsp_state *vd, int device){
     return rc;
   }
   g.vd = vd; g.setup_key = (void*)vi->codec_setup; g.analysisp = vd->analysisp; g.refs = 1;
-  return 0;
+  return bind_halfrate(vd);
 }
 
 /* drop the calling thread's current binding (the context goes with its last user) */
@@ -222,9 +237,10 @@ int vb200shim_select(vorbis_dsp_state *vd){
 
 unsigned long long vb200shim_launches(void){ return (g_cur && g.ctx) ? vb200_launch_count(g.ctx) : 0; }
 
+/* the block-size flag of a transform of n points; half-rate decode builds them at blocksizes[W]>>1 */
 static int W_of_n(int n){
   codec_setup_info *ci = (codec_setup_info*)g.vd->vi->codec_setup;
-  return n == ci->blocksizes[1] ? 1 : 0;
+  return n == ci->blocksizes[1] >> ci->halfrate_flag ? 1 : 0;
 }
 static int look_of(vorbis_look_psy *p){
   private_state *b = (private_state*)g.vd->backend_state;

@@ -29,7 +29,7 @@ EXPORTS = [
     "vb200_analysis_phaseA_dev", "vb200_analysis_phaseA", "vb200_analysis_phaseA_streams_dev",
     "vb200_analysis_phaseA_pcmstream_dev", "vb200_synthesis_s16_dev",
     "vb200_couple_quantize_normalize_dev", "vb200_couple_quantize_normalize",
-    "vb200_synthesis_dev", "vb200_synthesis", "vb200_decouple_dev", "vb200_decouple",
+    "vb200_synthesis_dev", "vb200_synthesis", "vb200_synthesis_halfrate", "vb200_decouple_dev", "vb200_decouple",
     "vb200_floor1_fit_dev", "vb200_floor1_fit", "vb200_floor1_render_dev", "vb200_floor1_render",
     "vb200_encode_dsp_dev", "vb200_encode_dsp", "vb200_encode_dsp_managed_dev", "vb200_encode_dsp_managed",
     "vb200_envelope_search_dev", "vb200_envelope_search", "vb200_envelope_search_var", "vb200_envelope_apply_marks",
@@ -90,6 +90,7 @@ def load():
     L.vb200_couple_quantize_normalize.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, vp, vp, vp]
     L.vb200_synthesis_dev.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, C.c_int64, vp]
     L.vb200_synthesis.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, C.c_int64, vp, vp, C.c_int64]
+    L.vb200_synthesis_halfrate.argtypes = [vp, C.c_int, vp]
     L.vb200_decouple_dev.argtypes = [vp, C.c_int, C.c_int, vp, vp]
     L.vb200_decouple.argtypes = [vp, C.c_int, C.c_int, vp]
     L.vb200_floor1_fit_dev.argtypes = [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp, vp, vp]
@@ -143,6 +144,7 @@ class Context:
         h = vp()
         self._chk(self.L.vb200_ctx_create(C.byref(setup.c), device, C.byref(h)))
         self.h = h
+        self.halfrate = 0
 
     def _chk(self, rc):
         if rc != 0:
@@ -196,8 +198,10 @@ class Context:
         return out
 
     def mdct_backward(self, W, x):
-        x = np.ascontiguousarray(x, np.float32).reshape(-1, self.bs[W] // 2)
-        out = np.empty((x.shape[0], self.bs[W]), np.float32)
+        """in half-rate mode the transform of size blocksizes[W]/2"""
+        N = self.bs[W] >> self.halfrate
+        x = np.ascontiguousarray(x, np.float32).reshape(-1, N // 2)
+        out = np.empty((x.shape[0], N), np.float32)
         self._chk(self.L.vb200_mdct_backward(self.h, W, x.shape[0], _ptr(x), _ptr(out)))
         return out
 
@@ -567,14 +571,24 @@ class Context:
                                          _ptr(pcm_off), _ptr(pcm), pcm_stride))
         return pcm
 
+    def synthesis_halfrate(self, flag, windows=None):
+        """vb200_synthesis_halfrate: half-rate decode on (flag true) or off for the decode entry points.
+        windows: the half windows of blocksizes[w]/2 (SetupHolder.halfrate_windows()); None = closed form.
+        Use synthesis_layout(..., halfrate=True) for the offsets while it is on."""
+        keep, ptrs = abi.halfrate_window_ptrs(windows)
+        self._chk(self.L.vb200_synthesis_halfrate(self.h, 1 if flag else 0, ptrs))
+        self.halfrate = 1 if flag else 0
+
     def synthesis_dev(self, nstreams, nblk, d_Wseq, d_coef_off, d_coef, d_pcm_off, d_pcm, pcm_stride, stream=None):
         self._chk(self.L.vb200_synthesis_dev(self.h, nstreams, nblk, _ptr(d_Wseq), _ptr(d_coef_off), _ptr(d_coef),
                                              _ptr(d_pcm_off), _ptr(d_pcm), pcm_stride, _ptr(stream)))
 
 
-def synthesis_layout(Wseq, bs, channels):
+def synthesis_layout(Wseq, bs, channels, halfrate=False):
     """Offsets for vb200_synthesis: Wseq [nstreams][nblk] -> (coef_off, pcm_off, coef_len, pcm_len)
-    with every stream's spectra packed back to back (block-major, channel-minor)."""
+    with every stream's spectra packed back to back (block-major, channel-minor).  halfrate: the spectra
+    keep this layout, the finished samples are counted at half rate ((bs[lW]/4 + bs[W]/4) >> 1 per block,
+    lib/block.c:840-842)."""
     Wseq = np.asarray(Wseq, np.int32)
     ns, nblk = Wseq.shape
     N = np.where(Wseq == 1, bs[1], bs[0]).astype(np.int64)
@@ -583,7 +597,7 @@ def synthesis_layout(Wseq, bs, channels):
     flat = per_block.reshape(-1)
     coef_off.reshape(-1)[1:] = np.cumsum(flat)[:-1]
     fin = np.zeros((ns, nblk), np.int64)
-    fin[:, 1:] = N[:, :-1] // 4 + N[:, 1:] // 4
+    fin[:, 1:] = (N[:, :-1] // 4 + N[:, 1:] // 4) >> (1 if halfrate else 0)
     pcm_off = np.cumsum(fin, axis=1) - fin      # finished samples before block k's contribution
     # block k's finished samples start where block k-1's ended
     pcm_off = np.concatenate([np.zeros((ns, 1), np.int64), np.cumsum(fin, axis=1)[:, :-1]], axis=1)
