@@ -466,6 +466,23 @@ typedef struct vb200_streams_io {
 } vb200_streams_io;
 int vb200_encode_streams_dev(vb200_ctx*, int nstreams, int blobno, vb200_streams_io *d_io, void *stream);
 int vb200_encode_streams    (vb200_ctx*, int nstreams, int blobno, vb200_streams_io *io);
+/* Bitrate-managed whole streams: the same envelope search, plan, transforms and ampmax chain, then per size the
+ * psy stage and every step of vb200_encode_dsp_managed (three masks and fits, twelve interpolated curves, floor
+ * render and couple/quantise/normalise of all VB200_PACKETBLOBS curves).  Same vb200_streams_io; the curve
+ * outputs are blob-major with cap[W] blocks from one curve to the next, so their layout is fixed before count[W]
+ * is known:
+ *   posts[W]      [VB200_PACKETBLOBS][cap[W]*ch][VB200_FLOOR1_STRIDE]   (all zero where the curve is NULL)
+ *   nonzero[W]    [VB200_PACKETBLOBS][cap[W]*ch]
+ *   iwork[W]      [VB200_PACKETBLOBS][cap[W]*ch][blocksizes[W]/2]        int32
+ *   ampmax_out[W] [cap[W]]
+ * Block `slot` of curve k is row k*cap[W]*ch + slot*ch + channel; rows past count[W] of a curve are not
+ * written.  count[] and the error when count > cap as vb200_encode_streams.  The host form makes one
+ * synchronous H2D - compute - D2H round trip (no chunk pipeline) and copies back count[W] blocks of every
+ * curve into the same cap-strided host layout.  Device scratch per size besides that of vb200_encode_streams:
+ * the psy stage's noise and tone taps and the low-/high-noise mask (3 x count*ch*blocksizes[W]/2 floats), the
+ * three fits' flags (3 x count*ch) and the curves' present flags (VB200_PACKETBLOBS x cap*ch), int32.          */
+int vb200_encode_streams_managed_dev(vb200_ctx*, int nstreams, vb200_streams_io *d_io, void *stream);
+int vb200_encode_streams_managed    (vb200_ctx*, int nstreams, vb200_streams_io *io);
 
 /* ---- decode: mdct_backward (lib/mapping0.c:792-795) fused with the windowed
  *      overlap-add of vorbis_synthesis_blockin (lib/block.c:767-823).

@@ -81,7 +81,7 @@ struct vb200_ctx {
   cudaStream_t s_split[2] = {nullptr, nullptr};       // vb200_encode_dsp_dev: two concurrent half-batches
   cudaEvent_t ev_fork = nullptr, ev_join[2] = {nullptr, nullptr};
   DevBuf enc_buf[8];                 // scratch of vb200_encode_dsp_dev
-  DevBuf str_buf[40];                // scratch of vb200_plan_blocks / vb200_encode_streams[_dev]
+  DevBuf str_buf[50];                // scratch of vb200_plan_blocks / vb200_encode_streams[_managed][_dev]
   DevBuf mgd_buf[24];                // scratch + host-call staging of vb200_encode_dsp_managed[_dev]
   // vb200_encode_dsp (host buffers): chunks rotate over ENC_SETS buffer sets; one stream per copy direction and
   // two compute streams, ordered by events (see there)
@@ -1503,7 +1503,45 @@ static int cqn_launch(vb200_ctx *c, const CqnDev &Q0, const CqnDev &Q1, const vb
   }
   if ((rc = post_launch(c))) return rc;
   if (Q0.steps > 0) {
-    k_cqn_nonzero<<<(nblocks + 127) / 128, 128, 0, st>>>(nblocks, Q0.ch, Q0.steps, Q0.mag, Q0.ang, d_nonzero);
+    k_cqn_nonzero<<<(nblocks + 127) / 128, 128, 0, st>>>(nblocks, Q0.ch, Q0.steps, Q0.mag, Q0.ang, d_nonzero, 0);
+    if ((rc = post_launch(c))) return rc;
+  }
+  return 0;
+}
+
+// bitrate-managed mode: couple/quantise/normalise of all VB200_PACKETBLOBS curves, curve k with blob k's
+// parameters; curve k's iwork / nonzero rows start k * blob_blocks blocks in.  Mono and stereo with at most one
+// coupling step take every curve in one k_cqn_fast_curves launch; other setups run k_cqn once per curve.
+static int cqn_curves_launch(vb200_ctx *c, int W, const vb200_block_desc *d_desc, int nblocks, long long blob_blocks,
+                             const float *d_mdct, int32_t *d_iwork, int32_t *d_nonzero, cudaStream_t st) {
+  constexpr int NB = VB200_PACKETBLOBS;
+  const int ch = c->setup.channels, n = c->dx[W].N / 2;
+  CqnDev Q[2];                       // the kernel takes only the fields that do not depend on the blob from these
+  CqnCurveTab T;
+  int rc;
+  for (int k = 0; k < NB; k++)
+    for (int bt = 0; bt < 2; bt++) {
+      if ((rc = cqn_setup(c, W, bt, k, &Q[bt]))) return rc;
+      T.c[bt][k] = {Q[bt].limit, Q[bt].sliding_lowpass, Q[bt].prepoint, Q[bt].postpoint};
+    }
+  const long tasks = (long)nblocks * (n / 32);
+  if (!(tasks < (1L << 30) && (n & (n - 1)) == 0 && (ch == 1 || (ch == 2 && Q[0].steps <= 1)))) {
+    for (int k = 0; k < NB; k++) {
+      CqnDev Q0, Q1;
+      if ((rc = cqn_setup(c, W, 0, k, &Q0))) return rc;
+      if ((rc = cqn_setup(c, W, 1, k, &Q1))) return rc;
+      const size_t r0 = (size_t)k * blob_blocks * ch;
+      if ((rc = cqn_launch(c, Q0, Q1, d_desc, nblocks, d_mdct, d_iwork + r0 * n, d_nonzero + r0, st))) return rc;
+    }
+    return 0;
+  }
+  const int wpb = 4, grid = grid_for(c, (int)((tasks + wpb - 1) / wpb), 16);
+  if (ch == 1) k_cqn_fast_curves<1><<<grid, wpb * 32, 0, st>>>(Q[0], Q[1], T, d_desc, nblocks, blob_blocks, d_mdct, d_iwork, d_nonzero);
+  else k_cqn_fast_curves<2><<<grid, wpb * 32, 0, st>>>(Q[0], Q[1], T, d_desc, nblocks, blob_blocks, d_mdct, d_iwork, d_nonzero);
+  if ((rc = post_launch(c))) return rc;
+  if (Q[0].steps > 0) {
+    k_cqn_nonzero<<<dim3((nblocks + 127) / 128, NB), 128, 0, st>>>(nblocks, ch, Q[0].steps, Q[0].mag, Q[0].ang, d_nonzero,
+                                                                   blob_blocks);
     if ((rc = post_launch(c))) return rc;
   }
   return 0;
@@ -1670,16 +1708,25 @@ extern "C" int vb200_floor1_fit_dev(vb200_ctx *c, int W, int floor_sel, int nrow
   return post_launch(c);
 }
 
+// `curves` curves of nrows rows each in one launch; curve k's rows start k * blob_rows rows in
+static int floor1_render_launch(vb200_ctx *c, int W, int floor_sel, int nrows, int curves, long long blob_rows,
+                                int32_t *d_posts, const int32_t *d_fit_nonzero, int32_t *d_ilogmask,
+                                int32_t *d_nonzero, cudaStream_t st) {
+  Floor1Args a; int rc;
+  if ((rc = floor1_args(c, W, floor_sel, nrows, &a))) return rc;
+  const int ctas = (nrows + F1_WARPS - 1) / F1_WARPS;
+  k_floor1_render<<<dim3(grid_for(c, ctas, 8), curves), 32 * F1_WARPS, 0, st>>>(a, d_posts, d_fit_nonzero, d_ilogmask,
+                                                                             d_nonzero, blob_rows);
+  return post_launch(c);
+}
+
 extern "C" int vb200_floor1_render_dev(vb200_ctx *c, int W, int floor_sel, int nrows, int32_t *d_posts,
                                        const int32_t *d_fit_nonzero, int32_t *d_ilogmask, int32_t *d_nonzero,
                                        void *stream) {
   CHECK_CTX(c); CHECK_W(W);
   if (nrows <= 0) return 0;
-  Floor1Args a; int rc;
-  if ((rc = floor1_args(c, W, floor_sel, nrows, &a))) return rc;
-  const int ctas = (nrows + F1_WARPS - 1) / F1_WARPS;
-  k_floor1_render<<<grid_for(c, ctas, 8), 32 * F1_WARPS, 0, (cudaStream_t)stream>>>(a, d_posts, d_fit_nonzero, d_ilogmask, d_nonzero);
-  return post_launch(c);
+  return floor1_render_launch(c, W, floor_sel, nrows, 1, 0, d_posts, d_fit_nonzero, d_ilogmask, d_nonzero,
+                              (cudaStream_t)stream);
 }
 
 extern "C" int vb200_floor1_fit(vb200_ctx *c, int W, int floor_sel, int nrows, const float *logmdct,
@@ -1901,6 +1948,56 @@ static int managed_check(vb200_ctx *c, int W, int nstreams, int bps, const vb200
   return 0;
 }
 
+// scratch of the managed tail: the psy stage's noise and tone taps, the low- / high-noise mask, the flags of the
+// three fits and the present flag of every curve
+struct MgdScratch {
+  float *noise, *tone, *alt;
+  int32_t *fz3, *present;
+};
+
+static int mgd_scratch(DevBuf *B, size_t rows, size_t blob_rows, size_t n, MgdScratch *M) {
+  void *p; int rc;
+  const size_t big = sizeof(float) * rows * n;
+  if ((rc = ensure_buf(B[0], big, &p))) return rc; M->noise = (float *)p;
+  if ((rc = ensure_buf(B[1], big, &p))) return rc; M->tone = (float *)p;
+  if ((rc = ensure_buf(B[2], big, &p))) return rc; M->alt = (float *)p;
+  if ((rc = ensure_buf(B[3], sizeof(int32_t) * rows * 3, &p))) return rc; M->fz3 = (int32_t *)p;
+  if ((rc = ensure_buf(B[4], sizeof(int32_t) * blob_rows * VB200_PACKETBLOBS, &p))) return rc; M->present = (int32_t *)p;
+  return 0;
+}
+
+// Bitrate-managed mode after the psy stage (run with the noise and tone taps into M): the middle fit, the
+// low-noise (2) and high-noise (0) masks and their fits, the twelve interpolated curves, then the floor render,
+// couple/quantise/normalise and nonzero propagation of all 15 curves.  posts / nonzero / iwork are blob-major
+// with blob_blocks blocks (>= nblocks) from one curve to the next.
+static int managed_tail(vb200_ctx *c, int W, int nblocks, long long blob_blocks, const vb200_block_desc *d_desc,
+                        const float *mdct, const float *logmdct, const float *logmask, const MgdScratch &M,
+                        int32_t *posts, int32_t *nonzero, int32_t *iwork, cudaStream_t st) {
+  constexpr int NB = VB200_PACKETBLOBS, MID = VB200_PACKETBLOBS / 2;
+  const int ch = c->setup.channels, n = c->dx[W].N / 2;
+  const size_t rows = (size_t)nblocks * ch, brows = (size_t)blob_blocks * ch, pblob = brows * VB200_FLOOR1_STRIDE;
+  int32_t *fz_lo = M.fz3, *fz_mid = M.fz3 + rows, *fz_hi = M.fz3 + 2 * rows;
+  int rc;
+  // the middle curve (select 1, what un-managed mode codes), then the low-noise (2) and high-noise (0) masks
+  if ((rc = vb200_floor1_fit_dev(c, W, -1, (int)rows, logmdct, logmask, posts + MID * pblob, fz_mid, st))) return rc;
+  const PsyDev &P0 = c->dpsy[(W ? 2 : 0)], &P1 = c->dpsy[(W ? 2 : 0) + 1];
+  const long long total = (long long)rows * n;
+  for (int pass = 0; pass < 2; pass++) {
+    const int sel = pass ? 0 : 2;
+    k_mix_select<<<grid_for(c, (int)((total + 255) / 256), 8), 256, 0, st>>>(P0, P1, d_desc, ch, total, sel, M.noise,
+                                                                            M.tone, logmdct, M.alt);
+    if ((rc = post_launch(c))) return rc;
+    if ((rc = vb200_floor1_fit_dev(c, W, -1, (int)rows, logmdct, M.alt, posts + (sel ? NB - 1 : 0) * pblob,
+                                   sel ? fz_hi : fz_lo, st))) return rc;
+  }
+  k_floor1_interpolate<<<grid_for(c, (int)((rows * VB200_FLOOR1_STRIDE + 255) / 256), 8), 256, 0, st>>>(
+      (long long)rows, (long long)brows, posts, fz_lo, fz_mid, fz_hi, M.present);
+  if ((rc = post_launch(c))) return rc;
+  if ((rc = floor1_render_launch(c, W, -1, (int)rows, NB, (long long)brows, posts, M.present, iwork, nonzero, st)))
+    return rc;
+  return cqn_curves_launch(c, W, d_desc, nblocks, blob_blocks, mdct, iwork, nonzero, st);
+}
+
 extern "C" int vb200_encode_dsp_managed_dev(vb200_ctx *c, int W, int nstreams, int bps, const vb200_encode_io *d,
                                             void *stream) {
   CHECK_CTX(c); CHECK_W(W);
@@ -1909,58 +2006,29 @@ extern "C" int vb200_encode_dsp_managed_dev(vb200_ctx *c, int W, int nstreams, i
   cudaStream_t st = (cudaStream_t)stream;
   const int ch = c->setup.channels, n = c->dx[W].N / 2, nblocks = nstreams * bps;
   const size_t rows = (size_t)nblocks * ch, big = sizeof(float) * rows * n;
-  constexpr int NB = VB200_PACKETBLOBS, MID = VB200_PACKETBLOBS / 2;
   DevBuf *B = c->mgd_buf;
   void *p;
-  float *mdct, *logmdct, *logmask, *logfft, *lmax, *gmax, *noise, *tone, *alt;
-  int32_t *fz3, *present;
+  float *mdct, *logmdct, *logmask, *logfft, *lmax, *gmax;
+  MgdScratch M;
   if ((rc = ensure_buf(B[0], big, &p))) return rc; mdct = (float *)p;
   if ((rc = ensure_buf(B[1], big, &p))) return rc; logmdct = (float *)p;
   if ((rc = ensure_buf(B[2], big, &p))) return rc; logmask = (float *)p;
   if ((rc = ensure_buf(B[3], big, &p))) return rc; logfft = (float *)p;
   if ((rc = ensure_buf(B[4], sizeof(float) * rows, &p))) return rc; lmax = (float *)p;
   if ((rc = ensure_buf(B[5], sizeof(float) * nblocks, &p))) return rc; gmax = (float *)p;
-  if ((rc = ensure_buf(B[6], big, &p))) return rc; noise = (float *)p;
-  if ((rc = ensure_buf(B[7], big, &p))) return rc; tone = (float *)p;
-  if ((rc = ensure_buf(B[8], big, &p))) return rc; alt = (float *)p;
-  if ((rc = ensure_buf(B[9], sizeof(int32_t) * rows * 3, &p))) return rc; fz3 = (int32_t *)p;
-  if ((rc = ensure_buf(B[10], sizeof(int32_t) * rows * NB, &p))) return rc; present = (int32_t *)p;
+  if ((rc = mgd_scratch(B + 6, rows, rows, n, &M))) return rc;
   if ((rc = scratch_begin(c, st))) return rc;
   vb200_phaseA_io a;
   memset(&a, 0, sizeof(a));
   a.desc = d->desc; a.mdct = mdct; a.logmdct = logmdct; a.logmask = logmask; a.ampmax_out = d->ampmax_out;
-  a.tap_noise = noise; a.tap_tone = tone;
+  a.tap_noise = M.noise; a.tap_tone = M.tone;
   PcmSrc ps; const PcmSrc *pp = nullptr;
   if (d->pcm_fmt == VB200_PCM_F32_BLOCKS) a.pcm = (const float *)d->pcm;
   else { ps.base = d->pcm; ps.fmt = d->pcm_fmt; ps.bps = bps; ps.hop = d->hop; ps.stride = d->stream_stride; ps.blk_src = nullptr; pp = &ps; }
   if ((rc = phaseA_launch(c, W, nblocks, &a, d->independent ? 0 : nstreams, bps, d->ampmax0, st, logfft, lmax, gmax, pp)))
     return rc;
-  const size_t pblob = rows * VB200_FLOOR1_STRIDE;
-  int32_t *fz_lo = fz3, *fz_mid = fz3 + rows, *fz_hi = fz3 + 2 * rows;
-  // the middle curve (select 1, what un-managed mode codes), then the low-noise (2) and high-noise (0) masks
-  if ((rc = vb200_floor1_fit_dev(c, W, -1, (int)rows, logmdct, logmask, d->posts + MID * pblob, fz_mid, st))) return rc;
-  const PsyDev &P0 = c->dpsy[(W ? 2 : 0)], &P1 = c->dpsy[(W ? 2 : 0) + 1];
-  const long long total = (long long)rows * n;
-  for (int pass = 0; pass < 2; pass++) {
-    const int sel = pass ? 0 : 2;
-    k_mix_select<<<grid_for(c, (int)((total + 255) / 256), 8), 256, 0, st>>>(P0, P1, d->desc, ch, total, sel, noise, tone,
-                                                                            logmdct, alt);
-    if ((rc = post_launch(c))) return rc;
-    if ((rc = vb200_floor1_fit_dev(c, W, -1, (int)rows, logmdct, alt, d->posts + (sel ? NB - 1 : 0) * pblob,
-                                   sel ? fz_hi : fz_lo, st))) return rc;
-  }
-  k_floor1_interpolate<<<grid_for(c, (int)((rows * VB200_FLOOR1_STRIDE + 255) / 256), 8), 256, 0, st>>>(
-      (long long)rows, d->posts, fz_lo, fz_mid, fz_hi, present);
-  if ((rc = post_launch(c))) return rc;
-  for (int k = 0; k < NB; k++) {
-    int32_t *iw = (int32_t *)d->iwork + (size_t)k * rows * n, *nz = d->nonzero + (size_t)k * rows;
-    if ((rc = vb200_floor1_render_dev(c, W, -1, (int)rows, d->posts + k * pblob, present + (size_t)k * rows, iw, nz, st)))
-      return rc;
-    CqnDev Q0, Q1;
-    if ((rc = cqn_setup(c, W, 0, k, &Q0))) return rc;
-    if ((rc = cqn_setup(c, W, 1, k, &Q1))) return rc;
-    if ((rc = cqn_launch(c, Q0, Q1, d->desc, nblocks, mdct, iw, nz, st))) return rc;
-  }
+  if ((rc = managed_tail(c, W, nblocks, nblocks, d->desc, mdct, logmdct, logmask, M, d->posts, d->nonzero,
+                         (int32_t *)d->iwork, st))) return rc;
   return scratch_end(c, st);
 }
 
@@ -2148,8 +2216,8 @@ extern "C" int vb200_plan_blocks(vb200_ctx *c, int nstreams, const int32_t *mark
   return 0;
 }
 
-extern "C" int vb200_encode_streams_dev(vb200_ctx *c, int nstreams, int blobno, vb200_streams_io *d, void *stream) {
-  CHECK_CTX(c);
+// arguments of both streams calls; zeroes count[] (nstreams <= 0: nothing to do)
+static int streams_check(vb200_ctx *c, int nstreams, vb200_streams_io *d) {
   int rc;
   if ((rc = plan_check(c))) return rc;
   if (!d) return fail(VB200_EINVAL, "null io");
@@ -2157,12 +2225,19 @@ extern "C" int vb200_encode_streams_dev(vb200_ctx *c, int nstreams, int blobno, 
   if (nstreams <= 0) return 0;
   if (!d->pcm || !d->pcm_len || !d->plan || !d->nblocks || d->max_blocks < 1) return fail(VB200_EINVAL, "encode_streams: pcm, pcm_len, plan, nblocks");
   if (d->pcm_fmt != VB200_PCM_F32_PLANAR && d->pcm_fmt != VB200_PCM_S16_INTERLEAVED) return fail(VB200_EINVAL, "pcm_fmt");
-  if (blobno < 0 || blobno >= VB200_PACKETBLOBS) return fail(VB200_EINVAL, "blobno");
   for (int w = 0; w < 2; w++)
     if (d->cap[w] < 0 || (d->cap[w] > 0 && (!d->posts[w] || !d->nonzero[w] || !d->iwork[w] || !d->ampmax_out[w])))
       return fail(VB200_EINVAL, "encode_streams: outputs of a size with capacity > 0");
   if (d->stream_stride < c->setup.blocksizes[1]) return fail(VB200_EINVAL, "stream_stride");
-  cudaStream_t st = (cudaStream_t)stream;
+  return 0;
+}
+
+// The front half of both streams calls, up to the psy stage: envelope search, marks, plan, the transforms of
+// both sizes and the ampmax chain along every stream.  Sets count[]; for each size with blocks, S[w] holds the
+// transforms, a[w] the psy stage's io and d_desc[w] the batch's block descriptors.
+static int streams_front(vb200_ctx *c, int nstreams, vb200_streams_io *d, cudaStream_t st, EncScratch S[2],
+                         vb200_phaseA_io a[2], vb200_block_desc *d_desc[2]) {
+  int rc;
   const int ch = c->setup.channels;
   // 1. envelope search over the whole timeline (fresh detector state), 2. marks, 3. plan
   const int nsteps = (int)(d->stream_stride / PLAN_STEP) - PLAN_VE_WIN;
@@ -2174,7 +2249,7 @@ extern "C" int vb200_encode_streams_dev(vb200_ctx *c, int nstreams, int blobno, 
   if ((rc = ensure_buf(c->str_buf[11], (size_t)nstreams * nsteps, &p))) return rc; uint8_t *d_ret = (uint8_t *)p;
   if ((rc = ensure_buf(c->str_buf[2], sizeof(int32_t) * (size_t)nstreams * mark_stride, &p))) return rc; int32_t *d_mark = (int32_t *)p;
   if ((rc = ensure_buf(c->str_buf[5], sizeof(int32_t) * 2, &p))) return rc; int32_t *d_tot = (int32_t *)p;
-  int2 *d_src[2]; vb200_block_desc *d_desc[2];
+  int2 *d_src[2];
   for (int w = 0; w < 2; w++) {
     const size_t cw = d->cap[w] > 0 ? d->cap[w] : 1;
     if ((rc = ensure_buf(c->str_buf[6 + w], sizeof(int2) * cw, &p))) return rc; d_src[w] = (int2 *)p;
@@ -2194,9 +2269,7 @@ extern "C" int vb200_encode_streams_dev(vb200_ctx *c, int nstreams, int blobno, 
   CU(cudaStreamSynchronize(st));                       // the launches below are sized by the plan
   d->count[0] = tot[0]; d->count[1] = tot[1];
   if (tot[0] > d->cap[0] || tot[1] > d->cap[1]) return fail(VB200_EINVAL, "encode_streams: more blocks than cap[] (count[] holds the need)");
-  // 4. transforms of both sizes, 5. the ampmax chain along every stream, 6. the rest of the chain per size
-  EncScratch S[2];
-  vb200_phaseA_io a[2];
+  // 4. transforms of both sizes, 5. the ampmax chain along every stream
   for (int w = 0; w < 2; w++) {
     memset(&a[w], 0, sizeof(a[w]));
     if (!tot[w]) continue;
@@ -2215,9 +2288,24 @@ extern "C" int vb200_encode_streams_dev(vb200_ctx *c, int nstreams, int blobno, 
                                                           sa[0], sa[1], tot[0] ? S[0].gmax : nullptr, tot[1] ? S[1].gmax : nullptr);
     if ((rc = post_launch(c))) return rc;
   }
+  return 0;
+}
+
+extern "C" int vb200_encode_streams_dev(vb200_ctx *c, int nstreams, int blobno, vb200_streams_io *d, void *stream) {
+  CHECK_CTX(c);
+  int rc;
+  if ((rc = streams_check(c, nstreams, d)) || nstreams <= 0) return rc;
+  if (blobno < 0 || blobno >= VB200_PACKETBLOBS) return fail(VB200_EINVAL, "blobno");
+  cudaStream_t st = (cudaStream_t)stream;
+  const int ch = c->setup.channels;
+  EncScratch S[2];
+  vb200_phaseA_io a[2];
+  vb200_block_desc *d_desc[2];
+  if ((rc = streams_front(c, nstreams, d, st, S, a, d_desc))) return rc;
+  // 6. the rest of the chain per size
   for (int w = 0; w < 2; w++) {
-    if (!tot[w]) continue;
-    const int nb = tot[w], rows = nb * ch;
+    if (!d->count[w]) continue;
+    const int nb = d->count[w], rows = nb * ch;
     if ((rc = phaseA_psy_launch(c, w, nb, &a[w], st, S[w].logfft, S[w].lmax, S[w].gmax))) return rc;
     if ((rc = vb200_floor1_fit_dev(c, w, -1, rows, S[w].logmdct, S[w].logmask, d->posts[w], S[w].fitnz, st))) return rc;
     if ((rc = vb200_floor1_render_dev(c, w, -1, rows, d->posts[w], S[w].fitnz, d->iwork[w], d->nonzero[w], st))) return rc;
@@ -2229,8 +2317,33 @@ extern "C" int vb200_encode_streams_dev(vb200_ctx *c, int nstreams, int blobno, 
   return scratch_end(c, st);
 }
 
-extern "C" int vb200_encode_streams(vb200_ctx *c, int nstreams, int blobno, vb200_streams_io *h) {
+extern "C" int vb200_encode_streams_managed_dev(vb200_ctx *c, int nstreams, vb200_streams_io *d, void *stream) {
   CHECK_CTX(c);
+  int rc;
+  if ((rc = streams_check(c, nstreams, d)) || nstreams <= 0) return rc;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int ch = c->setup.channels;
+  EncScratch S[2];
+  vb200_phaseA_io a[2];
+  vb200_block_desc *d_desc[2];
+  if ((rc = streams_front(c, nstreams, d, st, S, a, d_desc))) return rc;
+  for (int w = 0; w < 2; w++) {
+    if (!d->count[w]) continue;
+    const int nb = d->count[w];
+    MgdScratch M;
+    if ((rc = mgd_scratch(c->str_buf + 40 + 5 * w, (size_t)nb * ch, (size_t)d->cap[w] * ch, c->dx[w].N / 2, &M))) return rc;
+    a[w].tap_noise = M.noise; a[w].tap_tone = M.tone;
+    if ((rc = phaseA_psy_launch(c, w, nb, &a[w], st, S[w].logfft, S[w].lmax, S[w].gmax))) return rc;
+    if ((rc = managed_tail(c, w, nb, d->cap[w], d_desc[w], S[w].mdct, S[w].logmdct, S[w].logmask, M, d->posts[w],
+                           d->nonzero[w], d->iwork[w], st))) return rc;
+  }
+  return scratch_end(c, st);
+}
+
+// host buffers of both streams calls: one synchronous H2D - compute - D2H round trip.  curves = 1: un-managed
+// (blob blobno); VB200_PACKETBLOBS: bitrate-managed, every output but ampmax_out holds the curves one after the
+// other, cap[W] blocks apart, and count[W] blocks of each come back.
+static int streams_host(vb200_ctx *c, int nstreams, int blobno, int curves, vb200_streams_io *h) {
   int rc;
   if ((rc = plan_check(c))) return rc;
   if (!h) return fail(VB200_EINVAL, "null io");
@@ -2252,29 +2365,43 @@ extern "C" int vb200_encode_streams(vb200_ctx *c, int nstreams, int blobno, vb20
   for (int w = 0; w < 2; w++) {
     const size_t cw = h->cap[w] > 0 ? h->cap[w] : 0, n = c->dx[w].N / 2;
     if (!cw) continue;
-    if ((rc = ensure_buf(c->str_buf[30 + 4 * w], sizeof(int32_t) * cw * ch * VB200_FLOOR1_STRIDE, &p))) return rc; d.posts[w] = (int32_t *)p;
-    if ((rc = ensure_buf(c->str_buf[31 + 4 * w], sizeof(int32_t) * cw * ch, &p))) return rc; d.nonzero[w] = (int32_t *)p;
-    if ((rc = ensure_buf(c->str_buf[32 + 4 * w], sizeof(int32_t) * cw * ch * n, &p))) return rc; d.iwork[w] = (int32_t *)p;
+    if ((rc = ensure_buf(c->str_buf[30 + 4 * w], sizeof(int32_t) * curves * cw * ch * VB200_FLOOR1_STRIDE, &p))) return rc; d.posts[w] = (int32_t *)p;
+    if ((rc = ensure_buf(c->str_buf[31 + 4 * w], sizeof(int32_t) * curves * cw * ch, &p))) return rc; d.nonzero[w] = (int32_t *)p;
+    if ((rc = ensure_buf(c->str_buf[32 + 4 * w], sizeof(int32_t) * curves * cw * ch * n, &p))) return rc; d.iwork[w] = (int32_t *)p;
     if ((rc = ensure_buf(c->str_buf[33 + 4 * w], sizeof(float) * cw, &p))) return rc; d.ampmax_out[w] = (float *)p;
   }
   CU(cudaMemcpyAsync((void *)d.pcm, h->pcm, pcm_bytes, cudaMemcpyHostToDevice, st));
   CU(cudaMemcpyAsync((void *)d.pcm_len, h->pcm_len, sizeof(int64_t) * nstreams, cudaMemcpyHostToDevice, st));
   if (h->eof) CU(cudaMemcpyAsync((void *)d.eof, h->eof, sizeof(int64_t) * nstreams, cudaMemcpyHostToDevice, st));
-  rc = vb200_encode_streams_dev(c, nstreams, blobno, &d, st);
+  rc = curves == 1 ? vb200_encode_streams_dev(c, nstreams, blobno, &d, st) : vb200_encode_streams_managed_dev(c, nstreams, &d, st);
   h->count[0] = d.count[0]; h->count[1] = d.count[1];
   if (rc) return rc;
   CU(cudaMemcpyAsync(h->plan, d.plan, sizeof(vb200_stream_block) * pcap, cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(h->nblocks, d.nblocks, sizeof(int32_t) * nstreams, cudaMemcpyDeviceToHost, st));
   for (int w = 0; w < 2; w++) {
-    const size_t nb = d.count[w], n = c->dx[w].N / 2;
+    const size_t nb = d.count[w], n = c->dx[w].N / 2, cw = h->cap[w];
     if (!nb) continue;
-    CU(cudaMemcpyAsync(h->posts[w], d.posts[w], sizeof(int32_t) * nb * ch * VB200_FLOOR1_STRIDE, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(h->nonzero[w], d.nonzero[w], sizeof(int32_t) * nb * ch, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(h->iwork[w], d.iwork[w], sizeof(int32_t) * nb * ch * n, cudaMemcpyDeviceToHost, st));
+    for (int k = 0; k < curves; k++) {
+      const size_t r0 = k * cw * ch;
+      CU(cudaMemcpyAsync(h->posts[w] + r0 * VB200_FLOOR1_STRIDE, d.posts[w] + r0 * VB200_FLOOR1_STRIDE,
+                         sizeof(int32_t) * nb * ch * VB200_FLOOR1_STRIDE, cudaMemcpyDeviceToHost, st));
+      CU(cudaMemcpyAsync(h->nonzero[w] + r0, d.nonzero[w] + r0, sizeof(int32_t) * nb * ch, cudaMemcpyDeviceToHost, st));
+      CU(cudaMemcpyAsync(h->iwork[w] + r0 * n, d.iwork[w] + r0 * n, sizeof(int32_t) * nb * ch * n, cudaMemcpyDeviceToHost, st));
+    }
     CU(cudaMemcpyAsync(h->ampmax_out[w], d.ampmax_out[w], sizeof(float) * nb, cudaMemcpyDeviceToHost, st));
   }
   CU(cudaStreamSynchronize(st));
   return 0;
+}
+
+extern "C" int vb200_encode_streams(vb200_ctx *c, int nstreams, int blobno, vb200_streams_io *h) {
+  CHECK_CTX(c);
+  return streams_host(c, nstreams, blobno, 1, h);
+}
+
+extern "C" int vb200_encode_streams_managed(vb200_ctx *c, int nstreams, vb200_streams_io *h) {
+  CHECK_CTX(c);
+  return streams_host(c, nstreams, 0, VB200_PACKETBLOBS, h);
 }
 
 // ======================================================================== //

@@ -121,6 +121,65 @@ __device__ __forceinline__ CqnDev cqn_pick(const CqnDev &a, const CqnDev &b, boo
 // shared memory except the 256-entry floor table, and the next task's four loads are in flight
 // while the current one is computed (the kernel is latency bound: two dependent global loads,
 // two IEEE divisions and an fp64 sqrt per channel on the critical path).
+//
+// One (block, 32 lines) task of one curve: slot 0 = magnitude channel, slot 1 = angle channel.
+template <int CH>
+__device__ __forceinline__ void cqn_fast_lines(const CqnDev &Q, const float *s_fromdB, bool coupled, int line,
+                                               int lane, const float (&mv)[CH], const int (&il)[CH],
+                                               const int (&nzr)[CH], int (&out)[CH]) {
+  const int width = Q.partition;
+  const int i = line & ~(width - 1), j = line - i;
+  float R[CH], Qe[CH], F[CH];
+  int G[CH];
+#pragma unroll
+  for (int k = 0; k < CH; k++) {
+    R[k] = 0.f; Qe[k] = 0.f; F[k] = 1e-10f; G[k] = 0; out[k] = 0;
+    if (nzr[k]) {
+      const float fl = s_fromdB[il[k] & 255];
+      const float point = j >= Q.limit - i ? Q.postpoint : Q.prepoint;      // flag_lossless
+      G[k] = (fabsf(mv[k]) / fl < point) ? 0 : 1;
+      Qe[k] = R[k] = mv[k] * mv[k];
+      if (mv[k] < 0.f) R[k] *= -1.f;
+      F[k] = fl * fl;
+      cqn_normalize(Q, R[k], Qe[k], F[k], false, 0, i, j, out[k], width, lane);
+    }
+  }
+  if (CH == 2 && coupled && (nzr[0] || nzr[1])) {
+    float reM = R[0], reA = R[1], qeM = Qe[0], qeA = Qe[1];
+    int gM = G[0], gA = G[1], iM = out[0], iA = out[1];
+    if (j < Q.sliding_lowpass - i) {
+      if (gM || gA) {                                    // lossless: integer square-polar map
+        const int A = iM, B = iA;
+        reM = fabsf(reM) + fabsf(reA);
+        qeM = qeM + qeA;
+        gM = gA = 1;
+        if (abs(A) > abs(B)) {
+          iA = (A > 0 ? A - B : B - A);
+        } else {
+          iA = (B > 0 ? A - B : B - A);
+          iM = B;
+        }
+        if (iA >= abs(iM) * 2) { iA = -iA; iM = -iM; }
+      } else {                                           // point stereo
+        if (j < Q.limit - i) {
+          reM += reA;
+          qeM = fabsf(reM);
+        } else {
+          const float e = fabsf(reM) + fabsf(reA);
+          qeM = e;
+          reM = (reM + reA < 0.f) ? -e : e;
+        }
+        reA = qeA = 0.f;
+        gA = 1;
+        iA = 0;
+      }
+    }
+    const float fM = F[0] + F[1];
+    cqn_normalize(Q, reM, qeM, fM, true, gM, i, j, iM, width, lane);
+    out[0] = iM; out[1] = iA;
+  }
+}
+
 template <int CH>
 __global__ void __launch_bounds__(128)
 k_cqn_fast(CqnDev Q0, CqnDev Q1, const vb200_block_desc *__restrict__ desc, int nblocks,
@@ -155,59 +214,76 @@ k_cqn_fast(CqnDev Q0, CqnDev Q1, const vb200_block_desc *__restrict__ desc, int 
     if (t < tasks - stride) fetch(t + stride, nmv, nil, nnz);
     const int blk = t >> csh, line = ((t & ((1 << csh) - 1)) << 5) + lane;
     const CqnDev Q = cqn_pick(Q0, Q1, desc && desc[blk].blocktype);
-    const int width = Q.partition;
-    const int i = line & ~(width - 1), j = line - i;
-    float R[CH], Qe[CH], F[CH];
-    int G[CH], out[CH];
-#pragma unroll
-    for (int k = 0; k < CH; k++) {
-      R[k] = 0.f; Qe[k] = 0.f; F[k] = 1e-10f; G[k] = 0; out[k] = 0;
-      if (nzr[k]) {
-        const float fl = s_fromdB[il[k] & 255];
-        const float point = j >= Q.limit - i ? Q.postpoint : Q.prepoint;      // flag_lossless
-        G[k] = (fabsf(mv[k]) / fl < point) ? 0 : 1;
-        Qe[k] = R[k] = mv[k] * mv[k];
-        if (mv[k] < 0.f) R[k] *= -1.f;
-        F[k] = fl * fl;
-        cqn_normalize(Q, R[k], Qe[k], F[k], false, 0, i, j, out[k], width, lane);
-      }
-    }
-    if (CH == 2 && coupled && (nzr[0] || nzr[1])) {
-      float reM = R[0], reA = R[1], qeM = Qe[0], qeA = Qe[1];
-      int gM = G[0], gA = G[1], iM = out[0], iA = out[1];
-      if (j < Q.sliding_lowpass - i) {
-        if (gM || gA) {                                    // lossless: integer square-polar map
-          const int A = iM, B = iA;
-          reM = fabsf(reM) + fabsf(reA);
-          qeM = qeM + qeA;
-          gM = gA = 1;
-          if (abs(A) > abs(B)) {
-            iA = (A > 0 ? A - B : B - A);
-          } else {
-            iA = (B > 0 ? A - B : B - A);
-            iM = B;
-          }
-          if (iA >= abs(iM) * 2) { iA = -iA; iM = -iM; }
-        } else {                                           // point stereo
-          if (j < Q.limit - i) {
-            reM += reA;
-            qeM = fabsf(reM);
-          } else {
-            const float e = fabsf(reM) + fabsf(reA);
-            qeM = e;
-            reM = (reM + reA < 0.f) ? -e : e;
-          }
-          reA = qeA = 0.f;
-          gA = 1;
-          iA = 0;
-        }
-      }
-      const float fM = F[0] + F[1];
-      cqn_normalize(Q, reM, qeM, fM, true, gM, i, j, iM, width, lane);
-      out[0] = iM; out[1] = iA;
-    }
+    int out[CH];
+    cqn_fast_lines<CH>(Q, s_fromdB, coupled, line, lane, mv, il, nzr, out);
     {
       int *iw = iwork + (size_t)blk * CH * n + line;
+      __stcs(iw + (size_t)c0 * n, out[0]);
+      if (CH == 2) __stcs(iw + (size_t)c1 * n, out[CH - 1]);
+    }
+  }
+}
+
+// ---- bitrate-managed mode: all VB200_PACKETBLOBS curves in one launch (same channel cases as k_cqn_fast).
+// The curves share the MDCT and differ in the floor (iwork[k] holds curve k's ilogmask on entry), the
+// nonzero flags and four parameters of the blob, kept per (blocktype, blob) in shared memory.  One warp owns
+// 32 lines of one block for every curve: the MDCT lines are loaded once per task, and the next curve's (or
+// the next task's first curve's) floor and flags are in flight while the current curve is computed.
+struct CqnCurve {
+  int limit, sliding_lowpass;   // coupling_pointlimit[blockflag][blob], sliding_lowpass[W][blob]
+  float prepoint, postpoint;    // the coupling point amplitudes of the blob
+};
+struct CqnCurveTab { CqnCurve c[2][VB200_PACKETBLOBS]; };   // [blocktype][blob]
+
+template <int CH>
+__global__ void __launch_bounds__(128)
+k_cqn_fast_curves(CqnDev Q0, CqnDev Q1, const __grid_constant__ CqnCurveTab T,
+                  const vb200_block_desc *__restrict__ desc, int nblocks, long long blob_blocks,
+                  const float *__restrict__ mdct, int *__restrict__ iwork, const int *__restrict__ nonzero) {
+  constexpr int NB = VB200_PACKETBLOBS;
+  __shared__ float s_fromdB[256];
+  __shared__ CqnCurve s_cur[2 * NB];
+  for (int i = threadIdx.x; i < 256; i += blockDim.x) s_fromdB[i] = __ldg(Q0.fromdB + i);
+  if (threadIdx.x < 2 * NB) s_cur[threadIdx.x] = (&T.c[0][0])[threadIdx.x];
+  __syncthreads();
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5, wpb = blockDim.x >> 5;
+  const int n = Q0.n, csh = 31 - __clz(n >> 5);          // n is a power of two: chunks = 1 << csh
+  const int tasks = nblocks << csh, stride = gridDim.x * wpb;   // the launcher keeps tasks < 2^31
+  const size_t brows = (size_t)blob_blocks * CH;         // rows between consecutive curves
+  const bool coupled = CH == 2 && Q0.steps > 0;
+  const int c0 = coupled ? __ldg(Q0.mag) : 0, c1 = coupled ? __ldg(Q0.ang) : 1;
+  float mv[CH], nmv[CH];
+  int il[CH], nil[CH], nzr[CH], nnz[CH];
+  // curve k's floor and flags of task t; with curve 0 also the task's MDCT lines
+  auto fetch = [&](int t, int k) {
+    const int blk = t >> csh, line = ((t & ((1 << csh) - 1)) << 5) + lane;
+#pragma unroll
+    for (int s = 0; s < CH; s++) {
+      const size_t row = (size_t)blk * CH + (s == 0 ? c0 : c1), crow = (size_t)k * brows + row;
+      nnz[s] = __ldg(nonzero + crow);
+      nil[s] = __ldcs(iwork + crow * n + line);
+      if (k == 0) nmv[s] = __ldcs(mdct + row * n + line);
+    }
+  };
+  int t = blockIdx.x * wpb + wid;
+  if (t < tasks) fetch(t, 0);
+  for (; t < tasks; t += stride) {
+    const int blk = t >> csh, line = ((t & ((1 << csh) - 1)) << 5) + lane;
+    const int bt = desc && desc[blk].blocktype ? 1 : 0;
+    CqnDev Q = cqn_pick(Q0, Q1, bt);
+#pragma unroll
+    for (int s = 0; s < CH; s++) mv[s] = nmv[s];
+#pragma unroll 1
+    for (int k = 0; k < NB; k++) {
+#pragma unroll
+      for (int s = 0; s < CH; s++) { il[s] = nil[s]; nzr[s] = nnz[s]; }
+      if (k + 1 < NB) fetch(t, k + 1);
+      else if (t < tasks - stride) fetch(t + stride, 0);
+      const CqnCurve cv = s_cur[bt * NB + k];
+      Q.limit = cv.limit; Q.sliding_lowpass = cv.sliding_lowpass; Q.prepoint = cv.prepoint; Q.postpoint = cv.postpoint;
+      int out[CH];
+      cqn_fast_lines<CH>(Q, s_fromdB, coupled, line, lane, mv, il, nzr, out);
+      int *iw = iwork + ((size_t)k * brows + (size_t)blk * CH) * n + line;
       __stcs(iw + (size_t)c0 * n, out[0]);
       if (CH == 2) __stcs(iw + (size_t)c1 * n, out[CH - 1]);
     }
@@ -308,12 +384,13 @@ k_cqn(CqnDev Q0, CqnDev Q1, const vb200_block_desc *__restrict__ desc, int nbloc
   }
 }
 
-// nonzero[] propagation over coupling steps (lib/psy.c:1203-1212); runs after k_cqn
+// nonzero[] propagation over coupling steps (lib/psy.c:1203-1212); runs after k_cqn.  blockIdx.y = curve,
+// curve y's flags start blob_blocks blocks after curve y-1's (one curve: gridDim.y = 1)
 __global__ void k_cqn_nonzero(int nblocks, int ch, int steps, const int *__restrict__ mag,
-                              const int *__restrict__ ang, int *__restrict__ nonzero) {
+                              const int *__restrict__ ang, int *__restrict__ nonzero, long long blob_blocks) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= nblocks) return;
-  int *nz = nonzero + (size_t)b * ch;
+  int *nz = nonzero + ((size_t)blockIdx.y * (size_t)blob_blocks + b) * ch;
   for (int s = 0; s < steps; s++)
     if (nz[mag[s]] || nz[ang[s]]) { nz[mag[s]] = 1; nz[ang[s]] = 1; }
 }

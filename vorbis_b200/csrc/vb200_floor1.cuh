@@ -325,9 +325,15 @@ k_floor1_fit(Floor1Args a, const float *__restrict__ logmdct, const float *__res
   }
 }
 
+// blockIdx.y = curve: rows a.nrows of every curve, curve y's arrays start blob_rows rows after curve y-1's
+// (bitrate-managed mode renders its 15 curves in one launch; one curve: gridDim.y = 1)
 __global__ void __launch_bounds__(32 * F1_WARPS)
 k_floor1_render(Floor1Args a, int32_t *__restrict__ posts, const int32_t *__restrict__ fit_nonzero,
-                int32_t *__restrict__ ilogmask, int32_t *__restrict__ nonzero) {
+                int32_t *__restrict__ ilogmask, int32_t *__restrict__ nonzero, long long blob_rows) {
+  {
+    const size_t b = (size_t)blockIdx.y * (size_t)blob_rows;
+    posts += b * VB200_FLOOR1_STRIDE; fit_nonzero += b; ilogmask += b * a.n; nonzero += b;
+  }
   __shared__ Floor1Dev sF[VB200_MAX_SUBMAPS];
   __shared__ int s_post[F1_WARPS][VB200_VIF_POSIT + 2];
   __shared__ short s_segx[F1_WARPS][VB200_VIF_POSIT + 3];

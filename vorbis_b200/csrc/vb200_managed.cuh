@@ -28,9 +28,10 @@ k_mix_select(PsyDev P0, PsyDev P1, const vb200_block_desc *__restrict__ desc, in
   }
 }
 
-// one thread per (row, post slot); present[k][row] for all VB200_PACKETBLOBS curves
+// one thread per (row, post slot); present[k][row] for all VB200_PACKETBLOBS curves.  Curve k of posts and
+// present starts k * blob_rows rows in (blob_rows >= rows).
 __global__ void __launch_bounds__(256)
-k_floor1_interpolate(long long rows, int32_t *__restrict__ posts, const int32_t *__restrict__ fz_lo,
+k_floor1_interpolate(long long rows, long long blob_rows, int32_t *__restrict__ posts, const int32_t *__restrict__ fz_lo,
                      const int32_t *__restrict__ fz_mid, const int32_t *__restrict__ fz_hi,
                      int32_t *__restrict__ present) {
   constexpr int NB = VB200_PACKETBLOBS, MID = VB200_PACKETBLOBS / 2, S = VB200_FLOOR1_STRIDE;
@@ -39,7 +40,7 @@ k_floor1_interpolate(long long rows, int32_t *__restrict__ posts, const int32_t 
     const long long row = e / S;
     const int i = (int)(e - row * S);
     const int mid = fz_mid[row] != 0, lo = mid && fz_lo[row] != 0, hi = mid && fz_hi[row] != 0;
-    const size_t blob = (size_t)rows * S;
+    const size_t blob = (size_t)blob_rows * S;
     int32_t *p = posts + (size_t)row * S + i;
     const int a = lo ? p[0] : 0, b = mid ? p[(size_t)MID * blob] : 0, c = hi ? p[(size_t)(NB - 1) * blob] : 0;
     p[0] = a; p[(size_t)(NB - 1) * blob] = c;
@@ -63,7 +64,7 @@ k_floor1_interpolate(long long rows, int32_t *__restrict__ posts, const int32_t 
     }
     if (i == 0) {
       for (int k = 0; k < NB; k++)
-        present[(size_t)k * rows + row] = k < MID ? lo : (k == MID ? mid : hi);
+        present[(size_t)k * blob_rows + row] = k < MID ? lo : (k == MID ? mid : hi);
     }
   }
 }

@@ -21,9 +21,9 @@
  * have written for the fit (its own render into a scratch curve is redundant host work of ~n integer ops per
  * channel; the curve the residue was built from is the device's).  No reference source is restated here.
  *
- * Bitrate-managed encoders (vorbis_encode_init) take the same seam: one vb200_encode_dsp_managed call per block
- * returns all PACKETBLOBS curves and the host writes all PACKETBLOBS packets (the multi-stream driver below is
- * un-managed only).  A CUDA failure surfaces as OV_EFAULT from vorbis_analysis and latches in
+ * Bitrate-managed encoders (vorbis_encode_init) take the same path: one vb200_encode_dsp_managed call per batch
+ * returns all PACKETBLOBS curves of every block and the host writes all PACKETBLOBS packets of each (the seam is
+ * the batch of one block; vb200ms_open_managed opens a managed multi-stream driver).  A CUDA failure surfaces as OV_EFAULT from vorbis_analysis and latches in
  * the binding (vb200shim_error).  Compiled like any libvorbis-internal backend against lib/codec_internal.h
  * (oracle/Makefile target `dropin`); INTEGRATION.md shows the registry line a maintainer changes.
  */
@@ -138,36 +138,42 @@ static int pack_block(vorbis_block *vb, const int32_t *posts, const int32_t *non
 /* ---- device half for a set of blocks of ONE size ------------------------------------------------------------ */
 typedef struct {
   float *pcm; vb200_block_desc *desc; int32_t *posts, *nonzero, *iwork; float *ampmax;
-  size_t cap_blocks; int ch, N;
+  size_t cap_blocks; int ch, N, curves;
 } ms_batch;
 
-static int batch_reserve(ms_batch *B, size_t nb, int ch, int N){
-  if(B->cap_blocks >= nb && B->ch == ch && B->N == N) return 0;
+/* curves: 1 (un-managed) or PACKETBLOBS (bitrate-managed: posts / nonzero / iwork hold every curve, blob-major) */
+static int batch_reserve(ms_batch *B, size_t nb, int ch, int N, int curves){
+  if(B->cap_blocks >= nb && B->ch == ch && B->N == N && B->curves == curves) return 0;
   free(B->pcm); free(B->desc); free(B->posts); free(B->nonzero); free(B->iwork); free(B->ampmax);
   memset(B, 0, sizeof(*B));
   B->pcm = (float*)malloc(sizeof(float)*nb*ch*N);
   B->desc = (vb200_block_desc*)malloc(sizeof(vb200_block_desc)*nb);
-  B->posts = (int32_t*)malloc(sizeof(int32_t)*nb*ch*VB200_FLOOR1_STRIDE);
-  B->nonzero = (int32_t*)malloc(sizeof(int32_t)*nb*ch);
-  B->iwork = (int32_t*)malloc(sizeof(int32_t)*nb*ch*(N/2));
+  B->posts = (int32_t*)malloc(sizeof(int32_t)*curves*nb*ch*VB200_FLOOR1_STRIDE);
+  B->nonzero = (int32_t*)malloc(sizeof(int32_t)*curves*nb*ch);
+  B->iwork = (int32_t*)malloc(sizeof(int32_t)*curves*nb*ch*(N/2));
   B->ampmax = (float*)malloc(sizeof(float)*nb);
   if(!B->pcm || !B->desc || !B->posts || !B->nonzero || !B->iwork || !B->ampmax) return OV_EFAULT;
-  B->cap_blocks = nb; B->ch = ch; B->N = N;
+  B->cap_blocks = nb; B->ch = ch; B->N = N; B->curves = curves;
   return 0;
 }
 
-/* blocks[0..nb) all have vb->W == W and belong to states of ONE binding.  The staging copies and the host half
- * (bits) of different blocks are independent - different vorbis_dsp_states share nothing that is written - so
- * both loops run on all host threads; `after` (optional) is called by the thread that packed block i. */
+/* blocks[0..nb) all have vb->W == W and belong to states of ONE binding, all bitrate-managed or all not.  The
+ * staging copies and the host half (bits) of different blocks are independent - different vorbis_dsp_states share
+ * nothing that is written - so both loops run on all host threads; `after` (optional) is called by the thread that
+ * packed block i.  Bitrate-managed (lib/mapping0.c:507-573, 596-687): ONE vb200_encode_dsp_managed call gives the
+ * posts, nonzero flags and quantised residue of all PACKETBLOBS curves of every block; the host then writes
+ * packetblob[k] for every k exactly as it writes the single packet of un-managed mode, and lib/bitrate.c picks among
+ * them afterwards. */
 typedef void (*batch_after)(void *user, int i);
 static int forward_batch(vb200_binding *bind, ms_batch *B, vorbis_block **blocks, int nb, int W, batch_after after, void *user){
   vorbis_info *vi = blocks[0]->vd->vi;
-  const int ch = vi->channels, N = (int)blocks[0]->pcmend;
+  const int ch = vi->channels, N = (int)blocks[0]->pcmend, n = N/2;
+  const int managed = vorbis_bitrate_managed(blocks[0]);
   vb200_encode_io io;
   int i, c, rc;
   int err = 0;
   PROF_T0();
-  if((rc = batch_reserve(B, (size_t)nb, ch, N))) return rc;
+  if((rc = batch_reserve(B, (size_t)nb, ch, N, managed ? PACKETBLOBS : 1))) return rc;
 #pragma omp parallel for private(c) schedule(static) if(nb > 8)
   for(i = 0; i < nb; i++){
     vorbis_block_internal *vbi = (vorbis_block_internal*)blocks[i]->internal;
@@ -179,20 +185,26 @@ static int forward_batch(vb200_binding *bind, ms_batch *B, vorbis_block **blocks
   io.pcm = B->pcm; io.pcm_fmt = VB200_PCM_F32_BLOCKS; io.desc = B->desc; io.independent = 1;
   io.posts = B->posts; io.nonzero = B->nonzero; io.iwork = B->iwork; io.ampmax_out = B->ampmax;
   PROF_ADD(2);
-  rc = vb200_encode_dsp(vb200shim_ctx(bind), W, nb, 1, PACKETBLOBS/2, &io);      /* one H2D, the six kernels, one D2H */
+  rc = managed ? vb200_encode_dsp_managed(vb200shim_ctx(bind), W, nb, 1, &io)
+               : vb200_encode_dsp(vb200shim_ctx(bind), W, nb, 1, PACKETBLOBS/2, &io);   /* one H2D, the kernels, one D2H */
   PROF_ADD(3);
   if(rc){
     vb200shim_set_error(bind, rc);
-    fprintf(stderr, "vb200 mapping0: vb200_encode_dsp failed (%d): %s\n", rc, vb200_last_error());
+    fprintf(stderr, "vb200 mapping0: vb200_encode_dsp%s failed (%d): %s\n", managed ? "_managed" : "", rc, vb200_last_error());
     return OV_EFAULT;
   }
 #pragma omp parallel for schedule(dynamic, 4) if(nb > 8)
   for(i = 0; i < nb; i++){
     vorbis_block_internal *vbi = (vorbis_block_internal*)blocks[i]->internal;
-    int r;
+    int r = 0, k;
     vbi->ampmax = B->ampmax[i];                                /* lib/mapping0.c:576 */
-    r = pack_block(blocks[i], B->posts + (size_t)i*ch*VB200_FLOOR1_STRIDE, B->nonzero + (size_t)i*ch,
-                   B->iwork + (size_t)i*ch*(N/2));
+    if(!managed)
+      r = pack_block(blocks[i], B->posts + (size_t)i*ch*VB200_FLOOR1_STRIDE, B->nonzero + (size_t)i*ch,
+                     B->iwork + (size_t)i*ch*n);
+    for(k = 0; managed && k < PACKETBLOBS && !r; k++){          /* curve k of block i: row (k*nb + i)*ch */
+      const size_t r0 = ((size_t)k*nb + i)*ch;
+      r = pack_block_blob(blocks[i], k, B->posts + r0*VB200_FLOOR1_STRIDE, B->nonzero + r0, B->iwork + r0*n);
+    }
     if(r){
 #pragma omp atomic write
       err = r;
@@ -205,50 +217,9 @@ static int forward_batch(vb200_binding *bind, ms_batch *B, vorbis_block **blocks
 /* ---- seam 1: vorbis_func_mapping ---------------------------------------------------------------------------- */
 static ms_batch g_single[2];                                   /* the single-block path's staging (one per block size) */
 
-/* bitrate-managed mode (lib/mapping0.c:507-573, 596-687): ONE vb200_encode_dsp_managed call gives the posts, nonzero
- * flags and quantised residue of all PACKETBLOBS curves of the block; the host then writes packetblob[k] for every k
- * exactly as it writes the single packet of un-managed mode.  lib/bitrate.c picks among them afterwards. */
-static int forward_managed(vb200_binding *bind, vorbis_block *vb){
-  static __thread int32_t *posts, *nonzero, *iwork; static __thread float *pcm; static __thread size_t cap;
-  vorbis_info *vi = vb->vd->vi;
-  vorbis_block_internal *vbi = (vorbis_block_internal*)vb->internal;
-  const int ch = vi->channels, N = (int)vb->pcmend, n = N/2, W = (int)vb->W;
-  const size_t need = (size_t)ch*N;
-  vb200_encode_io io;
-  vb200_block_desc desc;
-  float ampmax;
-  int c, k, rc;
-  if(cap < need){
-    free(posts); free(nonzero); free(iwork); free(pcm);
-    pcm = (float*)malloc(sizeof(float)*need);
-    posts = (int32_t*)malloc(sizeof(int32_t)*PACKETBLOBS*ch*VB200_FLOOR1_STRIDE);
-    nonzero = (int32_t*)malloc(sizeof(int32_t)*PACKETBLOBS*ch);
-    iwork = (int32_t*)malloc(sizeof(int32_t)*PACKETBLOBS*ch*n);
-    cap = (pcm && posts && nonzero && iwork) ? need : 0;
-    if(!cap) return OV_EFAULT;
-  }
-  for(c = 0; c < ch; c++) memcpy(pcm + (size_t)c*N, vb->pcm[c], sizeof(float)*N);
-  desc.lW = (int32_t)vb->lW; desc.nW = (int32_t)vb->nW; desc.blocktype = vbi->blocktype; desc.ampmax = vbi->ampmax;
-  memset(&io, 0, sizeof(io));
-  io.pcm = pcm; io.pcm_fmt = VB200_PCM_F32_BLOCKS; io.desc = &desc; io.independent = 1;
-  io.posts = posts; io.nonzero = nonzero; io.iwork = iwork; io.ampmax_out = &ampmax;
-  rc = vb200_encode_dsp_managed(vb200shim_ctx(bind), W, 1, 1, &io);
-  if(rc){
-    vb200shim_set_error(bind, rc);
-    fprintf(stderr, "vb200 mapping0: vb200_encode_dsp_managed failed (%d): %s\n", rc, vb200_last_error());
-    return OV_EFAULT;
-  }
-  vbi->ampmax = ampmax;                                        /* lib/mapping0.c:576 */
-  for(k = 0; k < PACKETBLOBS; k++)
-    if((rc = pack_block_blob(vb, k, posts + (size_t)k*ch*VB200_FLOOR1_STRIDE, nonzero + (size_t)k*ch, iwork + (size_t)k*ch*n)))
-      return rc;
-  return 0;
-}
-
 static int vb200_mapping0_forward(vorbis_block *vb){
   vb200_binding *bind = vb200shim_binding(vb->vd);
   if(!bind){ fprintf(stderr, "vb200 mapping0: vorbis_dsp_state is not attached (vb200shim_attach)\n"); return OV_EFAULT; }
-  if(vorbis_bitrate_managed(vb)) return forward_managed(bind, vb);
   return forward_batch(bind, &g_single[vb->W ? 1 : 0], &vb, 1, (int)vb->W, NULL, NULL);
 }
 static void vb_pack(vorbis_info *vi, vorbis_info_mapping *vm, oggpack_buffer *opb){ mapping0_exportbundle.pack(vi, vm, opb); }
@@ -340,8 +311,10 @@ static int host_threads(void){
 #endif
 }
 
-/* N encoders of one configuration (vorbis_encode_init_vbr), all bound to one device context */
-vb200ms *vb200ms_open(int nstreams, int channels, long rate, float quality, int device){
+/* N encoders of one configuration, all bound to one device context: vorbis_encode_init_vbr(quality) or, when
+ * managed, vorbis_encode_init(max, nominal, min bitrate; -1 = unset) */
+static vb200ms *ms_open(int nstreams, int channels, long rate, float quality, int managed, long max_br, long nominal_br,
+                        long min_br, int device){
   vb200ms *m = (vb200ms*)calloc(1, sizeof(*m));
   int i, w;
   if(!m || nstreams < 1) { free(m); return NULL; }
@@ -362,7 +335,8 @@ vb200ms *vb200ms_open(int nstreams, int channels, long rate, float quality, int 
 #endif
   vorbis_comment_init(&m->vc);
   vorbis_info_init(&m->vi[0]);
-  if(vorbis_encode_init_vbr(&m->vi[0], channels, rate, quality)){ vb200ms_close(m); return NULL; }
+  if(managed ? vorbis_encode_init(&m->vi[0], channels, rate, max_br, nominal_br, min_br)
+             : vorbis_encode_init_vbr(&m->vi[0], channels, rate, quality)){ vb200ms_close(m); return NULL; }
   /* every state reads the same (read-only) setup; the first vorbis_analysis_init also builds the setup's shared
    * encode codebooks (ci->fullbooks, lib/block.c:211-224), so it runs alone, the others on all host threads
    * (each builds its own psy / floor / residue lookups, ~1.5 ms) */
@@ -376,6 +350,16 @@ vb200ms *vb200ms_open(int nstreams, int channels, long rate, float quality, int 
   if(vb200shim_attach(&m->vd[0], device)){ vb200ms_close(m); return NULL; }
   m->bind = vb200shim_binding(&m->vd[0]);
   return m;
+}
+
+vb200ms *vb200ms_open(int nstreams, int channels, long rate, float quality, int device){
+  return ms_open(nstreams, channels, rate, quality, 0, -1, -1, -1, device);
+}
+
+/* bitrate-managed encoders (CBR / ABR): each round's blocks of a size go to the device in one
+ * vb200_encode_dsp_managed call, and every stream's bitrate manager picks its packets in round_after */
+vb200ms *vb200ms_open_managed(int nstreams, int channels, long rate, long max_br, long nominal_br, long min_br, int device){
+  return ms_open(nstreams, channels, rate, 0.f, 1, max_br, nominal_br, min_br, device);
 }
 
 vorbis_dsp_state *vb200ms_state(vb200ms *m, int stream){ return &m->vd[stream]; }

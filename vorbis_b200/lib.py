@@ -36,6 +36,7 @@ EXPORTS = [
     "vb200_floor1_inverse2_dev", "vb200_floor1_inverse2", "vb200_decode_dsp_dev", "vb200_decode_dsp",
     "vb200_residue_partvals", "vb200_residue_classify_dev", "vb200_residue_classify",
     "vb200_plan_blocks", "vb200_encode_streams_dev", "vb200_encode_streams",
+    "vb200_encode_streams_managed_dev", "vb200_encode_streams_managed",
     "vb200_malloc_device", "vb200_free_device", "vb200_memcpy_h2d", "vb200_memcpy_d2h", "vb200_synchronize",
 ]
 
@@ -115,6 +116,8 @@ def load():
     L.vb200_plan_blocks.argtypes = [vp, C.c_int, vp, C.c_int64, C.c_int, vp, vp, C.c_int, vp, vp]
     L.vb200_encode_streams.argtypes = [vp, C.c_int, C.c_int, C.POINTER(abi.StreamsIO)]
     L.vb200_encode_streams_dev.argtypes = [vp, C.c_int, C.c_int, C.POINTER(abi.StreamsIO), vp]
+    L.vb200_encode_streams_managed.argtypes = [vp, C.c_int, C.POINTER(abi.StreamsIO)]
+    L.vb200_encode_streams_managed_dev.argtypes = [vp, C.c_int, C.POINTER(abi.StreamsIO), vp]
     L.vb200_malloc_device.argtypes = [vp, C.c_size_t, C.POINTER(vp)]
     L.vb200_free_device.argtypes = [vp, vp]
     L.vb200_memcpy_h2d.argtypes = [vp, vp, vp, C.c_size_t]
@@ -350,6 +353,14 @@ class Context:
     def encode_streams(self, pcm, pcm_len, eof=None, fmt=PCM_F32_PLANAR, max_blocks=None, cap=None, blobno=7):
         """pcm: timeline buffers, PCM_F32_PLANAR [streams][ch][stride] float32 or PCM_S16_INTERLEAVED
         [streams][stride][ch] int16.  Returns plan, nblocks and per block size W the batch outputs."""
+        return self._encode_streams(pcm, pcm_len, eof, fmt, max_blocks, cap, blobno, None)
+
+    def encode_streams_managed(self, pcm, pcm_len, eof=None, fmt=PCM_F32_PLANAR, max_blocks=None, cap=None):
+        """Bitrate-managed vb200_encode_streams_managed: inputs and result as encode_streams, with the per-size
+        posts / nonzero / iwork shaped [15][count][ch][...] (curve k = blob k); ampmax_out [count]."""
+        return self._encode_streams(pcm, pcm_len, eof, fmt, max_blocks, cap, 0, abi.PACKETBLOBS)
+
+    def _encode_streams(self, pcm, pcm_len, eof, fmt, max_blocks, cap, blobno, curves):
         ch = self.channels
         if fmt == PCM_F32_PLANAR:
             pcm = np.ascontiguousarray(pcm, np.float32)
@@ -373,16 +384,22 @@ class Context:
         nb = np.zeros(ns, np.int32)
         io.plan, io.nblocks = plan.ctypes.data, nb.ctypes.data
         out = {}
+        lead = () if curves is None else (curves,)
         for w in range(2):
             n = self.bs[w] // 2
             io.cap[w] = int(cap[w])
-            out[w] = {"posts": np.zeros((cap[w], ch, abi.FLOOR1_STRIDE), np.int32), "nonzero": np.zeros((cap[w], ch), np.int32),
-                      "iwork": np.zeros((cap[w], ch, n), np.int32), "ampmax_out": np.zeros(cap[w], np.float32)}
+            out[w] = {"posts": np.zeros(lead + (cap[w], ch, abi.FLOOR1_STRIDE), np.int32),
+                      "nonzero": np.zeros(lead + (cap[w], ch), np.int32),
+                      "iwork": np.zeros(lead + (cap[w], ch, n), np.int32), "ampmax_out": np.zeros(cap[w], np.float32)}
             io.posts[w], io.nonzero[w] = out[w]["posts"].ctypes.data, out[w]["nonzero"].ctypes.data
             io.iwork[w], io.ampmax_out[w] = out[w]["iwork"].ctypes.data, out[w]["ampmax_out"].ctypes.data
-        self._chk(self.L.vb200_encode_streams(self.h, ns, blobno, C.byref(io)))
+        if curves is None:
+            self._chk(self.L.vb200_encode_streams(self.h, ns, blobno, C.byref(io)))
+        else:
+            self._chk(self.L.vb200_encode_streams_managed(self.h, ns, C.byref(io)))
         for w in range(2):
-            out[w] = {k: v[:io.count[w]] for k, v in out[w].items()}
+            cnt = io.count[w]
+            out[w] = {k: (v[:cnt] if k == "ampmax_out" or curves is None else v[:, :cnt]) for k, v in out[w].items()}
         return {"plan": plan, "nblocks": nb, "count": [io.count[0], io.count[1]], 0: out[0], 1: out[1]}
 
     # ---- whole per-block encode DSP (Phase A -> floor1 -> Phase B) in one call ---------------
