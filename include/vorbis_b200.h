@@ -547,6 +547,38 @@ int vb200_decode_dsp    (vb200_ctx*, int nstreams, int nblk, const int32_t *Wseq
                          float *res, int64_t res_len, const int32_t *posts, const int32_t *present,
                          const int64_t *pcm_off, void *pcm, int pcm_s16, int64_t pcm_stride);
 
+/* ---- decode resumed across calls: vb200_decode_dsp for a decoder that receives its packets over time.
+ * The overlap state that vorbis_synthesis_blockin keeps between blocks (lib/block.c:767-823) lives in a
+ * carry, one entry per (stream, channel):
+ *   tail [nstreams][ch][blocksizes[1]/2]  the right half of that channel's last IMDCT (n_W/2 floats used;
+ *                                         n_W/4 in half-rate mode)
+ *   W    [nstreams][ch]                   that block's size flag, -1 = nothing decoded yet
+ * A new decoder starts with every W = -1.  Stream s decodes count[s] <= nblk blocks (count NULL: nblk);
+ * the Wseq, coef_off, pcm_off, posts and present entries of blocks past count[s] are not read and those
+ * blocks write nothing, and a stream with count[s] = 0 leaves its carry as it was.  Where the carried W is
+ * >= 0, block 0 overlap-adds onto the carried tail and finishes (N_W'/4 + N_W/4) samples (halved in half-rate
+ * mode) at pcm_off[s][0], W' the carried flag; where it is -1, block 0 only primes, as in vb200_decode_dsp.
+ * After the call the carry holds the last decoded block of every stream that decoded one.
+ * Contract: cutting a stream's blocks into any sequence of calls that pass the carry along gives the PCM of
+ * one vb200_decode_dsp call over all of them, bit for bit.  A carry is only valid in the mode (full or half
+ * rate) that produced it.  Otherwise layout and arguments as vb200_decode_dsp.  Two kernel launches.
+ * _dev: every pointer is device memory except `carry` itself, a host struct holding device pointers; the
+ * values of count and of the carried W are used as they are (as Wseq in vb200_decode_dsp_dev).
+ * Host form: the carry's arrays are host memory, copied in and back out.  Returns VB200_EINVAL for a null
+ * pointer, count[s] outside [0, nblk], a carried W outside {-1, 0, 1} or a counted Wseq entry outside {0, 1}. */
+typedef struct vb200_decode_carry {
+  float   *tail;
+  int32_t *W;
+} vb200_decode_carry;
+int vb200_decode_dsp_resume_dev(vb200_ctx*, int nstreams, int nblk, const int32_t *d_count, const int32_t *d_Wseq,
+                                const int64_t *d_coef_off, float *d_res, const int32_t *d_posts,
+                                const int32_t *d_present, const int64_t *d_pcm_off, void *d_pcm, int pcm_s16,
+                                int64_t pcm_stride, const vb200_decode_carry *carry, void *stream);
+int vb200_decode_dsp_resume    (vb200_ctx*, int nstreams, int nblk, const int32_t *count, const int32_t *Wseq,
+                                const int64_t *coef_off, float *res, int64_t res_len, const int32_t *posts,
+                                const int32_t *present, const int64_t *pcm_off, void *pcm, int pcm_s16,
+                                int64_t pcm_stride, vb200_decode_carry *carry);
+
 /* ---- device memory helpers for non-CUDA hosts (C callers) -------------- */
 int  vb200_malloc_device(vb200_ctx*, size_t bytes, void **dptr);
 int  vb200_free_device  (vb200_ctx*, void *dptr);

@@ -185,6 +185,15 @@ class StreamsIO(C.Structure):
     ]
 
 
+class DecodeCarry(C.Structure):
+    """vb200_decode_carry (include/vorbis_b200.h): tail [nstreams][ch][blocksizes[1]/2] float32, W [nstreams][ch]
+    int32 (-1 = nothing decoded yet)"""
+    _fields_ = [
+        ("tail", C.c_void_p),
+        ("W", C.c_void_p),
+    ]
+
+
 _PSY_SCALARS = [
     "n", "blockflag", "ath_adjatt", "ath_maxatt", "tone_abs_limit", "noisemaxsupp",
     "noisewindowfixed", "max_curve_dB", "normal_p", "normal_start", "normal_partition",

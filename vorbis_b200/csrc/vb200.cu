@@ -884,12 +884,19 @@ struct SinkS16 {
   }
 };
 
-template <bool S16, bool HS>
-__global__ void __launch_bounds__(256)
-k_synthesis(XformDev X0, XformDev X1, WinDev Wd, int ch, int nstreams, int nblk,
-            const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
-            const float *__restrict__ coef, const long long *__restrict__ pcm_off,
-            void *__restrict__ pcm_out, long long pcm_stride) {
+// CARRY (vb200_decode_dsp_resume): stream st decodes count[st] <= nblk blocks, and the overlap of every
+// (stream, channel) = task comes from / goes back to carry_W[task] and carry_tail[task * tail_stride]: the
+// block flag and the right half of the last IMDCT (what v->pcm holds after lib/block.c:817-823).  With a
+// carried W >= 0, block 0 overlap-adds onto that tail and finishes samples like any later block; with -1 it
+// only primes.  A stream with count 0 is not touched.  W is kept per (stream, channel) because the CTA of
+// one channel must not read what the CTA of another channel of the same stream writes.
+template <bool S16, bool HS, bool CARRY>
+__device__ __forceinline__ void
+synthesis_body(const XformDev &X0, const XformDev &X1, const WinDev &Wd, int ch, int nstreams, int nblk,
+               const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
+               const float *__restrict__ coef, const long long *__restrict__ pcm_off,
+               void *__restrict__ pcm_out, long long pcm_stride, const int *__restrict__ count,
+               float *__restrict__ carry_tail, int *__restrict__ carry_W, int tail_stride) {
   extern __shared__ __align__(16) float sm[];
   const int tid = threadIdx.x, nt = blockDim.x;
   const int n0 = X0.N >> 1, n1 = X1.N >> 1;
@@ -899,7 +906,20 @@ k_synthesis(XformDev X0, XformDev X1, WinDev Wd, int ch, int nstreams, int nblk,
   for (int task = blockIdx.x; task < nstreams * ch; task += gridDim.x) {
     const int st = task / ch, c = task - st * ch;
     int lW = 0;
-    for (int k = 0; k < nblk; k++) {
+    int cnt = nblk, first_out = 1;
+    if constexpr (CARRY) {
+      if (count) cnt = min(max(count[st], 0), nblk);
+      if (cnt == 0) continue;
+      const int cw = carry_W[task];
+      if (cw >= 0) {
+        // the loads finish before block 0's first __syncthreads; s_prev is read only after it
+        lW = cw ? 1 : 0;
+        first_out = 0;
+        const float *t = carry_tail + (size_t)task * tail_stride;
+        for (int i = tid; i < ((lW ? X1.N : X0.N) >> 1); i += nt) s_prev[i] = t[i];
+      }
+    }
+    for (int k = 0; k < cnt; k++) {
       const int W = Wseq[(size_t)st * nblk + k];
       const XformDev &X = W ? X1 : X0;
       const int N = X.N, n2 = N >> 1;
@@ -908,7 +928,7 @@ k_synthesis(XformDev X0, XformDev X1, WinDev Wd, int ch, int nstreams, int nblk,
       for (int i = tid; i < (n2 >> 2); i += nt) reinterpret_cast<float4 *>(s_in)[i] = __ldg(src + i);
       __syncthreads();
       dev_mdct_backward<0>(X, s_in, s_out, tid, nt);
-      if (k > 0) {
+      if (k >= first_out) {
         const long long o = pcm_off[(size_t)st * nblk + k];
         typename std::conditional<S16, SinkS16, SinkF32>::type dst;
         if constexpr (S16) {
@@ -935,7 +955,34 @@ k_synthesis(XformDev X0, XformDev X1, WinDev Wd, int ch, int nstreams, int nblk,
       lW = W;
       __syncthreads();
     }
+    if constexpr (CARRY) {
+      float *t = carry_tail + (size_t)task * tail_stride;
+      for (int i = tid; i < ((lW ? X1.N : X0.N) >> 1); i += nt) t[i] = s_prev[i];
+      if (tid == 0) carry_W[task] = lW;
+      __syncthreads();                 // the next task's carry-in overwrites s_prev
+    }
   }
+}
+
+template <bool S16, bool HS>
+__global__ void __launch_bounds__(256)
+k_synthesis(XformDev X0, XformDev X1, WinDev Wd, int ch, int nstreams, int nblk,
+            const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
+            const float *__restrict__ coef, const long long *__restrict__ pcm_off,
+            void *__restrict__ pcm_out, long long pcm_stride) {
+  synthesis_body<S16, HS, false>(X0, X1, Wd, ch, nstreams, nblk, Wseq, coef_off, coef, pcm_off, pcm_out, pcm_stride,
+                                 nullptr, nullptr, nullptr, 0);
+}
+
+template <bool S16, bool HS>
+__global__ void __launch_bounds__(256)
+k_synthesis_carry(XformDev X0, XformDev X1, WinDev Wd, int ch, int nstreams, int nblk,
+                  const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
+                  const float *__restrict__ coef, const long long *__restrict__ pcm_off,
+                  void *__restrict__ pcm_out, long long pcm_stride, const int *__restrict__ count,
+                  float *__restrict__ carry_tail, int *__restrict__ carry_W, int tail_stride) {
+  synthesis_body<S16, HS, true>(X0, X1, Wd, ch, nstreams, nblk, Wseq, coef_off, coef, pcm_off, pcm_out, pcm_stride,
+                                count, carry_tail, carry_W, tail_stride);
 }
 
 // ---- decode: undo channel coupling, lib/mapping0.c:754-779 (square polar -> L/R), in place
@@ -2486,6 +2533,20 @@ extern "C" int vb200_floor1_inverse2(vb200_ctx *c, int W, int floor_sel, int nro
   return io.sync();
 }
 
+static int decode_prep_args(vb200_ctx *c, int nstreams, int nblk, DecodePrepArgs *A) {
+  const int ch = c->setup.channels;
+  for (int w = 0; w < 2; w++) {
+    for (int k = 0; k < ch; k++)
+      if (c->setup.floor1[w][c->setup.chmux[w][k]].posts <= 0)
+        return fail(VB200_EINVAL, "no floor1 setup for a channel's submap");
+    A->floors[w] = c->d_floor[w]; A->chmux[w] = c->d_chmux[w];
+    A->mag[w] = c->d_mag[w]; A->ang[w] = c->d_ang[w];
+    A->steps[w] = c->setup.coupling_steps[w]; A->n[w] = c->dx[w].N / 2;
+  }
+  A->ch = ch; A->nblk = nblk; A->nitems = (long)nstreams * nblk;
+  return 0;
+}
+
 extern "C" int vb200_decode_dsp_dev(vb200_ctx *c, int nstreams, int nblk, const int32_t *d_Wseq, const int64_t *d_coef_off,
                                     float *d_res, const int32_t *d_posts, const int32_t *d_present,
                                     const int64_t *d_pcm_off, void *d_pcm, int pcm_s16, int64_t pcm_stride, void *stream) {
@@ -2493,18 +2554,9 @@ extern "C" int vb200_decode_dsp_dev(vb200_ctx *c, int nstreams, int nblk, const 
   if (nstreams <= 0 || nblk <= 0) return 0;
   if (!d_Wseq || !d_coef_off || !d_res || !d_posts || !d_present || !d_pcm_off || !d_pcm)
     return fail(VB200_EINVAL, "decode pointers");
-  const int ch = c->setup.channels;
   DecodePrepArgs A;
-  for (int w = 0; w < 2; w++) {
-    for (int k = 0; k < ch; k++)
-      if (c->setup.floor1[w][c->setup.chmux[w][k]].posts <= 0)
-        return fail(VB200_EINVAL, "no floor1 setup for a channel's submap");
-    A.floors[w] = c->d_floor[w]; A.chmux[w] = c->d_chmux[w];
-    A.mag[w] = c->d_mag[w]; A.ang[w] = c->d_ang[w];
-    A.steps[w] = c->setup.coupling_steps[w]; A.n[w] = c->dx[w].N / 2;
-  }
-  A.ch = ch; A.nblk = nblk; A.nitems = (long)nstreams * nblk;
   int rc;
+  if ((rc = decode_prep_args(c, nstreams, nblk, &A))) return rc;
   k_decode_prepare<<<grid_for(c, (int)A.nitems, 8), 128, 0, (cudaStream_t)stream>>>(
       A, d_Wseq, (const long long *)d_coef_off, d_res, d_posts, d_present, c->d_fromdB);
   if ((rc = post_launch(c))) return rc;
@@ -2537,6 +2589,93 @@ extern "C" int vb200_decode_dsp(vb200_ctx *c, int nstreams, int nblk, const int3
                                  (const int32_t *)dps, (const int32_t *)dpr, (const int64_t *)dpo, dp, pcm_s16,
                                  pcm_stride, c->s_main))) return rc;
   if ((rc = io.d2h(pcm, dp, pbytes))) return rc;
+  return io.sync();
+}
+
+// ---- decode resumed across calls: the overlap of every (stream, channel) carried in vb200_decode_carry
+template <bool S16, bool HS>
+static int synthesis_carry_launch(vb200_ctx *c, int nstreams, int nblk, const int32_t *d_count, const int32_t *d_Wseq,
+                                  const int64_t *d_coef_off, const float *d_coef, const int64_t *d_pcm_off,
+                                  void *d_pcm, int64_t pcm_stride, const vb200_decode_carry *k, void *stream) {
+  const XformDev *X = HS ? c->dx_hs : c->dx;
+  const int ch = c->setup.channels, N1 = X[1].N;
+  const size_t smem = sizeof(float) * ((size_t)N1 / 2 + N1 + N1 / 2);
+  int rc = set_smem(k_synthesis_carry<S16, HS>, smem); if (rc) return rc;
+  k_synthesis_carry<S16, HS><<<grid_for(c, nstreams * ch, 8), threads_for(N1), smem, (cudaStream_t)stream>>>(
+      X[0], X[1], HS ? c->dwin_hs : c->dwin, ch, nstreams, nblk, d_Wseq, (const long long *)d_coef_off, d_coef,
+      (const long long *)d_pcm_off, d_pcm, (long long)pcm_stride, d_count, k->tail, k->W, c->setup.blocksizes[1] / 2);
+  return post_launch(c);
+}
+
+extern "C" int vb200_decode_dsp_resume_dev(vb200_ctx *c, int nstreams, int nblk, const int32_t *d_count,
+                                           const int32_t *d_Wseq, const int64_t *d_coef_off, float *d_res,
+                                           const int32_t *d_posts, const int32_t *d_present, const int64_t *d_pcm_off,
+                                           void *d_pcm, int pcm_s16, int64_t pcm_stride,
+                                           const vb200_decode_carry *d_carry, void *stream) {
+  CHECK_CTX(c);
+  if (nstreams <= 0 || nblk <= 0) return 0;
+  if (!d_Wseq || !d_coef_off || !d_res || !d_posts || !d_present || !d_pcm_off || !d_pcm || !d_carry ||
+      !d_carry->tail || !d_carry->W)
+    return fail(VB200_EINVAL, "decode pointers");
+  DecodePrepArgs A;
+  int rc;
+  if ((rc = decode_prep_args(c, nstreams, nblk, &A))) return rc;
+  if (d_count)
+    k_decode_prepare_counted<<<grid_for(c, (int)A.nitems, 8), 128, 0, (cudaStream_t)stream>>>(
+        A, d_Wseq, (const long long *)d_coef_off, d_res, d_posts, d_present, c->d_fromdB, d_count);
+  else
+    k_decode_prepare<<<grid_for(c, (int)A.nitems, 8), 128, 0, (cudaStream_t)stream>>>(
+        A, d_Wseq, (const long long *)d_coef_off, d_res, d_posts, d_present, c->d_fromdB);
+  if ((rc = post_launch(c))) return rc;
+  const bool hs = c->halfrate;
+  if (pcm_s16)
+    return hs ? synthesis_carry_launch<true, true>(c, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_pcm_off, d_pcm, pcm_stride, d_carry, stream)
+              : synthesis_carry_launch<true, false>(c, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_pcm_off, d_pcm, pcm_stride, d_carry, stream);
+  return hs ? synthesis_carry_launch<false, true>(c, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_pcm_off, d_pcm, pcm_stride, d_carry, stream)
+            : synthesis_carry_launch<false, false>(c, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_pcm_off, d_pcm, pcm_stride, d_carry, stream);
+}
+
+extern "C" int vb200_decode_dsp_resume(vb200_ctx *c, int nstreams, int nblk, const int32_t *count, const int32_t *Wseq,
+                                       const int64_t *coef_off, float *res, int64_t res_len, const int32_t *posts,
+                                       const int32_t *present, const int64_t *pcm_off, void *pcm, int pcm_s16,
+                                       int64_t pcm_stride, vb200_decode_carry *carry) {
+  CHECK_CTX(c);
+  if (nstreams <= 0 || nblk <= 0) return 0;
+  if (!Wseq || !coef_off || !res || !posts || !present || !pcm_off || !pcm || !carry || !carry->tail || !carry->W)
+    return fail(VB200_EINVAL, "decode pointers");
+  const int ch = c->setup.channels;
+  const size_t nb = (size_t)nstreams * nblk, ntask = (size_t)nstreams * ch;
+  for (int s = 0; s < nstreams; s++) {
+    const int n = count ? count[s] : nblk;
+    if (n < 0 || n > nblk) return fail(VB200_EINVAL, "count[s] must be in [0, nblk]");
+    for (int k = 0; k < n; k++)
+      if (Wseq[(size_t)s * nblk + k] < 0 || Wseq[(size_t)s * nblk + k] > 1) return fail(VB200_EINVAL, "Wseq values must be 0/1");
+  }
+  for (size_t i = 0; i < ntask; i++)
+    if (carry->W[i] < -1 || carry->W[i] > 1) return fail(VB200_EINVAL, "carried W must be -1, 0 or 1");
+  std::lock_guard<std::mutex> lk(c->mu);
+  const size_t tbytes = sizeof(float) * ntask * (size_t)(c->setup.blocksizes[1] / 2);
+  HostIO io{c};
+  void *dW, *dco, *dc, *dpo, *dp, *dps, *dpr, *dn = nullptr, *dkt, *dkw; int rc;
+  if ((rc = io.h2d(Wseq, sizeof(int32_t) * nb, &dW))) return rc;
+  if ((rc = io.h2d(coef_off, sizeof(int64_t) * nb, &dco))) return rc;
+  if ((rc = io.h2d(res, sizeof(float) * (size_t)res_len, &dc))) return rc;
+  if ((rc = io.h2d(pcm_off, sizeof(int64_t) * nb, &dpo))) return rc;
+  const size_t pbytes = (pcm_s16 ? sizeof(int16_t) : sizeof(float)) * (size_t)nstreams * ch * (size_t)pcm_stride;
+  if ((rc = io.h2d(nullptr, pbytes, &dp))) return rc;
+  if ((rc = io.h2d(posts, sizeof(int32_t) * nb * ch * VB200_FLOOR1_STRIDE, &dps))) return rc;
+  if ((rc = io.h2d(present, sizeof(int32_t) * nb * ch, &dpr))) return rc;
+  if (count && (rc = io.h2d(count, sizeof(int32_t) * nstreams, &dn))) return rc;
+  if ((rc = io.h2d(carry->tail, tbytes, &dkt))) return rc;
+  if ((rc = io.h2d(carry->W, sizeof(int32_t) * ntask, &dkw))) return rc;
+  CU(cudaMemsetAsync(dp, 0, pbytes, c->s_main));
+  const vb200_decode_carry dk{(float *)dkt, (int32_t *)dkw};
+  if ((rc = vb200_decode_dsp_resume_dev(c, nstreams, nblk, (const int32_t *)dn, (const int32_t *)dW,
+                                        (const int64_t *)dco, (float *)dc, (const int32_t *)dps, (const int32_t *)dpr,
+                                        (const int64_t *)dpo, dp, pcm_s16, pcm_stride, &dk, c->s_main))) return rc;
+  if ((rc = io.d2h(pcm, dp, pbytes))) return rc;
+  if ((rc = io.d2h(carry->tail, dkt, tbytes))) return rc;
+  if ((rc = io.d2h(carry->W, dkw, sizeof(int32_t) * ntask))) return rc;
   return io.sync();
 }
 

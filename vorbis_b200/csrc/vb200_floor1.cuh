@@ -507,10 +507,13 @@ struct DecodePrepArgs {
   long nitems;                         // nstreams * nblk
 };
 
-__global__ void __launch_bounds__(128)
-k_decode_prepare(DecodePrepArgs A, const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
-                 float *__restrict__ res, const int32_t *__restrict__ posts, const int32_t *__restrict__ present,
-                 const float *__restrict__ fromdB) {
+// COUNTED (vb200_decode_dsp_resume): item it = (stream it / nblk, block it % nblk) is skipped when the block
+// lies past count[stream]
+template <bool COUNTED>
+__device__ __forceinline__ void
+decode_prepare_body(const DecodePrepArgs &A, const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
+                    float *__restrict__ res, const int32_t *__restrict__ posts, const int32_t *__restrict__ present,
+                    const float *__restrict__ fromdB, const int *__restrict__ count) {
   __shared__ Floor1Dev sF[2][VB200_MAX_SUBMAPS];
   __shared__ short s_segx[4][VB200_VIF_POSIT + 3];
   __shared__ short s_segy[4][VB200_VIF_POSIT + 3];
@@ -523,6 +526,8 @@ k_decode_prepare(DecodePrepArgs A, const int *__restrict__ Wseq, const long long
   __syncthreads();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   for (long it = blockIdx.x; it < A.nitems; it += gridDim.x) {
+    if constexpr (COUNTED)
+      if ((int)it % A.nblk >= count[(int)it / A.nblk]) continue;   // nitems fits an int (grid_for)
     const int W = Wseq[it] ? 1 : 0, n = A.n[W];
     float *base = res + coef_off[it];
     for (int j = threadIdx.x; j < n; j += blockDim.x) {
@@ -546,4 +551,19 @@ k_decode_prepare(DecodePrepArgs A, const int *__restrict__ Wseq, const long long
     }
     __syncthreads();
   }
+}
+
+__global__ void __launch_bounds__(128)
+k_decode_prepare(DecodePrepArgs A, const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
+                 float *__restrict__ res, const int32_t *__restrict__ posts, const int32_t *__restrict__ present,
+                 const float *__restrict__ fromdB) {
+  decode_prepare_body<false>(A, Wseq, coef_off, res, posts, present, fromdB, nullptr);
+}
+
+__global__ void __launch_bounds__(128)
+k_decode_prepare_counted(DecodePrepArgs A, const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
+                         float *__restrict__ res, const int32_t *__restrict__ posts,
+                         const int32_t *__restrict__ present, const float *__restrict__ fromdB,
+                         const int *__restrict__ count) {
+  decode_prepare_body<true>(A, Wseq, coef_off, res, posts, present, fromdB, count);
 }

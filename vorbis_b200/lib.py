@@ -34,6 +34,7 @@ EXPORTS = [
     "vb200_encode_dsp_dev", "vb200_encode_dsp", "vb200_encode_dsp_managed_dev", "vb200_encode_dsp_managed",
     "vb200_envelope_search_dev", "vb200_envelope_search", "vb200_envelope_search_var", "vb200_envelope_apply_marks",
     "vb200_floor1_inverse2_dev", "vb200_floor1_inverse2", "vb200_decode_dsp_dev", "vb200_decode_dsp",
+    "vb200_decode_dsp_resume_dev", "vb200_decode_dsp_resume",
     "vb200_residue_partvals", "vb200_residue_classify_dev", "vb200_residue_classify",
     "vb200_plan_blocks", "vb200_encode_streams_dev", "vb200_encode_streams",
     "vb200_encode_streams_managed_dev", "vb200_encode_streams_managed",
@@ -109,6 +110,10 @@ def load():
     L.vb200_floor1_inverse2.argtypes = [vp, C.c_int, C.c_int, C.c_int, vp, vp, vp]
     L.vb200_decode_dsp_dev.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int64, vp]
     L.vb200_decode_dsp.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, C.c_int64, vp, vp, vp, vp, C.c_int, C.c_int64]
+    L.vb200_decode_dsp_resume_dev.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int, C.c_int64,
+                                              C.POINTER(abi.DecodeCarry), vp]
+    L.vb200_decode_dsp_resume.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int64, vp, vp, vp, vp, C.c_int,
+                                          C.c_int64, C.POINTER(abi.DecodeCarry)]
     L.vb200_envelope_search_dev.argtypes = [vp, C.c_int, vp, C.c_int, C.c_int64, C.c_int, C.c_int, vp, vp, vp]
     L.vb200_envelope_search.argtypes = [vp, C.c_int, vp, C.c_int, C.c_int64, C.c_int, C.c_int, vp, vp]
     L.vb200_envelope_apply_marks.argtypes = [vp, C.c_int, C.c_int, vp]
@@ -539,6 +544,43 @@ class Context:
                                           pcm_stride))
         return pcm
 
+    def new_decode_carry(self, nstreams):
+        """the overlap state of nstreams fresh decoders for decode_dsp_resume: (tail, W)"""
+        return (np.zeros((nstreams, self.channels, self.bs[1] // 2), np.float32),
+                np.full((nstreams, self.channels), -1, np.int32))
+
+    def decode_dsp_resume(self, Wseq, coef_off, res, posts, present, pcm_off, pcm_stride, carry, count=None,
+                          s16=False):
+        """vb200_decode_dsp_resume: decode_dsp that continues each stream from carry = (tail, W) (new_decode_carry)
+        and leaves the overlap of its last decoded block there, in place.  count [nstreams]: blocks per stream
+        (None = all).  Offsets from synthesis_layout(..., carry_W=carry[1], count=count)."""
+        Wseq = np.ascontiguousarray(Wseq, np.int32)
+        ns, nblk = Wseq.shape
+        tail, W = carry
+        assert tail.dtype == np.float32 and W.dtype == np.int32 and tail.flags.c_contiguous and W.flags.c_contiguous
+        assert tail.shape == (ns, self.channels, self.bs[1] // 2) and W.shape == (ns, self.channels)
+        res = np.array(res, np.float32)
+        posts = np.ascontiguousarray(posts, np.int32)
+        present = np.ascontiguousarray(present, np.int32)
+        coef_off = np.ascontiguousarray(coef_off, np.int64)
+        pcm_off = np.ascontiguousarray(pcm_off, np.int64)
+        count = None if count is None else np.ascontiguousarray(count, np.int32)
+        pcm = (np.zeros((ns, pcm_stride, self.channels), np.int16) if s16
+               else np.zeros((ns, self.channels, pcm_stride), np.float32))
+        k = abi.DecodeCarry(tail.ctypes.data, W.ctypes.data)
+        self._chk(self.L.vb200_decode_dsp_resume(self.h, ns, nblk, _ptr(count), _ptr(Wseq), _ptr(coef_off), _ptr(res),
+                                                 res.size, _ptr(posts), _ptr(present), _ptr(pcm_off), _ptr(pcm),
+                                                 1 if s16 else 0, pcm_stride, C.byref(k)))
+        return pcm
+
+    def decode_dsp_resume_dev(self, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_posts, d_present, d_pcm_off,
+                              d_pcm, pcm_s16, pcm_stride, d_tail, d_W, stream=None):
+        k = abi.DecodeCarry(_ptr(d_tail), _ptr(d_W))
+        self._chk(self.L.vb200_decode_dsp_resume_dev(self.h, nstreams, nblk, _ptr(d_count), _ptr(d_Wseq),
+                                                     _ptr(d_coef_off), _ptr(d_res), _ptr(d_posts), _ptr(d_present),
+                                                     _ptr(d_pcm_off), _ptr(d_pcm), pcm_s16, pcm_stride, C.byref(k),
+                                                     _ptr(stream)))
+
     # ---- envelope / block-switch detector (lib/envelope.c) --------------------------------------
     def envelope_search(self, pcm, first_step, nsteps, state=None, fmt=PCM_F32_PLANAR):
         """Host buffers.  pcm: float [streams][ch][stride] (PCM_F32_PLANAR) or int16 [streams][stride][ch].
@@ -601,20 +643,31 @@ class Context:
                                              _ptr(d_pcm_off), _ptr(d_pcm), pcm_stride, _ptr(stream)))
 
 
-def synthesis_layout(Wseq, bs, channels, halfrate=False):
+def synthesis_layout(Wseq, bs, channels, halfrate=False, carry_W=None, count=None):
     """Offsets for vb200_synthesis: Wseq [nstreams][nblk] -> (coef_off, pcm_off, coef_len, pcm_len)
     with every stream's spectra packed back to back (block-major, channel-minor).  halfrate: the spectra
     keep this layout, the finished samples are counted at half rate ((bs[lW]/4 + bs[W]/4) >> 1 per block,
-    lib/block.c:840-842)."""
+    lib/block.c:840-842).
+    For vb200_decode_dsp_resume: carry_W [nstreams] or [nstreams][ch] = the carried block flags (-1 = none):
+    where one is >= 0, block 0 finishes samples as well; count [nstreams]: blocks past count[s] get no spectra
+    and finish nothing."""
     Wseq = np.asarray(Wseq, np.int32)
     ns, nblk = Wseq.shape
     N = np.where(Wseq == 1, bs[1], bs[0]).astype(np.int64)
+    if count is not None:
+        N = np.where(np.arange(nblk)[None, :] < np.asarray(count).reshape(ns, 1), N, 0)
     per_block = channels * (N // 2)
     coef_off = np.zeros((ns, nblk), np.int64)
     flat = per_block.reshape(-1)
     coef_off.reshape(-1)[1:] = np.cumsum(flat)[:-1]
     fin = np.zeros((ns, nblk), np.int64)
-    fin[:, 1:] = (N[:, :-1] // 4 + N[:, 1:] // 4) >> (1 if halfrate else 0)
+    fin[:, 1:] = np.where(N[:, 1:] > 0, N[:, :-1] // 4 + N[:, 1:] // 4, 0) >> (1 if halfrate else 0)
+    if carry_W is not None:
+        cw = np.asarray(carry_W).reshape(ns, -1)
+        assert (cw == cw[:, :1]).all(), "the carried W of a stream differs between its channels"
+        cw = cw[:, 0]
+        fin[:, 0] = np.where((cw >= 0) & (N[:, 0] > 0), np.where(cw == 1, bs[1], bs[0]) // 4 + N[:, 0] // 4, 0) >> (
+            1 if halfrate else 0)
     pcm_off = np.cumsum(fin, axis=1) - fin      # finished samples before block k's contribution
     # block k's finished samples start where block k-1's ended
     pcm_off = np.concatenate([np.zeros((ns, 1), np.int64), np.cumsum(fin, axis=1)[:, :-1]], axis=1)
