@@ -579,6 +579,97 @@ int vb200_decode_dsp_resume    (vb200_ctx*, int nstreams, int nblk, const int32_
                                 const int32_t *present, const int64_t *pcm_off, void *pcm, int pcm_s16,
                                 int64_t pcm_stride, vb200_decode_carry *carry);
 
+/* ---- decode: the entropy half of mapping0_inverse (lib/mapping0.c:714-751) on the device.
+ * What floor1_inverse1 (lib/floor1.c:955-1039) and the residue inverse of types 1 and 2 (lib/res0.c:651-711,
+ * 812-864) read, in a plain form registered on a context with vb200_decode_entropy_setup.
+ *
+ * vb200_codebook: one codebook as vorbis_book_decode sees it.  Codeword i has length length[i] (1..32) and the
+ * bits bits[i], the first bit of the stream in bit 0 (what oggpack_read(length[i]) returns when the codeword is
+ * next); vorbis_book_decode returns entry[i] for it, and the residue adds value[i*dim .. i*dim+dim) (NULL for a
+ * book without a value mapping).  used == 0: a book with no codelist, for which vorbis_book_decode returns -1
+ * and the residue adds read nothing (lib/codebook.c:389-403, 428-443, 472-495).                               */
+typedef struct vb200_codebook {
+  int32_t dim;                     /* elements per vector, 1..127                    */
+  int32_t used;                    /* codewords                                      */
+  const uint8_t  *length;          /* [used]                                         */
+  const uint32_t *bits;            /* [used]                                         */
+  const int32_t  *entry;           /* [used]                                         */
+  const float    *value;           /* [used][dim] or NULL                            */
+} vb200_codebook;
+
+/* the decode fields of vorbis_info_floor1 (lib/backends.h:60-68); the posts and mult come from the context's
+ * vb200_floor1_setup of the same (W, submap) */
+typedef struct vb200_floor_decode {
+  int32_t type;                    /* the floor type; only 1 is taken (else VB200_EIMPL) */
+  int32_t partitions;              /* 0..31                                          */
+  int32_t partitionclass[31];      /* 0..15                                          */
+  int32_t class_dim[16];           /* 1..8                                           */
+  int32_t class_subs[16];          /* 0..3                                           */
+  int32_t class_book[16];          /* read where class_subs > 0                      */
+  int32_t class_subbook[16][8];    /* -1 = none                                      */
+} vb200_floor_decode;
+
+/* the decode fields of vorbis_info_residue0 (lib/backends.h:103-118) with its stage books laid out as res0_look
+ * lays them out (lib/res0.c:274-299): stagebook[class][s] for the ilog(secondstages) stages of each class, -1
+ * where a stage bit is clear */
+typedef struct vb200_residue_decode {
+  int32_t type;                    /* 1 or 2 (0: VB200_EIMPL); -1 = submap not used  */
+  int32_t begin, end, grouping;
+  int32_t partitions;              /* classes, 1..64                                 */
+  int32_t partvals;                /* partitions ^ dim(groupbook)                    */
+  int32_t groupbook;
+  int32_t stagebook[64][8];
+} vb200_residue_decode;
+
+typedef struct vb200_entropy_setup {
+  int32_t nbooks;
+  const vb200_codebook *books;     /* [nbooks], ci->decbooks                         */
+  int32_t modebits;                /* bits of the mode number (private_state.modebits) */
+  vb200_floor_decode   floor[2][VB200_MAX_SUBMAPS];     /* [W][submap], submaps[W] used */
+  vb200_residue_decode residue[2][VB200_MAX_SUBMAPS];
+} vb200_entropy_setup;
+
+/* Copies everything and builds the device lookup tables.  Returns VB200_EINVAL for inconsistent input (a code
+ * that is not a complete prefix code, except the single-entry length-1 book; a book index out of range; a
+ * residue range or grouping that does not fit the block; partition counts that do not match the floor's posts)
+ * and VB200_EIMPL for residue type 0 or a floor that is not type 1.  Replaces an earlier registration.  After it,
+ * no value read from a packet can index outside a table or a row.                                             */
+int vb200_decode_entropy_setup(vb200_ctx*, const vb200_entropy_setup*);
+
+/* The entropy half of mapping0_inverse for nblocks packets, into the staging layout of vb200_decode_dsp:
+ *   Wseq [nblocks]        block flag of each packet (its header already parsed by the caller)
+ *   pkt_off [nblocks] int64, pkt_bytes [nblocks] int32: packet i is data[pkt_off[i] .. pkt_off[i]+pkt_bytes[i])
+ *   res  at coef_off[i] + c*n_W/2: channel c's residue vector, zeroed and then decoded (n_W/2 floats)
+ *   posts [nblocks][ch][VB200_FLOOR1_STRIDE]: fit_value as floor1_inverse1 returns it, zeros past the posts
+ *         and in absent rows; present [nblocks][ch]: 0 where floor1_inverse1 returned NULL.
+ * Decoding starts at bit 1 + modebits + (W ? 2 : 0).  Damaged and truncated packets decode as the reference
+ * decodes them.  One kernel launch.  Host form: data_bytes and res_len give the sizes of data and res; returns
+ * VB200_EINVAL for a null pointer, a packet outside data, a Wseq entry outside {0, 1} or a row outside res.  */
+int vb200_decode_entropy_dev(vb200_ctx*, int nblocks, const int32_t *d_Wseq, const int64_t *d_pkt_off,
+                             const int32_t *d_pkt_bytes, const uint8_t *d_data, const int64_t *d_coef_off,
+                             float *d_res, int32_t *d_posts, int32_t *d_present, void *stream);
+int vb200_decode_entropy    (vb200_ctx*, int nblocks, const int32_t *Wseq, const int64_t *pkt_off,
+                             const int32_t *pkt_bytes, const uint8_t *data, int64_t data_bytes,
+                             const int64_t *coef_off, float *res, int64_t res_len, int32_t *posts, int32_t *present);
+
+/* vb200_decode_dsp_resume from the packets: the entropy decode fused in front of the de-coupling and floor
+ * multiply, then the IMDCT and overlap-add.  Arguments as vb200_decode_dsp_resume with the packets (pkt_off,
+ * pkt_bytes, data, indexed like Wseq) in place of posts / present; res is scratch laid out by coef_off.
+ * Contract: the PCM and the carry equal vb200_decode_entropy followed by vb200_decode_dsp_resume, bit for bit,
+ * at full and half rate.  Two kernel launches.  Needs a registered vb200_decode_entropy_setup (else
+ * VB200_EINVAL).  _dev: checks its pointers only.  Host form: res_len floats of scratch are allocated on the
+ * device; returns VB200_EINVAL as vb200_decode_dsp_resume does and for a packet outside data (data_bytes).   */
+int vb200_decode_packets_resume_dev(vb200_ctx*, int nstreams, int nblk, const int32_t *d_count,
+                                    const int32_t *d_Wseq, const int64_t *d_coef_off, float *d_res,
+                                    const int64_t *d_pkt_off, const int32_t *d_pkt_bytes, const uint8_t *d_data,
+                                    const int64_t *d_pcm_off, void *d_pcm, int pcm_s16, int64_t pcm_stride,
+                                    const vb200_decode_carry *carry, void *stream);
+int vb200_decode_packets_resume    (vb200_ctx*, int nstreams, int nblk, const int32_t *count, const int32_t *Wseq,
+                                    const int64_t *coef_off, int64_t res_len, const int64_t *pkt_off,
+                                    const int32_t *pkt_bytes, const uint8_t *data, int64_t data_bytes,
+                                    const int64_t *pcm_off, void *pcm, int pcm_s16, int64_t pcm_stride,
+                                    vb200_decode_carry *carry);
+
 /* ---- device memory helpers for non-CUDA hosts (C callers) -------------- */
 int  vb200_malloc_device(vb200_ctx*, size_t bytes, void **dptr);
 int  vb200_free_device  (vb200_ctx*, void *dptr);

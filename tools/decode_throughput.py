@@ -1,7 +1,8 @@
 #!/usr/bin/env python
 """Decode throughput of many streams: the stock decoder (vorbis_synthesis -> blockin -> pcmout) on all host threads
 against the multi-stream decode driver (vb200md_*, vorbis_b200/host/vb200_decode.c) fed 1, 4 and 16 packets per
-stream per round.  Default workload: 1000 streams of 44.1 kHz stereo at q = 0.5, 30 s each (8 distinct encoded
+stream per round, on its device path (packets decoded by vb200_decode_packets_resume_dev) and on the forced host
+entropy path (vb200md_set_host_entropy).  Default workload: 1000 streams of 44.1 kHz stereo at q = 0.5, 30 s each (8 distinct encoded
 streams, repeated).  Prints one JSON line per configuration and the GPU's name and power limit read in the same run.
 
 usage: python tools/decode_throughput.py [--streams 1000] [--seconds 30] [--distinct 8] [--out DIR]
@@ -20,6 +21,7 @@ ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 
 from oracle import decode  # noqa: E402
+from oracle import decode_packets  # noqa: E402
 
 
 def gpu_identity():
@@ -44,7 +46,7 @@ def main():
     ap.add_argument("--distinct", type=int, default=8)
     ap.add_argument("--out", default=None, help="also write the JSON lines to DIR/decode_throughput.jsonl")
     a = ap.parse_args()
-    if not decode.available():
+    if not (decode.available() and decode_packets.available()):
         sys.exit("oracle/_ref/libvorbis_{ref,dropin}_decode.so not built")
     ch, rate, q = 2, 44100, 0.5
     enc = [decode.encode(ch, rate, q, signal(ch, rate, a.seconds, seed=i)) for i in range(a.distinct)]
@@ -73,16 +75,19 @@ def main():
         sched = np.full((1, a.streams), per, np.int32)
         rounds = int(np.ceil(joined[4].max() / per)) + 1
         sched = np.repeat(sched, rounds, axis=0)
-        t0 = time.perf_counter()
-        _, st = decode.md_run(joined, sched, ch, keep=False)
-        dt = time.perf_counter() - t0
-        n = int(st["samples"].sum())
-        assert n == samples, "driver samples %d != stock %d" % (n, samples)
-        lines.append(dict(ident, config="vb200md, %d packets per stream per round" % per, streams=a.streams,
-                          packets=packets, seconds=dt, packets_per_s=packets / dt, samples_per_s=n / dt,
-                          rounds=st["rounds"], device_ms_per_round=1e3 * st["device_s"] / st["rounds"],
-                          host_ms_per_round=1e3 * st["host_s"] / st["rounds"],
-                          launches_per_round=st["launches"] / st["rounds"]))
+        for host in (False, True):
+            t0 = time.perf_counter()
+            _, st = decode_packets.md_run(joined, sched, ch, host_entropy=host, keep=False)
+            dt = time.perf_counter() - t0
+            n = int(st["samples"].sum())
+            assert n == samples, "driver samples %d != stock %d" % (n, samples)
+            assert st["entropy_on_device"] == (not host)
+            lines.append(dict(ident, config="vb200md %s path, %d packets per stream per round"
+                              % ("host" if host else "device", per), streams=a.streams,
+                              packets=packets, seconds=dt, packets_per_s=packets / dt, samples_per_s=n / dt,
+                              rounds=st["rounds"], device_ms_per_round=1e3 * st["device_s"] / st["rounds"],
+                              host_ms_per_round=1e3 * st["host_s"] / st["rounds"],
+                              launches_per_round=st["launches"] / st["rounds"]))
     for ln in lines:
         print(json.dumps(ln))
     if a.out:

@@ -185,6 +185,56 @@ class StreamsIO(C.Structure):
     ]
 
 
+class Codebook(C.Structure):
+    """vb200_codebook (include/vorbis_b200.h)"""
+    _fields_ = [
+        ("dim", C.c_int32),
+        ("used", C.c_int32),
+        ("length", C.c_void_p),
+        ("bits", C.c_void_p),
+        ("entry", C.c_void_p),
+        ("value", C.c_void_p),
+    ]
+
+
+class FloorDecode(C.Structure):
+    """vb200_floor_decode"""
+    _fields_ = [
+        ("type", C.c_int32),
+        ("partitions", C.c_int32),
+        ("partitionclass", C.c_int32 * 31),
+        ("class_dim", C.c_int32 * 16),
+        ("class_subs", C.c_int32 * 16),
+        ("class_book", C.c_int32 * 16),
+        ("class_subbook", (C.c_int32 * 8) * 16),
+    ]
+
+
+class ResidueDecode(C.Structure):
+    """vb200_residue_decode"""
+    _fields_ = [
+        ("type", C.c_int32),
+        ("begin", C.c_int32),
+        ("end", C.c_int32),
+        ("grouping", C.c_int32),
+        ("partitions", C.c_int32),
+        ("partvals", C.c_int32),
+        ("groupbook", C.c_int32),
+        ("stagebook", (C.c_int32 * 8) * 64),
+    ]
+
+
+class EntropySetup(C.Structure):
+    """vb200_entropy_setup"""
+    _fields_ = [
+        ("nbooks", C.c_int32),
+        ("books", C.POINTER(Codebook)),
+        ("modebits", C.c_int32),
+        ("floor", (FloorDecode * MAX_SUBMAPS) * 2),
+        ("residue", (ResidueDecode * MAX_SUBMAPS) * 2),
+    ]
+
+
 class DecodeCarry(C.Structure):
     """vb200_decode_carry (include/vorbis_b200.h): tail [nstreams][ch][blocksizes[1]/2] float32, W [nstreams][ch]
     int32 (-1 = nothing decoded yet)"""

@@ -101,6 +101,9 @@ struct vb200_ctx {
   const Floor1Dev *d_floor[2] = {nullptr, nullptr};   // [VB200_MAX_SUBMAPS] per block size
   const unsigned char *d_chmux[2] = {nullptr, nullptr};
   cudaStream_t s_main = nullptr;
+  // vb200_decode_entropy_setup: the device tables of the entropy decoders (ent.books == nullptr: none registered)
+  EntDev ent{};
+  std::vector<void *> ent_owned;
   std::mutex mu;
   // optional per-kernel timing of the last Phase-A call (bench roofline evidence)
   bool profiling = false;
@@ -420,6 +423,7 @@ extern "C" void vb200_ctx_destroy(vb200_ctx *c) {
   if (c->s_main) cudaStreamDestroy(c->s_main);
   for (auto &e : c->ev) if (e) cudaEventDestroy(e);
   if (c->ev_scratch) cudaEventDestroy(c->ev_scratch);
+  for (void *p : c->ent_owned) cudaFree(p);
   delete c;
 }
 
@@ -2673,6 +2677,372 @@ extern "C" int vb200_decode_dsp_resume(vb200_ctx *c, int nstreams, int nblk, con
   if ((rc = vb200_decode_dsp_resume_dev(c, nstreams, nblk, (const int32_t *)dn, (const int32_t *)dW,
                                         (const int64_t *)dco, (float *)dc, (const int32_t *)dps, (const int32_t *)dpr,
                                         (const int64_t *)dpo, dp, pcm_s16, pcm_stride, &dk, c->s_main))) return rc;
+  if ((rc = io.d2h(pcm, dp, pbytes))) return rc;
+  if ((rc = io.d2h(carry->tail, dkt, tbytes))) return rc;
+  if ((rc = io.d2h(carry->W, dkw, sizeof(int32_t) * ntask))) return rc;
+  return io.sync();
+}
+
+// ---- decode: the entropy half of mapping0_inverse on the device (vb200_entropy.cuh)
+static const int ENT_FIRST_BITS = 10, ENT_SUB_BITS = 8;
+static const size_t ENT_SMEM_MAX = 160 * 1024;
+
+static int ilog_u(unsigned v) { int r = 0; while (v) { r++; v >>= 1; } return r; }
+
+// the table of codewords cws (of book b) past their first `consumed` bits, k bits wide, appended to tab; base:
+// where the book's tables start.  False where two codewords claim one index or an index stays empty.
+static bool ent_fill(const vb200_codebook &b, const std::vector<int> &cws, int consumed, int k, size_t base,
+                     std::vector<uint32_t> &tab) {
+  const size_t at = tab.size();
+  tab.resize(at + ((size_t)1 << k), 0u);
+  std::vector<std::vector<int>> sub((size_t)1 << k);
+  for (int i : cws) {
+    const int len = b.length[i] - consumed;
+    const uint32_t bits = b.bits[i] >> consumed;
+    if (len <= k) {
+      for (uint32_t j = 0; j < (1u << (k - len)); j++) {
+        const size_t slot = at + ((bits & ((1u << len) - 1)) | (j << len));
+        if (tab[slot]) return false;
+        tab[slot] = ((uint32_t)i << 6) | (uint32_t)b.length[i];
+      }
+    } else {
+      sub[bits & ((1u << k) - 1)].push_back(i);
+    }
+  }
+  for (size_t v = 0; v < sub.size(); v++) {
+    if (sub[v].empty()) continue;
+    if (tab[at + v]) return false;
+    int longest = 0;
+    for (int i : sub[v]) longest = std::max(longest, b.length[i] - consumed - k);
+    const int sk = std::min(longest, ENT_SUB_BITS);
+    const size_t off = tab.size() - base;
+    if (off >= ((size_t)1 << 26)) return false;
+    tab[at + v] = 0x80000000u | ((uint32_t)off << 5) | (uint32_t)sk;
+    if (!ent_fill(b, sub[v], consumed + k, sk, base, tab)) return false;
+  }
+  for (size_t v = 0; v < sub.size(); v++) if (!tab[at + v]) return false;
+  return true;
+}
+
+static int ent_book(const vb200_codebook &b, EntBook &d, std::vector<uint32_t> &tab, std::vector<float> &vec,
+                    std::vector<int> &ent) {
+  memset(&d, 0, sizeof(d));
+  if (b.dim < 1 || b.dim > 127 || b.used < 0 || b.used >= (1 << 24)) return fail(VB200_EINVAL, "codebook dim / used");
+  d.dim = b.dim; d.used = b.used;
+  if (b.used == 0) return 0;
+  if (!b.length || !b.bits || !b.entry) return fail(VB200_EINVAL, "codebook arrays");
+  unsigned long long kraft = 0;
+  int longest = 0;
+  for (int i = 0; i < b.used; i++) {
+    const int len = b.length[i];
+    if (len < 1 || len > 32 || (len < 32 && (b.bits[i] >> len)) || b.entry[i] < 0)
+      return fail(VB200_EINVAL, "codeword length / bits / entry");
+    kraft += 1ull << (32 - len);
+    longest = std::max(longest, len);
+  }
+  d.tab_off = (int)tab.size(); d.ent_off = (int)ent.size(); d.vec_off = (int)vec.size();
+  if (tab.size() > (1u << 30) || vec.size() + (size_t)b.used * b.dim > (1u << 30)) return fail(VB200_EINVAL, "codebooks too large");
+  if (b.used == 1 && b.length[0] == 1) {          // the single-entry book reads one bit whatever its value
+    d.k = 1;
+    tab.push_back(1u); tab.push_back(1u);
+  } else {
+    if (kraft != (1ull << 32)) return fail(VB200_EINVAL, "codebook is not a complete prefix code");
+    std::vector<int> all(b.used);
+    for (int i = 0; i < b.used; i++) all[i] = i;
+    d.k = std::min(longest, ENT_FIRST_BITS);
+    if (!ent_fill(b, all, 0, d.k, tab.size(), tab)) return fail(VB200_EINVAL, "codebook is not a prefix code");
+  }
+  for (int i = 0; i < b.used; i++) ent.push_back(b.entry[i]);
+  if (b.value) vec.insert(vec.end(), b.value, b.value + (size_t)b.used * b.dim);
+  else d.vec_off = -1;
+  return 0;
+}
+
+extern "C" int vb200_decode_entropy_setup(vb200_ctx *c, const vb200_entropy_setup *es) {
+  CHECK_CTX(c);
+  if (!es || es->nbooks < 0 || (es->nbooks > 0 && !es->books)) return fail(VB200_EINVAL, "entropy setup");
+  if (es->modebits < 0 || es->modebits > 8) return fail(VB200_EINVAL, "modebits");
+  const vb200_setup &S = c->setup;
+  const int nb = es->nbooks, ch = S.channels;
+  std::vector<EntBook> books(nb > 0 ? nb : 1);
+  std::vector<uint32_t> tab;
+  std::vector<float> vec;
+  std::vector<int> ent;
+  int rc;
+  for (int i = 0; i < nb; i++)
+    if ((rc = ent_book(es->books[i], books[i], tab, vec, ent))) return rc;
+  auto book_ok = [&](int b) { return b >= 0 && b < nb; };
+  EntFloor hf[2][VB200_MAX_SUBMAPS];
+  EntRes hr[2][VB200_MAX_SUBMAPS];
+  memset(hf, 0, sizeof(hf));
+  memset(hr, 0, sizeof(hr));
+  size_t cls_cap = 1;
+  for (int w = 0; w < 2; w++) {
+    const int n = S.blocksizes[w] / 2, subs = S.submaps[w];
+    if (subs < 1) return fail(VB200_EINVAL, "no submaps in the context setup");
+    for (int k = 0; k < ch; k++)
+      if (S.chmux[w][k] >= subs) return fail(VB200_EINVAL, "chmux past submaps");
+    for (int sm = 0; sm < VB200_MAX_SUBMAPS; sm++) hr[w][sm].type = -1;
+    for (int sm = 0; sm < subs; sm++) {
+      const vb200_floor_decode &f = es->floor[w][sm];
+      const vb200_floor1_setup &f1 = S.floor1[w][sm];
+      EntFloor &F = hf[w][sm];
+      if (f.type != 1) return fail(VB200_EIMPL, "only floor type 1 decodes on the device");
+      if (f1.posts <= 0) return fail(VB200_EINVAL, "no floor1 setup for a submap");
+      if (f.partitions < 0 || f.partitions > 31) return fail(VB200_EINVAL, "floor partitions");
+      int posts = 2;
+      for (int i = 0; i < f.partitions; i++) {
+        const int cl = f.partitionclass[i];
+        if (cl < 0 || cl > 15) return fail(VB200_EINVAL, "floor partition class");
+        posts += f.class_dim[cl];
+      }
+      if (posts != f1.posts) return fail(VB200_EINVAL, "floor partitions do not give the floor's posts");
+      F.partitions = f.partitions; F.posts = f1.posts;
+      static const int quant_q[4] = {256, 128, 86, 64};
+      F.quant_q = quant_q[f1.mult - 1]; F.qbits = ilog_u((unsigned)F.quant_q - 1);
+      for (int i = 0; i < f.partitions; i++) F.pclass[i] = (unsigned char)f.partitionclass[i];
+      for (int cl = 0; cl < 16; cl++) {
+        for (int j = 0; j < 8; j++) F.subbook[cl][j] = -1;
+        bool used = false;
+        for (int i = 0; i < f.partitions; i++) used |= f.partitionclass[i] == cl;
+        if (!used) continue;
+        if (f.class_dim[cl] < 1 || f.class_dim[cl] > 8 || f.class_subs[cl] < 0 || f.class_subs[cl] > 3)
+          return fail(VB200_EINVAL, "floor class dim / subs");
+        if (f.class_subs[cl] && !book_ok(f.class_book[cl])) return fail(VB200_EINVAL, "floor class book");
+        F.cdim[cl] = (unsigned char)f.class_dim[cl]; F.csubs[cl] = (unsigned char)f.class_subs[cl];
+        F.cbook[cl] = (short)(f.class_subs[cl] ? f.class_book[cl] : 0);
+        for (int j = 0; j < (1 << f.class_subs[cl]); j++) {
+          const int b = f.class_subbook[cl][j];
+          if (b != -1 && !book_ok(b)) return fail(VB200_EINVAL, "floor subclass book");
+          F.subbook[cl][j] = (short)b;
+        }
+      }
+      const vb200_residue_decode &r = es->residue[w][sm];
+      EntRes &R = hr[w][sm];
+      if (r.type == 0) return fail(VB200_EIMPL, "residue type 0 does not decode on the device");
+      if (r.type != 1 && r.type != 2) return fail(VB200_EINVAL, "residue type");
+      int bundle = 0;
+      for (int k = 0; k < ch; k++) bundle += S.chmux[w][k] == sm;
+      const long limit = r.type == 2 ? (long)bundle * n : n;
+      if (r.grouping < 1 || r.begin < 0 || r.end < r.begin || r.begin > limit)
+        return fail(VB200_EINVAL, "residue begin / end / grouping do not fit the block");
+      if (r.partitions < 1 || r.partitions > 64 || !book_ok(r.groupbook)) return fail(VB200_EINVAL, "residue partitions / groupbook");
+      const int ppw = es->books[r.groupbook].dim;
+      long long pv = 1;
+      for (int j = 0; j < ppw && pv <= (1ll << 31); j++) pv *= r.partitions;
+      if (pv != r.partvals) return fail(VB200_EINVAL, "residue partvals != partitions ^ dim(groupbook)");
+      R.type = r.type; R.begin = r.begin; R.end = r.end; R.grouping = r.grouping; R.partvals = r.partvals;
+      R.groupbook = r.groupbook; R.ppw = ppw; R.partitions = r.partitions; R.stages = 0;
+      for (int cl = 0; cl < 64; cl++)
+        for (int st = 0; st < 8; st++) {
+          const int b = cl < r.partitions ? r.stagebook[cl][st] : -1;
+          if (b != -1 && !book_ok(b)) return fail(VB200_EINVAL, "residue stage book");
+          if (b >= 0 && es->books[b].used > 0 && !es->books[b].value)
+            return fail(VB200_EINVAL, "residue stage book without values");
+          R.stagebook[cl][st] = (short)b;
+          if (b >= 0) R.stages = std::max(R.stages, st + 1);
+        }
+      const long end = std::min((long)r.end, limit);
+      const size_t need = (size_t)((end - r.begin) / r.grouping) * (r.type == 2 ? 1 : bundle);
+      cls_cap = std::max(cls_cap, need);
+    }
+  }
+  const size_t smem = sizeof(int32_t) * (size_t)ch * (VB200_FLOOR1_STRIDE + 1) + 2 * (size_t)ch + cls_cap;
+  if (smem > ENT_SMEM_MAX) return fail(VB200_EIMPL, "partition classes of a block exceed the shared memory");
+  std::lock_guard<std::mutex> lk(c->mu);
+  CU(cudaStreamSynchronize(c->s_main));
+  for (void *p : c->ent_owned) cudaFree(p);
+  c->ent_owned.clear();
+  c->ent = EntDev{};
+  auto up = [&](const void *src, size_t bytes, const void **dst) -> int {
+    void *d = nullptr;
+    CU(cudaMalloc(&d, bytes ? bytes : 4));
+    c->ent_owned.push_back(d);
+    if (bytes) CU(cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice));
+    *dst = d;
+    return 0;
+  };
+  EntDev E{};
+  const void *p;
+  if ((rc = up(books.data(), sizeof(EntBook) * books.size(), &p))) return rc;
+  E.books = (const EntBook *)p;
+  if ((rc = up(tab.data(), sizeof(uint32_t) * tab.size(), &p))) return rc;
+  E.tab = (const uint32_t *)p;
+  if ((rc = up(vec.data(), sizeof(float) * vec.size(), &p))) return rc;
+  E.vec = (const float *)p;
+  if ((rc = up(ent.data(), sizeof(int) * ent.size(), &p))) return rc;
+  E.ent = (const int *)p;
+  for (int w = 0; w < 2; w++) {
+    if ((rc = up(hf[w], sizeof(hf[w]), &p))) return rc;
+    E.floor[w] = (const EntFloor *)p;
+    if ((rc = up(hr[w], sizeof(hr[w]), &p))) return rc;
+    E.res[w] = (const EntRes *)p;
+    E.chmux[w] = c->d_chmux[w]; E.mag[w] = c->d_mag[w]; E.ang[w] = c->d_ang[w];
+    E.steps[w] = S.coupling_steps[w]; E.submaps[w] = S.submaps[w]; E.n[w] = S.blocksizes[w] / 2;
+  }
+  E.ch = ch; E.modebits = es->modebits; E.cls_cap = (int)cls_cap;
+  c->ent = E;
+  return 0;
+}
+
+static size_t entropy_smem(const EntDev &E, bool fused) {
+  return (fused ? sizeof(int32_t) * (size_t)E.ch * (VB200_FLOOR1_STRIDE + 1) : 0) + 2 * (size_t)E.ch + E.cls_cap;
+}
+
+extern "C" int vb200_decode_entropy_dev(vb200_ctx *c, int nblocks, const int32_t *d_Wseq, const int64_t *d_pkt_off,
+                                        const int32_t *d_pkt_bytes, const uint8_t *d_data, const int64_t *d_coef_off,
+                                        float *d_res, int32_t *d_posts, int32_t *d_present, void *stream) {
+  CHECK_CTX(c);
+  if (nblocks <= 0) return 0;
+  if (!d_Wseq || !d_pkt_off || !d_pkt_bytes || !d_data || !d_coef_off || !d_res || !d_posts || !d_present)
+    return fail(VB200_EINVAL, "decode_entropy pointers");
+  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
+  const size_t smem = entropy_smem(c->ent, false);
+  int rc = set_smem(k_decode_entropy, smem); if (rc) return rc;
+  const DecodePackets P{(const long long *)d_pkt_off, d_pkt_bytes, d_data};
+  k_decode_entropy<<<grid_for(c, nblocks, 16), 32, smem, (cudaStream_t)stream>>>(
+      c->ent, c->d_floor[0], c->d_floor[1], P, nblocks, d_Wseq, (const long long *)d_coef_off, d_res, d_posts,
+      d_present);
+  return post_launch(c);
+}
+
+// host-form checks of the packet arrays: every counted packet inside data
+static int packets_check(const int64_t *pkt_off, const int32_t *pkt_bytes, int64_t data_bytes, size_t i) {
+  if (pkt_bytes[i] < 0 || pkt_off[i] < 0 || pkt_off[i] > data_bytes || pkt_bytes[i] > data_bytes - pkt_off[i])
+    return fail(VB200_EINVAL, "packet outside data");
+  return 0;
+}
+
+extern "C" int vb200_decode_entropy(vb200_ctx *c, int nblocks, const int32_t *Wseq, const int64_t *pkt_off,
+                                    const int32_t *pkt_bytes, const uint8_t *data, int64_t data_bytes,
+                                    const int64_t *coef_off, float *res, int64_t res_len, int32_t *posts,
+                                    int32_t *present) {
+  CHECK_CTX(c);
+  if (nblocks <= 0) return 0;
+  if (!Wseq || !pkt_off || !pkt_bytes || !data || !coef_off || !res || !posts || !present || data_bytes < 0)
+    return fail(VB200_EINVAL, "decode_entropy pointers");
+  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
+  const int ch = c->setup.channels;
+  int rc;
+  for (int i = 0; i < nblocks; i++) {
+    if (Wseq[i] < 0 || Wseq[i] > 1) return fail(VB200_EINVAL, "Wseq values must be 0/1");
+    if ((rc = packets_check(pkt_off, pkt_bytes, data_bytes, i))) return rc;
+    if (coef_off[i] < 0 || coef_off[i] + (int64_t)ch * (c->setup.blocksizes[Wseq[i]] / 2) > res_len)
+      return fail(VB200_EINVAL, "block rows outside res");
+  }
+  std::lock_guard<std::mutex> lk(c->mu);
+  const size_t nb = (size_t)nblocks;
+  HostIO io{c};
+  void *dW, *dpo, *dpb, *dd, *dco, *dr, *dps, *dpr;
+  if ((rc = io.h2d(Wseq, sizeof(int32_t) * nb, &dW))) return rc;
+  if ((rc = io.h2d(pkt_off, sizeof(int64_t) * nb, &dpo))) return rc;
+  if ((rc = io.h2d(pkt_bytes, sizeof(int32_t) * nb, &dpb))) return rc;
+  if ((rc = io.h2d(nullptr, (size_t)data_bytes + 1, &dd))) return rc;
+  if (data_bytes) CU(cudaMemcpyAsync(dd, data, (size_t)data_bytes, cudaMemcpyHostToDevice, c->s_main));
+  if ((rc = io.h2d(coef_off, sizeof(int64_t) * nb, &dco))) return rc;
+  if ((rc = io.h2d(res, sizeof(float) * (size_t)res_len, &dr))) return rc;
+  if ((rc = io.h2d(nullptr, sizeof(int32_t) * nb * ch * VB200_FLOOR1_STRIDE, &dps))) return rc;
+  if ((rc = io.h2d(nullptr, sizeof(int32_t) * nb * ch, &dpr))) return rc;
+  if ((rc = vb200_decode_entropy_dev(c, nblocks, (const int32_t *)dW, (const int64_t *)dpo, (const int32_t *)dpb,
+                                     (const uint8_t *)dd, (const int64_t *)dco, (float *)dr, (int32_t *)dps,
+                                     (int32_t *)dpr, c->s_main))) return rc;
+  if ((rc = io.d2h(res, dr, sizeof(float) * (size_t)res_len))) return rc;
+  if ((rc = io.d2h(posts, dps, sizeof(int32_t) * nb * ch * VB200_FLOOR1_STRIDE))) return rc;
+  if ((rc = io.d2h(present, dpr, sizeof(int32_t) * nb * ch))) return rc;
+  return io.sync();
+}
+
+// CTAs per SM of k_decode_packets' grid.  One thread of each CTA decodes a packet serially while the others wait,
+// but the kernel takes 80 registers (-Xptxas -v, sm_90a), so at most 6 CTAs of 128 threads are resident per SM;
+// a grid of more than k_decode_prepare's 8 per SM would only queue
+static const int DECODE_PACKETS_CTAS = 8;
+
+extern "C" int vb200_decode_packets_resume_dev(vb200_ctx *c, int nstreams, int nblk, const int32_t *d_count,
+                                               const int32_t *d_Wseq, const int64_t *d_coef_off, float *d_res,
+                                               const int64_t *d_pkt_off, const int32_t *d_pkt_bytes,
+                                               const uint8_t *d_data, const int64_t *d_pcm_off, void *d_pcm,
+                                               int pcm_s16, int64_t pcm_stride, const vb200_decode_carry *d_carry,
+                                               void *stream) {
+  CHECK_CTX(c);
+  if (nstreams <= 0 || nblk <= 0) return 0;
+  if (!d_Wseq || !d_coef_off || !d_res || !d_pkt_off || !d_pkt_bytes || !d_data || !d_pcm_off || !d_pcm || !d_carry ||
+      !d_carry->tail || !d_carry->W)
+    return fail(VB200_EINVAL, "decode pointers");
+  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
+  DecodePrepArgs A;
+  int rc;
+  if ((rc = decode_prep_args(c, nstreams, nblk, &A))) return rc;
+  const size_t smem = entropy_smem(c->ent, true);
+  const DecodePackets P{(const long long *)d_pkt_off, d_pkt_bytes, d_data};
+  const int grid = grid_for(c, (int)A.nitems, DECODE_PACKETS_CTAS);
+  if (d_count) {
+    if ((rc = set_smem(k_decode_packets<true>, smem))) return rc;
+    k_decode_packets<true><<<grid, 128, smem, (cudaStream_t)stream>>>(A, c->ent, P, d_Wseq, (const long long *)d_coef_off,
+                                                                      d_res, c->d_fromdB, d_count);
+  } else {
+    if ((rc = set_smem(k_decode_packets<false>, smem))) return rc;
+    k_decode_packets<false><<<grid, 128, smem, (cudaStream_t)stream>>>(A, c->ent, P, d_Wseq, (const long long *)d_coef_off,
+                                                                       d_res, c->d_fromdB, nullptr);
+  }
+  if ((rc = post_launch(c))) return rc;
+  const bool hs = c->halfrate;
+  if (pcm_s16)
+    return hs ? synthesis_carry_launch<true, true>(c, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_pcm_off, d_pcm, pcm_stride, d_carry, stream)
+              : synthesis_carry_launch<true, false>(c, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_pcm_off, d_pcm, pcm_stride, d_carry, stream);
+  return hs ? synthesis_carry_launch<false, true>(c, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_pcm_off, d_pcm, pcm_stride, d_carry, stream)
+            : synthesis_carry_launch<false, false>(c, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_pcm_off, d_pcm, pcm_stride, d_carry, stream);
+}
+
+extern "C" int vb200_decode_packets_resume(vb200_ctx *c, int nstreams, int nblk, const int32_t *count,
+                                           const int32_t *Wseq, const int64_t *coef_off, int64_t res_len,
+                                           const int64_t *pkt_off, const int32_t *pkt_bytes, const uint8_t *data,
+                                           int64_t data_bytes, const int64_t *pcm_off, void *pcm, int pcm_s16,
+                                           int64_t pcm_stride, vb200_decode_carry *carry) {
+  CHECK_CTX(c);
+  if (nstreams <= 0 || nblk <= 0) return 0;
+  if (!Wseq || !coef_off || !pkt_off || !pkt_bytes || !data || !pcm_off || !pcm || !carry || !carry->tail ||
+      !carry->W || data_bytes < 0 || res_len < 0)
+    return fail(VB200_EINVAL, "decode pointers");
+  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
+  const int ch = c->setup.channels;
+  const size_t nb = (size_t)nstreams * nblk, ntask = (size_t)nstreams * ch;
+  int rc;
+  for (int s = 0; s < nstreams; s++) {
+    const int n = count ? count[s] : nblk;
+    if (n < 0 || n > nblk) return fail(VB200_EINVAL, "count[s] must be in [0, nblk]");
+    for (int k = 0; k < n; k++) {
+      const size_t i = (size_t)s * nblk + k;
+      if (Wseq[i] < 0 || Wseq[i] > 1) return fail(VB200_EINVAL, "Wseq values must be 0/1");
+      if ((rc = packets_check(pkt_off, pkt_bytes, data_bytes, i))) return rc;
+      if (coef_off[i] < 0 || coef_off[i] + (int64_t)ch * (c->setup.blocksizes[Wseq[i]] / 2) > res_len)
+        return fail(VB200_EINVAL, "block rows outside res");
+    }
+  }
+  for (size_t i = 0; i < ntask; i++)
+    if (carry->W[i] < -1 || carry->W[i] > 1) return fail(VB200_EINVAL, "carried W must be -1, 0 or 1");
+  std::lock_guard<std::mutex> lk(c->mu);
+  const size_t tbytes = sizeof(float) * ntask * (size_t)(c->setup.blocksizes[1] / 2);
+  HostIO io{c};
+  void *dW, *dco, *dc, *dpo, *dp, *dko, *dkb, *dd, *dn = nullptr, *dkt, *dkw;
+  if ((rc = io.h2d(Wseq, sizeof(int32_t) * nb, &dW))) return rc;
+  if ((rc = io.h2d(coef_off, sizeof(int64_t) * nb, &dco))) return rc;
+  if ((rc = io.h2d(nullptr, sizeof(float) * (size_t)(res_len ? res_len : 1), &dc))) return rc;
+  if ((rc = io.h2d(pcm_off, sizeof(int64_t) * nb, &dpo))) return rc;
+  const size_t pbytes = (pcm_s16 ? sizeof(int16_t) : sizeof(float)) * (size_t)nstreams * ch * (size_t)pcm_stride;
+  if ((rc = io.h2d(nullptr, pbytes, &dp))) return rc;
+  if ((rc = io.h2d(pkt_off, sizeof(int64_t) * nb, &dko))) return rc;
+  if ((rc = io.h2d(pkt_bytes, sizeof(int32_t) * nb, &dkb))) return rc;
+  if ((rc = io.h2d(nullptr, (size_t)data_bytes + 1, &dd))) return rc;
+  if (data_bytes) CU(cudaMemcpyAsync(dd, data, (size_t)data_bytes, cudaMemcpyHostToDevice, c->s_main));
+  if (count && (rc = io.h2d(count, sizeof(int32_t) * nstreams, &dn))) return rc;
+  if ((rc = io.h2d(carry->tail, tbytes, &dkt))) return rc;
+  if ((rc = io.h2d(carry->W, sizeof(int32_t) * ntask, &dkw))) return rc;
+  CU(cudaMemsetAsync(dp, 0, pbytes, c->s_main));
+  const vb200_decode_carry dk{(float *)dkt, (int32_t *)dkw};
+  if ((rc = vb200_decode_packets_resume_dev(c, nstreams, nblk, (const int32_t *)dn, (const int32_t *)dW,
+                                            (const int64_t *)dco, (float *)dc, (const int64_t *)dko,
+                                            (const int32_t *)dkb, (const uint8_t *)dd, (const int64_t *)dpo, dp,
+                                            pcm_s16, pcm_stride, &dk, c->s_main))) return rc;
   if ((rc = io.d2h(pcm, dp, pbytes))) return rc;
   if ((rc = io.d2h(carry->tail, dkt, tbytes))) return rc;
   if ((rc = io.d2h(carry->W, dkw, sizeof(int32_t) * ntask))) return rc;

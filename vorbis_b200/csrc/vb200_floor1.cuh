@@ -495,6 +495,8 @@ k_floor1_inverse2(Floor1Args a, const int32_t *__restrict__ posts, const int32_t
   }
 }
 
+#include "vb200_entropy.cuh"
+
 // ---- decode, fused front half of mapping0_inverse for packed mixed-size streams: one CTA per
 // (stream, block): channel de-coupling (lib/mapping0.c:754-779, last step first) then the floor
 // multiply of every channel (:781-790), in place on the residue vectors; k_synthesis follows.
@@ -507,13 +509,24 @@ struct DecodePrepArgs {
   long nitems;                         // nstreams * nblk
 };
 
+// the packets of the ENTROPY instances: item it is data[off[it] .. off[it] + bytes[it])
+struct DecodePackets {
+  const long long *off;
+  const int *bytes;
+  const unsigned char *data;
+};
+
 // COUNTED (vb200_decode_dsp_resume): item it = (stream it / nblk, block it % nblk) is skipped when the block
 // lies past count[stream]
-template <bool COUNTED>
+// ENTROPY (vb200_decode_packets_resume): the CTA zero-fills the block's rows, one thread decodes its packet
+// (ent_block) with the posts and presence in shared memory, then the de-coupling and floor multiply read them
+// from there; posts / present are not read.  Dynamic shared memory: entropy_smem(E).
+template <bool COUNTED, bool ENTROPY = false>
 __device__ __forceinline__ void
 decode_prepare_body(const DecodePrepArgs &A, const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
                     float *__restrict__ res, const int32_t *__restrict__ posts, const int32_t *__restrict__ present,
-                    const float *__restrict__ fromdB, const int *__restrict__ count) {
+                    const float *__restrict__ fromdB, const int *__restrict__ count,
+                    const EntDev *E = nullptr, DecodePackets P = DecodePackets{}) {
   __shared__ Floor1Dev sF[2][VB200_MAX_SUBMAPS];
   __shared__ short s_segx[4][VB200_VIF_POSIT + 3];
   __shared__ short s_segy[4][VB200_VIF_POSIT + 3];
@@ -530,6 +543,19 @@ decode_prepare_body(const DecodePrepArgs &A, const int *__restrict__ Wseq, const
       if ((int)it % A.nblk >= count[(int)it / A.nblk]) continue;   // nitems fits an int (grid_for)
     const int W = Wseq[it] ? 1 : 0, n = A.n[W];
     float *base = res + coef_off[it];
+    if constexpr (ENTROPY) {
+      extern __shared__ __align__(16) unsigned char ent_smem[];
+      int32_t *s_posts = reinterpret_cast<int32_t *>(ent_smem), *s_present = s_posts + A.ch * VB200_FLOOR1_STRIDE;
+      for (int j = threadIdx.x; j < A.ch * n; j += blockDim.x) base[j] = 0.f;
+      for (int j = threadIdx.x; j < A.ch * VB200_FLOOR1_STRIDE; j += blockDim.x) s_posts[j] = 0;
+      __syncthreads();
+      if (threadIdx.x == 0) {
+        unsigned char *nz = reinterpret_cast<unsigned char *>(s_present + A.ch);
+        ent_block(*E, sF[W], W, P.data + P.off[it], P.bytes[it], base, s_posts, s_present, nz, nz + A.ch,
+                  nz + 2 * A.ch);
+      }
+      __syncthreads();
+    }
     for (int j = threadIdx.x; j < n; j += blockDim.x) {
       for (int s = A.steps[W] - 1; s >= 0; s--) {
         float *pM = base + (size_t)A.mag[W][s] * n + j, *pA = base + (size_t)A.ang[W][s] * n + j;
@@ -545,9 +571,17 @@ decode_prepare_body(const DecodePrepArgs &A, const int *__restrict__ Wseq, const
     }
     __syncthreads();
     for (int c = warp; c < A.ch; c += 4) {
-      const size_t row = (size_t)it * A.ch + c;
-      dev_floor1_inverse2_row(sF[W][A.chmux[W][c]], posts + row * VB200_FLOOR1_STRIDE, present[row] != 0,
-                              base + (size_t)c * n, n, fromdB, s_segx[warp], s_segy[warp], lane);
+      if constexpr (ENTROPY) {
+        extern __shared__ __align__(16) unsigned char ent_smem[];
+        const int32_t *s_posts = reinterpret_cast<const int32_t *>(ent_smem);
+        dev_floor1_inverse2_row(sF[W][A.chmux[W][c]], s_posts + (size_t)c * VB200_FLOOR1_STRIDE,
+                                s_posts[A.ch * VB200_FLOOR1_STRIDE + c] != 0, base + (size_t)c * n, n, fromdB,
+                                s_segx[warp], s_segy[warp], lane);
+      } else {
+        const size_t row = (size_t)it * A.ch + c;
+        dev_floor1_inverse2_row(sF[W][A.chmux[W][c]], posts + row * VB200_FLOOR1_STRIDE, present[row] != 0,
+                                base + (size_t)c * n, n, fromdB, s_segx[warp], s_segy[warp], lane);
+      }
     }
     __syncthreads();
   }
@@ -566,4 +600,33 @@ k_decode_prepare_counted(DecodePrepArgs A, const int *__restrict__ Wseq, const l
                          const int32_t *__restrict__ present, const float *__restrict__ fromdB,
                          const int *__restrict__ count) {
   decode_prepare_body<true>(A, Wseq, coef_off, res, posts, present, fromdB, count);
+}
+
+// vb200_decode_packets_resume: the entropy decode of each block's packet in front of the same body
+template <bool COUNTED>
+__global__ void __launch_bounds__(128)
+k_decode_packets(DecodePrepArgs A, EntDev E, DecodePackets P, const int *__restrict__ Wseq,
+                 const long long *__restrict__ coef_off, float *__restrict__ res, const float *__restrict__ fromdB,
+                 const int *__restrict__ count) {
+  decode_prepare_body<COUNTED, true>(A, Wseq, coef_off, res, nullptr, nullptr, fromdB, count, &E, P);
+}
+
+// vb200_decode_entropy: the entropy decode alone, into the staging rows of vb200_decode_dsp; one CTA per block
+__global__ void __launch_bounds__(32)
+k_decode_entropy(EntDev E, const Floor1Dev *__restrict__ floors0, const Floor1Dev *__restrict__ floors1,
+                 DecodePackets P, int nblocks, const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
+                 float *__restrict__ res, int32_t *__restrict__ posts, int32_t *__restrict__ present) {
+  extern __shared__ __align__(16) unsigned char ent_smem[];
+  for (int it = blockIdx.x; it < nblocks; it += gridDim.x) {
+    const int W = Wseq[it] ? 1 : 0, n = E.n[W], ch = E.ch;
+    float *base = res + coef_off[it];
+    int32_t *po = posts + (size_t)it * ch * VB200_FLOOR1_STRIDE;
+    for (int j = threadIdx.x; j < ch * n; j += blockDim.x) base[j] = 0.f;
+    for (int j = threadIdx.x; j < ch * VB200_FLOOR1_STRIDE; j += blockDim.x) po[j] = 0;
+    __syncthreads();
+    if (threadIdx.x == 0)
+      ent_block(E, W ? floors1 : floors0, W, P.data + P.off[it], P.bytes[it], base, po, present + (size_t)it * ch,
+                ent_smem, ent_smem + ch, ent_smem + 2 * ch);
+    __syncthreads();
+  }
 }

@@ -1,21 +1,27 @@
 /* vb200_decode.c — many libvorbis decoders of one codec setup, one device call per round: vb200md_*.
  *
  * The decode counterpart of vb200ms_* (vb200_mapping0.c).  A round decodes every packet queued since the last
- * round, for all streams at once:
- *   1. host, all threads (OpenMP, one stream per thread at a time): the packet header as vorbis_synthesis reads it
- *      (lib/synthesis.c:37-82) and the entropy half of mapping0_inverse (lib/mapping0.c:714-751) through the
- *      reference's own _floor_P[]->inverse1 and _residue_P[]->inverse, straight into the staging area of
- *      vb200_decode_dsp_resume (residue vectors, floor-1 fit_value memo, block flags).  A packet whose header does
- *      not parse is dropped, as examples/decoder_example.c drops it when vorbis_synthesis fails.
- *   2. device: ONE vb200_decode_dsp_resume_dev call for every stream and both block sizes (de-coupling, floor
- *      multiply, IMDCT, overlap-add; two kernel launches); the overlap of every (stream, channel) stays in device
- *      memory between rounds.
+ * round, for all streams at once.  On the device path (taken when vb200_decode_entropy_setup accepts the setup
+ * that vb200md_entropy_new derives from the decoder's codebooks, floors and residues):
+ *   1. host: the packet header as vorbis_synthesis reads it (lib/synthesis.c:37-82); the packets of all streams
+ *      are laid out back to back in one byte buffer with per-block offsets and sizes.  A packet whose header
+ *      does not parse is dropped, as examples/decoder_example.c drops it when vorbis_synthesis fails.
+ *   2. device: the packet buffer and the small per-block arrays go up, then ONE vb200_decode_packets_resume_dev
+ *      call for every stream and both block sizes (entropy decode, de-coupling, floor multiply, IMDCT,
+ *      overlap-add; two kernel launches), and the PCM comes back.  The overlap of every (stream, channel) stays
+ *      in device memory between rounds.
+ * On the host path (any other setup, or vb200md_set_host_entropy) step 1 also runs the entropy half of
+ * mapping0_inverse (lib/mapping0.c:714-751) on all host threads (OpenMP, one stream per thread at a time)
+ * through the reference's own _floor_P[]->inverse1 and _residue_P[]->inverse, straight into the staging area of
+ * vb200_decode_dsp_resume (residue vectors, floor-1 fit_value memo, block flags), and step 2 uploads that
+ * staging and makes one vb200_decode_dsp_resume_dev call instead.
  *   3. host: the sample bookkeeping of vorbis_synthesis_blockin / pcmout (lib/block.c:741-751, 835-941) on each
  *      stream's counters (the first block returns nothing, a sequence gap loses the granule count, granulepos trims
  *      the first and the last packet), then each stream's finished samples go to the sink in order.
  * The device context is built here from the decoder's own lookups (floor-1 setups included) rather than through
  * vb200shim_attach, whose decoder bindings carry only what the function-level mdct_backward shim needs.
- * Limits: floor type 1 only (OV_EIMPL otherwise), two modes with blockflag 0 and 1, full-rate decode.
+ * Limits: floor type 1 only (OV_EIMPL otherwise), two modes with blockflag 0 and 1, full-rate decode; the device
+ * path also needs residue types 1 and 2 (type 0 keeps the host path).
  * Compiled like any libvorbis-internal backend against lib/codec_internal.h (oracle/decode.py builds it).
  */
 #include <stdint.h>
@@ -75,6 +81,13 @@ typedef struct vb200md {
   void *d_Wseq, *d_count, *d_posts, *d_present, *d_coef_off, *d_pcm_off, *d_res, *d_pcm;
   float *gather;                      /* float output of one stream, [ch][samples] for the sink */
   size_t cap_gather;
+  /* device entropy decode: ent_dev = the context took the entropy setup; host_entropy = forced host path */
+  int ent_dev, host_entropy;
+  size_t cap_pkt;
+  unsigned char *pkt;                 /* the packets of one round, back to back */
+  int64_t *pkt_off;
+  int32_t *pkt_bytes;
+  void *d_pkt, *d_pkt_off, *d_pkt_bytes;
   /* counters */
   long rounds, blocks, packets;
   double device_s, host_s;
@@ -87,7 +100,7 @@ void vb200md_close(vb200md *m){
   if(!m) return;
   if(m->ctx){
     void *d[] = {m->carry.tail, m->carry.W, m->d_Wseq, m->d_count, m->d_posts, m->d_present, m->d_coef_off,
-                 m->d_pcm_off, m->d_res, m->d_pcm};
+                 m->d_pcm_off, m->d_res, m->d_pcm, m->d_pkt, m->d_pkt_off, m->d_pkt_bytes};
     for(i = 0; i < (int)(sizeof(d)/sizeof(d[0])); i++) if(d[i]) vb200_free_device(m->ctx, d[i]);
     vb200_ctx_destroy(m->ctx);
   }
@@ -101,6 +114,7 @@ void vb200md_close(vb200md *m){
   }
   free(m->Wseq); free(m->count); free(m->posts); free(m->present); free(m->coef_off); free(m->pcm_off);
   free(m->fin); free(m->res); free(m->pcm); free(m->gather);
+  free(m->pkt); free(m->pkt_off); free(m->pkt_bytes);
   free(m);
 }
 
@@ -147,6 +161,154 @@ static int md_setup(vb200md *m, vb200_setup *s){
   return 0;
 }
 
+
+/* ---- the entropy setup of the device decoder, derived from the decoder's own tables ---------------------------- */
+typedef struct {
+  vb200_entropy_setup es;             /* first: the struct handed out */
+  vb200_codebook *books;
+  uint8_t *length;
+  uint32_t *bits;
+  int32_t *entry;
+} md_entropy_tables;
+
+static uint32_t md_bitrev(uint32_t x){
+  x = ((x >> 16) & 0x0000ffffU) | ((x << 16) & 0xffff0000U);
+  x = ((x >>  8) & 0x00ff00ffU) | ((x <<  8) & 0xff00ff00U);
+  x = ((x >>  4) & 0x0f0f0f0fU) | ((x <<  4) & 0xf0f0f0f0U);
+  x = ((x >>  2) & 0x33333333U) | ((x <<  2) & 0xccccccccU);
+  return ((x >> 1) & 0x55555555U) | ((x << 1) & 0xaaaaaaaaU);
+}
+
+static int md_ilog(unsigned v){ int r = 0; while(v){ r++; v >>= 1; } return r; }
+
+/* the codewords of one decode book (NULL arrays: count only), for both layouts of lib/codebook.h:73-110
+ * (lib/sharedbook.c:393-519).  Unordered: codelist holds each codeword left-aligned, codelengths its length and
+ * index its entry, n = hi_max (1 for the single-entry book, which has no hi_max).  Ordered: index[l] counts the
+ * entries of lengths minlength..minlength+l, codelist[l] is the last codeword of that length left-aligned with
+ * trailing ones, and the entries of one length take consecutive codes. */
+static long md_book_codewords(const dec_codebook *db, uint8_t *len, uint32_t *bits, int32_t *entry){
+  long i, n = 0;
+  if(!db->codelist) return 0;
+  if(db->codelengths){
+    n = db->hi_max > 0 ? db->hi_max : 1;
+    if(len)
+      for(i = 0; i < n; i++){
+        len[i] = (uint8_t)db->codelengths[i];
+        bits[i] = md_bitrev(db->codelist[i]);
+        entry[i] = db->index[i];
+      }
+  }else{
+    int l, nl = db->maxlength - db->minlength + 1;
+    long prev = 0;
+    n = db->entries;
+    if(len)
+      for(l = 0; l < nl; l++){
+        const int length = db->minlength + l;
+        long e;
+        for(e = prev; e < db->index[l]; e++){
+          const uint32_t code = db->codelist[l] + 1U - ((uint32_t)(db->index[l] - e) << (32 - length));
+          len[e] = (uint8_t)length;
+          bits[e] = md_bitrev(code);
+          entry[e] = (int32_t)e;
+        }
+        prev = db->index[l];
+      }
+  }
+  return n;
+}
+
+void vb200md_entropy_free(vb200_entropy_setup *es){
+  md_entropy_tables *t = (md_entropy_tables*)es;
+  if(!t) return;
+  free(t->books); free(t->length); free(t->bits); free(t->entry);
+  free(t);
+}
+
+/* The vb200_entropy_setup of a decoder after vorbis_synthesis_init: every book of ci->decbooks, the floor and
+ * residue decode fields of both modes' submaps, modebits.  Checks once that every codeword decodes to its entry
+ * through the reference's vorbis_book_decode.  NULL on failure with *err = OV_EIMPL (a mode layout the driver
+ * does not take), OV_EFAULT (no memory) or OV_EBADHEADER (a codeword that does not decode to its entry).
+ * Free with vb200md_entropy_free. */
+vb200_entropy_setup *vb200md_entropy_new(vorbis_info *vi, vorbis_dsp_state *vd, int *err){
+  codec_setup_info *ci = (codec_setup_info*)vi->codec_setup;
+  private_state *b = (private_state*)vd->backend_state;
+  md_entropy_tables *t = (md_entropy_tables*)calloc(1, sizeof(*t));
+  long total = 0, at = 0;
+  int i, w, j, k, rc = OV_EFAULT;
+  oggpack_buffer opb;
+  if(!t) goto fail;
+  for(i = 0; i < ci->books; i++) total += md_book_codewords(ci->decbooks + i, NULL, NULL, NULL);
+  t->books = (vb200_codebook*)calloc(ci->books > 0 ? ci->books : 1, sizeof(*t->books));
+  t->length = (uint8_t*)malloc(total > 0 ? total : 1);
+  t->bits = (uint32_t*)malloc(sizeof(uint32_t) * (total > 0 ? total : 1));
+  t->entry = (int32_t*)malloc(sizeof(int32_t) * (total > 0 ? total : 1));
+  if(!t->books || !t->length || !t->bits || !t->entry) goto fail;
+  t->es.nbooks = ci->books;
+  t->es.books = t->books;
+  t->es.modebits = b->modebits;
+  rc = OV_EBADHEADER;
+  oggpack_writeinit(&opb);
+  for(i = 0; i < ci->books; i++){
+    dec_codebook *db = ci->decbooks + i;
+    vb200_codebook *o = &t->books[i];
+    const long n = md_book_codewords(db, t->length + at, t->bits + at, t->entry + at);
+    o->dim = db->dim; o->used = (int32_t)n;
+    o->length = t->length + at; o->bits = t->bits + at; o->entry = t->entry + at;
+    o->value = db->valuelist;
+    for(k = 0; k < n; k++){                      /* self-check: the codeword decodes to its entry */
+      oggpack_buffer rd;
+      oggpack_reset(&opb);
+      oggpack_write(&opb, o->bits[k], o->length[k]);
+      oggpack_readinit(&rd, oggpack_get_buffer(&opb), (int)oggpack_bytes(&opb));
+      if(vorbis_book_decode(db, &rd) != o->entry[k]){ oggpack_writeclear(&opb); goto fail; }
+    }
+    at += n;
+  }
+  oggpack_writeclear(&opb);
+  rc = OV_EIMPL;
+  if(ci->modes != 2) goto fail;
+  for(w = 0; w < 2; w++){
+    vorbis_info_mapping0 *mp;
+    if(ci->mode_param[w]->blockflag != w || ci->map_type[ci->mode_param[w]->mapping] != 0) goto fail;
+    mp = (vorbis_info_mapping0*)ci->map_param[ci->mode_param[w]->mapping];
+    if(mp->submaps > VB200_MAX_SUBMAPS) goto fail;
+    for(j = 0; j < mp->submaps; j++){
+      const int fl = mp->floorsubmap[j], rs = mp->residuesubmap[j];
+      vb200_floor_decode *f = &t->es.floor[w][j];
+      vb200_residue_decode *r = &t->es.residue[w][j];
+      f->type = ci->floor_type[fl];
+      if(f->type == 1){
+        const vorbis_info_floor1 *fi = (const vorbis_info_floor1*)ci->floor_param[fl];
+        f->partitions = fi->partitions;
+        for(k = 0; k < fi->partitions && k < 31; k++) f->partitionclass[k] = fi->partitionclass[k];
+        for(k = 0; k < 16; k++){
+          int s;
+          f->class_dim[k] = fi->class_dim[k]; f->class_subs[k] = fi->class_subs[k]; f->class_book[k] = fi->class_book[k];
+          for(s = 0; s < 8; s++) f->class_subbook[k][s] = fi->class_subbook[k][s];
+        }
+      }
+      r->type = ci->residue_type[rs];
+      {
+        const vorbis_info_residue0 *ri = (const vorbis_info_residue0*)ci->residue_param[rs];
+        int acc = 0, c;
+        r->begin = (int32_t)ri->begin; r->end = (int32_t)ri->end; r->grouping = ri->grouping;
+        r->partitions = ri->partitions; r->partvals = ri->partvals; r->groupbook = ri->groupbook;
+        for(c = 0; c < 64; c++){                  /* as res0_look lays them out, lib/res0.c:274-292 */
+          const int stages = c < ri->partitions ? md_ilog((unsigned)ri->secondstages[c]) : 0;
+          for(k = 0; k < 8; k++)
+            r->stagebook[c][k] = k < stages && (ri->secondstages[c] & (1 << k)) ? ri->booklist[acc++] : -1;
+        }
+      }
+    }
+  }
+  if(err) *err = 0;
+  return &t->es;
+fail:
+  if(err) *err = rc;
+  vb200md_entropy_free(t ? &t->es : NULL);
+  return NULL;
+}
+
 static void md_reset(md_stream *t){
   t->fresh = 1; t->sequence = -1; t->granulepos = -1; t->sample_count = -1; t->lastW = -1;
 }
@@ -190,6 +352,15 @@ vb200md *vb200md_open_err(int nstreams, ogg_packet hdr[3], int pcm_s16, int devi
     free(neg);
     if(i) goto fail;
   }
+  {                                   /* the device path where the context takes the entropy setup */
+    int e;
+    vb200_entropy_setup *es = vb200md_entropy_new(&m->vi, &m->vd, &e);
+    if(!es){ rc = e; goto fail; }
+    e = vb200_decode_entropy_setup(m->ctx, es);
+    vb200md_entropy_free(es);
+    if(e == VB200_EFAULT){ rc = OV_EFAULT; goto fail; }
+    m->ent_dev = e == 0;
+  }
   if(err) *err = 0;
   return m;
 fail:
@@ -203,6 +374,14 @@ vb200md *vb200md_open(int nstreams, ogg_packet hdr[3], int pcm_s16, int device){
 }
 
 int vb200md_channels(vb200md *m){ return m->ch; }
+/* the device context the driver built (its entropy setup registered where the device path is taken) */
+vb200_ctx *vb200md_context(vb200md *m){ return m->ctx; }
+/* 1 where rounds decode the packets on the device (vb200_decode_packets_resume_dev), 0 where the entropy half
+ * runs on the host */
+int vb200md_entropy_on_device(vb200md *m){ return m->ent_dev && !m->host_entropy; }
+/* Diagnostic: on != 0 forces the host entropy path (to compare the two paths and to keep the fallback covered);
+ * 0 returns to the path the setup allows.  Takes effect at the next round. */
+void vb200md_set_host_entropy(vb200md *m, int on){ m->host_entropy = on ? 1 : 0; }
 unsigned long long vb200md_launches(vb200md *m){ return vb200_launch_count(m->ctx); }
 /* rounds that decoded blocks, blocks, audio packets; seconds in step 2 (copies in, the call, copies out) and in
  * steps 1 + 3 */
@@ -317,7 +496,7 @@ static void md_entropy(vb200md *m, vorbis_block *vb, float *res, int32_t *posts,
 
 #define GROW(ptr, cap_needed, cap, T) do { T *q_ = (T*)realloc((ptr), sizeof(T) * (cap_needed)); if(!q_) return OV_EFAULT; (ptr) = q_; } while(0)
 
-static int md_reserve(vb200md *m, size_t nblk_total, size_t nres, size_t npcm){
+static int md_reserve(vb200md *m, size_t nblk_total, size_t nres, size_t npcm, size_t npkt){
   const int ch = m->ch;
   const size_t pcm_el = m->pcm_s16 ? sizeof(int16_t) : sizeof(float);
   if(nblk_total > m->cap_blk){
@@ -325,6 +504,11 @@ static int md_reserve(vb200md *m, size_t nblk_total, size_t nres, size_t npcm){
     GROW(m->Wseq, c, 0, int32_t); GROW(m->coef_off, c, 0, int64_t); GROW(m->pcm_off, c, 0, int64_t);
     GROW(m->fin, c, 0, int32_t); GROW(m->present, c * ch, 0, int32_t);
     GROW(m->posts, c * ch * VB200_FLOOR1_STRIDE, 0, int32_t);
+    GROW(m->pkt_off, c, 0, int64_t); GROW(m->pkt_bytes, c, 0, int32_t);
+    if(m->d_pkt_off){ vb200_free_device(m->ctx, m->d_pkt_off); vb200_free_device(m->ctx, m->d_pkt_bytes); }
+    m->d_pkt_off = m->d_pkt_bytes = NULL;
+    if(vb200_malloc_device(m->ctx, sizeof(int64_t) * c, &m->d_pkt_off) ||
+       vb200_malloc_device(m->ctx, sizeof(int32_t) * c, &m->d_pkt_bytes)) return OV_EFAULT;
     if(m->d_Wseq){ vb200_free_device(m->ctx, m->d_Wseq); vb200_free_device(m->ctx, m->d_coef_off);
                    vb200_free_device(m->ctx, m->d_pcm_off); vb200_free_device(m->ctx, m->d_present);
                    vb200_free_device(m->ctx, m->d_posts); }
@@ -339,6 +523,14 @@ static int md_reserve(vb200md *m, size_t nblk_total, size_t nres, size_t npcm){
   if(!m->count){
     m->count = (int32_t*)malloc(sizeof(int32_t) * m->nstreams);
     if(!m->count || vb200_malloc_device(m->ctx, sizeof(int32_t) * m->nstreams, &m->d_count)) return OV_EFAULT;
+  }
+  if(npkt > m->cap_pkt){
+    size_t c = npkt + npkt / 2;
+    GROW(m->pkt, c, 0, unsigned char);
+    if(m->d_pkt) vb200_free_device(m->ctx, m->d_pkt);
+    m->d_pkt = NULL;
+    if(vb200_malloc_device(m->ctx, c, &m->d_pkt)) return OV_EFAULT;
+    m->cap_pkt = c;
   }
   if(nres > m->cap_res){
     size_t c = nres + nres / 2;
@@ -409,7 +601,8 @@ int vb200md_round(vb200md *m, vb200md_sink sink, void *user){
   double t0 = md_now(), t1, t2;
   int s, nblk = 0, rc;
   long total = 0, maxpcm = 0;
-  size_t nres = 0;
+  size_t nres = 0, npkt = 0;
+  const int on_dev = vb200md_entropy_on_device(m);
   /* step 1a: headers (cheap), block counts and the packed layout */
   for(s = 0; s < ns; s++){
     md_stream *t = &m->st[s];
@@ -423,7 +616,7 @@ int vb200md_round(vb200md *m, vb200md_sink sink, void *user){
     m->host_s += md_now() - t0;
     return 0;
   }
-  if((rc = md_reserve(m, (size_t)ns * nblk, 0, 0))) return rc;
+  if((rc = md_reserve(m, (size_t)ns * nblk, 0, 0, 0))) return rc;
   for(s = 0; s < ns; s++){
     md_stream *t = &m->st[s];
     int k, j = 0, prev = t->lastW;
@@ -433,6 +626,9 @@ int vb200md_round(vb200md *m, vb200md_sink sink, void *user){
       const size_t it = (size_t)s * nblk + j;
       if(W < 0) continue;
       m->Wseq[it] = W;
+      m->pkt_off[it] = (int64_t)npkt;
+      m->pkt_bytes[it] = (int32_t)t->q[k].bytes;
+      npkt += (size_t)t->q[k].bytes;
       m->coef_off[it] = (int64_t)nres;
       m->pcm_off[it] = pos;
       m->fin[it] = prev >= 0 ? (int32_t)(m->bs[prev] / 4 + m->bs[W] / 4) : 0;
@@ -441,14 +637,28 @@ int vb200md_round(vb200md *m, vb200md_sink sink, void *user){
       prev = W; j++;
     }
     m->count[s] = j;
-    for(; j < nblk; j++){ const size_t it = (size_t)s * nblk + j; m->Wseq[it] = 0; m->coef_off[it] = 0; m->pcm_off[it] = 0; m->fin[it] = 0; }
+    for(; j < nblk; j++){
+      const size_t it = (size_t)s * nblk + j;
+      m->Wseq[it] = 0; m->coef_off[it] = 0; m->pcm_off[it] = 0; m->fin[it] = 0; m->pkt_off[it] = 0; m->pkt_bytes[it] = 0;
+    }
     if(pos > maxpcm) maxpcm = pos;
   }
   if(maxpcm < 1) maxpcm = 1;
-  if((rc = md_reserve(m, (size_t)ns * nblk, nres ? nres : 1, (size_t)ns * ch * maxpcm))) return rc;
-  /* step 1b: the entropy half, one stream per thread at a time */
+  if((rc = md_reserve(m, (size_t)ns * nblk, nres ? nres : 1, (size_t)ns * ch * maxpcm, npkt + 1))) return rc;
+  /* step 1b, device path: the packets back to back */
+  if(on_dev)
+    for(s = 0; s < ns; s++){
+      md_stream *t = &m->st[s];
+      int k, j = 0;
+      for(k = 0; k < t->nq; k++)
+        if(t->q[k].W >= 0){
+          const size_t it = (size_t)s * nblk + j++;
+          memcpy(m->pkt + m->pkt_off[it], t->q[k].data, (size_t)t->q[k].bytes);
+        }
+    }
+  /* step 1b, host path: the entropy half, one stream per thread at a time */
 #pragma omp parallel for schedule(dynamic, 1)
-  for(s = 0; s < ns; s++){
+  for(s = 0; s < (on_dev ? 0 : ns); s++){
     md_stream *t = &m->st[s];
 #ifdef _OPENMP
     vorbis_block *vb = &m->vb[omp_get_thread_num()];
@@ -472,14 +682,25 @@ int vb200md_round(vb200md *m, vb200md_sink sink, void *user){
     if(vb200_memcpy_h2d(m->ctx, m->d_Wseq, m->Wseq, sizeof(int32_t) * nb) ||
        vb200_memcpy_h2d(m->ctx, m->d_count, m->count, sizeof(int32_t) * ns) ||
        vb200_memcpy_h2d(m->ctx, m->d_coef_off, m->coef_off, sizeof(int64_t) * nb) ||
-       vb200_memcpy_h2d(m->ctx, m->d_pcm_off, m->pcm_off, sizeof(int64_t) * nb) ||
-       vb200_memcpy_h2d(m->ctx, m->d_res, m->res, sizeof(float) * nres) ||
-       vb200_memcpy_h2d(m->ctx, m->d_posts, m->posts, sizeof(int32_t) * nb * ch * VB200_FLOOR1_STRIDE) ||
-       vb200_memcpy_h2d(m->ctx, m->d_present, m->present, sizeof(int32_t) * nb * ch)) return OV_EFAULT;
-    if(vb200_decode_dsp_resume_dev(m->ctx, ns, nblk, (const int32_t*)m->d_count, (const int32_t*)m->d_Wseq,
-                                   (const int64_t*)m->d_coef_off, (float*)m->d_res, (const int32_t*)m->d_posts,
-                                   (const int32_t*)m->d_present, (const int64_t*)m->d_pcm_off, m->d_pcm, m->pcm_s16,
-                                   maxpcm, &m->carry, NULL)) return OV_EFAULT;
+       vb200_memcpy_h2d(m->ctx, m->d_pcm_off, m->pcm_off, sizeof(int64_t) * nb)) return OV_EFAULT;
+    if(on_dev){
+      if((npkt && vb200_memcpy_h2d(m->ctx, m->d_pkt, m->pkt, npkt)) ||
+         vb200_memcpy_h2d(m->ctx, m->d_pkt_off, m->pkt_off, sizeof(int64_t) * nb) ||
+         vb200_memcpy_h2d(m->ctx, m->d_pkt_bytes, m->pkt_bytes, sizeof(int32_t) * nb)) return OV_EFAULT;
+      if(vb200_decode_packets_resume_dev(m->ctx, ns, nblk, (const int32_t*)m->d_count, (const int32_t*)m->d_Wseq,
+                                         (const int64_t*)m->d_coef_off, (float*)m->d_res,
+                                         (const int64_t*)m->d_pkt_off, (const int32_t*)m->d_pkt_bytes,
+                                         (const uint8_t*)m->d_pkt, (const int64_t*)m->d_pcm_off, m->d_pcm,
+                                         m->pcm_s16, maxpcm, &m->carry, NULL)) return OV_EFAULT;
+    }else{
+      if(vb200_memcpy_h2d(m->ctx, m->d_res, m->res, sizeof(float) * nres) ||
+         vb200_memcpy_h2d(m->ctx, m->d_posts, m->posts, sizeof(int32_t) * nb * ch * VB200_FLOOR1_STRIDE) ||
+         vb200_memcpy_h2d(m->ctx, m->d_present, m->present, sizeof(int32_t) * nb * ch)) return OV_EFAULT;
+      if(vb200_decode_dsp_resume_dev(m->ctx, ns, nblk, (const int32_t*)m->d_count, (const int32_t*)m->d_Wseq,
+                                     (const int64_t*)m->d_coef_off, (float*)m->d_res, (const int32_t*)m->d_posts,
+                                     (const int32_t*)m->d_present, (const int64_t*)m->d_pcm_off, m->d_pcm,
+                                     m->pcm_s16, maxpcm, &m->carry, NULL)) return OV_EFAULT;
+    }
     if(vb200_memcpy_d2h(m->ctx, m->pcm, m->d_pcm, pbytes) || vb200_synchronize(m->ctx)) return OV_EFAULT;
   }
   t2 = md_now();

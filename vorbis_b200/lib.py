@@ -35,6 +35,8 @@ EXPORTS = [
     "vb200_envelope_search_dev", "vb200_envelope_search", "vb200_envelope_search_var", "vb200_envelope_apply_marks",
     "vb200_floor1_inverse2_dev", "vb200_floor1_inverse2", "vb200_decode_dsp_dev", "vb200_decode_dsp",
     "vb200_decode_dsp_resume_dev", "vb200_decode_dsp_resume",
+    "vb200_decode_entropy_setup", "vb200_decode_entropy_dev", "vb200_decode_entropy",
+    "vb200_decode_packets_resume_dev", "vb200_decode_packets_resume",
     "vb200_residue_partvals", "vb200_residue_classify_dev", "vb200_residue_classify",
     "vb200_plan_blocks", "vb200_encode_streams_dev", "vb200_encode_streams",
     "vb200_encode_streams_managed_dev", "vb200_encode_streams_managed",
@@ -114,6 +116,13 @@ def load():
                                               C.POINTER(abi.DecodeCarry), vp]
     L.vb200_decode_dsp_resume.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int64, vp, vp, vp, vp, C.c_int,
                                           C.c_int64, C.POINTER(abi.DecodeCarry)]
+    L.vb200_decode_entropy_setup.argtypes = [vp, C.POINTER(abi.EntropySetup)]
+    L.vb200_decode_entropy_dev.argtypes = [vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.vb200_decode_entropy.argtypes = [vp, C.c_int, vp, vp, vp, vp, C.c_int64, vp, vp, C.c_int64, vp, vp]
+    L.vb200_decode_packets_resume_dev.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_int,
+                                                  C.c_int64, C.POINTER(abi.DecodeCarry), vp]
+    L.vb200_decode_packets_resume.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, C.c_int64, vp, vp, vp, C.c_int64, vp,
+                                              vp, C.c_int, C.c_int64, C.POINTER(abi.DecodeCarry)]
     L.vb200_envelope_search_dev.argtypes = [vp, C.c_int, vp, C.c_int, C.c_int64, C.c_int, C.c_int, vp, vp, vp]
     L.vb200_envelope_search.argtypes = [vp, C.c_int, vp, C.c_int, C.c_int64, C.c_int, C.c_int, vp, vp]
     L.vb200_envelope_apply_marks.argtypes = [vp, C.c_int, C.c_int, vp]
@@ -154,14 +163,25 @@ class Context:
         self.h = h
         self.halfrate = 0
 
+    @classmethod
+    def wrap(cls, handle, channels, blocksizes):
+        """a Context on a vb200_ctx created elsewhere (e.g. by the decode driver), which keeps owning it"""
+        self = cls.__new__(cls)
+        self.L = load()
+        self.setup = None
+        self.h = vp(handle)
+        self.halfrate = 0
+        self.channels, self.bs = channels, list(blocksizes)
+        return self
+
+    def close(self):
+        if getattr(self, "h", None) and self.setup is not None:
+            self.L.vb200_ctx_destroy(self.h)
+        self.h = None
+
     def _chk(self, rc):
         if rc != 0:
             raise VB200Error("vb200 error %d: %s" % (rc, (self.L.vb200_last_error() or b"").decode()))
-
-    def close(self):
-        if getattr(self, "h", None):
-            self.L.vb200_ctx_destroy(self.h)
-            self.h = None
 
     def __del__(self):
         try:
@@ -580,6 +600,59 @@ class Context:
                                                      _ptr(d_coef_off), _ptr(d_res), _ptr(d_posts), _ptr(d_present),
                                                      _ptr(d_pcm_off), _ptr(d_pcm), pcm_s16, pcm_stride, C.byref(k),
                                                      _ptr(stream)))
+
+    # ---- decode from the packets: the entropy decoders on the device ---------------------------------
+    def decode_entropy_setup(self, es):
+        """vb200_decode_entropy_setup with an abi.EntropySetup"""
+        self._chk(self.L.vb200_decode_entropy_setup(self.h, C.byref(es)))
+
+    def decode_entropy(self, Wseq, pkt_off, pkt_bytes, data, coef_off, res_len):
+        """vb200_decode_entropy: (res [res_len], posts [nblocks][ch][FLOOR1_STRIDE], present [nblocks][ch])"""
+        Wseq = np.ascontiguousarray(Wseq, np.int32)
+        nb = len(Wseq)
+        pkt_off = np.ascontiguousarray(pkt_off, np.int64)
+        pkt_bytes = np.ascontiguousarray(pkt_bytes, np.int32)
+        data = np.ascontiguousarray(data, np.uint8)
+        coef_off = np.ascontiguousarray(coef_off, np.int64)
+        res = np.zeros(max(res_len, 1), np.float32)
+        posts = np.zeros((nb, self.channels, abi.FLOOR1_STRIDE), np.int32)
+        present = np.zeros((nb, self.channels), np.int32)
+        self._chk(self.L.vb200_decode_entropy(self.h, nb, _ptr(Wseq), _ptr(pkt_off), _ptr(pkt_bytes), _ptr(data),
+                                              data.size, _ptr(coef_off), _ptr(res), res_len, _ptr(posts),
+                                              _ptr(present)))
+        return res, posts, present
+
+    def decode_packets_resume(self, Wseq, coef_off, res_len, pkt_off, pkt_bytes, data, pcm_off, pcm_stride, carry,
+                              count=None, s16=False):
+        """vb200_decode_packets_resume: decode_dsp_resume from the packets (pkt_off, pkt_bytes [nstreams][nblk] into
+        data); carry = (tail, W) as for decode_dsp_resume, updated in place"""
+        Wseq = np.ascontiguousarray(Wseq, np.int32)
+        ns, nblk = Wseq.shape
+        tail, W = carry
+        assert tail.dtype == np.float32 and W.dtype == np.int32 and tail.flags.c_contiguous and W.flags.c_contiguous
+        coef_off = np.ascontiguousarray(coef_off, np.int64)
+        pcm_off = np.ascontiguousarray(pcm_off, np.int64)
+        pkt_off = np.ascontiguousarray(pkt_off, np.int64)
+        pkt_bytes = np.ascontiguousarray(pkt_bytes, np.int32)
+        data = np.ascontiguousarray(data, np.uint8)
+        count = None if count is None else np.ascontiguousarray(count, np.int32)
+        pcm = (np.zeros((ns, pcm_stride, self.channels), np.int16) if s16
+               else np.zeros((ns, self.channels, pcm_stride), np.float32))
+        k = abi.DecodeCarry(tail.ctypes.data, W.ctypes.data)
+        self._chk(self.L.vb200_decode_packets_resume(self.h, ns, nblk, _ptr(count), _ptr(Wseq), _ptr(coef_off),
+                                                     res_len, _ptr(pkt_off), _ptr(pkt_bytes), _ptr(data), data.size,
+                                                     _ptr(pcm_off), _ptr(pcm), 1 if s16 else 0, pcm_stride,
+                                                     C.byref(k)))
+        return pcm
+
+    def decode_packets_resume_dev(self, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_pkt_off, d_pkt_bytes,
+                                  d_data, d_pcm_off, d_pcm, pcm_s16, pcm_stride, d_tail, d_W, stream=None):
+        k = abi.DecodeCarry(_ptr(d_tail), _ptr(d_W))
+        self._chk(self.L.vb200_decode_packets_resume_dev(self.h, nstreams, nblk, _ptr(d_count), _ptr(d_Wseq),
+                                                         _ptr(d_coef_off), _ptr(d_res), _ptr(d_pkt_off),
+                                                         _ptr(d_pkt_bytes), _ptr(d_data), _ptr(d_pcm_off),
+                                                         _ptr(d_pcm), pcm_s16, pcm_stride, C.byref(k),
+                                                         _ptr(stream)))
 
     # ---- envelope / block-switch detector (lib/envelope.c) --------------------------------------
     def envelope_search(self, pcm, first_step, nsteps, state=None, fmt=PCM_F32_PLANAR):
