@@ -670,6 +670,74 @@ int vb200_decode_packets_resume    (vb200_ctx*, int nstreams, int nblk, const in
                                     const int64_t *pcm_off, void *pcm, int pcm_s16, int64_t pcm_stride,
                                     vb200_decode_carry *carry);
 
+/* ---- encode: the entropy coding of mapping0_forward (lib/mapping0.c:596-687) on the device, un-managed bitrate.
+ * What floor1_encode (lib/floor1.c:753-921) and the residue class / forward of types 1 and 2 (lib/res0.c:534-648,
+ * 725-809) read, registered on a context with vb200_encode_entropy_setup.
+ *
+ * vb200_enc_codebook: one codebook as the encoder uses it (codec_setup_info.fullbooks).  Entry i has the codeword
+ * codeword[i] of length[i] bits (0 = unused entry), written LSb first as oggpack_write(codeword[i], length[i])
+ * writes it; minval / delta / quantvals are the integer lattice of a residue stage book (book->minval, ->delta,
+ * ->quantvals; 0 for books without a value mapping).                                                           */
+typedef struct vb200_enc_codebook {
+  int32_t dim;
+  int32_t entries;
+  const uint8_t  *length;          /* [entries] c->lengthlist                        */
+  const uint32_t *codeword;        /* [entries] book->codelist                       */
+  int32_t minval, delta, quantvals;
+} vb200_enc_codebook;
+
+/* floor[W][submap] and residue[W][submap] carry exactly the fields the encoder reads; their layout is the decoder's
+ * (stagebook[class][stage] as res0_look lays out partbooks, -1 where the stage bit is clear).  The struct shares
+ * its name with the function that registers it, so C callers name it `struct vb200_encode_entropy_setup`. */
+struct vb200_encode_entropy_setup {
+  int32_t nbooks;
+  const vb200_enc_codebook *books; /* [nbooks]                                       */
+  int32_t modebits;                /* private_state.modebits                         */
+  vb200_floor_decode   floor[2][VB200_MAX_SUBMAPS];
+  vb200_residue_decode residue[2][VB200_MAX_SUBMAPS];
+};
+
+/* Copies and uploads everything.  Returns VB200_EINVAL for a book index out of range, a stage book with dim > 8,
+ * quantvals <= 0 or a lattice larger than its entries, a codeword longer than 32 bits, a residue range that does
+ * not fit the block or differs from the context's vb200_residue_setup (which classifies), a floor class with
+ * class_dim > 8 or class_subs > 3, floor partitions that do not give the floor's posts; VB200_EIMPL for residue
+ * type 0 or a floor that is not type 1.  Unused entries (length 0) are legal.  Replaces an earlier registration. */
+int vb200_encode_entropy_setup(vb200_ctx*, const struct vb200_encode_entropy_setup*);
+
+/* Worst-case bytes of one packet of block size W under the registered setup, a multiple of 4: the header, per
+ * channel 1 + 2*ilog(quant_q-1) bits and the longest class and sub-book codewords of every partition, and per
+ * residue stage the longest phrase codeword per partition word plus grouping/dim times the longest codeword of
+ * the stage's class books per partition.  < 0: no setup registered (VB200_EINVAL).                              */
+int vb200_encode_packet_bound(vb200_ctx*, int W);
+
+/* The packets of nblocks blocks of size W (what mapping0_forward writes into packetblob[PACKETBLOBS/2]): packet
+ * type bit, mode W in modebits bits, lW / nW for long blocks, the floor of every channel, then classification and
+ * residue per submap.  byte-identical to the reference.
+ *   desc    [nblocks]          lW / nW of every block (blocktype and ampmax are not read)
+ *   posts   [nblocks][ch][VB200_FLOOR1_STRIDE], nonzero [nblocks][ch], iwork [nblocks][ch][n] int32: exactly
+ *           what vb200_encode_dsp returns (a silent channel is an all-zero posts row); iwork is not modified.
+ * _dev: block b goes to data + b*pkt_stride and pkt_bits[b] is its length in bits; pkt_stride must be a multiple
+ *       of 4 and >= vb200_encode_packet_bound(W).  Two kernel launches (classification, then the coder).
+ * Host form: packets back to back, block b at data + pkt_off[b] (int64 bytes), (pkt_bits[b] + 7) / 8 bytes long;
+ *       only the packet bytes and the per-block counts are copied back.  If they do not fit data_cap bytes it returns
+ *       VB200_EINVAL with pkt_bits filled (as count > cap does for vb200_encode_streams).  Four kernel launches.
+ * Without a registered setup, all of these return VB200_EINVAL.                                                  */
+int vb200_encode_entropy_dev(vb200_ctx*, int W, int nblocks, const vb200_block_desc *d_desc, const int32_t *d_posts,
+                             const int32_t *d_nonzero, const int32_t *d_iwork, int64_t pkt_stride, int32_t *d_pkt_bits,
+                             uint8_t *d_data, void *stream);
+int vb200_encode_entropy    (vb200_ctx*, int W, int nblocks, const vb200_block_desc *desc, const int32_t *posts,
+                             const int32_t *nonzero, const int32_t *iwork, int64_t *pkt_off, int32_t *pkt_bits,
+                             uint8_t *data, int64_t data_cap);
+
+/* PCM in, packets out: vb200_encode_dsp's chain, then classification and entropy coding, in one synchronous round
+ * trip (host buffers; no chunk pipeline).  io as for vb200_encode_dsp except that posts, nonzero, iwork, classes,
+ * overflow, mdct, logmdct and logmask must be NULL (they stay in device scratch) and iwork_fmt must be
+ * VB200_IWORK_S32; io->ampmax_out is filled.  Packed output as vb200_encode_entropy.  Launches: those of
+ * vb200_encode_dsp on one batch plus four.  A caller with device buffers chains vb200_encode_dsp_dev and
+ * vb200_encode_entropy_dev on one stream instead; there is no fused _dev form.                                   */
+int vb200_encode_packets(vb200_ctx*, int W, int nstreams, int blocks_per_stream, int blobno, const vb200_encode_io *io,
+                         int64_t *pkt_off, int32_t *pkt_bits, uint8_t *data, int64_t data_cap);
+
 /* ---- device memory helpers for non-CUDA hosts (C callers) -------------- */
 int  vb200_malloc_device(vb200_ctx*, size_t bytes, void **dptr);
 int  vb200_free_device  (vb200_ctx*, void *dptr);

@@ -32,6 +32,7 @@
 #define __restrict__ __restrict
 #define __align__(n) __attribute__((aligned(n)))
 #define __shared__ static
+#define __grid_constant__
 
 // ---- vector types -------------------------------------------------------------------------
 struct uint3 { unsigned x, y, z; };
@@ -212,6 +213,7 @@ template <class T> static inline void __stwt(T *p, T v) { *p = v; }
 static inline size_t __cvta_generic_to_shared(const void *p) { return (size_t)((const unsigned char *)p - (const unsigned char *)nullptr); }
 template <class T> static inline T atomicAdd(T *p, T v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
 static inline int atomicAnd(int *p, int v) { return __atomic_fetch_and(p, v, __ATOMIC_RELAXED); }
+static inline unsigned atomicOr(unsigned *p, unsigned v) { return __atomic_fetch_or(p, v, __ATOMIC_RELAXED); }
 static inline int atomicMax(int *p, int v) { int o = __atomic_load_n(p, __ATOMIC_RELAXED); while (o < v && !__atomic_compare_exchange_n(p, &o, v, true, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {} return o; }
 static inline long long clock64() { return 0; }
 

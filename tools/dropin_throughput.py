@@ -1,8 +1,10 @@
 #!/usr/bin/env python
 """Drop-in throughput (VERDICT r1 #5): N concurrent encoders driven by the multi-stream driver of
-vorbis_b200/host/vb200_mapping0.c (their ready blocks go to the device together, the reference's own floor1_encode
-and residue backend write the bits on ONE host thread) against the stock reference encoder on one host thread,
-same streams, same box.  Prints one JSON object; packets are cross-checked by hash.
+vorbis_b200/host/vb200_mapping0.c (their ready blocks go to the device together) on its device path (the packets are
+entropy coded on the device) and with the host path forced (the reference's own floor1_encode and residue backend
+write the bits on the host threads), against the stock reference encoder on one host thread, same streams, same box.
+Prints one JSON object; packets are cross-checked by hash.  With VB200MS_PROFILE=1 the driver prints its phases
+(envelope, blockout, stage, device call, host half; seconds) to stderr when each run closes.
 
 usage: python tools/dropin_throughput.py [--streams 1000] [--seconds 2.0]
 Needs oracle/_ref/*.so (built by __graft_entry__.build() where the reference sources exist)."""
@@ -34,15 +36,20 @@ for k in range(8):                                          # a few transients s
         base[k, :, a:a + 200] *= 0.02
         base[k, :, a + 200:a + 260] = rng.uniform(-0.9, 0.9, (ch, 60))
 pcm = np.ascontiguousarray(base[np.arange(ns) % 8])         # [ns][ch][n]: 8 distinct signals, cycled
-D = pyref.dropin_lib()
-D.ref_ms_encode.restype = C.c_long
-hashes, nbytes, counts = (C.c_uint64 * ns)(), (C.c_long * ns)(), (C.c_long * ns)()
-small = min(ns, 16)
-D.ref_ms_encode(small, ch, C.c_long(rate), C.c_float(q), 0, pcm.ctypes.data_as(C.c_void_p), C.c_long(n), hashes, nbytes, counts)  # warm-up
-t0 = time.perf_counter()
-blocks = D.ref_ms_encode(ns, ch, C.c_long(rate), C.c_float(q), 0, pcm.ctypes.data_as(C.c_void_p), C.c_long(n), hashes, nbytes, counts)
-dt_ms = time.perf_counter() - t0
-assert blocks > 0, "multi-stream driver failed"
+from oracle import encode_packets  # noqa: E402
+runs = {}
+for host in (True, False):
+    encode_packets.ms_encode(pcm[:min(ns, 16)], ch, rate, q, host_entropy=host)     # warm-up
+    t0 = time.perf_counter()
+    blocks, summ, on_device = encode_packets.ms_encode(pcm, ch, rate, q, host_entropy=host)
+    runs[host] = (blocks, summ, on_device, time.perf_counter() - t0)
+    assert on_device == (not host)
+    assert blocks > 0, "multi-stream driver failed"
+blocks, summ, _, dt_ms = runs[False]
+assert [s for s in runs[True][1]] == summ, "the host and the device path give different packets"
+counts = [s[0] for s in summ]
+nbytes = [s[1] for s in summ]
+hashes = [s[2] for s in summ]
 L = pyref.lib()
 L.ref_stock_encode_summary.restype = C.c_long
 k = min(args.stock_streams, ns)
@@ -59,9 +66,10 @@ print(json.dumps({
     "streams": ns, "blocks": int(blocks), "packets": int(pk),
     "dropin_packets_per_s": pk / dt_ms, "dropin_blocks_per_s": blocks / dt_ms, "dropin_seconds": dt_ms,
     "dropin_realtime_factor": ns * args.seconds / dt_ms,
+    "host_path_packets_per_s": pk / runs[True][3], "host_path_seconds": runs[True][3],
     "stock_streams_timed": k, "stock_packets_per_s": sum(counts[i] for i in range(k)) / dt_stock, "stock_blocks_per_s": sb / dt_stock,
     "stock_realtime_factor": k * args.seconds / dt_stock,
     "speedup_one_host_thread": (blocks / dt_ms) / (sb / dt_stock),
     "packets_identical_to_stock": True,
-    "note": "the host thread of the drop-in still runs the reference's floor1_encode and residue VQ/Huffman packing for every block "
-            "(north_star keeps them on the host); the device does the rest in one call per block size and round"}))
+    "note": "dropin_*: the device path (one vb200_encode_packets call per block size and round); host_path_*: the same "
+            "driver with the reference's floor1_encode and residue packing on the host threads"}))

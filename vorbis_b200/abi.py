@@ -235,6 +235,30 @@ class EntropySetup(C.Structure):
     ]
 
 
+class EncCodebook(C.Structure):
+    """vb200_enc_codebook"""
+    _fields_ = [
+        ("dim", C.c_int32),
+        ("entries", C.c_int32),
+        ("length", C.c_void_p),
+        ("codeword", C.c_void_p),
+        ("minval", C.c_int32),
+        ("delta", C.c_int32),
+        ("quantvals", C.c_int32),
+    ]
+
+
+class EncodeEntropySetup(C.Structure):
+    """struct vb200_encode_entropy_setup"""
+    _fields_ = [
+        ("nbooks", C.c_int32),
+        ("books", C.POINTER(EncCodebook)),
+        ("modebits", C.c_int32),
+        ("floor", (FloorDecode * MAX_SUBMAPS) * 2),
+        ("residue", (ResidueDecode * MAX_SUBMAPS) * 2),
+    ]
+
+
 class DecodeCarry(C.Structure):
     """vb200_decode_carry (include/vorbis_b200.h): tail [nstreams][ch][blocksizes[1]/2] float32, W [nstreams][ch]
     int32 (-1 = nothing decoded yet)"""

@@ -24,6 +24,7 @@
 #include "vb200_res.cuh"
 #include "vb200_streams.cuh"
 #include "vb200_managed.cuh"
+#include "vb200_entropy_enc.cuh"
 #include "floor1_db_table.h"
 
 using namespace vb200;
@@ -104,6 +105,11 @@ struct vb200_ctx {
   // vb200_decode_entropy_setup: the device tables of the entropy decoders (ent.books == nullptr: none registered)
   EntDev ent{};
   std::vector<void *> ent_owned;
+  // vb200_encode_entropy_setup: the tables of the entropy coder (eent.books == nullptr: none registered), and the
+  // scratch of the encode entropy entry points
+  EncEntDev eent{};
+  std::vector<void *> eent_owned;
+  DevBuf eent_buf[24];
   std::mutex mu;
   // optional per-kernel timing of the last Phase-A call (bench roofline evidence)
   bool profiling = false;
@@ -424,6 +430,8 @@ extern "C" void vb200_ctx_destroy(vb200_ctx *c) {
   for (auto &e : c->ev) if (e) cudaEventDestroy(e);
   if (c->ev_scratch) cudaEventDestroy(c->ev_scratch);
   for (void *p : c->ent_owned) cudaFree(p);
+  for (void *p : c->eent_owned) cudaFree(p);
+  for (auto &b : c->eent_buf) if (b.p) cudaFree(b.p);
   delete c;
 }
 
@@ -3047,6 +3055,310 @@ extern "C" int vb200_decode_packets_resume(vb200_ctx *c, int nstreams, int nblk,
   if ((rc = io.d2h(carry->tail, dkt, tbytes))) return rc;
   if ((rc = io.d2h(carry->W, dkw, sizeof(int32_t) * ntask))) return rc;
   return io.sync();
+}
+
+// ======================================================================== //
+// encode: the entropy coding of mapping0_forward on the device (vb200_entropy_enc.cuh)
+static const size_t EENT_SMEM_MAX = 200 * 1024;
+
+extern "C" int vb200_encode_entropy_setup(vb200_ctx *c, const struct vb200_encode_entropy_setup *es) {
+  CHECK_CTX(c);
+  if (!es || es->nbooks < 0 || (es->nbooks > 0 && !es->books)) return fail(VB200_EINVAL, "encode entropy setup");
+  if (es->modebits < 0 || es->modebits > 8) return fail(VB200_EINVAL, "modebits");
+  const vb200_setup &S = c->setup;
+  const int nb = es->nbooks, ch = S.channels;
+  std::vector<EncBook> books(nb > 0 ? nb : 1);
+  std::vector<unsigned char> len;
+  std::vector<uint32_t> cw;
+  std::vector<int> longest(nb > 0 ? nb : 1, 0);
+  for (int i = 0; i < nb; i++) {
+    const vb200_enc_codebook &b = es->books[i];
+    if (b.dim < 1 || b.entries < 0 || b.entries >= (1 << 24) || (b.entries > 0 && (!b.length || !b.codeword)))
+      return fail(VB200_EINVAL, "codebook dim / entries / arrays");
+    if (len.size() + (size_t)b.entries > (1u << 30)) return fail(VB200_EINVAL, "codebooks too large");
+    books[i] = EncBook{b.dim, b.entries, b.minval, b.delta, b.quantvals, (int)len.size()};
+    for (int e = 0; e < b.entries; e++) {
+      if (b.length[e] > 32) return fail(VB200_EINVAL, "codeword longer than 32 bits");
+      longest[i] = std::max(longest[i], (int)b.length[e]);
+    }
+    len.insert(len.end(), b.length, b.length + b.entries);
+    cw.insert(cw.end(), b.codeword, b.codeword + b.entries);
+  }
+  auto book_ok = [&](int b) { return b >= 0 && b < nb; };
+  EntFloor hf[2][VB200_MAX_SUBMAPS];
+  EntRes hr[2][VB200_MAX_SUBMAPS];
+  memset(hf, 0, sizeof(hf));
+  memset(hr, 0, sizeof(hr));
+  int slots[2] = {0, 0}, bound[2] = {0, 0};
+  for (int w = 0; w < 2; w++) {
+    const int n = S.blocksizes[w] / 2, subs = S.submaps[w];
+    if (subs < 1) return fail(VB200_EINVAL, "no submaps in the context setup");
+    for (int k = 0; k < ch; k++)
+      if (S.chmux[w][k] >= subs) return fail(VB200_EINVAL, "chmux past submaps");
+    for (int sm = 0; sm < VB200_MAX_SUBMAPS; sm++) hr[w][sm].type = -1;
+    long long nslot = 1 + ch, bits = 1 + es->modebits + (w ? 2 : 0);
+    for (int sm = 0; sm < subs; sm++) {
+      const vb200_floor_decode &f = es->floor[w][sm];
+      const vb200_floor1_setup &f1 = S.floor1[w][sm];
+      EntFloor &F = hf[w][sm];
+      if (f.type != 1) return fail(VB200_EIMPL, "only floor type 1 encodes on the device");
+      if (f1.posts <= 0) return fail(VB200_EINVAL, "no floor1 setup for a submap");
+      if (f.partitions < 0 || f.partitions > 31) return fail(VB200_EINVAL, "floor partitions");
+      int posts = 2;
+      for (int i = 0; i < f.partitions; i++) {
+        const int cl = f.partitionclass[i];
+        if (cl < 0 || cl > 15) return fail(VB200_EINVAL, "floor partition class");
+        if (f.class_dim[cl] < 1 || f.class_dim[cl] > 8 || f.class_subs[cl] < 0 || f.class_subs[cl] > 3)
+          return fail(VB200_EINVAL, "floor class dim / subs");
+        posts += f.class_dim[cl];
+      }
+      if (posts != f1.posts) return fail(VB200_EINVAL, "floor partitions do not give the floor's posts");
+      static const int quant_q[4] = {256, 128, 86, 64};
+      F.partitions = f.partitions; F.posts = f1.posts;
+      F.quant_q = quant_q[f1.mult - 1]; F.qbits = ilog_u((unsigned)F.quant_q - 1);
+      long long fbits = 1 + 2 * F.qbits;
+      for (int cl = 0; cl < 16; cl++) for (int j = 0; j < 8; j++) F.subbook[cl][j] = -1;
+      for (int i = 0; i < f.partitions; i++) {
+        const int cl = f.partitionclass[i];
+        F.pclass[i] = (unsigned char)cl;
+        F.cdim[cl] = (unsigned char)f.class_dim[cl]; F.csubs[cl] = (unsigned char)f.class_subs[cl];
+        if (f.class_subs[cl] && !book_ok(f.class_book[cl])) return fail(VB200_EINVAL, "floor class book");
+        F.cbook[cl] = (short)(f.class_subs[cl] ? f.class_book[cl] : 0);
+        int sub_longest = 0;
+        for (int j = 0; j < (1 << f.class_subs[cl]); j++) {
+          const int b = f.class_subbook[cl][j];
+          if (b != -1 && !book_ok(b)) return fail(VB200_EINVAL, "floor subclass book");
+          F.subbook[cl][j] = (short)b;
+          if (b >= 0) sub_longest = std::max(sub_longest, longest[b]);
+        }
+        fbits += (f.class_subs[cl] ? longest[f.class_book[cl]] : 0) + (long long)f.class_dim[cl] * sub_longest;
+      }
+      for (int k = 0; k < ch; k++) bits += S.chmux[w][k] == sm ? fbits : 0;
+      const vb200_residue_decode &r = es->residue[w][sm];
+      const vb200_residue_setup &rc = S.residue[w][sm];
+      EntRes &R = hr[w][sm];
+      if (r.type == 0) return fail(VB200_EIMPL, "residue type 0 does not encode on the device");
+      if (r.type != 1 && r.type != 2) return fail(VB200_EINVAL, "residue type");
+      int bundle = 0;
+      for (int k = 0; k < ch; k++) bundle += S.chmux[w][k] == sm;
+      const long limit = r.type == 2 ? (long)bundle * n : n;
+      if (r.grouping < 1 || r.begin < 0 || r.end < r.begin || r.end > limit)
+        return fail(VB200_EINVAL, "residue begin / end / grouping do not fit the block");
+      if (rc.type != r.type || rc.begin != r.begin || rc.end != r.end || rc.grouping != r.grouping ||
+          rc.partitions != r.partitions)
+        return fail(VB200_EINVAL, "residue differs from the context's classification setup");
+      if (r.partitions < 1 || r.partitions > 64 || !book_ok(r.groupbook)) return fail(VB200_EINVAL, "residue partitions / groupbook");
+      const int ppw = es->books[r.groupbook].dim;
+      long long pv = 1;
+      for (int j = 0; j < ppw && pv <= (1ll << 31); j++) pv *= r.partitions;
+      if (pv != r.partvals) return fail(VB200_EINVAL, "residue partvals != partitions ^ dim(groupbook)");
+      R.type = r.type; R.begin = r.begin; R.end = r.end; R.grouping = r.grouping; R.partvals = (r.end - r.begin) / r.grouping;
+      R.groupbook = r.groupbook; R.ppw = ppw; R.partitions = r.partitions; R.stages = 0;
+      int stage_longest[8] = {0, 0, 0, 0, 0, 0, 0, 0};
+      for (int cl = 0; cl < 64; cl++)
+        for (int st = 0; st < 8; st++) {
+          const int b = cl < r.partitions ? r.stagebook[cl][st] : -1;
+          if (b != -1 && !book_ok(b)) return fail(VB200_EINVAL, "residue stage book");
+          R.stagebook[cl][st] = (short)b;
+          if (b < 0) continue;
+          const vb200_enc_codebook &B = es->books[b];
+          long long lattice = 1;
+          for (int j = 0; j < B.dim && lattice <= B.entries; j++) lattice *= B.quantvals;
+          if (B.dim > 8 || B.quantvals <= 0 || lattice > B.entries)
+            return fail(VB200_EINVAL, "residue stage book: dim > 8 or a lattice that does not fit its entries");
+          R.stages = std::max(R.stages, st + 1);
+          stage_longest[st] = std::max(stage_longest[st], (r.grouping / B.dim) * longest[b]);
+        }
+      const long long nvec = r.type == 2 ? 1 : bundle, groups = (R.partvals + ppw - 1) / ppw;
+      nslot += groups * nvec + (long long)R.stages * R.partvals * nvec;
+      bits += nvec * groups * longest[r.groupbook];
+      for (int st = 0; st < R.stages; st++) bits += nvec * R.partvals * stage_longest[st];
+    }
+    if (sizeof(int) * (size_t)nslot > EENT_SMEM_MAX) return fail(VB200_EIMPL, "pieces of one packet exceed the shared memory");
+    if (bits >= (1ll << 31) - 64) return fail(VB200_EIMPL, "packet bound exceeds 2^31 bits");
+    slots[w] = (int)nslot;
+    bound[w] = (int)(((bits + 7) / 8 + 3) & ~3ll);
+  }
+  std::lock_guard<std::mutex> lk(c->mu);
+  CU(cudaStreamSynchronize(c->s_main));
+  CU(cudaDeviceSynchronize());                       // no kernel may still read the tables being replaced
+  for (void *p : c->eent_owned) cudaFree(p);
+  c->eent_owned.clear();
+  c->eent = EncEntDev{};
+  auto up = [&](const void *src, size_t bytes, const void **dst) -> int {
+    void *d = nullptr;
+    CU(cudaMalloc(&d, bytes ? bytes : 4));
+    c->eent_owned.push_back(d);
+    if (bytes) CU(cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice));
+    *dst = d;
+    return 0;
+  };
+  EncEntDev E{};
+  const void *p;
+  int rc;
+  if ((rc = up(books.data(), sizeof(EncBook) * books.size(), &p))) return rc;
+  E.books = (const EncBook *)p;
+  if ((rc = up(len.data(), len.size(), &p))) return rc;
+  E.len = (const unsigned char *)p;
+  if ((rc = up(cw.data(), sizeof(uint32_t) * cw.size(), &p))) return rc;
+  E.cw = (const uint32_t *)p;
+  for (int w = 0; w < 2; w++) {
+    if ((rc = up(hf[w], sizeof(hf[w]), &p))) return rc;
+    E.floor[w] = (const EntFloor *)p;
+    if ((rc = up(hr[w], sizeof(hr[w]), &p))) return rc;
+    E.res[w] = (const EntRes *)p;
+    E.submaps[w] = S.submaps[w]; E.slots[w] = slots[w]; E.bound[w] = bound[w];
+  }
+  E.ch = ch; E.modebits = es->modebits;
+  c->eent = E;
+  return 0;
+}
+
+extern "C" int vb200_encode_packet_bound(vb200_ctx *c, int W) {
+  CHECK_CTX(c); CHECK_W(W);
+  if (!c->eent.books) return fail(VB200_EINVAL, "no vb200_encode_entropy_setup registered");
+  return c->eent.bound[W];
+}
+
+// classification into scratch (k_residue_classify), then k_encode_packets; all pointers device
+static int encode_entropy_launch(vb200_ctx *c, int W, int nblocks, const vb200_block_desc *d_desc,
+                                 const int32_t *d_posts, const int32_t *d_nonzero, const int32_t *d_iwork,
+                                 int64_t pkt_stride, int32_t *d_bits, uint8_t *d_data, cudaStream_t st) {
+  const int ch = c->setup.channels, n = c->dx[W].N / 2, stride = c->res_partvals[W] > 0 ? c->res_partvals[W] : 1;
+  const int grid = grid_for(c, nblocks, 8);
+  void *cls, *work;
+  int rc;
+  if ((rc = ensure_buf(c->eent_buf[0], sizeof(int32_t) * (size_t)nblocks * ch * stride, &cls))) return rc;
+  if ((rc = ensure_buf(c->eent_buf[1], sizeof(int32_t) * (size_t)grid * ch * n, &work))) return rc;
+  if ((rc = vb200_residue_classify_dev(c, W, nblocks, d_iwork, d_nonzero, (int32_t *)cls, stride, st))) return rc;
+  EncArgs A;
+  A.E = c->eent; A.f1 = c->d_floor[W]; A.chmux = c->d_chmux[W]; A.desc = d_desc;
+  A.posts = d_posts; A.nonzero = d_nonzero; A.iwork = d_iwork; A.classes = (const int *)cls;
+  A.curve_rows = 0; A.work = (int *)work; A.W = W; A.nblocks = nblocks; A.n = n; A.class_stride = stride;
+  A.pkt_stride = pkt_stride; A.pkt_bits = d_bits; A.data = d_data;
+  const size_t smem = sizeof(int) * (size_t)c->eent.slots[W];
+  if ((rc = set_smem(k_encode_packets, smem))) return rc;
+  k_encode_packets<<<dim3(grid, 1), ENC_THREADS, smem, st>>>(A);
+  return post_launch(c);
+}
+
+static int encode_entropy_check(vb200_ctx *c, int nblocks) {
+  if (!c->eent.books) return fail(VB200_EINVAL, "no vb200_encode_entropy_setup registered");
+  if (nblocks < 0) return fail(VB200_EINVAL, "nblocks");
+  return 0;
+}
+
+extern "C" int vb200_encode_entropy_dev(vb200_ctx *c, int W, int nblocks, const vb200_block_desc *d_desc,
+                                        const int32_t *d_posts, const int32_t *d_nonzero, const int32_t *d_iwork,
+                                        int64_t pkt_stride, int32_t *d_pkt_bits, uint8_t *d_data, void *stream) {
+  CHECK_CTX(c); CHECK_W(W);
+  int rc;
+  if ((rc = encode_entropy_check(c, nblocks))) return rc;
+  if (pkt_stride % 4 || pkt_stride < c->eent.bound[W]) return fail(VB200_EINVAL, "pkt_stride: a multiple of 4, >= the packet bound");
+  if (nblocks == 0) return 0;
+  if (!d_desc || !d_posts || !d_nonzero || !d_iwork || !d_pkt_bits || !d_data) return fail(VB200_EINVAL, "encode_entropy pointers");
+  cudaStream_t st = (cudaStream_t)stream;
+  if ((rc = scratch_begin(c, st))) return rc;
+  if ((rc = encode_entropy_launch(c, W, nblocks, d_desc, d_posts, d_nonzero, d_iwork, pkt_stride, d_pkt_bits, d_data, st)))
+    return rc;
+  return scratch_end(c, st);
+}
+
+// host forms: packets of the strided device buffer packed back to back, then the counts, offsets and bytes copied
+// back (the bytes only when they fit data_cap).  Synchronises.
+static int packets_pack_d2h(vb200_ctx *c, int nblocks, const uint8_t *d_strided, int64_t stride, const int32_t *d_bits,
+                            int64_t *pkt_off, int32_t *pkt_bits, uint8_t *data, int64_t data_cap, cudaStream_t st) {
+  void *doff, *dpk;
+  int rc;
+  if ((rc = ensure_buf(c->eent_buf[2], sizeof(int64_t) * ((size_t)nblocks + 1), &doff))) return rc;
+  if ((rc = ensure_buf(c->eent_buf[3], (size_t)std::max<int64_t>(data_cap, 1), &dpk))) return rc;
+  k_packet_offsets<<<1, 1024, 0, st>>>(d_bits, nblocks, (long long *)doff);
+  if ((rc = post_launch(c))) return rc;
+  k_packet_gather<<<grid_for(c, nblocks, 8), 256, 0, st>>>(d_strided, stride, d_bits, (const long long *)doff, nblocks,
+                                                           data_cap, (uint8_t *)dpk);
+  if ((rc = post_launch(c))) return rc;
+  int64_t total = 0;
+  CU(cudaMemcpyAsync(pkt_bits, d_bits, sizeof(int32_t) * nblocks, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(pkt_off, doff, sizeof(int64_t) * nblocks, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(&total, (int64_t *)doff + nblocks, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  if (total > data_cap) return fail(VB200_EINVAL, "packets exceed data_cap (pkt_bits filled)");
+  if (total) CU(cudaMemcpyAsync(data, dpk, (size_t)total, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return 0;
+}
+
+extern "C" int vb200_encode_entropy(vb200_ctx *c, int W, int nblocks, const vb200_block_desc *desc, const int32_t *posts,
+                                    const int32_t *nonzero, const int32_t *iwork, int64_t *pkt_off, int32_t *pkt_bits,
+                                    uint8_t *data, int64_t data_cap) {
+  CHECK_CTX(c); CHECK_W(W);
+  int rc;
+  if ((rc = encode_entropy_check(c, nblocks))) return rc;
+  if (nblocks == 0) return 0;
+  if (!desc || !posts || !nonzero || !iwork || !pkt_off || !pkt_bits || (!data && data_cap > 0) || data_cap < 0)
+    return fail(VB200_EINVAL, "encode_entropy pointers");
+  std::lock_guard<std::mutex> lk(c->mu);
+  const size_t nb = (size_t)nblocks, ch = c->setup.channels, n = c->dx[W].N / 2;
+  const int64_t stride = c->eent.bound[W];
+  HostIO io{c};
+  void *dd, *dp, *dz, *di, *db, *ds;
+  if ((rc = io.h2d(desc, sizeof(vb200_block_desc) * nb, &dd))) return rc;
+  if ((rc = io.h2d(posts, sizeof(int32_t) * nb * ch * VB200_FLOOR1_STRIDE, &dp))) return rc;
+  if ((rc = io.h2d(nonzero, sizeof(int32_t) * nb * ch, &dz))) return rc;
+  if ((rc = io.h2d(iwork, sizeof(int32_t) * nb * ch * n, &di))) return rc;
+  if ((rc = io.h2d(nullptr, sizeof(int32_t) * nb, &db))) return rc;
+  if ((rc = io.h2d(nullptr, (size_t)stride * nb, &ds))) return rc;
+  if ((rc = vb200_encode_entropy_dev(c, W, nblocks, (const vb200_block_desc *)dd, (const int32_t *)dp,
+                                     (const int32_t *)dz, (const int32_t *)di, stride, (int32_t *)db, (uint8_t *)ds,
+                                     c->s_main))) return rc;
+  return packets_pack_d2h(c, nblocks, (const uint8_t *)ds, stride, (const int32_t *)db, pkt_off, pkt_bits, data,
+                          data_cap, c->s_main);
+}
+
+extern "C" int vb200_encode_packets(vb200_ctx *c, int W, int nstreams, int bps, int blobno, const vb200_encode_io *h,
+                                    int64_t *pkt_off, int32_t *pkt_bits, uint8_t *data, int64_t data_cap) {
+  CHECK_CTX(c); CHECK_W(W);
+  int rc;
+  if (!c->eent.books) return fail(VB200_EINVAL, "no vb200_encode_entropy_setup registered");
+  if (!h || h->posts || h->nonzero || h->iwork || h->classes || h->overflow || h->mdct || h->logmdct || h->logmask ||
+      h->iwork_fmt != VB200_IWORK_S32)
+    return fail(VB200_EINVAL, "encode_packets: posts / nonzero / iwork / classes / overflow / spectra must be NULL");
+  if (!pkt_off || !pkt_bits || (!data && data_cap > 0) || data_cap < 0) return fail(VB200_EINVAL, "encode_packets outputs");
+  vb200_encode_io d = *h;
+  int32_t one = 0;                                   // enc_check wants the outputs it does not see here
+  d.posts = d.nonzero = &one; d.iwork = &one;
+  if ((rc = enc_check(c, W, nstreams, bps, blobno, &d))) return rc;
+  std::lock_guard<std::mutex> lk(c->mu);
+  const int ch = c->setup.channels, N = c->dx[W].N, n = N / 2;
+  const size_t nb = (size_t)nstreams * bps, rows = nb * ch;
+  const int64_t stride = c->eent.bound[W];
+  cudaStream_t st = c->s_main;
+  DevBuf *B = c->eent_buf + 4;
+  void *p;
+  const size_t pcm_bytes = enc_pcm_bytes(h, ch, N, nstreams, bps);
+  if ((rc = ensure_buf(B[0], pcm_bytes, &p))) return rc; d.pcm = p;
+  if ((rc = ensure_buf(B[1], sizeof(vb200_block_desc) * nb, &p))) return rc; d.desc = (const vb200_block_desc *)p;
+  if ((rc = ensure_buf(B[2], sizeof(float) * nstreams, &p))) return rc; d.ampmax0 = h->ampmax0 ? (const float *)p : nullptr;
+  if ((rc = ensure_buf(B[3], sizeof(int32_t) * rows * VB200_FLOOR1_STRIDE, &p))) return rc; d.posts = (int32_t *)p;
+  if ((rc = ensure_buf(B[4], sizeof(int32_t) * rows, &p))) return rc; d.nonzero = (int32_t *)p;
+  if ((rc = ensure_buf(B[5], sizeof(int32_t) * rows * n, &p))) return rc; d.iwork = p;
+  if ((rc = ensure_buf(B[6], sizeof(float) * nb, &p))) return rc; d.ampmax_out = (float *)p;
+  if ((rc = ensure_buf(B[7], sizeof(int32_t) * nb, &p))) return rc;
+  int32_t *dbits = (int32_t *)p;
+  if ((rc = ensure_buf(B[8], (size_t)stride * nb, &p))) return rc;
+  uint8_t *dstr = (uint8_t *)p;
+  EncScratch S;
+  if ((rc = enc_scratch(B + 9, rows, nb, n, nullptr, false, &S))) return rc;
+  CU(cudaMemcpyAsync((void *)d.pcm, h->pcm, pcm_bytes, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync((void *)d.desc, h->desc, sizeof(vb200_block_desc) * nb, cudaMemcpyHostToDevice, st));
+  if (h->ampmax0) CU(cudaMemcpyAsync((void *)d.ampmax0, h->ampmax0, sizeof(float) * nstreams, cudaMemcpyHostToDevice, st));
+  if ((rc = scratch_begin(c, st))) return rc;
+  if ((rc = encode_launch(c, W, nstreams, bps, blobno, &d, S, st))) return rc;
+  if ((rc = encode_entropy_launch(c, W, (int)nb, d.desc, d.posts, d.nonzero, (const int32_t *)d.iwork, stride, dbits,
+                                  dstr, st))) return rc;
+  if ((rc = scratch_end(c, st))) return rc;
+  CU(cudaMemcpyAsync(h->ampmax_out, d.ampmax_out, sizeof(float) * nb, cudaMemcpyDeviceToHost, st));
+  return packets_pack_d2h(c, (int)nb, dstr, stride, dbits, pkt_off, pkt_bits, data, data_cap, st);
 }
 
 // ======================================================================== //

@@ -14,7 +14,9 @@
  *                                                        floor bits and _residue_P[]->class / ->forward
  *                                                        (lib/mapping0.c:660-683) for the residue
  *   a loop of vorbis_analysis over N encoders        ->  vb200ms_*: blockout for every stream, the blocks that are
- *                                                        ready go to the device together, packets come back per stream
+ *                                                        ready go to the device together, packets come back per stream;
+ *                                                        un-managed, the packets are entropy coded on the device too
+ *                                                        (one vb200_encode_packets call per block size and round)
  *
  * floor1_encode is fed the device's posts re-expanded to the fit scale: its quantise step maps them back to
  * the same integers and its predict/flag pass is idempotent on them, so it writes exactly the bits it would
@@ -139,12 +141,14 @@ static int pack_block(vorbis_block *vb, const int32_t *posts, const int32_t *non
 typedef struct {
   float *pcm; vb200_block_desc *desc; int32_t *posts, *nonzero, *iwork; float *ampmax;
   size_t cap_blocks; int ch, N, curves;
+  uint8_t *pkt; int64_t *pkt_off; int32_t *pkt_bits; size_t pkt_cap;   /* the device coder's packed packets */
 } ms_batch;
 
 /* curves: 1 (un-managed) or PACKETBLOBS (bitrate-managed: posts / nonzero / iwork hold every curve, blob-major) */
 static int batch_reserve(ms_batch *B, size_t nb, int ch, int N, int curves){
   if(B->cap_blocks >= nb && B->ch == ch && B->N == N && B->curves == curves) return 0;
   free(B->pcm); free(B->desc); free(B->posts); free(B->nonzero); free(B->iwork); free(B->ampmax);
+  free(B->pkt); free(B->pkt_off); free(B->pkt_bits);
   memset(B, 0, sizeof(*B));
   B->pcm = (float*)malloc(sizeof(float)*nb*ch*N);
   B->desc = (vb200_block_desc*)malloc(sizeof(vb200_block_desc)*nb);
@@ -214,6 +218,131 @@ static int forward_batch(vb200_binding *bind, ms_batch *B, vorbis_block **blocks
   return err;
 }
 
+/* ---- the device entropy coder ------------------------------------------------------------------------------------ */
+static int ms_ilog(unsigned v){ int r = 0; while(v){ r++; v >>= 1; } return r; }
+
+/* The struct vb200_encode_entropy_setup of an encoder after vorbis_analysis_init: every book of ci->fullbooks (its
+ * lengthlist, codelist and integer lattice), the floor-1 and residue fields of both modes' submaps with the stage
+ * books laid out as res0_look lays out partbooks (lib/res0.c:274-292), modebits.  The codeword arrays point into the
+ * encoder's own books, so the setup is valid as long as that vorbis_info; es->books is malloc'd (free() it).
+ * Returns 0, OV_EIMPL for a mode layout the device coder does not take, or OV_EFAULT. */
+int vb200ms_entropy_setup_build(vorbis_dsp_state *vd, struct vb200_encode_entropy_setup *es){
+  codec_setup_info *ci = (codec_setup_info*)vd->vi->codec_setup;
+  private_state *b = (private_state*)vd->backend_state;
+  vb200_enc_codebook *books;
+  int i, w, j, k;
+  memset(es, 0, sizeof(*es));
+  if(ci->modes != 2 || !ci->fullbooks) return OV_EIMPL;
+  books = (vb200_enc_codebook*)calloc(ci->books > 0 ? ci->books : 1, sizeof(*books));
+  if(!books) return OV_EFAULT;
+  for(i = 0; i < ci->books; i++){
+    const codebook *cb = ci->fullbooks + i;
+    books[i].dim = (int32_t)cb->dim; books[i].entries = (int32_t)cb->entries;
+    books[i].length = (const uint8_t*)cb->c->lengthlist; books[i].codeword = cb->codelist;
+    books[i].minval = cb->minval; books[i].delta = cb->delta; books[i].quantvals = cb->quantvals;
+  }
+  es->nbooks = ci->books; es->books = books; es->modebits = b->modebits;
+  for(w = 0; w < 2; w++){
+    vorbis_info_mapping0 *mp;
+    if(ci->mode_param[w]->blockflag != w || ci->map_type[ci->mode_param[w]->mapping] != 0) goto impl;
+    mp = (vorbis_info_mapping0*)ci->map_param[ci->mode_param[w]->mapping];
+    if(mp->submaps > VB200_MAX_SUBMAPS) goto impl;
+    for(j = 0; j < VB200_MAX_SUBMAPS; j++) es->residue[w][j].type = -1;
+    for(j = 0; j < mp->submaps; j++){
+      const int fl = mp->floorsubmap[j], rs = mp->residuesubmap[j];
+      vb200_floor_decode *f = &es->floor[w][j];
+      vb200_residue_decode *r = &es->residue[w][j];
+      const vorbis_info_residue0 *ri = (const vorbis_info_residue0*)ci->residue_param[rs];
+      int acc = 0, c;
+      f->type = ci->floor_type[fl];
+      if(f->type == 1){
+        const vorbis_info_floor1 *fi = (const vorbis_info_floor1*)ci->floor_param[fl];
+        f->partitions = fi->partitions;
+        for(k = 0; k < fi->partitions && k < 31; k++) f->partitionclass[k] = fi->partitionclass[k];
+        for(k = 0; k < 16; k++){
+          int s;
+          f->class_dim[k] = fi->class_dim[k]; f->class_subs[k] = fi->class_subs[k]; f->class_book[k] = fi->class_book[k];
+          for(s = 0; s < 8; s++) f->class_subbook[k][s] = fi->class_subbook[k][s];
+        }
+      }
+      r->type = ci->residue_type[rs];
+      r->begin = (int32_t)ri->begin; r->end = (int32_t)ri->end; r->grouping = ri->grouping;
+      r->partitions = ri->partitions; r->groupbook = ri->groupbook;
+      r->partvals = 1;                                     /* look->partvals of res0_look (lib/res0.c:296) */
+      for(k = 0; k < ci->fullbooks[ri->groupbook].dim; k++) r->partvals *= ri->partitions;
+      for(c = 0; c < 64; c++){
+        const int stages = c < ri->partitions ? ms_ilog((unsigned)ri->secondstages[c]) : 0;
+        for(k = 0; k < 8; k++)
+          r->stagebook[c][k] = k < stages && (ri->secondstages[c] & (1 << k)) ? ri->booklist[acc++] : -1;
+      }
+    }
+  }
+  return 0;
+impl:
+  free(books);
+  es->books = NULL;
+  return OV_EIMPL;
+}
+
+/* blocks[0..nb) of one size, un-managed, entropy coded on the device: ONE vb200_encode_packets call (PCM in, packets
+ * out), then per block on all host threads the state mapping0_forward leaves (vbi->ampmax, vb->mode) and the packet
+ * bits into packetblob[PACKETBLOBS/2], in pieces of up to 32 bits (oggpack_write is all that libogg and the
+ * stand-in both provide) */
+static int forward_batch_packets(vb200_binding *bind, ms_batch *B, vorbis_block **blocks, int nb, int W, batch_after after,
+                                 void *user){
+  vb200_ctx *ctx = vb200shim_ctx(bind);
+  vorbis_info *vi = blocks[0]->vd->vi;
+  const int ch = vi->channels, N = (int)blocks[0]->pcmend;
+  const int bound = vb200_encode_packet_bound(ctx, W);
+  vb200_encode_io io;
+  int i, c, rc;
+  PROF_T0();
+  if(bound < 0) return OV_EFAULT;
+  if((rc = batch_reserve(B, (size_t)nb, ch, N, 1))) return rc;
+  if(B->pkt_cap < (size_t)nb*bound || !B->pkt_off){
+    free(B->pkt); free(B->pkt_off); free(B->pkt_bits);
+    B->pkt = (uint8_t*)malloc((size_t)nb*bound); B->pkt_off = (int64_t*)malloc(sizeof(int64_t)*B->cap_blocks);
+    B->pkt_bits = (int32_t*)malloc(sizeof(int32_t)*B->cap_blocks);
+    B->pkt_cap = B->pkt ? (size_t)nb*bound : 0;
+    if(!B->pkt || !B->pkt_off || !B->pkt_bits) return OV_EFAULT;
+  }
+#pragma omp parallel for private(c) schedule(static) if(nb > 8)
+  for(i = 0; i < nb; i++){
+    vorbis_block_internal *vbi = (vorbis_block_internal*)blocks[i]->internal;
+    for(c = 0; c < ch; c++) memcpy(B->pcm + ((size_t)i*ch + c)*N, blocks[i]->pcm[c], sizeof(float)*N);
+    B->desc[i].lW = (int32_t)blocks[i]->lW; B->desc[i].nW = (int32_t)blocks[i]->nW;
+    B->desc[i].blocktype = vbi->blocktype; B->desc[i].ampmax = vbi->ampmax;
+  }
+  memset(&io, 0, sizeof(io));
+  io.pcm = B->pcm; io.pcm_fmt = VB200_PCM_F32_BLOCKS; io.desc = B->desc; io.independent = 1; io.ampmax_out = B->ampmax;
+  PROF_ADD(2);
+  rc = vb200_encode_packets(ctx, W, nb, 1, PACKETBLOBS/2, &io, B->pkt_off, B->pkt_bits, B->pkt, (int64_t)B->pkt_cap);
+  PROF_ADD(3);
+  if(rc){
+    vb200shim_set_error(bind, rc);
+    fprintf(stderr, "vb200 mapping0: vb200_encode_packets failed (%d): %s\n", rc, vb200_last_error());
+    return OV_EFAULT;
+  }
+#pragma omp parallel for schedule(dynamic, 4) if(nb > 8)
+  for(i = 0; i < nb; i++){
+    vorbis_block_internal *vbi = (vorbis_block_internal*)blocks[i]->internal;
+    oggpack_buffer *opb = vbi->packetblob[PACKETBLOBS/2];
+    const uint8_t *p = B->pkt + B->pkt_off[i];
+    long k;
+    vbi->ampmax = B->ampmax[i];                                /* lib/mapping0.c:576 */
+    blocks[i]->mode = W;
+    for(k = 0; k < B->pkt_bits[i]; k += 32){
+      const int take = B->pkt_bits[i] - k < 32 ? (int)(B->pkt_bits[i] - k) : 32, nbytes = (take + 7) >> 3;
+      unsigned long v = 0;
+      for(c = 0; c < nbytes; c++) v |= (unsigned long)p[(k >> 3) + c] << (8*c);
+      oggpack_write(opb, v, take);
+    }
+    if(after) after(user, i);
+  }
+  PROF_ADD(4);
+  return 0;
+}
+
 /* ---- seam 1: vorbis_func_mapping ---------------------------------------------------------------------------- */
 static ms_batch g_single[2];                                   /* the single-block path's staging (one per block size) */
 
@@ -266,6 +395,8 @@ typedef struct vb200ms {
   int32_t *env_state; uint8_t *env_ret; size_t env_ret_cap;
   int threads;
   vb200ms_sink_t sink; void *sink_user; int cur_w;
+  int entropy_dev;               /* the context took the encoder's vb200_encode_entropy_setup (un-managed only) */
+  int host_entropy;              /* diagnostic: code on the host anyway (vb200ms_set_host_entropy) */
 } vb200ms;
 
 void vb200ms_close(vb200ms *m){
@@ -286,6 +417,7 @@ void vb200ms_close(vb200ms *m){
   for(w = 0; w < 2; w++){
     free(m->batch[w].pcm); free(m->batch[w].desc); free(m->batch[w].posts); free(m->batch[w].nonzero);
     free(m->batch[w].iwork); free(m->batch[w].ampmax); free(m->ready[w]); free(m->ready_stream[w]);
+    free(m->batch[w].pkt); free(m->batch[w].pkt_off); free(m->batch[w].pkt_bits);
   }
   free(m->env_first); free(m->env_steps); free(m->env_list); free(m->env_nsteps); free(m->env_pcm); free(m->env_state); free(m->env_ret);
   free(m->vi); free(m->vd); free(m->vb); free(m);
@@ -349,8 +481,26 @@ static vb200ms *ms_open(int nstreams, int channels, long rate, float quality, in
   }
   if(vb200shim_attach(&m->vd[0], device)){ vb200ms_close(m); return NULL; }
   m->bind = vb200shim_binding(&m->vd[0]);
+  if(!managed){                  /* the device coder where the context takes this setup, else the host path */
+    struct vb200_encode_entropy_setup es;
+    int rc = vb200ms_entropy_setup_build(&m->vd[0], &es);
+    if(!rc){
+      rc = vb200_encode_entropy_setup(vb200shim_ctx(m->bind), &es);
+      free((void*)es.books);
+    }
+    if(rc && rc != VB200_EIMPL){                      /* == OV_EIMPL */
+      fprintf(stderr, "vb200 multistream: encode entropy setup failed (%d): %s\n", rc, vb200_last_error());
+      vb200ms_close(m);
+      return NULL;
+    }
+    m->entropy_dev = rc == 0;
+  }
   return m;
 }
+
+int vb200ms_entropy_on_device(vb200ms *m){ return m->entropy_dev && !m->host_entropy; }
+void vb200ms_set_host_entropy(vb200ms *m, int on){ m->host_entropy = on ? 1 : 0; }
+vb200_ctx *vb200ms_context(vb200ms *m){ return vb200shim_ctx(m->bind); }
 
 vb200ms *vb200ms_open(int nstreams, int channels, long rate, float quality, int device){
   return ms_open(nstreams, channels, rate, quality, 0, -1, -1, -1, device);
@@ -453,7 +603,9 @@ int vb200ms_round(vb200ms *m, vb200ms_sink sink, void *user){
   for(w = 0; w < 2; w++){
     if(!cnt[w]) continue;
     m->cur_w = w;
-    if((rc = forward_batch(m->bind, &m->batch[w], m->ready[w], cnt[w], w, round_after, m))) return rc;
+    rc = vb200ms_entropy_on_device(m) ? forward_batch_packets(m->bind, &m->batch[w], m->ready[w], cnt[w], w, round_after, m)
+                                      : forward_batch(m->bind, &m->batch[w], m->ready[w], cnt[w], w, round_after, m);
+    if(rc) return rc;
     total += cnt[w];
   }
   return total;

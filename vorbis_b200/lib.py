@@ -37,6 +37,8 @@ EXPORTS = [
     "vb200_decode_dsp_resume_dev", "vb200_decode_dsp_resume",
     "vb200_decode_entropy_setup", "vb200_decode_entropy_dev", "vb200_decode_entropy",
     "vb200_decode_packets_resume_dev", "vb200_decode_packets_resume",
+    "vb200_encode_entropy_setup", "vb200_encode_packet_bound", "vb200_encode_entropy_dev", "vb200_encode_entropy",
+    "vb200_encode_packets",
     "vb200_residue_partvals", "vb200_residue_classify_dev", "vb200_residue_classify",
     "vb200_plan_blocks", "vb200_encode_streams_dev", "vb200_encode_streams",
     "vb200_encode_streams_managed_dev", "vb200_encode_streams_managed",
@@ -123,6 +125,12 @@ def load():
                                                   C.c_int64, C.POINTER(abi.DecodeCarry), vp]
     L.vb200_decode_packets_resume.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, C.c_int64, vp, vp, vp, C.c_int64, vp,
                                               vp, C.c_int, C.c_int64, C.POINTER(abi.DecodeCarry)]
+    L.vb200_encode_entropy_setup.argtypes = [vp, C.POINTER(abi.EncodeEntropySetup)]
+    L.vb200_encode_packet_bound.argtypes = [vp, C.c_int]
+    L.vb200_encode_entropy_dev.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int64, vp, vp, vp]
+    L.vb200_encode_entropy.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp, C.c_int64]
+    L.vb200_encode_packets.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(abi.EncodeIO), vp, vp, vp,
+                                       C.c_int64]
     L.vb200_envelope_search_dev.argtypes = [vp, C.c_int, vp, C.c_int, C.c_int64, C.c_int, C.c_int, vp, vp, vp]
     L.vb200_envelope_search.argtypes = [vp, C.c_int, vp, C.c_int, C.c_int64, C.c_int, C.c_int, vp, vp]
     L.vb200_envelope_apply_marks.argtypes = [vp, C.c_int, C.c_int, vp]
@@ -653,6 +661,84 @@ class Context:
                                                          _ptr(d_pkt_bytes), _ptr(d_data), _ptr(d_pcm_off),
                                                          _ptr(d_pcm), pcm_s16, pcm_stride, C.byref(k),
                                                          _ptr(stream)))
+
+    # ---- encode: the entropy coding of mapping0_forward on the device -----------------------------
+    def encode_entropy_setup(self, es):
+        """vb200_encode_entropy_setup with an abi.EncodeEntropySetup"""
+        self._chk(self.L.vb200_encode_entropy_setup(self.h, C.byref(es)))
+
+    def packet_bound(self, W):
+        b = self.L.vb200_encode_packet_bound(self.h, W)
+        if b < 0:
+            self._chk(b)
+        return b
+
+    @staticmethod
+    def _packets(out, nb):
+        off, bits, data = out["pkt_off"], out["pkt_bits"], out["data"]
+        out["packets"] = [bytes(data[off[i]:off[i] + (bits[i] + 7) // 8]) for i in range(nb)]
+        return out
+
+    def encode_entropy(self, W, desc, posts, nonzero, iwork, data_cap=None, check=True):
+        """vb200_encode_entropy on vb200_encode_dsp's outputs: {"packets": [bytes], "pkt_bits", "pkt_off", "data"}
+        (and "rc" when check is False, in which case an error does not raise)"""
+        ch, n = self.channels, self.bs[W] // 2
+        desc = np.ascontiguousarray(desc, abi.BLOCKDESC_DTYPE)
+        nb = desc.shape[0]
+        posts = np.ascontiguousarray(posts, np.int32).reshape(nb, ch, abi.FLOOR1_STRIDE)
+        nonzero = np.ascontiguousarray(nonzero, np.int32).reshape(nb, ch)
+        iwork = np.ascontiguousarray(iwork, np.int32).reshape(nb, ch, n)
+        cap = nb * self.packet_bound(W) if data_cap is None else data_cap
+        out = {"pkt_off": np.zeros(nb, np.int64), "pkt_bits": np.zeros(nb, np.int32),
+               "data": np.zeros(max(cap, 1), np.uint8)}
+        rc = self.L.vb200_encode_entropy(self.h, W, nb, _ptr(desc), _ptr(posts), _ptr(nonzero), _ptr(iwork),
+                                         _ptr(out["pkt_off"]), _ptr(out["pkt_bits"]), _ptr(out["data"]), cap)
+        if not check:
+            out["rc"] = rc
+            return out
+        self._chk(rc)
+        return self._packets(out, nb)
+
+    def encode_entropy_dev(self, W, nblocks, d_desc, d_posts, d_nonzero, d_iwork, pkt_stride, d_pkt_bits, d_data,
+                           stream=None, check=True):
+        rc = self.L.vb200_encode_entropy_dev(self.h, W, nblocks, _ptr(d_desc), _ptr(d_posts), _ptr(d_nonzero),
+                                             _ptr(d_iwork), pkt_stride, _ptr(d_pkt_bits), _ptr(d_data), _ptr(stream))
+        if check:
+            self._chk(rc)
+        return rc
+
+    def encode_packets(self, W, pcm, desc, nstreams=None, fmt=0, hop=0, ampmax0=None, independent=None, blobno=7,
+                       data_cap=None):
+        """vb200_encode_packets: PCM as for encode_dsp in, {"packets", "pkt_bits", "pkt_off", "data", "ampmax_out"}
+        out"""
+        ch, N = self.channels, self.bs[W]
+        desc = np.ascontiguousarray(desc, abi.BLOCKDESC_DTYPE)
+        nb = desc.shape[0]
+        if nstreams is None:
+            nstreams = nb
+            if independent is None:
+                independent = True
+        io = abi.EncodeIO()
+        if fmt == 0:
+            pcm = np.ascontiguousarray(pcm, np.float32).reshape(nb, ch, N)
+        elif fmt == PCM_F32_PLANAR:
+            pcm = np.ascontiguousarray(pcm, np.float32)
+            io.stream_stride = pcm.shape[2]
+        else:
+            pcm = np.ascontiguousarray(pcm, np.int16)
+            io.stream_stride = pcm.shape[1]
+        io.pcm, io.pcm_fmt, io.hop, io.desc = pcm.ctypes.data, fmt, hop, desc.ctypes.data
+        io.independent = 1 if independent else 0
+        if ampmax0 is not None:
+            ampmax0 = np.ascontiguousarray(ampmax0, np.float32)
+            io.ampmax0 = ampmax0.ctypes.data
+        cap = nb * self.packet_bound(W) if data_cap is None else data_cap
+        out = {"pkt_off": np.zeros(nb, np.int64), "pkt_bits": np.zeros(nb, np.int32),
+               "data": np.zeros(max(cap, 1), np.uint8), "ampmax_out": np.zeros(nb, np.float32)}
+        io.ampmax_out = out["ampmax_out"].ctypes.data
+        self._chk(self.L.vb200_encode_packets(self.h, W, nstreams, nb // nstreams, blobno, C.byref(io),
+                                              _ptr(out["pkt_off"]), _ptr(out["pkt_bits"]), _ptr(out["data"]), cap))
+        return self._packets(out, nb)
 
     # ---- envelope / block-switch detector (lib/envelope.c) --------------------------------------
     def envelope_search(self, pcm, first_step, nsteps, state=None, fmt=PCM_F32_PLANAR):
