@@ -180,7 +180,9 @@ int  vb200_phaseA_kernel_ms(vb200_ctx *ctx, float *ms3);
  * couple_quantize_normalize (+ nonzero propagation)                                            */
 int  vb200_encode_dsp_kernel_ms(vb200_ctx *ctx, float *ms6);
 /* development aid: with env VB200_PHASE_TIMING set, the psy kernel adds the SM cycles each of
- * its 11 barrier-delimited phases took (thread 0 of every CTA) into a 16-slot counter array. */
+ * its 11 barrier-delimited phases took (thread 0 of every CTA) into a 16-slot counter array;
+ * with env VB200_FLOOR1_TIMING set, the floor-1 fit adds its per-phase cycles and per-row counts
+ * (summed over its warps, layout in tools/floor1_phase_timing.py) into the same array.          */
 int  vb200_debug_phase_cycles(vb200_ctx *ctx, unsigned long long *out16, int reset);
 
 /* ---- transforms (SURVEY §8 a2-a5) ------------------------------------- */

@@ -276,6 +276,8 @@ static inline cudaError_t cudaEventRecord(cudaEvent_t, cudaStream_t = nullptr) {
 static inline cudaError_t cudaEventSynchronize(cudaEvent_t) { return cudaSuccess; }
 static inline cudaError_t cudaEventElapsedTime(float *ms, cudaEvent_t, cudaEvent_t) { *ms = 0.f; return cudaSuccess; }
 template <class K> static inline cudaError_t cudaFuncSetAttribute(K, cudaFuncAttribute, int) { return cudaSuccess; }
+enum { cudaSharedmemCarveoutMaxShared = 100 };
+template <class K> static inline cudaError_t cudaOccupancyMaxActiveBlocksPerMultiprocessor(int *n, K, int, size_t) { *n = 1; return cudaSuccess; }
 
 // ---- launch --------------------------------------------------------------------------------
 namespace cuemu {

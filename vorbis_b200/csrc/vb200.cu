@@ -461,7 +461,8 @@ extern "C" int vb200_set_profiling(vb200_ctx *c, int on) {
   return 0;
 }
 
-// dev aid: per-phase cycle sums of k_phaseA_psy3 (its DBG instance) accumulated while VB200_PHASE_TIMING is set
+// dev aid: per-phase cycle sums of k_phaseA_psy3 (its DBG instance) accumulated while VB200_PHASE_TIMING is set,
+// and of k_floor1_fit (its DBG instance) while VB200_FLOOR1_TIMING is set
 extern "C" int vb200_debug_phase_cycles(vb200_ctx *c, unsigned long long *out16, int reset) {
   if (!c || !out16) return fail(VB200_EINVAL, "null argument");
   CU(cudaSetDevice(c->device));
@@ -1760,10 +1761,23 @@ extern "C" int vb200_floor1_fit_dev(vb200_ctx *c, int W, int floor_sel, int nrow
   if (nrows <= 0) return 0;
   Floor1Args a; int rc;
   if ((rc = floor1_args(c, W, floor_sel, nrows, &a))) return rc;
-  const size_t smem = sizeof(Floor1Dev) * VB200_MAX_SUBMAPS + floor1_fit_smem_per_warp(a.n) * F1_WARPS;
-  if ((rc = set_smem(k_floor1_fit, smem))) return rc;
+  // the per-warp area holds floors of the largest post count this block size has, not VB200_VIF_POSIT
+  int pcap = 2;
+  for (int k = 0; k < VB200_MAX_SUBMAPS; k++) pcap = std::max(pcap, c->setup.floor1[W][k].posts);
+  const size_t smem = sizeof(Floor1Dev) * VB200_MAX_SUBMAPS + floor1_fit_smem_per_warp(a.n, pcap) * F1_WARPS;
   const int ctas = (nrows + F1_WARPS - 1) / F1_WARPS;
-  k_floor1_fit<<<grid_for(c, ctas, 8), 32 * F1_WARPS, smem, (cudaStream_t)stream>>>(a, d_logmdct, d_logmask, d_posts, d_fit_nonzero);
+  const bool dbg = getenv("VB200_FLOOR1_TIMING") != nullptr;   // the instance with clock marks (tools/floor1_phase_timing.py)
+  void (*kern)(Floor1Args, int, const float *, const float *, int32_t *, int32_t *, unsigned long long *) =
+      dbg ? k_floor1_fit<true> : k_floor1_fit<false>;
+  void *p = nullptr;
+  if (dbg && (rc = ensure(c, 10, 16 * sizeof(unsigned long long), &p))) return rc;
+  if ((rc = set_smem(kern, smem))) return rc;
+  // one wave: as many CTAs per SM as registers and this shared-memory size let be resident
+  CU(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+  int per_sm = 0;
+  CU(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, 32 * F1_WARPS, smem));
+  kern<<<grid_for(c, ctas, std::max(per_sm, 1)), 32 * F1_WARPS, smem, (cudaStream_t)stream>>>(
+      a, pcap, d_logmdct, d_logmask, d_posts, d_fit_nonzero, (unsigned long long *)p);
   return post_launch(c);
 }
 

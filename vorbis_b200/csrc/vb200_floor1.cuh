@@ -45,11 +45,23 @@ struct Floor1Args {
 };
 
 #define F1_WARPS 8
+// k_floor1_fit's register bound: 4 CTAs (32 warps) per SM.  The fit is bound by instruction issue rather than by
+// latency: on an H100 forcing 5 or 6 CTAs per SM (48 or 40 registers, a few spills) made it 1-2 % slower, not faster
+#define F1_FIT_CTAS 4
 #define F1_ACC 12                      // xa ya x2a y2a xya an | xb yb x2b y2b xyb bn
-#define F1_STATE (3 * (VB200_VIF_POSIT + 2) + 3 * ((VB200_VIF_POSIT + 2 + 1) / 2))   // A, B, out int; lon, hin, memo short
 
-__host__ __device__ inline size_t floor1_fit_smem_per_warp(int n) {
-  return ((sizeof(unsigned short) * (size_t)n + 7) & ~(size_t)7) + sizeof(int) * ((VB200_VIF_POSIT + 1) * F1_ACC + F1_STATE);
+struct F1Post {                        // the split loop's state of one post (fitA, fitB, loneighbor, hineighbor, memo)
+  int A, B, out;
+  signed char lon, hin, memo, pad;     // post indices (< VB200_VIF_POSIT + 2) or -1
+};
+static_assert(sizeof(F1Post) % 8 == 0 && VB200_VIF_POSIT + 2 <= 127,
+              "every warp's area in k_floor1_fit starts 8-byte aligned (its fp64 terms come first)");
+
+// a warp's shared memory in k_floor1_fit, for floors of at most `posts` posts and rows of n lines: the fit terms
+// (12 ints or 6 doubles per gap), the per-post state, the quantised row
+__host__ __device__ inline size_t floor1_fit_smem_per_warp(int n, int posts) {
+  return sizeof(int) * F1_ACC * (size_t)(posts - 1) + sizeof(F1Post) * (size_t)posts +
+         ((sizeof(unsigned short) * (size_t)n + 7) & ~(size_t)7);
 }
 
 __device__ __forceinline__ int f1_dBquant(float x) {               // lib/floor1.c:278-283
@@ -96,56 +108,96 @@ struct F1Line {
   }
 };
 
-__device__ __forceinline__ int f1_postY(const int *A, const int *B, int pos) {
-  const int a = A[pos], b = B[pos];
+__device__ __forceinline__ int f1_postY(const F1Post *st, int pos) {
+  const int a = st[pos].A, b = st[pos].B;
   if (a < 0) return b;
   if (b < 0) return a;
   return (a + b) >> 1;
 }
 
+// inspect_error's closing tests (lib/floor1.c:558-563) without a division per call.  fl(fl(maxover*maxover)/cnt) >
+// maxerr cannot turn from false to true as cnt grows (correctly rounded division is monotone), nor can the maxunder
+// test, so "either holds" is exactly cnt < skip for the smallest failing cnt, found by bisection.  (float)k > maxerr is
+// monotone in the integer k, so with kerr the smallest k for which it holds, (float)(mse / cnt) > maxerr is exactly
+// mse / cnt >= kerr, i.e. mse >= kerr * cnt (mse >= 0, cnt >= 1).  Computed once per floor per CTA.
+struct F1Tests { int skip, kerr; };
+__device__ inline F1Tests f1_inspect_tests(const Floor1Dev &F) {
+  const auto either = [&](int cnt) {
+    return F.maxover * F.maxover / (float)cnt > F.maxerr || F.maxunder * F.maxunder / (float)cnt > F.maxerr;
+  };
+  F1Tests t;
+  if (!either(1)) {
+    t.skip = 1;
+  } else {                                             // either(lo) holds; cnt never reaches hi = 2^20
+    int lo = 1, hi = 1 << 20;
+    while (hi - lo > 1) { const int mid = lo + (hi - lo) / 2; if (either(mid)) lo = mid; else hi = mid; }
+    t.skip = hi;
+  }
+  if ((float)0 > F.maxerr) {
+    t.kerr = 0;
+  } else {                                             // (float)lo > maxerr fails; hi = INT_MAX stands for "never"
+    int lo = 0, hi = 0x7fffffff;
+    while (hi - lo > 1) { const int mid = lo + (hi - lo) / 2; if ((float)mid > F.maxerr) hi = mid; else lo = mid; }
+    t.kerr = hi;
+  }
+  return t;
+}
+
+// inspect_error's scan over one lane's abscissae x, x + 32, ... < x1, y = the line at x.  ITH: maxover / maxunder are
+// whole numbers (F.int_thresh), so the integer compares are exact; the thresholds are hoisted out of the loop and the
+// body is branch-free
+template <bool ITH>
+__device__ __forceinline__ void f1_scan(const Floor1Dev &F, const unsigned short *q, int x, int x0, int x1, int y,
+                                        int r, int m32, int ystep, int adx, int step, int &mse, int &viol) {
+  const int mo_i = F.maxover_i, mu_i = F.maxunder_i;
+  const float mo = F.maxover, mu = F.maxunder;
+  for (; x < x1; x += 32) {
+    const int v = q[x];
+    const int val = v & 0x7fff;
+    mse += (y - val) * (y - val);
+    bool over;
+    if (ITH) over = (y + mo_i < val) | (y - mu_i > val);
+    else     over = ((float)y + mo < (float)val) | ((float)y - mu > (float)val);
+    viol |= (int)(over & ((v & 0x8000) != 0) & ((x == x0) | (val != 0)));
+    r += m32;
+    y += ystep;
+    if (r >= adx) { r -= adx; y += step; }
+  }
+}
+
 // inspect_error: 1 = this line is not good enough.  q[x] = dBquant(mask[x]) | (audible << 15)
-__device__ __forceinline__ int f1_inspect(const Floor1Dev &F, const unsigned short *q, int x0, int x1,
+__device__ __forceinline__ int f1_inspect(const Floor1Dev &F, F1Tests T, const unsigned short *q, int x0, int x1,
                                           int y0, int y1, int lane) {
-  const F1Line L(x0, x1, y0, y1);
   int mse = 0, viol = 0;
   int x = x0 + lane;
   if (x < x1) {
-    // the line at this lane's first x in closed form, then 32 abscissae per step: the error term advances by
-    // (32*ady) mod adx and wraps at most once more than floor(32*ady / adx) times
-    int y = L.at(x);
-    int r = (x - x0) * L.ady;
-    { int qq = __float2int_rz((float)r * L.rcp); int t = r - qq * L.adx; if (t < 0) t += L.adx; else if (t >= L.adx) t -= L.adx; r = t; }
-    const int n32 = 32 * L.ady;
-    int d32 = __float2int_rz((float)n32 * L.rcp);
-    int m32 = n32 - d32 * L.adx;
-    if (m32 < 0) { d32--; m32 += L.adx; } else if (m32 >= L.adx) { d32++; m32 -= L.adx; }
-    const int ystep = 32 * L.base + d32 * L.step;
-    const bool ith = F.int_thresh != 0;                // maxover / maxunder are whole numbers: integer compares are exact
-    for (; x < x1; x += 32) {
-      const int v = q[x];
-      const int val = v & 0x7fff;
-      mse += (y - val) * (y - val);
-      if ((v & 0x8000) && (x == x0 || val)) {
-        if (ith) {
-          if (y + F.maxover_i < val) viol = 1;
-          if (y - F.maxunder_i > val) viol = 1;
-        } else {
-          if ((float)y + F.maxover < (float)val) viol = 1;
-          if ((float)y - F.maxunder > (float)val) viol = 1;
-        }
-      }
-      r += m32;
-      y += ystep;
-      if (r >= L.adx) { r -= L.adx; y += L.step; }
-    }
+    // F1Line's integer line in closed form at this lane's first x, then 32 abscissae per step: the error term
+    // advances by (32*ady) mod adx and wraps at most once more than floor(32*ady / adx) times.  Every quotient
+    // here is floor(num / adx) with 0 <= num < 2^24 (exact in fp32) and num / adx < 2^12 (|dy| < 1224, k < n <= 4096,
+    // ady < adx): from an approximate reciprocal (relative error < 2^-21) the estimate is off by at most one, and
+    // the remainder test makes it exact
+    const int adx = x1 - x0, dy = y1 - y0, step = dy < 0 ? -1 : 1;
+    const float rcp = __fdividef(1.f, (float)adx);
+    const auto qr = [&](int num, int &rem) {
+      int qq = __float2int_rz((float)num * rcp), t = num - qq * adx;
+      if (t < 0) { qq--; t += adx; } else if (t >= adx) { qq++; t -= adx; }
+      rem = t;
+      return qq;
+    };
+    int ady, r, m32;
+    const int b = qr(abs(dy), ady);                    // |dy / adx|; ady = |dy| - |base| * adx
+    const int base = dy < 0 ? -b : b;
+    const int k = x - x0;
+    const int y = y0 + k * base + qr(k * ady, r) * step;
+    const int ystep = 32 * base + qr(32 * ady, m32) * step;
+    if (F.int_thresh) f1_scan<true>(F, q, x, x0, x1, y, r, m32, ystep, adx, step, mse, viol);
+    else              f1_scan<false>(F, q, x, x0, x1, y, r, m32, ystep, adx, step, mse, viol);
   }
   if (__any_sync(0xffffffffu, viol)) return 1;
   mse = __reduce_add_sync(0xffffffffu, mse);
   const int cnt = x1 - x0;
-  if (F.maxover * F.maxover / (float)cnt > F.maxerr) return 0;
-  if (F.maxunder * F.maxunder / (float)cnt > F.maxerr) return 0;
-  if ((float)(mse / cnt) > F.maxerr) return 1;
-  return 0;
+  if (cnt < T.skip) return 0;
+  return (long long)mse >= (long long)T.kerr * cnt;
 }
 
 // fit_line (lib/floor1.c:456-521) for up to two runs of gaps at once.  term[gap*6 + f] holds what
@@ -187,9 +239,23 @@ __device__ __forceinline__ int f1_fit_lines(const Floor1Dev &F, const double *te
   return __shfl_sync(full, bad, 0) | (__shfl_sync(full, bad, 16) << 1);
 }
 
-__global__ void __launch_bounds__(32 * F1_WARPS)
-k_floor1_fit(Floor1Args a, const float *__restrict__ logmdct, const float *__restrict__ logmask,
-             int32_t *__restrict__ posts_out, int32_t *__restrict__ fit_nonzero) {
+// DBG = true: the instance with per-phase clock marks and per-row counters (tools/floor1_phase_timing.py).  Every
+// warp sums its own marks and lane 0 adds them into dbg[F1_DBG_SLOTS] once, at the end: the production instance
+// (DBG = false) carries none of it.
+enum { F1_T_Q, F1_T_ACC, F1_T_TERMS, F1_T_FIT0, F1_T_INSPECT, F1_T_FIT, F1_T_SPLIT, F1_T_OUT,
+       F1_C_INSPECT, F1_C_FIT, F1_C_NULL, F1_C_ROWS, F1_DBG_SLOTS };
+
+template <bool DBG>
+__global__ void __launch_bounds__(32 * F1_WARPS, DBG ? 1 : F1_FIT_CTAS)
+k_floor1_fit(Floor1Args a, int pcap, const float *__restrict__ logmdct, const float *__restrict__ logmask,
+             int32_t *__restrict__ posts_out, int32_t *__restrict__ fit_nonzero, unsigned long long *dbg) {
+  unsigned dsum[F1_DBG_SLOTS] = {};          // per-warp sums: a warp's rows take far fewer than 2^32 cycles
+  long long tmark = 0;
+#define F1_MARK(slot)                                                            \
+  do {                                                                           \
+    if (DBG) { const long long t_ = clock64(); dsum[slot] += (unsigned)(t_ - tmark); tmark = t_; } \
+  } while (0)
+#define F1_COUNT(slot) do { if (DBG) dsum[slot]++; } while (0)
   extern __shared__ __align__(16) unsigned char f1_smem[];
   Floor1Dev *sF = reinterpret_cast<Floor1Dev *>(f1_smem);
   {
@@ -198,30 +264,37 @@ k_floor1_fit(Floor1Args a, const float *__restrict__ logmdct, const float *__res
     int *dst = reinterpret_cast<int *>(sF);
     for (int i = threadIdx.x; i < words; i += blockDim.x) dst[i] = src[i];
   }
+  __shared__ F1Tests sT[VB200_MAX_SUBMAPS];
+  if (threadIdx.x < VB200_MAX_SUBMAPS) sT[threadIdx.x] = f1_inspect_tests(a.floors[threadIdx.x]);
   __syncthreads();
+  if (DBG) tmark = clock64();
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  unsigned char *wbase = f1_smem + sizeof(Floor1Dev) * VB200_MAX_SUBMAPS + floor1_fit_smem_per_warp(a.n) * warp;
+  unsigned char *wbase = f1_smem + sizeof(Floor1Dev) * VB200_MAX_SUBMAPS + floor1_fit_smem_per_warp(a.n, pcap) * warp;
   double *term = reinterpret_cast<double *>(wbase);          // [gaps][6], same bytes as 12 ints per gap
-  int *A = reinterpret_cast<int *>(wbase) + (VB200_VIF_POSIT + 1) * F1_ACC;
-  int *B = A + (VB200_VIF_POSIT + 2), *out = B + (VB200_VIF_POSIT + 2);
-  short *lon = reinterpret_cast<short *>(out + (VB200_VIF_POSIT + 2));
-  short *hin = lon + 2 * ((VB200_VIF_POSIT + 2 + 1) / 2), *memo = hin + 2 * ((VB200_VIF_POSIT + 2 + 1) / 2);
-  unsigned short *q = reinterpret_cast<unsigned short *>(memo + 2 * ((VB200_VIF_POSIT + 2 + 1) / 2));
+  F1Post *st = reinterpret_cast<F1Post *>(wbase + sizeof(int) * F1_ACC * (pcap - 1));
+  unsigned short *q = reinterpret_cast<unsigned short *>(st + pcap);
 
-  for (long row = (long)blockIdx.x * F1_WARPS + warp; row < a.nrows; row += (long)gridDim.x * F1_WARPS) {
+  for (int row = blockIdx.x * F1_WARPS + warp; row < a.nrows; row += gridDim.x * F1_WARPS) {   // grid_for: no overflow
     const int sel = a.floor_sel >= 0 ? a.floor_sel : a.chmux[row % a.channels];
     const Floor1Dev &F = sF[sel];
     const int P = F.posts, n = F.n;
     const float *md = logmdct + (size_t)row * a.n, *mk = logmask + (size_t)row * a.n;
     int32_t *po = posts_out + (size_t)row * VB200_FLOOR1_STRIDE;
     __syncwarp();
-    for (int x = lane; x < n; x += 32) {
-      const float m = mk[x];
-      const int v = f1_dBquant(m);
-      q[x] = (unsigned short)(v | ((md[x] + F.twofitatten >= m) ? 0x8000 : 0));
+    F1_COUNT(F1_C_ROWS);
+    const float att = F.twofitatten;
+    const auto qv = [att](float d, float m) { return (unsigned)f1_dBquant(m) | ((d + att >= m) ? 0x8000u : 0u); };
+    if ((n & 3) == 0 && (((uintptr_t)md | (uintptr_t)mk) & 15) == 0) {   // four lines per load and store
+      for (int x = 4 * lane; x < n; x += 128) {
+        const float4 d = *reinterpret_cast<const float4 *>(md + x), m = *reinterpret_cast<const float4 *>(mk + x);
+        *reinterpret_cast<uint2 *>(q + x) = make_uint2(qv(d.x, m.x) | qv(d.y, m.y) << 16, qv(d.z, m.z) | qv(d.w, m.w) << 16);
+      }
+    } else {
+      for (int x = lane; x < n; x += 32) q[x] = (unsigned short)qv(md[x], mk[x]);
     }
-    for (int i = lane; i < P; i += 32) { A[i] = -200; B[i] = -200; lon[i] = 0; hin[i] = 1; memo[i] = -1; }
+    for (int i = lane; i < P; i += 32) { st[i].A = -200; st[i].B = -200; st[i].lon = 0; st[i].hin = 1; st[i].memo = -1; }
     __syncwarp();
+    F1_MARK(F1_T_Q);
     // accumulate_fit: one accumulator per gap, both ends inclusive
     int nonzero = 0;
     for (int j = 0; j < P - 1; j++) {
@@ -231,24 +304,27 @@ k_floor1_fit(Floor1Args a, const float *__restrict__ logmdct, const float *__res
       int s[F1_ACC];
 #pragma unroll
       for (int k = 0; k < F1_ACC; k++) s[k] = 0;
-      for (int x = x0 + lane; x <= x1; x += 32) {
-        const int v = q[x], val = v & 0x7fff;
-        if (val) {
-          if (v & 0x8000) { s[0] += x; s[1] += val; s[2] += x * x; s[3] += val * val; s[4] += x * val; s[5]++; }
-          else            { s[6] += x; s[7] += val; s[8] += x * x; s[9] += val * val; s[10] += x * val; s[11]++; }
-        }
-      }
+      // a warp-uniform trip count (every gap holds at least one line): no zero-trip path to set up twice
+      const int iters = (x1 - x0 + 32) >> 5;
+      int x = x0 + lane, it = 0;
+      do {
+        const int v = x <= x1 ? q[x] : 0, val = v & 0x7fff;
+        const bool ua = val != 0 && (v & 0x8000), ub = val != 0 && !(v & 0x8000);   // predicated, no branch
+        if (ua) { s[0] += x; s[1] += val; s[2] += x * x; s[3] += val * val; s[4] += x * val; s[5]++; }
+        if (ub) { s[6] += x; s[7] += val; s[8] += x * x; s[9] += val * val; s[10] += x * val; s[11]++; }
+        x += 32;
+      } while (++it < iters);
 #pragma unroll
       for (int k = 0; k < F1_ACC; k++) s[k] = __reduce_add_sync(0xffffffffu, s[k]);
-      if (lane < F1_ACC) {                               // raw sums; turned into fit_line's terms below
-        int v = s[0];
+      if (lane == 0) {                                   // raw sums; turned into fit_line's terms below
+        int2 *dst = reinterpret_cast<int2 *>(term + j * (F1_ACC / 2));
 #pragma unroll
-        for (int k = 1; k < F1_ACC; k++) if (lane == k) v = s[k];
-        reinterpret_cast<int *>(term)[j * F1_ACC + lane] = v;
+        for (int k = 0; k < F1_ACC / 2; k++) dst[k] = make_int2(s[2 * k], s[2 * k + 1]);
       }
       nonzero += s[5];
     }
     __syncwarp();
+    F1_MARK(F1_T_ACC);
     // what fit_line adds for a gap, chain f: (double)Xb + (double)Xa * weight (lib/floor1.c:465-474).  One
     // lane per gap turns its 12 ints into the 6 doubles in place (same 48 bytes, private to the lane).
     for (int g = lane; g < P - 1; g += 32) {
@@ -261,53 +337,64 @@ k_floor1_fit(Floor1Args a, const float *__restrict__ logmdct, const float *__res
       for (int f = 0; f < 6; f++) term[g * 6 + f] = (double)a[6 + f] + (double)a[f] * w;
     }
     __syncwarp();
+    F1_MARK(F1_T_TERMS);
     if (!nonzero) {                                      // the reference returns NULL
       for (int i = lane; i < VB200_FLOOR1_STRIDE; i += 32) po[i] = 0;
       if (lane == 0) fit_nonzero[row] = 0;
+      F1_COUNT(F1_C_NULL);
+      F1_MARK(F1_T_OUT);
       continue;
     }
     int y[4];
     f1_fit_lines(F, term, 0, P - 1, 0, 0, lane, y);
-    if (lane == 0) { A[0] = y[0]; B[0] = y[0]; A[1] = y[1]; B[1] = y[1]; }
+    if (lane == 0) { st[0].A = y[0]; st[0].B = y[0]; st[1].A = y[1]; st[1].B = y[1]; }
     __syncwarp();
+    F1_MARK(F1_T_FIT0);
     for (int i = 2; i < P; i++) {
       const int sortpos = F.rev[i];
-      const int ln = lon[sortpos], hn = hin[sortpos];
-      if (memo[ln] == hn) continue;                      // this span was already judged
+      const int ln = st[sortpos].lon, hn = st[sortpos].hin;
+      if (st[ln].memo == hn) continue;                      // this span was already judged
       const int lsortpos = F.rev[ln], hsortpos = F.rev[hn];
       const int lx = F.postlist[ln], hx = F.postlist[hn];
-      const int ly = f1_postY(A, B, ln), hy = f1_postY(A, B, hn);
+      const int ly = f1_postY(st, ln), hy = f1_postY(st, hn);
       __syncwarp();
-      if (lane == 0) memo[ln] = (short)hn;
-      if (f1_inspect(F, q, lx, hx, ly, hy, lane)) {
+      if (lane == 0) st[ln].memo = (signed char)hn;
+      F1_MARK(F1_T_SPLIT);
+      const int bad = f1_inspect(F, sT[sel], q, lx, hx, ly, hy, lane);
+      F1_COUNT(F1_C_INSPECT);
+      F1_MARK(F1_T_INSPECT);
+      if (bad) {
         const int ret = f1_fit_lines(F, term, lsortpos, sortpos - lsortpos, sortpos, hsortpos - sortpos, lane, y);
+        F1_COUNT(F1_C_FIT);
+        F1_MARK(F1_T_FIT);
         int ly0 = y[0], ly1 = y[1], hy0 = y[2], hy1 = y[3];
         if (ret & 1) { ly0 = ly; ly1 = hy0; }
         if (ret & 2) { hy0 = ly1; hy1 = hy; }
         if (lane == 0) {
           if (ret == 3) {
-            A[i] = -200; B[i] = -200;
+            st[i].A = -200; st[i].B = -200;
           } else {
-            B[ln] = ly0;
-            if (ln == 0) A[ln] = ly0;
-            A[i] = ly1; B[i] = hy0;
-            A[hn] = hy1;
-            if (hn == 1) B[hn] = hy1;
+            st[ln].B = ly0;
+            if (ln == 0) st[ln].A = ly0;
+            st[i].A = ly1; st[i].B = hy0;
+            st[hn].A = hy1;
+            if (hn == 1) st[hn].B = hy1;
             if (ly1 >= 0 || hy0 >= 0) {
-              for (int j = sortpos - 1; j >= 0; j--) { if (hin[j] == hn) hin[j] = (short)i; else break; }
-              for (int j = sortpos + 1; j < P; j++) { if (lon[j] == ln) lon[j] = (short)i; else break; }
+              for (int j = sortpos - 1; j >= 0; j--) { if (st[j].hin == hn) st[j].hin = (signed char)i; else break; }
+              for (int j = sortpos + 1; j < P; j++) { if (st[j].lon == ln) st[j].lon = (signed char)i; else break; }
             }
           }
         }
       } else if (lane == 0) {
-        A[i] = -200; B[i] = -200;
+        st[i].A = -200; st[i].B = -200;
       }
       __syncwarp();
     }
+    F1_MARK(F1_T_SPLIT);
     // posts as the reference returns them: fitted value, or predicted | 0x8000 when unused
     if (lane == 0) {
-      out[0] = f1_postY(A, B, 0);
-      out[1] = f1_postY(A, B, 1);
+      st[0].out = f1_postY(st, 0);
+      st[1].out = f1_postY(st, 1);
       fit_nonzero[row] = 1;
     }
     __syncwarp();
@@ -315,14 +402,20 @@ k_floor1_fit(Floor1Args a, const float *__restrict__ logmdct, const float *__res
       for (int t = F.lvl_start[lv] + lane; t < F.lvl_start[lv + 1]; t += 32) {
         const int i = F.lvl_order[t];
         const int ln = F.lo[i - 2], hn = F.hi[i - 2];
-        const int predicted = f1_point(F.postlist[ln], F.postlist[hn], out[ln], out[hn], F.postlist[i], F.prcp[i - 2]);
-        const int vx = f1_postY(A, B, i);
-        out[i] = (vx >= 0 && predicted != vx) ? vx : (predicted | 0x8000);
+        const int predicted = f1_point(F.postlist[ln], F.postlist[hn], st[ln].out, st[hn].out, F.postlist[i],
+                                       F.prcp[i - 2]);
+        const int vx = f1_postY(st, i);
+        st[i].out = (vx >= 0 && predicted != vx) ? vx : (predicted | 0x8000);
       }
       __syncwarp();
     }
-    for (int i = lane; i < VB200_FLOOR1_STRIDE; i += 32) po[i] = i < P ? out[i] : 0;
+    for (int i = lane; i < VB200_FLOOR1_STRIDE; i += 32) po[i] = i < P ? st[i].out : 0;
+    F1_MARK(F1_T_OUT);
   }
+  if (DBG && lane == 0)
+    for (int k = 0; k < F1_DBG_SLOTS; k++) atomicAdd(dbg + k, (unsigned long long)dsum[k]);
+#undef F1_MARK
+#undef F1_COUNT
 }
 
 // blockIdx.y = curve: rows a.nrows of every curve, curve y's arrays start blob_rows rows after curve y-1's
