@@ -740,6 +740,27 @@ int vb200_encode_entropy    (vb200_ctx*, int W, int nblocks, const vb200_block_d
 int vb200_encode_packets(vb200_ctx*, int W, int nstreams, int blocks_per_stream, int blobno, const vb200_encode_io *io,
                          int64_t *pkt_off, int32_t *pkt_bits, uint8_t *data, int64_t data_cap);
 
+/* Bitrate-managed: all VB200_PACKETBLOBS packets of every block (what mapping0_forward writes into packetblob[0..14]
+ * when vorbis_bitrate_managed), byte-identical to the reference; the bitrate manager then picks one of them.
+ *   posts / nonzero / iwork  blob-major as vb200_encode_dsp_managed / vb200_encode_streams_managed write them: block b
+ *           of curve k is row k*blob_blocks*ch + b*ch + channel, blob_blocks >= nblocks (nblocks for
+ *           vb200_encode_dsp_managed, cap[W] for vb200_encode_streams_managed); rows past nblocks of a curve are never
+ *           read.  A NULL curve (all-zero posts rows) codes as silent floors.
+ * _dev: packet (k, b) goes to data + (k*nblocks + b)*pkt_stride and pkt_bits[k*nblocks + b] is its length in bits;
+ *       pkt_stride as for vb200_encode_entropy_dev (the bound holds for every curve).  Two kernel launches
+ *       (classification of all curves, then the coder); the scratch does not grow with the curve count.
+ * vb200_encode_packets_managed: PCM in, packets out in one synchronous round trip; io as for vb200_encode_dsp_managed
+ *       with posts, nonzero, iwork, classes, overflow and the spectra NULL; io->ampmax_out is filled.  Packet (k, b)
+ *       at data + pkt_off[k*nblocks + b], (pkt_bits[k*nblocks + b] + 7) / 8 bytes; when they do not fit data_cap it
+ *       returns VB200_EINVAL with pkt_bits filled.  Launches: those of vb200_encode_dsp_managed plus four.
+ * VB200_EINVAL without a registered setup, for blob_blocks < nblocks, a bad pkt_stride and null pointers.       */
+int vb200_encode_entropy_managed_dev(vb200_ctx*, int W, int nblocks, int64_t blob_blocks,
+                                     const vb200_block_desc *d_desc, const int32_t *d_posts, const int32_t *d_nonzero,
+                                     const int32_t *d_iwork, int64_t pkt_stride, int32_t *d_pkt_bits, uint8_t *d_data,
+                                     void *stream);
+int vb200_encode_packets_managed(vb200_ctx*, int W, int nstreams, int blocks_per_stream, const vb200_encode_io *io,
+                                 int64_t *pkt_off, int32_t *pkt_bits, uint8_t *data, int64_t data_cap);
+
 /* ---- device memory helpers for non-CUDA hosts (C callers) -------------- */
 int  vb200_malloc_device(vb200_ctx*, size_t bytes, void **dptr);
 int  vb200_free_device  (vb200_ctx*, void *dptr);

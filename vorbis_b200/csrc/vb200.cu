@@ -2484,11 +2484,11 @@ extern "C" int vb200_residue_partvals(vb200_ctx *c, int W) {
   return c->res_partvals[W];
 }
 
-extern "C" int vb200_residue_classify_dev(vb200_ctx *c, int W, int nblocks, const int32_t *d_iwork,
-                                          const int32_t *d_nonzero, int32_t *d_classes, int class_stride, void *stream) {
-  CHECK_CTX(c); CHECK_W(W);
-  if (nblocks <= 0) return 0;
-  if (!d_iwork || !d_nonzero || !d_classes) return fail(VB200_EINVAL, "residue_classify pointers");
+// curves == 1: nblocks blocks; curves == VB200_PACKETBLOBS: every curve of nblocks blocks, iwork / nonzero rows
+// curve_rows apart (k_residue_classify_curves), classes [curves][nblocks][ch][class_stride]
+static int residue_classify_launch(vb200_ctx *c, int W, int nblocks, int curves, long long curve_rows,
+                                   const int32_t *d_iwork, const int32_t *d_nonzero, int32_t *d_classes,
+                                   int class_stride, cudaStream_t st) {
   if (c->res_partvals[W] <= 0) return fail(VB200_EINVAL, "no residue setup for this block size");
   if (class_stride < c->res_partvals[W]) return fail(VB200_EINVAL, "class_stride < partvals");
   const int ch = c->setup.channels, n = c->dx[W].N / 2, submaps = c->setup.submaps[W] > 0 ? c->setup.submaps[W] : 1;
@@ -2501,15 +2501,23 @@ extern "C" int vb200_residue_classify_dev(vb200_ctx *c, int W, int nblocks, cons
                                    : (long)r.begin + (long)((r.end - r.begin) / r.grouping) * r.grouping;
     if (reach > n) return fail(VB200_EINVAL, "residue range exceeds the block");
   }
-  cudaStream_t st = (cudaStream_t)stream;
-  CU(cudaMemsetAsync(d_classes, 0, sizeof(int32_t) * (size_t)nblocks * ch * class_stride, st));
+  CU(cudaMemsetAsync(d_classes, 0, sizeof(int32_t) * curves * (size_t)nblocks * ch * class_stride, st));
   ResArgs A;
   A.res = c->d_res[W]; A.chmux = c->d_chmux[W]; A.ch = ch; A.n = n; A.submaps = submaps; A.nblocks = nblocks;
   A.stride = class_stride;
-  const long tasks = (long)nblocks * submaps;
-  k_residue_classify<<<grid_for(c, (int)((tasks + RES_WARPS - 1) / RES_WARPS), 16), 32 * RES_WARPS, 0, st>>>(
-      A, d_iwork, d_nonzero, d_classes);
+  const long tasks = (long)curves * nblocks * submaps;
+  const int grid = grid_for(c, (int)((tasks + RES_WARPS - 1) / RES_WARPS), 16);
+  if (curves == 1) k_residue_classify<<<grid, 32 * RES_WARPS, 0, st>>>(A, d_iwork, d_nonzero, d_classes);
+  else k_residue_classify_curves<<<grid, 32 * RES_WARPS, 0, st>>>(A, curve_rows, d_iwork, d_nonzero, d_classes);
   return post_launch(c);
+}
+
+extern "C" int vb200_residue_classify_dev(vb200_ctx *c, int W, int nblocks, const int32_t *d_iwork,
+                                          const int32_t *d_nonzero, int32_t *d_classes, int class_stride, void *stream) {
+  CHECK_CTX(c); CHECK_W(W);
+  if (nblocks <= 0) return 0;
+  if (!d_iwork || !d_nonzero || !d_classes) return fail(VB200_EINVAL, "residue_classify pointers");
+  return residue_classify_launch(c, W, nblocks, 1, 0, d_iwork, d_nonzero, d_classes, class_stride, (cudaStream_t)stream);
 }
 
 extern "C" int vb200_residue_classify(vb200_ctx *c, int W, int nblocks, const int32_t *iwork, const int32_t *nonzero,
@@ -3234,25 +3242,36 @@ extern "C" int vb200_encode_packet_bound(vb200_ctx *c, int W) {
   return c->eent.bound[W];
 }
 
-// classification into scratch (k_residue_classify), then k_encode_packets; all pointers device
+// classification into scratch (k_residue_classify), then k_encode_packets; all pointers device.  Managed
+// (k_residue_classify_curves, k_encode_packets_curves): the VB200_PACKETBLOBS curves of every block, blob_blocks
+// blocks from one curve of posts / nonzero / iwork to the next; packet k*nblocks + b.  The private residue copies
+// stay one per CTA either way.
 static int encode_entropy_launch(vb200_ctx *c, int W, int nblocks, const vb200_block_desc *d_desc,
                                  const int32_t *d_posts, const int32_t *d_nonzero, const int32_t *d_iwork,
-                                 int64_t pkt_stride, int32_t *d_bits, uint8_t *d_data, cudaStream_t st) {
+                                 int64_t pkt_stride, int32_t *d_bits, uint8_t *d_data, cudaStream_t st,
+                                 bool managed = false, long long blob_blocks = 0) {
   const int ch = c->setup.channels, n = c->dx[W].N / 2, stride = c->res_partvals[W] > 0 ? c->res_partvals[W] : 1;
-  const int grid = grid_for(c, nblocks, 8);
+  const int curves = managed ? VB200_PACKETBLOBS : 1;
+  const int grid = grid_for(c, curves * nblocks, 8);
   void *cls, *work;
   int rc;
-  if ((rc = ensure_buf(c->eent_buf[0], sizeof(int32_t) * (size_t)nblocks * ch * stride, &cls))) return rc;
+  if ((rc = ensure_buf(c->eent_buf[0], sizeof(int32_t) * curves * (size_t)nblocks * ch * stride, &cls))) return rc;
   if ((rc = ensure_buf(c->eent_buf[1], sizeof(int32_t) * (size_t)grid * ch * n, &work))) return rc;
-  if ((rc = vb200_residue_classify_dev(c, W, nblocks, d_iwork, d_nonzero, (int32_t *)cls, stride, st))) return rc;
+  if ((rc = residue_classify_launch(c, W, nblocks, curves, blob_blocks * ch, d_iwork, d_nonzero, (int32_t *)cls, stride,
+                                    st))) return rc;
   EncArgs A;
   A.E = c->eent; A.f1 = c->d_floor[W]; A.chmux = c->d_chmux[W]; A.desc = d_desc;
   A.posts = d_posts; A.nonzero = d_nonzero; A.iwork = d_iwork; A.classes = (const int *)cls;
-  A.curve_rows = 0; A.work = (int *)work; A.W = W; A.nblocks = nblocks; A.n = n; A.class_stride = stride;
+  A.curve_rows = blob_blocks * ch; A.work = (int *)work; A.W = W; A.nblocks = nblocks; A.n = n; A.class_stride = stride;
   A.pkt_stride = pkt_stride; A.pkt_bits = d_bits; A.data = d_data;
   const size_t smem = sizeof(int) * (size_t)c->eent.slots[W];
-  if ((rc = set_smem(k_encode_packets, smem))) return rc;
-  k_encode_packets<<<dim3(grid, 1), ENC_THREADS, smem, st>>>(A);
+  if (managed) {
+    if ((rc = set_smem(k_encode_packets_curves, smem))) return rc;
+    k_encode_packets_curves<<<grid, ENC_THREADS, smem, st>>>(A);
+  } else {
+    if ((rc = set_smem(k_encode_packets, smem))) return rc;
+    k_encode_packets<<<dim3(grid, 1), ENC_THREADS, smem, st>>>(A);
+  }
   return post_launch(c);
 }
 
@@ -3373,6 +3392,70 @@ extern "C" int vb200_encode_packets(vb200_ctx *c, int W, int nstreams, int bps, 
   if ((rc = scratch_end(c, st))) return rc;
   CU(cudaMemcpyAsync(h->ampmax_out, d.ampmax_out, sizeof(float) * nb, cudaMemcpyDeviceToHost, st));
   return packets_pack_d2h(c, (int)nb, dstr, stride, dbits, pkt_off, pkt_bits, data, data_cap, st);
+}
+
+// ---- bitrate-managed: all VB200_PACKETBLOBS packets of every block ----
+extern "C" int vb200_encode_entropy_managed_dev(vb200_ctx *c, int W, int nblocks, int64_t blob_blocks,
+                                                const vb200_block_desc *d_desc, const int32_t *d_posts,
+                                                const int32_t *d_nonzero, const int32_t *d_iwork, int64_t pkt_stride,
+                                                int32_t *d_pkt_bits, uint8_t *d_data, void *stream) {
+  CHECK_CTX(c); CHECK_W(W);
+  int rc;
+  if ((rc = encode_entropy_check(c, nblocks))) return rc;
+  if (blob_blocks < nblocks) return fail(VB200_EINVAL, "blob_blocks < nblocks");
+  if ((int64_t)VB200_PACKETBLOBS * nblocks > INT32_MAX) return fail(VB200_EINVAL, "nblocks");
+  if (pkt_stride % 4 || pkt_stride < c->eent.bound[W]) return fail(VB200_EINVAL, "pkt_stride: a multiple of 4, >= the packet bound");
+  if (nblocks == 0) return 0;
+  if (!d_desc || !d_posts || !d_nonzero || !d_iwork || !d_pkt_bits || !d_data) return fail(VB200_EINVAL, "encode_entropy pointers");
+  cudaStream_t st = (cudaStream_t)stream;
+  if ((rc = scratch_begin(c, st))) return rc;
+  if ((rc = encode_entropy_launch(c, W, nblocks, d_desc, d_posts, d_nonzero, d_iwork, pkt_stride, d_pkt_bits, d_data, st,
+                                  true, blob_blocks))) return rc;
+  return scratch_end(c, st);
+}
+
+extern "C" int vb200_encode_packets_managed(vb200_ctx *c, int W, int nstreams, int bps, const vb200_encode_io *h,
+                                            int64_t *pkt_off, int32_t *pkt_bits, uint8_t *data, int64_t data_cap) {
+  CHECK_CTX(c); CHECK_W(W);
+  int rc;
+  if (!c->eent.books) return fail(VB200_EINVAL, "no vb200_encode_entropy_setup registered");
+  if (!h || h->posts || h->nonzero || h->iwork || h->classes || h->overflow || h->mdct || h->logmdct || h->logmask ||
+      h->iwork_fmt != VB200_IWORK_S32)
+    return fail(VB200_EINVAL, "encode_packets_managed: posts / nonzero / iwork / classes / overflow / spectra must be NULL");
+  if (!pkt_off || !pkt_bits || (!data && data_cap > 0) || data_cap < 0) return fail(VB200_EINVAL, "encode_packets_managed outputs");
+  vb200_encode_io d = *h;
+  int32_t one = 0;                                   // managed_check wants the outputs it does not see here
+  d.posts = d.nonzero = &one; d.iwork = &one;
+  if ((rc = managed_check(c, W, nstreams, bps, &d))) return rc;
+  if ((int64_t)VB200_PACKETBLOBS * nstreams * bps > INT32_MAX) return fail(VB200_EINVAL, "nblocks");
+  std::lock_guard<std::mutex> lk(c->mu);
+  constexpr int NB = VB200_PACKETBLOBS;
+  const int ch = c->setup.channels, N = c->dx[W].N, n = N / 2;
+  const size_t nb = (size_t)nstreams * bps, rows = nb * ch;
+  const int64_t stride = c->eent.bound[W];
+  cudaStream_t st = c->s_main;
+  DevBuf *B = c->mgd_buf;                            // the host-call staging of vb200_encode_dsp_managed, and two more
+  void *p;
+  const size_t pcm_bytes = enc_pcm_bytes(h, ch, N, nstreams, bps);
+  if ((rc = ensure_buf(B[12], pcm_bytes, &p))) return rc; d.pcm = p;
+  if ((rc = ensure_buf(B[13], sizeof(vb200_block_desc) * nb, &p))) return rc; d.desc = (const vb200_block_desc *)p;
+  if ((rc = ensure_buf(B[14], sizeof(float) * nstreams, &p))) return rc; d.ampmax0 = h->ampmax0 ? (const float *)p : nullptr;
+  if ((rc = ensure_buf(B[15], sizeof(int32_t) * NB * rows * VB200_FLOOR1_STRIDE, &p))) return rc; d.posts = (int32_t *)p;
+  if ((rc = ensure_buf(B[16], sizeof(int32_t) * NB * rows, &p))) return rc; d.nonzero = (int32_t *)p;
+  if ((rc = ensure_buf(B[17], sizeof(int32_t) * NB * rows * n, &p))) return rc; d.iwork = p;
+  if ((rc = ensure_buf(B[18], sizeof(float) * nb, &p))) return rc; d.ampmax_out = (float *)p;
+  if ((rc = ensure_buf(B[19], sizeof(int32_t) * NB * nb, &p))) return rc;
+  int32_t *dbits = (int32_t *)p;
+  if ((rc = ensure_buf(B[20], (size_t)stride * NB * nb, &p))) return rc;
+  uint8_t *dstr = (uint8_t *)p;
+  CU(cudaMemcpyAsync((void *)d.pcm, h->pcm, pcm_bytes, cudaMemcpyHostToDevice, st));
+  CU(cudaMemcpyAsync((void *)d.desc, h->desc, sizeof(vb200_block_desc) * nb, cudaMemcpyHostToDevice, st));
+  if (h->ampmax0) CU(cudaMemcpyAsync((void *)d.ampmax0, h->ampmax0, sizeof(float) * nstreams, cudaMemcpyHostToDevice, st));
+  if ((rc = vb200_encode_dsp_managed_dev(c, W, nstreams, bps, &d, st))) return rc;
+  if ((rc = vb200_encode_entropy_managed_dev(c, W, (int)nb, (int64_t)nb, d.desc, d.posts, d.nonzero,
+                                             (const int32_t *)d.iwork, stride, dbits, dstr, st))) return rc;
+  CU(cudaMemcpyAsync(h->ampmax_out, d.ampmax_out, sizeof(float) * nb, cudaMemcpyDeviceToHost, st));
+  return packets_pack_d2h(c, NB * (int)nb, dstr, stride, dbits, pkt_off, pkt_bits, data, data_cap, st);
 }
 
 // ======================================================================== //

@@ -43,7 +43,7 @@ struct EncArgs {
   const unsigned char *chmux;
   const vb200_block_desc *desc;
   const int *posts, *nonzero, *iwork, *classes;
-  long long curve_rows;                // rows (block x channel) from one curve to the next: blockIdx.y
+  long long curve_rows;                // rows (block x channel) from one curve to the next: blockIdx.y (curves: k)
   int *work;                           // [gridDim.y][gridDim.x][ch*n] private copies of the residue
   int W, nblocks, n, class_stride;
   long long pkt_stride;
@@ -259,8 +259,13 @@ __device__ void enc_pass(const EncArgs &A, const EncSub *subs, int blk, const in
   }
 }
 
-__global__ void __launch_bounds__(ENC_THREADS)
-k_encode_packets(EncArgs A) {
+// CURVES = false: one packet per block of curve blockIdx.y (posts and nonzero rows blockIdx.y * curve_rows on;
+// classes and iwork of curve 0).  CURVES = true (bitrate-managed): the VB200_PACKETBLOBS packets of every block, the
+// (curve, block) pairs folded into the CTA's grid-stride loop so that work stays [gridDim.x][ch*n]; curve k of block
+// b reads posts / nonzero / iwork row k*curve_rows + b*ch and classes row (k*nblocks + b)*ch, and writes packet
+// k*nblocks + b (gridDim.y must be 1).
+template <bool CURVES>
+__device__ __forceinline__ void encode_packets_body(const EncArgs &A) {
   extern __shared__ int s_slot[];
   __shared__ EncSub s_sub[VB200_MAX_SUBMAPS];
   __shared__ int s_warp[ENC_THREADS / 32], s_total;
@@ -268,10 +273,18 @@ k_encode_packets(EncArgs A) {
   const int tid = threadIdx.x, ch = E.ch;
   const long long row_y = (long long)blockIdx.y * A.curve_rows;
   int *work = A.work + ((size_t)blockIdx.y * gridDim.x + blockIdx.x) * ch * A.n;
-  for (int blk = blockIdx.x; blk < A.nblocks; blk += gridDim.x) {
-    const size_t row0 = (size_t)row_y + (size_t)blk * ch;
+  EncArgs C;                                            // CURVES: A with iwork and classes moved to the curve
+  if constexpr (CURVES) C = A;
+  for (int it = blockIdx.x; it < (CURVES ? VB200_PACKETBLOBS : 1) * A.nblocks; it += gridDim.x) {
+    const int curve = CURVES ? it / A.nblocks : 0, blk = it - curve * A.nblocks;
+    if constexpr (CURVES) {
+      C.iwork = A.iwork + (size_t)curve * A.curve_rows * A.n;
+      C.classes = A.classes + (size_t)curve * A.nblocks * ch * A.class_stride;
+    }
+    const EncArgs &P = CURVES ? C : A;
+    const size_t row0 = (size_t)(CURVES ? curve * A.curve_rows : row_y) + (size_t)blk * ch;
     const int *posts = A.posts + row0 * VB200_FLOOR1_STRIDE, *nz = A.nonzero + row0;
-    const long long pk = (long long)blockIdx.y * A.nblocks + blk;
+    const long long pk = CURVES ? it : (long long)blockIdx.y * A.nblocks + blk;
     uint32_t *out = (uint32_t *)(A.data + pk * A.pkt_stride);
     if (tid < E.submaps[A.W]) {                         // the bundles (lib/mapping0.c:660-683, lib/res0.c:725-809)
       EncSub &S = s_sub[tid];
@@ -297,16 +310,26 @@ k_encode_packets(EncArgs A) {
     }
     __syncthreads();
     const int nslots = s_total;
-    enc_pass<false>(A, s_sub, blk, posts, s_slot, out, work);
+    enc_pass<false>(P, s_sub, blk, posts, s_slot, out, work);
     __syncthreads();
     enc_scan(s_slot, nslots, s_warp, &s_total);
     const int bits = s_total;
     for (int k = tid; k < (bits + 31) >> 5; k += ENC_THREADS) out[k] = 0u;
     __syncthreads();
-    enc_pass<true>(A, s_sub, blk, posts, s_slot, out, work);
+    enc_pass<true>(P, s_sub, blk, posts, s_slot, out, work);
     if (tid == 0) A.pkt_bits[pk] = bits;
     __syncthreads();
   }
+}
+
+__global__ void __launch_bounds__(ENC_THREADS)
+k_encode_packets(EncArgs A) {
+  encode_packets_body<false>(A);
+}
+
+__global__ void __launch_bounds__(ENC_THREADS)
+k_encode_packets_curves(EncArgs A) {
+  encode_packets_body<true>(A);
 }
 
 // host forms: byte offsets of the packed packets (one CTA, an exclusive scan of (bits + 7) / 8) ...

@@ -24,19 +24,29 @@ struct ResArgs {
 
 constexpr int RES_WARPS = 4;
 
-__global__ void __launch_bounds__(32 * RES_WARPS)
-k_residue_classify(ResArgs A, const int *__restrict__ iwork, const int *__restrict__ nonzero,
-                   int *__restrict__ classes) {
+// CURVES = false: nblocks blocks, rows blk*ch.  CURVES = true (bitrate-managed): the VB200_PACKETBLOBS curves of
+// nblocks blocks; block b of curve k reads iwork / nonzero row k*curve_rows + b*ch (only rows < nblocks of each
+// curve) and writes classes row (k*nblocks + b)*ch.
+// (the kernels' pointers are __restrict__; restating it here would change the existing kernel's code)
+template <bool CURVES>
+__device__ __forceinline__ void residue_classify_body(const ResArgs &A, long long curve_rows, const int *iwork,
+                                                      const int *nonzero, int *classes) {
   __shared__ unsigned char s_chan[RES_WARPS][256];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   unsigned char *chan = s_chan[wid];
-  const long tasks = (long)A.nblocks * A.submaps;
+  const long tasks = CURVES ? (long)VB200_PACKETBLOBS * A.nblocks * A.submaps : (long)A.nblocks * A.submaps;
   for (long t = (long)blockIdx.x * RES_WARPS + wid; t < tasks; t += (long)gridDim.x * RES_WARPS) {
     const int blk = (int)(t / A.submaps), sm = (int)(t - (long)blk * A.submaps);
     const ResDev &R = A.res[sm];
     if (R.type < 0) continue;
     const int *in = iwork + (size_t)blk * A.ch * A.n;
     const int *nz = nonzero + (size_t)blk * A.ch;
+    if constexpr (CURVES) {                                // blk = curve * nblocks + block
+      const int curve = blk / A.nblocks;
+      const size_t row0 = (size_t)curve * curve_rows + (size_t)(blk - curve * A.nblocks) * A.ch;
+      in = iwork + row0 * A.n;
+      nz = nonzero + row0;
+    }
     // the submap's channels in order, and whether any of them is in use
     __syncwarp();
     int cib = 0, used = 0;
@@ -95,6 +105,18 @@ k_residue_classify(ResArgs A, const int *__restrict__ iwork, const int *__restri
       }
     }
   }
+}
+
+__global__ void __launch_bounds__(32 * RES_WARPS)
+k_residue_classify(ResArgs A, const int *__restrict__ iwork, const int *__restrict__ nonzero,
+                   int *__restrict__ classes) {
+  residue_classify_body<false>(A, 0, iwork, nonzero, classes);
+}
+
+__global__ void __launch_bounds__(32 * RES_WARPS)
+k_residue_classify_curves(ResArgs A, long long curve_rows, const int *__restrict__ iwork,
+                          const int *__restrict__ nonzero, int *__restrict__ classes) {
+  residue_classify_body<true>(A, curve_rows, iwork, nonzero, classes);
 }
 
 }  // namespace vb200

@@ -15,8 +15,8 @@
  *                                                        (lib/mapping0.c:660-683) for the residue
  *   a loop of vorbis_analysis over N encoders        ->  vb200ms_*: blockout for every stream, the blocks that are
  *                                                        ready go to the device together, packets come back per stream;
- *                                                        un-managed, the packets are entropy coded on the device too
- *                                                        (one vb200_encode_packets call per block size and round)
+ *                                                        the packets are entropy coded on the device too (one
+ *                                                        vb200_encode_packets[_managed] call per block size and round)
  *
  * floor1_encode is fed the device's posts re-expanded to the fit scale: its quantise step maps them back to
  * the same integers and its predict/flag pass is idempotent on them, so it writes exactly the bits it would
@@ -25,7 +25,8 @@
  *
  * Bitrate-managed encoders (vorbis_encode_init) take the same path: one vb200_encode_dsp_managed call per batch
  * returns all PACKETBLOBS curves of every block and the host writes all PACKETBLOBS packets of each (the seam is
- * the batch of one block; vb200ms_open_managed opens a managed multi-stream driver).  A CUDA failure surfaces as OV_EFAULT from vorbis_analysis and latches in
+ * the batch of one block; vb200ms_open_managed opens a managed multi-stream driver, which codes all PACKETBLOBS
+ * packets on the device where the context takes the setup).  A CUDA failure surfaces as OV_EFAULT from vorbis_analysis and latches in
  * the binding (vb200shim_error).  Compiled like any libvorbis-internal backend against lib/codec_internal.h
  * (oracle/Makefile target `dropin`); INTEGRATION.md shows the registry line a maintainer changes.
  */
@@ -284,26 +285,41 @@ impl:
   return OV_EIMPL;
 }
 
-/* blocks[0..nb) of one size, un-managed, entropy coded on the device: ONE vb200_encode_packets call (PCM in, packets
- * out), then per block on all host threads the state mapping0_forward leaves (vbi->ampmax, vb->mode) and the packet
- * bits into packetblob[PACKETBLOBS/2], in pieces of up to 32 bits (oggpack_write is all that libogg and the
- * stand-in both provide) */
+/* bits bits of a device packet (bit k of the packet is bit k%8 of byte k/8) onto opb, in pieces of up to 32 bits
+ * (oggpack_write is all that libogg and the stand-in both provide) */
+static void write_packet_bits(oggpack_buffer *opb, const uint8_t *p, long bits){
+  long k;
+  int c;
+  for(k = 0; k < bits; k += 32){
+    const int take = bits - k < 32 ? (int)(bits - k) : 32, nbytes = (take + 7) >> 3;
+    unsigned long v = 0;
+    for(c = 0; c < nbytes; c++) v |= (unsigned long)p[(k >> 3) + c] << (8*c);
+    oggpack_write(opb, v, take);
+  }
+}
+
+/* blocks[0..nb) of one size, entropy coded on the device: ONE vb200_encode_packets call (PCM in, packets out; when
+ * bitrate-managed ONE vb200_encode_packets_managed call, all PACKETBLOBS packets of every block), then per block on
+ * all host threads the state mapping0_forward leaves (vbi->ampmax, vb->mode) and the packet bits into
+ * packetblob[PACKETBLOBS/2] (managed: packet k into packetblob[k], for lib/bitrate.c to choose from) */
 static int forward_batch_packets(vb200_binding *bind, ms_batch *B, vorbis_block **blocks, int nb, int W, batch_after after,
                                  void *user){
   vb200_ctx *ctx = vb200shim_ctx(bind);
   vorbis_info *vi = blocks[0]->vd->vi;
   const int ch = vi->channels, N = (int)blocks[0]->pcmend;
+  const int managed = vorbis_bitrate_managed(blocks[0]), curves = managed ? PACKETBLOBS : 1;
   const int bound = vb200_encode_packet_bound(ctx, W);
   vb200_encode_io io;
   int i, c, rc;
   PROF_T0();
   if(bound < 0) return OV_EFAULT;
   if((rc = batch_reserve(B, (size_t)nb, ch, N, 1))) return rc;
-  if(B->pkt_cap < (size_t)nb*bound || !B->pkt_off){
+  if(B->pkt_cap < (size_t)curves*nb*bound || !B->pkt_off){
     free(B->pkt); free(B->pkt_off); free(B->pkt_bits);
-    B->pkt = (uint8_t*)malloc((size_t)nb*bound); B->pkt_off = (int64_t*)malloc(sizeof(int64_t)*B->cap_blocks);
-    B->pkt_bits = (int32_t*)malloc(sizeof(int32_t)*B->cap_blocks);
-    B->pkt_cap = B->pkt ? (size_t)nb*bound : 0;
+    B->pkt = (uint8_t*)malloc((size_t)curves*nb*bound);
+    B->pkt_off = (int64_t*)malloc(sizeof(int64_t)*curves*B->cap_blocks);
+    B->pkt_bits = (int32_t*)malloc(sizeof(int32_t)*curves*B->cap_blocks);
+    B->pkt_cap = B->pkt ? (size_t)curves*nb*bound : 0;
     if(!B->pkt || !B->pkt_off || !B->pkt_bits) return OV_EFAULT;
   }
 #pragma omp parallel for private(c) schedule(static) if(nb > 8)
@@ -316,26 +332,23 @@ static int forward_batch_packets(vb200_binding *bind, ms_batch *B, vorbis_block 
   memset(&io, 0, sizeof(io));
   io.pcm = B->pcm; io.pcm_fmt = VB200_PCM_F32_BLOCKS; io.desc = B->desc; io.independent = 1; io.ampmax_out = B->ampmax;
   PROF_ADD(2);
-  rc = vb200_encode_packets(ctx, W, nb, 1, PACKETBLOBS/2, &io, B->pkt_off, B->pkt_bits, B->pkt, (int64_t)B->pkt_cap);
+  rc = managed ? vb200_encode_packets_managed(ctx, W, nb, 1, &io, B->pkt_off, B->pkt_bits, B->pkt, (int64_t)B->pkt_cap)
+               : vb200_encode_packets(ctx, W, nb, 1, PACKETBLOBS/2, &io, B->pkt_off, B->pkt_bits, B->pkt, (int64_t)B->pkt_cap);
   PROF_ADD(3);
   if(rc){
     vb200shim_set_error(bind, rc);
-    fprintf(stderr, "vb200 mapping0: vb200_encode_packets failed (%d): %s\n", rc, vb200_last_error());
+    fprintf(stderr, "vb200 mapping0: vb200_encode_packets%s failed (%d): %s\n", managed ? "_managed" : "", rc, vb200_last_error());
     return OV_EFAULT;
   }
 #pragma omp parallel for schedule(dynamic, 4) if(nb > 8)
   for(i = 0; i < nb; i++){
     vorbis_block_internal *vbi = (vorbis_block_internal*)blocks[i]->internal;
-    oggpack_buffer *opb = vbi->packetblob[PACKETBLOBS/2];
-    const uint8_t *p = B->pkt + B->pkt_off[i];
-    long k;
+    int k;
     vbi->ampmax = B->ampmax[i];                                /* lib/mapping0.c:576 */
     blocks[i]->mode = W;
-    for(k = 0; k < B->pkt_bits[i]; k += 32){
-      const int take = B->pkt_bits[i] - k < 32 ? (int)(B->pkt_bits[i] - k) : 32, nbytes = (take + 7) >> 3;
-      unsigned long v = 0;
-      for(c = 0; c < nbytes; c++) v |= (unsigned long)p[(k >> 3) + c] << (8*c);
-      oggpack_write(opb, v, take);
+    for(k = 0; k < curves; k++){                               /* curve k of block i: packet k*nb + i */
+      const size_t j = (size_t)k*nb + i;
+      write_packet_bits(vbi->packetblob[managed ? k : PACKETBLOBS/2], B->pkt + B->pkt_off[j], B->pkt_bits[j]);
     }
     if(after) after(user, i);
   }
@@ -395,7 +408,7 @@ typedef struct vb200ms {
   int32_t *env_state; uint8_t *env_ret; size_t env_ret_cap;
   int threads;
   vb200ms_sink_t sink; void *sink_user; int cur_w;
-  int entropy_dev;               /* the context took the encoder's vb200_encode_entropy_setup (un-managed only) */
+  int entropy_dev;               /* the context took the encoder's vb200_encode_entropy_setup */
   int host_entropy;              /* diagnostic: code on the host anyway (vb200ms_set_host_entropy) */
 } vb200ms;
 
@@ -481,7 +494,7 @@ static vb200ms *ms_open(int nstreams, int channels, long rate, float quality, in
   }
   if(vb200shim_attach(&m->vd[0], device)){ vb200ms_close(m); return NULL; }
   m->bind = vb200shim_binding(&m->vd[0]);
-  if(!managed){                  /* the device coder where the context takes this setup, else the host path */
+  {                              /* the device coder where the context takes this setup, else the host path */
     struct vb200_encode_entropy_setup es;
     int rc = vb200ms_entropy_setup_build(&m->vd[0], &es);
     if(!rc){
@@ -507,7 +520,8 @@ vb200ms *vb200ms_open(int nstreams, int channels, long rate, float quality, int 
 }
 
 /* bitrate-managed encoders (CBR / ABR): each round's blocks of a size go to the device in one
- * vb200_encode_dsp_managed call, and every stream's bitrate manager picks its packets in round_after */
+ * vb200_encode_packets_managed call (vb200_encode_dsp_managed on the host path), and every stream's bitrate manager
+ * picks its packets in round_after */
 vb200ms *vb200ms_open_managed(int nstreams, int channels, long rate, long max_br, long nominal_br, long min_br, int device){
   return ms_open(nstreams, channels, rate, 0.f, 1, max_br, nominal_br, min_br, device);
 }

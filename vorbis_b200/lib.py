@@ -38,7 +38,7 @@ EXPORTS = [
     "vb200_decode_entropy_setup", "vb200_decode_entropy_dev", "vb200_decode_entropy",
     "vb200_decode_packets_resume_dev", "vb200_decode_packets_resume",
     "vb200_encode_entropy_setup", "vb200_encode_packet_bound", "vb200_encode_entropy_dev", "vb200_encode_entropy",
-    "vb200_encode_packets",
+    "vb200_encode_packets", "vb200_encode_entropy_managed_dev", "vb200_encode_packets_managed",
     "vb200_residue_partvals", "vb200_residue_classify_dev", "vb200_residue_classify",
     "vb200_plan_blocks", "vb200_encode_streams_dev", "vb200_encode_streams",
     "vb200_encode_streams_managed_dev", "vb200_encode_streams_managed",
@@ -131,6 +131,10 @@ def load():
     L.vb200_encode_entropy.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp, C.c_int64]
     L.vb200_encode_packets.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.c_int, C.POINTER(abi.EncodeIO), vp, vp, vp,
                                        C.c_int64]
+    L.vb200_encode_entropy_managed_dev.argtypes = [vp, C.c_int, C.c_int, C.c_int64, vp, vp, vp, vp, C.c_int64, vp, vp,
+                                                   vp]
+    L.vb200_encode_packets_managed.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.POINTER(abi.EncodeIO), vp, vp, vp,
+                                               C.c_int64]
     L.vb200_envelope_search_dev.argtypes = [vp, C.c_int, vp, C.c_int, C.c_int64, C.c_int, C.c_int, vp, vp, vp]
     L.vb200_envelope_search.argtypes = [vp, C.c_int, vp, C.c_int, C.c_int64, C.c_int, C.c_int, vp, vp]
     L.vb200_envelope_apply_marks.argtypes = [vp, C.c_int, C.c_int, vp]
@@ -739,6 +743,59 @@ class Context:
         self._chk(self.L.vb200_encode_packets(self.h, W, nstreams, nb // nstreams, blobno, C.byref(io),
                                               _ptr(out["pkt_off"]), _ptr(out["pkt_bits"]), _ptr(out["data"]), cap))
         return self._packets(out, nb)
+
+    def encode_entropy_managed_dev(self, W, nblocks, blob_blocks, d_desc, d_posts, d_nonzero, d_iwork, pkt_stride,
+                                   d_pkt_bits, d_data, stream=None, check=True):
+        """vb200_encode_entropy_managed_dev: all 15 packets of every block, packet (k, b) at d_data +
+        (k*nblocks + b)*pkt_stride; returns the status"""
+        rc = self.L.vb200_encode_entropy_managed_dev(self.h, W, nblocks, blob_blocks, _ptr(d_desc), _ptr(d_posts),
+                                                     _ptr(d_nonzero), _ptr(d_iwork), pkt_stride, _ptr(d_pkt_bits),
+                                                     _ptr(d_data), _ptr(stream))
+        if check:
+            self._chk(rc)
+        return rc
+
+    def encode_packets_managed(self, W, pcm, desc, nstreams=None, fmt=0, hop=0, ampmax0=None, independent=None,
+                               data_cap=None, check=True):
+        """vb200_encode_packets_managed: PCM as for encode_dsp_managed in; {"packets": [15][nb] bytes, "pkt_bits"
+        [15][nb], "pkt_off" [15][nb], "data", "ampmax_out"} out (and "rc" when check is False, in which case an error
+        does not raise and "packets" is absent)"""
+        ch, N = self.channels, self.bs[W]
+        NB = abi.PACKETBLOBS
+        desc = np.ascontiguousarray(desc, abi.BLOCKDESC_DTYPE)
+        nb = desc.shape[0]
+        if nstreams is None:
+            nstreams = nb
+            if independent is None:
+                independent = True
+        io = abi.EncodeIO()
+        if fmt == 0:
+            pcm = np.ascontiguousarray(pcm, np.float32).reshape(nb, ch, N)
+        elif fmt == PCM_F32_PLANAR:
+            pcm = np.ascontiguousarray(pcm, np.float32)
+            io.stream_stride = pcm.shape[2]
+        else:
+            pcm = np.ascontiguousarray(pcm, np.int16)
+            io.stream_stride = pcm.shape[1]
+        io.pcm, io.pcm_fmt, io.hop, io.desc = pcm.ctypes.data, fmt, hop, desc.ctypes.data
+        io.independent = 1 if independent else 0
+        if ampmax0 is not None:
+            ampmax0 = np.ascontiguousarray(ampmax0, np.float32)
+            io.ampmax0 = ampmax0.ctypes.data
+        cap = NB * nb * self.packet_bound(W) if data_cap is None else data_cap
+        out = {"pkt_off": np.zeros((NB, nb), np.int64), "pkt_bits": np.zeros((NB, nb), np.int32),
+               "data": np.zeros(max(cap, 1), np.uint8), "ampmax_out": np.zeros(nb, np.float32)}
+        io.ampmax_out = out["ampmax_out"].ctypes.data
+        rc = self.L.vb200_encode_packets_managed(self.h, W, nstreams, nb // nstreams, C.byref(io), _ptr(out["pkt_off"]),
+                                                 _ptr(out["pkt_bits"]), _ptr(out["data"]), cap)
+        if not check:
+            out["rc"] = rc
+            return out
+        self._chk(rc)
+        off, bits, data = out["pkt_off"], out["pkt_bits"], out["data"]
+        out["packets"] = [[bytes(data[off[k, i]:off[k, i] + (bits[k, i] + 7) // 8]) for i in range(nb)]
+                          for k in range(NB)]
+        return out
 
     # ---- envelope / block-switch detector (lib/envelope.c) --------------------------------------
     def envelope_search(self, pcm, first_step, nsteps, state=None, fmt=PCM_F32_PLANAR):
