@@ -20,9 +20,11 @@
  *   - a context keeps grow-only device scratch: use one context per host thread
  *     (the reference is single threaded per vorbis_dsp_state as well, SURVEY §8b);
  *     the host-pointer entry points serialise on a per-context mutex.  _dev calls
- *     that use that scratch (Phase A, encode_dsp, encode_streams, envelope_search)
- *     may be issued on different CUDA streams: each waits (on the device, via an
- *     event) for the previous such call of the same context, so they never share
+ *     that use that scratch (Phase A, encode_dsp, encode_dsp_managed,
+ *     encode_streams, encode_streams_managed, envelope_search, encode_entropy,
+ *     encode_entropy_managed) may be issued on different CUDA streams: each waits
+ *     (on the device, via an event) for the previous such call of the same
+ *     context, so they never share
  *     the scratch in time.  Growing the scratch re-allocates (cudaFree/cudaMalloc
  *     synchronise the device): the first call at a new maximum size is not
  *     asynchronous.

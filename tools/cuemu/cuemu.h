@@ -233,6 +233,7 @@ static inline unsigned __brev(unsigned v) { unsigned r = 0; for (int i = 0; i < 
 static inline float __fadd_rn(float a, float b) { return a + b; }
 static inline float __fmul_rn(float a, float b) { return a * b; }
 static inline float __fdiv_rn(float a, float b) { return a / b; }
+static inline float __fdividef(float a, float b) { return a / b; }
 static inline float __fsqrt_rn(float a) { return sqrtf(a); }
 using std::max;
 using std::min;

@@ -47,10 +47,18 @@ extern "C" const char *vb200_last_error(void) { return g_err.c_str(); }
 
 // ======================================================================== //
 // context
+// a grow-only device buffer, freed with the context
 struct DevBuf {
   void *p = nullptr;
   size_t cap = 0;
+  DevBuf() = default;
+  DevBuf(const DevBuf &) = delete;
+  DevBuf &operator=(const DevBuf &) = delete;
+  ~DevBuf() { if (p) cudaFree(p); }
 };
+
+constexpr int STAGE_SLOTS = 16;      // device buffers one host form may stage (HostIO)
+constexpr int ENC_SETS = 4;          // buffer sets of the pipelined vb200_encode_dsp
 
 struct vb200_ctx {
   int device = 0;
@@ -70,27 +78,34 @@ struct vb200_ctx {
   PsyDev dpsy[4];
   std::vector<void *> owned;         // device allocations freed at destroy
   std::atomic<uint64_t> launches{0};
-  // grow-only scratch for the host-buffer entry points and phase A intermediates
-  DevBuf scratch[16];
-  DevBuf lane_buf[2][10];            // per-lane device buffers of the pipelined host Phase-A path
-  cudaStream_t s_lane[2] = {nullptr, nullptr};
+  // Device scratch: one arena (a grow-only buffer, cut into regions by carve()) per owning call family.  An arena
+  // is carved at most once per call, and the arenas one call uses at the same time are different arenas.
+  //   stage[]   HostIO: the device copies of a host form's inputs and outputs; nothing else uses it
+  //   cycles    the debug cycle counters (VB200_PHASE_TIMING, VB200_FLOOR1_TIMING), kept between calls
+  //   phaseA    phaseA_dev_common: log spectrum, row and block maxima
+  //   lane[]    the pipelined host vb200_analysis_phaseA, one per lane
+  //   enc       the encode chain of vb200_encode_dsp_dev and vb200_encode_packets
+  //   set[]     the pipelined host vb200_encode_dsp, one per buffer set: a chunk's copies and its chain
+  //   mgd       vb200_encode_dsp_managed_dev
+  //   plan      block planning: vb200_plan_blocks, and the envelope state, marks and plan tables of
+  //             vb200_encode_streams[_managed]_dev
+  //   chain     the chains of vb200_encode_streams[_managed]_dev, sized by the plan
+  //   env_scratch  vb200_envelope_search[_dev] (c->env holds the detector's tables)
+  //   coder     the entropy coder: residue classes and the per-CTA residue copies
+  //   pack      the host forms of the entropy coder: packet offsets and the packed bytes
+  DevBuf stage[STAGE_SLOTS], cycles, phaseA, lane[2], enc, set[ENC_SETS], mgd, plan, chain, env_scratch, coder, pack;
+  cudaStream_t s_pipe[2] = {nullptr, nullptr};
   const ResDev *d_res[2] = {nullptr, nullptr};        // [VB200_MAX_SUBMAPS] residue class parameters per block size
   int res_partvals[2] = {0, 0};
   EnvDev env;                        // envelope detector tables (N = 128 transform, windows, thresholds)
-  DevBuf env_buf[4];                 // scratch of vb200_envelope_search[_dev]
   int grid_div = 1;                  // see grid_for
   cudaStream_t s_split[2] = {nullptr, nullptr};       // vb200_encode_dsp_dev: two concurrent half-batches
   cudaEvent_t ev_fork = nullptr, ev_join[2] = {nullptr, nullptr};
-  DevBuf enc_buf[8];                 // scratch of vb200_encode_dsp_dev
-  DevBuf str_buf[50];                // scratch of vb200_plan_blocks / vb200_encode_streams[_managed][_dev]
-  DevBuf mgd_buf[24];                // scratch + host-call staging of vb200_encode_dsp_managed[_dev]
-  // vb200_encode_dsp (host buffers): chunks rotate over ENC_SETS buffer sets; one stream per copy direction and
+  // vb200_encode_dsp (host buffers): chunks rotate over the ENC_SETS buffer sets; one stream per copy direction and
   // two compute streams, ordered by events (see there)
-  DevBuf enc_lane[4][17];
   cudaStream_t s_enc[3] = {nullptr, nullptr, nullptr};   // compute 0, compute 1, host->device
   cudaStream_t s_d2h = nullptr;
-  cudaEvent_t ev_h2d[4] = {nullptr, nullptr, nullptr, nullptr}, ev_cmp[4] = {nullptr, nullptr, nullptr, nullptr},
-              ev_d2h[4] = {nullptr, nullptr, nullptr, nullptr};
+  cudaEvent_t ev_h2d[ENC_SETS] = {}, ev_cmp[ENC_SETS] = {}, ev_d2h[ENC_SETS] = {};
   int psy_ctas_per_sm = 5;
   int psy_carveout_ctas = -1;        // CTAs/SM the generic psy kernel's shared-memory carve-out was last set for (per device)
   // The *_dev entry points keep their intermediates in per-context scratch: two calls in flight on different
@@ -105,11 +120,9 @@ struct vb200_ctx {
   // vb200_decode_entropy_setup: the device tables of the entropy decoders (ent.books == nullptr: none registered)
   EntDev ent{};
   std::vector<void *> ent_owned;
-  // vb200_encode_entropy_setup: the tables of the entropy coder (eent.books == nullptr: none registered), and the
-  // scratch of the encode entropy entry points
+  // vb200_encode_entropy_setup: the tables of the entropy coder (eent.books == nullptr: none registered)
   EncEntDev eent{};
   std::vector<void *> eent_owned;
-  DevBuf eent_buf[24];
   std::mutex mu;
   // optional per-kernel timing of the last Phase-A call (bench roofline evidence)
   bool profiling = false;
@@ -137,8 +150,7 @@ static int upload(vb200_ctx *c, const T *src, size_t count, const T **dst) {
   return 0;
 }
 
-static int ensure(vb200_ctx *c, int slot, size_t bytes, void **out) {
-  DevBuf &b = c->scratch[slot];
+static int ensure_buf(DevBuf &b, size_t bytes, void **out) {
   if (b.cap < bytes) {
     if (b.p) CU(cudaFree(b.p));
     b.p = nullptr; b.cap = 0;
@@ -146,6 +158,29 @@ static int ensure(vb200_ctx *c, int slot, size_t bytes, void **out) {
     b.cap = bytes;
   }
   *out = b.p;
+  return 0;
+}
+
+// One call's regions of an arena.  carve() runs the layout twice: first to sum the sizes, then, once the arena
+// holds that sum, to hand out the pointers.  Every region starts on a 256-byte boundary, as a cudaMalloc'd buffer
+// does: the int4 / short4 loads of k_pack_s16 and the floor fit's four-lines-per-load path rely on it.
+struct Carve {
+  char *base;
+  size_t off;
+  template <class T> T *take(size_t n) {
+    T *p = base ? (T *)(base + off) : nullptr;
+    off += (sizeof(T) * n + 255) & ~(size_t)255;
+    return p;
+  }
+};
+
+template <class F> static int carve(DevBuf &arena, F &&layout) {
+  Carve sizes{nullptr, 0};
+  layout(sizes);
+  void *p; int rc;
+  if ((rc = ensure_buf(arena, sizes.off, &p))) return rc;
+  Carve place{(char *)p, 0};
+  layout(place);
   return 0;
 }
 
@@ -181,7 +216,7 @@ static int ctx_build(vb200_ctx *c, const vb200_setup *s, int device) {
   CU(cudaGetDeviceProperties(&prop, device));
   c->sm_count = prop.multiProcessorCount;
   CU(cudaStreamCreateWithFlags(&c->s_main, cudaStreamNonBlocking));
-  for (auto &st : c->s_lane) CU(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
+  for (auto &st : c->s_pipe) CU(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
   for (auto &st : c->s_enc) CU(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
   CU(cudaStreamCreateWithFlags(&c->s_d2h, cudaStreamNonBlocking));
   for (auto &e : c->ev_h2d) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
@@ -410,17 +445,10 @@ extern "C" void vb200_ctx_destroy(vb200_ctx *c) {
   if (!c) return;
   cudaSetDevice(c->device);
   for (void *p : c->owned) cudaFree(p);
-  for (auto &b : c->scratch) if (b.p) cudaFree(b.p);
-  for (auto &l : c->lane_buf) for (auto &b : l) if (b.p) cudaFree(b.p);
-  for (auto &st : c->s_lane) if (st) cudaStreamDestroy(st);
+  for (auto &st : c->s_pipe) if (st) cudaStreamDestroy(st);
   for (auto &st : c->s_split) if (st) cudaStreamDestroy(st);
   if (c->ev_fork) cudaEventDestroy(c->ev_fork);
   for (auto &e : c->ev_join) if (e) cudaEventDestroy(e);
-  for (auto &b : c->enc_buf) if (b.p) cudaFree(b.p);
-  for (auto &b : c->env_buf) if (b.p) cudaFree(b.p);
-  for (auto &l : c->enc_lane) for (auto &b : l) if (b.p) cudaFree(b.p);
-  for (auto &b : c->mgd_buf) if (b.p) cudaFree(b.p);
-  for (auto &b : c->str_buf) if (b.p) cudaFree(b.p);
   for (auto &st : c->s_enc) if (st) cudaStreamDestroy(st);
   if (c->s_d2h) cudaStreamDestroy(c->s_d2h);
   for (auto &e : c->ev_h2d) if (e) cudaEventDestroy(e);
@@ -431,8 +459,7 @@ extern "C" void vb200_ctx_destroy(vb200_ctx *c) {
   if (c->ev_scratch) cudaEventDestroy(c->ev_scratch);
   for (void *p : c->ent_owned) cudaFree(p);
   for (void *p : c->eent_owned) cudaFree(p);
-  for (auto &b : c->eent_buf) if (b.p) cudaFree(b.p);
-  delete c;
+  delete c;                                            // the arenas free themselves (DevBuf)
 }
 
 extern "C" int vb200_ctx_table(vb200_ctx *c, int W, int which, void *dst, int cap) {
@@ -467,7 +494,7 @@ extern "C" int vb200_debug_phase_cycles(vb200_ctx *c, unsigned long long *out16,
   if (!c || !out16) return fail(VB200_EINVAL, "null argument");
   CU(cudaSetDevice(c->device));
   void *p; int rc;
-  if ((rc = ensure(c, 10, 16 * sizeof(unsigned long long), &p))) return rc;
+  if ((rc = ensure_buf(c->cycles, 16 * sizeof(unsigned long long), &p))) return rc;
   CU(cudaDeviceSynchronize());
   CU(cudaMemcpy(out16, p, 16 * sizeof(unsigned long long), cudaMemcpyDeviceToHost));
   if (reset) CU(cudaMemset(p, 0, 16 * sizeof(unsigned long long)));
@@ -1107,12 +1134,14 @@ extern "C" int vb200_mdct_backward_dev(vb200_ctx *c, int W, int nvec, const floa
   return post_launch(c);
 }
 
-// generic "copy in, run, copy out" for the host-buffer variants
+// generic "copy in, run, copy out" for the host-buffer variants: every device buffer a host form stages, input
+// (src != nullptr: copied in on s_main) or output, takes the next buffer of the context's staging pool
 struct HostIO {
   vb200_ctx *c;
   int slot = 0;
   int h2d(const void *src, size_t bytes, void **d) {
-    int rc = ensure(c, slot++, bytes, d); if (rc) return rc;
+    if (slot == STAGE_SLOTS) return fail(VB200_EFAULT, "host call stages more buffers than the staging pool holds");
+    int rc = ensure_buf(c->stage[slot++], bytes, d); if (rc) return rc;
     if (src) CU(cudaMemcpyAsync(*d, src, bytes, cudaMemcpyHostToDevice, c->s_main));
     return 0;
   }
@@ -1320,7 +1349,7 @@ static int phaseA_psy_launch(vb200_ctx *c, int W, int nblocks, const vb200_phase
   A.tap_noise = io->tap_noise; A.tap_tone = io->tap_tone;
   A.dbg_cycles = nullptr;
   if (getenv("VB200_PHASE_TIMING")) {
-    void *p; if ((rc = ensure(c, 10, 16 * sizeof(unsigned long long), &p))) return rc;
+    void *p; if ((rc = ensure_buf(c->cycles, 16 * sizeof(unsigned long long), &p))) return rc;
     A.dbg_cycles = (unsigned long long *)p;
   }
   // VB200_PSY_V1=1 forces the generic kernel, so that the tests can check it on the setups the fast one takes
@@ -1383,17 +1412,6 @@ static int phaseA_launch(vb200_ctx *c, int W, int nblocks, const vb200_phaseA_io
   return 0;
 }
 
-static int ensure_buf(DevBuf &b, size_t bytes, void **out) {
-  if (b.cap < bytes) {
-    if (b.p) CU(cudaFree(b.p));
-    b.p = nullptr; b.cap = 0;
-    CU(cudaMalloc(&b.p, bytes));
-    b.cap = bytes;
-  }
-  *out = b.p;
-  return 0;
-}
-
 static int phaseA_dev_common(vb200_ctx *c, int W, int nblocks, const vb200_phaseA_io *io,
                              int nstreams, int bps, const float *d_amp0, void *stream,
                              const PcmSrc *pcmsrc = nullptr) {
@@ -1402,14 +1420,16 @@ static int phaseA_dev_common(vb200_ctx *c, int W, int nblocks, const vb200_phase
   if (!io || (!io->pcm && !pcmsrc) || !io->desc || !io->mdct || !io->logmdct || !io->logmask || !io->ampmax_out)
     return fail(VB200_EINVAL, "phase A io pointers");
   if (nblocks <= 0) return 0;
-  const int ch = c->setup.channels, n = c->dx[W].N / 2;
-  void *d_logfft = io->tap_logfft, *d_lmax, *d_gmax; int rc;
-  if (!d_logfft && (rc = ensure(c, 13, sizeof(float) * (size_t)nblocks * ch * n, &d_logfft))) return rc;
-  if ((rc = ensure(c, 14, sizeof(float) * (size_t)nblocks * ch, &d_lmax))) return rc;
-  if ((rc = ensure(c, 15, sizeof(float) * (size_t)nblocks, &d_gmax))) return rc;
+  const size_t rows = (size_t)nblocks * c->setup.channels, n = c->dx[W].N / 2;
+  float *d_logfft, *d_lmax, *d_gmax; int rc;
+  if ((rc = carve(c->phaseA, [&](Carve &k) {
+         d_logfft = io->tap_logfft ? io->tap_logfft : k.take<float>(rows * n);
+         d_lmax = k.take<float>(rows);
+         d_gmax = k.take<float>(nblocks);
+       }))) return rc;
   if ((rc = scratch_begin(c, (cudaStream_t)stream))) return rc;
-  if ((rc = phaseA_launch(c, W, nblocks, io, nstreams, bps, d_amp0, (cudaStream_t)stream,
-                          (float *)d_logfft, (float *)d_lmax, (float *)d_gmax, pcmsrc))) return rc;
+  if ((rc = phaseA_launch(c, W, nblocks, io, nstreams, bps, d_amp0, (cudaStream_t)stream, d_logfft, d_lmax, d_gmax,
+                          pcmsrc))) return rc;
   return scratch_end(c, (cudaStream_t)stream);
 }
 
@@ -1449,35 +1469,33 @@ static int phaseA_host_pipelined(vb200_ctx *c, int W, int nblocks, const vb200_p
   if (chunk > nblocks) chunk = nblocks;
   const size_t crow = (size_t)chunk * ch;
   int rc;
+  vb200_phaseA_io lane[2];
+  float *logfft[2], *lmax[2], *gmax[2];
   for (int L = 0; L < 2; L++) {
-    void *p;
-    const size_t sz[9] = {sizeof(float) * crow * N, sizeof(vb200_block_desc) * (size_t)chunk,
-                          sizeof(float) * crow * n, sizeof(float) * crow * n, sizeof(float) * crow * n,
-                          sizeof(float) * (size_t)chunk, sizeof(float) * crow * n, sizeof(float) * crow,
-                          sizeof(float) * (size_t)chunk};
-    for (int k = 0; k < 9; k++) if ((rc = ensure_buf(c->lane_buf[L][k], sz[k], &p))) return rc;
+    vb200_phaseA_io &d = lane[L];
+    memset(&d, 0, sizeof(d));
+    if ((rc = carve(c->lane[L], [&](Carve &k) {
+           d.pcm = k.take<float>(crow * N); d.desc = k.take<vb200_block_desc>(chunk);
+           d.mdct = k.take<float>(crow * n); d.logmdct = k.take<float>(crow * n); d.logmask = k.take<float>(crow * n);
+           d.ampmax_out = k.take<float>(chunk);
+           logfft[L] = k.take<float>(crow * n); lmax[L] = k.take<float>(crow); gmax[L] = k.take<float>(chunk);
+         }))) return rc;
   }
   for (int b0 = 0, it = 0; b0 < nblocks; b0 += chunk, it++) {
     const int L = it & 1, nb = nblocks - b0 < chunk ? nblocks - b0 : chunk;
     const size_t rows = (size_t)nb * ch, r0 = (size_t)b0 * ch;
-    cudaStream_t st = c->s_lane[L];
-    DevBuf *B = c->lane_buf[L];
-    CU(cudaMemcpyAsync(B[0].p, h->pcm + r0 * N, sizeof(float) * rows * N, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync(B[1].p, h->desc + b0, sizeof(vb200_block_desc) * nb, cudaMemcpyHostToDevice, st));
-    vb200_phaseA_io d;
-    memset(&d, 0, sizeof(d));
-    d.pcm = (const float *)B[0].p; d.desc = (const vb200_block_desc *)B[1].p;
-    d.mdct = (float *)B[2].p; d.logmdct = (float *)B[3].p; d.logmask = (float *)B[4].p;
-    d.ampmax_out = (float *)B[5].p;
-    if ((rc = phaseA_launch(c, W, nb, &d, 0, 0, nullptr, st, (float *)B[6].p, (float *)B[7].p, (float *)B[8].p)))
-      return rc;
+    cudaStream_t st = c->s_pipe[L];
+    const vb200_phaseA_io &d = lane[L];
+    CU(cudaMemcpyAsync((void *)d.pcm, h->pcm + r0 * N, sizeof(float) * rows * N, cudaMemcpyHostToDevice, st));
+    CU(cudaMemcpyAsync((void *)d.desc, h->desc + b0, sizeof(vb200_block_desc) * nb, cudaMemcpyHostToDevice, st));
+    if ((rc = phaseA_launch(c, W, nb, &d, 0, 0, nullptr, st, logfft[L], lmax[L], gmax[L]))) return rc;
     CU(cudaMemcpyAsync(h->mdct + r0 * n, d.mdct, sizeof(float) * rows * n, cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(h->logmdct + r0 * n, d.logmdct, sizeof(float) * rows * n, cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(h->logmask + r0 * n, d.logmask, sizeof(float) * rows * n, cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(h->ampmax_out + b0, d.ampmax_out, sizeof(float) * nb, cudaMemcpyDeviceToHost, st));
   }
-  CU(cudaStreamSynchronize(c->s_lane[0]));
-  CU(cudaStreamSynchronize(c->s_lane[1]));
+  CU(cudaStreamSynchronize(c->s_pipe[0]));
+  CU(cudaStreamSynchronize(c->s_pipe[1]));
   return 0;
 }
 
@@ -1505,8 +1523,8 @@ extern "C" int vb200_analysis_phaseA(vb200_ctx *c, int W, int nblocks, const vb2
   if ((rc = io.h2d(nullptr, sizeof(float) * nblocks, &p))) return rc; d.ampmax_out = (float *)p;
   if (h->tap_noise) { if ((rc = io.h2d(nullptr, sizeof(float) * rows * n, &p))) return rc; d.tap_noise = (float *)p; }
   if (h->tap_tone) { if ((rc = io.h2d(nullptr, sizeof(float) * rows * n, &p))) return rc; d.tap_tone = (float *)p; }
-  if (h->tap_logfft) { if ((rc = ensure(c, 11, sizeof(float) * rows * n, &p))) return rc; d.tap_logfft = (float *)p; }
-  if (h->tap_mdct_raw) { if ((rc = ensure(c, 12, sizeof(float) * rows * n, &p))) return rc; d.tap_mdct_raw = (float *)p; }
+  if (h->tap_logfft) { if ((rc = io.h2d(nullptr, sizeof(float) * rows * n, &p))) return rc; d.tap_logfft = (float *)p; }
+  if (h->tap_mdct_raw) { if ((rc = io.h2d(nullptr, sizeof(float) * rows * n, &p))) return rc; d.tap_mdct_raw = (float *)p; }
   if ((rc = phaseA_dev_common(c, W, nblocks, &d, 0, 0, nullptr, c->s_main))) return rc;
   if ((rc = io.d2h(h->mdct, d.mdct, sizeof(float) * rows * n))) return rc;
   if ((rc = io.d2h(h->logmdct, d.logmdct, sizeof(float) * rows * n))) return rc;
@@ -1770,7 +1788,7 @@ extern "C" int vb200_floor1_fit_dev(vb200_ctx *c, int W, int floor_sel, int nrow
   void (*kern)(Floor1Args, int, const float *, const float *, int32_t *, int32_t *, unsigned long long *) =
       dbg ? k_floor1_fit<true> : k_floor1_fit<false>;
   void *p = nullptr;
-  if (dbg && (rc = ensure(c, 10, 16 * sizeof(unsigned long long), &p))) return rc;
+  if (dbg && (rc = ensure_buf(c->cycles, 16 * sizeof(unsigned long long), &p))) return rc;
   if ((rc = set_smem(kern, smem))) return rc;
   // one wave: as many CTAs per SM as registers and this shared-memory size let be resident
   CU(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
@@ -1874,6 +1892,21 @@ static size_t enc_pcm_bytes(const vb200_encode_io *io, int ch, int N, int nstrea
   }
 }
 
+// host forms of the chain: the inputs copied in, and int32 outputs of `curves` curves staged, in d
+static int enc_stage(HostIO &io, const vb200_encode_io *h, vb200_encode_io *d, int ch, int N, int nstreams, int bps,
+                     int curves) {
+  const size_t nb = (size_t)nstreams * bps, rows = curves * nb * ch;
+  void *p; int rc;
+  if ((rc = io.h2d(h->pcm, enc_pcm_bytes(h, ch, N, nstreams, bps), &p))) return rc; d->pcm = p;
+  if ((rc = io.h2d(h->desc, sizeof(vb200_block_desc) * nb, &p))) return rc; d->desc = (const vb200_block_desc *)p;
+  if ((rc = io.h2d(h->ampmax0, sizeof(float) * nstreams, &p))) return rc; d->ampmax0 = h->ampmax0 ? (const float *)p : nullptr;
+  if ((rc = io.h2d(nullptr, sizeof(int32_t) * rows * VB200_FLOOR1_STRIDE, &p))) return rc; d->posts = (int32_t *)p;
+  if ((rc = io.h2d(nullptr, sizeof(int32_t) * rows, &p))) return rc; d->nonzero = (int32_t *)p;
+  if ((rc = io.h2d(nullptr, sizeof(int32_t) * rows * (N / 2), &p))) return rc; d->iwork = p;
+  if ((rc = io.h2d(nullptr, sizeof(float) * nb, &p))) return rc; d->ampmax_out = (float *)p;
+  return 0;
+}
+
 static int enc_check(vb200_ctx *c, int W, int nstreams, int bps, int blobno, const vb200_encode_io *io) {
   if (!io || !io->pcm || !io->desc || !io->posts || !io->nonzero || !io->iwork || !io->ampmax_out)
     return fail(VB200_EINVAL, "encode io pointers");
@@ -1934,19 +1967,17 @@ static int encode_launch(vb200_ctx *c, int W, int nstreams, int bps, int blobno,
   return 0;
 }
 
-static int enc_scratch(DevBuf *B, size_t rows, size_t nblocks, size_t n, const vb200_encode_io *d, bool s16, EncScratch *S) {
-  void *p; int rc;
-  const size_t big = sizeof(float) * rows * n;
-  if (d && d->mdct) S->mdct = d->mdct; else { if ((rc = ensure_buf(B[0], big, &p))) return rc; S->mdct = (float *)p; }
-  if (d && d->logmdct) S->logmdct = d->logmdct; else { if ((rc = ensure_buf(B[1], big, &p))) return rc; S->logmdct = (float *)p; }
-  if (d && d->logmask) S->logmask = d->logmask; else { if ((rc = ensure_buf(B[2], big, &p))) return rc; S->logmask = (float *)p; }
-  if ((rc = ensure_buf(B[3], big, &p))) return rc; S->logfft = (float *)p;
-  if ((rc = ensure_buf(B[4], sizeof(float) * rows, &p))) return rc; S->lmax = (float *)p;
-  if ((rc = ensure_buf(B[5], sizeof(float) * nblocks, &p))) return rc; S->gmax = (float *)p;
-  if ((rc = ensure_buf(B[6], sizeof(int32_t) * rows, &p))) return rc; S->fitnz = (int32_t *)p;
-  S->iw32 = nullptr;
-  if (s16) { if ((rc = ensure_buf(B[7], sizeof(int32_t) * rows * n, &p))) return rc; S->iw32 = (int32_t *)p; }
-  return 0;
+// the chain's regions of an arena; d: the caller's spectra where it gives them
+static void enc_layout(Carve &k, size_t rows, size_t nblocks, size_t n, const vb200_encode_io *d, bool s16,
+                       EncScratch *S) {
+  S->mdct = d && d->mdct ? d->mdct : k.take<float>(rows * n);
+  S->logmdct = d && d->logmdct ? d->logmdct : k.take<float>(rows * n);
+  S->logmask = d && d->logmask ? d->logmask : k.take<float>(rows * n);
+  S->logfft = k.take<float>(rows * n);
+  S->lmax = k.take<float>(rows);
+  S->gmax = k.take<float>(nblocks);
+  S->fitnz = k.take<int32_t>(rows);
+  S->iw32 = s16 ? k.take<int32_t>(rows * n) : nullptr;
 }
 
 extern "C" int vb200_encode_dsp_dev(vb200_ctx *c, int W, int nstreams, int bps, int blobno,
@@ -1956,7 +1987,8 @@ extern "C" int vb200_encode_dsp_dev(vb200_ctx *c, int W, int nstreams, int bps, 
   if ((rc = enc_check(c, W, nstreams, bps, blobno, d))) return rc;
   const size_t ch = c->setup.channels, n = c->dx[W].N / 2, nblocks = (size_t)nstreams * bps;
   EncScratch S;
-  if ((rc = enc_scratch(c->enc_buf, nblocks * ch, nblocks, n, d, d->iwork_fmt == VB200_IWORK_S16, &S))) return rc;
+  if ((rc = carve(c->enc, [&](Carve &k) { enc_layout(k, nblocks * ch, nblocks, n, d, d->iwork_fmt == VB200_IWORK_S16, &S); })))
+    return rc;
   // Two half-batches (whole streams each) on two internal streams, every kernel launched with half its
   // grid: the halves drift apart, so CTAs of different kernels (shared-memory bound transform, issue bound
   // psy, latency bound floor fit) share the SMs instead of one kernel type owning the machine at a time.
@@ -2028,15 +2060,12 @@ struct MgdScratch {
   int32_t *fz3, *present;
 };
 
-static int mgd_scratch(DevBuf *B, size_t rows, size_t blob_rows, size_t n, MgdScratch *M) {
-  void *p; int rc;
-  const size_t big = sizeof(float) * rows * n;
-  if ((rc = ensure_buf(B[0], big, &p))) return rc; M->noise = (float *)p;
-  if ((rc = ensure_buf(B[1], big, &p))) return rc; M->tone = (float *)p;
-  if ((rc = ensure_buf(B[2], big, &p))) return rc; M->alt = (float *)p;
-  if ((rc = ensure_buf(B[3], sizeof(int32_t) * rows * 3, &p))) return rc; M->fz3 = (int32_t *)p;
-  if ((rc = ensure_buf(B[4], sizeof(int32_t) * blob_rows * VB200_PACKETBLOBS, &p))) return rc; M->present = (int32_t *)p;
-  return 0;
+static void mgd_layout(Carve &k, size_t rows, size_t blob_rows, size_t n, MgdScratch *M) {
+  M->noise = k.take<float>(rows * n);
+  M->tone = k.take<float>(rows * n);
+  M->alt = k.take<float>(rows * n);
+  M->fz3 = k.take<int32_t>(rows * 3);
+  M->present = k.take<int32_t>(blob_rows * VB200_PACKETBLOBS);
 }
 
 // Bitrate-managed mode after the psy stage (run with the noise and tone taps into M): the middle fit, the
@@ -2078,18 +2107,14 @@ extern "C" int vb200_encode_dsp_managed_dev(vb200_ctx *c, int W, int nstreams, i
   if ((rc = managed_check(c, W, nstreams, bps, d))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
   const int ch = c->setup.channels, n = c->dx[W].N / 2, nblocks = nstreams * bps;
-  const size_t rows = (size_t)nblocks * ch, big = sizeof(float) * rows * n;
-  DevBuf *B = c->mgd_buf;
-  void *p;
+  const size_t rows = (size_t)nblocks * ch;
   float *mdct, *logmdct, *logmask, *logfft, *lmax, *gmax;
   MgdScratch M;
-  if ((rc = ensure_buf(B[0], big, &p))) return rc; mdct = (float *)p;
-  if ((rc = ensure_buf(B[1], big, &p))) return rc; logmdct = (float *)p;
-  if ((rc = ensure_buf(B[2], big, &p))) return rc; logmask = (float *)p;
-  if ((rc = ensure_buf(B[3], big, &p))) return rc; logfft = (float *)p;
-  if ((rc = ensure_buf(B[4], sizeof(float) * rows, &p))) return rc; lmax = (float *)p;
-  if ((rc = ensure_buf(B[5], sizeof(float) * nblocks, &p))) return rc; gmax = (float *)p;
-  if ((rc = mgd_scratch(B + 6, rows, rows, n, &M))) return rc;
+  if ((rc = carve(c->mgd, [&](Carve &k) {
+         mdct = k.take<float>(rows * n); logmdct = k.take<float>(rows * n); logmask = k.take<float>(rows * n);
+         logfft = k.take<float>(rows * n); lmax = k.take<float>(rows); gmax = k.take<float>(nblocks);
+         mgd_layout(k, rows, rows, n, &M);
+       }))) return rc;
   if ((rc = scratch_begin(c, st))) return rc;
   vb200_phaseA_io a;
   memset(&a, 0, sizeof(a));
@@ -2114,29 +2139,16 @@ extern "C" int vb200_encode_dsp_managed(vb200_ctx *c, int W, int nstreams, int b
   const int ch = c->setup.channels, N = c->dx[W].N, n = N / 2;
   const size_t nb = (size_t)nstreams * bps, rows = nb * ch;
   constexpr int NB = VB200_PACKETBLOBS;
-  cudaStream_t st = c->s_main;
-  DevBuf *B = c->mgd_buf;
-  void *p;
+  HostIO io{c};
   vb200_encode_io d = *h;
   d.mdct = d.logmdct = d.logmask = nullptr;
-  const size_t pcm_bytes = enc_pcm_bytes(h, ch, N, nstreams, bps);
-  if ((rc = ensure_buf(B[12], pcm_bytes, &p))) return rc; d.pcm = p;
-  if ((rc = ensure_buf(B[13], sizeof(vb200_block_desc) * nb, &p))) return rc; d.desc = (const vb200_block_desc *)p;
-  if ((rc = ensure_buf(B[14], sizeof(float) * nstreams, &p))) return rc; d.ampmax0 = h->ampmax0 ? (const float *)p : nullptr;
-  if ((rc = ensure_buf(B[15], sizeof(int32_t) * NB * rows * VB200_FLOOR1_STRIDE, &p))) return rc; d.posts = (int32_t *)p;
-  if ((rc = ensure_buf(B[16], sizeof(int32_t) * NB * rows, &p))) return rc; d.nonzero = (int32_t *)p;
-  if ((rc = ensure_buf(B[17], sizeof(int32_t) * NB * rows * n, &p))) return rc; d.iwork = p;
-  if ((rc = ensure_buf(B[18], sizeof(float) * nb, &p))) return rc; d.ampmax_out = (float *)p;
-  CU(cudaMemcpyAsync((void *)d.pcm, h->pcm, pcm_bytes, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync((void *)d.desc, h->desc, sizeof(vb200_block_desc) * nb, cudaMemcpyHostToDevice, st));
-  if (h->ampmax0) CU(cudaMemcpyAsync((void *)d.ampmax0, h->ampmax0, sizeof(float) * nstreams, cudaMemcpyHostToDevice, st));
-  if ((rc = vb200_encode_dsp_managed_dev(c, W, nstreams, bps, &d, st))) return rc;
-  CU(cudaMemcpyAsync(h->posts, d.posts, sizeof(int32_t) * NB * rows * VB200_FLOOR1_STRIDE, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(h->nonzero, d.nonzero, sizeof(int32_t) * NB * rows, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(h->iwork, d.iwork, sizeof(int32_t) * NB * rows * n, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(h->ampmax_out, d.ampmax_out, sizeof(float) * nb, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  return 0;
+  if ((rc = enc_stage(io, h, &d, ch, N, nstreams, bps, NB))) return rc;
+  if ((rc = vb200_encode_dsp_managed_dev(c, W, nstreams, bps, &d, c->s_main))) return rc;
+  if ((rc = io.d2h(h->posts, d.posts, sizeof(int32_t) * NB * rows * VB200_FLOOR1_STRIDE))) return rc;
+  if ((rc = io.d2h(h->nonzero, d.nonzero, sizeof(int32_t) * NB * rows))) return rc;
+  if ((rc = io.d2h(h->iwork, d.iwork, sizeof(int32_t) * NB * rows * n))) return rc;
+  if ((rc = io.d2h(h->ampmax_out, d.ampmax_out, sizeof(float) * nb))) return rc;
+  return io.sync();
 }
 
 extern "C" int vb200_encode_dsp(vb200_ctx *c, int W, int nstreams, int bps, int blobno, const vb200_encode_io *h) {
@@ -2175,32 +2187,31 @@ extern "C" int vb200_encode_dsp(vb200_ctx *c, int W, int nstreams, int bps, int 
   // compute streams (a chunk's kernel tails overlap the next chunk's kernels).  Events carry the order
   // H2D(k) -> kernels(k) -> D2H(k) -> H2D(k + ENC_SETS); nothing else is ordered, so the copy engines run ahead
   // of / behind the kernels instead of every lane alternating copy and compute on its own stream.
-  constexpr int ENC_SETS = 4;
   cudaStream_t s_h2d = c->s_enc[2], s_d2h = c->s_d2h;
+  const bool s16 = h->iwork_fmt == VB200_IWORK_S16;
+  const size_t isz = s16 ? sizeof(int16_t) : sizeof(int32_t), cb = (size_t)cs * bps, crow = cb * ch;
+  vb200_encode_io dset[ENC_SETS];
+  EncScratch sset[ENC_SETS];
   for (int s0 = 0, it = 0; it < (int)sched.size(); s0 += sched[it], it++) {
     const int L = it % ENC_SETS, ns = sched[it];
     const size_t nb = (size_t)ns * bps, b0 = (size_t)s0 * bps, rows = nb * ch, r0 = b0 * ch;
     cudaStream_t st = c->s_enc[it & 1];
-    DevBuf *B = c->enc_lane[L];
-    void *p;
-    vb200_encode_io d = *h;
-    d.mdct = d.logmdct = d.logmask = nullptr;
-    if ((rc = ensure_buf(B[8], pcm_per_stream * cs, &p))) return rc; d.pcm = p;
-    if ((rc = ensure_buf(B[9], sizeof(vb200_block_desc) * (size_t)cs * bps, &p))) return rc; d.desc = (const vb200_block_desc *)p;
-    if ((rc = ensure_buf(B[10], sizeof(float) * cs, &p))) return rc; d.ampmax0 = h->ampmax0 ? (const float *)p : nullptr;
-    if ((rc = ensure_buf(B[11], sizeof(int32_t) * (size_t)cs * bps * ch * VB200_FLOOR1_STRIDE, &p))) return rc; d.posts = (int32_t *)p;
-    if ((rc = ensure_buf(B[12], sizeof(int32_t) * (size_t)cs * bps * ch, &p))) return rc; d.nonzero = (int32_t *)p;
-    const bool s16 = h->iwork_fmt == VB200_IWORK_S16;
-    const size_t isz = s16 ? sizeof(int16_t) : sizeof(int32_t);
-    if ((rc = ensure_buf(B[13], isz * (size_t)cs * bps * ch * n, &p))) return rc; d.iwork = p;
-    if (s16) { if ((rc = ensure_buf(B[15], sizeof(int32_t) * (size_t)cs * bps, &p))) return rc; d.overflow = (int32_t *)p; }
-    if (h->classes) {
-      if ((rc = ensure_buf(B[16], sizeof(int32_t) * (size_t)cs * bps * ch * (size_t)h->class_stride, &p))) return rc;
-      d.classes = (int32_t *)p;
+    vb200_encode_io &d = dset[L];
+    EncScratch &S = sset[L];
+    if (it < ENC_SETS) {                             // the set's first chunk: every chunk fits cs streams
+      d = *h;
+      d.mdct = d.logmdct = d.logmask = nullptr;
+      if ((rc = carve(c->set[L], [&](Carve &k) {
+             d.pcm = k.take<char>(pcm_per_stream * cs); d.desc = k.take<vb200_block_desc>(cb);
+             d.ampmax0 = h->ampmax0 ? k.take<float>(cs) : nullptr;
+             d.posts = k.take<int32_t>(crow * VB200_FLOOR1_STRIDE); d.nonzero = k.take<int32_t>(crow);
+             d.iwork = k.take<char>(isz * crow * n);
+             d.overflow = s16 ? k.take<int32_t>(cb) : nullptr;
+             d.classes = h->classes ? k.take<int32_t>(crow * (size_t)h->class_stride) : nullptr;
+             d.ampmax_out = k.take<float>(cb);
+             enc_layout(k, crow, cb, n, nullptr, s16, &S);
+           }))) return rc;
     }
-    if ((rc = ensure_buf(B[14], sizeof(float) * (size_t)cs * bps, &p))) return rc; d.ampmax_out = (float *)p;
-    EncScratch S;
-    if ((rc = enc_scratch(B, (size_t)cs * bps * ch, (size_t)cs * bps, n, nullptr, s16, &S))) return rc;
     if (it >= ENC_SETS) CU(cudaStreamWaitEvent(s_h2d, c->ev_d2h[L], 0));   // this set's previous chunk is back on the host
     CU(cudaMemcpyAsync((void *)d.pcm, (const char *)h->pcm + pcm_per_stream * s0, pcm_per_stream * ns, cudaMemcpyHostToDevice, s_h2d));
     CU(cudaMemcpyAsync((void *)d.desc, h->desc + b0, sizeof(vb200_block_desc) * nb, cudaMemcpyHostToDevice, s_h2d));
@@ -2236,16 +2247,13 @@ static int plan_check(vb200_ctx *c) {
   return 0;
 }
 
-// device: marks -> plan (slots final), gather tables and descriptors of both sizes; d_totals[2] on the device
+// device: marks -> plan (slots final), gather tables and descriptors of both sizes; d_totals[2] on the device.
+// d_work: 4 * nstreams ints of scratch.
 static int plan_launch(vb200_ctx *c, int nstreams, const int32_t *d_mark, int64_t mark_stride, int nsteps,
                        const int64_t *d_len, const int64_t *d_eof, int max_blocks, vb200_stream_block *d_plan,
                        int32_t *d_nblocks, const int cap[2], int2 *d_src[2], vb200_block_desc *d_desc[2],
-                       int32_t *d_totals, cudaStream_t st) {
-  void *p; int rc;
-  if ((rc = ensure_buf(c->str_buf[0], sizeof(int32_t) * 2 * (size_t)nstreams, &p))) return rc;
-  int32_t *d_counts = (int32_t *)p;
-  if ((rc = ensure_buf(c->str_buf[1], sizeof(int32_t) * 2 * (size_t)nstreams, &p))) return rc;
-  int32_t *d_offs = (int32_t *)p;
+                       int32_t *d_totals, int32_t *d_work, cudaStream_t st) {
+  int32_t *d_counts = d_work, *d_offs = d_work + 2 * (size_t)nstreams;
   const int g = (nstreams + 127) / 128;
   k_plan_blocks<<<g, 128, 0, st>>>(nstreams, c->setup.blocksizes[0], c->setup.blocksizes[1], d_mark, mark_stride, nsteps,
                                    d_len, d_eof, max_blocks, d_plan, d_nblocks, d_counts);
@@ -2266,27 +2274,28 @@ extern "C" int vb200_plan_blocks(vb200_ctx *c, int nstreams, const int32_t *mark
     return fail(VB200_EINVAL, "plan_blocks arguments");
   std::lock_guard<std::mutex> lk(c->mu);
   cudaStream_t st = c->s_main;
-  void *p;
   const size_t cap = (size_t)nstreams * max_blocks;
-  if ((rc = ensure_buf(c->str_buf[2], sizeof(int32_t) * (size_t)nstreams * mark_stride, &p))) return rc; int32_t *d_mark = (int32_t *)p;
-  if ((rc = ensure_buf(c->str_buf[3], sizeof(int64_t) * 2 * (size_t)nstreams, &p))) return rc; int64_t *d_len = (int64_t *)p, *d_eof = d_len + nstreams;
-  if ((rc = ensure_buf(c->str_buf[4], sizeof(vb200_stream_block) * cap, &p))) return rc; vb200_stream_block *d_plan = (vb200_stream_block *)p;
-  if ((rc = ensure_buf(c->str_buf[5], sizeof(int32_t) * ((size_t)nstreams + 2), &p))) return rc; int32_t *d_nb = (int32_t *)p, *d_tot = d_nb + nstreams;
-  int2 *d_src[2]; vb200_block_desc *d_desc[2];
-  for (int w = 0; w < 2; w++) {
-    if ((rc = ensure_buf(c->str_buf[6 + w], sizeof(int2) * cap, &p))) return rc; d_src[w] = (int2 *)p;
-    if ((rc = ensure_buf(c->str_buf[8 + w], sizeof(vb200_block_desc) * cap, &p))) return rc; d_desc[w] = (vb200_block_desc *)p;
-  }
-  CU(cudaMemcpyAsync(d_mark, mark, sizeof(int32_t) * (size_t)nstreams * mark_stride, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync(d_len, pcm_len, sizeof(int64_t) * nstreams, cudaMemcpyHostToDevice, st));
-  if (eof) CU(cudaMemcpyAsync(d_eof, eof, sizeof(int64_t) * nstreams, cudaMemcpyHostToDevice, st));
+  HostIO io{c};
+  void *dm, *dl, *de = nullptr, *dp, *dn;
+  if ((rc = io.h2d(mark, sizeof(int32_t) * (size_t)nstreams * mark_stride, &dm))) return rc;
+  if ((rc = io.h2d(pcm_len, sizeof(int64_t) * nstreams, &dl))) return rc;
+  if (eof && (rc = io.h2d(eof, sizeof(int64_t) * nstreams, &de))) return rc;
+  if ((rc = io.h2d(nullptr, sizeof(vb200_stream_block) * cap, &dp))) return rc;
+  if ((rc = io.h2d(nullptr, sizeof(int32_t) * nstreams, &dn))) return rc;
+  int32_t *d_tot, *d_work; int2 *d_src[2]; vb200_block_desc *d_desc[2];
+  if ((rc = carve(c->plan, [&](Carve &k) {
+         d_tot = k.take<int32_t>(2); d_work = k.take<int32_t>(4 * (size_t)nstreams);
+         for (int w = 0; w < 2; w++) { d_src[w] = k.take<int2>(cap); d_desc[w] = k.take<vb200_block_desc>(cap); }
+       }))) return rc;
   const int caps[2] = {(int)cap, (int)cap};
-  if ((rc = plan_launch(c, nstreams, d_mark, mark_stride, nsteps, d_len, eof ? d_eof : nullptr, max_blocks, d_plan, d_nb,
-                        caps, d_src, d_desc, d_tot, st))) return rc;
-  CU(cudaMemcpyAsync(plan, d_plan, sizeof(vb200_stream_block) * cap, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(nblocks, d_nb, sizeof(int32_t) * nstreams, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  return 0;
+  if ((rc = scratch_begin(c, st))) return rc;
+  if ((rc = plan_launch(c, nstreams, (const int32_t *)dm, mark_stride, nsteps, (const int64_t *)dl, (const int64_t *)de,
+                        max_blocks, (vb200_stream_block *)dp, (int32_t *)dn, caps, d_src, d_desc, d_tot, d_work, st)))
+    return rc;
+  if ((rc = scratch_end(c, st))) return rc;
+  if ((rc = io.d2h(plan, dp, sizeof(vb200_stream_block) * cap))) return rc;
+  if ((rc = io.d2h(nblocks, dn, sizeof(int32_t) * nstreams))) return rc;
+  return io.sync();
 }
 
 // arguments of both streams calls; zeroes count[] (nstreams <= 0: nothing to do)
@@ -2307,27 +2316,28 @@ static int streams_check(vb200_ctx *c, int nstreams, vb200_streams_io *d) {
 
 // The front half of both streams calls, up to the psy stage: envelope search, marks, plan, the transforms of
 // both sizes and the ampmax chain along every stream.  Sets count[]; for each size with blocks, S[w] holds the
-// transforms, a[w] the psy stage's io and d_desc[w] the batch's block descriptors.
+// transforms, a[w] the psy stage's io, d_desc[w] the batch's block descriptors and, given M, M[w] the scratch of
+// the managed tail.  Begins the call's use of the context scratch.
 static int streams_front(vb200_ctx *c, int nstreams, vb200_streams_io *d, cudaStream_t st, EncScratch S[2],
-                         vb200_phaseA_io a[2], vb200_block_desc *d_desc[2]) {
+                         vb200_phaseA_io a[2], vb200_block_desc *d_desc[2], MgdScratch *M = nullptr) {
   int rc;
   const int ch = c->setup.channels;
   // 1. envelope search over the whole timeline (fresh detector state), 2. marks, 3. plan
   const int nsteps = (int)(d->stream_stride / PLAN_STEP) - PLAN_VE_WIN;
   if (nsteps < 1) return fail(VB200_EINVAL, "stream too short");
   const int64_t mark_stride = nsteps + 4;
-  void *p;
   const size_t sw = VB200_VE_STATE_WORDS(ch);
-  if ((rc = ensure_buf(c->str_buf[10], sizeof(int32_t) * sw * nstreams, &p))) return rc; int32_t *d_state = (int32_t *)p;
-  if ((rc = ensure_buf(c->str_buf[11], (size_t)nstreams * nsteps, &p))) return rc; uint8_t *d_ret = (uint8_t *)p;
-  if ((rc = ensure_buf(c->str_buf[2], sizeof(int32_t) * (size_t)nstreams * mark_stride, &p))) return rc; int32_t *d_mark = (int32_t *)p;
-  if ((rc = ensure_buf(c->str_buf[5], sizeof(int32_t) * 2, &p))) return rc; int32_t *d_tot = (int32_t *)p;
-  int2 *d_src[2];
-  for (int w = 0; w < 2; w++) {
-    const size_t cw = d->cap[w] > 0 ? d->cap[w] : 1;
-    if ((rc = ensure_buf(c->str_buf[6 + w], sizeof(int2) * cw, &p))) return rc; d_src[w] = (int2 *)p;
-    if ((rc = ensure_buf(c->str_buf[8 + w], sizeof(vb200_block_desc) * cw, &p))) return rc; d_desc[w] = (vb200_block_desc *)p;
-  }
+  int32_t *d_state, *d_mark, *d_tot, *d_work; uint8_t *d_ret; int2 *d_src[2];
+  if ((rc = carve(c->plan, [&](Carve &k) {
+         d_state = k.take<int32_t>(sw * nstreams); d_ret = k.take<uint8_t>((size_t)nstreams * nsteps);
+         d_mark = k.take<int32_t>((size_t)nstreams * mark_stride); d_tot = k.take<int32_t>(2);
+         d_work = k.take<int32_t>(4 * (size_t)nstreams);
+         for (int w = 0; w < 2; w++) {
+           const size_t cw = d->cap[w] > 0 ? d->cap[w] : 1;
+           d_src[w] = k.take<int2>(cw); d_desc[w] = k.take<vb200_block_desc>(cw);
+         }
+       }))) return rc;
+  if ((rc = scratch_begin(c, st))) return rc;
   CU(cudaMemsetAsync(d_state, 0, sizeof(int32_t) * sw * nstreams, st));
   if ((rc = vb200_envelope_search_dev(c, nstreams, d->pcm, d->pcm_fmt, d->stream_stride, 0, nsteps, d_state, d_ret, st))) return rc;
   {
@@ -2336,18 +2346,25 @@ static int streams_front(vb200_ctx *c, int nstreams, vb200_streams_io *d, cudaSt
     if ((rc = post_launch(c))) return rc;
   }
   if ((rc = plan_launch(c, nstreams, d_mark, mark_stride, nsteps, d->pcm_len, d->eof, d->max_blocks, d->plan, d->nblocks,
-                        d->cap, d_src, d_desc, d_tot, st))) return rc;
+                        d->cap, d_src, d_desc, d_tot, d_work, st))) return rc;
   int tot[2];
   CU(cudaMemcpyAsync(tot, d_tot, sizeof(tot), cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));                       // the launches below are sized by the plan
   d->count[0] = tot[0]; d->count[1] = tot[1];
   if (tot[0] > d->cap[0] || tot[1] > d->cap[1]) return fail(VB200_EINVAL, "encode_streams: more blocks than cap[] (count[] holds the need)");
   // 4. transforms of both sizes, 5. the ampmax chain along every stream
+  if ((rc = carve(c->chain, [&](Carve &k) {
+         for (int w = 0; w < 2; w++) {
+           const size_t n = c->dx[w].N / 2, nb = tot[w];
+           if (!nb) continue;
+           enc_layout(k, nb * ch, nb, n, nullptr, false, &S[w]);
+           if (M) mgd_layout(k, nb * ch, (size_t)d->cap[w] * ch, n, &M[w]);
+         }
+       }))) return rc;
   for (int w = 0; w < 2; w++) {
     memset(&a[w], 0, sizeof(a[w]));
     if (!tot[w]) continue;
-    const size_t n = c->dx[w].N / 2, nb = tot[w];
-    if ((rc = enc_scratch(c->str_buf + 12 + 8 * w, nb * ch, nb, n, nullptr, false, &S[w]))) return rc;
+    const size_t nb = tot[w];
     a[w].desc = d_desc[w]; a[w].mdct = S[w].mdct; a[w].logmdct = S[w].logmdct; a[w].logmask = S[w].logmask;
     a[w].ampmax_out = d->ampmax_out[w];
     PcmSrc ps; ps.base = d->pcm; ps.fmt = d->pcm_fmt; ps.bps = 1; ps.hop = 0; ps.stride = d->stream_stride; ps.blk_src = d_src[w];
@@ -2395,19 +2412,17 @@ extern "C" int vb200_encode_streams_managed_dev(vb200_ctx *c, int nstreams, vb20
   int rc;
   if ((rc = streams_check(c, nstreams, d)) || nstreams <= 0) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  const int ch = c->setup.channels;
   EncScratch S[2];
   vb200_phaseA_io a[2];
   vb200_block_desc *d_desc[2];
-  if ((rc = streams_front(c, nstreams, d, st, S, a, d_desc))) return rc;
+  MgdScratch M[2];
+  if ((rc = streams_front(c, nstreams, d, st, S, a, d_desc, M))) return rc;
   for (int w = 0; w < 2; w++) {
     if (!d->count[w]) continue;
     const int nb = d->count[w];
-    MgdScratch M;
-    if ((rc = mgd_scratch(c->str_buf + 40 + 5 * w, (size_t)nb * ch, (size_t)d->cap[w] * ch, c->dx[w].N / 2, &M))) return rc;
-    a[w].tap_noise = M.noise; a[w].tap_tone = M.tone;
+    a[w].tap_noise = M[w].noise; a[w].tap_tone = M[w].tone;
     if ((rc = phaseA_psy_launch(c, w, nb, &a[w], st, S[w].logfft, S[w].lmax, S[w].gmax))) return rc;
-    if ((rc = managed_tail(c, w, nb, d->cap[w], d_desc[w], S[w].mdct, S[w].logmdct, S[w].logmask, M, d->posts[w],
+    if ((rc = managed_tail(c, w, nb, d->cap[w], d_desc[w], S[w].mdct, S[w].logmdct, S[w].logmask, M[w], d->posts[w],
                            d->nonzero[w], d->iwork[w], st))) return rc;
   }
   return scratch_end(c, st);
@@ -2428,24 +2443,22 @@ static int streams_host(vb200_ctx *c, int nstreams, int blobno, int curves, vb20
   const size_t ch = c->setup.channels;
   const size_t pcm_bytes = (size_t)nstreams * ch * (size_t)h->stream_stride * (h->pcm_fmt == VB200_PCM_S16_INTERLEAVED ? 2 : 4);
   const size_t pcap = (size_t)nstreams * h->max_blocks;
+  HostIO io{c};
   void *p;
   vb200_streams_io d = *h;
-  if ((rc = ensure_buf(c->str_buf[28], pcm_bytes, &p))) return rc; d.pcm = p;
-  if ((rc = ensure_buf(c->str_buf[3], sizeof(int64_t) * 2 * (size_t)nstreams, &p))) return rc;
-  d.pcm_len = (int64_t *)p; d.eof = h->eof ? (int64_t *)p + nstreams : nullptr;
-  if ((rc = ensure_buf(c->str_buf[4], sizeof(vb200_stream_block) * pcap, &p))) return rc; d.plan = (vb200_stream_block *)p;
-  if ((rc = ensure_buf(c->str_buf[29], sizeof(int32_t) * nstreams, &p))) return rc; d.nblocks = (int32_t *)p;
+  if ((rc = io.h2d(h->pcm, pcm_bytes, &p))) return rc; d.pcm = p;
+  if ((rc = io.h2d(h->pcm_len, sizeof(int64_t) * nstreams, &p))) return rc; d.pcm_len = (const int64_t *)p;
+  if (h->eof) { if ((rc = io.h2d(h->eof, sizeof(int64_t) * nstreams, &p))) return rc; d.eof = (const int64_t *)p; }
+  if ((rc = io.h2d(nullptr, sizeof(vb200_stream_block) * pcap, &p))) return rc; d.plan = (vb200_stream_block *)p;
+  if ((rc = io.h2d(nullptr, sizeof(int32_t) * nstreams, &p))) return rc; d.nblocks = (int32_t *)p;
   for (int w = 0; w < 2; w++) {
     const size_t cw = h->cap[w] > 0 ? h->cap[w] : 0, n = c->dx[w].N / 2;
     if (!cw) continue;
-    if ((rc = ensure_buf(c->str_buf[30 + 4 * w], sizeof(int32_t) * curves * cw * ch * VB200_FLOOR1_STRIDE, &p))) return rc; d.posts[w] = (int32_t *)p;
-    if ((rc = ensure_buf(c->str_buf[31 + 4 * w], sizeof(int32_t) * curves * cw * ch, &p))) return rc; d.nonzero[w] = (int32_t *)p;
-    if ((rc = ensure_buf(c->str_buf[32 + 4 * w], sizeof(int32_t) * curves * cw * ch * n, &p))) return rc; d.iwork[w] = (int32_t *)p;
-    if ((rc = ensure_buf(c->str_buf[33 + 4 * w], sizeof(float) * cw, &p))) return rc; d.ampmax_out[w] = (float *)p;
+    if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * cw * ch * VB200_FLOOR1_STRIDE, &p))) return rc; d.posts[w] = (int32_t *)p;
+    if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * cw * ch, &p))) return rc; d.nonzero[w] = (int32_t *)p;
+    if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * cw * ch * n, &p))) return rc; d.iwork[w] = (int32_t *)p;
+    if ((rc = io.h2d(nullptr, sizeof(float) * cw, &p))) return rc; d.ampmax_out[w] = (float *)p;
   }
-  CU(cudaMemcpyAsync((void *)d.pcm, h->pcm, pcm_bytes, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync((void *)d.pcm_len, h->pcm_len, sizeof(int64_t) * nstreams, cudaMemcpyHostToDevice, st));
-  if (h->eof) CU(cudaMemcpyAsync((void *)d.eof, h->eof, sizeof(int64_t) * nstreams, cudaMemcpyHostToDevice, st));
   rc = curves == 1 ? vb200_encode_streams_dev(c, nstreams, blobno, &d, st) : vb200_encode_streams_managed_dev(c, nstreams, &d, st);
   h->count[0] = d.count[0]; h->count[1] = d.count[1];
   if (rc) return rc;
@@ -3253,16 +3266,18 @@ static int encode_entropy_launch(vb200_ctx *c, int W, int nblocks, const vb200_b
   const int ch = c->setup.channels, n = c->dx[W].N / 2, stride = c->res_partvals[W] > 0 ? c->res_partvals[W] : 1;
   const int curves = managed ? VB200_PACKETBLOBS : 1;
   const int grid = grid_for(c, curves * nblocks, 8);
-  void *cls, *work;
+  int32_t *cls, *work;
   int rc;
-  if ((rc = ensure_buf(c->eent_buf[0], sizeof(int32_t) * curves * (size_t)nblocks * ch * stride, &cls))) return rc;
-  if ((rc = ensure_buf(c->eent_buf[1], sizeof(int32_t) * (size_t)grid * ch * n, &work))) return rc;
-  if ((rc = residue_classify_launch(c, W, nblocks, curves, blob_blocks * ch, d_iwork, d_nonzero, (int32_t *)cls, stride,
-                                    st))) return rc;
+  if ((rc = carve(c->coder, [&](Carve &k) {
+         cls = k.take<int32_t>((size_t)curves * nblocks * ch * stride);
+         work = k.take<int32_t>((size_t)grid * ch * n);
+       }))) return rc;
+  if ((rc = residue_classify_launch(c, W, nblocks, curves, blob_blocks * ch, d_iwork, d_nonzero, cls, stride, st)))
+    return rc;
   EncArgs A;
   A.E = c->eent; A.f1 = c->d_floor[W]; A.chmux = c->d_chmux[W]; A.desc = d_desc;
-  A.posts = d_posts; A.nonzero = d_nonzero; A.iwork = d_iwork; A.classes = (const int *)cls;
-  A.curve_rows = blob_blocks * ch; A.work = (int *)work; A.W = W; A.nblocks = nblocks; A.n = n; A.class_stride = stride;
+  A.posts = d_posts; A.nonzero = d_nonzero; A.iwork = d_iwork; A.classes = cls;
+  A.curve_rows = blob_blocks * ch; A.work = work; A.W = W; A.nblocks = nblocks; A.n = n; A.class_stride = stride;
   A.pkt_stride = pkt_stride; A.pkt_bits = d_bits; A.data = d_data;
   const size_t smem = sizeof(int) * (size_t)c->eent.slots[W];
   if (managed) {
@@ -3301,14 +3316,16 @@ extern "C" int vb200_encode_entropy_dev(vb200_ctx *c, int W, int nblocks, const 
 // back (the bytes only when they fit data_cap).  Synchronises.
 static int packets_pack_d2h(vb200_ctx *c, int nblocks, const uint8_t *d_strided, int64_t stride, const int32_t *d_bits,
                             int64_t *pkt_off, int32_t *pkt_bits, uint8_t *data, int64_t data_cap, cudaStream_t st) {
-  void *doff, *dpk;
+  long long *doff;
+  uint8_t *dpk;
   int rc;
-  if ((rc = ensure_buf(c->eent_buf[2], sizeof(int64_t) * ((size_t)nblocks + 1), &doff))) return rc;
-  if ((rc = ensure_buf(c->eent_buf[3], (size_t)std::max<int64_t>(data_cap, 1), &dpk))) return rc;
-  k_packet_offsets<<<1, 1024, 0, st>>>(d_bits, nblocks, (long long *)doff);
+  if ((rc = carve(c->pack, [&](Carve &k) {
+         doff = k.take<long long>((size_t)nblocks + 1);
+         dpk = k.take<uint8_t>((size_t)std::max<int64_t>(data_cap, 1));
+       }))) return rc;
+  k_packet_offsets<<<1, 1024, 0, st>>>(d_bits, nblocks, doff);
   if ((rc = post_launch(c))) return rc;
-  k_packet_gather<<<grid_for(c, nblocks, 8), 256, 0, st>>>(d_strided, stride, d_bits, (const long long *)doff, nblocks,
-                                                           data_cap, (uint8_t *)dpk);
+  k_packet_gather<<<grid_for(c, nblocks, 8), 256, 0, st>>>(d_strided, stride, d_bits, doff, nblocks, data_cap, dpk);
   if ((rc = post_launch(c))) return rc;
   int64_t total = 0;
   CU(cudaMemcpyAsync(pkt_bits, d_bits, sizeof(int32_t) * nblocks, cudaMemcpyDeviceToHost, st));
@@ -3366,32 +3383,21 @@ extern "C" int vb200_encode_packets(vb200_ctx *c, int W, int nstreams, int bps, 
   const size_t nb = (size_t)nstreams * bps, rows = nb * ch;
   const int64_t stride = c->eent.bound[W];
   cudaStream_t st = c->s_main;
-  DevBuf *B = c->eent_buf + 4;
-  void *p;
-  const size_t pcm_bytes = enc_pcm_bytes(h, ch, N, nstreams, bps);
-  if ((rc = ensure_buf(B[0], pcm_bytes, &p))) return rc; d.pcm = p;
-  if ((rc = ensure_buf(B[1], sizeof(vb200_block_desc) * nb, &p))) return rc; d.desc = (const vb200_block_desc *)p;
-  if ((rc = ensure_buf(B[2], sizeof(float) * nstreams, &p))) return rc; d.ampmax0 = h->ampmax0 ? (const float *)p : nullptr;
-  if ((rc = ensure_buf(B[3], sizeof(int32_t) * rows * VB200_FLOOR1_STRIDE, &p))) return rc; d.posts = (int32_t *)p;
-  if ((rc = ensure_buf(B[4], sizeof(int32_t) * rows, &p))) return rc; d.nonzero = (int32_t *)p;
-  if ((rc = ensure_buf(B[5], sizeof(int32_t) * rows * n, &p))) return rc; d.iwork = p;
-  if ((rc = ensure_buf(B[6], sizeof(float) * nb, &p))) return rc; d.ampmax_out = (float *)p;
-  if ((rc = ensure_buf(B[7], sizeof(int32_t) * nb, &p))) return rc;
-  int32_t *dbits = (int32_t *)p;
-  if ((rc = ensure_buf(B[8], (size_t)stride * nb, &p))) return rc;
-  uint8_t *dstr = (uint8_t *)p;
+  HostIO io{c};
+  void *dbits, *dstr;
+  if ((rc = enc_stage(io, h, &d, ch, N, nstreams, bps, 1))) return rc;
+  if ((rc = io.h2d(nullptr, sizeof(int32_t) * nb, &dbits))) return rc;
+  if ((rc = io.h2d(nullptr, (size_t)stride * nb, &dstr))) return rc;
   EncScratch S;
-  if ((rc = enc_scratch(B + 9, rows, nb, n, nullptr, false, &S))) return rc;
-  CU(cudaMemcpyAsync((void *)d.pcm, h->pcm, pcm_bytes, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync((void *)d.desc, h->desc, sizeof(vb200_block_desc) * nb, cudaMemcpyHostToDevice, st));
-  if (h->ampmax0) CU(cudaMemcpyAsync((void *)d.ampmax0, h->ampmax0, sizeof(float) * nstreams, cudaMemcpyHostToDevice, st));
+  if ((rc = carve(c->enc, [&](Carve &k) { enc_layout(k, rows, nb, n, nullptr, false, &S); }))) return rc;
   if ((rc = scratch_begin(c, st))) return rc;
   if ((rc = encode_launch(c, W, nstreams, bps, blobno, &d, S, st))) return rc;
-  if ((rc = encode_entropy_launch(c, W, (int)nb, d.desc, d.posts, d.nonzero, (const int32_t *)d.iwork, stride, dbits,
-                                  dstr, st))) return rc;
+  if ((rc = encode_entropy_launch(c, W, (int)nb, d.desc, d.posts, d.nonzero, (const int32_t *)d.iwork, stride,
+                                  (int32_t *)dbits, (uint8_t *)dstr, st))) return rc;
   if ((rc = scratch_end(c, st))) return rc;
-  CU(cudaMemcpyAsync(h->ampmax_out, d.ampmax_out, sizeof(float) * nb, cudaMemcpyDeviceToHost, st));
-  return packets_pack_d2h(c, (int)nb, dstr, stride, dbits, pkt_off, pkt_bits, data, data_cap, st);
+  if ((rc = io.d2h(h->ampmax_out, d.ampmax_out, sizeof(float) * nb))) return rc;
+  return packets_pack_d2h(c, (int)nb, (const uint8_t *)dstr, stride, (const int32_t *)dbits, pkt_off, pkt_bits, data,
+                          data_cap, st);
 }
 
 // ---- bitrate-managed: all VB200_PACKETBLOBS packets of every block ----
@@ -3430,32 +3436,22 @@ extern "C" int vb200_encode_packets_managed(vb200_ctx *c, int W, int nstreams, i
   if ((int64_t)VB200_PACKETBLOBS * nstreams * bps > INT32_MAX) return fail(VB200_EINVAL, "nblocks");
   std::lock_guard<std::mutex> lk(c->mu);
   constexpr int NB = VB200_PACKETBLOBS;
-  const int ch = c->setup.channels, N = c->dx[W].N, n = N / 2;
-  const size_t nb = (size_t)nstreams * bps, rows = nb * ch;
+  const int ch = c->setup.channels, N = c->dx[W].N;
+  const size_t nb = (size_t)nstreams * bps;
   const int64_t stride = c->eent.bound[W];
   cudaStream_t st = c->s_main;
-  DevBuf *B = c->mgd_buf;                            // the host-call staging of vb200_encode_dsp_managed, and two more
-  void *p;
-  const size_t pcm_bytes = enc_pcm_bytes(h, ch, N, nstreams, bps);
-  if ((rc = ensure_buf(B[12], pcm_bytes, &p))) return rc; d.pcm = p;
-  if ((rc = ensure_buf(B[13], sizeof(vb200_block_desc) * nb, &p))) return rc; d.desc = (const vb200_block_desc *)p;
-  if ((rc = ensure_buf(B[14], sizeof(float) * nstreams, &p))) return rc; d.ampmax0 = h->ampmax0 ? (const float *)p : nullptr;
-  if ((rc = ensure_buf(B[15], sizeof(int32_t) * NB * rows * VB200_FLOOR1_STRIDE, &p))) return rc; d.posts = (int32_t *)p;
-  if ((rc = ensure_buf(B[16], sizeof(int32_t) * NB * rows, &p))) return rc; d.nonzero = (int32_t *)p;
-  if ((rc = ensure_buf(B[17], sizeof(int32_t) * NB * rows * n, &p))) return rc; d.iwork = p;
-  if ((rc = ensure_buf(B[18], sizeof(float) * nb, &p))) return rc; d.ampmax_out = (float *)p;
-  if ((rc = ensure_buf(B[19], sizeof(int32_t) * NB * nb, &p))) return rc;
-  int32_t *dbits = (int32_t *)p;
-  if ((rc = ensure_buf(B[20], (size_t)stride * NB * nb, &p))) return rc;
-  uint8_t *dstr = (uint8_t *)p;
-  CU(cudaMemcpyAsync((void *)d.pcm, h->pcm, pcm_bytes, cudaMemcpyHostToDevice, st));
-  CU(cudaMemcpyAsync((void *)d.desc, h->desc, sizeof(vb200_block_desc) * nb, cudaMemcpyHostToDevice, st));
-  if (h->ampmax0) CU(cudaMemcpyAsync((void *)d.ampmax0, h->ampmax0, sizeof(float) * nstreams, cudaMemcpyHostToDevice, st));
+  HostIO io{c};
+  void *dbits, *dstr;
+  if ((rc = enc_stage(io, h, &d, ch, N, nstreams, bps, NB))) return rc;
+  if ((rc = io.h2d(nullptr, sizeof(int32_t) * NB * nb, &dbits))) return rc;
+  if ((rc = io.h2d(nullptr, (size_t)stride * NB * nb, &dstr))) return rc;
   if ((rc = vb200_encode_dsp_managed_dev(c, W, nstreams, bps, &d, st))) return rc;
   if ((rc = vb200_encode_entropy_managed_dev(c, W, (int)nb, (int64_t)nb, d.desc, d.posts, d.nonzero,
-                                             (const int32_t *)d.iwork, stride, dbits, dstr, st))) return rc;
-  CU(cudaMemcpyAsync(h->ampmax_out, d.ampmax_out, sizeof(float) * nb, cudaMemcpyDeviceToHost, st));
-  return packets_pack_d2h(c, NB * (int)nb, dstr, stride, dbits, pkt_off, pkt_bits, data, data_cap, st);
+                                             (const int32_t *)d.iwork, stride, (int32_t *)dbits, (uint8_t *)dstr, st)))
+    return rc;
+  if ((rc = io.d2h(h->ampmax_out, d.ampmax_out, sizeof(float) * nb))) return rc;
+  return packets_pack_d2h(c, NB * (int)nb, (const uint8_t *)dstr, stride, (const int32_t *)dbits, pkt_off, pkt_bits,
+                          data, data_cap, st);
 }
 
 // ======================================================================== //
@@ -3485,19 +3481,21 @@ static int envelope_search_launch(vb200_ctx *c, int nstreams, const void *d_pcm,
   int chunk = (int)((1L << 22) / per_step);
   if (chunk < 1) chunk = 1;
   if (chunk > nsteps) chunk = nsteps;
-  void *p_t, *p_v;
-  if ((rc = ensure_buf(c->env_buf[0], sizeof(float) * (size_t)per_step * chunk, &p_t))) return rc;
-  if ((rc = ensure_buf(c->env_buf[1], sizeof(float) * (size_t)per_step * chunk * 32, &p_v))) return rc;
+  float *p_t, *p_v;
+  if ((rc = carve(c->env_scratch, [&](Carve &k) {
+         p_t = k.take<float>((size_t)per_step * chunk);
+         p_v = k.take<float>((size_t)per_step * chunk * 32);
+       }))) return rc;
   EnvSrc src; src.base = d_pcm; src.fmt = fmt; src.stride = stride; src.ch = ch;
   if ((rc = scratch_begin(c, st))) return rc;
   for (int j0 = 0; j0 < nsteps; j0 += chunk) {
     const int ns = nsteps - j0 < chunk ? nsteps - j0 : chunk;
     const long items = per_step * ns;
     const int grid = grid_for(c, (int)((items + ENV_WARPS - 1) / ENV_WARPS), 16);
-    k_env_spectrum<<<grid, 32 * ENV_WARPS, 0, st>>>(c->env, src, nstreams, first_step + j0, ns, (float *)p_t, (float *)p_v);
+    k_env_spectrum<<<grid, 32 * ENV_WARPS, 0, st>>>(c->env, src, nstreams, first_step + j0, ns, p_t, p_v);
     if ((rc = post_launch(c))) return rc;
     k_env_filter<<<(nstreams + ENV_WARPS - 1) / ENV_WARPS, 32 * ENV_WARPS, 0, st>>>(
-        c->env, nstreams, ch, ns, nsteps, j0, (const float *)p_t, (const float *)p_v, d_state, d_ret, d_steps_per_stream);
+        c->env, nstreams, ch, ns, nsteps, j0, p_t, p_v, d_state, d_ret, d_steps_per_stream);
     if ((rc = post_launch(c))) return rc;
   }
   return scratch_end(c, st);
@@ -3518,22 +3516,17 @@ static int envelope_search_host(vb200_ctx *c, int nstreams, const void *pcm, int
   const int ch = c->setup.channels;
   const size_t pcm_bytes = (fmt == VB200_PCM_S16_INTERLEAVED ? sizeof(int16_t) : sizeof(float)) * (size_t)nstreams * ch * (size_t)stride;
   const size_t st_bytes = sizeof(int32_t) * (size_t)nstreams * VB200_VE_STATE_WORDS(ch);
-  void *dp, *ds, *dr;
-  if ((rc = ensure_buf(c->env_buf[2], pcm_bytes, &dp))) return rc;
-  if ((rc = ensure_buf(c->env_buf[3], st_bytes + (size_t)nstreams * nsteps + sizeof(int32_t) * (size_t)nstreams + 16, &ds))) return rc;
-  dr = (char *)ds + st_bytes;
-  int32_t *dn = nullptr;
-  if (steps_per_stream) {
-    dn = (int32_t *)((char *)dr + (((size_t)nstreams * nsteps + 15) & ~(size_t)15));
-    CU(cudaMemcpyAsync(dn, steps_per_stream, sizeof(int32_t) * (size_t)nstreams, cudaMemcpyHostToDevice, c->s_main));
-  }
-  CU(cudaMemcpyAsync(dp, pcm, pcm_bytes, cudaMemcpyHostToDevice, c->s_main));
-  CU(cudaMemcpyAsync(ds, state, st_bytes, cudaMemcpyHostToDevice, c->s_main));
-  if ((rc = envelope_search_launch(c, nstreams, dp, fmt, stride, first_step, nsteps, (int32_t *)ds, (uint8_t *)dr, c->s_main, dn))) return rc;
-  CU(cudaMemcpyAsync(state, ds, st_bytes, cudaMemcpyDeviceToHost, c->s_main));
-  CU(cudaMemcpyAsync(ret, dr, (size_t)nstreams * nsteps, cudaMemcpyDeviceToHost, c->s_main));
-  CU(cudaStreamSynchronize(c->s_main));
-  return 0;
+  HostIO io{c};
+  void *dn = nullptr, *dp, *ds, *dr;
+  if (steps_per_stream && (rc = io.h2d(steps_per_stream, sizeof(int32_t) * (size_t)nstreams, &dn))) return rc;
+  if ((rc = io.h2d(pcm, pcm_bytes, &dp))) return rc;
+  if ((rc = io.h2d(state, st_bytes, &ds))) return rc;
+  if ((rc = io.h2d(nullptr, (size_t)nstreams * nsteps, &dr))) return rc;
+  if ((rc = envelope_search_launch(c, nstreams, dp, fmt, stride, first_step, nsteps, (int32_t *)ds, (uint8_t *)dr,
+                                   c->s_main, (const int32_t *)dn))) return rc;
+  if ((rc = io.d2h(state, ds, st_bytes))) return rc;
+  if ((rc = io.d2h(ret, dr, (size_t)nstreams * nsteps))) return rc;
+  return io.sync();
 }
 
 extern "C" int vb200_envelope_search(vb200_ctx *c, int nstreams, const void *pcm, int fmt, int64_t stride,
