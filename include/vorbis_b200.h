@@ -763,6 +763,83 @@ int vb200_encode_entropy_managed_dev(vb200_ctx*, int W, int nblocks, int64_t blo
 int vb200_encode_packets_managed(vb200_ctx*, int W, int nstreams, int blocks_per_stream, const vb200_encode_io *io,
                                  int64_t *pkt_off, int32_t *pkt_bits, uint8_t *data, int64_t data_cap);
 
+/* ---- the bitrate manager on the device: vorbis_bitrate_addblock (lib/bitrate.c:73-227), replayed exactly.
+ * vb200_bitrate_info is bitrate_manager_info (lib/bitrate.h:41-50), what a binding reads from ci->bi.
+ * vb200_bitrate_setup registers it on the context, which derives what vorbis_bitrate_init derives
+ * (lib/bitrate.c:28-56) from it, the context's rate and its block sizes: avg/min/max_bitsper, short_per_long and
+ * desired_fill.  reservoir_bits <= 0 is the un-managed case: the setup is kept, and every call below that manages
+ * the rate returns VB200_EINVAL for it.  Replaces an earlier registration.                                      */
+typedef struct vb200_bitrate_info {
+  int64_t avg_rate;                /* bits/s; <= 0: no average target */
+  int64_t min_rate;
+  int64_t max_rate;
+  int64_t reservoir_bits;
+  double  reservoir_bias;
+  double  slew_damp;
+} vb200_bitrate_info;
+/* The part of bitrate_manager_state (lib/bitrate.h:25-39) that changes from block to block. */
+typedef struct vb200_bitrate_state {
+  int64_t avg_reservoir;
+  int64_t minmax_reservoir;
+  double  avgfloat;
+  int32_t choice;                  /* the last block's choice */
+  int32_t pad;
+} vb200_bitrate_state;
+int vb200_bitrate_setup(vb200_ctx*, const vb200_bitrate_info*);
+/* plain host code: the state vorbis_bitrate_init leaves (both reservoirs at desired_fill, avgfloat 7, choice 0) */
+int vb200_bitrate_init(vb200_ctx*, vb200_bitrate_state *state);
+/* The choice for count[s] blocks of each of nstreams streams, in stream order, one thread per stream:
+ *   W        [nstreams][max_blocks]                      block-size flag of each block
+ *   pkt_bits [nstreams][max_blocks][VB200_PACKETBLOBS]   the 15 packets' lengths in bits as the coder reports them
+ *                                                        (rounded up to whole bytes, as oggpack_bytes does)
+ *   state    [nstreams]                                  read and written in place
+ *   choice   [nstreams][max_blocks]  the packet kept (bm->choice); bytes [nstreams][max_blocks] its final length:
+ *            cut to maxsize bytes when even packet 0 is too large, padded with zero bytes up to minsize when the
+ *            minimum demands it.
+ * Entries past count[s] are neither read nor written.  Contract: cutting a stream's blocks into any sequence of
+ * calls that carry the state along gives the result of one call.  One kernel launch.  VB200_EINVAL without a
+ * managed vb200_bitrate_setup, for a null pointer, max_blocks < 1 or (host form) count[s] outside [0, max_blocks]. */
+int vb200_bitrate_addblocks_dev(vb200_ctx*, int nstreams, int max_blocks, const int32_t *d_count, const int32_t *d_W,
+                                const int32_t *d_pkt_bits, vb200_bitrate_state *d_state, int32_t *d_choice,
+                                int32_t *d_bytes, void *stream);
+int vb200_bitrate_addblocks    (vb200_ctx*, int nstreams, int max_blocks, const int32_t *count, const int32_t *W,
+                                const int32_t *pkt_bits, vb200_bitrate_state *state, int32_t *choice, int32_t *bytes);
+
+/* ---- whole streams to packets: what the vorbis_analysis_blockout -> vorbis_analysis -> vorbis_bitrate_addblock ->
+ * vorbis_bitrate_flushpacket loop of a stock encoder hands its caller, for many fresh streams in one call.
+ * vb200_encode_streams[_managed]_dev, vb200_encode_entropy[_managed]_dev per block size, then on the device: the
+ * per-size bit counts moved into stream order through the plan, (managed) the chooser along every stream from
+ * vorbis_bitrate_init's state, an offset scan over the final lengths and a gather of each kept packet from its
+ * strided slot.  Only the plan, nblocks, info and the packed bytes are copied back.
+ *   io    as for vb200_encode_streams, host buffers, with posts, nonzero, iwork and ampmax_out NULL (they stay in
+ *         device scratch); plan, nblocks and count[] are returned as there
+ *   info  [nstreams][max_blocks]: packet k of stream s is data[offset .. offset+bytes), streams back to back in
+ *         stream order; e_o_s, granulepos and packetno as vorbis_bitrate_flushpacket sets them (lib/bitrate.c:
+ *         229-252) from vorbis_analysis_blockout (lib/block.c:311, 618-619, 645-687): packetno = 3 + k, granulepos =
+ *         the block's centre on the timeline minus blocksizes[1]/2, clipped at eof, e_o_s on the block whose centre
+ *         reaches eof (never where eof is 0 or NULL); choice = the packet kept (VB200_PACKETBLOBS/2 un-managed).
+ *         Entries past nblocks[s] are zero but for offset.
+ * When the packets do not fit data_cap bytes: VB200_EINVAL with info filled (as vb200_encode_packets).  VB200_EINVAL
+ * also without a registered vb200_encode_entropy_setup, (managed) without a managed vb200_bitrate_setup, and for null
+ * pointers.  Launches: those of the streams call, two per block size with blocks, then three (un-managed) or four.
+ * Device scratch of this call family, besides the staging of the streams call's io (posts, nonzero, iwork of cap[W]
+ * blocks, times VB200_PACKETBLOBS managed): per block size, curves x count[W] x (vb200_encode_packet_bound(W) + 4)
+ * bytes of strided packets and bit counts (curves = 1, or VB200_PACKETBLOBS managed), which dominates; then per
+ * (stream, block) 4 x (curves + 3) + 8 + sizeof(vb200_packet_info) bytes, and data_cap bytes for the packed output.
+ * Callers size their calls by that; nothing is cut into chunks.                                                  */
+typedef struct vb200_packet_info {
+  int64_t offset;
+  int64_t granulepos;
+  int32_t bytes;
+  int32_t e_o_s;
+  int32_t packetno;
+  int32_t choice;
+} vb200_packet_info;
+int vb200_encode_streams_packets        (vb200_ctx*, int nstreams, int blobno, vb200_streams_io *io,
+                                         vb200_packet_info *info, uint8_t *data, int64_t data_cap);
+int vb200_encode_streams_packets_managed(vb200_ctx*, int nstreams, vb200_streams_io *io,
+                                         vb200_packet_info *info, uint8_t *data, int64_t data_cap);
+
 /* ---- device memory helpers for non-CUDA hosts (C callers) -------------- */
 int  vb200_malloc_device(vb200_ctx*, size_t bytes, void **dptr);
 int  vb200_free_device  (vb200_ctx*, void *dptr);

@@ -185,6 +185,25 @@ class StreamsIO(C.Structure):
     ]
 
 
+class BitrateInfo(C.Structure):
+    """vb200_bitrate_info (include/vorbis_b200.h): bitrate_manager_info, lib/bitrate.h:41-50"""
+    _fields_ = [
+        ("avg_rate", C.c_int64),
+        ("min_rate", C.c_int64),
+        ("max_rate", C.c_int64),
+        ("reservoir_bits", C.c_int64),
+        ("reservoir_bias", C.c_double),
+        ("slew_damp", C.c_double),
+    ]
+
+
+BITRATE_STATE_DTYPE = np.dtype([("avg_reservoir", "<i8"), ("minmax_reservoir", "<i8"), ("avgfloat", "<f8"),
+                                ("choice", "<i4"), ("pad", "<i4")])           # vb200_bitrate_state
+PACKET_INFO_DTYPE = np.dtype([("offset", "<i8"), ("granulepos", "<i8"), ("bytes", "<i4"), ("e_o_s", "<i4"),
+                              ("packetno", "<i4"), ("choice", "<i4")])         # vb200_packet_info
+assert C.sizeof(BitrateInfo) == 48 and BITRATE_STATE_DTYPE.itemsize == 32 and PACKET_INFO_DTYPE.itemsize == 32
+
+
 class Codebook(C.Structure):
     """vb200_codebook (include/vorbis_b200.h)"""
     _fields_ = [

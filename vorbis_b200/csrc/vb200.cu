@@ -25,6 +25,7 @@
 #include "vb200_streams.cuh"
 #include "vb200_managed.cuh"
 #include "vb200_entropy_enc.cuh"
+#include "vb200_bitrate.cuh"
 #include "floor1_db_table.h"
 
 using namespace vb200;
@@ -93,7 +94,11 @@ struct vb200_ctx {
   //   env_scratch  vb200_envelope_search[_dev] (c->env holds the detector's tables)
   //   coder     the entropy coder: residue classes and the per-CTA residue copies
   //   pack      the host forms of the entropy coder: packet offsets and the packed bytes
-  DevBuf stage[STAGE_SLOTS], cycles, phaseA, lane[2], enc, set[ENC_SETS], mgd, plan, chain, env_scratch, coder, pack;
+  //   spk       vb200_encode_streams_packets[_managed]: strided packets and bit counts of both sizes, the stream-order
+  //             tables, offsets, packet infos and the packed bytes
+  //   brc       the host form of vb200_bitrate_addblocks
+  DevBuf stage[STAGE_SLOTS], cycles, phaseA, lane[2], enc, set[ENC_SETS], mgd, plan, chain, env_scratch, coder, pack,
+      spk, brc;
   cudaStream_t s_pipe[2] = {nullptr, nullptr};
   const ResDev *d_res[2] = {nullptr, nullptr};        // [VB200_MAX_SUBMAPS] residue class parameters per block size
   int res_partvals[2] = {0, 0};
@@ -123,6 +128,9 @@ struct vb200_ctx {
   // vb200_encode_entropy_setup: the tables of the entropy coder (eent.books == nullptr: none registered)
   EncEntDev eent{};
   std::vector<void *> eent_owned;
+  // vb200_bitrate_setup: what vorbis_bitrate_init derives (br_set: registered; br_managed: reservoir_bits > 0)
+  bool br_set = false, br_managed = false;
+  BitrateDev br{};
   std::mutex mu;
   // optional per-kernel timing of the last Phase-A call (bench roofline evidence)
   bool profiling = false;
@@ -2381,8 +2389,9 @@ static int streams_front(vb200_ctx *c, int nstreams, vb200_streams_io *d, cudaSt
   return 0;
 }
 
-extern "C" int vb200_encode_streams_dev(vb200_ctx *c, int nstreams, int blobno, vb200_streams_io *d, void *stream) {
-  CHECK_CTX(c);
+// desc_out (optional): the two batches' block descriptors, which stay in the plan arena until its next carve
+static int encode_streams_launch(vb200_ctx *c, int nstreams, int blobno, vb200_streams_io *d, cudaStream_t stream,
+                                 vb200_block_desc **desc_out) {
   int rc;
   if ((rc = streams_check(c, nstreams, d)) || nstreams <= 0) return rc;
   if (blobno < 0 || blobno >= VB200_PACKETBLOBS) return fail(VB200_EINVAL, "blobno");
@@ -2404,11 +2413,17 @@ extern "C" int vb200_encode_streams_dev(vb200_ctx *c, int nstreams, int blobno, 
     if ((rc = cqn_setup(c, w, 1, blobno, &Q1))) return rc;
     if ((rc = cqn_launch(c, Q0, Q1, d_desc[w], nb, S[w].mdct, d->iwork[w], d->nonzero[w], st))) return rc;
   }
+  if (desc_out) { desc_out[0] = d_desc[0]; desc_out[1] = d_desc[1]; }
   return scratch_end(c, st);
 }
 
-extern "C" int vb200_encode_streams_managed_dev(vb200_ctx *c, int nstreams, vb200_streams_io *d, void *stream) {
+extern "C" int vb200_encode_streams_dev(vb200_ctx *c, int nstreams, int blobno, vb200_streams_io *d, void *stream) {
   CHECK_CTX(c);
+  return encode_streams_launch(c, nstreams, blobno, d, (cudaStream_t)stream, nullptr);
+}
+
+static int encode_streams_managed_launch(vb200_ctx *c, int nstreams, vb200_streams_io *d, cudaStream_t stream,
+                                         vb200_block_desc **desc_out) {
   int rc;
   if ((rc = streams_check(c, nstreams, d)) || nstreams <= 0) return rc;
   cudaStream_t st = (cudaStream_t)stream;
@@ -2425,7 +2440,13 @@ extern "C" int vb200_encode_streams_managed_dev(vb200_ctx *c, int nstreams, vb20
     if ((rc = managed_tail(c, w, nb, d->cap[w], d_desc[w], S[w].mdct, S[w].logmdct, S[w].logmask, M[w], d->posts[w],
                            d->nonzero[w], d->iwork[w], st))) return rc;
   }
+  if (desc_out) { desc_out[0] = d_desc[0]; desc_out[1] = d_desc[1]; }
   return scratch_end(c, st);
+}
+
+extern "C" int vb200_encode_streams_managed_dev(vb200_ctx *c, int nstreams, vb200_streams_io *d, void *stream) {
+  CHECK_CTX(c);
+  return encode_streams_managed_launch(c, nstreams, d, (cudaStream_t)stream, nullptr);
 }
 
 // host buffers of both streams calls: one synchronous H2D - compute - D2H round trip.  curves = 1: un-managed
@@ -3452,6 +3473,216 @@ extern "C" int vb200_encode_packets_managed(vb200_ctx *c, int W, int nstreams, i
   if ((rc = io.d2h(h->ampmax_out, d.ampmax_out, sizeof(float) * nb))) return rc;
   return packets_pack_d2h(c, NB * (int)nb, (const uint8_t *)dstr, stride, (const int32_t *)dbits, pkt_off, pkt_bits,
                           data, data_cap, st);
+}
+
+// ======================================================================== //
+// the bitrate manager on the device and whole streams to packets (vb200_bitrate.cuh)
+static_assert(sizeof(vb200_bitrate_info) == 48, "vb200_bitrate_info layout (mirrored by vorbis_b200/abi.py)");
+static_assert(sizeof(vb200_bitrate_state) == 32, "vb200_bitrate_state layout (mirrored by vorbis_b200/abi.py)");
+static_assert(sizeof(vb200_packet_info) == 32, "vb200_packet_info layout (mirrored by vorbis_b200/abi.py)");
+
+extern "C" int vb200_bitrate_setup(vb200_ctx *c, const vb200_bitrate_info *bi) {
+  CHECK_CTX(c);
+  if (!bi) return fail(VB200_EINVAL, "null bitrate info");
+  std::lock_guard<std::mutex> lk(c->mu);
+  BitrateDev B{};
+  const long long rate = c->setup.rate;
+  const int halfsamples = c->setup.blocksizes[0] >> 1;
+  const bool managed = bi->reservoir_bits > 0;
+  if (managed) {                                     // lib/bitrate.c:34-54, in the reference's evaluation order
+    B.short_per_long = c->setup.blocksizes[1] / c->setup.blocksizes[0];
+    B.avg_bitsper = (long long)rint(1. * bi->avg_rate * halfsamples / rate);
+    B.min_bitsper = (long long)rint(1. * bi->min_rate * halfsamples / rate);
+    B.max_bitsper = (long long)rint(1. * bi->max_rate * halfsamples / rate);
+    B.desired_fill = (long long)(bi->reservoir_bits * bi->reservoir_bias);
+    B.reservoir_bits = bi->reservoir_bits;
+    B.slewlimit = 15. / bi->slew_damp;               // lib/bitrate.c:104
+    B.rate = (double)rate;
+    B.samples[0] = c->setup.blocksizes[0] >> 1;
+    B.samples[1] = c->setup.blocksizes[1] >> 1;
+  }
+  c->br = B;
+  c->br_set = true;
+  c->br_managed = managed;
+  return 0;
+}
+
+static int bitrate_check(vb200_ctx *c) {
+  if (!c->br_set || !c->br_managed) return fail(VB200_EINVAL, "no managed vb200_bitrate_setup registered");
+  return 0;
+}
+
+extern "C" int vb200_bitrate_init(vb200_ctx *c, vb200_bitrate_state *state) {
+  if (!c) return fail(VB200_EINVAL, "null context");
+  int rc;
+  if ((rc = bitrate_check(c))) return rc;
+  if (!state) return fail(VB200_EINVAL, "null state");
+  memset(state, 0, sizeof(*state));
+  state->avg_reservoir = state->minmax_reservoir = c->br.desired_fill;
+  state->avgfloat = VB200_PACKETBLOBS / 2;
+  return 0;
+}
+
+extern "C" int vb200_bitrate_addblocks_dev(vb200_ctx *c, int nstreams, int max_blocks, const int32_t *d_count,
+                                           const int32_t *d_W, const int32_t *d_pkt_bits, vb200_bitrate_state *d_state,
+                                           int32_t *d_choice, int32_t *d_bytes, void *stream) {
+  CHECK_CTX(c);
+  int rc;
+  if ((rc = bitrate_check(c))) return rc;
+  if (nstreams <= 0) return 0;
+  if (max_blocks < 1) return fail(VB200_EINVAL, "max_blocks");
+  if (!d_count || !d_W || !d_pkt_bits || !d_state || !d_choice || !d_bytes) return fail(VB200_EINVAL, "bitrate_addblocks pointers");
+  k_bitrate_choose<<<(nstreams + 127) / 128, 128, 0, (cudaStream_t)stream>>>(c->br, nstreams, max_blocks, d_count, d_W,
+                                                                            d_pkt_bits, d_state, d_choice, d_bytes, 1);
+  return post_launch(c);
+}
+
+extern "C" int vb200_bitrate_addblocks(vb200_ctx *c, int nstreams, int max_blocks, const int32_t *count, const int32_t *W,
+                                       const int32_t *pkt_bits, vb200_bitrate_state *state, int32_t *choice,
+                                       int32_t *bytes) {
+  CHECK_CTX(c);
+  int rc;
+  if ((rc = bitrate_check(c))) return rc;
+  if (nstreams <= 0) return 0;
+  if (max_blocks < 1) return fail(VB200_EINVAL, "max_blocks");
+  if (!count || !W || !pkt_bits || !state || !choice || !bytes) return fail(VB200_EINVAL, "bitrate_addblocks pointers");
+  for (int s = 0; s < nstreams; s++)
+    if (count[s] < 0 || count[s] > max_blocks) return fail(VB200_EINVAL, "count[s] outside [0, max_blocks]");
+  std::lock_guard<std::mutex> lk(c->mu);
+  const size_t n = (size_t)nstreams * max_blocks;
+  HostIO io{c};
+  void *dc, *dw, *db, *ds, *dch, *dby;
+  // choice and bytes go in as well: entries past count[s] come back as the caller left them
+  if ((rc = io.h2d(count, sizeof(int32_t) * nstreams, &dc))) return rc;
+  if ((rc = io.h2d(W, sizeof(int32_t) * n, &dw))) return rc;
+  if ((rc = io.h2d(pkt_bits, sizeof(int32_t) * n * VB200_PACKETBLOBS, &db))) return rc;
+  if ((rc = io.h2d(state, sizeof(vb200_bitrate_state) * nstreams, &ds))) return rc;
+  if ((rc = io.h2d(choice, sizeof(int32_t) * n, &dch))) return rc;
+  if ((rc = io.h2d(bytes, sizeof(int32_t) * n, &dby))) return rc;
+  if ((rc = vb200_bitrate_addblocks_dev(c, nstreams, max_blocks, (const int32_t *)dc, (const int32_t *)dw,
+                                        (const int32_t *)db, (vb200_bitrate_state *)ds, (int32_t *)dch, (int32_t *)dby,
+                                        c->s_main))) return rc;
+  if ((rc = io.d2h(state, ds, sizeof(vb200_bitrate_state) * nstreams))) return rc;
+  if ((rc = io.d2h(choice, dch, sizeof(int32_t) * n))) return rc;
+  if ((rc = io.d2h(bytes, dby, sizeof(int32_t) * n))) return rc;
+  return io.sync();
+}
+
+// Both whole-stream packet calls: the streams chain into staged device buffers, the entropy coder per size, then
+// (k_stream_bits, [k_bitrate_choose], k_packet_offsets, k_stream_gather) on the spk arena, carved once when the
+// per-size block counts are known.  One synchronous round trip on s_main.
+static int streams_packets(vb200_ctx *c, int nstreams, int blobno, bool managed, vb200_streams_io *h,
+                           vb200_packet_info *info, uint8_t *data, int64_t data_cap) {
+  int rc;
+  if ((rc = plan_check(c))) return rc;
+  if (!h) return fail(VB200_EINVAL, "null io");
+  h->count[0] = h->count[1] = 0;
+  if (!c->eent.books) return fail(VB200_EINVAL, "no vb200_encode_entropy_setup registered");
+  if (managed && (rc = bitrate_check(c))) return rc;
+  if (!managed && (blobno < 0 || blobno >= VB200_PACKETBLOBS)) return fail(VB200_EINVAL, "blobno");
+  if (nstreams <= 0) return 0;
+  if (!h->pcm || !h->pcm_len || !h->plan || !h->nblocks || h->max_blocks < 1) return fail(VB200_EINVAL, "encode_streams_packets: pcm, pcm_len, plan, nblocks");
+  for (int w = 0; w < 2; w++) {
+    if (h->posts[w] || h->nonzero[w] || h->iwork[w] || h->ampmax_out[w])
+      return fail(VB200_EINVAL, "encode_streams_packets: posts / nonzero / iwork / ampmax_out must be NULL");
+    if (h->cap[w] < 0) return fail(VB200_EINVAL, "cap");
+  }
+  if (!info || (!data && data_cap > 0) || data_cap < 0) return fail(VB200_EINVAL, "encode_streams_packets outputs");
+  if ((int64_t)nstreams * h->max_blocks > INT32_MAX / VB200_PACKETBLOBS) return fail(VB200_EINVAL, "nstreams x max_blocks");
+  std::lock_guard<std::mutex> lk(c->mu);
+  cudaStream_t st = c->s_main;
+  const int curves = managed ? VB200_PACKETBLOBS : 1;
+  const size_t ch = c->setup.channels;
+  const size_t pcm_bytes = (size_t)nstreams * ch * (size_t)h->stream_stride * (h->pcm_fmt == VB200_PCM_S16_INTERLEAVED ? 2 : 4);
+  const size_t n = (size_t)nstreams * h->max_blocks;
+  HostIO io{c};
+  void *p;
+  vb200_streams_io d = *h;
+  if ((rc = io.h2d(h->pcm, pcm_bytes, &p))) return rc; d.pcm = p;
+  if ((rc = io.h2d(h->pcm_len, sizeof(int64_t) * nstreams, &p))) return rc; d.pcm_len = (const int64_t *)p;
+  if (h->eof) { if ((rc = io.h2d(h->eof, sizeof(int64_t) * nstreams, &p))) return rc; d.eof = (const int64_t *)p; }
+  if ((rc = io.h2d(nullptr, sizeof(vb200_stream_block) * n, &p))) return rc; d.plan = (vb200_stream_block *)p;
+  if ((rc = io.h2d(nullptr, sizeof(int32_t) * nstreams, &p))) return rc; d.nblocks = (int32_t *)p;
+  for (int w = 0; w < 2; w++) {
+    const size_t cw = h->cap[w], nn = c->dx[w].N / 2;
+    if (!cw) continue;
+    if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * cw * ch * VB200_FLOOR1_STRIDE, &p))) return rc; d.posts[w] = (int32_t *)p;
+    if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * cw * ch, &p))) return rc; d.nonzero[w] = (int32_t *)p;
+    if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * cw * ch * nn, &p))) return rc; d.iwork[w] = (int32_t *)p;
+    if ((rc = io.h2d(nullptr, sizeof(float) * cw, &p))) return rc; d.ampmax_out[w] = (float *)p;
+  }
+  vb200_block_desc *desc[2] = {nullptr, nullptr};
+  rc = managed ? encode_streams_managed_launch(c, nstreams, &d, st, desc)
+               : encode_streams_launch(c, nstreams, blobno, &d, st, desc);
+  h->count[0] = d.count[0]; h->count[1] = d.count[1];
+  if (rc) return rc;
+  int32_t *bits[2] = {nullptr, nullptr}, *Wb, *sbits, *fbits, *choice = nullptr;
+  uint8_t *strided[2] = {nullptr, nullptr}, *dpk;
+  long long *off;
+  vb200_packet_info *dinfo;
+  if ((rc = carve(c->spk, [&](Carve &k) {
+         for (int w = 0; w < 2; w++) {
+           const size_t cnt = d.count[w];
+           if (!cnt) continue;
+           bits[w] = k.take<int32_t>(curves * cnt);
+           strided[w] = k.take<uint8_t>(curves * cnt * (size_t)c->eent.bound[w]);
+         }
+         Wb = k.take<int32_t>(n); sbits = k.take<int32_t>(n * curves); fbits = k.take<int32_t>(n);
+         if (managed) choice = k.take<int32_t>(n);
+         off = k.take<long long>(n + 1); dinfo = k.take<vb200_packet_info>(n);
+         dpk = k.take<uint8_t>((size_t)std::max<int64_t>(data_cap, 1));
+       }))) return rc;
+  for (int w = 0; w < 2; w++) {
+    const int cnt = d.count[w];
+    if (!cnt) continue;
+    rc = managed ? vb200_encode_entropy_managed_dev(c, w, cnt, d.cap[w], desc[w], d.posts[w], d.nonzero[w], d.iwork[w],
+                                                    c->eent.bound[w], bits[w], strided[w], st)
+                 : vb200_encode_entropy_dev(c, w, cnt, desc[w], d.posts[w], d.nonzero[w], d.iwork[w], c->eent.bound[w],
+                                            bits[w], strided[w], st);
+    if (rc) return rc;
+  }
+  k_stream_bits<<<grid_for(c, (int)((n + 255) / 256), 8), 256, 0, st>>>(nstreams, h->max_blocks, d.plan, d.nblocks, curves,
+                                                                        bits[0], bits[1], d.count[0], d.count[1], Wb,
+                                                                        sbits, fbits);
+  if ((rc = post_launch(c))) return rc;
+  if (managed) {
+    k_bitrate_choose<<<(nstreams + 127) / 128, 128, 0, st>>>(c->br, nstreams, h->max_blocks, d.nblocks, Wb, sbits,
+                                                             nullptr, choice, fbits, 8);
+    if ((rc = post_launch(c))) return rc;
+  }
+  k_packet_offsets<<<1, 1024, 0, st>>>(fbits, (int)n, off);
+  if ((rc = post_launch(c))) return rc;
+  GatherArgs A;
+  A.plan = d.plan; A.nblocks = d.nblocks; A.eof = d.eof; A.nstreams = nstreams; A.max_blocks = h->max_blocks;
+  A.curves = curves;
+  for (int w = 0; w < 2; w++) {
+    A.bs[w] = c->setup.blocksizes[w]; A.count[w] = d.count[w]; A.stride[w] = c->eent.bound[w]; A.data[w] = strided[w];
+  }
+  A.sbits = sbits; A.choice = choice; A.fbits = fbits; A.off = off; A.cap = data_cap; A.info = dinfo; A.dst = dpk;
+  k_stream_gather<<<grid_for(c, (int)n, 8), 256, 0, st>>>(A);
+  if ((rc = post_launch(c))) return rc;
+  int64_t total = 0;
+  CU(cudaMemcpyAsync(h->plan, d.plan, sizeof(vb200_stream_block) * n, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(h->nblocks, d.nblocks, sizeof(int32_t) * nstreams, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(info, dinfo, sizeof(vb200_packet_info) * n, cudaMemcpyDeviceToHost, st));
+  CU(cudaMemcpyAsync(&total, off + n, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  if (total > data_cap) return fail(VB200_EINVAL, "packets exceed data_cap (info filled)");
+  if (total) CU(cudaMemcpyAsync(data, dpk, (size_t)total, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  return 0;
+}
+
+extern "C" int vb200_encode_streams_packets(vb200_ctx *c, int nstreams, int blobno, vb200_streams_io *io,
+                                            vb200_packet_info *info, uint8_t *data, int64_t data_cap) {
+  CHECK_CTX(c);
+  return streams_packets(c, nstreams, blobno, false, io, info, data, data_cap);
+}
+
+extern "C" int vb200_encode_streams_packets_managed(vb200_ctx *c, int nstreams, vb200_streams_io *io,
+                                                    vb200_packet_info *info, uint8_t *data, int64_t data_cap) {
+  CHECK_CTX(c);
+  return streams_packets(c, nstreams, 0, true, io, info, data, data_cap);
 }
 
 // ======================================================================== //

@@ -42,6 +42,8 @@ EXPORTS = [
     "vb200_residue_partvals", "vb200_residue_classify_dev", "vb200_residue_classify",
     "vb200_plan_blocks", "vb200_encode_streams_dev", "vb200_encode_streams",
     "vb200_encode_streams_managed_dev", "vb200_encode_streams_managed",
+    "vb200_bitrate_setup", "vb200_bitrate_init", "vb200_bitrate_addblocks_dev", "vb200_bitrate_addblocks",
+    "vb200_encode_streams_packets", "vb200_encode_streams_packets_managed",
     "vb200_malloc_device", "vb200_free_device", "vb200_memcpy_h2d", "vb200_memcpy_d2h", "vb200_synchronize",
 ]
 
@@ -144,6 +146,12 @@ def load():
     L.vb200_encode_streams_dev.argtypes = [vp, C.c_int, C.c_int, C.POINTER(abi.StreamsIO), vp]
     L.vb200_encode_streams_managed.argtypes = [vp, C.c_int, C.POINTER(abi.StreamsIO)]
     L.vb200_encode_streams_managed_dev.argtypes = [vp, C.c_int, C.POINTER(abi.StreamsIO), vp]
+    L.vb200_bitrate_setup.argtypes = [vp, C.POINTER(abi.BitrateInfo)]
+    L.vb200_bitrate_init.argtypes = [vp, vp]
+    L.vb200_bitrate_addblocks_dev.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp, vp]
+    L.vb200_bitrate_addblocks.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]
+    L.vb200_encode_streams_packets.argtypes = [vp, C.c_int, C.c_int, C.POINTER(abi.StreamsIO), vp, vp, C.c_int64]
+    L.vb200_encode_streams_packets_managed.argtypes = [vp, C.c_int, C.POINTER(abi.StreamsIO), vp, vp, C.c_int64]
     L.vb200_malloc_device.argtypes = [vp, C.c_size_t, C.POINTER(vp)]
     L.vb200_free_device.argtypes = [vp, vp]
     L.vb200_memcpy_h2d.argtypes = [vp, vp, vp, C.c_size_t]
@@ -795,6 +803,89 @@ class Context:
         off, bits, data = out["pkt_off"], out["pkt_bits"], out["data"]
         out["packets"] = [[bytes(data[off[k, i]:off[k, i] + (bits[k, i] + 7) // 8]) for i in range(nb)]
                           for k in range(NB)]
+        return out
+
+    # ---- the bitrate manager on the device and whole streams to packets ------------------------------------
+    def bitrate_setup(self, info):
+        """vb200_bitrate_setup with an abi.BitrateInfo"""
+        self._chk(self.L.vb200_bitrate_setup(self.h, C.byref(info)))
+
+    def bitrate_init(self, nstreams=1):
+        """vorbis_bitrate_init's state for nstreams streams (abi.BITRATE_STATE_DTYPE [nstreams])"""
+        st = np.zeros(nstreams, abi.BITRATE_STATE_DTYPE)
+        for i in range(nstreams):
+            self._chk(self.L.vb200_bitrate_init(self.h, st[i:].ctypes.data))
+        return st
+
+    def bitrate_addblocks(self, count, W, pkt_bits, state, choice=None, nbytes=None, check=True):
+        """vb200_bitrate_addblocks: count [ns], W [ns][max_blocks], pkt_bits [ns][max_blocks][15]; state
+        (BITRATE_STATE_DTYPE [ns]) advanced in place.  Returns (choice, bytes) [ns][max_blocks] (entries past count as
+        passed in), or the status when check is False."""
+        W = np.ascontiguousarray(W, np.int32)
+        ns, mb = W.shape
+        count = np.ascontiguousarray(count, np.int32)
+        pkt_bits = np.ascontiguousarray(pkt_bits, np.int32).reshape(ns, mb, abi.PACKETBLOBS)
+        choice = np.zeros((ns, mb), np.int32) if choice is None else choice
+        nbytes = np.zeros((ns, mb), np.int32) if nbytes is None else nbytes
+        rc = self.L.vb200_bitrate_addblocks(self.h, ns, mb, _ptr(count), _ptr(W), _ptr(pkt_bits), _ptr(state),
+                                            _ptr(choice), _ptr(nbytes))
+        if not check:
+            return rc
+        self._chk(rc)
+        return choice, nbytes
+
+    def bitrate_addblocks_dev(self, nstreams, max_blocks, d_count, d_W, d_pkt_bits, d_state, d_choice, d_bytes,
+                              stream=None, check=True):
+        rc = self.L.vb200_bitrate_addblocks_dev(self.h, nstreams, max_blocks, _ptr(d_count), _ptr(d_W),
+                                                _ptr(d_pkt_bits), _ptr(d_state), _ptr(d_choice), _ptr(d_bytes),
+                                                _ptr(stream))
+        if check:
+            self._chk(rc)
+        return rc
+
+    def encode_streams_packets(self, pcm, pcm_len, eof=None, fmt=PCM_F32_PLANAR, max_blocks=None, cap=None, blobno=7,
+                               managed=False, data_cap=None, check=True):
+        """vb200_encode_streams_packets[_managed] on timeline buffers as for encode_streams: {"plan", "nblocks",
+        "count", "info" (PACKET_INFO_DTYPE [ns][max_blocks]), "data", "packets": per stream [bytes]} (and "rc" when
+        check is False, in which case an error does not raise and "packets" is absent)"""
+        ch = self.channels
+        if fmt == PCM_F32_PLANAR:
+            pcm = np.ascontiguousarray(pcm, np.float32)
+            ns, stride = pcm.shape[0], pcm.shape[2]
+            assert pcm.shape[1] == ch
+        else:
+            pcm = np.ascontiguousarray(pcm, np.int16)
+            ns, stride = pcm.shape[0], pcm.shape[1]
+            assert pcm.shape[2] == ch
+        pcm_len = np.ascontiguousarray(pcm_len, np.int64)
+        eofp = None if eof is None else np.ascontiguousarray(eof, np.int64)
+        if max_blocks is None:
+            max_blocks = stride // (self.bs[0] // 2) + 8
+        if cap is None:
+            cap = [ns * max_blocks, ns * (stride // (self.bs[1] // 2) + 8)]
+        io = abi.StreamsIO()
+        io.pcm, io.pcm_fmt, io.max_blocks, io.stream_stride = pcm.ctypes.data, fmt, max_blocks, stride
+        io.pcm_len = pcm_len.ctypes.data
+        io.eof = None if eofp is None else eofp.ctypes.data
+        plan = np.zeros((ns, max_blocks), abi.STREAM_BLOCK_DTYPE)
+        nb = np.zeros(ns, np.int32)
+        io.plan, io.nblocks = plan.ctypes.data, nb.ctypes.data
+        io.cap[0], io.cap[1] = int(cap[0]), int(cap[1])
+        info = np.zeros((ns, max_blocks), abi.PACKET_INFO_DTYPE)
+        if data_cap is None:
+            data_cap = ns * max_blocks * max(self.packet_bound(0), self.packet_bound(1))
+        data = np.zeros(max(data_cap, 1), np.uint8)
+        if managed:
+            rc = self.L.vb200_encode_streams_packets_managed(self.h, ns, C.byref(io), _ptr(info), _ptr(data), data_cap)
+        else:
+            rc = self.L.vb200_encode_streams_packets(self.h, ns, blobno, C.byref(io), _ptr(info), _ptr(data), data_cap)
+        out = {"plan": plan, "nblocks": nb, "count": [io.count[0], io.count[1]], "info": info, "data": data}
+        if not check:
+            out["rc"] = rc
+            return out
+        self._chk(rc)
+        out["packets"] = [[bytes(data[r["offset"]:r["offset"] + r["bytes"]]) for r in info[i, :nb[i]]]
+                          for i in range(ns)]
         return out
 
     # ---- envelope / block-switch detector (lib/envelope.c) --------------------------------------
