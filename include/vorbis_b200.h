@@ -840,6 +840,49 @@ int vb200_encode_streams_packets        (vb200_ctx*, int nstreams, int blobno, v
 int vb200_encode_streams_packets_managed(vb200_ctx*, int nstreams, vb200_streams_io *io,
                                          vb200_packet_info *info, uint8_t *data, int64_t data_cap);
 
+/* ---- whole streams to packets in pieces: the same calls with a carried per-stream encoder state, for PCM that arrives
+ * over time.  The carry is [nstreams][vb200_encode_carry_bytes] bytes; each begins with a vb200_encode_carry head that
+ * callers may read, the rest is opaque: the planner state of vorbis_analysis_blockout and the envelope search
+ * (lib/block.c:534-689, lib/envelope.c:215-374: W, lW, centerW, ve->cursor, ve->curmark, ve->current and the eof
+ * state), the envelope detector's VB200_VE_STATE_WORDS(ch) words, the window of ve->mark that _ve_envelope_shift keeps,
+ * the ampmax chain (g->ampmax and the previous block's vbi->ampmax) and a vb200_bitrate_state.
+ *   mark_steps  capacity of the mark window in 64-sample steps; <= 0 takes the default, (3*blocksizes[1]/2 +
+ *               blocksizes[0]/4)/64 + 8, which holds every window a call leaves unless max_blocks cut it short.  A call
+ *               cut by max_blocks keeps the marks of everything it analysed beyond the last block: about
+ *               (pcm_len - consumed)/64 + 2 steps.  A call whose window would not fit returns VB200_EINVAL and leaves
+ *               the carry as it was.
+ *   vb200_encode_carry_init writes fresh carries: a fresh vorbis_dsp_state (base 0, packetno 3) and, when a managed
+ *   vb200_bitrate_setup is registered, vorbis_bitrate_init's state (initialise after the setup for the managed form).
+ * Per call, stream s passes timeline samples [base, base + pcm_len[s]) in io->pcm (the layouts of vb200_streams_io):
+ * the samples the carry kept (the previous call's base + pcm_len minus the new base), then the new ones.  A stream with
+ * no new data passes just what it kept.  eof[s] is in timeline samples (v->eofflag plus base), and is given only in
+ * calls whose buffer ends at the end of the timeline (with the extrapolated tail of vorbis_analysis_wrote(v,0)); 0
+ * before.  A stream whose carry is done is skipped and emits nothing.  LPC pre- and post-extrapolation stay with the
+ * caller: the timeline is the one described at vb200_plan_blocks.
+ * Output as vb200_encode_streams_packets: info and data hold this call's packets only, with absolute granulepos and
+ * continuing packetno; plan[].pos is relative to this call's buffer (so int32 suffices for streams longer than 2^31
+ * samples).  max_blocks may cut a call short; the carry records where planning stopped.
+ * Contract: (a) a fresh carry with the whole timeline in one call gives vb200_encode_streams_packets[_managed]'s output;
+ * (b) cutting a stream's timeline into any sequence of calls, at any sample, including calls with no new samples and
+ * calls cut by max_blocks, gives the packets and infos of one call, byte for byte; (c) hence, fed the timeline of a
+ * stock encoder written in chunks, the result is that encoder's packets, granulepos, e_o_s and packetno.
+ * Errors: those of vb200_encode_streams_packets[_managed]; VB200_EINVAL for a null carry, a carry of another channel
+ * count, block-size setup or mark capacity than stream 0's, (managed) a carry initialised before a managed
+ * vb200_bitrate_setup, pcm_len[s] below what the carry kept, eof[s] at or before base, and a mark window overflow.  On any error the carries are left as they were.  The launches are those of the
+ * fresh calls.  Device scratch: that of the fresh calls plus the carries and nstreams x (the steps analysed) bytes.  */
+typedef struct vb200_encode_carry {
+  int64_t base;        /* timeline sample where the next call's buffer for this stream starts (the sum of movementW) */
+  int64_t granulepos;  /* the last packet's granulepos (0 before the first) */
+  int32_t packetno;    /* the next packet's number (v->sequence) */
+  int32_t done;        /* the e_o_s packet has been emitted */
+} vb200_encode_carry;
+int vb200_encode_carry_bytes(vb200_ctx*, int mark_steps);
+int vb200_encode_carry_init (vb200_ctx*, int nstreams, int mark_steps, void *carry);
+int vb200_encode_streams_packets_resume        (vb200_ctx*, int nstreams, int blobno, vb200_streams_io *io,
+                                                void *carry, vb200_packet_info *info, uint8_t *data, int64_t data_cap);
+int vb200_encode_streams_packets_managed_resume(vb200_ctx*, int nstreams, vb200_streams_io *io,
+                                                void *carry, vb200_packet_info *info, uint8_t *data, int64_t data_cap);
+
 /* ---- device memory helpers for non-CUDA hosts (C callers) -------------- */
 int  vb200_malloc_device(vb200_ctx*, size_t bytes, void **dptr);
 int  vb200_free_device  (vb200_ctx*, void *dptr);

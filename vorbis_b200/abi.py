@@ -202,6 +202,9 @@ BITRATE_STATE_DTYPE = np.dtype([("avg_reservoir", "<i8"), ("minmax_reservoir", "
 PACKET_INFO_DTYPE = np.dtype([("offset", "<i8"), ("granulepos", "<i8"), ("bytes", "<i4"), ("e_o_s", "<i4"),
                               ("packetno", "<i4"), ("choice", "<i4")])         # vb200_packet_info
 assert C.sizeof(BitrateInfo) == 48 and BITRATE_STATE_DTYPE.itemsize == 32 and PACKET_INFO_DTYPE.itemsize == 32
+# vb200_encode_carry: the public head of every stream's carry ([nstreams][vb200_encode_carry_bytes] bytes)
+ENCODE_CARRY_HEAD_DTYPE = np.dtype([("base", "<i8"), ("granulepos", "<i8"), ("packetno", "<i4"), ("done", "<i4")])
+assert ENCODE_CARRY_HEAD_DTYPE.itemsize == 24
 
 
 class Codebook(C.Structure):

@@ -2249,6 +2249,10 @@ extern "C" int vb200_encode_dsp(vb200_ctx *c, int W, int nstreams, int bps, int 
 
 // ======================================================================== //
 // whole streams: block planning and the two size batches
+static int envelope_search_launch(vb200_ctx *c, int nstreams, const void *d_pcm, int fmt, int64_t stride,
+                                  int first_step, int nsteps, int32_t *d_state, uint8_t *d_ret, void *stream,
+                                  const int32_t *d_steps_per_stream, const int32_t *d_first_per_stream);
+
 static int plan_check(vb200_ctx *c) {
   if (c->n_psy != 4) return fail(VB200_EINVAL, "context has no psy setup");
   if ((c->setup.blocksizes[0] / 4) % PLAN_STEP) return fail(VB200_EIMPL, "blocksizes[0]/4 must be a multiple of the 64-sample envelope step");
@@ -2260,11 +2264,15 @@ static int plan_check(vb200_ctx *c) {
 static int plan_launch(vb200_ctx *c, int nstreams, const int32_t *d_mark, int64_t mark_stride, int nsteps,
                        const int64_t *d_len, const int64_t *d_eof, int max_blocks, vb200_stream_block *d_plan,
                        int32_t *d_nblocks, const int cap[2], int2 *d_src[2], vb200_block_desc *d_desc[2],
-                       int32_t *d_totals, int32_t *d_work, cudaStream_t st) {
+                       int32_t *d_totals, int32_t *d_work, cudaStream_t st, const CarryDev *K = nullptr) {
   int32_t *d_counts = d_work, *d_offs = d_work + 2 * (size_t)nstreams;
   const int g = (nstreams + 127) / 128;
-  k_plan_blocks<<<g, 128, 0, st>>>(nstreams, c->setup.blocksizes[0], c->setup.blocksizes[1], d_mark, mark_stride, nsteps,
-                                   d_len, d_eof, max_blocks, d_plan, d_nblocks, d_counts);
+  if (K)
+    k_plan_blocks_carry<<<g, 128, 0, st>>>(nstreams, c->setup.blocksizes[0], c->setup.blocksizes[1], d_mark, mark_stride,
+                                           nsteps, d_len, d_eof, max_blocks, d_plan, d_nblocks, d_counts, *K);
+  else
+    k_plan_blocks<<<g, 128, 0, st>>>(nstreams, c->setup.blocksizes[0], c->setup.blocksizes[1], d_mark, mark_stride, nsteps,
+                                     d_len, d_eof, max_blocks, d_plan, d_nblocks, d_counts);
   k_plan_offsets<<<1, 32, 0, st>>>(nstreams, d_counts, d_offs, d_totals);
   k_plan_fill<<<g, 128, 0, st>>>(nstreams, max_blocks, d_plan, d_nblocks, d_offs, cap[0], cap[1],
                                  d_src[0], d_src[1], d_desc[0], d_desc[1]);
@@ -2325,9 +2333,11 @@ static int streams_check(vb200_ctx *c, int nstreams, vb200_streams_io *d) {
 // The front half of both streams calls, up to the psy stage: envelope search, marks, plan, the transforms of
 // both sizes and the ampmax chain along every stream.  Sets count[]; for each size with blocks, S[w] holds the
 // transforms, a[w] the psy stage's io, d_desc[w] the batch's block descriptors and, given M, M[w] the scratch of
-// the managed tail.  Begins the call's use of the context scratch.
+// the managed tail.  Begins the call's use of the context scratch.  K: carried streams (the envelope state, marks,
+// planner and ampmax chain start from the carries and go back to them); K->count's largest entry is nsteps_env.
 static int streams_front(vb200_ctx *c, int nstreams, vb200_streams_io *d, cudaStream_t st, EncScratch S[2],
-                         vb200_phaseA_io a[2], vb200_block_desc *d_desc[2], MgdScratch *M = nullptr) {
+                         vb200_phaseA_io a[2], vb200_block_desc *d_desc[2], MgdScratch *M = nullptr,
+                         const CarryDev *K = nullptr, int nsteps_env = 0) {
   int rc;
   const int ch = c->setup.channels;
   // 1. envelope search over the whole timeline (fresh detector state), 2. marks, 3. plan
@@ -2335,9 +2345,11 @@ static int streams_front(vb200_ctx *c, int nstreams, vb200_streams_io *d, cudaSt
   if (nsteps < 1) return fail(VB200_EINVAL, "stream too short");
   const int64_t mark_stride = nsteps + 4;
   const size_t sw = VB200_VE_STATE_WORDS(ch);
+  const int nret = K ? nsteps_env : nsteps;
   int32_t *d_state, *d_mark, *d_tot, *d_work; uint8_t *d_ret; int2 *d_src[2];
   if ((rc = carve(c->plan, [&](Carve &k) {
-         d_state = k.take<int32_t>(sw * nstreams); d_ret = k.take<uint8_t>((size_t)nstreams * nsteps);
+         d_state = K ? nullptr : k.take<int32_t>(sw * nstreams);      // carried streams use the carries' state
+         d_ret = k.take<uint8_t>((size_t)nstreams * (nret > 0 ? nret : 1));
          d_mark = k.take<int32_t>((size_t)nstreams * mark_stride); d_tot = k.take<int32_t>(2);
          d_work = k.take<int32_t>(4 * (size_t)nstreams);
          for (int w = 0; w < 2; w++) {
@@ -2346,19 +2358,30 @@ static int streams_front(vb200_ctx *c, int nstreams, vb200_streams_io *d, cudaSt
          }
        }))) return rc;
   if ((rc = scratch_begin(c, st))) return rc;
-  CU(cudaMemsetAsync(d_state, 0, sizeof(int32_t) * sw * nstreams, st));
-  if ((rc = vb200_envelope_search_dev(c, nstreams, d->pcm, d->pcm_fmt, d->stream_stride, 0, nsteps, d_state, d_ret, st))) return rc;
+  if (K) {
+    if (nret > 0 && (rc = envelope_search_launch(c, nstreams, d->pcm, d->pcm_fmt, d->stream_stride, 0, nret, K->env, d_ret,
+                                                 st, K->count, K->first))) return rc;
+  } else {
+    CU(cudaMemsetAsync(d_state, 0, sizeof(int32_t) * sw * nstreams, st));
+    if ((rc = vb200_envelope_search_dev(c, nstreams, d->pcm, d->pcm_fmt, d->stream_stride, 0, nsteps, d_state, d_ret, st))) return rc;
+  }
   {
     const long long total = (long long)nstreams * mark_stride;
-    k_env_marks<<<grid_for(c, (int)((total + 255) / 256), 8), 256, 0, st>>>(nstreams, nsteps, d_ret, d->pcm_len, d_mark, mark_stride);
+    if (K)
+      k_env_marks_carry<<<grid_for(c, (int)((total + 255) / 256), 8), 256, 0, st>>>(nstreams, nret, d_ret, d_mark,
+                                                                                    mark_stride, *K);
+    else
+      k_env_marks<<<grid_for(c, (int)((total + 255) / 256), 8), 256, 0, st>>>(nstreams, nsteps, d_ret, d->pcm_len, d_mark, mark_stride);
     if ((rc = post_launch(c))) return rc;
   }
   if ((rc = plan_launch(c, nstreams, d_mark, mark_stride, nsteps, d->pcm_len, d->eof, d->max_blocks, d->plan, d->nblocks,
-                        d->cap, d_src, d_desc, d_tot, d_work, st))) return rc;
-  int tot[2];
+                        d->cap, d_src, d_desc, d_tot, d_work, st, K))) return rc;
+  int tot[2], overflow = 0;
   CU(cudaMemcpyAsync(tot, d_tot, sizeof(tot), cudaMemcpyDeviceToHost, st));
+  if (K) CU(cudaMemcpyAsync(&overflow, K->overflow, sizeof(int), cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));                       // the launches below are sized by the plan
   d->count[0] = tot[0]; d->count[1] = tot[1];
+  if (overflow) return fail(VB200_EINVAL, "encode carry: the mark window does not fit the carry's mark capacity");
   if (tot[0] > d->cap[0] || tot[1] > d->cap[1]) return fail(VB200_EINVAL, "encode_streams: more blocks than cap[] (count[] holds the need)");
   // 4. transforms of both sizes, 5. the ampmax chain along every stream
   if ((rc = carve(c->chain, [&](Carve &k) {
@@ -2381,9 +2404,15 @@ static int streams_front(vb200_ctx *c, int nstreams, vb200_streams_io *d, cudaSt
   {
     float sa[2];
     for (int w = 0; w < 2; w++) sa[w] = ((float)(c->dx[w].N / 2) / (float)c->setup.rate) * c->setup.ampmax_att_per_sec;   // lib/psy.c:843
-    k_ampmax_plan<<<(nstreams + 127) / 128, 128, 0, st>>>(nstreams, d->max_blocks, ch, d->plan, d->nblocks,
-                                                          tot[0] ? S[0].lmax : nullptr, tot[1] ? S[1].lmax : nullptr,
-                                                          sa[0], sa[1], tot[0] ? S[0].gmax : nullptr, tot[1] ? S[1].gmax : nullptr);
+    if (K)
+      k_ampmax_plan_carry<<<(nstreams + 127) / 128, 128, 0, st>>>(nstreams, d->max_blocks, ch, d->plan, d->nblocks,
+                                                                  tot[0] ? S[0].lmax : nullptr, tot[1] ? S[1].lmax : nullptr,
+                                                                  sa[0], sa[1], tot[0] ? S[0].gmax : nullptr,
+                                                                  tot[1] ? S[1].gmax : nullptr, K->pc);
+    else
+      k_ampmax_plan<<<(nstreams + 127) / 128, 128, 0, st>>>(nstreams, d->max_blocks, ch, d->plan, d->nblocks,
+                                                            tot[0] ? S[0].lmax : nullptr, tot[1] ? S[1].lmax : nullptr,
+                                                            sa[0], sa[1], tot[0] ? S[0].gmax : nullptr, tot[1] ? S[1].gmax : nullptr);
     if ((rc = post_launch(c))) return rc;
   }
   return 0;
@@ -2391,7 +2420,7 @@ static int streams_front(vb200_ctx *c, int nstreams, vb200_streams_io *d, cudaSt
 
 // desc_out (optional): the two batches' block descriptors, which stay in the plan arena until its next carve
 static int encode_streams_launch(vb200_ctx *c, int nstreams, int blobno, vb200_streams_io *d, cudaStream_t stream,
-                                 vb200_block_desc **desc_out) {
+                                 vb200_block_desc **desc_out, const CarryDev *K = nullptr, int nsteps_env = 0) {
   int rc;
   if ((rc = streams_check(c, nstreams, d)) || nstreams <= 0) return rc;
   if (blobno < 0 || blobno >= VB200_PACKETBLOBS) return fail(VB200_EINVAL, "blobno");
@@ -2400,7 +2429,7 @@ static int encode_streams_launch(vb200_ctx *c, int nstreams, int blobno, vb200_s
   EncScratch S[2];
   vb200_phaseA_io a[2];
   vb200_block_desc *d_desc[2];
-  if ((rc = streams_front(c, nstreams, d, st, S, a, d_desc))) return rc;
+  if ((rc = streams_front(c, nstreams, d, st, S, a, d_desc, nullptr, K, nsteps_env))) return rc;
   // 6. the rest of the chain per size
   for (int w = 0; w < 2; w++) {
     if (!d->count[w]) continue;
@@ -2423,7 +2452,7 @@ extern "C" int vb200_encode_streams_dev(vb200_ctx *c, int nstreams, int blobno, 
 }
 
 static int encode_streams_managed_launch(vb200_ctx *c, int nstreams, vb200_streams_io *d, cudaStream_t stream,
-                                         vb200_block_desc **desc_out) {
+                                         vb200_block_desc **desc_out, const CarryDev *K = nullptr, int nsteps_env = 0) {
   int rc;
   if ((rc = streams_check(c, nstreams, d)) || nstreams <= 0) return rc;
   cudaStream_t st = (cudaStream_t)stream;
@@ -2431,7 +2460,7 @@ static int encode_streams_managed_launch(vb200_ctx *c, int nstreams, vb200_strea
   vb200_phaseA_io a[2];
   vb200_block_desc *d_desc[2];
   MgdScratch M[2];
-  if ((rc = streams_front(c, nstreams, d, st, S, a, d_desc, M))) return rc;
+  if ((rc = streams_front(c, nstreams, d, st, S, a, d_desc, M, K, nsteps_env))) return rc;
   for (int w = 0; w < 2; w++) {
     if (!d->count[w]) continue;
     const int nb = d->count[w];
@@ -3568,11 +3597,133 @@ extern "C" int vb200_bitrate_addblocks(vb200_ctx *c, int nstreams, int max_block
   return io.sync();
 }
 
+// ---- carried streams: the host carry is [nstreams][carry_bytes] of PlanCarry, the mark window (mark_cap bytes),
+// the envelope state and a vb200_bitrate_state, each part 8-byte aligned.  One call stages all carries as one buffer
+// of arrays (CarryBlob), laid out by carve's rule on the host and used at the same offsets on the device.
+static_assert(sizeof(PlanCarry) % 8 == 0 && offsetof(PlanCarry, base) == offsetof(vb200_encode_carry, base) &&
+              offsetof(PlanCarry, granulepos) == offsetof(vb200_encode_carry, granulepos) &&
+              offsetof(PlanCarry, packetno) == offsetof(vb200_encode_carry, packetno) &&
+              offsetof(PlanCarry, done) == offsetof(vb200_encode_carry, done) && sizeof(vb200_encode_carry) == 24,
+              "vb200_encode_carry is the head of PlanCarry (mirrored by vorbis_b200/abi.py)");
+
+struct CarryParts { size_t marks, env, br, bytes; };
+static CarryParts carry_parts(const vb200_ctx *c, int cap) {
+  CarryParts q;
+  q.marks = sizeof(PlanCarry);
+  q.env = q.marks + (((size_t)cap + 7) & ~(size_t)7);
+  q.br = q.env + ((sizeof(int32_t) * VB200_VE_STATE_WORDS(c->setup.channels) + 7) & ~(size_t)7);
+  q.bytes = q.br + sizeof(vb200_bitrate_state);
+  return q;
+}
+static int carry_cap(const vb200_ctx *c, int mark_steps) {
+  return mark_steps > 0 ? mark_steps : (3 * c->setup.blocksizes[1] / 2 + c->setup.blocksizes[0] / 4) / PLAN_STEP + 8;
+}
+
+extern "C" int vb200_encode_carry_bytes(vb200_ctx *c, int mark_steps) {
+  CHECK_CTX(c);
+  return (int)carry_parts(c, carry_cap(c, mark_steps)).bytes;
+}
+
+extern "C" int vb200_encode_carry_init(vb200_ctx *c, int nstreams, int mark_steps, void *carry) {
+  CHECK_CTX(c);
+  if (nstreams <= 0) return 0;
+  if (!carry) return fail(VB200_EINVAL, "null carry");
+  const int cap = carry_cap(c, mark_steps);
+  const CarryParts q = carry_parts(c, cap);
+  for (int s = 0; s < nstreams; s++) {
+    char *cs = (char *)carry + (size_t)s * q.bytes;
+    memset(cs, 0, q.bytes);
+    PlanCarry p{};
+    p.packetno = 3;                                  // lib/block.c:311
+    p.centerW = p.cursor = c->setup.blocksizes[1] / 2;
+    p.gmax = p.prev = -9999.f;
+    p.ch = c->setup.channels; p.bs0 = c->setup.blocksizes[0]; p.bs1 = c->setup.blocksizes[1]; p.mark_cap = cap;
+    p.br_ready = c->br_set && c->br_managed;
+    memcpy(cs, &p, sizeof(p));
+    if (p.br_ready) {
+      vb200_bitrate_state b;
+      vb200_bitrate_init(c, &b);
+      memcpy(cs + q.br, &b, sizeof(b));
+    }
+  }
+  return 0;
+}
+
+struct CarryBlob {
+  PlanCarry *pc; uint8_t *marks; int32_t *env; vb200_bitrate_state *br; int32_t *first, *count, *overflow;
+};
+static void carry_blob_layout(Carve &k, size_t n, int cap, size_t sw, CarryBlob *b) {
+  b->pc = k.take<PlanCarry>(n); b->marks = k.take<uint8_t>(n * cap); b->env = k.take<int32_t>(n * sw);
+  b->br = k.take<vb200_bitrate_state>(n); b->first = k.take<int32_t>(n); b->count = k.take<int32_t>(n);
+  b->overflow = k.take<int32_t>(1);
+}
+
+// checks the carries against the context and the call, and packs them into blob (host memory); *nsteps_env = the
+// most envelope steps one stream analyses
+static int carry_pack(vb200_ctx *c, int nstreams, bool managed, const vb200_streams_io *h, const void *carry,
+                      std::vector<char> &blob, CarryBlob &b, int *cap_out, int *nsteps_env) {
+  const PlanCarry *p0 = (const PlanCarry *)carry;
+  const int ch = c->setup.channels, cap = p0->mark_cap;
+  if (p0->ch != ch || p0->bs0 != c->setup.blocksizes[0] || p0->bs1 != c->setup.blocksizes[1] || cap < 1)
+    return fail(VB200_EINVAL, "encode carry of another setup");
+  const CarryParts q = carry_parts(c, cap);
+  const size_t sw = VB200_VE_STATE_WORDS(ch);
+  Carve sz{nullptr, 0};
+  carry_blob_layout(sz, nstreams, cap, sw, &b);
+  blob.assign(sz.off, 0);
+  Carve at{blob.data(), 0};
+  carry_blob_layout(at, nstreams, cap, sw, &b);
+  const long long nsteps = h->stream_stride / PLAN_STEP - PLAN_VE_WIN;
+  int most = 0;
+  for (int s = 0; s < nstreams; s++) {
+    const char *cs = (const char *)carry + (size_t)s * q.bytes;
+    PlanCarry p;
+    memcpy(&p, cs, sizeof(p));
+    if (p.ch != ch || p.bs0 != p0->bs0 || p.bs1 != p0->bs1 || p.mark_cap != cap)
+      return fail(VB200_EINVAL, "encode carries of different setups or mark capacities");
+    if (managed && !p.br_ready)
+      return fail(VB200_EINVAL, "encode carry made before a managed vb200_bitrate_setup (no bitrate state)");
+    int first = 0, count = 0;
+    if (!p.done) {
+      if (h->pcm_len[s] < p.kept) return fail(VB200_EINVAL, "pcm_len below the samples the carry kept");
+      if (h->pcm_len[s] > h->stream_stride) return fail(VB200_EINVAL, "pcm_len above stream_stride");
+      if (h->eof && h->eof[s] != 0 && h->eof[s] <= p.base) return fail(VB200_EINVAL, "eof at or before the carry's base");
+      long long last = h->pcm_len[s] / PLAN_STEP - PLAN_VE_WIN;    // lib/envelope.c:224-225, as k_plan_blocks clamps it
+      if (last > nsteps) last = nsteps;
+      first = (int)(p.current / PLAN_STEP);
+      count = last > first ? (int)(last - first) : 0;
+    }
+    b.pc[s] = p;
+    memcpy(b.marks + (size_t)s * cap, cs + q.marks, cap);
+    memcpy(b.env + (size_t)s * sw, cs + q.env, sizeof(int32_t) * sw);
+    memcpy(&b.br[s], cs + q.br, sizeof(vb200_bitrate_state));
+    b.first[s] = first; b.count[s] = count;
+    if (count > most) most = count;
+  }
+  *b.overflow = 0;
+  *cap_out = cap;
+  *nsteps_env = most;
+  return 0;
+}
+
+static void carry_unpack(vb200_ctx *c, int nstreams, int cap, const CarryBlob &b, void *carry) {
+  const CarryParts q = carry_parts(c, cap);
+  const size_t sw = VB200_VE_STATE_WORDS(c->setup.channels);
+  for (int s = 0; s < nstreams; s++) {
+    char *cs = (char *)carry + (size_t)s * q.bytes;
+    memcpy(cs, &b.pc[s], sizeof(PlanCarry));
+    memcpy(cs + q.marks, b.marks + (size_t)s * cap, cap);
+    memcpy(cs + q.env, b.env + (size_t)s * sw, sizeof(int32_t) * sw);
+    memcpy(cs + q.br, &b.br[s], sizeof(vb200_bitrate_state));
+  }
+}
+
 // Both whole-stream packet calls: the streams chain into staged device buffers, the entropy coder per size, then
 // (k_stream_bits, [k_bitrate_choose], k_packet_offsets, k_stream_gather) on the spk arena, carved once when the
-// per-size block counts are known.  One synchronous round trip on s_main.
+// per-size block counts are known.  One synchronous round trip on s_main.  carry (host): the _resume forms, whose
+// carries are staged as one more buffer and written back only when the call succeeds.
 static int streams_packets(vb200_ctx *c, int nstreams, int blobno, bool managed, vb200_streams_io *h,
-                           vb200_packet_info *info, uint8_t *data, int64_t data_cap) {
+                           vb200_packet_info *info, uint8_t *data, int64_t data_cap, void *carry = nullptr) {
   int rc;
   if ((rc = plan_check(c))) return rc;
   if (!h) return fail(VB200_EINVAL, "null io");
@@ -3589,6 +3740,10 @@ static int streams_packets(vb200_ctx *c, int nstreams, int blobno, bool managed,
   }
   if (!info || (!data && data_cap > 0) || data_cap < 0) return fail(VB200_EINVAL, "encode_streams_packets outputs");
   if ((int64_t)nstreams * h->max_blocks > INT32_MAX / VB200_PACKETBLOBS) return fail(VB200_EINVAL, "nstreams x max_blocks");
+  std::vector<char> cblob;
+  CarryBlob hb{};
+  int ccap = 0, nsteps_env = 0;
+  if (carry && (rc = carry_pack(c, nstreams, managed, h, carry, cblob, hb, &ccap, &nsteps_env))) return rc;
   std::lock_guard<std::mutex> lk(c->mu);
   cudaStream_t st = c->s_main;
   const int curves = managed ? VB200_PACKETBLOBS : 1;
@@ -3611,9 +3766,19 @@ static int streams_packets(vb200_ctx *c, int nstreams, int blobno, bool managed,
     if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * cw * ch * nn, &p))) return rc; d.iwork[w] = (int32_t *)p;
     if ((rc = io.h2d(nullptr, sizeof(float) * cw, &p))) return rc; d.ampmax_out[w] = (float *)p;
   }
+  CarryDev K{}, *Kp = nullptr;
+  char *dblob = nullptr;
+  if (carry) {
+    if ((rc = io.h2d(cblob.data(), cblob.size(), &p))) return rc;
+    dblob = (char *)p;
+    auto dev = [&](auto *hp) { return (decltype(hp))(dblob + ((char *)hp - cblob.data())); };
+    K.pc = dev(hb.pc); K.marks = dev(hb.marks); K.cap = ccap; K.env = dev(hb.env); K.br = dev(hb.br);
+    K.first = dev(hb.first); K.count = dev(hb.count); K.overflow = dev(hb.overflow);
+    Kp = &K;
+  }
   vb200_block_desc *desc[2] = {nullptr, nullptr};
-  rc = managed ? encode_streams_managed_launch(c, nstreams, &d, st, desc)
-               : encode_streams_launch(c, nstreams, blobno, &d, st, desc);
+  rc = managed ? encode_streams_managed_launch(c, nstreams, &d, st, desc, Kp, nsteps_env)
+               : encode_streams_launch(c, nstreams, blobno, &d, st, desc, Kp, nsteps_env);
   h->count[0] = d.count[0]; h->count[1] = d.count[1];
   if (rc) return rc;
   int32_t *bits[2] = {nullptr, nullptr}, *Wb, *sbits, *fbits, *choice = nullptr;
@@ -3647,7 +3812,7 @@ static int streams_packets(vb200_ctx *c, int nstreams, int blobno, bool managed,
   if ((rc = post_launch(c))) return rc;
   if (managed) {
     k_bitrate_choose<<<(nstreams + 127) / 128, 128, 0, st>>>(c->br, nstreams, h->max_blocks, d.nblocks, Wb, sbits,
-                                                             nullptr, choice, fbits, 8);
+                                                             Kp ? K.br : nullptr, choice, fbits, 8);
     if ((rc = post_launch(c))) return rc;
   }
   k_packet_offsets<<<1, 1024, 0, st>>>(fbits, (int)n, off);
@@ -3659,9 +3824,13 @@ static int streams_packets(vb200_ctx *c, int nstreams, int blobno, bool managed,
     A.bs[w] = c->setup.blocksizes[w]; A.count[w] = d.count[w]; A.stride[w] = c->eent.bound[w]; A.data[w] = strided[w];
   }
   A.sbits = sbits; A.choice = choice; A.fbits = fbits; A.off = off; A.cap = data_cap; A.info = dinfo; A.dst = dpk;
-  k_stream_gather<<<grid_for(c, (int)n, 8), 256, 0, st>>>(A);
+  if (Kp)
+    k_stream_gather_carry<<<grid_for(c, (int)n, 8), 256, 0, st>>>(A, K.pc);
+  else
+    k_stream_gather<<<grid_for(c, (int)n, 8), 256, 0, st>>>(A);
   if ((rc = post_launch(c))) return rc;
   int64_t total = 0;
+  if (carry) CU(cudaMemcpyAsync(cblob.data(), dblob, cblob.size(), cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(h->plan, d.plan, sizeof(vb200_stream_block) * n, cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(h->nblocks, d.nblocks, sizeof(int32_t) * nstreams, cudaMemcpyDeviceToHost, st));
   CU(cudaMemcpyAsync(info, dinfo, sizeof(vb200_packet_info) * n, cudaMemcpyDeviceToHost, st));
@@ -3670,6 +3839,7 @@ static int streams_packets(vb200_ctx *c, int nstreams, int blobno, bool managed,
   if (total > data_cap) return fail(VB200_EINVAL, "packets exceed data_cap (info filled)");
   if (total) CU(cudaMemcpyAsync(data, dpk, (size_t)total, cudaMemcpyDeviceToHost, st));
   CU(cudaStreamSynchronize(st));
+  if (carry) carry_unpack(c, nstreams, ccap, hb, carry);
   return 0;
 }
 
@@ -3685,6 +3855,22 @@ extern "C" int vb200_encode_streams_packets_managed(vb200_ctx *c, int nstreams, 
   return streams_packets(c, nstreams, 0, true, io, info, data, data_cap);
 }
 
+extern "C" int vb200_encode_streams_packets_resume(vb200_ctx *c, int nstreams, int blobno, vb200_streams_io *io,
+                                                   void *carry, vb200_packet_info *info, uint8_t *data,
+                                                   int64_t data_cap) {
+  CHECK_CTX(c);
+  if (!carry) return fail(VB200_EINVAL, "null carry");
+  return streams_packets(c, nstreams, blobno, false, io, info, data, data_cap, carry);
+}
+
+extern "C" int vb200_encode_streams_packets_managed_resume(vb200_ctx *c, int nstreams, vb200_streams_io *io,
+                                                           void *carry, vb200_packet_info *info, uint8_t *data,
+                                                           int64_t data_cap) {
+  CHECK_CTX(c);
+  if (!carry) return fail(VB200_EINVAL, "null carry");
+  return streams_packets(c, nstreams, 0, true, io, info, data, data_cap, carry);
+}
+
 // ======================================================================== //
 // envelope / block-switch detector
 static int env_check(vb200_ctx *c, int nstreams, const void *pcm, int fmt, int64_t stride, int first, int nsteps,
@@ -3698,9 +3884,11 @@ static int env_check(vb200_ctx *c, int nstreams, const void *pcm, int fmt, int64
   return 0;
 }
 
+// d_first_per_stream (with d_steps_per_stream): stream s analyses steps d_first_per_stream[s] + j, j < its count,
+// and first_step is 0
 static int envelope_search_launch(vb200_ctx *c, int nstreams, const void *d_pcm, int fmt, int64_t stride,
                                   int first_step, int nsteps, int32_t *d_state, uint8_t *d_ret, void *stream,
-                                  const int32_t *d_steps_per_stream) {
+                                  const int32_t *d_steps_per_stream, const int32_t *d_first_per_stream) {
   CHECK_CTX(c);
   int rc;
   if ((rc = env_check(c, nstreams, d_pcm, fmt, stride, first_step, nsteps, d_state, d_ret))) return rc;
@@ -3723,7 +3911,11 @@ static int envelope_search_launch(vb200_ctx *c, int nstreams, const void *d_pcm,
     const int ns = nsteps - j0 < chunk ? nsteps - j0 : chunk;
     const long items = per_step * ns;
     const int grid = grid_for(c, (int)((items + ENV_WARPS - 1) / ENV_WARPS), 16);
-    k_env_spectrum<<<grid, 32 * ENV_WARPS, 0, st>>>(c->env, src, nstreams, first_step + j0, ns, p_t, p_v);
+    if (d_first_per_stream)
+      k_env_spectrum_var<<<grid, 32 * ENV_WARPS, 0, st>>>(c->env, src, nstreams, j0, ns, p_t, p_v, d_first_per_stream,
+                                                          d_steps_per_stream);
+    else
+      k_env_spectrum<<<grid, 32 * ENV_WARPS, 0, st>>>(c->env, src, nstreams, first_step + j0, ns, p_t, p_v);
     if ((rc = post_launch(c))) return rc;
     k_env_filter<<<(nstreams + ENV_WARPS - 1) / ENV_WARPS, 32 * ENV_WARPS, 0, st>>>(
         c->env, nstreams, ch, ns, nsteps, j0, p_t, p_v, d_state, d_ret, d_steps_per_stream);
@@ -3734,7 +3926,8 @@ static int envelope_search_launch(vb200_ctx *c, int nstreams, const void *d_pcm,
 
 extern "C" int vb200_envelope_search_dev(vb200_ctx *c, int nstreams, const void *d_pcm, int fmt, int64_t stride,
                                          int first_step, int nsteps, int32_t *d_state, uint8_t *d_ret, void *stream) {
-  return envelope_search_launch(c, nstreams, d_pcm, fmt, stride, first_step, nsteps, d_state, d_ret, stream, nullptr);
+  return envelope_search_launch(c, nstreams, d_pcm, fmt, stride, first_step, nsteps, d_state, d_ret, stream, nullptr,
+                                nullptr);
 }
 
 static int envelope_search_host(vb200_ctx *c, int nstreams, const void *pcm, int fmt, int64_t stride,
@@ -3754,7 +3947,7 @@ static int envelope_search_host(vb200_ctx *c, int nstreams, const void *pcm, int
   if ((rc = io.h2d(state, st_bytes, &ds))) return rc;
   if ((rc = io.h2d(nullptr, (size_t)nstreams * nsteps, &dr))) return rc;
   if ((rc = envelope_search_launch(c, nstreams, dp, fmt, stride, first_step, nsteps, (int32_t *)ds, (uint8_t *)dr,
-                                   c->s_main, (const int32_t *)dn))) return rc;
+                                   c->s_main, (const int32_t *)dn, nullptr))) return rc;
   if ((rc = io.d2h(state, ds, st_bytes))) return rc;
   if ((rc = io.d2h(ret, dr, (size_t)nstreams * nsteps))) return rc;
   return io.sync();

@@ -11,11 +11,12 @@
 //  k_stream_gather    every block's vb200_packet_info (granulepos, e_o_s, packetno as vorbis_analysis_blockout
 //                     and vorbis_bitrate_flushpacket set them, lib/block.c:618-687, lib/bitrate.c:229-252) and the
 //                     chosen packet's bytes copied from its strided slot, cut at the truncation point or followed
-//                     by zero bytes of padding
+//                     by zero bytes of padding; k_stream_gather_carry the same for carried streams
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include "vorbis_b200.h"
+#include "vb200_streams.cuh"
 
 namespace vb200 {
 
@@ -183,9 +184,11 @@ struct GatherArgs {
   uint8_t *dst;
 };
 
-// one CTA per block in a grid-stride loop; info is always written, the bytes only when all of them fit cap
-__global__ void __launch_bounds__(256)
-k_stream_gather(GatherArgs A) {
+// one CTA per block in a grid-stride loop; info is always written, the bytes only when all of them fit cap.
+// CARRY: positions are relative to the call's buffer, which starts at timeline sample pc[s].base_in; packet numbers
+// continue from pc[s].packetno_in, and the last block's granulepos goes to the carry.
+template <bool CARRY>
+__device__ __forceinline__ void stream_gather_body(const GatherArgs &A, PlanCarry *pc) {
   const long long total = (long long)A.nstreams * A.max_blocks;
   const bool fits = A.off[total] <= A.cap;
   for (long long t = blockIdx.x; t < total; t += gridDim.x) {
@@ -206,21 +209,32 @@ k_stream_gather(GatherArgs A) {
     if (threadIdx.x == 0) {
       // vb->granulepos is v->granulepos when the block is cut: the sum of the moves so far (the block's centre
       // minus blocksizes[1]/2 on the timeline), clipped at the end of stream (lib/block.c:676-687)
-      const long long centre = (long long)b.pos + A.bs[b.W] / 2, half1 = A.bs[1] / 2;
+      const long long centre = (CARRY ? pc[s].base_in : 0) + (long long)b.pos + A.bs[b.W] / 2, half1 = A.bs[1] / 2;
       const long long e = A.eof ? (long long)A.eof[s] : 0;
       long long g = centre - half1;
       if (e > 0 && g > e - half1) g = e - half1;
       vb200_packet_info in;
       in.offset = o; in.granulepos = g; in.bytes = (int32_t)bytes;
       in.e_o_s = (e > 0 && centre >= e) ? 1 : 0;       // lib/block.c:649-655
-      in.packetno = 3 + k;                                // v->sequence starts at 3 (lib/block.c:311)
+      in.packetno = (CARRY ? pc[s].packetno_in : 3) + k;  // v->sequence starts at 3 (lib/block.c:311)
       in.choice = A.choice ? c : VB200_PACKETBLOBS / 2;
       A.info[t] = in;
+      if (CARRY && k == A.nblocks[s] - 1) pc[s].granulepos = g;
     }
     if (!fits) continue;
     const uint8_t *src = A.data[b.W] + ((long long)c * A.count[b.W] + b.slot) * A.stride[b.W];
     for (long long j = threadIdx.x; j < bytes; j += blockDim.x) A.dst[o + j] = j < natural ? src[j] : 0;
   }
+}
+
+__global__ void __launch_bounds__(256)
+k_stream_gather(GatherArgs A) {
+  stream_gather_body<false>(A, nullptr);
+}
+
+__global__ void __launch_bounds__(256)
+k_stream_gather_carry(GatherArgs A, PlanCarry *pc) {
+  stream_gather_body<true>(A, pc);
 }
 
 }  // namespace vb200

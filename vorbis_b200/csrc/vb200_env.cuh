@@ -3,6 +3,7 @@
 // k_env_spectrum   item = (stream, channel, step): squared-sine window, mdct_forward(128)
 //                  (lib/envelope.c:113-118), the near-DC energy `temp` (:125) and the 32 half-dB
 //                  pair powers (:147-149).  Independent items: one warp each, 4 warps per CTA.
+// k_env_spectrum_var  the same with a first step and a step count per stream (carried streams)
 // k_env_filter     everything of _ve_amp that carries state (near-DC running sum :124-145, spreading
 //                  and limiting :150-157, band amplitudes and the 17-deep amplitude history :162-203,
 //                  triggers :206-210) plus the stretch logic of _ve_envelope_search (:239-266).
@@ -29,9 +30,12 @@ constexpr int ENV_WARPS = 4;
 
 struct EnvSrc { const void *base; int fmt; long long stride; int ch; };
 
-__global__ void __launch_bounds__(32 * ENV_WARPS)
-k_env_spectrum(EnvDev E, EnvSrc src, int nstreams, int first_step, int nsteps,
-               float *__restrict__ temps, float *__restrict__ vals) {
+// VAR: stream s analyses steps first_ps[s] + first_step + j for j < count_ps[s] - first_step (first_step is the
+// chunk's offset then); items past a stream's count read its first samples and write nothing.
+template <bool VAR>
+__device__ __forceinline__ void env_spectrum_body(const EnvDev &E, const EnvSrc &src, int nstreams, int first_step,
+                                                  int nsteps, float *__restrict__ temps, float *__restrict__ vals,
+                                                  const int *__restrict__ first_ps, const int *__restrict__ count_ps) {
   __shared__ __align__(16) float s_in[ENV_WARPS][ENV_N];
   __shared__ __align__(16) float s_w[ENV_WARPS][ENV_N];
   __shared__ __align__(16) float s_out[ENV_WARPS][ENV_N / 2];
@@ -46,7 +50,13 @@ k_env_spectrum(EnvDev E, EnvSrc src, int nstreams, int first_step, int nsteps,
     if (!valid) item = items - 1;
     const int j = (int)(item % nsteps);
     const long sc = item / nsteps;                       // stream * ch + c
-    const long s0 = (long)ENV_STEP * (first_step + j);
+    long s0 = (long)ENV_STEP * (first_step + j);
+    bool store = valid;
+    if (VAR) {
+      const long sst = sc / src.ch;
+      store = valid && first_step + j < count_ps[sst];
+      s0 = store ? (long)ENV_STEP * (first_ps[sst] + first_step + j) : 0;
+    }
     if (src.fmt == VB200_PCM_S16_INTERLEAVED) {
       const long st = sc / src.ch; const int c = (int)(sc - st * src.ch);
       const short *p = reinterpret_cast<const short *>(src.base) + ((long long)st * src.stride + s0) * src.ch + c;
@@ -58,7 +68,7 @@ k_env_spectrum(EnvDev E, EnvSrc src, int nstreams, int first_step, int nsteps,
     __syncthreads();
     dev_mdct_forward<ENV_N>(E.X, s_in[wid], s_w[wid], s_out[wid], lane, 32);
     __syncthreads();
-    if (valid) {
+    if (VAR ? store : valid) {
       const float2 v = *reinterpret_cast<const float2 *>(&s_out[wid][2 * lane]);
       const float pw = v.x * v.x + v.y * v.y;
       vals[item * 32 + lane] = todB_dev(pw) * .5f;
@@ -70,6 +80,18 @@ k_env_spectrum(EnvDev E, EnvSrc src, int nstreams, int first_step, int nsteps,
     }
     __syncthreads();
   }
+}
+
+__global__ void __launch_bounds__(32 * ENV_WARPS)
+k_env_spectrum(EnvDev E, EnvSrc src, int nstreams, int first_step, int nsteps,
+               float *__restrict__ temps, float *__restrict__ vals) {
+  env_spectrum_body<false>(E, src, nstreams, first_step, nsteps, temps, vals, nullptr, nullptr);
+}
+
+__global__ void __launch_bounds__(32 * ENV_WARPS)
+k_env_spectrum_var(EnvDev E, EnvSrc src, int nstreams, int j0, int nsteps, float *__restrict__ temps,
+                   float *__restrict__ vals, const int *__restrict__ first_ps, const int *__restrict__ count_ps) {
+  env_spectrum_body<true>(E, src, nstreams, j0, nsteps, temps, vals, first_ps, count_ps);
 }
 
 __global__ void __launch_bounds__(32 * ENV_WARPS)

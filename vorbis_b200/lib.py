@@ -44,6 +44,8 @@ EXPORTS = [
     "vb200_encode_streams_managed_dev", "vb200_encode_streams_managed",
     "vb200_bitrate_setup", "vb200_bitrate_init", "vb200_bitrate_addblocks_dev", "vb200_bitrate_addblocks",
     "vb200_encode_streams_packets", "vb200_encode_streams_packets_managed",
+    "vb200_encode_carry_bytes", "vb200_encode_carry_init", "vb200_encode_streams_packets_resume",
+    "vb200_encode_streams_packets_managed_resume",
     "vb200_malloc_device", "vb200_free_device", "vb200_memcpy_h2d", "vb200_memcpy_d2h", "vb200_synchronize",
 ]
 
@@ -152,6 +154,12 @@ def load():
     L.vb200_bitrate_addblocks.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]
     L.vb200_encode_streams_packets.argtypes = [vp, C.c_int, C.c_int, C.POINTER(abi.StreamsIO), vp, vp, C.c_int64]
     L.vb200_encode_streams_packets_managed.argtypes = [vp, C.c_int, C.POINTER(abi.StreamsIO), vp, vp, C.c_int64]
+    L.vb200_encode_carry_bytes.argtypes = [vp, C.c_int]
+    L.vb200_encode_carry_init.argtypes = [vp, C.c_int, C.c_int, vp]
+    L.vb200_encode_streams_packets_resume.argtypes = [vp, C.c_int, C.c_int, C.POINTER(abi.StreamsIO), vp, vp, vp,
+                                                      C.c_int64]
+    L.vb200_encode_streams_packets_managed_resume.argtypes = [vp, C.c_int, C.POINTER(abi.StreamsIO), vp, vp, vp,
+                                                              C.c_int64]
     L.vb200_malloc_device.argtypes = [vp, C.c_size_t, C.POINTER(vp)]
     L.vb200_free_device.argtypes = [vp, vp]
     L.vb200_memcpy_h2d.argtypes = [vp, vp, vp, C.c_size_t]
@@ -843,11 +851,31 @@ class Context:
             self._chk(rc)
         return rc
 
+    def encode_carry_init(self, nstreams, mark_steps=0):
+        """vb200_encode_carry_init: fresh carries, uint8 [nstreams][vb200_encode_carry_bytes] (the managed form wants
+        them made after bitrate_setup); encode_carry_head(carry) reads their public heads"""
+        nbytes = self.L.vb200_encode_carry_bytes(self.h, mark_steps)
+        self._chk(min(nbytes, 0))
+        carry = np.zeros((nstreams, nbytes), np.uint8)
+        self._chk(self.L.vb200_encode_carry_init(self.h, nstreams, mark_steps, _ptr(carry)))
+        return carry
+
+    @staticmethod
+    def encode_carry_head(carry):
+        """the vb200_encode_carry heads of carries made by encode_carry_init (ENCODE_CARRY_HEAD_DTYPE [nstreams], a copy)"""
+        hs = abi.ENCODE_CARRY_HEAD_DTYPE.itemsize
+        return np.ascontiguousarray(carry[:, :hs]).view(abi.ENCODE_CARRY_HEAD_DTYPE)[:, 0]
+
+    def encode_streams_packets_resume(self, pcm, pcm_len, carry, eof=None, managed=False, **kw):
+        """vb200_encode_streams_packets[_managed]_resume: as encode_streams_packets, stream s's buffer starting at its
+        carry's base; carry (from encode_carry_init) is advanced in place when the call succeeds"""
+        return self.encode_streams_packets(pcm, pcm_len, eof, managed=managed, carry=carry, **kw)
+
     def encode_streams_packets(self, pcm, pcm_len, eof=None, fmt=PCM_F32_PLANAR, max_blocks=None, cap=None, blobno=7,
-                               managed=False, data_cap=None, check=True):
+                               managed=False, data_cap=None, check=True, carry=None):
         """vb200_encode_streams_packets[_managed] on timeline buffers as for encode_streams: {"plan", "nblocks",
         "count", "info" (PACKET_INFO_DTYPE [ns][max_blocks]), "data", "packets": per stream [bytes]} (and "rc" when
-        check is False, in which case an error does not raise and "packets" is absent)"""
+        check is False, in which case an error does not raise and "packets" is absent).  carry: the _resume forms"""
         ch = self.channels
         if fmt == PCM_F32_PLANAR:
             pcm = np.ascontiguousarray(pcm, np.float32)
@@ -875,7 +903,15 @@ class Context:
         if data_cap is None:
             data_cap = ns * max_blocks * max(self.packet_bound(0), self.packet_bound(1))
         data = np.zeros(max(data_cap, 1), np.uint8)
-        if managed:
+        if carry is not None:
+            assert carry.dtype == np.uint8 and carry.flags.c_contiguous and carry.shape[0] == ns
+            if managed:
+                rc = self.L.vb200_encode_streams_packets_managed_resume(self.h, ns, C.byref(io), _ptr(carry), _ptr(info),
+                                                                        _ptr(data), data_cap)
+            else:
+                rc = self.L.vb200_encode_streams_packets_resume(self.h, ns, blobno, C.byref(io), _ptr(carry), _ptr(info),
+                                                                _ptr(data), data_cap)
+        elif managed:
             rc = self.L.vb200_encode_streams_packets_managed(self.h, ns, C.byref(io), _ptr(info), _ptr(data), data_cap)
         else:
             rc = self.L.vb200_encode_streams_packets(self.h, ns, blobno, C.byref(io), _ptr(info), _ptr(data), data_cap)
