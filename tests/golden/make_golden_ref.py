@@ -229,12 +229,22 @@ def main():
               plan_cases, streams_cases):
         f()
         print(f.__name__, "done")
-    for f in glob.glob(os.path.join(REF, "*.npz")):
-        os.remove(f)
     for group, arrays in GROUPS.items():
         cases = {}
         for k, v in arrays.items():
             cases.setdefault(k.split("__", 1)[0], {})[k] = v
+        # cases already stored stay in their files, which must hold exactly what was just computed; new cases go
+        # to new files after the group's last one, so that adding a case never rewrites a stored fixture
+        files = sorted(glob.glob(os.path.join(REF, group + ".npz")) + glob.glob(os.path.join(REF, group + "-*.npz")))
+        for f in files:
+            with np.load(f) as z:
+                stored = {k: z[k] for k in z.files}
+            for case in {k.split("__", 1)[0] for k in stored}:
+                got = cases.pop(case, None)
+                assert got is not None, "%s: case %s is no longer computed" % (f, case)
+                want = {k: v for k, v in stored.items() if k.split("__", 1)[0] == case}
+                assert got.keys() == want.keys() and all(np.array_equal(got[k], want[k]) for k in want), \
+                    "%s: case %s changed" % (f, case)
         shards, cur = [], {}
         for c in cases.values():
             buf = io.BytesIO()
@@ -243,8 +253,9 @@ def main():
                 shards.append(cur)
                 cur = {}
             cur.update(c)
-        for i, s in enumerate(shards + [cur]):
-            np.savez_compressed(os.path.join(REF, group + ("-%d" % i if i else "") + ".npz"), **s)
+        first = len(files)
+        for i, s in enumerate(shards + [cur] if cur else []):
+            np.savez_compressed(os.path.join(REF, group + ("-%d" % (first + i) if first + i else "") + ".npz"), **s)
 
 
 if __name__ == "__main__":
