@@ -674,6 +674,59 @@ int vb200_decode_packets_resume    (vb200_ctx*, int nstreams, int nblk, const in
                                     const int64_t *pcm_off, void *pcm, int pcm_s16, int64_t pcm_stride,
                                     vb200_decode_carry *carry);
 
+/* ---- whole streams from packets: what a stock decoder's vorbis_synthesis -> vorbis_synthesis_blockin ->
+ * vorbis_synthesis_pcmout loop (examples/decoder_example.c) returns, for many streams in one call, on the device:
+ * the packet headers, the drops, the entropy decode, mapping0_inverse's DSP, the overlap-add and blockin's sample
+ * bookkeeping (lib/block.c:741-751, 835-941), with the PCM packed in stream order.
+ *   npkt  [nstreams]: stream s passes npkt[s] (0..max_packets) packets, info[s*max_packets + k] for k < npkt[s]:
+ *         data[offset .. offset+bytes) with granulepos, e_o_s and packetno as an ogg_packet carries them; choice is
+ *         not read.  The layout vb200_encode_streams_packets returns, so its info and data can be passed straight in.
+ *   carry [nstreams][vb200_decode_streams_carry_bytes], device memory in both forms: one decoder's state per stream
+ *         (the overlap tail of every channel, the last block flag, v->sequence, v->granulepos, b->sample_count, and
+ *         the mode, full or half rate, it belongs to).  vb200_decode_streams_carry_init is vorbis_synthesis_restart
+ *         for nstreams consecutive carries (pass one stream's slot to restart that stream); it is synchronous.
+ *   pcm_base [nstreams + 1] int64: stream s returns n_s = pcm_base[s+1] - pcm_base[s] samples at pcm + pcm_base[s]*ch,
+ *         planar float [ch][n_s], or with pcm_s16 interleaved int16 [n_s][ch] converted as decoder_example does
+ *         (floor(x*32767.f+.5f) clipped).  The samples are those the pcmout loop returns after each blockin, in order.
+ *   out   [nstreams][max_packets]: packet k of stream s (entries past npkt[s] are not written).
+ * The packet header is parsed as vorbis_synthesis parses it (lib/synthesis.c:41-71), with the mode layout of the
+ * entropy setup: modes 0 and 1 have block flags 0 and 1.  A packet whose type bit is not 0 (an empty packet too) is
+ * dropped as OV_ENOTAUDIO, a mode number >= 2 or a long block without its nW bit as OV_EBADPACKET; a dropped packet
+ * changes nothing, so the next one sees a packetno gap as the stock decoder does.  Truncated and damaged packets
+ * past the header decode as the reference decodes them.
+ * When pcm_base[nstreams]*ch > pcm_cap (elements), no PCM is written and every carry stays as it was; pcm_base and
+ * out are still filled, and the host form returns VB200_EINVAL.  sum(npkt[s]) * ((blocksizes[1]/2) >> halfrate)
+ * samples per channel never overflow.
+ * Contract: any cut of a stream's packets into calls that pass the carry along gives the PCM, out and pcm_base of
+ * one call, byte for byte (calls with no packets for some streams included); fed a stock decoder's packets the
+ * result is that decoder's pcmout sequence, bit for bit.  Full rate, and half rate after vb200_synthesis_halfrate.
+ * Needs a registered vb200_decode_entropy_setup (else VB200_EINVAL).  Five kernel launches per call, whatever
+ * nstreams and the packet counts: header parse, per-stream plan, prefix scan, entropy decode + DSP, synthesis.
+ * Device scratch (arena of its own, carved once per call): nstreams*max_packets*(ch*blocksizes[1]/2 floats of
+ * residue + 48 bytes of tables) + nstreams*48 bytes.
+ * _dev: every pointer is device memory; checks its pointers only.  Host form: host buffers except the carry;
+ * returns VB200_EINVAL for null pointers, max_packets < 1, npkt[s] outside [0, max_packets], a packet outside
+ * data (data_bytes), and a carry of the other rate mode (or not written by carry_init).                         */
+typedef struct vb200_decoded_packet {
+  int64_t pcm_offset;   /* first sample of this packet's PCM within stream s's output of this call */
+  int64_t granulepos;   /* v->granulepos after this packet's blockin; -1 = not known */
+  int32_t samples;      /* what vorbis_synthesis_pcmout returns after this packet's blockin */
+  int32_t status;       /* 0, or VB200_ENOTAUDIO / VB200_EBADPACKET where vorbis_synthesis rejects it (dropped) */
+} vb200_decoded_packet;
+#define VB200_ENOTAUDIO  (-135)   /* OV_ENOTAUDIO  */
+#define VB200_EBADPACKET (-136)   /* OV_EBADPACKET */
+struct vb200_packet_info;         /* defined with vb200_encode_streams_packets below */
+int vb200_decode_streams_carry_bytes(vb200_ctx*);
+int vb200_decode_streams_carry_init (vb200_ctx*, int nstreams, void *d_carry);
+int vb200_decode_streams_packets_dev(vb200_ctx*, int nstreams, int max_packets, const int32_t *d_npkt,
+                                     const struct vb200_packet_info *d_info, const uint8_t *d_data, void *d_carry,
+                                     int pcm_s16, void *d_pcm, int64_t pcm_cap, int64_t *d_pcm_base,
+                                     vb200_decoded_packet *d_out, void *stream);
+int vb200_decode_streams_packets    (vb200_ctx*, int nstreams, int max_packets, const int32_t *npkt,
+                                     const struct vb200_packet_info *info, const uint8_t *data, int64_t data_bytes,
+                                     void *d_carry, int pcm_s16, void *pcm, int64_t pcm_cap, int64_t *pcm_base,
+                                     vb200_decoded_packet *out);
+
 /* ---- encode: the entropy coding of mapping0_forward (lib/mapping0.c:596-687) on the device, un-managed bitrate.
  * What floor1_encode (lib/floor1.c:753-921) and the residue class / forward of types 1 and 2 (lib/res0.c:534-648,
  * 725-809) read, registered on a context with vb200_encode_entropy_setup.

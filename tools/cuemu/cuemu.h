@@ -263,6 +263,11 @@ template <class T> static inline cudaError_t cudaMallocHost(T **p, size_t n) { r
 static inline cudaError_t cudaFreeHost(void *p) { free(p); return cudaSuccess; }
 static inline cudaError_t cudaMemcpy(void *d, const void *s, size_t n, cudaMemcpyKind) { memmove(d, s, n); return cudaSuccess; }
 static inline cudaError_t cudaMemcpyAsync(void *d, const void *s, size_t n, cudaMemcpyKind, cudaStream_t = nullptr) { memmove(d, s, n); return cudaSuccess; }
+static inline cudaError_t cudaMemcpy2DAsync(void *d, size_t dp, const void *s, size_t sp, size_t w, size_t h,
+                                            cudaMemcpyKind, cudaStream_t = nullptr) {
+  for (size_t r = 0; r < h; r++) memmove((char *)d + r * dp, (const char *)s + r * sp, w);
+  return cudaSuccess;
+}
 static inline cudaError_t cudaMemset(void *d, int v, size_t n) { memset(d, v, n); return cudaSuccess; }
 static inline cudaError_t cudaMemsetAsync(void *d, int v, size_t n, cudaStream_t = nullptr) { memset(d, v, n); return cudaSuccess; }
 static inline cudaError_t cudaStreamCreateWithFlags(cudaStream_t *s, unsigned) { *s = (cudaStream_t)malloc(8); return cudaSuccess; }

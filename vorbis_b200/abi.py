@@ -205,6 +205,9 @@ assert C.sizeof(BitrateInfo) == 48 and BITRATE_STATE_DTYPE.itemsize == 32 and PA
 # vb200_encode_carry: the public head of every stream's carry ([nstreams][vb200_encode_carry_bytes] bytes)
 ENCODE_CARRY_HEAD_DTYPE = np.dtype([("base", "<i8"), ("granulepos", "<i8"), ("packetno", "<i4"), ("done", "<i4")])
 assert ENCODE_CARRY_HEAD_DTYPE.itemsize == 24
+# vb200_decoded_packet: what vb200_decode_streams_packets reports for every packet it was given
+DECODED_PACKET_DTYPE = np.dtype([("pcm_offset", "<i8"), ("granulepos", "<i8"), ("samples", "<i4"), ("status", "<i4")])
+assert DECODED_PACKET_DTYPE.itemsize == 24
 
 
 class Codebook(C.Structure):

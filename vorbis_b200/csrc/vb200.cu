@@ -26,6 +26,7 @@
 #include "vb200_managed.cuh"
 #include "vb200_entropy_enc.cuh"
 #include "vb200_bitrate.cuh"
+#include "vb200_decode_streams.cuh"
 #include "floor1_db_table.h"
 
 using namespace vb200;
@@ -97,8 +98,10 @@ struct vb200_ctx {
   //   spk       vb200_encode_streams_packets[_managed]: strided packets and bit counts of both sizes, the stream-order
   //             tables, offsets, packet infos and the packed bytes
   //   brc       the host form of vb200_bitrate_addblocks
+  //   dsk       vb200_decode_streams_packets[_dev]: the packet headers, the block tables, the per-stream plan and the
+  //             residue scratch, sized by nstreams x max_packets
   DevBuf stage[STAGE_SLOTS], cycles, phaseA, lane[2], enc, set[ENC_SETS], mgd, plan, chain, env_scratch, coder, pack,
-      spk, brc;
+      spk, brc, dsk;
   cudaStream_t s_pipe[2] = {nullptr, nullptr};
   const ResDev *d_res[2] = {nullptr, nullptr};        // [VB200_MAX_SUBMAPS] residue class parameters per block size
   int res_partvals[2] = {0, 0};
@@ -932,38 +935,49 @@ struct SinkS16 {
   }
 };
 
+// TRIM (vb200_decode_streams_packets): as CARRY, with the carry of stream st in its slot of T.carry and the carried
+// flag from T.W_in (what k_ds_plan read before anything wrote the heads); block k writes only [lo, hi) = T.win of
+// its finished samples, from pcm_off (relative to the stream's pcm_base) on, into the packed layout of the call.
+// Nothing is written, carries included, when the call's output does not fit T.cap.  Channel 0 commits the head.
 // CARRY (vb200_decode_dsp_resume): stream st decodes count[st] <= nblk blocks, and the overlap of every
 // (stream, channel) = task comes from / goes back to carry_W[task] and carry_tail[task * tail_stride]: the
 // block flag and the right half of the last IMDCT (what v->pcm holds after lib/block.c:817-823).  With a
 // carried W >= 0, block 0 overlap-adds onto that tail and finishes samples like any later block; with -1 it
 // only primes.  A stream with count 0 is not touched.  W is kept per (stream, channel) because the CTA of
 // one channel must not read what the CTA of another channel of the same stream writes.
-template <bool S16, bool HS, bool CARRY>
+template <bool S16, bool HS, bool CARRY, bool TRIM = false>
 __device__ __forceinline__ void
 synthesis_body(const XformDev &X0, const XformDev &X1, const WinDev &Wd, int ch, int nstreams, int nblk,
                const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
                const float *__restrict__ coef, const long long *__restrict__ pcm_off,
                void *__restrict__ pcm_out, long long pcm_stride, const int *__restrict__ count,
-               float *__restrict__ carry_tail, int *__restrict__ carry_W, int tail_stride) {
+               float *__restrict__ carry_tail, int *__restrict__ carry_W, int tail_stride,
+               const DsTrim &T = DsTrim{}) {
   extern __shared__ __align__(16) float sm[];
   const int tid = threadIdx.x, nt = blockDim.x;
   const int n0 = X0.N >> 1, n1 = X1.N >> 1;
   float *s_in = sm, *s_out = sm + n1, *s_prev = s_out + 2 * n1;
   const float *w0 = Wd.win[0], *w1 = Wd.win[1];
   const int off = n1 / 2 - n0 / 2;
+  if constexpr (TRIM)
+    if (T.base[nstreams] * ch > T.cap) return;
   for (int task = blockIdx.x; task < nstreams * ch; task += gridDim.x) {
     const int st = task / ch, c = task - st * ch;
     int lW = 0;
     int cnt = nblk, first_out = 1;
-    if constexpr (CARRY) {
+    if constexpr (CARRY || TRIM) {
       if (count) cnt = min(max(count[st], 0), nblk);
       if (cnt == 0) continue;
-      const int cw = carry_W[task];
+      int cw;
+      if constexpr (TRIM) cw = T.W_in[st];
+      else cw = carry_W[task];
       if (cw >= 0) {
         // the loads finish before block 0's first __syncthreads; s_prev is read only after it
         lW = cw ? 1 : 0;
         first_out = 0;
-        const float *t = carry_tail + (size_t)task * tail_stride;
+        const float *t;
+        if constexpr (TRIM) t = T.tail(st, c);
+        else t = carry_tail + (size_t)task * tail_stride;
         for (int i = tid; i < ((lW ? X1.N : X0.N) >> 1); i += nt) s_prev[i] = t[i];
       }
     }
@@ -978,8 +992,19 @@ synthesis_body(const XformDev &X0, const XformDev &X1, const WinDev &Wd, int ch,
       dev_mdct_backward<0>(X, s_in, s_out, tid, nt);
       if (k >= first_out) {
         const long long o = pcm_off[(size_t)st * nblk + k];
-        typename std::conditional<S16, SinkS16, SinkF32>::type dst;
-        if constexpr (S16) {
+        using Base = typename std::conditional<S16, SinkS16, SinkF32>::type;
+        typename std::conditional<TRIM, SinkTrim<Base>, Base>::type dst;
+        if constexpr (TRIM) {
+          const int2 w = T.win[(size_t)st * nblk + k];
+          const long long b = T.base[st];
+          dst.lo = w.x; dst.hi = w.y;
+          if constexpr (S16) {
+            dst.b.p = reinterpret_cast<short *>(pcm_out) + (b + o) * ch + c;
+            dst.b.ch = ch;
+          } else {
+            dst.b.p = reinterpret_cast<float *>(pcm_out) + b * ch + (T.base[st + 1] - b) * c + o;
+          }
+        } else if constexpr (S16) {
           dst.p = reinterpret_cast<short *>(pcm_out) + ((long long)st * pcm_stride + o) * ch + c;
           dst.ch = ch;
         } else {
@@ -1003,10 +1028,16 @@ synthesis_body(const XformDev &X0, const XformDev &X1, const WinDev &Wd, int ch,
       lW = W;
       __syncthreads();
     }
-    if constexpr (CARRY) {
-      float *t = carry_tail + (size_t)task * tail_stride;
+    if constexpr (CARRY || TRIM) {
+      float *t;
+      if constexpr (TRIM) t = T.tail(st, c);
+      else t = carry_tail + (size_t)task * tail_stride;
       for (int i = tid; i < ((lW ? X1.N : X0.N) >> 1); i += nt) t[i] = s_prev[i];
-      if (tid == 0) carry_W[task] = lW;
+      if constexpr (TRIM) {
+        if (tid == 0 && c == 0) *T.carried(st) = T.head[st];
+      } else {
+        if (tid == 0) carry_W[task] = lW;
+      }
       __syncthreads();                 // the next task's carry-in overwrites s_prev
     }
   }
@@ -1031,6 +1062,16 @@ k_synthesis_carry(XformDev X0, XformDev X1, WinDev Wd, int ch, int nstreams, int
                   float *__restrict__ carry_tail, int *__restrict__ carry_W, int tail_stride) {
   synthesis_body<S16, HS, true>(X0, X1, Wd, ch, nstreams, nblk, Wseq, coef_off, coef, pcm_off, pcm_out, pcm_stride,
                                 count, carry_tail, carry_W, tail_stride);
+}
+
+template <bool S16, bool HS>
+__global__ void __launch_bounds__(256)
+k_synthesis_trim(XformDev X0, XformDev X1, WinDev Wd, int ch, int nstreams, int nblk,
+                 const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
+                 const float *__restrict__ coef, const long long *__restrict__ pcm_off,
+                 void *__restrict__ pcm_out, const int *__restrict__ count, DsTrim T) {
+  synthesis_body<S16, HS, false, true>(X0, X1, Wd, ch, nstreams, nblk, Wseq, coef_off, coef, pcm_off, pcm_out, 0,
+                                       count, nullptr, nullptr, T.tail_stride, T);
 }
 
 // ---- decode: undo channel coupling, lib/mapping0.c:754-779 (square polar -> L/R), in place
@@ -3139,6 +3180,157 @@ extern "C" int vb200_decode_packets_resume(vb200_ctx *c, int nstreams, int nblk,
   if ((rc = io.d2h(pcm, dp, pbytes))) return rc;
   if ((rc = io.d2h(carry->tail, dkt, tbytes))) return rc;
   if ((rc = io.d2h(carry->W, dkw, sizeof(int32_t) * ntask))) return rc;
+  return io.sync();
+}
+
+// ---- whole streams from packets (vb200_decode_streams.cuh): header parse, per-stream plan, prefix scan, then the
+// fused entropy decode and the trimming synthesis on the plan's tables.  A stream's carry is a DsHead, then the
+// overlap tail of each channel.
+static size_t ds_carry_bytes(const vb200_ctx *c) {
+  return DS_HEAD_BYTES + sizeof(float) * (size_t)c->setup.channels * (c->setup.blocksizes[1] / 2);
+}
+
+extern "C" int vb200_decode_streams_carry_bytes(vb200_ctx *c) {
+  if (!c) return fail(VB200_EINVAL, "null context");
+  return (int)ds_carry_bytes(c);
+}
+
+extern "C" int vb200_decode_streams_carry_init(vb200_ctx *c, int nstreams, void *d_carry) {
+  CHECK_CTX(c);
+  if (nstreams <= 0) return 0;
+  if (!d_carry) return fail(VB200_EINVAL, "null carry");
+  DsHead h{};
+  h.granulepos = -1; h.sample_count = -1; h.sequence = -1; h.W = -1;
+  h.rate = c->halfrate ? DS_RATE_HALF : DS_RATE_FULL;
+  const size_t B = ds_carry_bytes(c);
+  std::vector<DsHead> heads((size_t)nstreams, h);
+  CU(cudaMemcpy2DAsync(d_carry, B, heads.data(), sizeof(DsHead), sizeof(DsHead), (size_t)nstreams,
+                       cudaMemcpyHostToDevice, c->s_main));
+  CU(cudaStreamSynchronize(c->s_main));
+  return 0;
+}
+
+template <bool S16, bool HS>
+static int synthesis_trim_launch(vb200_ctx *c, int nstreams, int nblk, const int32_t *d_count, const int32_t *d_Wseq,
+                                 const long long *d_coef_off, const float *d_coef, const long long *d_pcm_off,
+                                 void *d_pcm, const DsTrim &T, cudaStream_t st) {
+  const XformDev *X = HS ? c->dx_hs : c->dx;
+  const int ch = c->setup.channels, N1 = X[1].N;
+  const size_t smem = sizeof(float) * ((size_t)N1 / 2 + N1 + N1 / 2);
+  int rc = set_smem(k_synthesis_trim<S16, HS>, smem); if (rc) return rc;
+  k_synthesis_trim<S16, HS><<<grid_for(c, nstreams * ch, 8), threads_for(N1), smem, st>>>(
+      X[0], X[1], HS ? c->dwin_hs : c->dwin, ch, nstreams, nblk, d_Wseq, d_coef_off, d_coef, d_pcm_off, d_pcm,
+      d_count, T);
+  return post_launch(c);
+}
+
+extern "C" int vb200_decode_streams_packets_dev(vb200_ctx *c, int nstreams, int max_packets, const int32_t *d_npkt,
+                                                const vb200_packet_info *d_info, const uint8_t *d_data, void *d_carry,
+                                                int pcm_s16, void *d_pcm, int64_t pcm_cap, int64_t *d_pcm_base,
+                                                vb200_decoded_packet *d_out, void *stream) {
+  CHECK_CTX(c);
+  if (nstreams <= 0) return 0;
+  if (max_packets < 1) return fail(VB200_EINVAL, "max_packets must be >= 1");
+  if (!d_npkt || !d_info || !d_data || !d_carry || !d_pcm || !d_pcm_base || !d_out)
+    return fail(VB200_EINVAL, "decode streams pointers");
+  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
+  const long long n = (long long)nstreams * max_packets;
+  if (n > INT32_MAX) return fail(VB200_EINVAL, "nstreams * max_packets must fit an int");
+  const int ch = c->setup.channels;
+  const bool hs = c->halfrate;
+  const cudaStream_t st = (cudaStream_t)stream;
+  DsPlanArgs P;
+  float *res;
+  int rc;
+  if ((rc = carve(c->dsk, [&](Carve &k) {
+         P.Wseq = k.take<int>(n); P.pkt_bytes = k.take<int>(n); P.pkt_off = k.take<long long>(n);
+         P.coef_off = k.take<long long>(n); P.pcm_off = k.take<long long>(n); P.win = k.take<int2>(n);
+         P.count = k.take<int>(nstreams); P.W_in = k.take<int>(nstreams); P.head = k.take<DsHead>(nstreams);
+         res = k.take<float>(n * ch * (c->setup.blocksizes[1] / 2));
+       }))) return rc;
+  int *hdr = P.Wseq;                     // k_ds_plan reads slot k's header before it writes block j <= k there
+  P.nstreams = nstreams; P.max_packets = max_packets; P.ch = ch; P.hs = hs ? 1 : 0;
+  P.bs[0] = c->setup.blocksizes[0]; P.bs[1] = c->setup.blocksizes[1];
+  P.npkt = d_npkt; P.info = d_info; P.hdr = hdr; P.carry = (const unsigned char *)d_carry;
+  P.carry_bytes = (long long)ds_carry_bytes(c); P.pcm_base = (long long *)d_pcm_base; P.out = d_out;
+  if ((rc = scratch_begin(c, st))) return rc;
+  k_ds_header<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(nstreams, max_packets, c->ent.modebits, d_npkt, d_info,
+                                                             d_data, hdr);
+  if ((rc = post_launch(c))) return rc;
+  k_ds_plan<<<(nstreams + 127) / 128, 128, 0, st>>>(P);
+  if ((rc = post_launch(c))) return rc;
+  k_ds_scan<<<1, 1024, 0, st>>>(nstreams, (long long *)d_pcm_base);
+  if ((rc = post_launch(c))) return rc;
+  DecodePrepArgs A;
+  if ((rc = decode_prep_args(c, nstreams, max_packets, &A))) return rc;
+  const DecodePackets DP{P.pkt_off, P.pkt_bytes, d_data};
+  if ((rc = set_smem(k_decode_packets<true>, entropy_smem(c->ent, true)))) return rc;
+  k_decode_packets<true><<<grid_for(c, (int)n, DECODE_PACKETS_CTAS), 128, entropy_smem(c->ent, true), st>>>(
+      A, c->ent, DP, P.Wseq, P.coef_off, res, c->d_fromdB, P.count);
+  if ((rc = post_launch(c))) return rc;
+  DsTrim T;
+  T.win = P.win; T.base = P.pcm_base; T.W_in = P.W_in; T.head = P.head; T.carry = (unsigned char *)d_carry;
+  T.carry_bytes = P.carry_bytes; T.cap = pcm_cap; T.tail_stride = c->setup.blocksizes[1] / 2;
+  if (pcm_s16)
+    rc = hs ? synthesis_trim_launch<true, true>(c, nstreams, max_packets, P.count, P.Wseq, P.coef_off, res, P.pcm_off, d_pcm, T, st)
+            : synthesis_trim_launch<true, false>(c, nstreams, max_packets, P.count, P.Wseq, P.coef_off, res, P.pcm_off, d_pcm, T, st);
+  else
+    rc = hs ? synthesis_trim_launch<false, true>(c, nstreams, max_packets, P.count, P.Wseq, P.coef_off, res, P.pcm_off, d_pcm, T, st)
+            : synthesis_trim_launch<false, false>(c, nstreams, max_packets, P.count, P.Wseq, P.coef_off, res, P.pcm_off, d_pcm, T, st);
+  if (rc) return rc;
+  return scratch_end(c, st);
+}
+
+extern "C" int vb200_decode_streams_packets(vb200_ctx *c, int nstreams, int max_packets, const int32_t *npkt,
+                                            const vb200_packet_info *info, const uint8_t *data, int64_t data_bytes,
+                                            void *d_carry, int pcm_s16, void *pcm, int64_t pcm_cap, int64_t *pcm_base,
+                                            vb200_decoded_packet *out) {
+  CHECK_CTX(c);
+  if (nstreams <= 0) return 0;
+  if (max_packets < 1) return fail(VB200_EINVAL, "max_packets must be >= 1");
+  if (!npkt || !info || !data || !d_carry || !pcm || !pcm_base || !out || data_bytes < 0 || pcm_cap < 0)
+    return fail(VB200_EINVAL, "decode streams pointers");
+  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
+  const size_t n = (size_t)nstreams * max_packets;
+  for (int s = 0; s < nstreams; s++) {
+    if (npkt[s] < 0 || npkt[s] > max_packets) return fail(VB200_EINVAL, "npkt[s] must be in [0, max_packets]");
+    for (int k = 0; k < npkt[s]; k++) {
+      const vb200_packet_info &p = info[(size_t)s * max_packets + k];
+      if (p.offset < 0 || p.bytes < 0 || p.offset > data_bytes - p.bytes) return fail(VB200_EINVAL, "packet outside data");
+    }
+  }
+  std::lock_guard<std::mutex> lk(c->mu);
+  const size_t B = ds_carry_bytes(c);
+  std::vector<DsHead> heads((size_t)nstreams);
+  CU(cudaMemcpy2DAsync(heads.data(), sizeof(DsHead), d_carry, B, sizeof(DsHead), (size_t)nstreams,
+                       cudaMemcpyDeviceToHost, c->s_main));
+  CU(cudaStreamSynchronize(c->s_main));
+  const int rate = c->halfrate ? DS_RATE_HALF : DS_RATE_FULL;
+  for (const DsHead &h : heads)
+    if (h.rate != rate || h.W < -1 || h.W > 1)
+      return fail(VB200_EINVAL, "carry not initialised for this context's rate mode (vb200_decode_streams_carry_init)");
+  const int ch = c->setup.channels;
+  const size_t el = pcm_s16 ? sizeof(int16_t) : sizeof(float);
+  HostIO io{c};
+  void *dn, *di, *dd, *dp, *db, *dout;
+  int rc;
+  if ((rc = io.h2d(npkt, sizeof(int32_t) * nstreams, &dn))) return rc;
+  if ((rc = io.h2d(info, sizeof(vb200_packet_info) * n, &di))) return rc;
+  if ((rc = io.h2d(nullptr, (size_t)data_bytes + 1, &dd))) return rc;
+  if (data_bytes) CU(cudaMemcpyAsync(dd, data, (size_t)data_bytes, cudaMemcpyHostToDevice, c->s_main));
+  if ((rc = io.h2d(nullptr, el * (size_t)std::max<int64_t>(pcm_cap, 1), &dp))) return rc;
+  if ((rc = io.h2d(nullptr, sizeof(int64_t) * (nstreams + 1), &db))) return rc;
+  if ((rc = io.h2d(nullptr, sizeof(vb200_decoded_packet) * n, &dout))) return rc;
+  if ((rc = vb200_decode_streams_packets_dev(c, nstreams, max_packets, (const int32_t *)dn,
+                                             (const vb200_packet_info *)di, (const uint8_t *)dd, d_carry, pcm_s16, dp,
+                                             pcm_cap, (int64_t *)db, (vb200_decoded_packet *)dout, c->s_main)))
+    return rc;
+  if ((rc = io.d2h(pcm_base, db, sizeof(int64_t) * (nstreams + 1)))) return rc;
+  if ((rc = io.d2h(out, dout, sizeof(vb200_decoded_packet) * n))) return rc;
+  if ((rc = io.sync())) return rc;
+  const int64_t total = pcm_base[nstreams] * ch;
+  if (total > pcm_cap) return fail(VB200_EINVAL, "the PCM does not fit pcm_cap (pcm_base is filled)");
+  if (total && (rc = io.d2h(pcm, dp, el * (size_t)total))) return rc;
   return io.sync();
 }
 

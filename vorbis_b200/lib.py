@@ -37,6 +37,8 @@ EXPORTS = [
     "vb200_decode_dsp_resume_dev", "vb200_decode_dsp_resume",
     "vb200_decode_entropy_setup", "vb200_decode_entropy_dev", "vb200_decode_entropy",
     "vb200_decode_packets_resume_dev", "vb200_decode_packets_resume",
+    "vb200_decode_streams_carry_bytes", "vb200_decode_streams_carry_init", "vb200_decode_streams_packets_dev",
+    "vb200_decode_streams_packets",
     "vb200_encode_entropy_setup", "vb200_encode_packet_bound", "vb200_encode_entropy_dev", "vb200_encode_entropy",
     "vb200_encode_packets", "vb200_encode_entropy_managed_dev", "vb200_encode_packets_managed",
     "vb200_residue_partvals", "vb200_residue_classify_dev", "vb200_residue_classify",
@@ -129,6 +131,12 @@ def load():
                                                   C.c_int64, C.POINTER(abi.DecodeCarry), vp]
     L.vb200_decode_packets_resume.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, C.c_int64, vp, vp, vp, C.c_int64, vp,
                                               vp, C.c_int, C.c_int64, C.POINTER(abi.DecodeCarry)]
+    L.vb200_decode_streams_carry_bytes.argtypes = [vp]
+    L.vb200_decode_streams_carry_init.argtypes = [vp, C.c_int, vp]
+    L.vb200_decode_streams_packets_dev.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int, vp, C.c_int64, vp,
+                                                   vp, vp]
+    L.vb200_decode_streams_packets.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, C.c_int64, vp, C.c_int, vp,
+                                               C.c_int64, vp, vp]
     L.vb200_encode_entropy_setup.argtypes = [vp, C.POINTER(abi.EncodeEntropySetup)]
     L.vb200_encode_packet_bound.argtypes = [vp, C.c_int]
     L.vb200_encode_entropy_dev.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int64, vp, vp, vp]
@@ -682,6 +690,54 @@ class Context:
                                                          _ptr(d_pcm), pcm_s16, pcm_stride, C.byref(k),
                                                          _ptr(stream)))
 
+    # ---- whole streams from packets ----------------------------------------------------------------
+    def decode_streams_carry(self, nstreams):
+        """fresh decoder carries for decode_streams_packets, in device memory (a DecodeStreamsCarry)"""
+        nbytes = self.L.vb200_decode_streams_carry_bytes(self.h)
+        self._chk(min(nbytes, 0))
+        carry = DecodeStreamsCarry(self, nstreams, nbytes)
+        self.decode_streams_carry_init(carry)
+        return carry
+
+    def decode_streams_carry_init(self, carry, stream=None):
+        """vb200_decode_streams_carry_init (vorbis_synthesis_restart) on every carry, or on stream `stream`'s only"""
+        if stream is None:
+            self._chk(self.L.vb200_decode_streams_carry_init(self.h, carry.nstreams, carry.ptr))
+        else:
+            assert 0 <= stream < carry.nstreams
+            self._chk(self.L.vb200_decode_streams_carry_init(self.h, 1, carry.ptr + stream * carry.nbytes))
+
+    def decode_streams_packets(self, npkt, info, data, carry, s16=False, pcm_cap=None, check=True):
+        """vb200_decode_streams_packets: npkt [nstreams], info PACKET_INFO_DTYPE [nstreams][max_packets], data uint8;
+        carry from decode_streams_carry, advanced in place.  pcm_cap (elements) defaults to the bound
+        sum(npkt) * (blocksizes[1]/2 >> halfrate) * ch.  Returns {"pcm_base", "out" (DECODED_PACKET_DTYPE, shaped as
+        info), "pcm": per stream float [ch][n_s] or int16 [n_s][ch], "rc"}; check: raise on an error"""
+        npkt = np.ascontiguousarray(npkt, np.int32)
+        info = np.ascontiguousarray(info, abi.PACKET_INFO_DTYPE)
+        data = np.ascontiguousarray(data, np.uint8)
+        ns, mp = info.shape
+        ch = self.channels
+        if pcm_cap is None:
+            pcm_cap = int(npkt.sum()) * ((self.bs[1] // 2) >> self.halfrate) * ch
+        pcm = np.zeros(max(pcm_cap, 1), np.int16 if s16 else np.float32)
+        base = np.zeros(ns + 1, np.int64)
+        out = np.zeros((ns, mp), abi.DECODED_PACKET_DTYPE)
+        rc = self.L.vb200_decode_streams_packets(self.h, ns, mp, _ptr(npkt), _ptr(info), _ptr(data), data.size,
+                                                 carry.ptr, 1 if s16 else 0, _ptr(pcm), pcm_cap, _ptr(base), _ptr(out))
+        if check:
+            self._chk(rc)
+        res = {"pcm_base": base, "out": out, "rc": rc}
+        if rc == 0:
+            res["pcm"] = [pcm[base[s] * ch:base[s + 1] * ch].reshape(-1, ch) if s16
+                          else pcm[base[s] * ch:base[s + 1] * ch].reshape(ch, -1) for s in range(ns)]
+        return res
+
+    def decode_streams_packets_dev(self, nstreams, max_packets, d_npkt, d_info, d_data, d_carry, pcm_s16, d_pcm,
+                                   pcm_cap, d_pcm_base, d_out, stream=None):
+        self._chk(self.L.vb200_decode_streams_packets_dev(self.h, nstreams, max_packets, _ptr(d_npkt), _ptr(d_info),
+                                                          _ptr(d_data), _ptr(d_carry), pcm_s16, _ptr(d_pcm), pcm_cap,
+                                                          _ptr(d_pcm_base), _ptr(d_out), _ptr(stream)))
+
     # ---- encode: the entropy coding of mapping0_forward on the device -----------------------------
     def encode_entropy_setup(self, es):
         """vb200_encode_entropy_setup with an abi.EncodeEntropySetup"""
@@ -984,6 +1040,38 @@ class Context:
     def synthesis_dev(self, nstreams, nblk, d_Wseq, d_coef_off, d_coef, d_pcm_off, d_pcm, pcm_stride, stream=None):
         self._chk(self.L.vb200_synthesis_dev(self.h, nstreams, nblk, _ptr(d_Wseq), _ptr(d_coef_off), _ptr(d_coef),
                                              _ptr(d_pcm_off), _ptr(d_pcm), pcm_stride, _ptr(stream)))
+
+
+class DecodeStreamsCarry:
+    """nstreams carries of vb200_decode_streams_packets in device memory (vb200_malloc_device), freed with close()"""
+
+    def __init__(self, ctx, nstreams, nbytes):
+        self.ctx, self.nstreams, self.nbytes = ctx, nstreams, nbytes
+        p = vp()
+        ctx._chk(ctx.L.vb200_malloc_device(ctx.h, nstreams * nbytes, C.byref(p)))
+        self.ptr = p.value
+
+    def read(self):
+        """a host copy, uint8 [nstreams][nbytes]"""
+        a = np.zeros((self.nstreams, self.nbytes), np.uint8)
+        self.ctx._chk(self.ctx.L.vb200_memcpy_d2h(self.ctx.h, a.ctypes.data, self.ptr, a.nbytes))
+        return a
+
+    def write(self, a):
+        a = np.ascontiguousarray(a, np.uint8)
+        assert a.shape == (self.nstreams, self.nbytes)
+        self.ctx._chk(self.ctx.L.vb200_memcpy_h2d(self.ctx.h, self.ptr, a.ctypes.data, a.nbytes))
+
+    def close(self):
+        if self.ptr and self.ctx.h:
+            self.ctx.L.vb200_free_device(self.ctx.h, self.ptr)
+        self.ptr = None
+
+    def __del__(self):
+        try:
+            self.close()
+        except Exception:
+            pass
 
 
 def synthesis_layout(Wseq, bs, channels, halfrate=False, carry_W=None, count=None):
