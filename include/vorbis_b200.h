@@ -936,6 +936,66 @@ int vb200_encode_streams_packets_resume        (vb200_ctx*, int nstreams, int bl
 int vb200_encode_streams_packets_managed_resume(vb200_ctx*, int nstreams, vb200_streams_io *io,
                                                 void *carry, vb200_packet_info *info, uint8_t *data, int64_t data_cap);
 
+/* ---- raw PCM to packets: the _resume calls fed the caller's PCM instead of a timeline.  The LPC pre-extrapolation of
+ * vorbis_analysis_wrote (lib/block.c:426-466, 525: order 16 over all P samples written when more than blocksizes[1]
+ * have been, time-reversed, predicting the blocksizes[1]/2 preamble samples; the guard P > 32) and its post-
+ * extrapolation at the end (:474-514: order 32 over the timeline [eof - n, eof), n = min(eof - base, blocksizes[1]),
+ * primed with the 32 samples before eof, predicting 3*blocksizes[1] samples; the guard eof - base > 64) run on the
+ * device, bit for bit.  The carry is [nstreams][vb200_encode_pcm_carry_bytes] bytes; each begins with a readable
+ * vb200_pcm_carry, the rest is opaque: an encode carry and, per channel, the 16 preamble coefficients with their 16
+ * prime samples and the 32 tail coefficients with their 32 prime samples (filters, not samples: every call rebuilds
+ * the preamble or tail part of its timeline by replaying vorbis_lpc_predict from them).  mark_steps as for
+ * vb200_encode_carry_init; vb200_encode_pcm_carry_init after a managed vb200_bitrate_setup for the managed form.
+ * Per call, stream s passes in io->pcm the input samples from its carry's raw_base: the ones it kept (written -
+ * raw_base), then this call's new ones; pcm_len[s] counts both.
+ * The write rule: one call is one vorbis_analysis_wrote(v, new) followed by the blockout loop of encoder_example.c,
+ * run until it returns 0 (or max_blocks blocks).  A call with no new samples is a drain call.  A call with end[s]
+ * nonzero is vorbis_analysis_wrote(v, 0): it brings no new samples, and the carry must be drained (the last call
+ * planned fewer than max_blocks blocks for the stream).  Hence the packets, granulepos, e_o_s and packetno equal a
+ * stock encoder's fed the same writes; more generally they equal those of any stock encoder whose writes cross
+ * blocksizes[1] samples at the same count P (the write that does so fixes the preamble; the end's base is the drained
+ * planner's and does not depend on the cuts).  Streams without a preamble yet plan nothing.
+ *   pcm_fmt  VB200_PCM_F32_PLANAR [stream][ch][stream_stride] or VB200_PCM_S16_INTERLEAVED [stream][stream_stride][ch]
+ *            (read as x/32768.f, as encoder_example.c converts)
+ *   plan, nblocks, cap, count and the outputs as vb200_encode_streams_packets_resume; plan[].pos is relative to the
+ *            call's timeline buffer, which starts at enc.base (the input starts at timeline sample blocksizes[1]/2).
+ * Errors (VB200_EINVAL, every carry left as it was): those of the _resume calls, a pcm_fmt other than the two,
+ * pcm_len[s] below the kept samples or above stream_stride, an end call with new samples, an end on an undrained
+ * carry, a second end, and samples after the end.  Launches: four (the preamble filters, the timelines up to eof, the
+ * tail filters, the tails) plus those of the _resume call, whatever the stream count.  Device scratch: that of the
+ * _resume calls plus the input and nstreams x channels x (the longest timeline passed) floats.  Host pointers only. */
+typedef struct vb200_pcm_carry {
+  vb200_encode_carry enc;  /* the encode carry's head (base in timeline samples, granulepos, packetno, done) */
+  int64_t raw_base;        /* input sample where the next call's buffer starts: max(0, enc.base - blocksizes[1]/2) */
+  int64_t written;         /* input samples written so far */
+  int32_t ended;           /* vorbis_analysis_wrote(v, 0) has been made */
+  int32_t drained;         /* the last call planned fewer than max_blocks blocks for this stream (1 when fresh) */
+} vb200_pcm_carry;
+int vb200_encode_pcm_carry_bytes(vb200_ctx*, int mark_steps);
+int vb200_encode_pcm_carry_init (vb200_ctx*, int nstreams, int mark_steps, void *carry);
+typedef struct vb200_pcm_io {
+  const void *pcm;
+  int32_t pcm_fmt;
+  int32_t max_blocks;
+  int64_t stream_stride;
+  const int64_t *pcm_len;      /* [nstreams] input samples from raw_base: the kept ones, then this call's new ones */
+  const int32_t *end;          /* [nstreams] or NULL: nonzero = this call is vorbis_analysis_wrote(v, 0) */
+  vb200_stream_block *plan;    /* [nstreams][max_blocks] out */
+  int32_t *nblocks;            /* [nstreams] out */
+  int32_t cap[2];
+  int32_t count[2];            /* out */
+} vb200_pcm_io;
+int vb200_encode_pcm_packets        (vb200_ctx*, int nstreams, int blobno, vb200_pcm_io *io, void *carry,
+                                     vb200_packet_info *info, uint8_t *data, int64_t data_cap);
+int vb200_encode_pcm_packets_managed(vb200_ctx*, int nstreams, vb200_pcm_io *io, void *carry,
+                                     vb200_packet_info *info, uint8_t *data, int64_t data_cap);
+/* The stage call of those kernels: per row r, vorbis_lpc_from_data(data[r][0 .. n[r]), order) (lib/lpc.c:60-130), then
+ * vorbis_lpc_predict of `count` samples continuing the window, primed with its last `order` samples (:132-159).
+ * order 16 or 32; order <= n[r] <= data_stride; out_stride >= count.  coeff [nrows][order] and out [nrows][out_stride]
+ * (the first count of each row written).  No guard: a row of silence takes the reference's epsilon exit.          */
+int vb200_lpc_extrapolate(vb200_ctx*, int nrows, int order, const float *data, int64_t data_stride,
+                          const int32_t *n, int32_t count, float *coeff, float *out, int64_t out_stride);
+
 /* ---- device memory helpers for non-CUDA hosts (C callers) -------------- */
 int  vb200_malloc_device(vb200_ctx*, size_t bytes, void **dptr);
 int  vb200_free_device  (vb200_ctx*, void *dptr);

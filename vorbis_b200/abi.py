@@ -185,6 +185,22 @@ class StreamsIO(C.Structure):
     ]
 
 
+class PcmIO(C.Structure):
+    """vb200_pcm_io (include/vorbis_b200.h)"""
+    _fields_ = [
+        ("pcm", C.c_void_p),
+        ("pcm_fmt", C.c_int32),
+        ("max_blocks", C.c_int32),
+        ("stream_stride", C.c_int64),
+        ("pcm_len", C.c_void_p),
+        ("end", C.c_void_p),
+        ("plan", C.c_void_p),
+        ("nblocks", C.c_void_p),
+        ("cap", C.c_int32 * 2),
+        ("count", C.c_int32 * 2),
+    ]
+
+
 class BitrateInfo(C.Structure):
     """vb200_bitrate_info (include/vorbis_b200.h): bitrate_manager_info, lib/bitrate.h:41-50"""
     _fields_ = [
@@ -205,6 +221,10 @@ assert C.sizeof(BitrateInfo) == 48 and BITRATE_STATE_DTYPE.itemsize == 32 and PA
 # vb200_encode_carry: the public head of every stream's carry ([nstreams][vb200_encode_carry_bytes] bytes)
 ENCODE_CARRY_HEAD_DTYPE = np.dtype([("base", "<i8"), ("granulepos", "<i8"), ("packetno", "<i4"), ("done", "<i4")])
 assert ENCODE_CARRY_HEAD_DTYPE.itemsize == 24
+# vb200_pcm_carry: the public head of every raw-PCM carry ([nstreams][vb200_encode_pcm_carry_bytes] bytes)
+PCM_CARRY_HEAD_DTYPE = np.dtype([("enc", ENCODE_CARRY_HEAD_DTYPE), ("raw_base", "<i8"), ("written", "<i8"),
+                                 ("ended", "<i4"), ("drained", "<i4")])
+assert PCM_CARRY_HEAD_DTYPE.itemsize == 48
 # vb200_decoded_packet: what vb200_decode_streams_packets reports for every packet it was given
 DECODED_PACKET_DTYPE = np.dtype([("pcm_offset", "<i8"), ("granulepos", "<i8"), ("samples", "<i4"), ("status", "<i4")])
 assert DECODED_PACKET_DTYPE.itemsize == 24

@@ -27,6 +27,7 @@
 #include "vb200_entropy_enc.cuh"
 #include "vb200_bitrate.cuh"
 #include "vb200_decode_streams.cuh"
+#include "vb200_lpc.cuh"
 #include "floor1_db_table.h"
 
 using namespace vb200;
@@ -100,8 +101,10 @@ struct vb200_ctx {
   //   brc       the host form of vb200_bitrate_addblocks
   //   dsk       vb200_decode_streams_packets[_dev]: the packet headers, the block tables, the per-stream plan and the
   //             residue scratch, sized by nstreams x max_packets
+  //   ptl       vb200_encode_pcm_packets[_managed]: the planar float timelines [nstreams][ch][longest this call passes]
+  //             that the LPC kernels build and the streams packets path reads
   DevBuf stage[STAGE_SLOTS], cycles, phaseA, lane[2], enc, set[ENC_SETS], mgd, plan, chain, env_scratch, coder, pack,
-      spk, brc, dsk;
+      spk, brc, dsk, ptl;
   cudaStream_t s_pipe[2] = {nullptr, nullptr};
   const ResDev *d_res[2] = {nullptr, nullptr};        // [VB200_MAX_SUBMAPS] residue class parameters per block size
   int res_partvals[2] = {0, 0};
@@ -3913,9 +3916,12 @@ static void carry_unpack(vb200_ctx *c, int nstreams, int cap, const CarryBlob &b
 // Both whole-stream packet calls: the streams chain into staged device buffers, the entropy coder per size, then
 // (k_stream_bits, [k_bitrate_choose], k_packet_offsets, k_stream_gather) on the spk arena, carved once when the
 // per-size block counts are known.  One synchronous round trip on s_main.  carry (host): the _resume forms, whose
-// carries are staged as one more buffer and written back only when the call succeeds.
+// carries are staged as one more buffer and written back only when the call succeeds.  staged (the raw-PCM calls):
+// the caller holds c->mu, h->pcm is a float planar timeline already on the device, and the call stages through the
+// caller's HostIO.
 static int streams_packets(vb200_ctx *c, int nstreams, int blobno, bool managed, vb200_streams_io *h,
-                           vb200_packet_info *info, uint8_t *data, int64_t data_cap, void *carry = nullptr) {
+                           vb200_packet_info *info, uint8_t *data, int64_t data_cap, void *carry = nullptr,
+                           HostIO *staged = nullptr) {
   int rc;
   if ((rc = plan_check(c))) return rc;
   if (!h) return fail(VB200_EINVAL, "null io");
@@ -3936,16 +3942,18 @@ static int streams_packets(vb200_ctx *c, int nstreams, int blobno, bool managed,
   CarryBlob hb{};
   int ccap = 0, nsteps_env = 0;
   if (carry && (rc = carry_pack(c, nstreams, managed, h, carry, cblob, hb, &ccap, &nsteps_env))) return rc;
-  std::lock_guard<std::mutex> lk(c->mu);
+  std::unique_lock<std::mutex> lk(c->mu, std::defer_lock);
+  if (!staged) lk.lock();
   cudaStream_t st = c->s_main;
   const int curves = managed ? VB200_PACKETBLOBS : 1;
   const size_t ch = c->setup.channels;
   const size_t pcm_bytes = (size_t)nstreams * ch * (size_t)h->stream_stride * (h->pcm_fmt == VB200_PCM_S16_INTERLEAVED ? 2 : 4);
   const size_t n = (size_t)nstreams * h->max_blocks;
-  HostIO io{c};
+  HostIO own{c};
+  HostIO &io = staged ? *staged : own;
   void *p;
   vb200_streams_io d = *h;
-  if ((rc = io.h2d(h->pcm, pcm_bytes, &p))) return rc; d.pcm = p;
+  if (!staged) { if ((rc = io.h2d(h->pcm, pcm_bytes, &p))) return rc; d.pcm = p; }
   if ((rc = io.h2d(h->pcm_len, sizeof(int64_t) * nstreams, &p))) return rc; d.pcm_len = (const int64_t *)p;
   if (h->eof) { if ((rc = io.h2d(h->eof, sizeof(int64_t) * nstreams, &p))) return rc; d.eof = (const int64_t *)p; }
   if ((rc = io.h2d(nullptr, sizeof(vb200_stream_block) * n, &p))) return rc; d.plan = (vb200_stream_block *)p;
@@ -4061,6 +4069,250 @@ extern "C" int vb200_encode_streams_packets_managed_resume(vb200_ctx *c, int nst
   CHECK_CTX(c);
   if (!carry) return fail(VB200_EINVAL, "null carry");
   return streams_packets(c, nstreams, 0, true, io, info, data, data_cap, carry);
+}
+
+// ---- raw PCM to packets: vorbis_analysis_wrote's LPC preamble and tail on the device, in front of the carried streams
+// packets path.  The host carry of a stream is a PcmCarry, then the encode carry (carry_parts bytes), then the filters
+// of every channel (LPC_FILTER_FLOATS floats: the order-16 preamble coefficients and prime, the order-32 tail
+// coefficients and prime), each part 8-byte aligned.
+struct PcmCarry {
+  vb200_encode_carry enc;            // a copy of the encode carry's head, refreshed by every call (vb200_pcm_carry)
+  long long raw_base, written;
+  int ended, drained;
+  int pre_done;                      // v->preextrapolate: the preamble filter has been made
+  int ch, bs1, pad;
+};
+static_assert(offsetof(PcmCarry, raw_base) == offsetof(vb200_pcm_carry, raw_base) &&
+              offsetof(PcmCarry, written) == offsetof(vb200_pcm_carry, written) &&
+              offsetof(PcmCarry, ended) == offsetof(vb200_pcm_carry, ended) &&
+              offsetof(PcmCarry, drained) == offsetof(vb200_pcm_carry, drained) && sizeof(vb200_pcm_carry) == 48 &&
+              sizeof(PcmCarry) % 8 == 0, "vb200_pcm_carry is the head of PcmCarry (mirrored by vorbis_b200/abi.py)");
+
+static size_t pcm_filt_bytes(const vb200_ctx *c) { return sizeof(float) * LPC_FILTER_FLOATS * c->setup.channels; }
+
+extern "C" int vb200_encode_pcm_carry_bytes(vb200_ctx *c, int mark_steps) {
+  CHECK_CTX(c);
+  return (int)(sizeof(PcmCarry) + carry_parts(c, carry_cap(c, mark_steps)).bytes + pcm_filt_bytes(c));
+}
+
+extern "C" int vb200_encode_pcm_carry_init(vb200_ctx *c, int nstreams, int mark_steps, void *carry) {
+  CHECK_CTX(c);
+  if (nstreams <= 0) return 0;
+  if (!carry) return fail(VB200_EINVAL, "null carry");
+  const size_t eb = carry_parts(c, carry_cap(c, mark_steps)).bytes, pb = sizeof(PcmCarry) + eb + pcm_filt_bytes(c);
+  for (int s = 0; s < nstreams; s++) {
+    char *cs = (char *)carry + (size_t)s * pb;
+    memset(cs, 0, pb);
+    int rc;
+    if ((rc = vb200_encode_carry_init(c, 1, mark_steps, cs + sizeof(PcmCarry)))) return rc;
+    PcmCarry p{};
+    memcpy(&p.enc, cs + sizeof(PcmCarry), sizeof(p.enc));
+    p.drained = 1;
+    p.ch = c->setup.channels; p.bs1 = c->setup.blocksizes[1];
+    memcpy(cs, &p, sizeof(p));
+  }
+  return 0;
+}
+
+// Launches: k_lpc_filter<16> (the preamble filters due this call), k_pcm_timeline<false> (the timelines up to eof),
+// k_lpc_filter<32> (the tail filters due, which read those timelines), k_pcm_timeline<true> (the tails), then the
+// launches of the streams packets call on the timelines: four more than that call, whatever the stream count.
+static int pcm_packets(vb200_ctx *c, int nstreams, int blobno, bool managed, vb200_pcm_io *h, void *carry,
+                       vb200_packet_info *info, uint8_t *data, int64_t data_cap) {
+  int rc;
+  if (!h) return fail(VB200_EINVAL, "null io");
+  h->count[0] = h->count[1] = 0;
+  if (h->pcm_fmt != VB200_PCM_F32_PLANAR && h->pcm_fmt != VB200_PCM_S16_INTERLEAVED) return fail(VB200_EINVAL, "pcm format");
+  if (nstreams <= 0) return 0;
+  if (!carry) return fail(VB200_EINVAL, "null carry");
+  if (!h->pcm || !h->pcm_len || h->stream_stride < 0 || h->max_blocks < 1) return fail(VB200_EINVAL, "encode_pcm_packets: pcm, pcm_len, stride, max_blocks");
+  const int ch = c->setup.channels, bs1 = c->setup.blocksizes[1], half = bs1 / 2;
+  PcmCarry p0;
+  memcpy(&p0, carry, sizeof(p0));
+  if (p0.ch != ch || p0.bs1 != bs1) return fail(VB200_EINVAL, "pcm carry of another setup");
+  const int mark_cap = ((const PlanCarry *)((const char *)carry + sizeof(PcmCarry)))->mark_cap;
+  const size_t eb = carry_parts(c, mark_cap).bytes, fb = pcm_filt_bytes(c), pb = sizeof(PcmCarry) + eb + fb;
+  // the write of every stream, as vorbis_analysis_wrote would take it
+  std::vector<PcmCarry> pc(nstreams);
+  std::vector<PcmStream> ps(nstreams);
+  std::vector<int64_t> tl_len(nstreams), eof(nstreams);
+  std::vector<char> enc((size_t)nstreams * eb);
+  std::vector<int> pre_due(nstreams), tail_due(nstreams);
+  // the streams path wants a stride of at least blocksizes[1], a multiple of 4 for float PCM
+  long long tstride = bs1, njobs = 0;
+  for (int s = 0; s < nstreams; s++) {
+    const char *cs = (const char *)carry + (size_t)s * pb;
+    PcmCarry &p = pc[s];
+    memcpy(&p, cs, sizeof(p));
+    memcpy(enc.data() + (size_t)s * eb, cs + sizeof(PcmCarry), eb);
+    PlanCarry q;
+    memcpy(&q, cs + sizeof(PcmCarry), sizeof(q));
+    if (p.ch != ch || p.bs1 != bs1) return fail(VB200_EINVAL, "pcm carries of different setups");
+    const int64_t kept = p.written - p.raw_base, fresh = h->pcm_len[s] - kept;
+    const bool end = h->end && h->end[s];
+    if (fresh < 0) return fail(VB200_EINVAL, "pcm_len below the input samples the carry kept");
+    if (h->pcm_len[s] > h->stream_stride) return fail(VB200_EINVAL, "pcm_len above stream_stride");
+    if (p.ended && fresh) return fail(VB200_EINVAL, "samples after the end");
+    if (end && p.ended) return fail(VB200_EINVAL, "a second end");
+    if (end && fresh) return fail(VB200_EINVAL, "an end call with new samples (end is vorbis_analysis_wrote(v, 0))");
+    if (end && !p.drained) return fail(VB200_EINVAL, "an end call on a carry max_blocks left undrained");
+    p.written += fresh;
+    // lib/block.c:525 and :480 (pcm_current - centerW is the samples written until the preamble exists)
+    pre_due[s] = !p.pre_done && (p.written > bs1 || end);
+    tail_due[s] = end;
+    p.pre_done |= pre_due[s];
+    p.ended |= end;
+    PcmStream &t = ps[s];
+    t.base = q.base; t.raw_base = p.raw_base;
+    t.eof = p.ended ? half + p.written : 0;
+    t.len = q.done || !p.pre_done ? 0 : (p.ended ? t.eof + 3LL * bs1 : half + p.written) - q.base;
+    tl_len[s] = t.len; eof[s] = t.eof;
+    tstride = std::max(tstride, t.len);
+    njobs += (pre_due[s] + tail_due[s]) * ch;
+  }
+  tstride = (tstride + 3) & ~3LL;
+  std::lock_guard<std::mutex> lk(c->mu);
+  cudaStream_t st = c->s_main;
+  const bool s16 = h->pcm_fmt == VB200_PCM_S16_INTERLEAVED;
+  HostIO io{c};
+  void *din, *dblob;
+  const size_t in_bytes = (size_t)nstreams * ch * (size_t)h->stream_stride * (s16 ? 2 : 4);
+  if ((rc = io.h2d(in_bytes ? h->pcm : nullptr, std::max<size_t>(in_bytes, 1), &din))) return rc;
+  float *dtl;
+  if ((rc = carve(c->ptl, [&](Carve &k) { dtl = k.take<float>((size_t)nstreams * ch * tstride); }))) return rc;
+  CU(cudaMemsetAsync(dtl, 0, sizeof(float) * nstreams * ch * tstride, st));   // columns past a stream's len read as 0
+  // one staged buffer: the streams, the jobs (preamble jobs first) and the filters of every (stream, channel)
+  PcmStream *bs; LpcJob *bj; float *bf;
+  auto layout = [&](Carve &k) {
+    bs = k.take<PcmStream>(nstreams); bj = k.take<LpcJob>((size_t)std::max(njobs, 1LL));
+    bf = k.take<float>((size_t)nstreams * ch * LPC_FILTER_FLOATS);
+  };
+  Carve sz{nullptr, 0};
+  layout(sz);
+  std::vector<char> blob(sz.off);
+  Carve at{blob.data(), 0};
+  layout(at);
+  if ((rc = io.h2d(nullptr, blob.size(), &dblob))) return rc;
+  auto dev = [&](auto *hp) { return (decltype(hp))((char *)dblob + ((char *)hp - blob.data())); };
+  const long long stride = h->stream_stride;
+  int npre = 0, nj = 0;
+  for (int pass = 0; pass < 2; pass++)
+    for (int s = 0; s < nstreams; s++) {
+      if (!(pass ? tail_due[s] : pre_due[s])) continue;
+      const PcmStream &t = ps[s];
+      for (int k = 0; k < ch; k++) {
+        LpcJob &J = bj[nj++];
+        const long long q = (long long)s * ch + k;
+        float *f = dev(bf) + q * LPC_FILTER_FLOATS + (pass ? 2 * LPC_PRE : 0);
+        J.coef = f; J.prime = f + (pass ? LPC_TAIL : LPC_PRE);
+        if (!pass) {
+          // _preextrapolate_helper: the input [0, P) time-reversed (raw_base is 0 before the preamble exists)
+          const long long P = pc[s].written;
+          J.src = din; J.s16 = s16; J.n = P;
+          J.off = s16 ? ((long long)s * stride + P - 1) * ch + k : q * stride + P - 1;
+          J.step = s16 ? -ch : -1;
+        } else {
+          // vorbis_analysis_wrote(v, 0): timeline [eof - n, eof), n = min(eof - base, blocksizes[1])
+          const long long n = std::min<long long>(t.eof - t.base, bs1);
+          J.src = dtl; J.s16 = 0; J.n = n; J.off = q * tstride + t.eof - n - t.base; J.step = 1;
+        }
+      }
+      if (!pass) npre = nj;
+    }
+  for (int s = 0; s < nstreams; s++) {
+    bs[s] = ps[s];
+    memcpy(bf + (size_t)s * ch * LPC_FILTER_FLOATS, (const char *)carry + (size_t)s * pb + sizeof(PcmCarry) + eb, fb);
+  }
+  CU(cudaMemcpyAsync(dblob, blob.data(), blob.size(), cudaMemcpyHostToDevice, st));
+  PcmTimelineArgs A;
+  A.in = din; A.s16 = s16; A.ch = ch; A.half = half; A.in_stride = stride; A.tl_stride = tstride;
+  A.st = dev(bs); A.filt = dev(bf); A.tl = dtl; A.nstreams = nstreams;
+  const int pairs = nstreams * ch;
+  k_lpc_filter<LPC_PRE><<<grid_for(c, (npre + LPC_WARPS - 1) / LPC_WARPS, 8), 32 * LPC_WARPS, 0, st>>>(dev(bj), npre, 1);
+  if ((rc = post_launch(c))) return rc;
+  k_pcm_timeline<false><<<grid_for(c, pairs, 8), 256, 0, st>>>(A);
+  if ((rc = post_launch(c))) return rc;
+  k_lpc_filter<LPC_TAIL><<<grid_for(c, (nj - npre + LPC_WARPS - 1) / LPC_WARPS, 8), 32 * LPC_WARPS, 0, st>>>(
+      dev(bj) + npre, nj - npre, 1);
+  if ((rc = post_launch(c))) return rc;
+  k_pcm_timeline<true><<<(pairs + 255) / 256, 256, 0, st>>>(A);
+  if ((rc = post_launch(c))) return rc;
+  vb200_streams_io d{};
+  d.pcm = dtl; d.pcm_fmt = VB200_PCM_F32_PLANAR; d.max_blocks = h->max_blocks; d.stream_stride = tstride;
+  d.pcm_len = tl_len.data(); d.eof = eof.data(); d.plan = h->plan; d.nblocks = h->nblocks;
+  d.cap[0] = h->cap[0]; d.cap[1] = h->cap[1];
+  rc = streams_packets(c, nstreams, blobno, managed, &d, info, data, data_cap, enc.data(), &io);
+  h->count[0] = d.count[0]; h->count[1] = d.count[1];
+  if (rc) return rc;
+  CU(cudaMemcpyAsync(bf, dev(bf), (size_t)nstreams * fb, cudaMemcpyDeviceToHost, st));
+  CU(cudaStreamSynchronize(st));
+  for (int s = 0; s < nstreams; s++) {
+    char *cs = (char *)carry + (size_t)s * pb;
+    PcmCarry &p = pc[s];
+    memcpy(&p.enc, enc.data() + (size_t)s * eb, sizeof(p.enc));
+    p.raw_base = std::max<long long>(0, p.enc.base - half);
+    p.drained = h->nblocks[s] < h->max_blocks;
+    memcpy(cs, &p, sizeof(p));
+    memcpy(cs + sizeof(PcmCarry), enc.data() + (size_t)s * eb, eb);
+    memcpy(cs + sizeof(PcmCarry) + eb, bf + (size_t)s * ch * LPC_FILTER_FLOATS, fb);
+  }
+  return 0;
+}
+
+extern "C" int vb200_encode_pcm_packets(vb200_ctx *c, int nstreams, int blobno, vb200_pcm_io *io, void *carry,
+                                        vb200_packet_info *info, uint8_t *data, int64_t data_cap) {
+  CHECK_CTX(c);
+  return pcm_packets(c, nstreams, blobno, false, io, carry, info, data, data_cap);
+}
+
+extern "C" int vb200_encode_pcm_packets_managed(vb200_ctx *c, int nstreams, vb200_pcm_io *io, void *carry,
+                                                vb200_packet_info *info, uint8_t *data, int64_t data_cap) {
+  CHECK_CTX(c);
+  return pcm_packets(c, nstreams, 0, true, io, carry, info, data, data_cap);
+}
+
+extern "C" int vb200_lpc_extrapolate(vb200_ctx *c, int nrows, int order, const float *data, int64_t data_stride,
+                                     const int32_t *n, int32_t count, float *coeff, float *out, int64_t out_stride) {
+  CHECK_CTX(c);
+  if (order != LPC_PRE && order != LPC_TAIL) return fail(VB200_EINVAL, "lpc order must be 16 or 32");
+  if (nrows <= 0) return 0;
+  if (!data || !n || !coeff || (count > 0 && !out) || count < 0 || out_stride < count) return fail(VB200_EINVAL, "lpc_extrapolate arguments");
+  for (int r = 0; r < nrows; r++)
+    if (n[r] < order || n[r] > data_stride) return fail(VB200_EINVAL, "lpc_extrapolate: n[r] outside [order, data_stride]");
+  std::lock_guard<std::mutex> lk(c->mu);
+  cudaStream_t st = c->s_main;
+  HostIO io{c};
+  void *dd, *dj, *dc, *dp, *dout = nullptr;
+  int rc;
+  if ((rc = io.h2d(data, sizeof(float) * (size_t)nrows * data_stride, &dd))) return rc;
+  if ((rc = io.h2d(nullptr, sizeof(float) * (size_t)nrows * order, &dc))) return rc;
+  if ((rc = io.h2d(nullptr, sizeof(float) * (size_t)nrows * order, &dp))) return rc;
+  if (count > 0 && (rc = io.h2d(nullptr, sizeof(float) * (size_t)nrows * out_stride, &dout))) return rc;
+  std::vector<LpcJob> jobs(nrows);
+  for (int r = 0; r < nrows; r++) {
+    LpcJob &J = jobs[r];
+    J = LpcJob{};
+    J.src = dd; J.off = (long long)r * data_stride; J.step = 1; J.n = n[r];
+    J.coef = (float *)dc + (size_t)r * order; J.prime = (float *)dp + (size_t)r * order;
+  }
+  if ((rc = io.h2d(jobs.data(), sizeof(LpcJob) * nrows, &dj))) return rc;
+  const int grid = grid_for(c, (nrows + LPC_WARPS - 1) / LPC_WARPS, 8);
+  if (order == LPC_PRE) k_lpc_filter<LPC_PRE><<<grid, 32 * LPC_WARPS, 0, st>>>((const LpcJob *)dj, nrows, 0);
+  else k_lpc_filter<LPC_TAIL><<<grid, 32 * LPC_WARPS, 0, st>>>((const LpcJob *)dj, nrows, 0);
+  if ((rc = post_launch(c))) return rc;
+  if (count > 0) {
+    if (order == LPC_PRE)
+      k_lpc_predict<LPC_PRE><<<(nrows + 127) / 128, 128, 0, st>>>(nrows, (const float *)dc, (const float *)dp, count,
+                                                                  (float *)dout, out_stride);
+    else
+      k_lpc_predict<LPC_TAIL><<<(nrows + 127) / 128, 128, 0, st>>>(nrows, (const float *)dc, (const float *)dp, count,
+                                                                   (float *)dout, out_stride);
+    if ((rc = post_launch(c))) return rc;
+    CU(cudaMemcpy2DAsync(out, sizeof(float) * out_stride, dout, sizeof(float) * out_stride, sizeof(float) * count,
+                         nrows, cudaMemcpyDeviceToHost, st));
+  }
+  if ((rc = io.d2h(coeff, dc, sizeof(float) * (size_t)nrows * order))) return rc;
+  return io.sync();
 }
 
 // ======================================================================== //

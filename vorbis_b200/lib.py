@@ -48,6 +48,8 @@ EXPORTS = [
     "vb200_encode_streams_packets", "vb200_encode_streams_packets_managed",
     "vb200_encode_carry_bytes", "vb200_encode_carry_init", "vb200_encode_streams_packets_resume",
     "vb200_encode_streams_packets_managed_resume",
+    "vb200_encode_pcm_carry_bytes", "vb200_encode_pcm_carry_init", "vb200_encode_pcm_packets",
+    "vb200_encode_pcm_packets_managed", "vb200_lpc_extrapolate",
     "vb200_malloc_device", "vb200_free_device", "vb200_memcpy_h2d", "vb200_memcpy_d2h", "vb200_synchronize",
 ]
 
@@ -168,6 +170,11 @@ def load():
                                                       C.c_int64]
     L.vb200_encode_streams_packets_managed_resume.argtypes = [vp, C.c_int, C.POINTER(abi.StreamsIO), vp, vp, vp,
                                                               C.c_int64]
+    L.vb200_encode_pcm_carry_bytes.argtypes = [vp, C.c_int]
+    L.vb200_encode_pcm_carry_init.argtypes = [vp, C.c_int, C.c_int, vp]
+    L.vb200_encode_pcm_packets.argtypes = [vp, C.c_int, C.c_int, C.POINTER(abi.PcmIO), vp, vp, vp, C.c_int64]
+    L.vb200_encode_pcm_packets_managed.argtypes = [vp, C.c_int, C.POINTER(abi.PcmIO), vp, vp, vp, C.c_int64]
+    L.vb200_lpc_extrapolate.argtypes = [vp, C.c_int, C.c_int, vp, C.c_int64, vp, C.c_int32, vp, vp, C.c_int64]
     L.vb200_malloc_device.argtypes = [vp, C.c_size_t, C.POINTER(vp)]
     L.vb200_free_device.argtypes = [vp, vp]
     L.vb200_memcpy_h2d.argtypes = [vp, vp, vp, C.c_size_t]
@@ -979,6 +986,86 @@ class Context:
         out["packets"] = [[bytes(data[r["offset"]:r["offset"] + r["bytes"]]) for r in info[i, :nb[i]]]
                           for i in range(ns)]
         return out
+
+    def encode_pcm_carry_init(self, nstreams, mark_steps=0):
+        """vb200_encode_pcm_carry_init: fresh raw-PCM carries, uint8 [nstreams][vb200_encode_pcm_carry_bytes] (the
+        managed form wants them made after bitrate_setup); encode_pcm_carry_head(carry) reads their public heads"""
+        nbytes = self.L.vb200_encode_pcm_carry_bytes(self.h, mark_steps)
+        self._chk(min(nbytes, 0))
+        carry = np.zeros((nstreams, nbytes), np.uint8)
+        self._chk(self.L.vb200_encode_pcm_carry_init(self.h, nstreams, mark_steps, _ptr(carry)))
+        return carry
+
+    @staticmethod
+    def encode_pcm_carry_head(carry):
+        """the vb200_pcm_carry heads of carries made by encode_pcm_carry_init (PCM_CARRY_HEAD_DTYPE [nstreams], a copy)"""
+        hs = abi.PCM_CARRY_HEAD_DTYPE.itemsize
+        return np.ascontiguousarray(carry[:, :hs]).view(abi.PCM_CARRY_HEAD_DTYPE)[:, 0]
+
+    def encode_pcm_packets(self, pcm, pcm_len, carry, end=None, managed=False, max_blocks=None, cap=None, blobno=7,
+                           data_cap=None, check=True):
+        """vb200_encode_pcm_packets[_managed]: pcm float32 [ns][ch][stride] (VB200_PCM_F32_PLANAR) or int16
+        [ns][stride][ch] (VB200_PCM_S16_INTERLEAVED), stream s's input from its carry's raw_base; pcm_len [ns] the kept
+        plus the new samples; end [ns] (nonzero: vorbis_analysis_wrote(v, 0)) or None.  carry (from
+        encode_pcm_carry_init) is advanced in place when the call succeeds.  Returns as encode_streams_packets."""
+        ch, bs0, bs1 = self.channels, self.bs[0], self.bs[1]
+        if pcm.dtype == np.int16:
+            fmt, pcm = PCM_S16_INTERLEAVED, np.ascontiguousarray(pcm)
+            ns, stride = pcm.shape[0], pcm.shape[1]
+            assert pcm.shape[2] == ch
+        else:
+            fmt, pcm = PCM_F32_PLANAR, np.ascontiguousarray(pcm, np.float32)
+            ns, stride = pcm.shape[0], pcm.shape[2]
+            assert pcm.shape[1] == ch
+        assert carry.dtype == np.uint8 and carry.flags.c_contiguous and carry.shape[0] == ns
+        pcm_len = np.ascontiguousarray(pcm_len, np.int64)
+        endp = None if end is None else np.ascontiguousarray(end, np.int32)
+        span = stride + 4 * bs1                       # the timeline adds the preamble and the tail to the input
+        if max_blocks is None:
+            max_blocks = span // (bs0 // 2) + 8
+        if cap is None:
+            cap = [ns * max_blocks, ns * (span // (bs1 // 2) + 8)]
+        io = abi.PcmIO()
+        io.pcm, io.pcm_fmt, io.max_blocks, io.stream_stride = pcm.ctypes.data, fmt, max_blocks, stride
+        io.pcm_len = pcm_len.ctypes.data
+        io.end = None if endp is None else endp.ctypes.data
+        plan = np.zeros((ns, max_blocks), abi.STREAM_BLOCK_DTYPE)
+        nb = np.zeros(ns, np.int32)
+        io.plan, io.nblocks = plan.ctypes.data, nb.ctypes.data
+        io.cap[0], io.cap[1] = int(cap[0]), int(cap[1])
+        info = np.zeros((ns, max_blocks), abi.PACKET_INFO_DTYPE)
+        if data_cap is None:
+            data_cap = ns * max_blocks * max(self.packet_bound(0), self.packet_bound(1))
+        data = np.zeros(max(data_cap, 1), np.uint8)
+        if managed:
+            rc = self.L.vb200_encode_pcm_packets_managed(self.h, ns, C.byref(io), _ptr(carry), _ptr(info), _ptr(data),
+                                                         data_cap)
+        else:
+            rc = self.L.vb200_encode_pcm_packets(self.h, ns, blobno, C.byref(io), _ptr(carry), _ptr(info), _ptr(data),
+                                                 data_cap)
+        out = {"plan": plan, "nblocks": nb, "count": [io.count[0], io.count[1]], "info": info, "data": data}
+        if not check:
+            out["rc"] = rc
+            return out
+        self._chk(rc)
+        out["packets"] = [[bytes(data[r["offset"]:r["offset"] + r["bytes"]]) for r in info[i, :nb[i]]]
+                          for i in range(ns)]
+        return out
+
+    def lpc_extrapolate(self, data, n, order, count, check=True):
+        """vb200_lpc_extrapolate: data float32 [rows][stride], n [rows]; returns (coeff float32 [rows][order], out
+        float32 [rows][count]), or the status when check is False"""
+        data = np.ascontiguousarray(data, np.float32)
+        n = np.ascontiguousarray(n, np.int32)
+        rows = data.shape[0]
+        coeff = np.zeros((rows, order), np.float32)
+        out = np.zeros((rows, max(count, 1)), np.float32)
+        rc = self.L.vb200_lpc_extrapolate(self.h, rows, order, _ptr(data), data.shape[1], _ptr(n), count, _ptr(coeff),
+                                          _ptr(out), out.shape[1])
+        if not check:
+            return rc
+        self._chk(rc)
+        return coeff, out[:, :count]
 
     # ---- envelope / block-switch detector (lib/envelope.c) --------------------------------------
     def envelope_search(self, pcm, first_step, nsteps, state=None, fmt=PCM_F32_PLANAR):
