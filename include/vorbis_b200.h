@@ -727,6 +727,63 @@ int vb200_decode_streams_packets    (vb200_ctx*, int nstreams, int max_packets, 
                                      void *d_carry, int pcm_s16, void *pcm, int64_t pcm_cap, int64_t *pcm_base,
                                      vb200_decoded_packet *out);
 
+/* ---- sample ranges from packets: random access into many streams without decoding them whole (what vorbisfile's
+ * ov_pcm_seek + ov_read give one stream, without Ogg pages).  The inputs are those of vb200_decode_streams_packets:
+ * each stream given from its first packet, so vb200_encode_streams_packets' info and data go straight in; header
+ * packets passed in are dropped as OV_ENOTAUDIO.  Modes, floors and residue types are limited as there, and a
+ * registered vb200_decode_entropy_setup is needed (else VB200_EINVAL).  Full rate, and half rate after
+ * vb200_synthesis_halfrate.
+ *
+ * vb200_decode_streams_index[_dev]: the bookkeeping alone.  length[s] = the samples a fresh-carry
+ * vb200_decode_streams_packets call returns for stream s; out[s*max_packets + k] = its vb200_decoded_packet for
+ * packet k (pcm_offset, samples, granulepos, status), byte for byte.  No PCM, no carry, no residue scratch; two
+ * kernel launches (header parse, plan).  Device scratch (arena of its own with the ranges call, carved once per
+ * call): nstreams*max_packets*40 + nstreams*80 bytes.
+ *
+ * vb200_decode_ranges[_dev]: request r is samples [start, start + length) of stream `stream`'s output, counted as a
+ * fresh-carry vb200_decode_streams_packets call counts them (every pcmout sample, after the front and end trims).
+ * Its samples equal that slice bit for bit, for every stream that call accepts (dropped, truncated and empty
+ * packets, packetno gaps, beginning trims, granulepos on every packet or on page-final packets only).  Requests may
+ * come in any order, name one stream several times and overlap.  Only the blocks that finish the range's samples
+ * are decoded, after the one block before them, which primes the overlap.
+ *   pcm   float planar [nreq][ch][out_stride], or with pcm_s16 interleaved int16 [nreq][out_stride][ch] converted
+ *         as decoder_example does.  Row r holds got[r] samples from index 0 and zeros after them.
+ *   got   [nreq]: min(length, max(0, length_s - start)), so 0 for a start at or past the stream's end; or
+ *         VB200_EINVAL for a request whose stream, start or length is out of range (the _dev form checks them per
+ *         request) or that needs more blocks than its scratch holds (below).  Such a row is all zero.
+ * Capacity: a request's scratch is fixed by out_stride: (out_stride << halfrate) / (blocksizes[0]/2) + 3 blocks and
+ * ch * (2 * (out_stride << halfrate) + 3 * blocksizes[1]/2) floats of residue, rounded up to a multiple of 64.  That
+ * holds every range of a stream whose blocks return all the samples they finish away from its ends; a crafted stream
+ * (a packetno gap followed by a granulepos far behind the count) can need more, which gives got[r] = VB200_EINVAL
+ * and nothing written out of bounds.  A larger out_stride serves such a request.  Device scratch (arena of its own,
+ * carved once per call): nreq*(blocks*40 + 12 bytes + residue floats*4 bytes).  Three kernel launches per call
+ * (plan, entropy decode + DSP, synthesis) whatever nreq and nstreams are, after a memset of the output rows.  The
+ * plan of a request walks its stream's packets from the first to the range's end, so its cost does not grow with
+ * other streams or with packets past the range.
+ * _dev: every pointer is device memory; asynchronous; checks its pointers, max_packets >= 1, nreq >= 0 and
+ * out_stride >= 0 only.  Host forms: host buffers; return VB200_EINVAL for null pointers, nreq < 0, max_packets < 1,
+ * npkt[s] outside [0, max_packets], a packet outside data (data_bytes), a request's stream outside [0, nstreams),
+ * start < 0 or length outside [0, out_stride].                                                                  */
+typedef struct vb200_pcm_range {
+  int64_t start;
+  int32_t stream;
+  int32_t length;       /* 0 .. out_stride */
+} vb200_pcm_range;
+int vb200_decode_streams_index_dev(vb200_ctx*, int nstreams, int max_packets, const int32_t *d_npkt,
+                                   const struct vb200_packet_info *d_info, const uint8_t *d_data,
+                                   int64_t *d_length, vb200_decoded_packet *d_out, void *stream);
+int vb200_decode_streams_index    (vb200_ctx*, int nstreams, int max_packets, const int32_t *npkt,
+                                   const struct vb200_packet_info *info, const uint8_t *data, int64_t data_bytes,
+                                   int64_t *length, vb200_decoded_packet *out);
+int vb200_decode_ranges_dev(vb200_ctx*, int nstreams, int max_packets, const int32_t *d_npkt,
+                            const struct vb200_packet_info *d_info, const uint8_t *d_data,
+                            int nreq, const vb200_pcm_range *d_req, int pcm_s16, void *d_pcm, int32_t out_stride,
+                            int32_t *d_got, void *stream);
+int vb200_decode_ranges    (vb200_ctx*, int nstreams, int max_packets, const int32_t *npkt,
+                            const struct vb200_packet_info *info, const uint8_t *data, int64_t data_bytes,
+                            int nreq, const vb200_pcm_range *req, int pcm_s16, void *pcm, int32_t out_stride,
+                            int32_t *got);
+
 /* ---- encode: the entropy coding of mapping0_forward (lib/mapping0.c:596-687) on the device, un-managed bitrate.
  * What floor1_encode (lib/floor1.c:753-921) and the residue class / forward of types 1 and 2 (lib/res0.c:534-648,
  * 725-809) read, registered on a context with vb200_encode_entropy_setup.

@@ -228,6 +228,9 @@ assert PCM_CARRY_HEAD_DTYPE.itemsize == 48
 # vb200_decoded_packet: what vb200_decode_streams_packets reports for every packet it was given
 DECODED_PACKET_DTYPE = np.dtype([("pcm_offset", "<i8"), ("granulepos", "<i8"), ("samples", "<i4"), ("status", "<i4")])
 assert DECODED_PACKET_DTYPE.itemsize == 24
+# vb200_pcm_range: one request of vb200_decode_ranges, samples [start, start + length) of stream `stream`
+PCM_RANGE_DTYPE = np.dtype([("start", "<i8"), ("stream", "<i4"), ("length", "<i4")])
+assert PCM_RANGE_DTYPE.itemsize == 16
 
 
 class Codebook(C.Structure):

@@ -27,6 +27,7 @@
 #include "vb200_entropy_enc.cuh"
 #include "vb200_bitrate.cuh"
 #include "vb200_decode_streams.cuh"
+#include "vb200_decode_ranges.cuh"
 #include "vb200_lpc.cuh"
 #include "floor1_db_table.h"
 
@@ -103,8 +104,11 @@ struct vb200_ctx {
   //             residue scratch, sized by nstreams x max_packets
   //   ptl       vb200_encode_pcm_packets[_managed]: the planar float timelines [nstreams][ch][longest this call passes]
   //             that the LPC kernels build and the streams packets path reads
+  //   drg       vb200_decode_streams_index[_dev]: the packet headers, the per-stream plan tables and fresh heads,
+  //             sized by nstreams x max_packets; vb200_decode_ranges[_dev]: the per-request block tables and residue
+  //             scratch, sized by nreq and out_stride
   DevBuf stage[STAGE_SLOTS], cycles, phaseA, lane[2], enc, set[ENC_SETS], mgd, plan, chain, env_scratch, coder, pack,
-      spk, brc, dsk, ptl;
+      spk, brc, dsk, ptl, drg;
   cudaStream_t s_pipe[2] = {nullptr, nullptr};
   const ResDev *d_res[2] = {nullptr, nullptr};        // [VB200_MAX_SUBMAPS] residue class parameters per block size
   int res_partvals[2] = {0, 0};
@@ -948,7 +952,9 @@ struct SinkS16 {
 // carried W >= 0, block 0 overlap-adds onto that tail and finishes samples like any later block; with -1 it
 // only primes.  A stream with count 0 is not touched.  W is kept per (stream, channel) because the CTA of
 // one channel must not read what the CTA of another channel of the same stream writes.
-template <bool S16, bool HS, bool CARRY, bool TRIM = false>
+// FRESH (with TRIM, vb200_decode_ranges): every "stream" (a request) starts from a fresh state, so block 0 primes;
+// T.cap, T.W_in, T.head and the carries are neither read nor written.
+template <bool S16, bool HS, bool CARRY, bool TRIM = false, bool FRESH = false>
 __device__ __forceinline__ void
 synthesis_body(const XformDev &X0, const XformDev &X1, const WinDev &Wd, int ch, int nstreams, int nblk,
                const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
@@ -962,7 +968,7 @@ synthesis_body(const XformDev &X0, const XformDev &X1, const WinDev &Wd, int ch,
   float *s_in = sm, *s_out = sm + n1, *s_prev = s_out + 2 * n1;
   const float *w0 = Wd.win[0], *w1 = Wd.win[1];
   const int off = n1 / 2 - n0 / 2;
-  if constexpr (TRIM)
+  if constexpr (TRIM && !FRESH)
     if (T.base[nstreams] * ch > T.cap) return;
   for (int task = blockIdx.x; task < nstreams * ch; task += gridDim.x) {
     const int st = task / ch, c = task - st * ch;
@@ -972,7 +978,8 @@ synthesis_body(const XformDev &X0, const XformDev &X1, const WinDev &Wd, int ch,
       if (count) cnt = min(max(count[st], 0), nblk);
       if (cnt == 0) continue;
       int cw;
-      if constexpr (TRIM) cw = T.W_in[st];
+      if constexpr (FRESH) cw = -1;
+      else if constexpr (TRIM) cw = T.W_in[st];
       else cw = carry_W[task];
       if (cw >= 0) {
         // the loads finish before block 0's first __syncthreads; s_prev is read only after it
@@ -1031,7 +1038,7 @@ synthesis_body(const XformDev &X0, const XformDev &X1, const WinDev &Wd, int ch,
       lW = W;
       __syncthreads();
     }
-    if constexpr (CARRY || TRIM) {
+    if constexpr ((CARRY || TRIM) && !FRESH) {
       float *t;
       if constexpr (TRIM) t = T.tail(st, c);
       else t = carry_tail + (size_t)task * tail_stride;
@@ -1075,6 +1082,17 @@ k_synthesis_trim(XformDev X0, XformDev X1, WinDev Wd, int ch, int nstreams, int 
                  void *__restrict__ pcm_out, const int *__restrict__ count, DsTrim T) {
   synthesis_body<S16, HS, false, true>(X0, X1, Wd, ch, nstreams, nblk, Wseq, coef_off, coef, pcm_off, pcm_out, 0,
                                        count, nullptr, nullptr, T.tail_stride, T);
+}
+
+// vb200_decode_ranges: request r is "stream" r, its row of the output at T.base[r] = r * out_stride; block 0 primes
+template <bool S16, bool HS>
+__global__ void __launch_bounds__(256)
+k_synthesis_range(XformDev X0, XformDev X1, WinDev Wd, int ch, int nreq, int nblk,
+                  const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
+                  const float *__restrict__ coef, const long long *__restrict__ pcm_off,
+                  void *__restrict__ pcm_out, const int *__restrict__ count, DsTrim T) {
+  synthesis_body<S16, HS, false, true, true>(X0, X1, Wd, ch, nreq, nblk, Wseq, coef_off, coef, pcm_off, pcm_out, 0,
+                                             count, nullptr, nullptr, 0, T);
 }
 
 // ---- decode: undo channel coupling, lib/mapping0.c:754-779 (square polar -> L/R), in place
@@ -3334,6 +3352,202 @@ extern "C" int vb200_decode_streams_packets(vb200_ctx *c, int nstreams, int max_
   const int64_t total = pcm_base[nstreams] * ch;
   if (total > pcm_cap) return fail(VB200_EINVAL, "the PCM does not fit pcm_cap (pcm_base is filled)");
   if (total && (rc = io.d2h(pcm, dp, el * (size_t)total))) return rc;
+  return io.sync();
+}
+
+// ---- sample ranges from packets (vb200_decode_ranges.cuh).  The index is k_ds_header and k_ds_plan on fresh
+// heads; the ranges are k_dr_plan, k_decode_packets<true> and k_synthesis_range.
+static int ds_check_packets(int nstreams, int max_packets, const int32_t *npkt, const vb200_packet_info *info,
+                            int64_t data_bytes) {
+  for (int s = 0; s < nstreams; s++) {
+    if (npkt[s] < 0 || npkt[s] > max_packets) return fail(VB200_EINVAL, "npkt[s] must be in [0, max_packets]");
+    for (int k = 0; k < npkt[s]; k++) {
+      const vb200_packet_info &p = info[(size_t)s * max_packets + k];
+      if (p.offset < 0 || p.bytes < 0 || p.offset > data_bytes - p.bytes) return fail(VB200_EINVAL, "packet outside data");
+    }
+  }
+  return 0;
+}
+
+extern "C" int vb200_decode_streams_index_dev(vb200_ctx *c, int nstreams, int max_packets, const int32_t *d_npkt,
+                                              const vb200_packet_info *d_info, const uint8_t *d_data,
+                                              int64_t *d_length, vb200_decoded_packet *d_out, void *stream) {
+  CHECK_CTX(c);
+  if (nstreams <= 0) return 0;
+  if (max_packets < 1) return fail(VB200_EINVAL, "max_packets must be >= 1");
+  if (!d_npkt || !d_info || !d_data || !d_length || !d_out) return fail(VB200_EINVAL, "decode streams index pointers");
+  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
+  const long long n = (long long)nstreams * max_packets;
+  if (n > INT32_MAX) return fail(VB200_EINVAL, "nstreams * max_packets must fit an int");
+  const cudaStream_t st = (cudaStream_t)stream;
+  DsPlanArgs P;
+  DsHead *fresh;
+  int rc;
+  if ((rc = carve(c->drg, [&](Carve &k) {
+         P.Wseq = k.take<int>(n); P.pkt_bytes = k.take<int>(n); P.pkt_off = k.take<long long>(n);
+         P.coef_off = k.take<long long>(n); P.pcm_off = k.take<long long>(n); P.win = k.take<int2>(n);
+         P.count = k.take<int>(nstreams); P.W_in = k.take<int>(nstreams); P.head = k.take<DsHead>(nstreams);
+         P.pcm_base = k.take<long long>(nstreams + 1); fresh = k.take<DsHead>(nstreams);
+       }))) return rc;
+  P.nstreams = nstreams; P.max_packets = max_packets; P.ch = c->setup.channels; P.hs = c->halfrate ? 1 : 0;
+  P.bs[0] = c->setup.blocksizes[0]; P.bs[1] = c->setup.blocksizes[1];
+  P.npkt = d_npkt; P.info = d_info; P.hdr = P.Wseq; P.out = d_out;
+  // vorbis_synthesis_restart's head has every field k_ds_plan reads at -1 (granulepos, sample_count, sequence, W);
+  // rate is not read there
+  P.carry = (const unsigned char *)fresh; P.carry_bytes = sizeof(DsHead);
+  if ((rc = scratch_begin(c, st))) return rc;
+  CU(cudaMemsetAsync(fresh, 0xff, sizeof(DsHead) * (size_t)nstreams, st));
+  k_ds_header<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(nstreams, max_packets, c->ent.modebits, d_npkt, d_info,
+                                                             d_data, P.Wseq);
+  if ((rc = post_launch(c))) return rc;
+  k_ds_plan<<<(nstreams + 127) / 128, 128, 0, st>>>(P);
+  if ((rc = post_launch(c))) return rc;
+  CU(cudaMemcpyAsync(d_length, P.pcm_base + 1, sizeof(int64_t) * (size_t)nstreams, cudaMemcpyDeviceToDevice, st));
+  return scratch_end(c, st);
+}
+
+extern "C" int vb200_decode_streams_index(vb200_ctx *c, int nstreams, int max_packets, const int32_t *npkt,
+                                          const vb200_packet_info *info, const uint8_t *data, int64_t data_bytes,
+                                          int64_t *length, vb200_decoded_packet *out) {
+  CHECK_CTX(c);
+  if (nstreams <= 0) return 0;
+  if (max_packets < 1) return fail(VB200_EINVAL, "max_packets must be >= 1");
+  if (!npkt || !info || !data || !length || !out || data_bytes < 0) return fail(VB200_EINVAL, "decode streams index pointers");
+  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
+  int rc;
+  if ((rc = ds_check_packets(nstreams, max_packets, npkt, info, data_bytes))) return rc;
+  std::lock_guard<std::mutex> lk(c->mu);
+  const size_t n = (size_t)nstreams * max_packets;
+  HostIO io{c};
+  void *dn, *di, *dd, *dl, *dout;
+  if ((rc = io.h2d(npkt, sizeof(int32_t) * nstreams, &dn))) return rc;
+  if ((rc = io.h2d(info, sizeof(vb200_packet_info) * n, &di))) return rc;
+  if ((rc = io.h2d(nullptr, (size_t)data_bytes + 1, &dd))) return rc;
+  if (data_bytes) CU(cudaMemcpyAsync(dd, data, (size_t)data_bytes, cudaMemcpyHostToDevice, c->s_main));
+  if ((rc = io.h2d(nullptr, sizeof(int64_t) * nstreams, &dl))) return rc;
+  if ((rc = io.h2d(nullptr, sizeof(vb200_decoded_packet) * n, &dout))) return rc;
+  if ((rc = vb200_decode_streams_index_dev(c, nstreams, max_packets, (const int32_t *)dn, (const vb200_packet_info *)di,
+                                           (const uint8_t *)dd, (int64_t *)dl, (vb200_decoded_packet *)dout,
+                                           c->s_main))) return rc;
+  if ((rc = io.d2h(length, dl, sizeof(int64_t) * nstreams))) return rc;
+  if ((rc = io.d2h(out, dout, sizeof(vb200_decoded_packet) * n))) return rc;
+  return io.sync();
+}
+
+// a request's block slots and residue floats (vb200_decode_ranges.cuh proves they hold every ordinary range); the
+// residue is rounded up to 64 floats so that every request's region, and so every block in it, is 16-byte aligned
+static long long dr_blocks(const vb200_ctx *c, int32_t out_stride) {
+  return ((long long)out_stride << (c->halfrate ? 1 : 0)) / (c->setup.blocksizes[0] / 2) + 3;
+}
+static long long dr_residue(const vb200_ctx *c, int32_t out_stride) {
+  const long long f = (long long)c->setup.channels *
+                      (2 * ((long long)out_stride << (c->halfrate ? 1 : 0)) + 3ll * (c->setup.blocksizes[1] / 2));
+  return (f + 63) & ~63ll;
+}
+
+template <bool S16, bool HS>
+static int synthesis_range_launch(vb200_ctx *c, int nreq, int nblk, const int32_t *d_count, const int32_t *d_Wseq,
+                                  const long long *d_coef_off, const float *d_coef, const long long *d_pcm_off,
+                                  void *d_pcm, const DsTrim &T, cudaStream_t st) {
+  const XformDev *X = HS ? c->dx_hs : c->dx;
+  const int ch = c->setup.channels, N1 = X[1].N;
+  const size_t smem = sizeof(float) * ((size_t)N1 / 2 + N1 + N1 / 2);
+  int rc = set_smem(k_synthesis_range<S16, HS>, smem); if (rc) return rc;
+  k_synthesis_range<S16, HS><<<grid_for(c, nreq * ch, 8), threads_for(N1), smem, st>>>(
+      X[0], X[1], HS ? c->dwin_hs : c->dwin, ch, nreq, nblk, d_Wseq, d_coef_off, d_coef, d_pcm_off, d_pcm, d_count, T);
+  return post_launch(c);
+}
+
+extern "C" int vb200_decode_ranges_dev(vb200_ctx *c, int nstreams, int max_packets, const int32_t *d_npkt,
+                                       const vb200_packet_info *d_info, const uint8_t *d_data,
+                                       int nreq, const vb200_pcm_range *d_req, int pcm_s16, void *d_pcm,
+                                       int32_t out_stride, int32_t *d_got, void *stream) {
+  CHECK_CTX(c);
+  if (nreq < 0) return fail(VB200_EINVAL, "nreq must be >= 0");
+  if (nreq == 0) return 0;
+  if (max_packets < 1) return fail(VB200_EINVAL, "max_packets must be >= 1");
+  if (out_stride < 0) return fail(VB200_EINVAL, "out_stride must be >= 0");
+  if (nstreams < 0 || (nstreams > 0 && (!d_npkt || !d_info || !d_data)) || !d_req || !d_pcm || !d_got)
+    return fail(VB200_EINVAL, "decode ranges pointers");
+  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
+  const long long nblk = dr_blocks(c, out_stride), rescap = dr_residue(c, out_stride);
+  if ((long long)nreq * nblk > INT32_MAX) return fail(VB200_EINVAL, "nreq * block slots must fit an int");
+  const int ch = c->setup.channels;
+  const bool hs = c->halfrate;
+  const cudaStream_t st = (cudaStream_t)stream;
+  const size_t nb = (size_t)nreq * nblk;
+  DrPlanArgs P;
+  float *res;
+  int rc;
+  if ((rc = carve(c->drg, [&](Carve &k) {
+         P.Wseq = k.take<int>(nb); P.pkt_bytes = k.take<int>(nb); P.pkt_off = k.take<long long>(nb);
+         P.coef_off = k.take<long long>(nb); P.pcm_off = k.take<long long>(nb); P.win = k.take<int2>(nb);
+         P.count = k.take<int>(nreq); P.base = k.take<long long>(nreq + 1);
+         res = k.take<float>((size_t)nreq * rescap);
+       }))) return rc;
+  P.nstreams = nstreams; P.max_packets = max_packets; P.nreq = nreq; P.ch = ch; P.hs = hs ? 1 : 0;
+  P.modebits = c->ent.modebits;
+  P.bs[0] = c->setup.blocksizes[0]; P.bs[1] = c->setup.blocksizes[1];
+  P.out_stride = out_stride; P.nblk = (int)nblk; P.res_cap = rescap;
+  P.npkt = d_npkt; P.info = d_info; P.data = d_data; P.req = d_req; P.got = d_got;
+  if ((rc = scratch_begin(c, st))) return rc;
+  const size_t el = pcm_s16 ? sizeof(int16_t) : sizeof(float);
+  CU(cudaMemsetAsync(d_pcm, 0, el * (size_t)nreq * ch * (size_t)out_stride, st));
+  k_dr_plan<<<(unsigned)(((long long)nreq * 32 + 127) / 128), 128, 0, st>>>(P);
+  if ((rc = post_launch(c))) return rc;
+  DecodePrepArgs A;
+  if ((rc = decode_prep_args(c, nreq, (int)nblk, &A))) return rc;
+  const DecodePackets DP{P.pkt_off, P.pkt_bytes, d_data};
+  if ((rc = set_smem(k_decode_packets<true>, entropy_smem(c->ent, true)))) return rc;
+  k_decode_packets<true><<<grid_for(c, (int)nb, DECODE_PACKETS_CTAS), 128, entropy_smem(c->ent, true), st>>>(
+      A, c->ent, DP, P.Wseq, P.coef_off, res, c->d_fromdB, P.count);
+  if ((rc = post_launch(c))) return rc;
+  DsTrim T{};
+  T.win = P.win; T.base = P.base;
+  if (pcm_s16)
+    rc = hs ? synthesis_range_launch<true, true>(c, nreq, (int)nblk, P.count, P.Wseq, P.coef_off, res, P.pcm_off, d_pcm, T, st)
+            : synthesis_range_launch<true, false>(c, nreq, (int)nblk, P.count, P.Wseq, P.coef_off, res, P.pcm_off, d_pcm, T, st);
+  else
+    rc = hs ? synthesis_range_launch<false, true>(c, nreq, (int)nblk, P.count, P.Wseq, P.coef_off, res, P.pcm_off, d_pcm, T, st)
+            : synthesis_range_launch<false, false>(c, nreq, (int)nblk, P.count, P.Wseq, P.coef_off, res, P.pcm_off, d_pcm, T, st);
+  if (rc) return rc;
+  return scratch_end(c, st);
+}
+
+extern "C" int vb200_decode_ranges(vb200_ctx *c, int nstreams, int max_packets, const int32_t *npkt,
+                                   const vb200_packet_info *info, const uint8_t *data, int64_t data_bytes,
+                                   int nreq, const vb200_pcm_range *req, int pcm_s16, void *pcm, int32_t out_stride,
+                                   int32_t *got) {
+  CHECK_CTX(c);
+  if (nreq < 0) return fail(VB200_EINVAL, "nreq must be >= 0");
+  if (max_packets < 1) return fail(VB200_EINVAL, "max_packets must be >= 1");
+  if (nstreams < 0 || !npkt || !info || !data || !req || !pcm || !got || data_bytes < 0 || out_stride < 0)
+    return fail(VB200_EINVAL, "decode ranges pointers");
+  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
+  int rc;
+  if ((rc = ds_check_packets(nstreams, max_packets, npkt, info, data_bytes))) return rc;
+  for (int r = 0; r < nreq; r++)
+    if (req[r].stream < 0 || req[r].stream >= nstreams || req[r].start < 0 || req[r].length < 0 ||
+        req[r].length > out_stride)
+      return fail(VB200_EINVAL, "a request's stream, start or length is out of range");
+  if (nreq == 0) return 0;
+  std::lock_guard<std::mutex> lk(c->mu);
+  const size_t n = (size_t)nstreams * max_packets;      // nstreams >= 1: a request names a stream
+  const size_t pbytes = (pcm_s16 ? sizeof(int16_t) : sizeof(float)) * (size_t)nreq * c->setup.channels * out_stride;
+  HostIO io{c};
+  void *dn, *di, *dd, *dq, *dp, *dg;
+  if ((rc = io.h2d(npkt, sizeof(int32_t) * nstreams, &dn))) return rc;
+  if ((rc = io.h2d(info, sizeof(vb200_packet_info) * n, &di))) return rc;
+  if ((rc = io.h2d(nullptr, (size_t)data_bytes + 1, &dd))) return rc;
+  if (data_bytes) CU(cudaMemcpyAsync(dd, data, (size_t)data_bytes, cudaMemcpyHostToDevice, c->s_main));
+  if ((rc = io.h2d(req, sizeof(vb200_pcm_range) * nreq, &dq))) return rc;
+  if ((rc = io.h2d(nullptr, std::max<size_t>(pbytes, 1), &dp))) return rc;
+  if ((rc = io.h2d(nullptr, sizeof(int32_t) * nreq, &dg))) return rc;
+  if ((rc = vb200_decode_ranges_dev(c, nstreams, max_packets, (const int32_t *)dn, (const vb200_packet_info *)di,
+                                    (const uint8_t *)dd, nreq, (const vb200_pcm_range *)dq, pcm_s16, dp, out_stride,
+                                    (int32_t *)dg, c->s_main))) return rc;
+  if (pbytes && (rc = io.d2h(pcm, dp, pbytes))) return rc;
+  if ((rc = io.d2h(got, dg, sizeof(int32_t) * nreq))) return rc;
   return io.sync();
 }
 

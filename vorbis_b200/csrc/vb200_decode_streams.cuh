@@ -56,17 +56,8 @@ struct SinkTrim {
 };
 
 // the packet header as vorbis_synthesis reads it: the block flag, or OV_ENOTAUDIO / OV_EBADPACKET.  Modes 0 and 1
-// have block flags 0 and 1 (every vorbisenc setup); a higher mode number has no mode_param.  hdr of slots past
-// npkt[s] is not written.
-__global__ void __launch_bounds__(256)
-k_ds_header(int nstreams, int max_packets, int modebits, const int *__restrict__ npkt,
-            const vb200_packet_info *__restrict__ info, const unsigned char *__restrict__ data, int *__restrict__ hdr) {
-  const long long slot = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-  if (slot >= (long long)nstreams * max_packets) return;
-  const int st = (int)(slot / max_packets), k = (int)(slot - (long long)st * max_packets);
-  if (k >= npkt[st]) return;
-  const vb200_packet_info p = info[slot];
-  EntReader r{data + p.offset, 8ll * (p.bytes > 0 ? p.bytes : 0), 0};
+// have block flags 0 and 1 (every vorbisenc setup); a higher mode number has no mode_param.  r: the packet's bits.
+__device__ __forceinline__ int ds_packet_header(EntReader r, int modebits) {
   int v;
   if (r.read(1) != 0) v = -135;                            // OV_ENOTAUDIO, also for an empty packet
   else {
@@ -77,7 +68,66 @@ k_ds_header(int nstreams, int max_packets, int modebits, const int *__restrict__
       v = r.read(1) == -1 ? -136 : 1;                      // nW
     } else v = 0;
   }
-  hdr[slot] = v;
+  return v;
+}
+
+// one packet slot per thread; hdr of slots past npkt[s] is not written
+__global__ void __launch_bounds__(256)
+k_ds_header(int nstreams, int max_packets, int modebits, const int *__restrict__ npkt,
+            const vb200_packet_info *__restrict__ info, const unsigned char *__restrict__ data, int *__restrict__ hdr) {
+  const long long slot = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (slot >= (long long)nstreams * max_packets) return;
+  const int st = (int)(slot / max_packets), k = (int)(slot - (long long)st * max_packets);
+  if (k >= npkt[st]) return;
+  const vb200_packet_info p = info[slot];
+  hdr[slot] = ds_packet_header(EntReader{data + p.offset, 8ll * (p.bytes > 0 ? p.bytes : 0), 0}, modebits);
+}
+
+// blockin's bookkeeping for one packet that vorbis_synthesis accepted (block flag W): h advances, and [lo, hi) is
+// the window of the block's finished samples that pcmout returns (lib/block.c:741-751, 835-941, >> hs at half rate).
+// bs: blocksizes.  k_ds_plan runs the same step written out in its loop: called from there, this function changes
+// that kernel's register allocation, so its SASS would not stay as it was; the index and ranges tests check that the
+// two give the same windows.
+__device__ __forceinline__ void ds_blockin(DsHead &h, int W, const vb200_packet_info &p, const int *bs, int hs,
+                                           long long &lo_, long long &hi_) {
+  const int lW = h.W;
+  const long long fin = lW >= 0 ? (long long)((bs[lW] / 4 + bs[W] / 4) >> hs) : 0;
+  if (h.sequence == -1 || h.sequence + 1 != (long long)p.packetno) { h.granulepos = -1; h.sample_count = -1; }
+  h.sequence = p.packetno;
+  long long lo = 0, hi = fin;                              // pcm_returned, pcm_current past prevCenter
+  if (h.sample_count == -1) h.sample_count = 0;
+  else h.sample_count += bs[lW] / 4 + bs[W] / 4;
+  if (h.granulepos == -1) {
+    if (p.granulepos != -1) {
+      h.granulepos = p.granulepos;
+      if (h.sample_count > h.granulepos) {
+        long long extra = h.sample_count - p.granulepos;
+        if (extra < 0) extra = 0;
+        if (p.e_o_s) {                                     // trim the end
+          if (extra > (hi - lo) << hs) extra = (hi - lo) << hs;
+          hi -= extra >> hs;
+        } else {                                           // trim the beginning
+          lo += extra >> hs;
+          if (lo > hi) lo = hi;
+        }
+      }
+    }
+  } else {
+    h.granulepos += bs[lW] / 4 + bs[W] / 4;
+    if (p.granulepos != -1 && h.granulepos != p.granulepos) {
+      if (h.granulepos > p.granulepos) {
+        long long extra = h.granulepos - p.granulepos;
+        if (extra && p.e_o_s) {                            // partial last frame
+          if (extra > (hi - lo) << hs) extra = (hi - lo) << hs;
+          if (extra < 0) extra = 0;
+          hi -= extra >> hs;
+        }
+      }
+      h.granulepos = p.granulepos;
+    }
+  }
+  h.W = W;
+  lo_ = lo; hi_ = hi;
 }
 
 struct DsPlanArgs {

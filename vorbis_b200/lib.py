@@ -38,7 +38,8 @@ EXPORTS = [
     "vb200_decode_entropy_setup", "vb200_decode_entropy_dev", "vb200_decode_entropy",
     "vb200_decode_packets_resume_dev", "vb200_decode_packets_resume",
     "vb200_decode_streams_carry_bytes", "vb200_decode_streams_carry_init", "vb200_decode_streams_packets_dev",
-    "vb200_decode_streams_packets",
+    "vb200_decode_streams_packets", "vb200_decode_streams_index_dev", "vb200_decode_streams_index",
+    "vb200_decode_ranges_dev", "vb200_decode_ranges",
     "vb200_encode_entropy_setup", "vb200_encode_packet_bound", "vb200_encode_entropy_dev", "vb200_encode_entropy",
     "vb200_encode_packets", "vb200_encode_entropy_managed_dev", "vb200_encode_packets_managed",
     "vb200_residue_partvals", "vb200_residue_classify_dev", "vb200_residue_classify",
@@ -139,6 +140,12 @@ def load():
                                                    vp, vp]
     L.vb200_decode_streams_packets.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, C.c_int64, vp, C.c_int, vp,
                                                C.c_int64, vp, vp]
+    L.vb200_decode_streams_index_dev.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp, vp, vp]
+    L.vb200_decode_streams_index.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, C.c_int64, vp, vp]
+    L.vb200_decode_ranges_dev.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, C.c_int, vp, C.c_int, vp, C.c_int32, vp,
+                                          vp]
+    L.vb200_decode_ranges.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, C.c_int64, C.c_int, vp, C.c_int, vp,
+                                      C.c_int32, vp]
     L.vb200_encode_entropy_setup.argtypes = [vp, C.POINTER(abi.EncodeEntropySetup)]
     L.vb200_encode_packet_bound.argtypes = [vp, C.c_int]
     L.vb200_encode_entropy_dev.argtypes = [vp, C.c_int, C.c_int, vp, vp, vp, vp, C.c_int64, vp, vp, vp]
@@ -744,6 +751,51 @@ class Context:
         self._chk(self.L.vb200_decode_streams_packets_dev(self.h, nstreams, max_packets, _ptr(d_npkt), _ptr(d_info),
                                                           _ptr(d_data), _ptr(d_carry), pcm_s16, _ptr(d_pcm), pcm_cap,
                                                           _ptr(d_pcm_base), _ptr(d_out), _ptr(stream)))
+
+    # ---- sample ranges from packets ---------------------------------------------------------------
+    def decode_streams_index(self, npkt, info, data, check=True):
+        """vb200_decode_streams_index: the bookkeeping of a fresh-carry decode_streams_packets call without decoding.
+        Returns {"length" int64 [nstreams], "out" (DECODED_PACKET_DTYPE, shaped as info), "rc"}"""
+        npkt = np.ascontiguousarray(npkt, np.int32)
+        info = np.ascontiguousarray(info, abi.PACKET_INFO_DTYPE)
+        data = np.ascontiguousarray(data, np.uint8)
+        ns, mp = info.shape
+        length = np.zeros(ns, np.int64)
+        out = np.zeros((ns, mp), abi.DECODED_PACKET_DTYPE)
+        rc = self.L.vb200_decode_streams_index(self.h, ns, mp, _ptr(npkt), _ptr(info), _ptr(data), data.size,
+                                               _ptr(length), _ptr(out))
+        if check:
+            self._chk(rc)
+        return {"length": length, "out": out, "rc": rc}
+
+    def decode_streams_index_dev(self, nstreams, max_packets, d_npkt, d_info, d_data, d_length, d_out, stream=None):
+        self._chk(self.L.vb200_decode_streams_index_dev(self.h, nstreams, max_packets, _ptr(d_npkt), _ptr(d_info),
+                                                        _ptr(d_data), _ptr(d_length), _ptr(d_out), _ptr(stream)))
+
+    def decode_ranges(self, npkt, info, data, req, out_stride, s16=False, check=True):
+        """vb200_decode_ranges: req PCM_RANGE_DTYPE [nreq] (or (start, stream, length) rows).  Returns {"pcm": float
+        [nreq][ch][out_stride] or int16 [nreq][out_stride][ch], "got" int32 [nreq], "rc"}"""
+        npkt = np.ascontiguousarray(npkt, np.int32)
+        info = np.ascontiguousarray(info, abi.PACKET_INFO_DTYPE)
+        data = np.ascontiguousarray(data, np.uint8)
+        if not (isinstance(req, np.ndarray) and req.dtype == abi.PCM_RANGE_DTYPE):
+            req = np.array([tuple(r) for r in req], abi.PCM_RANGE_DTYPE)
+        req = np.ascontiguousarray(req)
+        ns, mp = info.shape
+        nreq, ch = len(req), self.channels
+        pcm = np.zeros((nreq, out_stride, ch) if s16 else (nreq, ch, out_stride), np.int16 if s16 else np.float32)
+        got = np.zeros(nreq, np.int32)
+        rc = self.L.vb200_decode_ranges(self.h, ns, mp, _ptr(npkt), _ptr(info), _ptr(data), data.size, nreq,
+                                        _ptr(req), 1 if s16 else 0, _ptr(pcm), out_stride, _ptr(got))
+        if check:
+            self._chk(rc)
+        return {"pcm": pcm, "got": got, "rc": rc}
+
+    def decode_ranges_dev(self, nstreams, max_packets, d_npkt, d_info, d_data, nreq, d_req, pcm_s16, d_pcm,
+                          out_stride, d_got, stream=None):
+        self._chk(self.L.vb200_decode_ranges_dev(self.h, nstreams, max_packets, _ptr(d_npkt), _ptr(d_info),
+                                                 _ptr(d_data), nreq, _ptr(d_req), pcm_s16, _ptr(d_pcm), out_stride,
+                                                 _ptr(d_got), _ptr(stream)))
 
     # ---- encode: the entropy coding of mapping0_forward on the device -----------------------------
     def encode_entropy_setup(self, es):
