@@ -40,11 +40,11 @@ CAPTURE = {(2, 32000, -0.1): ("floor1", T.floor1_signal), (2, 44100, -0.1): ("ch
 GENERIC = [(64, 8192), (128, 4096)]
 
 
-def _encoder_blocks(args, o):
+def _encoder_blocks(args, o, capture=CAPTURE):
     """the blocks the reference encoder cut from its stream (tests/golden/ref), in the layout of the golden encode
     fixtures that the tests of test_gpu_parity.py read: <tag>_pcm, _W, _lW, _nW, _blocktype, _ampmax_in, and the
     reference's quantised residue and nonzero flags (the oracle's, checked against the reference's digest)"""
-    group, signal = CAPTURE[args]
+    group, signal = capture[args]
     rec = G.load("%s_%s" % (group, G.case_id(*args)))
     tl = G.timeline(rec, signal(*args))
     bs = o.bs

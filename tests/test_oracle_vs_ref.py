@@ -10,19 +10,24 @@ import refgold as G
 from conftest import assert_bits_equal, probe_signal
 from vorbis_b200 import abi, lib as vlib
 
+# the setups vorbisenc picks above q = 0.5: full-band residue with the _residue_44_high / _hi_un / _44p_hi books,
+# uncoupled 5.1 (no coupling steps, two submaps), 96 kHz and coupled 22.05 kHz stereo (tests/test_gpu_high_quality.py)
+HIGH = [(2, 44100, 0.6), (2, 44100, 1.0), (1, 44100, 0.9), (6, 48000, 0.5), (6, 48000, 0.9), (2, 96000, 0.7),
+        (2, 22050, 0.9)]
+HIGH_NEW = [a for a in HIGH if a != (2, 96000, 0.7)]          # the lists that already hold (2, 96000, 0.7)
 GRID = [(2, 44100, 0.5), (1, 44100, 0.4), (2, 44100, 0.1), (2, 44100, 0.3), (1, 44100, 0.2),
-        (2, 48000, 0.9), (2, 32000, 0.0), (1, 22050, 0.3), (2, 44100, -0.1), (6, 48000, -0.1)]
-FLOOR1_ARGS = [(2, 44100, 0.5), (6, 48000, 0.2), (2, 32000, -0.1), (1, 16000, 0.5), (2, 96000, 0.7)]
+        (2, 48000, 0.9), (2, 32000, 0.0), (1, 22050, 0.3), (2, 44100, -0.1), (6, 48000, -0.1)] + HIGH
+FLOOR1_ARGS = [(2, 44100, 0.5), (6, 48000, 0.2), (2, 32000, -0.1), (1, 16000, 0.5), (2, 96000, 0.7)] + HIGH_NEW
 CHAIN_ARGS = [(2, 44100, 0.5), (2, 44100, 0.1), (1, 44100, 0.4), (6, 48000, 0.2),
-              (2, 44100, -0.1), (6, 48000, -0.1), (2, 96000, -0.1)]
+              (2, 44100, -0.1), (6, 48000, -0.1), (2, 96000, -0.1)] + HIGH
 MANAGED_ARGS = [(2, 44100, 0.5), (1, 44100, 0.4), (6, 48000, 0.2),
-                (2, 44100, -0.1), (6, 48000, -0.1), (2, 96000, -0.1)]
+                (2, 44100, -0.1), (6, 48000, -0.1), (2, 96000, -0.1)] + HIGH
 ENVELOPE_ARGS = [(2, 44100, 0.5), (1, 44100, 0.4), (6, 48000, 0.2), (1, 22050, 0.3), (2, 32000, 0.0), (2, 96000, 0.7),
-                 (2, 44100, -0.1), (6, 48000, -0.1), (2, 96000, -0.1)]
+                 (2, 44100, -0.1), (6, 48000, -0.1), (2, 96000, -0.1)] + HIGH_NEW
 INVERSE2_ARGS = [(2, 44100, 0.5), (6, 48000, 0.2), (1, 22050, 0.3),
-                 (2, 44100, -0.1), (6, 48000, -0.1), (2, 96000, -0.1)]
+                 (2, 44100, -0.1), (6, 48000, -0.1), (2, 96000, -0.1)] + HIGH
 RESIDUE_ARGS = [(2, 44100, 0.5), (1, 44100, 0.4), (6, 48000, 0.2), (1, 22050, 0.3), (2, 44100, 0.1),
-                (2, 44100, -0.1), (6, 48000, -0.1), (2, 96000, -0.1)]
+                (2, 44100, -0.1), (6, 48000, -0.1), (2, 96000, -0.1)] + HIGH
 IDS = lambda g: G.case_id(*g)  # noqa: E731
 
 
