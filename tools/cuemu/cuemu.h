@@ -214,6 +214,7 @@ static inline size_t __cvta_generic_to_shared(const void *p) { return (size_t)((
 template <class T> static inline T atomicAdd(T *p, T v) { return __atomic_fetch_add(p, v, __ATOMIC_RELAXED); }
 static inline int atomicAnd(int *p, int v) { return __atomic_fetch_and(p, v, __ATOMIC_RELAXED); }
 static inline unsigned atomicOr(unsigned *p, unsigned v) { return __atomic_fetch_or(p, v, __ATOMIC_RELAXED); }
+static inline int atomicOr(int *p, int v) { return __atomic_fetch_or(p, v, __ATOMIC_RELAXED); }
 static inline int atomicMax(int *p, int v) { int o = __atomic_load_n(p, __ATOMIC_RELAXED); while (o < v && !__atomic_compare_exchange_n(p, &o, v, true, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {} return o; }
 static inline long long clock64() { return 0; }
 

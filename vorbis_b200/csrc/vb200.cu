@@ -942,26 +942,33 @@ struct SinkS16 {
   }
 };
 
+// The four forms of the synthesis, one instance each per sink and rate:
+// PLAIN (vb200_synthesis[_s16], vb200_decode_dsp): every stream decodes nblk blocks from a fresh state; block 0 primes.
+// CARRY (vb200_decode_dsp_resume, vb200_decode_packets_resume): stream st decodes count[st] <= nblk blocks, and the
+// overlap of every (stream, channel) = task comes from / goes back to carry_W[task] and
+// carry_tail[task * tail_stride]: the block flag and the right half of the last IMDCT (what v->pcm holds after
+// lib/block.c:817-823).  With a carried W >= 0, block 0 overlap-adds onto that tail and finishes samples like any
+// later block; with -1 it only primes.  A stream with count 0 is not touched.  W is kept per (stream, channel)
+// because the CTA of one channel must not read what the CTA of another channel of the same stream writes.
 // TRIM (vb200_decode_streams_packets): as CARRY, with the carry of stream st in its slot of T.carry and the carried
 // flag from T.W_in (what k_ds_plan read before anything wrote the heads); block k writes only [lo, hi) = T.win of
 // its finished samples, from pcm_off (relative to the stream's pcm_base) on, into the packed layout of the call.
 // Nothing is written, carries included, when the call's output does not fit T.cap.  Channel 0 commits the head.
-// CARRY (vb200_decode_dsp_resume): stream st decodes count[st] <= nblk blocks, and the overlap of every
-// (stream, channel) = task comes from / goes back to carry_W[task] and carry_tail[task * tail_stride]: the
-// block flag and the right half of the last IMDCT (what v->pcm holds after lib/block.c:817-823).  With a
-// carried W >= 0, block 0 overlap-adds onto that tail and finishes samples like any later block; with -1 it
-// only primes.  A stream with count 0 is not touched.  W is kept per (stream, channel) because the CTA of
-// one channel must not read what the CTA of another channel of the same stream writes.
-// FRESH (with TRIM, vb200_decode_ranges): every "stream" (a request) starts from a fresh state, so block 0 primes;
-// T.cap, T.W_in, T.head and the carries are neither read nor written.
-template <bool S16, bool HS, bool CARRY, bool TRIM = false, bool FRESH = false>
-__device__ __forceinline__ void
-synthesis_body(const XformDev &X0, const XformDev &X1, const WinDev &Wd, int ch, int nstreams, int nblk,
-               const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
-               const float *__restrict__ coef, const long long *__restrict__ pcm_off,
-               void *__restrict__ pcm_out, long long pcm_stride, const int *__restrict__ count,
-               float *__restrict__ carry_tail, int *__restrict__ carry_W, int tail_stride,
-               const DsTrim &T = DsTrim{}) {
+// RANGE (vb200_decode_ranges): as TRIM, but every "stream" is a request that starts from a fresh state, so block 0
+// primes; request r's row of the output is at T.base[r] = r * out_stride.  T.cap, T.W_in, T.head and the carries
+// are neither read nor written.
+// Arguments a form does not name are not read: carry_* in all but CARRY, pcm_stride in TRIM and RANGE, T in PLAIN
+// and CARRY.
+enum SynthMode { SYN_PLAIN, SYN_CARRY, SYN_TRIM, SYN_RANGE };
+
+template <bool S16, bool HS, SynthMode MODE>
+__global__ void __launch_bounds__(256)
+k_synthesis(XformDev X0, XformDev X1, WinDev Wd, int ch, int nstreams, int nblk,
+            const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
+            const float *__restrict__ coef, const long long *__restrict__ pcm_off,
+            void *__restrict__ pcm_out, long long pcm_stride, const int *__restrict__ count,
+            float *__restrict__ carry_tail, int *__restrict__ carry_W, int tail_stride, DsTrim T) {
+  constexpr bool CARRY = MODE == SYN_CARRY, TRIM = MODE == SYN_TRIM || MODE == SYN_RANGE, FRESH = MODE == SYN_RANGE;
   extern __shared__ __align__(16) float sm[];
   const int tid = threadIdx.x, nt = blockDim.x;
   const int n0 = X0.N >> 1, n1 = X1.N >> 1;
@@ -1053,48 +1060,6 @@ synthesis_body(const XformDev &X0, const XformDev &X1, const WinDev &Wd, int ch,
   }
 }
 
-template <bool S16, bool HS>
-__global__ void __launch_bounds__(256)
-k_synthesis(XformDev X0, XformDev X1, WinDev Wd, int ch, int nstreams, int nblk,
-            const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
-            const float *__restrict__ coef, const long long *__restrict__ pcm_off,
-            void *__restrict__ pcm_out, long long pcm_stride) {
-  synthesis_body<S16, HS, false>(X0, X1, Wd, ch, nstreams, nblk, Wseq, coef_off, coef, pcm_off, pcm_out, pcm_stride,
-                                 nullptr, nullptr, nullptr, 0);
-}
-
-template <bool S16, bool HS>
-__global__ void __launch_bounds__(256)
-k_synthesis_carry(XformDev X0, XformDev X1, WinDev Wd, int ch, int nstreams, int nblk,
-                  const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
-                  const float *__restrict__ coef, const long long *__restrict__ pcm_off,
-                  void *__restrict__ pcm_out, long long pcm_stride, const int *__restrict__ count,
-                  float *__restrict__ carry_tail, int *__restrict__ carry_W, int tail_stride) {
-  synthesis_body<S16, HS, true>(X0, X1, Wd, ch, nstreams, nblk, Wseq, coef_off, coef, pcm_off, pcm_out, pcm_stride,
-                                count, carry_tail, carry_W, tail_stride);
-}
-
-template <bool S16, bool HS>
-__global__ void __launch_bounds__(256)
-k_synthesis_trim(XformDev X0, XformDev X1, WinDev Wd, int ch, int nstreams, int nblk,
-                 const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
-                 const float *__restrict__ coef, const long long *__restrict__ pcm_off,
-                 void *__restrict__ pcm_out, const int *__restrict__ count, DsTrim T) {
-  synthesis_body<S16, HS, false, true>(X0, X1, Wd, ch, nstreams, nblk, Wseq, coef_off, coef, pcm_off, pcm_out, 0,
-                                       count, nullptr, nullptr, T.tail_stride, T);
-}
-
-// vb200_decode_ranges: request r is "stream" r, its row of the output at T.base[r] = r * out_stride; block 0 primes
-template <bool S16, bool HS>
-__global__ void __launch_bounds__(256)
-k_synthesis_range(XformDev X0, XformDev X1, WinDev Wd, int ch, int nreq, int nblk,
-                  const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
-                  const float *__restrict__ coef, const long long *__restrict__ pcm_off,
-                  void *__restrict__ pcm_out, const int *__restrict__ count, DsTrim T) {
-  synthesis_body<S16, HS, false, true, true>(X0, X1, Wd, ch, nreq, nblk, Wseq, coef_off, coef, pcm_off, pcm_out, 0,
-                                             count, nullptr, nullptr, 0, T);
-}
-
 // ---- decode: undo channel coupling, lib/mapping0.c:754-779 (square polar -> L/R), in place
 __global__ void __launch_bounds__(256)
 k_decouple(int n, int ch, int steps, const int *__restrict__ mag, const int *__restrict__ ang,
@@ -1104,17 +1069,7 @@ k_decouple(int n, int ch, int steps, const int *__restrict__ mag, const int *__r
     const long long blk = e / n;
     const int j = (int)(e - blk * n);
     float *base = res + blk * (long long)ch * n + j;
-    for (int s = steps - 1; s >= 0; s--) {
-      float *pM = base + (long long)mag[s] * n, *pA = base + (long long)ang[s] * n;
-      const float m = *pM, a = *pA;
-      if (m > 0.f) {
-        if (a > 0.f) { *pM = m; *pA = m - a; }
-        else         { *pA = m; *pM = m + a; }
-      } else {
-        if (a > 0.f) { *pM = m; *pA = m + a; }
-        else         { *pA = m; *pM = m - a; }
-      }
-    }
+    for (int s = steps - 1; s >= 0; s--) dev_decouple(base + (long long)mag[s] * n, base + (long long)ang[s] * n);
   }
 }
 
@@ -1213,6 +1168,12 @@ struct HostIO {
     if (slot == STAGE_SLOTS) return fail(VB200_EFAULT, "host call stages more buffers than the staging pool holds");
     int rc = ensure_buf(c->stage[slot++], bytes, d); if (rc) return rc;
     if (src) CU(cudaMemcpyAsync(*d, src, bytes, cudaMemcpyHostToDevice, c->s_main));
+    return 0;
+  }
+  // packet bytes: the buffer is one byte longer, so that it exists when there are none
+  int h2d_packets(const uint8_t *src, int64_t bytes, void **d) {
+    int rc = h2d(nullptr, (size_t)bytes + 1, d); if (rc) return rc;
+    if (bytes) CU(cudaMemcpyAsync(*d, src, (size_t)bytes, cudaMemcpyHostToDevice, c->s_main));
     return 0;
   }
   int d2h(void *dst, const void *d, size_t bytes) {
@@ -1754,17 +1715,24 @@ extern "C" int vb200_synthesis_halfrate(vb200_ctx *c, int flag, const float *con
   return 0;
 }
 
-template <bool S16, bool HS>
-static int synthesis_launch(vb200_ctx *c, int nstreams, int nblk, const int32_t *d_Wseq, const int64_t *d_coef_off,
-                            const float *d_coef, const int64_t *d_pcm_off, void *d_pcm, int64_t pcm_stride,
-                            void *stream) {
-  const XformDev *X = HS ? c->dx_hs : c->dx;
+// every synthesis launch: smem, threads and grid from the context's transforms (half-rate or full), then the
+// S16 x half-rate instance of MODE.  k: the carry of CARRY; T: the tables of TRIM and RANGE.
+template <SynthMode MODE>
+static int synthesis_launch(vb200_ctx *c, bool s16, int nstreams, int nblk, const int32_t *d_count,
+                            const int32_t *d_Wseq, const int64_t *d_coef_off, const float *d_coef,
+                            const int64_t *d_pcm_off, void *d_pcm, int64_t pcm_stride, const vb200_decode_carry *k,
+                            const DsTrim &T, cudaStream_t st) {
+  const bool hs = c->halfrate;
+  const XformDev *X = hs ? c->dx_hs : c->dx;
   const int ch = c->setup.channels, N1 = X[1].N;
   const size_t smem = sizeof(float) * ((size_t)N1 / 2 + N1 + N1 / 2);
-  int rc = set_smem(k_synthesis<S16, HS>, smem); if (rc) return rc;
-  k_synthesis<S16, HS><<<grid_for(c, nstreams * ch, 8), threads_for(N1), smem, (cudaStream_t)stream>>>(
-      X[0], X[1], HS ? c->dwin_hs : c->dwin, ch, nstreams, nblk, d_Wseq, (const long long *)d_coef_off, d_coef,
-      (const long long *)d_pcm_off, d_pcm, (long long)pcm_stride);
+  auto *kern = s16 ? (hs ? k_synthesis<true, true, MODE> : k_synthesis<true, false, MODE>)
+                   : (hs ? k_synthesis<false, true, MODE> : k_synthesis<false, false, MODE>);
+  int rc = set_smem(kern, smem); if (rc) return rc;
+  kern<<<grid_for(c, nstreams * ch, 8), threads_for(N1), smem, st>>>(
+      X[0], X[1], hs ? c->dwin_hs : c->dwin, ch, nstreams, nblk, d_Wseq, (const long long *)d_coef_off, d_coef,
+      (const long long *)d_pcm_off, d_pcm, (long long)pcm_stride, d_count, k ? k->tail : nullptr,
+      k ? k->W : nullptr, c->setup.blocksizes[1] / 2, T);
   return post_launch(c);
 }
 
@@ -1773,9 +1741,8 @@ extern "C" int vb200_synthesis_dev(vb200_ctx *c, int nstreams, int nblk, const i
                                    const int64_t *d_pcm_off, float *d_pcm, int64_t pcm_stride, void *stream) {
   CHECK_CTX(c);
   if (nstreams <= 0 || nblk <= 0) return 0;
-  return c->halfrate
-      ? synthesis_launch<false, true>(c, nstreams, nblk, d_Wseq, d_coef_off, d_coef, d_pcm_off, d_pcm, pcm_stride, stream)
-      : synthesis_launch<false, false>(c, nstreams, nblk, d_Wseq, d_coef_off, d_coef, d_pcm_off, d_pcm, pcm_stride, stream);
+  return synthesis_launch<SYN_PLAIN>(c, false, nstreams, nblk, nullptr, d_Wseq, d_coef_off, d_coef, d_pcm_off, d_pcm,
+                                     pcm_stride, nullptr, DsTrim{}, (cudaStream_t)stream);
 }
 
 extern "C" int vb200_synthesis_s16_dev(vb200_ctx *c, int nstreams, int nblk, const int32_t *d_Wseq,
@@ -1783,9 +1750,8 @@ extern "C" int vb200_synthesis_s16_dev(vb200_ctx *c, int nstreams, int nblk, con
                                        const int64_t *d_pcm_off, int16_t *d_pcm16, int64_t pcm_stride, void *stream) {
   CHECK_CTX(c);
   if (nstreams <= 0 || nblk <= 0) return 0;
-  return c->halfrate
-      ? synthesis_launch<true, true>(c, nstreams, nblk, d_Wseq, d_coef_off, d_coef, d_pcm_off, d_pcm16, pcm_stride, stream)
-      : synthesis_launch<true, false>(c, nstreams, nblk, d_Wseq, d_coef_off, d_coef, d_pcm_off, d_pcm16, pcm_stride, stream);
+  return synthesis_launch<SYN_PLAIN>(c, true, nstreams, nblk, nullptr, d_Wseq, d_coef_off, d_coef, d_pcm_off, d_pcm16,
+                                     pcm_stride, nullptr, DsTrim{}, (cudaStream_t)stream);
 }
 
 extern "C" int vb200_synthesis(vb200_ctx *c, int nstreams, int nblk, const int32_t *Wseq,
@@ -2703,18 +2669,51 @@ extern "C" int vb200_floor1_inverse2(vb200_ctx *c, int W, int floor_sel, int nro
   return io.sync();
 }
 
-static int decode_prep_args(vb200_ctx *c, int nstreams, int nblk, DecodePrepArgs *A) {
+static size_t entropy_smem(const EntDev &E, bool fused) {
+  return (fused ? sizeof(int32_t) * (size_t)E.ch * (VB200_FLOOR1_STRIDE + 1) : 0) + 2 * (size_t)E.ch + E.cls_cap;
+}
+
+// CTAs per SM of k_decode_packets' grid.  One thread of each CTA decodes a packet serially while the others wait,
+// but the kernel takes 80 registers (-Xptxas -v, sm_90a), so at most 6 CTAs of 128 threads are resident per SM;
+// a grid of more than k_decode_prepare's 8 per SM would only queue
+static const int DECODE_PACKETS_CTAS = 8;
+
+static int ent_check(const vb200_ctx *c) {
+  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
+  return 0;
+}
+
+// the front half of every decode chain on nstreams x nblk blocks: de-coupling and the floor-1 multiply of each
+// block's rows in d_res, from the posts and presence of vb200_decode_entropy (k_decode_prepare) or, with packets P,
+// from the entropy decode of each block's packet in front of them (k_decode_packets).  With d_count, the blocks of a
+// stream past its count are skipped.
+static int decode_front(vb200_ctx *c, int nstreams, int nblk, const int32_t *d_count, const int32_t *d_Wseq,
+                        const int64_t *d_coef_off, float *d_res, const int32_t *d_posts, const int32_t *d_present,
+                        const DecodePackets *P, cudaStream_t st) {
   const int ch = c->setup.channels;
+  DecodePrepArgs A;
   for (int w = 0; w < 2; w++) {
     for (int k = 0; k < ch; k++)
       if (c->setup.floor1[w][c->setup.chmux[w][k]].posts <= 0)
         return fail(VB200_EINVAL, "no floor1 setup for a channel's submap");
-    A->floors[w] = c->d_floor[w]; A->chmux[w] = c->d_chmux[w];
-    A->mag[w] = c->d_mag[w]; A->ang[w] = c->d_ang[w];
-    A->steps[w] = c->setup.coupling_steps[w]; A->n[w] = c->dx[w].N / 2;
+    A.floors[w] = c->d_floor[w]; A.chmux[w] = c->d_chmux[w];
+    A.mag[w] = c->d_mag[w]; A.ang[w] = c->d_ang[w];
+    A.steps[w] = c->setup.coupling_steps[w]; A.n[w] = c->dx[w].N / 2;
   }
-  A->ch = ch; A->nblk = nblk; A->nitems = (long)nstreams * nblk;
-  return 0;
+  A.ch = ch; A.nblk = nblk; A.nitems = (long)nstreams * nblk;
+  const long long *coef_off = (const long long *)d_coef_off;
+  if (P) {
+    const size_t smem = entropy_smem(c->ent, true);
+    auto *kern = d_count ? k_decode_packets<true> : k_decode_packets<false>;
+    int rc = set_smem(kern, smem); if (rc) return rc;
+    kern<<<grid_for(c, (int)A.nitems, DECODE_PACKETS_CTAS), 128, smem, st>>>(A, c->ent, *P, d_Wseq, coef_off, d_res,
+                                                                            c->d_fromdB, d_count);
+  } else {
+    auto *kern = d_count ? k_decode_prepare<true> : k_decode_prepare<false>;
+    kern<<<grid_for(c, (int)A.nitems, 8), 128, 0, st>>>(A, d_Wseq, coef_off, d_res, d_posts, d_present, c->d_fromdB,
+                                                        d_count);
+  }
+  return post_launch(c);
 }
 
 extern "C" int vb200_decode_dsp_dev(vb200_ctx *c, int nstreams, int nblk, const int32_t *d_Wseq, const int64_t *d_coef_off,
@@ -2724,14 +2723,12 @@ extern "C" int vb200_decode_dsp_dev(vb200_ctx *c, int nstreams, int nblk, const 
   if (nstreams <= 0 || nblk <= 0) return 0;
   if (!d_Wseq || !d_coef_off || !d_res || !d_posts || !d_present || !d_pcm_off || !d_pcm)
     return fail(VB200_EINVAL, "decode pointers");
-  DecodePrepArgs A;
+  const cudaStream_t st = (cudaStream_t)stream;
   int rc;
-  if ((rc = decode_prep_args(c, nstreams, nblk, &A))) return rc;
-  k_decode_prepare<<<grid_for(c, (int)A.nitems, 8), 128, 0, (cudaStream_t)stream>>>(
-      A, d_Wseq, (const long long *)d_coef_off, d_res, d_posts, d_present, c->d_fromdB);
-  if ((rc = post_launch(c))) return rc;
-  if (pcm_s16) return vb200_synthesis_s16_dev(c, nstreams, nblk, d_Wseq, d_coef_off, d_res, d_pcm_off, (int16_t *)d_pcm, pcm_stride, stream);
-  return vb200_synthesis_dev(c, nstreams, nblk, d_Wseq, d_coef_off, d_res, d_pcm_off, (float *)d_pcm, pcm_stride, stream);
+  if ((rc = decode_front(c, nstreams, nblk, nullptr, d_Wseq, d_coef_off, d_res, d_posts, d_present, nullptr, st)))
+    return rc;
+  return synthesis_launch<SYN_PLAIN>(c, pcm_s16, nstreams, nblk, nullptr, d_Wseq, d_coef_off, d_res, d_pcm_off, d_pcm,
+                                     pcm_stride, nullptr, DsTrim{}, st);
 }
 
 extern "C" int vb200_decode_dsp(vb200_ctx *c, int nstreams, int nblk, const int32_t *Wseq, const int64_t *coef_off,
@@ -2763,19 +2760,56 @@ extern "C" int vb200_decode_dsp(vb200_ctx *c, int nstreams, int nblk, const int3
 }
 
 // ---- decode resumed across calls: the overlap of every (stream, channel) carried in vb200_decode_carry
-template <bool S16, bool HS>
-static int synthesis_carry_launch(vb200_ctx *c, int nstreams, int nblk, const int32_t *d_count, const int32_t *d_Wseq,
-                                  const int64_t *d_coef_off, const float *d_coef, const int64_t *d_pcm_off,
-                                  void *d_pcm, int64_t pcm_stride, const vb200_decode_carry *k, void *stream) {
-  const XformDev *X = HS ? c->dx_hs : c->dx;
-  const int ch = c->setup.channels, N1 = X[1].N;
-  const size_t smem = sizeof(float) * ((size_t)N1 / 2 + N1 + N1 / 2);
-  int rc = set_smem(k_synthesis_carry<S16, HS>, smem); if (rc) return rc;
-  k_synthesis_carry<S16, HS><<<grid_for(c, nstreams * ch, 8), threads_for(N1), smem, (cudaStream_t)stream>>>(
-      X[0], X[1], HS ? c->dwin_hs : c->dwin, ch, nstreams, nblk, d_Wseq, (const long long *)d_coef_off, d_coef,
-      (const long long *)d_pcm_off, d_pcm, (long long)pcm_stride, d_count, k->tail, k->W, c->setup.blocksizes[1] / 2);
-  return post_launch(c);
+// host-form checks of the blocks of nstreams x nblk: count[s] in [0, nblk] (all nblk without count), then of each
+// counted block in order its flag and, for the packet forms (pkt_off given), its packet inside data and its rows
+// inside res
+static int blocks_check(const vb200_ctx *c, int nstreams, int nblk, const int32_t *count, const int32_t *Wseq,
+                        const int64_t *pkt_off, const int32_t *pkt_bytes, int64_t data_bytes, const int64_t *coef_off,
+                        int64_t res_len) {
+  const int ch = c->setup.channels;
+  for (int s = 0; s < nstreams; s++) {
+    const int n = count ? count[s] : nblk;
+    if (n < 0 || n > nblk) return fail(VB200_EINVAL, "count[s] must be in [0, nblk]");
+    for (int k = 0; k < n; k++) {
+      const size_t i = (size_t)s * nblk + k;
+      if (Wseq[i] < 0 || Wseq[i] > 1) return fail(VB200_EINVAL, "Wseq values must be 0/1");
+      if (!pkt_off) continue;
+      if (pkt_bytes[i] < 0 || pkt_off[i] < 0 || pkt_off[i] > data_bytes || pkt_bytes[i] > data_bytes - pkt_off[i])
+        return fail(VB200_EINVAL, "packet outside data");
+      if (coef_off[i] < 0 || coef_off[i] + (int64_t)ch * (c->setup.blocksizes[Wseq[i]] / 2) > res_len)
+        return fail(VB200_EINVAL, "block rows outside res");
+    }
+  }
+  return 0;
 }
+
+// the vb200_decode_carry of a _resume host form: checked, staged after the call's other inputs, and written back
+// after its PCM
+struct HostCarry {
+  vb200_decode_carry *h;
+  size_t ntask, tbytes;
+  vb200_decode_carry d{};
+  HostCarry(const vb200_ctx *c, int nstreams, vb200_decode_carry *carry)
+      : h(carry), ntask((size_t)nstreams * c->setup.channels),
+        tbytes(sizeof(float) * ntask * (size_t)(c->setup.blocksizes[1] / 2)) {}
+  int check() const {
+    for (size_t i = 0; i < ntask; i++)
+      if (h->W[i] < -1 || h->W[i] > 1) return fail(VB200_EINVAL, "carried W must be -1, 0 or 1");
+    return 0;
+  }
+  int stage(HostIO &io) {
+    void *t, *w; int rc;
+    if ((rc = io.h2d(h->tail, tbytes, &t))) return rc;
+    if ((rc = io.h2d(h->W, sizeof(int32_t) * ntask, &w))) return rc;
+    d = vb200_decode_carry{(float *)t, (int32_t *)w};
+    return 0;
+  }
+  int write_back(HostIO &io) const {
+    int rc;
+    if ((rc = io.d2h(h->tail, d.tail, tbytes))) return rc;
+    return io.d2h(h->W, d.W, sizeof(int32_t) * ntask);
+  }
+};
 
 extern "C" int vb200_decode_dsp_resume_dev(vb200_ctx *c, int nstreams, int nblk, const int32_t *d_count,
                                            const int32_t *d_Wseq, const int64_t *d_coef_off, float *d_res,
@@ -2787,22 +2821,12 @@ extern "C" int vb200_decode_dsp_resume_dev(vb200_ctx *c, int nstreams, int nblk,
   if (!d_Wseq || !d_coef_off || !d_res || !d_posts || !d_present || !d_pcm_off || !d_pcm || !d_carry ||
       !d_carry->tail || !d_carry->W)
     return fail(VB200_EINVAL, "decode pointers");
-  DecodePrepArgs A;
+  const cudaStream_t st = (cudaStream_t)stream;
   int rc;
-  if ((rc = decode_prep_args(c, nstreams, nblk, &A))) return rc;
-  if (d_count)
-    k_decode_prepare_counted<<<grid_for(c, (int)A.nitems, 8), 128, 0, (cudaStream_t)stream>>>(
-        A, d_Wseq, (const long long *)d_coef_off, d_res, d_posts, d_present, c->d_fromdB, d_count);
-  else
-    k_decode_prepare<<<grid_for(c, (int)A.nitems, 8), 128, 0, (cudaStream_t)stream>>>(
-        A, d_Wseq, (const long long *)d_coef_off, d_res, d_posts, d_present, c->d_fromdB);
-  if ((rc = post_launch(c))) return rc;
-  const bool hs = c->halfrate;
-  if (pcm_s16)
-    return hs ? synthesis_carry_launch<true, true>(c, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_pcm_off, d_pcm, pcm_stride, d_carry, stream)
-              : synthesis_carry_launch<true, false>(c, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_pcm_off, d_pcm, pcm_stride, d_carry, stream);
-  return hs ? synthesis_carry_launch<false, true>(c, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_pcm_off, d_pcm, pcm_stride, d_carry, stream)
-            : synthesis_carry_launch<false, false>(c, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_pcm_off, d_pcm, pcm_stride, d_carry, stream);
+  if ((rc = decode_front(c, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_posts, d_present, nullptr, st)))
+    return rc;
+  return synthesis_launch<SYN_CARRY>(c, pcm_s16, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_pcm_off, d_pcm,
+                                     pcm_stride, d_carry, DsTrim{}, st);
 }
 
 extern "C" int vb200_decode_dsp_resume(vb200_ctx *c, int nstreams, int nblk, const int32_t *count, const int32_t *Wseq,
@@ -2814,19 +2838,14 @@ extern "C" int vb200_decode_dsp_resume(vb200_ctx *c, int nstreams, int nblk, con
   if (!Wseq || !coef_off || !res || !posts || !present || !pcm_off || !pcm || !carry || !carry->tail || !carry->W)
     return fail(VB200_EINVAL, "decode pointers");
   const int ch = c->setup.channels;
-  const size_t nb = (size_t)nstreams * nblk, ntask = (size_t)nstreams * ch;
-  for (int s = 0; s < nstreams; s++) {
-    const int n = count ? count[s] : nblk;
-    if (n < 0 || n > nblk) return fail(VB200_EINVAL, "count[s] must be in [0, nblk]");
-    for (int k = 0; k < n; k++)
-      if (Wseq[(size_t)s * nblk + k] < 0 || Wseq[(size_t)s * nblk + k] > 1) return fail(VB200_EINVAL, "Wseq values must be 0/1");
-  }
-  for (size_t i = 0; i < ntask; i++)
-    if (carry->W[i] < -1 || carry->W[i] > 1) return fail(VB200_EINVAL, "carried W must be -1, 0 or 1");
+  const size_t nb = (size_t)nstreams * nblk;
+  HostCarry k(c, nstreams, carry);
+  int rc;
+  if ((rc = blocks_check(c, nstreams, nblk, count, Wseq, nullptr, nullptr, 0, nullptr, 0))) return rc;
+  if ((rc = k.check())) return rc;
   std::lock_guard<std::mutex> lk(c->mu);
-  const size_t tbytes = sizeof(float) * ntask * (size_t)(c->setup.blocksizes[1] / 2);
   HostIO io{c};
-  void *dW, *dco, *dc, *dpo, *dp, *dps, *dpr, *dn = nullptr, *dkt, *dkw; int rc;
+  void *dW, *dco, *dc, *dpo, *dp, *dps, *dpr, *dn = nullptr;
   if ((rc = io.h2d(Wseq, sizeof(int32_t) * nb, &dW))) return rc;
   if ((rc = io.h2d(coef_off, sizeof(int64_t) * nb, &dco))) return rc;
   if ((rc = io.h2d(res, sizeof(float) * (size_t)res_len, &dc))) return rc;
@@ -2836,16 +2855,13 @@ extern "C" int vb200_decode_dsp_resume(vb200_ctx *c, int nstreams, int nblk, con
   if ((rc = io.h2d(posts, sizeof(int32_t) * nb * ch * VB200_FLOOR1_STRIDE, &dps))) return rc;
   if ((rc = io.h2d(present, sizeof(int32_t) * nb * ch, &dpr))) return rc;
   if (count && (rc = io.h2d(count, sizeof(int32_t) * nstreams, &dn))) return rc;
-  if ((rc = io.h2d(carry->tail, tbytes, &dkt))) return rc;
-  if ((rc = io.h2d(carry->W, sizeof(int32_t) * ntask, &dkw))) return rc;
+  if ((rc = k.stage(io))) return rc;
   CU(cudaMemsetAsync(dp, 0, pbytes, c->s_main));
-  const vb200_decode_carry dk{(float *)dkt, (int32_t *)dkw};
   if ((rc = vb200_decode_dsp_resume_dev(c, nstreams, nblk, (const int32_t *)dn, (const int32_t *)dW,
                                         (const int64_t *)dco, (float *)dc, (const int32_t *)dps, (const int32_t *)dpr,
-                                        (const int64_t *)dpo, dp, pcm_s16, pcm_stride, &dk, c->s_main))) return rc;
+                                        (const int64_t *)dpo, dp, pcm_s16, pcm_stride, &k.d, c->s_main))) return rc;
   if ((rc = io.d2h(pcm, dp, pbytes))) return rc;
-  if ((rc = io.d2h(carry->tail, dkt, tbytes))) return rc;
-  if ((rc = io.d2h(carry->W, dkw, sizeof(int32_t) * ntask))) return rc;
+  if ((rc = k.write_back(io))) return rc;
   return io.sync();
 }
 
@@ -3051,10 +3067,6 @@ extern "C" int vb200_decode_entropy_setup(vb200_ctx *c, const vb200_entropy_setu
   return 0;
 }
 
-static size_t entropy_smem(const EntDev &E, bool fused) {
-  return (fused ? sizeof(int32_t) * (size_t)E.ch * (VB200_FLOOR1_STRIDE + 1) : 0) + 2 * (size_t)E.ch + E.cls_cap;
-}
-
 extern "C" int vb200_decode_entropy_dev(vb200_ctx *c, int nblocks, const int32_t *d_Wseq, const int64_t *d_pkt_off,
                                         const int32_t *d_pkt_bytes, const uint8_t *d_data, const int64_t *d_coef_off,
                                         float *d_res, int32_t *d_posts, int32_t *d_present, void *stream) {
@@ -3062,21 +3074,15 @@ extern "C" int vb200_decode_entropy_dev(vb200_ctx *c, int nblocks, const int32_t
   if (nblocks <= 0) return 0;
   if (!d_Wseq || !d_pkt_off || !d_pkt_bytes || !d_data || !d_coef_off || !d_res || !d_posts || !d_present)
     return fail(VB200_EINVAL, "decode_entropy pointers");
-  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
+  int rc;
+  if ((rc = ent_check(c))) return rc;
   const size_t smem = entropy_smem(c->ent, false);
-  int rc = set_smem(k_decode_entropy, smem); if (rc) return rc;
+  if ((rc = set_smem(k_decode_entropy, smem))) return rc;
   const DecodePackets P{(const long long *)d_pkt_off, d_pkt_bytes, d_data};
   k_decode_entropy<<<grid_for(c, nblocks, 16), 32, smem, (cudaStream_t)stream>>>(
       c->ent, c->d_floor[0], c->d_floor[1], P, nblocks, d_Wseq, (const long long *)d_coef_off, d_res, d_posts,
       d_present);
   return post_launch(c);
-}
-
-// host-form checks of the packet arrays: every counted packet inside data
-static int packets_check(const int64_t *pkt_off, const int32_t *pkt_bytes, int64_t data_bytes, size_t i) {
-  if (pkt_bytes[i] < 0 || pkt_off[i] < 0 || pkt_off[i] > data_bytes || pkt_bytes[i] > data_bytes - pkt_off[i])
-    return fail(VB200_EINVAL, "packet outside data");
-  return 0;
 }
 
 extern "C" int vb200_decode_entropy(vb200_ctx *c, int nblocks, const int32_t *Wseq, const int64_t *pkt_off,
@@ -3087,15 +3093,10 @@ extern "C" int vb200_decode_entropy(vb200_ctx *c, int nblocks, const int32_t *Ws
   if (nblocks <= 0) return 0;
   if (!Wseq || !pkt_off || !pkt_bytes || !data || !coef_off || !res || !posts || !present || data_bytes < 0)
     return fail(VB200_EINVAL, "decode_entropy pointers");
-  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
-  const int ch = c->setup.channels;
   int rc;
-  for (int i = 0; i < nblocks; i++) {
-    if (Wseq[i] < 0 || Wseq[i] > 1) return fail(VB200_EINVAL, "Wseq values must be 0/1");
-    if ((rc = packets_check(pkt_off, pkt_bytes, data_bytes, i))) return rc;
-    if (coef_off[i] < 0 || coef_off[i] + (int64_t)ch * (c->setup.blocksizes[Wseq[i]] / 2) > res_len)
-      return fail(VB200_EINVAL, "block rows outside res");
-  }
+  if ((rc = ent_check(c))) return rc;
+  if ((rc = blocks_check(c, 1, nblocks, nullptr, Wseq, pkt_off, pkt_bytes, data_bytes, coef_off, res_len))) return rc;
+  const int ch = c->setup.channels;
   std::lock_guard<std::mutex> lk(c->mu);
   const size_t nb = (size_t)nblocks;
   HostIO io{c};
@@ -3103,8 +3104,7 @@ extern "C" int vb200_decode_entropy(vb200_ctx *c, int nblocks, const int32_t *Ws
   if ((rc = io.h2d(Wseq, sizeof(int32_t) * nb, &dW))) return rc;
   if ((rc = io.h2d(pkt_off, sizeof(int64_t) * nb, &dpo))) return rc;
   if ((rc = io.h2d(pkt_bytes, sizeof(int32_t) * nb, &dpb))) return rc;
-  if ((rc = io.h2d(nullptr, (size_t)data_bytes + 1, &dd))) return rc;
-  if (data_bytes) CU(cudaMemcpyAsync(dd, data, (size_t)data_bytes, cudaMemcpyHostToDevice, c->s_main));
+  if ((rc = io.h2d_packets(data, data_bytes, &dd))) return rc;
   if ((rc = io.h2d(coef_off, sizeof(int64_t) * nb, &dco))) return rc;
   if ((rc = io.h2d(res, sizeof(float) * (size_t)res_len, &dr))) return rc;
   if ((rc = io.h2d(nullptr, sizeof(int32_t) * nb * ch * VB200_FLOOR1_STRIDE, &dps))) return rc;
@@ -3118,11 +3118,6 @@ extern "C" int vb200_decode_entropy(vb200_ctx *c, int nblocks, const int32_t *Ws
   return io.sync();
 }
 
-// CTAs per SM of k_decode_packets' grid.  One thread of each CTA decodes a packet serially while the others wait,
-// but the kernel takes 80 registers (-Xptxas -v, sm_90a), so at most 6 CTAs of 128 threads are resident per SM;
-// a grid of more than k_decode_prepare's 8 per SM would only queue
-static const int DECODE_PACKETS_CTAS = 8;
-
 extern "C" int vb200_decode_packets_resume_dev(vb200_ctx *c, int nstreams, int nblk, const int32_t *d_count,
                                                const int32_t *d_Wseq, const int64_t *d_coef_off, float *d_res,
                                                const int64_t *d_pkt_off, const int32_t *d_pkt_bytes,
@@ -3134,29 +3129,13 @@ extern "C" int vb200_decode_packets_resume_dev(vb200_ctx *c, int nstreams, int n
   if (!d_Wseq || !d_coef_off || !d_res || !d_pkt_off || !d_pkt_bytes || !d_data || !d_pcm_off || !d_pcm || !d_carry ||
       !d_carry->tail || !d_carry->W)
     return fail(VB200_EINVAL, "decode pointers");
-  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
-  DecodePrepArgs A;
   int rc;
-  if ((rc = decode_prep_args(c, nstreams, nblk, &A))) return rc;
-  const size_t smem = entropy_smem(c->ent, true);
+  if ((rc = ent_check(c))) return rc;
+  const cudaStream_t st = (cudaStream_t)stream;
   const DecodePackets P{(const long long *)d_pkt_off, d_pkt_bytes, d_data};
-  const int grid = grid_for(c, (int)A.nitems, DECODE_PACKETS_CTAS);
-  if (d_count) {
-    if ((rc = set_smem(k_decode_packets<true>, smem))) return rc;
-    k_decode_packets<true><<<grid, 128, smem, (cudaStream_t)stream>>>(A, c->ent, P, d_Wseq, (const long long *)d_coef_off,
-                                                                      d_res, c->d_fromdB, d_count);
-  } else {
-    if ((rc = set_smem(k_decode_packets<false>, smem))) return rc;
-    k_decode_packets<false><<<grid, 128, smem, (cudaStream_t)stream>>>(A, c->ent, P, d_Wseq, (const long long *)d_coef_off,
-                                                                       d_res, c->d_fromdB, nullptr);
-  }
-  if ((rc = post_launch(c))) return rc;
-  const bool hs = c->halfrate;
-  if (pcm_s16)
-    return hs ? synthesis_carry_launch<true, true>(c, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_pcm_off, d_pcm, pcm_stride, d_carry, stream)
-              : synthesis_carry_launch<true, false>(c, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_pcm_off, d_pcm, pcm_stride, d_carry, stream);
-  return hs ? synthesis_carry_launch<false, true>(c, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_pcm_off, d_pcm, pcm_stride, d_carry, stream)
-            : synthesis_carry_launch<false, false>(c, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_pcm_off, d_pcm, pcm_stride, d_carry, stream);
+  if ((rc = decode_front(c, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, nullptr, nullptr, &P, st))) return rc;
+  return synthesis_launch<SYN_CARRY>(c, pcm_s16, nstreams, nblk, d_count, d_Wseq, d_coef_off, d_res, d_pcm_off, d_pcm,
+                                     pcm_stride, d_carry, DsTrim{}, st);
 }
 
 extern "C" int vb200_decode_packets_resume(vb200_ctx *c, int nstreams, int nblk, const int32_t *count,
@@ -3169,27 +3148,16 @@ extern "C" int vb200_decode_packets_resume(vb200_ctx *c, int nstreams, int nblk,
   if (!Wseq || !coef_off || !pkt_off || !pkt_bytes || !data || !pcm_off || !pcm || !carry || !carry->tail ||
       !carry->W || data_bytes < 0 || res_len < 0)
     return fail(VB200_EINVAL, "decode pointers");
-  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
-  const int ch = c->setup.channels;
-  const size_t nb = (size_t)nstreams * nblk, ntask = (size_t)nstreams * ch;
   int rc;
-  for (int s = 0; s < nstreams; s++) {
-    const int n = count ? count[s] : nblk;
-    if (n < 0 || n > nblk) return fail(VB200_EINVAL, "count[s] must be in [0, nblk]");
-    for (int k = 0; k < n; k++) {
-      const size_t i = (size_t)s * nblk + k;
-      if (Wseq[i] < 0 || Wseq[i] > 1) return fail(VB200_EINVAL, "Wseq values must be 0/1");
-      if ((rc = packets_check(pkt_off, pkt_bytes, data_bytes, i))) return rc;
-      if (coef_off[i] < 0 || coef_off[i] + (int64_t)ch * (c->setup.blocksizes[Wseq[i]] / 2) > res_len)
-        return fail(VB200_EINVAL, "block rows outside res");
-    }
-  }
-  for (size_t i = 0; i < ntask; i++)
-    if (carry->W[i] < -1 || carry->W[i] > 1) return fail(VB200_EINVAL, "carried W must be -1, 0 or 1");
+  if ((rc = ent_check(c))) return rc;
+  const int ch = c->setup.channels;
+  const size_t nb = (size_t)nstreams * nblk;
+  HostCarry k(c, nstreams, carry);
+  if ((rc = blocks_check(c, nstreams, nblk, count, Wseq, pkt_off, pkt_bytes, data_bytes, coef_off, res_len))) return rc;
+  if ((rc = k.check())) return rc;
   std::lock_guard<std::mutex> lk(c->mu);
-  const size_t tbytes = sizeof(float) * ntask * (size_t)(c->setup.blocksizes[1] / 2);
   HostIO io{c};
-  void *dW, *dco, *dc, *dpo, *dp, *dko, *dkb, *dd, *dn = nullptr, *dkt, *dkw;
+  void *dW, *dco, *dc, *dpo, *dp, *dko, *dkb, *dd, *dn = nullptr;
   if ((rc = io.h2d(Wseq, sizeof(int32_t) * nb, &dW))) return rc;
   if ((rc = io.h2d(coef_off, sizeof(int64_t) * nb, &dco))) return rc;
   if ((rc = io.h2d(nullptr, sizeof(float) * (size_t)(res_len ? res_len : 1), &dc))) return rc;
@@ -3198,20 +3166,16 @@ extern "C" int vb200_decode_packets_resume(vb200_ctx *c, int nstreams, int nblk,
   if ((rc = io.h2d(nullptr, pbytes, &dp))) return rc;
   if ((rc = io.h2d(pkt_off, sizeof(int64_t) * nb, &dko))) return rc;
   if ((rc = io.h2d(pkt_bytes, sizeof(int32_t) * nb, &dkb))) return rc;
-  if ((rc = io.h2d(nullptr, (size_t)data_bytes + 1, &dd))) return rc;
-  if (data_bytes) CU(cudaMemcpyAsync(dd, data, (size_t)data_bytes, cudaMemcpyHostToDevice, c->s_main));
+  if ((rc = io.h2d_packets(data, data_bytes, &dd))) return rc;
   if (count && (rc = io.h2d(count, sizeof(int32_t) * nstreams, &dn))) return rc;
-  if ((rc = io.h2d(carry->tail, tbytes, &dkt))) return rc;
-  if ((rc = io.h2d(carry->W, sizeof(int32_t) * ntask, &dkw))) return rc;
+  if ((rc = k.stage(io))) return rc;
   CU(cudaMemsetAsync(dp, 0, pbytes, c->s_main));
-  const vb200_decode_carry dk{(float *)dkt, (int32_t *)dkw};
   if ((rc = vb200_decode_packets_resume_dev(c, nstreams, nblk, (const int32_t *)dn, (const int32_t *)dW,
                                             (const int64_t *)dco, (float *)dc, (const int64_t *)dko,
                                             (const int32_t *)dkb, (const uint8_t *)dd, (const int64_t *)dpo, dp,
-                                            pcm_s16, pcm_stride, &dk, c->s_main))) return rc;
+                                            pcm_s16, pcm_stride, &k.d, c->s_main))) return rc;
   if ((rc = io.d2h(pcm, dp, pbytes))) return rc;
-  if ((rc = io.d2h(carry->tail, dkt, tbytes))) return rc;
-  if ((rc = io.d2h(carry->W, dkw, sizeof(int32_t) * ntask))) return rc;
+  if ((rc = k.write_back(io))) return rc;
   return io.sync();
 }
 
@@ -3242,17 +3206,37 @@ extern "C" int vb200_decode_streams_carry_init(vb200_ctx *c, int nstreams, void 
   return 0;
 }
 
-template <bool S16, bool HS>
-static int synthesis_trim_launch(vb200_ctx *c, int nstreams, int nblk, const int32_t *d_count, const int32_t *d_Wseq,
-                                 const long long *d_coef_off, const float *d_coef, const long long *d_pcm_off,
-                                 void *d_pcm, const DsTrim &T, cudaStream_t st) {
-  const XformDev *X = HS ? c->dx_hs : c->dx;
-  const int ch = c->setup.channels, N1 = X[1].N;
-  const size_t smem = sizeof(float) * ((size_t)N1 / 2 + N1 + N1 / 2);
-  int rc = set_smem(k_synthesis_trim<S16, HS>, smem); if (rc) return rc;
-  k_synthesis_trim<S16, HS><<<grid_for(c, nstreams * ch, 8), threads_for(N1), smem, st>>>(
-      X[0], X[1], HS ? c->dwin_hs : c->dwin, ch, nstreams, nblk, d_Wseq, d_coef_off, d_coef, d_pcm_off, d_pcm,
-      d_count, T);
+// the plan front of vb200_decode_streams_packets_dev and vb200_decode_streams_index_dev: the plan's tables carved
+// from arena, then own(k) carves the caller's scratch (and P.pcm_base where the caller has none); then k_ds_header
+// and k_ds_plan on st.  The heads are d_carry's, ds_carry_bytes apart, or without d_carry fresh ones carved here.
+template <class Own>
+static int ds_plan_front(vb200_ctx *c, DevBuf &arena, DsPlanArgs &P, int nstreams, int max_packets,
+                         const int32_t *d_npkt, const vb200_packet_info *d_info, const uint8_t *d_data,
+                         const void *d_carry, vb200_decoded_packet *d_out, cudaStream_t st, Own &&own) {
+  const long long n = (long long)nstreams * max_packets;
+  DsHead *fresh = nullptr;
+  int rc;
+  if ((rc = carve(arena, [&](Carve &k) {
+         P.Wseq = k.take<int>(n); P.pkt_bytes = k.take<int>(n); P.pkt_off = k.take<long long>(n);
+         P.coef_off = k.take<long long>(n); P.pcm_off = k.take<long long>(n); P.win = k.take<int2>(n);
+         P.count = k.take<int>(nstreams); P.W_in = k.take<int>(nstreams); P.head = k.take<DsHead>(nstreams);
+         own(k);
+         if (!d_carry) fresh = k.take<DsHead>(nstreams);
+       }))) return rc;
+  int *hdr = P.Wseq;                     // k_ds_plan reads slot k's header before it writes block j <= k there
+  P.nstreams = nstreams; P.max_packets = max_packets; P.ch = c->setup.channels; P.hs = c->halfrate ? 1 : 0;
+  P.bs[0] = c->setup.blocksizes[0]; P.bs[1] = c->setup.blocksizes[1];
+  P.npkt = d_npkt; P.info = d_info; P.hdr = hdr; P.out = d_out;
+  // vorbis_synthesis_restart's head has every field k_ds_plan reads at -1 (granulepos, sample_count, sequence, W);
+  // rate is not read there
+  P.carry = d_carry ? (const unsigned char *)d_carry : (const unsigned char *)fresh;
+  P.carry_bytes = d_carry ? (long long)ds_carry_bytes(c) : (long long)sizeof(DsHead);
+  if ((rc = scratch_begin(c, st))) return rc;
+  if (!d_carry) CU(cudaMemsetAsync(fresh, 0xff, sizeof(DsHead) * (size_t)nstreams, st));
+  k_ds_header<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(nstreams, max_packets, c->ent.modebits, d_npkt, d_info,
+                                                             d_data, hdr);
+  if ((rc = post_launch(c))) return rc;
+  k_ds_plan<<<(nstreams + 127) / 128, 128, 0, st>>>(P);
   return post_launch(c);
 }
 
@@ -3265,52 +3249,42 @@ extern "C" int vb200_decode_streams_packets_dev(vb200_ctx *c, int nstreams, int 
   if (max_packets < 1) return fail(VB200_EINVAL, "max_packets must be >= 1");
   if (!d_npkt || !d_info || !d_data || !d_carry || !d_pcm || !d_pcm_base || !d_out)
     return fail(VB200_EINVAL, "decode streams pointers");
-  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
+  int rc;
+  if ((rc = ent_check(c))) return rc;
   const long long n = (long long)nstreams * max_packets;
   if (n > INT32_MAX) return fail(VB200_EINVAL, "nstreams * max_packets must fit an int");
   const int ch = c->setup.channels;
-  const bool hs = c->halfrate;
   const cudaStream_t st = (cudaStream_t)stream;
   DsPlanArgs P;
   float *res;
-  int rc;
-  if ((rc = carve(c->dsk, [&](Carve &k) {
-         P.Wseq = k.take<int>(n); P.pkt_bytes = k.take<int>(n); P.pkt_off = k.take<long long>(n);
-         P.coef_off = k.take<long long>(n); P.pcm_off = k.take<long long>(n); P.win = k.take<int2>(n);
-         P.count = k.take<int>(nstreams); P.W_in = k.take<int>(nstreams); P.head = k.take<DsHead>(nstreams);
-         res = k.take<float>(n * ch * (c->setup.blocksizes[1] / 2));
-       }))) return rc;
-  int *hdr = P.Wseq;                     // k_ds_plan reads slot k's header before it writes block j <= k there
-  P.nstreams = nstreams; P.max_packets = max_packets; P.ch = ch; P.hs = hs ? 1 : 0;
-  P.bs[0] = c->setup.blocksizes[0]; P.bs[1] = c->setup.blocksizes[1];
-  P.npkt = d_npkt; P.info = d_info; P.hdr = hdr; P.carry = (const unsigned char *)d_carry;
-  P.carry_bytes = (long long)ds_carry_bytes(c); P.pcm_base = (long long *)d_pcm_base; P.out = d_out;
-  if ((rc = scratch_begin(c, st))) return rc;
-  k_ds_header<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(nstreams, max_packets, c->ent.modebits, d_npkt, d_info,
-                                                             d_data, hdr);
+  P.pcm_base = (long long *)d_pcm_base;
+  if ((rc = ds_plan_front(c, c->dsk, P, nstreams, max_packets, d_npkt, d_info, d_data, d_carry, d_out, st,
+                          [&](Carve &k) { res = k.take<float>(n * ch * (c->setup.blocksizes[1] / 2)); })))
+    return rc;
+  k_ds_scan<<<1, 1024, 0, st>>>(nstreams, P.pcm_base);
   if ((rc = post_launch(c))) return rc;
-  k_ds_plan<<<(nstreams + 127) / 128, 128, 0, st>>>(P);
-  if ((rc = post_launch(c))) return rc;
-  k_ds_scan<<<1, 1024, 0, st>>>(nstreams, (long long *)d_pcm_base);
-  if ((rc = post_launch(c))) return rc;
-  DecodePrepArgs A;
-  if ((rc = decode_prep_args(c, nstreams, max_packets, &A))) return rc;
   const DecodePackets DP{P.pkt_off, P.pkt_bytes, d_data};
-  if ((rc = set_smem(k_decode_packets<true>, entropy_smem(c->ent, true)))) return rc;
-  k_decode_packets<true><<<grid_for(c, (int)n, DECODE_PACKETS_CTAS), 128, entropy_smem(c->ent, true), st>>>(
-      A, c->ent, DP, P.Wseq, P.coef_off, res, c->d_fromdB, P.count);
-  if ((rc = post_launch(c))) return rc;
+  if ((rc = decode_front(c, nstreams, max_packets, P.count, P.Wseq, (const int64_t *)P.coef_off, res, nullptr, nullptr,
+                         &DP, st))) return rc;
   DsTrim T;
   T.win = P.win; T.base = P.pcm_base; T.W_in = P.W_in; T.head = P.head; T.carry = (unsigned char *)d_carry;
   T.carry_bytes = P.carry_bytes; T.cap = pcm_cap; T.tail_stride = c->setup.blocksizes[1] / 2;
-  if (pcm_s16)
-    rc = hs ? synthesis_trim_launch<true, true>(c, nstreams, max_packets, P.count, P.Wseq, P.coef_off, res, P.pcm_off, d_pcm, T, st)
-            : synthesis_trim_launch<true, false>(c, nstreams, max_packets, P.count, P.Wseq, P.coef_off, res, P.pcm_off, d_pcm, T, st);
-  else
-    rc = hs ? synthesis_trim_launch<false, true>(c, nstreams, max_packets, P.count, P.Wseq, P.coef_off, res, P.pcm_off, d_pcm, T, st)
-            : synthesis_trim_launch<false, false>(c, nstreams, max_packets, P.count, P.Wseq, P.coef_off, res, P.pcm_off, d_pcm, T, st);
-  if (rc) return rc;
+  if ((rc = synthesis_launch<SYN_TRIM>(c, pcm_s16, nstreams, max_packets, P.count, P.Wseq, (const int64_t *)P.coef_off,
+                                       res, (const int64_t *)P.pcm_off, d_pcm, 0, nullptr, T, st))) return rc;
   return scratch_end(c, st);
+}
+
+// host-form checks of the packet-stream forms: npkt[s] in [0, max_packets], every counted packet inside data
+static int ds_check_packets(int nstreams, int max_packets, const int32_t *npkt, const vb200_packet_info *info,
+                            int64_t data_bytes) {
+  for (int s = 0; s < nstreams; s++) {
+    if (npkt[s] < 0 || npkt[s] > max_packets) return fail(VB200_EINVAL, "npkt[s] must be in [0, max_packets]");
+    for (int k = 0; k < npkt[s]; k++) {
+      const vb200_packet_info &p = info[(size_t)s * max_packets + k];
+      if (p.offset < 0 || p.bytes < 0 || p.offset > data_bytes - p.bytes) return fail(VB200_EINVAL, "packet outside data");
+    }
+  }
+  return 0;
 }
 
 extern "C" int vb200_decode_streams_packets(vb200_ctx *c, int nstreams, int max_packets, const int32_t *npkt,
@@ -3322,15 +3296,10 @@ extern "C" int vb200_decode_streams_packets(vb200_ctx *c, int nstreams, int max_
   if (max_packets < 1) return fail(VB200_EINVAL, "max_packets must be >= 1");
   if (!npkt || !info || !data || !d_carry || !pcm || !pcm_base || !out || data_bytes < 0 || pcm_cap < 0)
     return fail(VB200_EINVAL, "decode streams pointers");
-  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
+  int rc;
+  if ((rc = ent_check(c))) return rc;
+  if ((rc = ds_check_packets(nstreams, max_packets, npkt, info, data_bytes))) return rc;
   const size_t n = (size_t)nstreams * max_packets;
-  for (int s = 0; s < nstreams; s++) {
-    if (npkt[s] < 0 || npkt[s] > max_packets) return fail(VB200_EINVAL, "npkt[s] must be in [0, max_packets]");
-    for (int k = 0; k < npkt[s]; k++) {
-      const vb200_packet_info &p = info[(size_t)s * max_packets + k];
-      if (p.offset < 0 || p.bytes < 0 || p.offset > data_bytes - p.bytes) return fail(VB200_EINVAL, "packet outside data");
-    }
-  }
   std::lock_guard<std::mutex> lk(c->mu);
   const size_t B = ds_carry_bytes(c);
   std::vector<DsHead> heads((size_t)nstreams);
@@ -3345,11 +3314,9 @@ extern "C" int vb200_decode_streams_packets(vb200_ctx *c, int nstreams, int max_
   const size_t el = pcm_s16 ? sizeof(int16_t) : sizeof(float);
   HostIO io{c};
   void *dn, *di, *dd, *dp, *db, *dout;
-  int rc;
   if ((rc = io.h2d(npkt, sizeof(int32_t) * nstreams, &dn))) return rc;
   if ((rc = io.h2d(info, sizeof(vb200_packet_info) * n, &di))) return rc;
-  if ((rc = io.h2d(nullptr, (size_t)data_bytes + 1, &dd))) return rc;
-  if (data_bytes) CU(cudaMemcpyAsync(dd, data, (size_t)data_bytes, cudaMemcpyHostToDevice, c->s_main));
+  if ((rc = io.h2d_packets(data, data_bytes, &dd))) return rc;
   if ((rc = io.h2d(nullptr, el * (size_t)std::max<int64_t>(pcm_cap, 1), &dp))) return rc;
   if ((rc = io.h2d(nullptr, sizeof(int64_t) * (nstreams + 1), &db))) return rc;
   if ((rc = io.h2d(nullptr, sizeof(vb200_decoded_packet) * n, &dout))) return rc;
@@ -3367,19 +3334,7 @@ extern "C" int vb200_decode_streams_packets(vb200_ctx *c, int nstreams, int max_
 }
 
 // ---- sample ranges from packets (vb200_decode_ranges.cuh).  The index is k_ds_header and k_ds_plan on fresh
-// heads; the ranges are k_dr_plan, k_decode_packets<true> and k_synthesis_range.
-static int ds_check_packets(int nstreams, int max_packets, const int32_t *npkt, const vb200_packet_info *info,
-                            int64_t data_bytes) {
-  for (int s = 0; s < nstreams; s++) {
-    if (npkt[s] < 0 || npkt[s] > max_packets) return fail(VB200_EINVAL, "npkt[s] must be in [0, max_packets]");
-    for (int k = 0; k < npkt[s]; k++) {
-      const vb200_packet_info &p = info[(size_t)s * max_packets + k];
-      if (p.offset < 0 || p.bytes < 0 || p.offset > data_bytes - p.bytes) return fail(VB200_EINVAL, "packet outside data");
-    }
-  }
-  return 0;
-}
-
+// heads; the ranges are k_dr_plan, k_decode_packets<true> and k_synthesis<*, *, SYN_RANGE>.
 extern "C" int vb200_decode_streams_index_dev(vb200_ctx *c, int nstreams, int max_packets, const int32_t *d_npkt,
                                               const vb200_packet_info *d_info, const uint8_t *d_data,
                                               int64_t *d_length, vb200_decoded_packet *d_out, void *stream) {
@@ -3387,32 +3342,14 @@ extern "C" int vb200_decode_streams_index_dev(vb200_ctx *c, int nstreams, int ma
   if (nstreams <= 0) return 0;
   if (max_packets < 1) return fail(VB200_EINVAL, "max_packets must be >= 1");
   if (!d_npkt || !d_info || !d_data || !d_length || !d_out) return fail(VB200_EINVAL, "decode streams index pointers");
-  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
-  const long long n = (long long)nstreams * max_packets;
-  if (n > INT32_MAX) return fail(VB200_EINVAL, "nstreams * max_packets must fit an int");
+  int rc;
+  if ((rc = ent_check(c))) return rc;
+  if ((long long)nstreams * max_packets > INT32_MAX) return fail(VB200_EINVAL, "nstreams * max_packets must fit an int");
   const cudaStream_t st = (cudaStream_t)stream;
   DsPlanArgs P;
-  DsHead *fresh;
-  int rc;
-  if ((rc = carve(c->drg, [&](Carve &k) {
-         P.Wseq = k.take<int>(n); P.pkt_bytes = k.take<int>(n); P.pkt_off = k.take<long long>(n);
-         P.coef_off = k.take<long long>(n); P.pcm_off = k.take<long long>(n); P.win = k.take<int2>(n);
-         P.count = k.take<int>(nstreams); P.W_in = k.take<int>(nstreams); P.head = k.take<DsHead>(nstreams);
-         P.pcm_base = k.take<long long>(nstreams + 1); fresh = k.take<DsHead>(nstreams);
-       }))) return rc;
-  P.nstreams = nstreams; P.max_packets = max_packets; P.ch = c->setup.channels; P.hs = c->halfrate ? 1 : 0;
-  P.bs[0] = c->setup.blocksizes[0]; P.bs[1] = c->setup.blocksizes[1];
-  P.npkt = d_npkt; P.info = d_info; P.hdr = P.Wseq; P.out = d_out;
-  // vorbis_synthesis_restart's head has every field k_ds_plan reads at -1 (granulepos, sample_count, sequence, W);
-  // rate is not read there
-  P.carry = (const unsigned char *)fresh; P.carry_bytes = sizeof(DsHead);
-  if ((rc = scratch_begin(c, st))) return rc;
-  CU(cudaMemsetAsync(fresh, 0xff, sizeof(DsHead) * (size_t)nstreams, st));
-  k_ds_header<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(nstreams, max_packets, c->ent.modebits, d_npkt, d_info,
-                                                             d_data, P.Wseq);
-  if ((rc = post_launch(c))) return rc;
-  k_ds_plan<<<(nstreams + 127) / 128, 128, 0, st>>>(P);
-  if ((rc = post_launch(c))) return rc;
+  if ((rc = ds_plan_front(c, c->drg, P, nstreams, max_packets, d_npkt, d_info, d_data, nullptr, d_out, st,
+                          [&](Carve &k) { P.pcm_base = k.take<long long>(nstreams + 1); })))
+    return rc;
   CU(cudaMemcpyAsync(d_length, P.pcm_base + 1, sizeof(int64_t) * (size_t)nstreams, cudaMemcpyDeviceToDevice, st));
   return scratch_end(c, st);
 }
@@ -3424,8 +3361,8 @@ extern "C" int vb200_decode_streams_index(vb200_ctx *c, int nstreams, int max_pa
   if (nstreams <= 0) return 0;
   if (max_packets < 1) return fail(VB200_EINVAL, "max_packets must be >= 1");
   if (!npkt || !info || !data || !length || !out || data_bytes < 0) return fail(VB200_EINVAL, "decode streams index pointers");
-  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
   int rc;
+  if ((rc = ent_check(c))) return rc;
   if ((rc = ds_check_packets(nstreams, max_packets, npkt, info, data_bytes))) return rc;
   std::lock_guard<std::mutex> lk(c->mu);
   const size_t n = (size_t)nstreams * max_packets;
@@ -3433,8 +3370,7 @@ extern "C" int vb200_decode_streams_index(vb200_ctx *c, int nstreams, int max_pa
   void *dn, *di, *dd, *dl, *dout;
   if ((rc = io.h2d(npkt, sizeof(int32_t) * nstreams, &dn))) return rc;
   if ((rc = io.h2d(info, sizeof(vb200_packet_info) * n, &di))) return rc;
-  if ((rc = io.h2d(nullptr, (size_t)data_bytes + 1, &dd))) return rc;
-  if (data_bytes) CU(cudaMemcpyAsync(dd, data, (size_t)data_bytes, cudaMemcpyHostToDevice, c->s_main));
+  if ((rc = io.h2d_packets(data, data_bytes, &dd))) return rc;
   if ((rc = io.h2d(nullptr, sizeof(int64_t) * nstreams, &dl))) return rc;
   if ((rc = io.h2d(nullptr, sizeof(vb200_decoded_packet) * n, &dout))) return rc;
   if ((rc = vb200_decode_streams_index_dev(c, nstreams, max_packets, (const int32_t *)dn, (const vb200_packet_info *)di,
@@ -3456,19 +3392,6 @@ static long long dr_residue(const vb200_ctx *c, int32_t out_stride) {
   return (f + 63) & ~63ll;
 }
 
-template <bool S16, bool HS>
-static int synthesis_range_launch(vb200_ctx *c, int nreq, int nblk, const int32_t *d_count, const int32_t *d_Wseq,
-                                  const long long *d_coef_off, const float *d_coef, const long long *d_pcm_off,
-                                  void *d_pcm, const DsTrim &T, cudaStream_t st) {
-  const XformDev *X = HS ? c->dx_hs : c->dx;
-  const int ch = c->setup.channels, N1 = X[1].N;
-  const size_t smem = sizeof(float) * ((size_t)N1 / 2 + N1 + N1 / 2);
-  int rc = set_smem(k_synthesis_range<S16, HS>, smem); if (rc) return rc;
-  k_synthesis_range<S16, HS><<<grid_for(c, nreq * ch, 8), threads_for(N1), smem, st>>>(
-      X[0], X[1], HS ? c->dwin_hs : c->dwin, ch, nreq, nblk, d_Wseq, d_coef_off, d_coef, d_pcm_off, d_pcm, d_count, T);
-  return post_launch(c);
-}
-
 extern "C" int vb200_decode_ranges_dev(vb200_ctx *c, int nstreams, int max_packets, const int32_t *d_npkt,
                                        const vb200_packet_info *d_info, const uint8_t *d_data,
                                        int nreq, const vb200_pcm_range *d_req, int pcm_s16, void *d_pcm,
@@ -3480,7 +3403,8 @@ extern "C" int vb200_decode_ranges_dev(vb200_ctx *c, int nstreams, int max_packe
   if (out_stride < 0) return fail(VB200_EINVAL, "out_stride must be >= 0");
   if (nstreams < 0 || (nstreams > 0 && (!d_npkt || !d_info || !d_data)) || !d_req || !d_pcm || !d_got)
     return fail(VB200_EINVAL, "decode ranges pointers");
-  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
+  int rc;
+  if ((rc = ent_check(c))) return rc;
   const long long nblk = dr_blocks(c, out_stride), rescap = dr_residue(c, out_stride);
   if ((long long)nreq * nblk > INT32_MAX) return fail(VB200_EINVAL, "nreq * block slots must fit an int");
   const int ch = c->setup.channels;
@@ -3489,7 +3413,6 @@ extern "C" int vb200_decode_ranges_dev(vb200_ctx *c, int nstreams, int max_packe
   const size_t nb = (size_t)nreq * nblk;
   DrPlanArgs P;
   float *res;
-  int rc;
   if ((rc = carve(c->drg, [&](Carve &k) {
          P.Wseq = k.take<int>(nb); P.pkt_bytes = k.take<int>(nb); P.pkt_off = k.take<long long>(nb);
          P.coef_off = k.take<long long>(nb); P.pcm_off = k.take<long long>(nb); P.win = k.take<int2>(nb);
@@ -3506,22 +3429,13 @@ extern "C" int vb200_decode_ranges_dev(vb200_ctx *c, int nstreams, int max_packe
   CU(cudaMemsetAsync(d_pcm, 0, el * (size_t)nreq * ch * (size_t)out_stride, st));
   k_dr_plan<<<(unsigned)(((long long)nreq * 32 + 127) / 128), 128, 0, st>>>(P);
   if ((rc = post_launch(c))) return rc;
-  DecodePrepArgs A;
-  if ((rc = decode_prep_args(c, nreq, (int)nblk, &A))) return rc;
   const DecodePackets DP{P.pkt_off, P.pkt_bytes, d_data};
-  if ((rc = set_smem(k_decode_packets<true>, entropy_smem(c->ent, true)))) return rc;
-  k_decode_packets<true><<<grid_for(c, (int)nb, DECODE_PACKETS_CTAS), 128, entropy_smem(c->ent, true), st>>>(
-      A, c->ent, DP, P.Wseq, P.coef_off, res, c->d_fromdB, P.count);
-  if ((rc = post_launch(c))) return rc;
+  if ((rc = decode_front(c, nreq, (int)nblk, P.count, P.Wseq, (const int64_t *)P.coef_off, res, nullptr, nullptr, &DP,
+                         st))) return rc;
   DsTrim T{};
   T.win = P.win; T.base = P.base;
-  if (pcm_s16)
-    rc = hs ? synthesis_range_launch<true, true>(c, nreq, (int)nblk, P.count, P.Wseq, P.coef_off, res, P.pcm_off, d_pcm, T, st)
-            : synthesis_range_launch<true, false>(c, nreq, (int)nblk, P.count, P.Wseq, P.coef_off, res, P.pcm_off, d_pcm, T, st);
-  else
-    rc = hs ? synthesis_range_launch<false, true>(c, nreq, (int)nblk, P.count, P.Wseq, P.coef_off, res, P.pcm_off, d_pcm, T, st)
-            : synthesis_range_launch<false, false>(c, nreq, (int)nblk, P.count, P.Wseq, P.coef_off, res, P.pcm_off, d_pcm, T, st);
-  if (rc) return rc;
+  if ((rc = synthesis_launch<SYN_RANGE>(c, pcm_s16, nreq, (int)nblk, P.count, P.Wseq, (const int64_t *)P.coef_off, res,
+                                        (const int64_t *)P.pcm_off, d_pcm, 0, nullptr, T, st))) return rc;
   return scratch_end(c, st);
 }
 
@@ -3534,8 +3448,8 @@ extern "C" int vb200_decode_ranges(vb200_ctx *c, int nstreams, int max_packets, 
   if (max_packets < 1) return fail(VB200_EINVAL, "max_packets must be >= 1");
   if (nstreams < 0 || !npkt || !info || !data || !req || !pcm || !got || data_bytes < 0 || out_stride < 0)
     return fail(VB200_EINVAL, "decode ranges pointers");
-  if (!c->ent.books) return fail(VB200_EINVAL, "no vb200_decode_entropy_setup registered");
   int rc;
+  if ((rc = ent_check(c))) return rc;
   if ((rc = ds_check_packets(nstreams, max_packets, npkt, info, data_bytes))) return rc;
   for (int r = 0; r < nreq; r++)
     if (req[r].stream < 0 || req[r].stream >= nstreams || req[r].start < 0 || req[r].length < 0 ||
@@ -3549,8 +3463,7 @@ extern "C" int vb200_decode_ranges(vb200_ctx *c, int nstreams, int max_packets, 
   void *dn, *di, *dd, *dq, *dp, *dg;
   if ((rc = io.h2d(npkt, sizeof(int32_t) * nstreams, &dn))) return rc;
   if ((rc = io.h2d(info, sizeof(vb200_packet_info) * n, &di))) return rc;
-  if ((rc = io.h2d(nullptr, (size_t)data_bytes + 1, &dd))) return rc;
-  if (data_bytes) CU(cudaMemcpyAsync(dd, data, (size_t)data_bytes, cudaMemcpyHostToDevice, c->s_main));
+  if ((rc = io.h2d_packets(data, data_bytes, &dd))) return rc;
   if ((rc = io.h2d(req, sizeof(vb200_pcm_range) * nreq, &dq))) return rc;
   if ((rc = io.h2d(nullptr, std::max<size_t>(pbytes, 1), &dp))) return rc;
   if ((rc = io.h2d(nullptr, sizeof(int32_t) * nreq, &dg))) return rc;

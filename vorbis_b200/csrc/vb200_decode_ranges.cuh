@@ -6,7 +6,7 @@
 //                32 packets at a time (ds_packet_header, one per lane), then blockin's bookkeeping over them in order
 //                (ds_blockin, the step of k_ds_plan), the compacted block tables k_decode_packets<true> reads and each
 //                block's window, intersected with the range, with its offset in the request's output row
-// then k_decode_packets<true> with requests as its streams and k_synthesis_range (vb200.cu).
+// then k_decode_packets<true> with requests as its streams and k_synthesis<*, *, SYN_RANGE> (vb200.cu).
 //
 // A block's finished samples depend on its own packet and on the previous decoded block's (the right half of its
 // IMDCT and its flag); nothing else of the stream's past reaches them.  So block j0, the first whose returned
@@ -50,7 +50,7 @@ struct DrPlanArgs {
   long long *pkt_off, *coef_off, *pcm_off;
   int2 *win;
   // ... and per request
-  long long *base;           // [nreq + 1] r * out_stride: the output rows, as pcm_base of k_synthesis_trim
+  long long *base;           // [nreq + 1] r * out_stride: the output rows, as pcm_base of SYN_TRIM
   int *got;
 };
 

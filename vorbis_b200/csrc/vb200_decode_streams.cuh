@@ -8,7 +8,7 @@
 //                835-941), which never reads a sample value: each block's returned window [lo, hi) of the samples
 //                it finishes, its samples and granulepos
 //   k_ds_scan    pcm_base, the prefix sums of the streams' returned samples
-// then k_decode_packets<true> and k_synthesis_trim (vb200.cu), which writes only [lo, hi) of each block.
+// then k_decode_packets<true> and k_synthesis<*, *, SYN_TRIM> (vb200.cu), which writes only [lo, hi) of each block.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -29,7 +29,7 @@ constexpr int DS_HEAD_BYTES = 64;
 constexpr int DS_RATE_FULL = 1, DS_RATE_HALF = 2;
 static_assert(sizeof(DsHead) <= DS_HEAD_BYTES, "carry head");
 
-// what k_synthesis_trim needs besides the arguments of k_synthesis_carry
+// what k_synthesis needs in SYN_TRIM and SYN_RANGE besides the arguments of SYN_CARRY
 struct DsTrim {
   const int2 *win;           // [nstreams][nblk] the returned window [lo, hi) of each block's finished samples
   const long long *base;     // [nstreams + 1] pcm_base

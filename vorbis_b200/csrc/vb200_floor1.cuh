@@ -602,6 +602,18 @@ struct DecodePrepArgs {
   long nitems;                         // nstreams * nblk
 };
 
+// undo channel coupling, lib/mapping0.c:754-779 (square polar -> L/R), in place: one step's pair of bins
+__device__ __forceinline__ void dev_decouple(float *pM, float *pA) {
+  const float m = *pM, a = *pA;
+  if (m > 0.f) {
+    if (a > 0.f) { *pM = m; *pA = m - a; }
+    else         { *pA = m; *pM = m + a; }
+  } else {
+    if (a > 0.f) { *pM = m; *pA = m + a; }
+    else         { *pA = m; *pM = m - a; }
+  }
+}
+
 // the packets of the ENTROPY instances: item it is data[off[it] .. off[it] + bytes[it])
 struct DecodePackets {
   const long long *off;
@@ -649,19 +661,9 @@ decode_prepare_body(const DecodePrepArgs &A, const int *__restrict__ Wseq, const
       }
       __syncthreads();
     }
-    for (int j = threadIdx.x; j < n; j += blockDim.x) {
-      for (int s = A.steps[W] - 1; s >= 0; s--) {
-        float *pM = base + (size_t)A.mag[W][s] * n + j, *pA = base + (size_t)A.ang[W][s] * n + j;
-        const float m = *pM, a = *pA;
-        if (m > 0.f) {
-          if (a > 0.f) { *pM = m; *pA = m - a; }
-          else         { *pA = m; *pM = m + a; }
-        } else {
-          if (a > 0.f) { *pM = m; *pA = m + a; }
-          else         { *pA = m; *pM = m - a; }
-        }
-      }
-    }
+    for (int j = threadIdx.x; j < n; j += blockDim.x)
+      for (int s = A.steps[W] - 1; s >= 0; s--)
+        dev_decouple(base + (size_t)A.mag[W][s] * n + j, base + (size_t)A.ang[W][s] * n + j);
     __syncthreads();
     for (int c = warp; c < A.ch; c += 4) {
       if constexpr (ENTROPY) {
@@ -680,19 +682,12 @@ decode_prepare_body(const DecodePrepArgs &A, const int *__restrict__ Wseq, const
   }
 }
 
+template <bool COUNTED>
 __global__ void __launch_bounds__(128)
 k_decode_prepare(DecodePrepArgs A, const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
                  float *__restrict__ res, const int32_t *__restrict__ posts, const int32_t *__restrict__ present,
-                 const float *__restrict__ fromdB) {
-  decode_prepare_body<false>(A, Wseq, coef_off, res, posts, present, fromdB, nullptr);
-}
-
-__global__ void __launch_bounds__(128)
-k_decode_prepare_counted(DecodePrepArgs A, const int *__restrict__ Wseq, const long long *__restrict__ coef_off,
-                         float *__restrict__ res, const int32_t *__restrict__ posts,
-                         const int32_t *__restrict__ present, const float *__restrict__ fromdB,
-                         const int *__restrict__ count) {
-  decode_prepare_body<true>(A, Wseq, coef_off, res, posts, present, fromdB, count);
+                 const float *__restrict__ fromdB, const int *__restrict__ count) {
+  decode_prepare_body<COUNTED>(A, Wseq, coef_off, res, posts, present, fromdB, count);
 }
 
 // vb200_decode_packets_resume: the entropy decode of each block's packet in front of the same body
