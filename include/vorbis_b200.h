@@ -639,7 +639,8 @@ typedef struct vb200_entropy_setup {
 
 /* Copies everything and builds the device lookup tables.  Returns VB200_EINVAL for inconsistent input (a code
  * that is not a complete prefix code, except the single-entry length-1 book; a book index out of range; a
- * residue range or grouping that does not fit the block; partition counts that do not match the floor's posts)
+ * residue that begins past the block or has grouping < 1 (an end past the block is clamped to it, as the
+ * reference's residue inverse clamps it); partition counts that do not match the floor's posts)
  * and VB200_EIMPL for residue type 0 or a floor that is not type 1.  Replaces an earlier registration.  After it,
  * no value read from a packet can index outside a table or a row.                                             */
 int vb200_decode_entropy_setup(vb200_ctx*, const vb200_entropy_setup*);

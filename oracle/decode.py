@@ -77,6 +77,16 @@ def _lib(dropin):
     return _libs[dropin]
 
 
+def ref_window(n):
+    """the reference's tabulated rising half window of an n-sample block (lib/window.c, n = 64..8192): n/2 floats"""
+    L = _lib(False)
+    L._vorbis_window_get.restype = C.POINTER(C.c_float)
+    L._vorbis_window_get.argtypes = [C.c_int]
+    k = n.bit_length() - 7
+    assert n == 64 << k and 0 <= k < 8, n
+    return np.ctypeslib.as_array(L._vorbis_window_get(k), (n // 2,)).copy()
+
+
 class Packets:
     """the packets of one encoded stream: buf uint8, meta int64 [n][META] (3 headers first)"""
 

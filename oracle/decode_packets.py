@@ -158,6 +158,28 @@ class Driver:
             self.m = None
 
 
+class _OggPacket(C.Structure):
+    _fields_ = [("packet", C.c_void_p), ("bytes", C.c_long), ("b_o_s", C.c_long), ("e_o_s", C.c_long),
+                ("granulepos", C.c_int64), ("packetno", C.c_int64)]
+
+
+def open_error(p, device=0):
+    """what vb200md_open_err reports for p's headers: 0 (the driver opened, and is closed again) or the OV_* code"""
+    L = _lib(True)
+    L.vb200md_open_err.restype = C.c_void_p
+    L.vb200md_open_err.argtypes = [C.c_int, C.POINTER(_OggPacket), C.c_int, C.c_int, C.POINTER(C.c_int)]
+    L.vb200md_close.argtypes = [C.c_void_p]
+    hdr = (_OggPacket * 3)()
+    for k in range(3):
+        o, n = int(p.meta[k, 0]), int(p.meta[k, 1])
+        hdr[k] = _OggPacket(p.buf.ctypes.data + o, n, 1 if k == 0 else 0, 0, 0, k)
+    err = C.c_int(0)
+    m = L.vb200md_open_err(1, hdr, 0, device, C.byref(err))
+    if m:
+        L.vb200md_close(m)
+    return err.value
+
+
 def dev_staging(ctx, pkts, W, bs, ch):
     """vb200_decode_entropy on the packets with W >= 0, in the layout of ref_staging"""
     data, off, lens = _packed(pkts)

@@ -1,7 +1,8 @@
 """The oracle's transforms at every block size the library accepts (64 ... 8192) against float64 direct formulas.
 
-vorbisenc only produces 256/2048 and 512/4096 block pairs (and single-size setups), so the reference cannot be driven at
-64, 128 or 8192 and the oracle's restatement is pinned to it only at 256 ... 4096.  Here the oracle's mdct_forward,
+vorbisenc only produces 256/2048 and 512/4096 block pairs (and single-size setups).  Streams with hand-written setup
+headers drive the reference at every size: tests/test_generated_setups_oracle.py pins the oracle's decode (inverse MDCT,
+windows, overlap-add) to the stock decoder bit for bit from 64 to 8192.  Here the oracle's mdct_forward,
 mdct_backward and drft_forward (float32, the reference's own arithmetic) are compared with the textbook transforms
 evaluated in float64.  The error bound is calibrated at N = 2048, where the oracle is pinned to the reference bit for
 bit: the float32 rounding error measured there, times a small factor, grows with log2 N.  An indexing or twiddle mistake
