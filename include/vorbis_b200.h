@@ -789,6 +789,69 @@ int vb200_decode_ranges    (vb200_ctx*, int nstreams, int max_packets, const int
                             int nreq, const vb200_pcm_range *req, int pcm_s16, void *pcm, int32_t out_stride,
                             int32_t *got);
 
+/* ---- Ogg Vorbis files in: the page demux of libogg (ogg_sync_pageseek, ogg_stream_pagein, ogg_stream_packetout) and
+ * vorbisfile's choice of the logical stream, on the device, for many files in one call.  No context: the setup is not
+ * known before the headers are read.  The output is what vb200_decode_streams_packets / vb200_decode_ranges read.
+ *
+ * Input: file f is bytes[file_off[f] .. file_off[f+1]), one Ogg file; file_off [nfiles+1] int64, non-decreasing.
+ * Rules, per file:
+ *   Capture.  A page is "OggS", 27 header bytes, the lacing table (header byte 26 segments) and a body of the lacing
+ *     sum.  Its CRC-32 (polynomial 0x04c11db7, not reflected, initial 0, no final xor, over the whole page with bytes
+ *     22..25 taken as zero) must equal bytes 22..25 read little-endian.  A bad capture pattern or CRC counts one
+ *     `dropped` and the scan resumes at the next 'O' after the failed position.  Fewer than 27 bytes left, or a page cut
+ *     short by the end of the file, end the scan.
+ *   Stream.  The first captured page with the BOS flag, version 0 and a first packet that begins "\x01vorbis" fixes
+ *     `serial`.  Before it, and after it for pages of other serials or a version other than 0, pages are skipped and
+ *     counted in `foreign`.  The walk ends after that serial's EOS page; `chained` = 1 when the next captured page has
+ *     the BOS flag.  Links after the first are not read.
+ *   Packets.  Lacing value 255 continues a packet.  A page sequence number other than the previous page's plus one
+ *     drops the pending partial packet and leaves one hole: packetno advances by one with no packet.  A continued page
+ *     with nothing pending skips its leading fragment.  A page without the continued flag while a partial packet is
+ *     pending appends to that packet (libogg does the same).  A page's granulepos goes to the last packet that ends on
+ *     it, every other packet gets -1; e_o_s marks the packet that ends on the EOS page's last segment.  packetno counts
+ *     from 0 with the headers as 0, 1, 2; a packet still incomplete when the walk ends is lost.
+ * Output:
+ *   data  packet bytes.  File f writes only inside [file_off[f], file_off[f+1]) of data (the packets of a file never
+ *         hold more bytes than the file), its packets back to back from file_off[f]; data must not overlap bytes.
+ *   info  [nfiles][max_packets] vb200_packet_info: audio packet k of file f (packetno 3 onwards) at absolute offsets
+ *         into data, choice 0; npkt [nfiles] how many (rows past it are not written).  A group of files is the
+ *         slice info + first*max_packets.
+ *   streams [nfiles]: status 0, VB200_ENOTVORBIS (no Vorbis BOS page), VB200_EBADHEADER (a hole or the end of the walk
+ *         before the third packet; no audio packet is kept) or VB200_EINVAL (max_packets cut the table, which then holds
+ *         the first max_packets audio packets); the header packets' offsets into data and sizes; the counters.
+ * One kernel launch whatever nfiles is: one warp per file walks its pages in order; the lanes split the lacing sum and
+ * the CRC (chunk CRCs shifted by x^(8*bytes after) mod P and xor-ed) and copy each page's kept body.  No device scratch.
+ * _dev: device pointers, asynchronous on `stream`; checks its pointers, nfiles >= 0 and max_packets >= 1 only.
+ * Host form: host buffers, on the current CUDA device; also checks file_off (non-decreasing from >= 0); data holds
+ * file_off[nfiles] bytes.                                                                                         */
+#define VB200_ENOTVORBIS (-132)   /* OV_ENOTVORBIS */
+#define VB200_EBADHEADER (-133)   /* OV_EBADHEADER */
+typedef struct vb200_ogg_stream {
+  int32_t  status;
+  uint32_t serial;      /* the Vorbis stream's serial number (0 when none was found) */
+  int32_t  pages;       /* pages of that serial taken, the EOS page included */
+  int32_t  dropped;     /* failed captures: bad capture pattern or CRC */
+  int32_t  holes;       /* page sequence gaps */
+  int32_t  foreign;     /* captured pages skipped: other serials, version != 0, before the Vorbis BOS page */
+  int32_t  chained;     /* a BOS page follows the EOS page */
+  int32_t  pad;
+  int64_t  hdr_offset[3];  /* header packets 0, 1, 2 in data; offset and bytes -1 for one not found */
+  int32_t  hdr_bytes[3];
+  int32_t  pad2;
+} vb200_ogg_stream;
+int vb200_ogg_demux_dev(int nfiles, const uint8_t *d_bytes, const int64_t *d_file_off, int max_packets,
+                        struct vb200_packet_info *d_info, int32_t *d_npkt, uint8_t *d_data, vb200_ogg_stream *d_streams,
+                        void *stream);
+int vb200_ogg_demux    (int nfiles, const uint8_t *bytes, const int64_t *file_off, int max_packets,
+                        struct vb200_packet_info *info, int32_t *npkt, uint8_t *data, vb200_ogg_stream *streams);
+
+/* The rising half window of an n-sample block as the reference tabulates it (lib/window.c vwin64 .. vwin8192): out[i] =
+ * sin(.5*pi*sin^2((i+.5)/n*pi)) evaluated in double, printed with "%.10f" and read back with strtof, for i < n/2.
+ * That equals every entry of the reference's tables; the closed form the context uses for vb200_setup.window = NULL
+ * is up to 1 ulp off.  Pass these as vb200_setup.window for a bit-exact decoder, and the tables of blocksizes[w]/2 to
+ * vb200_synthesis_halfrate.  Plain host code.  Returns VB200_EINVAL unless n is a power of two in [64, 8192].       */
+int vb200_vorbis_window(int n, float *out);
+
 /* ---- encode: the entropy coding of mapping0_forward (lib/mapping0.c:596-687) on the device, un-managed bitrate.
  * What floor1_encode (lib/floor1.c:753-921) and the residue class / forward of types 1 and 2 (lib/res0.c:534-648,
  * 725-809) read, registered on a context with vb200_encode_entropy_setup.

@@ -231,6 +231,11 @@ assert DECODED_PACKET_DTYPE.itemsize == 24
 # vb200_pcm_range: one request of vb200_decode_ranges, samples [start, start + length) of stream `stream`
 PCM_RANGE_DTYPE = np.dtype([("start", "<i8"), ("stream", "<i4"), ("length", "<i4")])
 assert PCM_RANGE_DTYPE.itemsize == 16
+# vb200_ogg_stream: what vb200_ogg_demux reports per file
+OGG_STREAM_DTYPE = np.dtype([("status", "<i4"), ("serial", "<u4"), ("pages", "<i4"), ("dropped", "<i4"),
+                             ("holes", "<i4"), ("foreign", "<i4"), ("chained", "<i4"), ("pad", "<i4"),
+                             ("hdr_offset", "<i8", (3,)), ("hdr_bytes", "<i4", (3,)), ("pad2", "<i4")])
+assert OGG_STREAM_DTYPE.itemsize == 72 and OGG_STREAM_DTYPE.fields["hdr_offset"][1] == 32
 
 
 class Codebook(C.Structure):

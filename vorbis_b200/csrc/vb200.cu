@@ -29,6 +29,7 @@
 #include "vb200_decode_streams.cuh"
 #include "vb200_decode_ranges.cuh"
 #include "vb200_lpc.cuh"
+#include "vb200_ogg.cuh"
 #include "floor1_db_table.h"
 
 using namespace vb200;
@@ -4556,6 +4557,71 @@ extern "C" void vb200_envelope_apply_marks(const uint8_t *ret, int first_step, i
     if (ret[k] & 1) { mark[j] = 1; mark[j + 1] = 1; }
     if (ret[k] & 2) { mark[j] = 1; if (j > 0) mark[j - 1] = 1; }
   }
+}
+
+// ======================================================================== //
+// Ogg files in: the page demux (vb200_ogg.cuh) and the reference's tabulated windows
+static_assert(sizeof(vb200_ogg_stream) == 72 && offsetof(vb200_ogg_stream, hdr_offset) == 32 &&
+              offsetof(vb200_ogg_stream, hdr_bytes) == 56, "vb200_ogg_stream layout (OGG_STREAM_DTYPE in abi.py)");
+extern "C" int vb200_ogg_demux_dev(int nfiles, const uint8_t *d_bytes, const int64_t *d_file_off, int max_packets,
+                                   vb200_packet_info *d_info, int32_t *d_npkt, uint8_t *d_data,
+                                   vb200_ogg_stream *d_streams, void *stream) {
+  if (nfiles < 0 || max_packets < 1) return fail(VB200_EINVAL, "ogg_demux: nfiles < 0 or max_packets < 1");
+  if (nfiles == 0) return 0;
+  if (!d_bytes || !d_file_off || !d_info || !d_npkt || !d_data || !d_streams)
+    return fail(VB200_EINVAL, "ogg_demux: null pointer");
+  const int grid = (nfiles + OGG_WARPS - 1) / OGG_WARPS;
+  k_ogg_demux<<<grid, 32 * OGG_WARPS, 0, (cudaStream_t)stream>>>(nfiles, d_bytes, d_file_off, max_packets, d_info,
+                                                                  d_npkt, d_data, d_streams);
+  CU(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int vb200_ogg_demux(int nfiles, const uint8_t *bytes, const int64_t *file_off, int max_packets,
+                               vb200_packet_info *info, int32_t *npkt, uint8_t *data, vb200_ogg_stream *streams) {
+  if (nfiles < 0 || max_packets < 1) return fail(VB200_EINVAL, "ogg_demux: nfiles < 0 or max_packets < 1");
+  if (nfiles == 0) return 0;
+  if (!file_off || !info || !npkt || !streams) return fail(VB200_EINVAL, "ogg_demux: null pointer");
+  if (file_off[0] < 0) return fail(VB200_EINVAL, "ogg_demux: file_off[0] < 0");
+  for (int f = 0; f < nfiles; f++)
+    if (file_off[f + 1] < file_off[f]) return fail(VB200_EINVAL, "ogg_demux: file_off decreases");
+  const size_t total = (size_t)file_off[nfiles];
+  if (total && (!bytes || !data)) return fail(VB200_EINVAL, "ogg_demux: null pointer");
+  const size_t n_info = (size_t)nfiles * max_packets;
+  DevBuf buf;                                             // freed on return
+  uint8_t *db, *dd;
+  int64_t *doff;
+  vb200_packet_info *dinfo;
+  int32_t *dn;
+  vb200_ogg_stream *ds;
+  int rc = carve(buf, [&](Carve &c) {
+    db = c.take<uint8_t>(total); doff = c.take<int64_t>(nfiles + 1); dinfo = c.take<vb200_packet_info>(n_info);
+    dn = c.take<int32_t>(nfiles); dd = c.take<uint8_t>(total); ds = c.take<vb200_ogg_stream>(nfiles);
+  });
+  if (rc) return rc;
+  if (total) CU(cudaMemcpy(db, bytes, total, cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(doff, file_off, sizeof(int64_t) * (nfiles + 1), cudaMemcpyHostToDevice));
+  if (total) CU(cudaMemset(dd, 0, total));
+  if ((rc = vb200_ogg_demux_dev(nfiles, db, doff, max_packets, dinfo, dn, dd, ds, nullptr))) return rc;
+  CU(cudaMemcpy(npkt, dn, sizeof(int32_t) * nfiles, cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(streams, ds, sizeof(vb200_ogg_stream) * nfiles, cudaMemcpyDeviceToHost));
+  std::vector<vb200_packet_info> rows(n_info);
+  CU(cudaMemcpy(rows.data(), dinfo, sizeof(vb200_packet_info) * n_info, cudaMemcpyDeviceToHost));
+  for (int f = 0; f < nfiles; f++)                        // entries past npkt[f] are not written
+    memcpy(info + (size_t)f * max_packets, rows.data() + (size_t)f * max_packets, sizeof(vb200_packet_info) * npkt[f]);
+  if (total) CU(cudaMemcpy(data, dd, total, cudaMemcpyDeviceToHost));
+  return 0;
+}
+
+extern "C" int vb200_vorbis_window(int n, float *out) {
+  if (n < 64 || n > 8192 || !pow2(n) || !out) return fail(VB200_EINVAL, "vorbis_window: n must be 64, 128, .. 8192");
+  char txt[64];
+  for (int i = 0; i < n / 2; i++) {
+    const double s = sin((i + .5) / n * M_PI);
+    snprintf(txt, sizeof(txt), "%.10f", sin(.5 * M_PI * (s * s)));
+    out[i] = strtof(txt, nullptr);
+  }
+  return 0;
 }
 
 // ======================================================================== //

@@ -51,6 +51,7 @@ EXPORTS = [
     "vb200_encode_streams_packets_managed_resume",
     "vb200_encode_pcm_carry_bytes", "vb200_encode_pcm_carry_init", "vb200_encode_pcm_packets",
     "vb200_encode_pcm_packets_managed", "vb200_lpc_extrapolate",
+    "vb200_ogg_demux_dev", "vb200_ogg_demux", "vb200_vorbis_window",
     "vb200_malloc_device", "vb200_free_device", "vb200_memcpy_h2d", "vb200_memcpy_d2h", "vb200_synchronize",
 ]
 
@@ -182,6 +183,9 @@ def load():
     L.vb200_encode_pcm_packets.argtypes = [vp, C.c_int, C.c_int, C.POINTER(abi.PcmIO), vp, vp, vp, C.c_int64]
     L.vb200_encode_pcm_packets_managed.argtypes = [vp, C.c_int, C.POINTER(abi.PcmIO), vp, vp, vp, C.c_int64]
     L.vb200_lpc_extrapolate.argtypes = [vp, C.c_int, C.c_int, vp, C.c_int64, vp, C.c_int32, vp, vp, C.c_int64]
+    L.vb200_ogg_demux_dev.argtypes = [C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, vp]
+    L.vb200_ogg_demux.argtypes = [C.c_int, vp, vp, C.c_int, vp, vp, vp, vp]
+    L.vb200_vorbis_window.argtypes = [C.c_int, vp]
     L.vb200_malloc_device.argtypes = [vp, C.c_size_t, C.POINTER(vp)]
     L.vb200_free_device.argtypes = [vp, vp]
     L.vb200_memcpy_h2d.argtypes = [vp, vp, vp, C.c_size_t]
@@ -1243,3 +1247,48 @@ def synthesis_layout(Wseq, bs, channels, halfrate=False, carry_W=None, count=Non
     pcm_off = np.concatenate([np.zeros((ns, 1), np.int64), np.cumsum(fin, axis=1)[:, :-1]], axis=1)
     pcm_len = int(np.cumsum(fin, axis=1)[:, -1].max())
     return coef_off, pcm_off, int(flat.sum()), pcm_len
+
+
+# ---- Ogg Vorbis files in ----------------------------------------------------------------------------
+def _check(L, rc):
+    if rc != 0:
+        raise VB200Error("vb200 error %d: %s" % (rc, (L.vb200_last_error() or b"").decode()))
+
+
+def ogg_demux(files, max_packets=None, check=True):
+    """vb200_ogg_demux on a list of Ogg files (bytes or uint8 arrays), on the current CUDA device.  Returns {"data"
+    uint8 (every file's packets inside its own byte range, zeros elsewhere), "file_off" int64 [n+1], "info"
+    PACKET_INFO_DTYPE [n][max_packets], "npkt" int32 [n], "streams" OGG_STREAM_DTYPE [n], "rc"}.  max_packets
+    defaults to the most packets any of the files can hold: a page of 27 + k bytes or more ends at most k packets."""
+    L = load()
+    arrs = [np.frombuffer(bytes(f), np.uint8) for f in files]
+    n = len(arrs)
+    file_off = np.zeros(n + 1, np.int64)
+    file_off[1:] = np.cumsum([len(a) for a in arrs])
+    buf = np.ascontiguousarray(np.concatenate(arrs) if n else np.zeros(0, np.uint8))
+    if max_packets is None:
+        max_packets = max([1] + [len(a) * 255 // 282 + 1 for a in arrs])
+    info = np.zeros((n, max_packets), abi.PACKET_INFO_DTYPE)
+    npkt = np.zeros(n, np.int32)
+    data = np.zeros(max(len(buf), 1), np.uint8)
+    streams = np.zeros(n, abi.OGG_STREAM_DTYPE)
+    rc = L.vb200_ogg_demux(n, _ptr(buf), _ptr(file_off), max_packets, _ptr(info), _ptr(npkt), _ptr(data),
+                           _ptr(streams))
+    if check:
+        _check(L, rc)
+    return {"data": data[:len(buf)], "file_off": file_off, "info": info, "npkt": npkt, "streams": streams, "rc": rc}
+
+
+def ogg_demux_dev(nfiles, d_bytes, d_file_off, max_packets, d_info, d_npkt, d_data, d_streams, stream=None):
+    """vb200_ogg_demux_dev: device pointers (ints, e.g. torch tensors' data_ptr()), asynchronous on `stream`"""
+    L = load()
+    _check(L, L.vb200_ogg_demux_dev(nfiles, _ptr(d_bytes), _ptr(d_file_off), max_packets, _ptr(d_info), _ptr(d_npkt),
+                                    _ptr(d_data), _ptr(d_streams), _ptr(stream)))
+
+
+def vorbis_window(n):
+    """vb200_vorbis_window: the reference's tabulated rising half window of an n-sample block, float32 [n/2]"""
+    L = load()
+    out = np.zeros(max(n // 2, 1), np.float32)
+    _check(L, L.vb200_vorbis_window(n, _ptr(out)))
+    return out[:n // 2]
