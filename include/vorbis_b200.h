@@ -852,6 +852,83 @@ int vb200_ogg_demux    (int nfiles, const uint8_t *bytes, const int64_t *file_of
  * vb200_synthesis_halfrate.  Plain host code.  Returns VB200_EINVAL unless n is a power of two in [64, 8192].       */
 int vb200_vorbis_window(int n, float *out);
 
+/* ---- the three header packets to a decode context, without libvorbis (host code, vorbis_b200/csrc/vb200_headers.h).
+ * vb200_vorbis_headers_parse reads the identification, comment and setup packets as vorbis_synthesis_headerin x3 and
+ * vorbis_synthesis_init read them (lib/info.c:211-450 with the unpacks of lib/codebook.c, floor1.c, floor0.c, res0.c
+ * and mapping0.c; lib/block.c:170-292 with vorbis_book_init_decode, lib/sharedbook.c:393-519), bit reader included
+ * (a read past the end returns -1 and so does every later one).  The comment header is validated, its tags are not
+ * returned.  On success *out holds:
+ *   setup    what vb200_ctx_create takes for a decoder: channels, rate, block sizes, the vb200_vorbis_window tables,
+ *            coupling, submaps, chmux and the floor-1 setups of both modes' submaps; n_psy 0, residue types -1
+ *   entropy  what vb200_decode_entropy_setup takes: every book as its codewords (original entry numbers; the value rows
+ *            the reference's valuelist holds, bit for bit), the floor and residue decode fields of both modes'
+ *            submaps, modebits
+ * so a decoder is vb200_ctx_create(&h->setup, ..) then vb200_decode_entropy_setup(ctx, &h->entropy).  Everything it
+ * points to belongs to it; free it with vb200_vorbis_headers_free.  Returns:
+ *   the reference's own code where the reference refuses the set: VB200_ENOTVORBIS (a packet without the "vorbis"
+ *     magic), VB200_EVERSION (version != 0), VB200_EBADHEADER (every other refusal, a vorbis_synthesis_init failure
+ *     included);
+ *   VB200_EIMPL where the reference takes the set but these structs cannot describe it: modes other than exactly two
+ *     with block flags 0 and 1, a submap of either mode on a floor of type 0, more than VB200_MAX_SUBMAPS submaps in
+ *     either mode, a book whose dimension is outside 1..127, or tables beyond the caps below (more than
+ *     VB200_HEADERS_MAX_CODEWORDS codewords or VB200_HEADERS_MAX_VALUES value-row floats over all books);
+ *   0 otherwise, also where vb200_ctx_create or vb200_decode_entropy_setup will refuse the result (a floor wider than
+ *     the block, residue type 0): those keep their own checks.
+ * VB200_EINVAL for a null pointer or a negative size, VB200_EFAULT when memory runs out.  The packet bytes are never
+ * read outside [0, bytes).  The tables hold one row per codeword, and an ordered book states up to 2^24 entries in a
+ * few bytes, so the totals are capped (VB200_EIMPL past them, decided before anything per codeword is allocated):
+ * about 150 MB of codewords and 256 MB of value rows at most, whatever the header says.                             */
+#define VB200_EVERSION (-134)   /* OV_EVERSION */
+#define VB200_HEADERS_MAX_CODEWORDS (1L << 24)   /* codewords over all books (one full-size book)      */
+#define VB200_HEADERS_MAX_VALUES    (1L << 26)   /* value-row floats over all books                    */
+typedef struct vb200_vorbis_headers {
+  int32_t channels, rate, bitrate_upper, bitrate_nominal, bitrate_lower, blocksizes[2];
+  int32_t pad;
+  vb200_setup setup;
+  vb200_entropy_setup entropy;
+} vb200_vorbis_headers;
+int  vb200_vorbis_headers_parse(const uint8_t *id, int32_t id_bytes, const uint8_t *comment, int32_t comment_bytes,
+                                const uint8_t *setup, int32_t setup_bytes, vb200_vorbis_headers **out);
+void vb200_vorbis_headers_free(vb200_vorbis_headers *h);
+
+/* ---- Ogg files grouped by setup on the device: after vb200_ogg_demux[_dev], the files whose identification and setup
+ * header packets are byte-identical form one group, whatever their comment headers hold.  Inputs are the demux's
+ * outputs (data, streams, max_packets, npkt, info).  Outputs:
+ *   status [nfiles]   the demux status, or VB200_EBADHEADER where a file with its three header packets (status 0 or
+ *                     VB200_EINVAL) has a comment header that vorbis_synthesis_headerin refuses (packet type, magic,
+ *                     _vorbis_unpack_comment's rules).  Files whose status stays 0 or VB200_EINVAL are grouped: an
+ *                     VB200_EINVAL file (max_packets cut its table) keeps that status and joins its group with the
+ *                     first max_packets audio packets.
+ *   order [nfiles]    the original file index at each position: the groups in order of their lowest file index, the
+ *                     files of a group in their original order, then every file left out (any other status) in its
+ *                     order
+ *   npkt_out [nfiles], info_out [nfiles][max_packets]   npkt and info rows in that order (rows past npkt are not
+ *                     written).  The offsets stay absolute into data, so group g is npkt_out + first and
+ *                     info_out + first * max_packets, what vb200_decode_streams_packets and vb200_decode_ranges take.
+ *   groups [ngroups]  {first position, files, rep}: rep is the group's lowest original file index; its hdr_offset /
+ *                     hdr_bytes in streams locate the header packets to copy back for vb200_vorbis_headers_parse.
+ *   ngroups [1]
+ * Membership is decided by comparing bytes: a hash only proposes the candidate, and a hash collision costs a scan over
+ * the lower files, never a wrong merge.  Five kernel launches whatever nfiles and the number of groups are; device
+ * scratch of vb200_ogg_group_scratch_bytes(nfiles, max_packets) bytes comes from the caller (max_packets does not
+ * change it today).
+ * _dev: device pointers, asynchronous on `stream`; checks its pointers (info 16-byte and scratch 8-byte aligned),
+ * nfiles >= 0, max_packets >= 1 and the scratch size only.  Host form: host buffers on the current CUDA device; also checks that every header range of a file with
+ * status 0 or VB200_EINVAL lies inside data (data_bytes) and that npkt is within 0..max_packets.                     */
+typedef struct vb200_file_group {
+  int32_t first, files, rep;
+} vb200_file_group;
+size_t vb200_ogg_group_scratch_bytes(int nfiles, int max_packets);
+int vb200_ogg_group_dev(int nfiles, const uint8_t *d_data, const vb200_ogg_stream *d_streams, int max_packets,
+                        const int32_t *d_npkt, const struct vb200_packet_info *d_info, int32_t *d_status,
+                        int32_t *d_order, int32_t *d_npkt_out, struct vb200_packet_info *d_info_out,
+                        vb200_file_group *d_groups, int32_t *d_ngroups, void *d_scratch, size_t scratch_bytes,
+                        void *stream);
+int vb200_ogg_group    (int nfiles, const uint8_t *data, int64_t data_bytes, const vb200_ogg_stream *streams,
+                        int max_packets, const int32_t *npkt, const struct vb200_packet_info *info, int32_t *status,
+                        int32_t *order, int32_t *npkt_out, struct vb200_packet_info *info_out,
+                        vb200_file_group *groups, int32_t *ngroups);
+
 /* ---- encode: the entropy coding of mapping0_forward (lib/mapping0.c:596-687) on the device, un-managed bitrate.
  * What floor1_encode (lib/floor1.c:753-921) and the residue class / forward of types 1 and 2 (lib/res0.c:534-648,
  * 725-809) read, registered on a context with vb200_encode_entropy_setup.

@@ -288,6 +288,22 @@ class EntropySetup(C.Structure):
     ]
 
 
+class VorbisHeaders(C.Structure):
+    """vb200_vorbis_headers: what vb200_vorbis_headers_parse returns"""
+    _fields_ = [
+        ("channels", C.c_int32), ("rate", C.c_int32), ("bitrate_upper", C.c_int32), ("bitrate_nominal", C.c_int32),
+        ("bitrate_lower", C.c_int32), ("blocksizes", C.c_int32 * 2), ("pad", C.c_int32),
+        ("setup", Setup),
+        ("entropy", EntropySetup),
+    ]
+
+
+assert VorbisHeaders.setup.offset == 32 and VorbisHeaders.entropy.offset == 32 + C.sizeof(Setup)
+# vb200_file_group: one group of vb200_ogg_group
+FILE_GROUP_DTYPE = np.dtype([("first", "<i4"), ("files", "<i4"), ("rep", "<i4")])
+assert FILE_GROUP_DTYPE.itemsize == 12
+
+
 class EncCodebook(C.Structure):
     """vb200_enc_codebook"""
     _fields_ = [

@@ -30,6 +30,8 @@
 #include "vb200_decode_ranges.cuh"
 #include "vb200_lpc.cuh"
 #include "vb200_ogg.cuh"
+#include "vb200_headers.h"
+#include "vb200_ogg_group.cuh"
 #include "floor1_db_table.h"
 
 using namespace vb200;
@@ -4615,12 +4617,113 @@ extern "C" int vb200_ogg_demux(int nfiles, const uint8_t *bytes, const int64_t *
 
 extern "C" int vb200_vorbis_window(int n, float *out) {
   if (n < 64 || n > 8192 || !pow2(n) || !out) return fail(VB200_EINVAL, "vorbis_window: n must be 64, 128, .. 8192");
-  char txt[64];
-  for (int i = 0; i < n / 2; i++) {
-    const double s = sin((i + .5) / n * M_PI);
-    snprintf(txt, sizeof(txt), "%.10f", sin(.5 * M_PI * (s * s)));
-    out[i] = strtof(txt, nullptr);
+  vbh::window(n, out);
+  return 0;
+}
+
+// ======================================================================== //
+// Ogg files grouped by setup (vb200_ogg_group.cuh) and the header packets to a decode description (vb200_headers.h)
+static_assert(sizeof(vb200_file_group) == 12, "vb200_file_group layout (FILE_GROUP_DTYPE in abi.py)");
+static_assert(offsetof(vb200_vorbis_headers, setup) == 32 &&
+              offsetof(vb200_vorbis_headers, entropy) == 32 + sizeof(vb200_setup),
+              "vb200_vorbis_headers layout (abi.VorbisHeaders)");
+
+// the scratch of one grouping call, in the order k_ogg_group_* use it; base = nullptr: sizes only
+static size_t ogg_group_layout(int nfiles, char *base, OggGroupScratch *sc) {
+  Carve c{base, 0};
+  const uint32_t slots = ogg_group_slots(nfiles);
+  sc->hash = c.take<unsigned long long>(nfiles);
+  sc->rep = c.take<int32_t>(nfiles);
+  sc->cnt = c.take<int32_t>(nfiles);
+  sc->first = c.take<int32_t>(nfiles);
+  sc->run = c.take<int32_t>(nfiles);
+  sc->tkey = c.take<unsigned long long>(slots);
+  sc->tmin = c.take<int32_t>(slots);
+  sc->slots = slots;
+  return c.off;
+}
+
+extern "C" size_t vb200_ogg_group_scratch_bytes(int nfiles, int max_packets) {
+  (void)max_packets;
+  OggGroupScratch sc;
+  return ogg_group_layout(nfiles < 0 ? 0 : nfiles, nullptr, &sc);
+}
+
+extern "C" int vb200_ogg_group_dev(int nfiles, const uint8_t *d_data, const vb200_ogg_stream *d_streams,
+                                   int max_packets, const int32_t *d_npkt, const vb200_packet_info *d_info,
+                                   int32_t *d_status, int32_t *d_order, int32_t *d_npkt_out,
+                                   vb200_packet_info *d_info_out, vb200_file_group *d_groups, int32_t *d_ngroups,
+                                   void *d_scratch, size_t scratch_bytes, void *stream) {
+  if (nfiles < 0 || max_packets < 1) return fail(VB200_EINVAL, "ogg_group: nfiles < 0 or max_packets < 1");
+  if (!d_ngroups) return fail(VB200_EINVAL, "ogg_group: null pointer");
+  cudaStream_t s = (cudaStream_t)stream;
+  if (nfiles == 0) { CU(cudaMemsetAsync(d_ngroups, 0, sizeof(int32_t), s)); return 0; }
+  if (!d_data || !d_streams || !d_npkt || !d_info || !d_status || !d_order || !d_npkt_out || !d_info_out ||
+      !d_groups || !d_scratch)
+    return fail(VB200_EINVAL, "ogg_group: null pointer");
+  if (((uintptr_t)d_info | (uintptr_t)d_info_out) & 15) return fail(VB200_EINVAL, "ogg_group: info not 16-byte aligned");
+  if ((uintptr_t)d_scratch & 7) return fail(VB200_EINVAL, "ogg_group: scratch not 8-byte aligned");
+  OggGroupScratch sc;
+  if (scratch_bytes < ogg_group_layout(nfiles, nullptr, &sc)) return fail(VB200_EINVAL, "ogg_group: scratch too small");
+  ogg_group_layout(nfiles, (char *)d_scratch, &sc);
+  const int wgrid = (nfiles + OGG_GROUP_WARPS - 1) / OGG_GROUP_WARPS;
+  k_ogg_group_key<<<wgrid, 32 * OGG_GROUP_WARPS, 0, s>>>(nfiles, d_data, d_streams, d_status, sc);
+  k_ogg_group_insert<<<(nfiles + 255) / 256, 256, 0, s>>>(nfiles, d_status, sc);
+  k_ogg_group_rep<<<wgrid, 32 * OGG_GROUP_WARPS, 0, s>>>(nfiles, d_data, d_streams, d_status, sc);
+  k_ogg_group_order<<<1, OGG_GROUP_ORDER_THREADS, 0, s>>>(nfiles, d_status, d_order, d_groups, d_ngroups, sc);
+  k_ogg_group_gather<<<wgrid, 32 * OGG_GROUP_WARPS, 0, s>>>(nfiles, max_packets, d_order, d_npkt, d_info, d_npkt_out,
+                                                            d_info_out);
+  CU(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int vb200_ogg_group(int nfiles, const uint8_t *data, int64_t data_bytes, const vb200_ogg_stream *streams,
+                               int max_packets, const int32_t *npkt, const vb200_packet_info *info, int32_t *status,
+                               int32_t *order, int32_t *npkt_out, vb200_packet_info *info_out,
+                               vb200_file_group *groups, int32_t *ngroups) {
+  if (nfiles < 0 || max_packets < 1 || data_bytes < 0) return fail(VB200_EINVAL, "ogg_group: bad sizes");
+  if (!ngroups) return fail(VB200_EINVAL, "ogg_group: null pointer");
+  *ngroups = 0;
+  if (nfiles == 0) return 0;
+  if (!streams || !npkt || !info || !status || !order || !npkt_out || !info_out || !groups || (data_bytes && !data))
+    return fail(VB200_EINVAL, "ogg_group: null pointer");
+  for (int f = 0; f < nfiles; f++) {
+    if (npkt[f] < 0 || npkt[f] > max_packets) return fail(VB200_EINVAL, "ogg_group: npkt outside 0..max_packets");
+    if (streams[f].status != 0 && streams[f].status != VB200_EINVAL) continue;
+    for (int k = 0; k < 3; k++)
+      if (streams[f].hdr_offset[k] < 0 || streams[f].hdr_bytes[k] < 0 ||
+          streams[f].hdr_offset[k] + streams[f].hdr_bytes[k] > data_bytes)
+        return fail(VB200_EINVAL, "ogg_group: a header packet outside data");
   }
+  const size_t n_info = (size_t)nfiles * max_packets;
+  const size_t sbytes = vb200_ogg_group_scratch_bytes(nfiles, max_packets);
+  DevBuf buf;                                             // freed on return
+  uint8_t *dd; vb200_ogg_stream *ds; int32_t *dn, *dst, *dord, *dno, *dng; vb200_packet_info *di, *dio;
+  vb200_file_group *dg; char *dscr;
+  int rc = carve(buf, [&](Carve &c) {
+    dd = c.take<uint8_t>((size_t)data_bytes); ds = c.take<vb200_ogg_stream>(nfiles); dn = c.take<int32_t>(nfiles);
+    di = c.take<vb200_packet_info>(n_info); dst = c.take<int32_t>(nfiles); dord = c.take<int32_t>(nfiles);
+    dno = c.take<int32_t>(nfiles); dio = c.take<vb200_packet_info>(n_info); dg = c.take<vb200_file_group>(nfiles);
+    dng = c.take<int32_t>(1); dscr = c.take<char>(sbytes);
+  });
+  if (rc) return rc;
+  if (data_bytes) CU(cudaMemcpy(dd, data, (size_t)data_bytes, cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(ds, streams, sizeof(vb200_ogg_stream) * nfiles, cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(dn, npkt, sizeof(int32_t) * nfiles, cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(di, info, sizeof(vb200_packet_info) * n_info, cudaMemcpyHostToDevice));
+  if ((rc = vb200_ogg_group_dev(nfiles, dd, ds, max_packets, dn, di, dst, dord, dno, dio, dg, dng, dscr, sbytes,
+                                nullptr)))
+    return rc;
+  CU(cudaMemcpy(status, dst, sizeof(int32_t) * nfiles, cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(order, dord, sizeof(int32_t) * nfiles, cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(npkt_out, dno, sizeof(int32_t) * nfiles, cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(ngroups, dng, sizeof(int32_t), cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(groups, dg, sizeof(vb200_file_group) * *ngroups, cudaMemcpyDeviceToHost));
+  std::vector<vb200_packet_info> rows(n_info);
+  CU(cudaMemcpy(rows.data(), dio, sizeof(vb200_packet_info) * n_info, cudaMemcpyDeviceToHost));
+  for (int p = 0; p < nfiles; p++)                        // rows past npkt_out[p] are not written
+    memcpy(info_out + (size_t)p * max_packets, rows.data() + (size_t)p * max_packets,
+           sizeof(vb200_packet_info) * npkt_out[p]);
   return 0;
 }
 

@@ -52,6 +52,8 @@ EXPORTS = [
     "vb200_encode_pcm_carry_bytes", "vb200_encode_pcm_carry_init", "vb200_encode_pcm_packets",
     "vb200_encode_pcm_packets_managed", "vb200_lpc_extrapolate",
     "vb200_ogg_demux_dev", "vb200_ogg_demux", "vb200_vorbis_window",
+    "vb200_vorbis_headers_parse", "vb200_vorbis_headers_free",
+    "vb200_ogg_group_scratch_bytes", "vb200_ogg_group_dev", "vb200_ogg_group",
     "vb200_malloc_device", "vb200_free_device", "vb200_memcpy_h2d", "vb200_memcpy_d2h", "vb200_synchronize",
 ]
 
@@ -186,6 +188,14 @@ def load():
     L.vb200_ogg_demux_dev.argtypes = [C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, vp]
     L.vb200_ogg_demux.argtypes = [C.c_int, vp, vp, C.c_int, vp, vp, vp, vp]
     L.vb200_vorbis_window.argtypes = [C.c_int, vp]
+    L.vb200_vorbis_headers_parse.argtypes = [vp, C.c_int32, vp, C.c_int32, vp, C.c_int32,
+                                             C.POINTER(C.POINTER(abi.VorbisHeaders))]
+    L.vb200_vorbis_headers_free.argtypes = [C.POINTER(abi.VorbisHeaders)]
+    L.vb200_vorbis_headers_free.restype = None
+    L.vb200_ogg_group_scratch_bytes.argtypes = [C.c_int, C.c_int]
+    L.vb200_ogg_group_scratch_bytes.restype = C.c_size_t
+    L.vb200_ogg_group_dev.argtypes = [C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_size_t, vp]
+    L.vb200_ogg_group.argtypes = [C.c_int, vp, C.c_int64, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp]
     L.vb200_malloc_device.argtypes = [vp, C.c_size_t, C.POINTER(vp)]
     L.vb200_free_device.argtypes = [vp, vp]
     L.vb200_memcpy_h2d.argtypes = [vp, vp, vp, C.c_size_t]
@@ -1292,3 +1302,83 @@ def vorbis_window(n):
     out = np.zeros(max(n // 2, 1), np.float32)
     _check(L, L.vb200_vorbis_window(n, _ptr(out)))
     return out[:n // 2]
+
+
+# ---- the header packets to a decode context, and files grouped by setup ---------------------------------------
+class VorbisHeaders:
+    """vb200_vorbis_headers_parse of three header packets (bytes).  .info: channels, rate, the three bitrates and
+    blocksizes; .c / .entropy: the vb200_setup and vb200_entropy_setup it holds (views into it); .context(device)
+    a Context with the entropy setup registered.  Raises VB200Error with .code where the parse refuses the headers."""
+
+    def __init__(self, id_, comment, setup):
+        self.L = load()
+        self._p = C.POINTER(abi.VorbisHeaders)()
+        bufs = [np.frombuffer(bytes(b) + b"\0", np.uint8) for b in (id_, comment, setup)]
+        rc = self.L.vb200_vorbis_headers_parse(_ptr(bufs[0]), len(id_), _ptr(bufs[1]), len(comment), _ptr(bufs[2]),
+                                               len(setup), C.byref(self._p))
+        if rc != 0:
+            self._p = None
+            e = VB200Error("vb200_vorbis_headers_parse: %d" % rc)
+            e.code = rc
+            raise e
+        h = self._p.contents
+        self.h = h
+        self.c = h.setup
+        self.entropy = h.entropy
+        self.channels = int(h.channels)
+        self.rate = int(h.rate)
+        self.blocksizes = [int(h.blocksizes[0]), int(h.blocksizes[1])]
+        self.bitrates = (int(h.bitrate_upper), int(h.bitrate_nominal), int(h.bitrate_lower))
+
+    def blocksize(self, W):
+        return self.blocksizes[W]
+
+    def context(self, device=0):
+        """a Context on these headers' setup, with the entropy setup registered; it keeps this object alive"""
+        ctx = Context(self, device)
+        ctx.decode_entropy_setup(self.entropy)
+        return ctx
+
+    def __del__(self):
+        if getattr(self, "_p", None):
+            self.L.vb200_vorbis_headers_free(self._p)
+            self._p = None
+
+
+def vorbis_headers(id_, comment, setup):
+    """vb200_vorbis_headers_parse: a VorbisHeaders (see there)"""
+    return VorbisHeaders(id_, comment, setup)
+
+
+def ogg_group(res, check=True):
+    """vb200_ogg_group on the outputs of ogg_demux (a dict as it returns).  Returns {"status", "order", "npkt",
+    "info" (permuted), "groups" FILE_GROUP_DTYPE [ngroups], "rc"}"""
+    L = load()
+    st = np.ascontiguousarray(res["streams"])
+    info = np.ascontiguousarray(res["info"])
+    n, mp = info.shape
+    npkt = np.ascontiguousarray(res["npkt"], np.int32)
+    data = np.ascontiguousarray(res["data"], np.uint8)
+    status, order, npkt_out = (np.zeros(n, np.int32) for _ in range(3))
+    info_out = np.zeros_like(info)
+    groups = np.zeros(max(n, 1), abi.FILE_GROUP_DTYPE)
+    ng = np.zeros(1, np.int32)
+    rc = L.vb200_ogg_group(n, _ptr(data), data.size, _ptr(st), mp, _ptr(npkt), _ptr(info), _ptr(status), _ptr(order),
+                           _ptr(npkt_out), _ptr(info_out), _ptr(groups), _ptr(ng))
+    if check:
+        _check(L, rc)
+    return {"status": status, "order": order, "npkt": npkt_out, "info": info_out, "groups": groups[:int(ng[0])],
+            "rc": rc}
+
+
+def ogg_group_scratch_bytes(nfiles, max_packets):
+    return int(load().vb200_ogg_group_scratch_bytes(nfiles, max_packets))
+
+
+def ogg_group_dev(nfiles, d_data, d_streams, max_packets, d_npkt, d_info, d_status, d_order, d_npkt_out, d_info_out,
+                  d_groups, d_ngroups, d_scratch, scratch_bytes, stream=None):
+    """vb200_ogg_group_dev: device pointers (ints, e.g. torch tensors' data_ptr()), asynchronous on `stream`"""
+    L = load()
+    _check(L, L.vb200_ogg_group_dev(nfiles, _ptr(d_data), _ptr(d_streams), max_packets, _ptr(d_npkt), _ptr(d_info),
+                                    _ptr(d_status), _ptr(d_order), _ptr(d_npkt_out), _ptr(d_info_out),
+                                    _ptr(d_groups), _ptr(d_ngroups), _ptr(d_scratch), scratch_bytes, _ptr(stream)))
