@@ -1955,8 +1955,10 @@ static int enc_stage(HostIO &io, const vb200_encode_io *h, vb200_encode_io *d, i
   return 0;
 }
 
-static int enc_check(vb200_ctx *c, int W, int nstreams, int bps, int blobno, const vb200_encode_io *io) {
-  if (!io || !io->pcm || !io->desc || !io->posts || !io->nonzero || !io->iwork || !io->ampmax_out)
+// own_outputs: the call stages posts / nonzero / iwork itself, so the io need not give them
+static int enc_check(vb200_ctx *c, int W, int nstreams, int bps, int blobno, const vb200_encode_io *io,
+                     bool own_outputs = false) {
+  if (!io || !io->pcm || !io->desc || !io->ampmax_out || (!own_outputs && (!io->posts || !io->nonzero || !io->iwork)))
     return fail(VB200_EINVAL, "encode io pointers");
   if (io->iwork_fmt != VB200_IWORK_S32 && io->iwork_fmt != VB200_IWORK_S16) return fail(VB200_EINVAL, "iwork format");
   if (io->iwork_fmt == VB200_IWORK_S16 && !io->overflow) return fail(VB200_EINVAL, "int16 residue needs the overflow array");
@@ -1978,19 +1980,74 @@ static int enc_check(vb200_ctx *c, int W, int nstreams, int bps, int blobno, con
   return 0;
 }
 
-// all pointers device; S holds the float intermediates
+// ---- bitrate-managed mode (lib/mapping0.c:507-573, 596-646): the chain with three masks, three fits, the twelve
+// interpolated curves, and the floor render + couple/quantise/normalise of every one of the 15 curves
+
+// scratch of the managed tail: the psy stage's noise and tone taps, the low- / high-noise mask, the flags of the
+// three fits and the present flag of every curve
+struct MgdScratch {
+  float *noise, *tone, *alt;
+  int32_t *fz3, *present;
+};
+
+static void mgd_layout(Carve &k, size_t rows, size_t blob_rows, size_t n, MgdScratch *M) {
+  M->noise = k.take<float>(rows * n);
+  M->tone = k.take<float>(rows * n);
+  M->alt = k.take<float>(rows * n);
+  M->fz3 = k.take<int32_t>(rows * 3);
+  M->present = k.take<int32_t>(blob_rows * VB200_PACKETBLOBS);
+}
+
+// Bitrate-managed mode after the psy stage (run with the noise and tone taps into M): the middle fit, the
+// low-noise (2) and high-noise (0) masks and their fits, the twelve interpolated curves, then the floor render,
+// couple/quantise/normalise and nonzero propagation of all 15 curves.  posts / nonzero / iwork are blob-major
+// with blob_blocks blocks (>= nblocks) from one curve to the next.
+static int managed_tail(vb200_ctx *c, int W, int nblocks, long long blob_blocks, const vb200_block_desc *d_desc,
+                        const float *mdct, const float *logmdct, const float *logmask, const MgdScratch &M,
+                        int32_t *posts, int32_t *nonzero, int32_t *iwork, cudaStream_t st) {
+  constexpr int NB = VB200_PACKETBLOBS, MID = VB200_PACKETBLOBS / 2;
+  const int ch = c->setup.channels, n = c->dx[W].N / 2;
+  const size_t rows = (size_t)nblocks * ch, brows = (size_t)blob_blocks * ch, pblob = brows * VB200_FLOOR1_STRIDE;
+  int32_t *fz_lo = M.fz3, *fz_mid = M.fz3 + rows, *fz_hi = M.fz3 + 2 * rows;
+  int rc;
+  // the middle curve (select 1, what un-managed mode codes), then the low-noise (2) and high-noise (0) masks
+  if ((rc = vb200_floor1_fit_dev(c, W, -1, (int)rows, logmdct, logmask, posts + MID * pblob, fz_mid, st))) return rc;
+  const PsyDev &P0 = c->dpsy[(W ? 2 : 0)], &P1 = c->dpsy[(W ? 2 : 0) + 1];
+  const long long total = (long long)rows * n;
+  for (int pass = 0; pass < 2; pass++) {
+    const int sel = pass ? 0 : 2;
+    k_mix_select<<<grid_for(c, (int)((total + 255) / 256), 8), 256, 0, st>>>(P0, P1, d_desc, ch, total, sel, M.noise,
+                                                                            M.tone, logmdct, M.alt);
+    if ((rc = post_launch(c))) return rc;
+    if ((rc = vb200_floor1_fit_dev(c, W, -1, (int)rows, logmdct, M.alt, posts + (sel ? NB - 1 : 0) * pblob,
+                                   sel ? fz_hi : fz_lo, st))) return rc;
+  }
+  k_floor1_interpolate<<<grid_for(c, (int)((rows * VB200_FLOOR1_STRIDE + 255) / 256), 8), 256, 0, st>>>(
+      (long long)rows, (long long)brows, posts, fz_lo, fz_mid, fz_hi, M.present);
+  if ((rc = post_launch(c))) return rc;
+  if ((rc = floor1_render_launch(c, W, -1, (int)rows, NB, (long long)brows, posts, M.present, iwork, nonzero, st)))
+    return rc;
+  return cqn_curves_launch(c, W, d_desc, nblocks, blob_blocks, mdct, iwork, nonzero, st);
+}
+
+// all pointers device; S holds the float intermediates.  M: bitrate-managed, the psy stage taps into M and
+// managed_tail codes every curve (blobno unused); null: the curve of blob blobno
 static int encode_launch(vb200_ctx *c, int W, int nstreams, int bps, int blobno, const vb200_encode_io *d,
-                         const EncScratch &S, cudaStream_t st) {
+                         const EncScratch &S, cudaStream_t st, const MgdScratch *M = nullptr) {
   const int ch = c->setup.channels, nblocks = nstreams * bps, rows = nblocks * ch;
   vb200_phaseA_io a;
   memset(&a, 0, sizeof(a));
   a.desc = d->desc; a.mdct = S.mdct; a.logmdct = S.logmdct; a.logmask = S.logmask; a.ampmax_out = d->ampmax_out;
+  if (M) { a.tap_noise = M->noise; a.tap_tone = M->tone; }
   PcmSrc ps; const PcmSrc *pp = nullptr;
   if (d->pcm_fmt == VB200_PCM_F32_BLOCKS) a.pcm = (const float *)d->pcm;
   else { ps.base = d->pcm; ps.fmt = d->pcm_fmt; ps.bps = bps; ps.hop = d->hop; ps.stride = d->stream_stride; ps.blk_src = nullptr; pp = &ps; }
   int rc;
   if ((rc = phaseA_launch(c, W, nblocks, &a, d->independent ? 0 : nstreams, bps, d->ampmax0, st,
                           S.logfft, S.lmax, S.gmax, pp))) return rc;
+  if (M)
+    return managed_tail(c, W, nblocks, nblocks, d->desc, S.mdct, S.logmdct, S.logmask, *M, d->posts, d->nonzero,
+                        (int32_t *)d->iwork, st);
   if ((rc = vb200_floor1_fit_dev(c, W, -1, rows, S.logmdct, S.logmask, d->posts, S.fitnz, st))) return rc;
   if (c->profiling) CU(cudaEventRecord(c->ev[4], st));
   const bool s16 = d->iwork_fmt == VB200_IWORK_S16;
@@ -2093,61 +2150,13 @@ extern "C" int vb200_encode_dsp_dev(vb200_ctx *c, int W, int nstreams, int bps, 
   return scratch_end(c, user);
 }
 
-// ---- bitrate-managed mode (lib/mapping0.c:507-573, 596-646): the chain above with three masks, three fits, the
-// twelve interpolated curves, and the floor render + couple/quantise/normalise of every one of the 15 curves
-static int managed_check(vb200_ctx *c, int W, int nstreams, int bps, const vb200_encode_io *io) {
+static int managed_check(vb200_ctx *c, int W, int nstreams, int bps, const vb200_encode_io *io,
+                         bool own_outputs = false) {
   int rc;
-  if ((rc = enc_check(c, W, nstreams, bps, VB200_PACKETBLOBS / 2, io))) return rc;
+  if ((rc = enc_check(c, W, nstreams, bps, VB200_PACKETBLOBS / 2, io, own_outputs))) return rc;
   if (io->iwork_fmt != VB200_IWORK_S32) return fail(VB200_EINVAL, "managed mode writes int32 residue");
   if (io->classes) return fail(VB200_EINVAL, "managed mode does not classify");
   return 0;
-}
-
-// scratch of the managed tail: the psy stage's noise and tone taps, the low- / high-noise mask, the flags of the
-// three fits and the present flag of every curve
-struct MgdScratch {
-  float *noise, *tone, *alt;
-  int32_t *fz3, *present;
-};
-
-static void mgd_layout(Carve &k, size_t rows, size_t blob_rows, size_t n, MgdScratch *M) {
-  M->noise = k.take<float>(rows * n);
-  M->tone = k.take<float>(rows * n);
-  M->alt = k.take<float>(rows * n);
-  M->fz3 = k.take<int32_t>(rows * 3);
-  M->present = k.take<int32_t>(blob_rows * VB200_PACKETBLOBS);
-}
-
-// Bitrate-managed mode after the psy stage (run with the noise and tone taps into M): the middle fit, the
-// low-noise (2) and high-noise (0) masks and their fits, the twelve interpolated curves, then the floor render,
-// couple/quantise/normalise and nonzero propagation of all 15 curves.  posts / nonzero / iwork are blob-major
-// with blob_blocks blocks (>= nblocks) from one curve to the next.
-static int managed_tail(vb200_ctx *c, int W, int nblocks, long long blob_blocks, const vb200_block_desc *d_desc,
-                        const float *mdct, const float *logmdct, const float *logmask, const MgdScratch &M,
-                        int32_t *posts, int32_t *nonzero, int32_t *iwork, cudaStream_t st) {
-  constexpr int NB = VB200_PACKETBLOBS, MID = VB200_PACKETBLOBS / 2;
-  const int ch = c->setup.channels, n = c->dx[W].N / 2;
-  const size_t rows = (size_t)nblocks * ch, brows = (size_t)blob_blocks * ch, pblob = brows * VB200_FLOOR1_STRIDE;
-  int32_t *fz_lo = M.fz3, *fz_mid = M.fz3 + rows, *fz_hi = M.fz3 + 2 * rows;
-  int rc;
-  // the middle curve (select 1, what un-managed mode codes), then the low-noise (2) and high-noise (0) masks
-  if ((rc = vb200_floor1_fit_dev(c, W, -1, (int)rows, logmdct, logmask, posts + MID * pblob, fz_mid, st))) return rc;
-  const PsyDev &P0 = c->dpsy[(W ? 2 : 0)], &P1 = c->dpsy[(W ? 2 : 0) + 1];
-  const long long total = (long long)rows * n;
-  for (int pass = 0; pass < 2; pass++) {
-    const int sel = pass ? 0 : 2;
-    k_mix_select<<<grid_for(c, (int)((total + 255) / 256), 8), 256, 0, st>>>(P0, P1, d_desc, ch, total, sel, M.noise,
-                                                                            M.tone, logmdct, M.alt);
-    if ((rc = post_launch(c))) return rc;
-    if ((rc = vb200_floor1_fit_dev(c, W, -1, (int)rows, logmdct, M.alt, posts + (sel ? NB - 1 : 0) * pblob,
-                                   sel ? fz_hi : fz_lo, st))) return rc;
-  }
-  k_floor1_interpolate<<<grid_for(c, (int)((rows * VB200_FLOOR1_STRIDE + 255) / 256), 8), 256, 0, st>>>(
-      (long long)rows, (long long)brows, posts, fz_lo, fz_mid, fz_hi, M.present);
-  if ((rc = post_launch(c))) return rc;
-  if ((rc = floor1_render_launch(c, W, -1, (int)rows, NB, (long long)brows, posts, M.present, iwork, nonzero, st)))
-    return rc;
-  return cqn_curves_launch(c, W, d_desc, nblocks, blob_blocks, mdct, iwork, nonzero, st);
 }
 
 extern "C" int vb200_encode_dsp_managed_dev(vb200_ctx *c, int W, int nstreams, int bps, const vb200_encode_io *d,
@@ -2156,27 +2165,15 @@ extern "C" int vb200_encode_dsp_managed_dev(vb200_ctx *c, int W, int nstreams, i
   int rc;
   if ((rc = managed_check(c, W, nstreams, bps, d))) return rc;
   cudaStream_t st = (cudaStream_t)stream;
-  const int ch = c->setup.channels, n = c->dx[W].N / 2, nblocks = nstreams * bps;
-  const size_t rows = (size_t)nblocks * ch;
-  float *mdct, *logmdct, *logmask, *logfft, *lmax, *gmax;
+  const size_t ch = c->setup.channels, n = c->dx[W].N / 2, nblocks = (size_t)nstreams * bps, rows = nblocks * ch;
+  EncScratch S;
   MgdScratch M;
   if ((rc = carve(c->mgd, [&](Carve &k) {
-         mdct = k.take<float>(rows * n); logmdct = k.take<float>(rows * n); logmask = k.take<float>(rows * n);
-         logfft = k.take<float>(rows * n); lmax = k.take<float>(rows); gmax = k.take<float>(nblocks);
+         enc_layout(k, rows, nblocks, n, nullptr, false, &S);        // the caller's spectra are not used
          mgd_layout(k, rows, rows, n, &M);
        }))) return rc;
   if ((rc = scratch_begin(c, st))) return rc;
-  vb200_phaseA_io a;
-  memset(&a, 0, sizeof(a));
-  a.desc = d->desc; a.mdct = mdct; a.logmdct = logmdct; a.logmask = logmask; a.ampmax_out = d->ampmax_out;
-  a.tap_noise = M.noise; a.tap_tone = M.tone;
-  PcmSrc ps; const PcmSrc *pp = nullptr;
-  if (d->pcm_fmt == VB200_PCM_F32_BLOCKS) a.pcm = (const float *)d->pcm;
-  else { ps.base = d->pcm; ps.fmt = d->pcm_fmt; ps.bps = bps; ps.hop = d->hop; ps.stride = d->stream_stride; ps.blk_src = nullptr; pp = &ps; }
-  if ((rc = phaseA_launch(c, W, nblocks, &a, d->independent ? 0 : nstreams, bps, d->ampmax0, st, logfft, lmax, gmax, pp)))
-    return rc;
-  if ((rc = managed_tail(c, W, nblocks, nblocks, d->desc, mdct, logmdct, logmask, M, d->posts, d->nonzero,
-                         (int32_t *)d->iwork, st))) return rc;
+  if ((rc = encode_launch(c, W, nstreams, bps, VB200_PACKETBLOBS / 2, d, S, st, &M))) return rc;
   return scratch_end(c, st);
 }
 
@@ -2356,14 +2353,28 @@ extern "C" int vb200_plan_blocks(vb200_ctx *c, int nstreams, const int32_t *mark
   return io.sync();
 }
 
-// arguments of both streams calls; zeroes count[] (nstreams <= 0: nothing to do)
-static int streams_check(vb200_ctx *c, int nstreams, vb200_streams_io *d) {
+// The start of every streams call: the context's plan setup and the io, whose count[] is zeroed.  A call that has
+// checks of its own runs them next, then returns for nstreams <= 0, then checks streams_inputs.
+static int streams_open(vb200_ctx *c, vb200_streams_io *h) {
   int rc;
   if ((rc = plan_check(c))) return rc;
-  if (!d) return fail(VB200_EINVAL, "null io");
-  d->count[0] = d->count[1] = 0;
-  if (nstreams <= 0) return 0;
-  if (!d->pcm || !d->pcm_len || !d->plan || !d->nblocks || d->max_blocks < 1) return fail(VB200_EINVAL, "encode_streams: pcm, pcm_len, plan, nblocks");
+  if (!h) return fail(VB200_EINVAL, "null io");
+  h->count[0] = h->count[1] = 0;
+  return 0;
+}
+
+// the inputs every streams call reads; name: the call, for the message
+static int streams_inputs(const vb200_streams_io *h, const char *name) {
+  if (!h->pcm || !h->pcm_len || !h->plan || !h->nblocks || h->max_blocks < 1)
+    return fail(VB200_EINVAL, (std::string(name) + ": pcm, pcm_len, plan, nblocks").c_str());
+  return 0;
+}
+
+// arguments of the device streams calls; zeroes count[] (nstreams <= 0: nothing to do)
+static int streams_check(vb200_ctx *c, int nstreams, vb200_streams_io *d) {
+  int rc;
+  if ((rc = streams_open(c, d)) || nstreams <= 0) return rc;
+  if ((rc = streams_inputs(d, "encode_streams"))) return rc;
   if (d->pcm_fmt != VB200_PCM_F32_PLANAR && d->pcm_fmt != VB200_PCM_S16_INTERLEAVED) return fail(VB200_EINVAL, "pcm_fmt");
   for (int w = 0; w < 2; w++)
     if (d->cap[w] < 0 || (d->cap[w] > 0 && (!d->posts[w] || !d->nonzero[w] || !d->iwork[w] || !d->ampmax_out[w])))
@@ -2375,8 +2386,9 @@ static int streams_check(vb200_ctx *c, int nstreams, vb200_streams_io *d) {
 // The front half of both streams calls, up to the psy stage: envelope search, marks, plan, the transforms of
 // both sizes and the ampmax chain along every stream.  Sets count[]; for each size with blocks, S[w] holds the
 // transforms, a[w] the psy stage's io, d_desc[w] the batch's block descriptors and, given M, M[w] the scratch of
-// the managed tail.  Begins the call's use of the context scratch.  K: carried streams (the envelope state, marks,
-// planner and ampmax chain start from the carries and go back to them); K->count's largest entry is nsteps_env.
+// the managed tail, which a[w] taps the noise and tone masks into.  Begins the call's use of the context scratch.
+// K: carried streams (the envelope state, marks, planner and ampmax chain start from the carries and go back to
+// them); K->count's largest entry is nsteps_env.
 static int streams_front(vb200_ctx *c, int nstreams, vb200_streams_io *d, cudaStream_t st, EncScratch S[2],
                          vb200_phaseA_io a[2], vb200_block_desc *d_desc[2], MgdScratch *M = nullptr,
                          const CarryDev *K = nullptr, int nsteps_env = 0) {
@@ -2440,6 +2452,7 @@ static int streams_front(vb200_ctx *c, int nstreams, vb200_streams_io *d, cudaSt
     const size_t nb = tot[w];
     a[w].desc = d_desc[w]; a[w].mdct = S[w].mdct; a[w].logmdct = S[w].logmdct; a[w].logmask = S[w].logmask;
     a[w].ampmax_out = d->ampmax_out[w];
+    if (M) { a[w].tap_noise = M[w].noise; a[w].tap_tone = M[w].tone; }
     PcmSrc ps; ps.base = d->pcm; ps.fmt = d->pcm_fmt; ps.bps = 1; ps.hop = 0; ps.stride = d->stream_stride; ps.blk_src = d_src[w];
     if ((rc = phaseA_transform_launch(c, w, (int)nb, &a[w], ps, st, S[w].logfft, S[w].lmax))) return rc;
   }
@@ -2460,23 +2473,30 @@ static int streams_front(vb200_ctx *c, int nstreams, vb200_streams_io *d, cudaSt
   return 0;
 }
 
-// desc_out (optional): the two batches' block descriptors, which stay in the plan arena until its next carve
-static int encode_streams_launch(vb200_ctx *c, int nstreams, int blobno, vb200_streams_io *d, cudaStream_t stream,
-                                 vb200_block_desc **desc_out, const CarryDev *K = nullptr, int nsteps_env = 0) {
+// managed: the bitrate-managed chain, every curve cap[w] blocks after the one before (blobno unused).  desc_out
+// (optional): the two batches' block descriptors, which stay in the plan arena until its next carve
+static int encode_streams_launch(vb200_ctx *c, int nstreams, int blobno, bool managed, vb200_streams_io *d,
+                                 cudaStream_t st, vb200_block_desc **desc_out, const CarryDev *K = nullptr,
+                                 int nsteps_env = 0) {
   int rc;
   if ((rc = streams_check(c, nstreams, d)) || nstreams <= 0) return rc;
-  if (blobno < 0 || blobno >= VB200_PACKETBLOBS) return fail(VB200_EINVAL, "blobno");
-  cudaStream_t st = (cudaStream_t)stream;
+  if (!managed && (blobno < 0 || blobno >= VB200_PACKETBLOBS)) return fail(VB200_EINVAL, "blobno");
   const int ch = c->setup.channels;
   EncScratch S[2];
   vb200_phaseA_io a[2];
   vb200_block_desc *d_desc[2];
-  if ((rc = streams_front(c, nstreams, d, st, S, a, d_desc, nullptr, K, nsteps_env))) return rc;
+  MgdScratch M[2];
+  if ((rc = streams_front(c, nstreams, d, st, S, a, d_desc, managed ? M : nullptr, K, nsteps_env))) return rc;
   // 6. the rest of the chain per size
   for (int w = 0; w < 2; w++) {
     if (!d->count[w]) continue;
     const int nb = d->count[w], rows = nb * ch;
     if ((rc = phaseA_psy_launch(c, w, nb, &a[w], st, S[w].logfft, S[w].lmax, S[w].gmax))) return rc;
+    if (managed) {
+      if ((rc = managed_tail(c, w, nb, d->cap[w], d_desc[w], S[w].mdct, S[w].logmdct, S[w].logmask, M[w], d->posts[w],
+                             d->nonzero[w], d->iwork[w], st))) return rc;
+      continue;
+    }
     if ((rc = vb200_floor1_fit_dev(c, w, -1, rows, S[w].logmdct, S[w].logmask, d->posts[w], S[w].fitnz, st))) return rc;
     if ((rc = vb200_floor1_render_dev(c, w, -1, rows, d->posts[w], S[w].fitnz, d->iwork[w], d->nonzero[w], st))) return rc;
     CqnDev Q0, Q1;
@@ -2490,68 +2510,55 @@ static int encode_streams_launch(vb200_ctx *c, int nstreams, int blobno, vb200_s
 
 extern "C" int vb200_encode_streams_dev(vb200_ctx *c, int nstreams, int blobno, vb200_streams_io *d, void *stream) {
   CHECK_CTX(c);
-  return encode_streams_launch(c, nstreams, blobno, d, (cudaStream_t)stream, nullptr);
-}
-
-static int encode_streams_managed_launch(vb200_ctx *c, int nstreams, vb200_streams_io *d, cudaStream_t stream,
-                                         vb200_block_desc **desc_out, const CarryDev *K = nullptr, int nsteps_env = 0) {
-  int rc;
-  if ((rc = streams_check(c, nstreams, d)) || nstreams <= 0) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  EncScratch S[2];
-  vb200_phaseA_io a[2];
-  vb200_block_desc *d_desc[2];
-  MgdScratch M[2];
-  if ((rc = streams_front(c, nstreams, d, st, S, a, d_desc, M, K, nsteps_env))) return rc;
-  for (int w = 0; w < 2; w++) {
-    if (!d->count[w]) continue;
-    const int nb = d->count[w];
-    a[w].tap_noise = M[w].noise; a[w].tap_tone = M[w].tone;
-    if ((rc = phaseA_psy_launch(c, w, nb, &a[w], st, S[w].logfft, S[w].lmax, S[w].gmax))) return rc;
-    if ((rc = managed_tail(c, w, nb, d->cap[w], d_desc[w], S[w].mdct, S[w].logmdct, S[w].logmask, M[w], d->posts[w],
-                           d->nonzero[w], d->iwork[w], st))) return rc;
-  }
-  if (desc_out) { desc_out[0] = d_desc[0]; desc_out[1] = d_desc[1]; }
-  return scratch_end(c, st);
+  return encode_streams_launch(c, nstreams, blobno, false, d, (cudaStream_t)stream, nullptr);
 }
 
 extern "C" int vb200_encode_streams_managed_dev(vb200_ctx *c, int nstreams, vb200_streams_io *d, void *stream) {
   CHECK_CTX(c);
-  return encode_streams_managed_launch(c, nstreams, d, (cudaStream_t)stream, nullptr);
+  return encode_streams_launch(c, nstreams, 0, true, d, (cudaStream_t)stream, nullptr);
 }
 
-// host buffers of both streams calls: one synchronous H2D - compute - D2H round trip.  curves = 1: un-managed
-// (blob blobno); VB200_PACKETBLOBS: bitrate-managed, every output but ampmax_out holds the curves one after the
-// other, cap[W] blocks apart, and count[W] blocks of each come back.
-static int streams_host(vb200_ctx *c, int nstreams, int blobno, int curves, vb200_streams_io *h) {
+// A host vb200_streams_io staged through io into the device copy d: the inputs copied in (the pcm only when
+// stage_pcm, else h->pcm is already on the device), the plan and nblocks, and for each size with cap[w] > 0 the
+// outputs of cap[w] blocks, of every curve for managed.
+static int streams_stage(vb200_ctx *c, HostIO &io, int nstreams, bool managed, bool stage_pcm,
+                         const vb200_streams_io *h, vb200_streams_io *d) {
+  const size_t ch = c->setup.channels, curves = managed ? VB200_PACKETBLOBS : 1;
+  const size_t pcm_bytes = (size_t)nstreams * ch * (size_t)h->stream_stride * (h->pcm_fmt == VB200_PCM_S16_INTERLEAVED ? 2 : 4);
+  void *p;
   int rc;
-  if ((rc = plan_check(c))) return rc;
-  if (!h) return fail(VB200_EINVAL, "null io");
-  h->count[0] = h->count[1] = 0;
-  if (nstreams <= 0) return 0;
-  if (!h->pcm || !h->pcm_len || !h->plan || !h->nblocks || h->max_blocks < 1) return fail(VB200_EINVAL, "encode_streams: pcm, pcm_len, plan, nblocks");
+  *d = *h;
+  if (stage_pcm) { if ((rc = io.h2d(h->pcm, pcm_bytes, &p))) return rc; d->pcm = p; }
+  if ((rc = io.h2d(h->pcm_len, sizeof(int64_t) * nstreams, &p))) return rc; d->pcm_len = (const int64_t *)p;
+  if (h->eof) { if ((rc = io.h2d(h->eof, sizeof(int64_t) * nstreams, &p))) return rc; d->eof = (const int64_t *)p; }
+  if ((rc = io.h2d(nullptr, sizeof(vb200_stream_block) * nstreams * h->max_blocks, &p))) return rc; d->plan = (vb200_stream_block *)p;
+  if ((rc = io.h2d(nullptr, sizeof(int32_t) * nstreams, &p))) return rc; d->nblocks = (int32_t *)p;
+  for (int w = 0; w < 2; w++) {
+    if (h->cap[w] <= 0) continue;
+    const size_t cw = h->cap[w], n = c->dx[w].N / 2;
+    if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * cw * ch * VB200_FLOOR1_STRIDE, &p))) return rc; d->posts[w] = (int32_t *)p;
+    if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * cw * ch, &p))) return rc; d->nonzero[w] = (int32_t *)p;
+    if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * cw * ch * n, &p))) return rc; d->iwork[w] = (int32_t *)p;
+    if ((rc = io.h2d(nullptr, sizeof(float) * cw, &p))) return rc; d->ampmax_out[w] = (float *)p;
+  }
+  return 0;
+}
+
+// host buffers of both streams calls: one synchronous H2D - compute - D2H round trip.  managed: every output but
+// ampmax_out holds the VB200_PACKETBLOBS curves one after the other, cap[W] blocks apart, and count[W] blocks of each
+// come back.
+static int streams_host(vb200_ctx *c, int nstreams, int blobno, bool managed, vb200_streams_io *h) {
+  int rc;
+  if ((rc = streams_open(c, h)) || nstreams <= 0) return rc;
+  if ((rc = streams_inputs(h, "encode_streams"))) return rc;
   std::lock_guard<std::mutex> lk(c->mu);
   cudaStream_t st = c->s_main;
-  const size_t ch = c->setup.channels;
-  const size_t pcm_bytes = (size_t)nstreams * ch * (size_t)h->stream_stride * (h->pcm_fmt == VB200_PCM_S16_INTERLEAVED ? 2 : 4);
-  const size_t pcap = (size_t)nstreams * h->max_blocks;
+  const size_t ch = c->setup.channels, pcap = (size_t)nstreams * h->max_blocks;
+  const int curves = managed ? VB200_PACKETBLOBS : 1;
   HostIO io{c};
-  void *p;
-  vb200_streams_io d = *h;
-  if ((rc = io.h2d(h->pcm, pcm_bytes, &p))) return rc; d.pcm = p;
-  if ((rc = io.h2d(h->pcm_len, sizeof(int64_t) * nstreams, &p))) return rc; d.pcm_len = (const int64_t *)p;
-  if (h->eof) { if ((rc = io.h2d(h->eof, sizeof(int64_t) * nstreams, &p))) return rc; d.eof = (const int64_t *)p; }
-  if ((rc = io.h2d(nullptr, sizeof(vb200_stream_block) * pcap, &p))) return rc; d.plan = (vb200_stream_block *)p;
-  if ((rc = io.h2d(nullptr, sizeof(int32_t) * nstreams, &p))) return rc; d.nblocks = (int32_t *)p;
-  for (int w = 0; w < 2; w++) {
-    const size_t cw = h->cap[w] > 0 ? h->cap[w] : 0, n = c->dx[w].N / 2;
-    if (!cw) continue;
-    if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * cw * ch * VB200_FLOOR1_STRIDE, &p))) return rc; d.posts[w] = (int32_t *)p;
-    if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * cw * ch, &p))) return rc; d.nonzero[w] = (int32_t *)p;
-    if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * cw * ch * n, &p))) return rc; d.iwork[w] = (int32_t *)p;
-    if ((rc = io.h2d(nullptr, sizeof(float) * cw, &p))) return rc; d.ampmax_out[w] = (float *)p;
-  }
-  rc = curves == 1 ? vb200_encode_streams_dev(c, nstreams, blobno, &d, st) : vb200_encode_streams_managed_dev(c, nstreams, &d, st);
+  vb200_streams_io d;
+  if ((rc = streams_stage(c, io, nstreams, managed, true, h, &d))) return rc;
+  rc = encode_streams_launch(c, nstreams, blobno, managed, &d, st, nullptr);
   h->count[0] = d.count[0]; h->count[1] = d.count[1];
   if (rc) return rc;
   CU(cudaMemcpyAsync(h->plan, d.plan, sizeof(vb200_stream_block) * pcap, cudaMemcpyDeviceToHost, st));
@@ -2574,12 +2581,12 @@ static int streams_host(vb200_ctx *c, int nstreams, int blobno, int curves, vb20
 
 extern "C" int vb200_encode_streams(vb200_ctx *c, int nstreams, int blobno, vb200_streams_io *h) {
   CHECK_CTX(c);
-  return streams_host(c, nstreams, blobno, 1, h);
+  return streams_host(c, nstreams, blobno, false, h);
 }
 
 extern "C" int vb200_encode_streams_managed(vb200_ctx *c, int nstreams, vb200_streams_io *h) {
   CHECK_CTX(c);
-  return streams_host(c, nstreams, 0, VB200_PACKETBLOBS, h);
+  return streams_host(c, nstreams, 0, true, h);
 }
 
 // ======================================================================== //
@@ -3682,20 +3689,32 @@ static int encode_entropy_check(vb200_ctx *c, int nblocks) {
   return 0;
 }
 
+// both device entropy calls: checks, then encode_entropy_launch in the context scratch
+static int encode_entropy_dev(vb200_ctx *c, int W, int nblocks, bool managed, int64_t blob_blocks,
+                              const vb200_block_desc *d_desc, const int32_t *d_posts, const int32_t *d_nonzero,
+                              const int32_t *d_iwork, int64_t pkt_stride, int32_t *d_pkt_bits, uint8_t *d_data,
+                              cudaStream_t st) {
+  int rc;
+  if ((rc = encode_entropy_check(c, nblocks))) return rc;
+  if (managed) {
+    if (blob_blocks < nblocks) return fail(VB200_EINVAL, "blob_blocks < nblocks");
+    if ((int64_t)VB200_PACKETBLOBS * nblocks > INT32_MAX) return fail(VB200_EINVAL, "nblocks");
+  }
+  if (pkt_stride % 4 || pkt_stride < c->eent.bound[W]) return fail(VB200_EINVAL, "pkt_stride: a multiple of 4, >= the packet bound");
+  if (nblocks == 0) return 0;
+  if (!d_desc || !d_posts || !d_nonzero || !d_iwork || !d_pkt_bits || !d_data) return fail(VB200_EINVAL, "encode_entropy pointers");
+  if ((rc = scratch_begin(c, st))) return rc;
+  if ((rc = encode_entropy_launch(c, W, nblocks, d_desc, d_posts, d_nonzero, d_iwork, pkt_stride, d_pkt_bits, d_data, st,
+                                  managed, blob_blocks))) return rc;
+  return scratch_end(c, st);
+}
+
 extern "C" int vb200_encode_entropy_dev(vb200_ctx *c, int W, int nblocks, const vb200_block_desc *d_desc,
                                         const int32_t *d_posts, const int32_t *d_nonzero, const int32_t *d_iwork,
                                         int64_t pkt_stride, int32_t *d_pkt_bits, uint8_t *d_data, void *stream) {
   CHECK_CTX(c); CHECK_W(W);
-  int rc;
-  if ((rc = encode_entropy_check(c, nblocks))) return rc;
-  if (pkt_stride % 4 || pkt_stride < c->eent.bound[W]) return fail(VB200_EINVAL, "pkt_stride: a multiple of 4, >= the packet bound");
-  if (nblocks == 0) return 0;
-  if (!d_desc || !d_posts || !d_nonzero || !d_iwork || !d_pkt_bits || !d_data) return fail(VB200_EINVAL, "encode_entropy pointers");
-  cudaStream_t st = (cudaStream_t)stream;
-  if ((rc = scratch_begin(c, st))) return rc;
-  if ((rc = encode_entropy_launch(c, W, nblocks, d_desc, d_posts, d_nonzero, d_iwork, pkt_stride, d_pkt_bits, d_data, st)))
-    return rc;
-  return scratch_end(c, st);
+  return encode_entropy_dev(c, W, nblocks, false, 0, d_desc, d_posts, d_nonzero, d_iwork, pkt_stride, d_pkt_bits,
+                            d_data, (cudaStream_t)stream);
 }
 
 // host forms: packets of the strided device buffer packed back to back, then the counts, offsets and bytes copied
@@ -3751,39 +3770,55 @@ extern "C" int vb200_encode_entropy(vb200_ctx *c, int W, int nblocks, const vb20
                           data_cap, c->s_main);
 }
 
-extern "C" int vb200_encode_packets(vb200_ctx *c, int W, int nstreams, int bps, int blobno, const vb200_encode_io *h,
-                                    int64_t *pkt_off, int32_t *pkt_bits, uint8_t *data, int64_t data_cap) {
-  CHECK_CTX(c); CHECK_W(W);
+// Both block packet calls: the chain into staged outputs, the entropy coder, the packets packed back to back.
+// managed: all VB200_PACKETBLOBS packets of every block.  name: the call, for the messages.
+static int encode_packets(vb200_ctx *c, int W, int nstreams, int bps, int blobno, bool managed, const char *name,
+                          const vb200_encode_io *h, int64_t *pkt_off, int32_t *pkt_bits, uint8_t *data,
+                          int64_t data_cap) {
   int rc;
   if (!c->eent.books) return fail(VB200_EINVAL, "no vb200_encode_entropy_setup registered");
   if (!h || h->posts || h->nonzero || h->iwork || h->classes || h->overflow || h->mdct || h->logmdct || h->logmask ||
       h->iwork_fmt != VB200_IWORK_S32)
-    return fail(VB200_EINVAL, "encode_packets: posts / nonzero / iwork / classes / overflow / spectra must be NULL");
-  if (!pkt_off || !pkt_bits || (!data && data_cap > 0) || data_cap < 0) return fail(VB200_EINVAL, "encode_packets outputs");
-  vb200_encode_io d = *h;
-  int32_t one = 0;                                   // enc_check wants the outputs it does not see here
-  d.posts = d.nonzero = &one; d.iwork = &one;
-  if ((rc = enc_check(c, W, nstreams, bps, blobno, &d))) return rc;
+    return fail(VB200_EINVAL, (std::string(name) + ": posts / nonzero / iwork / classes / overflow / spectra must be NULL").c_str());
+  if (!pkt_off || !pkt_bits || (!data && data_cap > 0) || data_cap < 0)
+    return fail(VB200_EINVAL, (std::string(name) + " outputs").c_str());
+  if (managed) {
+    if ((rc = managed_check(c, W, nstreams, bps, h, true))) return rc;
+    if ((int64_t)VB200_PACKETBLOBS * nstreams * bps > INT32_MAX) return fail(VB200_EINVAL, "nblocks");
+  } else if ((rc = enc_check(c, W, nstreams, bps, blobno, h, true))) {
+    return rc;
+  }
   std::lock_guard<std::mutex> lk(c->mu);
-  const int ch = c->setup.channels, N = c->dx[W].N, n = N / 2;
-  const size_t nb = (size_t)nstreams * bps, rows = nb * ch;
+  const int ch = c->setup.channels, N = c->dx[W].N, curves = managed ? VB200_PACKETBLOBS : 1;
+  const size_t n = N / 2, nb = (size_t)nstreams * bps, rows = nb * ch;
   const int64_t stride = c->eent.bound[W];
   cudaStream_t st = c->s_main;
   HostIO io{c};
+  vb200_encode_io d = *h;
   void *dbits, *dstr;
-  if ((rc = enc_stage(io, h, &d, ch, N, nstreams, bps, 1))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(int32_t) * nb, &dbits))) return rc;
-  if ((rc = io.h2d(nullptr, (size_t)stride * nb, &dstr))) return rc;
+  if ((rc = enc_stage(io, h, &d, ch, N, nstreams, bps, curves))) return rc;
+  if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * nb, &dbits))) return rc;
+  if ((rc = io.h2d(nullptr, (size_t)stride * curves * nb, &dstr))) return rc;
   EncScratch S;
-  if ((rc = carve(c->enc, [&](Carve &k) { enc_layout(k, rows, nb, n, nullptr, false, &S); }))) return rc;
+  MgdScratch M;
+  if ((rc = carve(managed ? c->mgd : c->enc, [&](Carve &k) {
+         enc_layout(k, rows, nb, n, nullptr, false, &S);
+         if (managed) mgd_layout(k, rows, rows, n, &M);
+       }))) return rc;
   if ((rc = scratch_begin(c, st))) return rc;
-  if ((rc = encode_launch(c, W, nstreams, bps, blobno, &d, S, st))) return rc;
+  if ((rc = encode_launch(c, W, nstreams, bps, blobno, &d, S, st, managed ? &M : nullptr))) return rc;
   if ((rc = encode_entropy_launch(c, W, (int)nb, d.desc, d.posts, d.nonzero, (const int32_t *)d.iwork, stride,
-                                  (int32_t *)dbits, (uint8_t *)dstr, st))) return rc;
+                                  (int32_t *)dbits, (uint8_t *)dstr, st, managed, managed ? (long long)nb : 0))) return rc;
   if ((rc = scratch_end(c, st))) return rc;
   if ((rc = io.d2h(h->ampmax_out, d.ampmax_out, sizeof(float) * nb))) return rc;
-  return packets_pack_d2h(c, (int)nb, (const uint8_t *)dstr, stride, (const int32_t *)dbits, pkt_off, pkt_bits, data,
-                          data_cap, st);
+  return packets_pack_d2h(c, curves * (int)nb, (const uint8_t *)dstr, stride, (const int32_t *)dbits, pkt_off, pkt_bits,
+                          data, data_cap, st);
+}
+
+extern "C" int vb200_encode_packets(vb200_ctx *c, int W, int nstreams, int bps, int blobno, const vb200_encode_io *h,
+                                    int64_t *pkt_off, int32_t *pkt_bits, uint8_t *data, int64_t data_cap) {
+  CHECK_CTX(c); CHECK_W(W);
+  return encode_packets(c, W, nstreams, bps, blobno, false, "encode_packets", h, pkt_off, pkt_bits, data, data_cap);
 }
 
 // ---- bitrate-managed: all VB200_PACKETBLOBS packets of every block ----
@@ -3792,52 +3827,15 @@ extern "C" int vb200_encode_entropy_managed_dev(vb200_ctx *c, int W, int nblocks
                                                 const int32_t *d_nonzero, const int32_t *d_iwork, int64_t pkt_stride,
                                                 int32_t *d_pkt_bits, uint8_t *d_data, void *stream) {
   CHECK_CTX(c); CHECK_W(W);
-  int rc;
-  if ((rc = encode_entropy_check(c, nblocks))) return rc;
-  if (blob_blocks < nblocks) return fail(VB200_EINVAL, "blob_blocks < nblocks");
-  if ((int64_t)VB200_PACKETBLOBS * nblocks > INT32_MAX) return fail(VB200_EINVAL, "nblocks");
-  if (pkt_stride % 4 || pkt_stride < c->eent.bound[W]) return fail(VB200_EINVAL, "pkt_stride: a multiple of 4, >= the packet bound");
-  if (nblocks == 0) return 0;
-  if (!d_desc || !d_posts || !d_nonzero || !d_iwork || !d_pkt_bits || !d_data) return fail(VB200_EINVAL, "encode_entropy pointers");
-  cudaStream_t st = (cudaStream_t)stream;
-  if ((rc = scratch_begin(c, st))) return rc;
-  if ((rc = encode_entropy_launch(c, W, nblocks, d_desc, d_posts, d_nonzero, d_iwork, pkt_stride, d_pkt_bits, d_data, st,
-                                  true, blob_blocks))) return rc;
-  return scratch_end(c, st);
+  return encode_entropy_dev(c, W, nblocks, true, blob_blocks, d_desc, d_posts, d_nonzero, d_iwork, pkt_stride,
+                            d_pkt_bits, d_data, (cudaStream_t)stream);
 }
 
 extern "C" int vb200_encode_packets_managed(vb200_ctx *c, int W, int nstreams, int bps, const vb200_encode_io *h,
                                             int64_t *pkt_off, int32_t *pkt_bits, uint8_t *data, int64_t data_cap) {
   CHECK_CTX(c); CHECK_W(W);
-  int rc;
-  if (!c->eent.books) return fail(VB200_EINVAL, "no vb200_encode_entropy_setup registered");
-  if (!h || h->posts || h->nonzero || h->iwork || h->classes || h->overflow || h->mdct || h->logmdct || h->logmask ||
-      h->iwork_fmt != VB200_IWORK_S32)
-    return fail(VB200_EINVAL, "encode_packets_managed: posts / nonzero / iwork / classes / overflow / spectra must be NULL");
-  if (!pkt_off || !pkt_bits || (!data && data_cap > 0) || data_cap < 0) return fail(VB200_EINVAL, "encode_packets_managed outputs");
-  vb200_encode_io d = *h;
-  int32_t one = 0;                                   // managed_check wants the outputs it does not see here
-  d.posts = d.nonzero = &one; d.iwork = &one;
-  if ((rc = managed_check(c, W, nstreams, bps, &d))) return rc;
-  if ((int64_t)VB200_PACKETBLOBS * nstreams * bps > INT32_MAX) return fail(VB200_EINVAL, "nblocks");
-  std::lock_guard<std::mutex> lk(c->mu);
-  constexpr int NB = VB200_PACKETBLOBS;
-  const int ch = c->setup.channels, N = c->dx[W].N;
-  const size_t nb = (size_t)nstreams * bps;
-  const int64_t stride = c->eent.bound[W];
-  cudaStream_t st = c->s_main;
-  HostIO io{c};
-  void *dbits, *dstr;
-  if ((rc = enc_stage(io, h, &d, ch, N, nstreams, bps, NB))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(int32_t) * NB * nb, &dbits))) return rc;
-  if ((rc = io.h2d(nullptr, (size_t)stride * NB * nb, &dstr))) return rc;
-  if ((rc = vb200_encode_dsp_managed_dev(c, W, nstreams, bps, &d, st))) return rc;
-  if ((rc = vb200_encode_entropy_managed_dev(c, W, (int)nb, (int64_t)nb, d.desc, d.posts, d.nonzero,
-                                             (const int32_t *)d.iwork, stride, (int32_t *)dbits, (uint8_t *)dstr, st)))
-    return rc;
-  if ((rc = io.d2h(h->ampmax_out, d.ampmax_out, sizeof(float) * nb))) return rc;
-  return packets_pack_d2h(c, NB * (int)nb, (const uint8_t *)dstr, stride, (const int32_t *)dbits, pkt_off, pkt_bits,
-                          data, data_cap, st);
+  return encode_packets(c, W, nstreams, bps, VB200_PACKETBLOBS / 2, true, "encode_packets_managed", h, pkt_off,
+                        pkt_bits, data, data_cap);
 }
 
 // ======================================================================== //
@@ -4064,14 +4062,12 @@ static int streams_packets(vb200_ctx *c, int nstreams, int blobno, bool managed,
                            vb200_packet_info *info, uint8_t *data, int64_t data_cap, void *carry = nullptr,
                            HostIO *staged = nullptr) {
   int rc;
-  if ((rc = plan_check(c))) return rc;
-  if (!h) return fail(VB200_EINVAL, "null io");
-  h->count[0] = h->count[1] = 0;
+  if ((rc = streams_open(c, h))) return rc;
   if (!c->eent.books) return fail(VB200_EINVAL, "no vb200_encode_entropy_setup registered");
   if (managed && (rc = bitrate_check(c))) return rc;
   if (!managed && (blobno < 0 || blobno >= VB200_PACKETBLOBS)) return fail(VB200_EINVAL, "blobno");
   if (nstreams <= 0) return 0;
-  if (!h->pcm || !h->pcm_len || !h->plan || !h->nblocks || h->max_blocks < 1) return fail(VB200_EINVAL, "encode_streams_packets: pcm, pcm_len, plan, nblocks");
+  if ((rc = streams_inputs(h, "encode_streams_packets"))) return rc;
   for (int w = 0; w < 2; w++) {
     if (h->posts[w] || h->nonzero[w] || h->iwork[w] || h->ampmax_out[w])
       return fail(VB200_EINVAL, "encode_streams_packets: posts / nonzero / iwork / ampmax_out must be NULL");
@@ -4087,26 +4083,12 @@ static int streams_packets(vb200_ctx *c, int nstreams, int blobno, bool managed,
   if (!staged) lk.lock();
   cudaStream_t st = c->s_main;
   const int curves = managed ? VB200_PACKETBLOBS : 1;
-  const size_t ch = c->setup.channels;
-  const size_t pcm_bytes = (size_t)nstreams * ch * (size_t)h->stream_stride * (h->pcm_fmt == VB200_PCM_S16_INTERLEAVED ? 2 : 4);
   const size_t n = (size_t)nstreams * h->max_blocks;
   HostIO own{c};
   HostIO &io = staged ? *staged : own;
   void *p;
-  vb200_streams_io d = *h;
-  if (!staged) { if ((rc = io.h2d(h->pcm, pcm_bytes, &p))) return rc; d.pcm = p; }
-  if ((rc = io.h2d(h->pcm_len, sizeof(int64_t) * nstreams, &p))) return rc; d.pcm_len = (const int64_t *)p;
-  if (h->eof) { if ((rc = io.h2d(h->eof, sizeof(int64_t) * nstreams, &p))) return rc; d.eof = (const int64_t *)p; }
-  if ((rc = io.h2d(nullptr, sizeof(vb200_stream_block) * n, &p))) return rc; d.plan = (vb200_stream_block *)p;
-  if ((rc = io.h2d(nullptr, sizeof(int32_t) * nstreams, &p))) return rc; d.nblocks = (int32_t *)p;
-  for (int w = 0; w < 2; w++) {
-    const size_t cw = h->cap[w], nn = c->dx[w].N / 2;
-    if (!cw) continue;
-    if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * cw * ch * VB200_FLOOR1_STRIDE, &p))) return rc; d.posts[w] = (int32_t *)p;
-    if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * cw * ch, &p))) return rc; d.nonzero[w] = (int32_t *)p;
-    if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * cw * ch * nn, &p))) return rc; d.iwork[w] = (int32_t *)p;
-    if ((rc = io.h2d(nullptr, sizeof(float) * cw, &p))) return rc; d.ampmax_out[w] = (float *)p;
-  }
+  vb200_streams_io d;
+  if ((rc = streams_stage(c, io, nstreams, managed, !staged, h, &d))) return rc;
   CarryDev K{}, *Kp = nullptr;
   char *dblob = nullptr;
   if (carry) {
@@ -4118,8 +4100,7 @@ static int streams_packets(vb200_ctx *c, int nstreams, int blobno, bool managed,
     Kp = &K;
   }
   vb200_block_desc *desc[2] = {nullptr, nullptr};
-  rc = managed ? encode_streams_managed_launch(c, nstreams, &d, st, desc, Kp, nsteps_env)
-               : encode_streams_launch(c, nstreams, blobno, &d, st, desc, Kp, nsteps_env);
+  rc = encode_streams_launch(c, nstreams, blobno, managed, &d, st, desc, Kp, nsteps_env);
   h->count[0] = d.count[0]; h->count[1] = d.count[1];
   if (rc) return rc;
   int32_t *bits[2] = {nullptr, nullptr}, *Wb, *sbits, *fbits, *choice = nullptr;
@@ -4141,11 +4122,8 @@ static int streams_packets(vb200_ctx *c, int nstreams, int blobno, bool managed,
   for (int w = 0; w < 2; w++) {
     const int cnt = d.count[w];
     if (!cnt) continue;
-    rc = managed ? vb200_encode_entropy_managed_dev(c, w, cnt, d.cap[w], desc[w], d.posts[w], d.nonzero[w], d.iwork[w],
-                                                    c->eent.bound[w], bits[w], strided[w], st)
-                 : vb200_encode_entropy_dev(c, w, cnt, desc[w], d.posts[w], d.nonzero[w], d.iwork[w], c->eent.bound[w],
-                                            bits[w], strided[w], st);
-    if (rc) return rc;
+    if ((rc = encode_entropy_dev(c, w, cnt, managed, managed ? d.cap[w] : 0, desc[w], d.posts[w], d.nonzero[w],
+                                 d.iwork[w], c->eent.bound[w], bits[w], strided[w], st))) return rc;
   }
   k_stream_bits<<<grid_for(c, (int)((n + 255) / 256), 8), 256, 0, st>>>(nstreams, h->max_blocks, d.plan, d.nblocks, curves,
                                                                         bits[0], bits[1], d.count[0], d.count[1], Wb,

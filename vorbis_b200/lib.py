@@ -449,7 +449,9 @@ class Context:
         posts / nonzero / iwork shaped [15][count][ch][...] (curve k = blob k); ampmax_out [count]."""
         return self._encode_streams(pcm, pcm_len, eof, fmt, max_blocks, cap, 0, abi.PACKETBLOBS)
 
-    def _encode_streams(self, pcm, pcm_len, eof, fmt, max_blocks, cap, blobno, curves):
+    def _streams_io(self, pcm, pcm_len, eof, fmt, max_blocks, cap):
+        """the inputs of the whole-stream encode calls as an abi.StreamsIO, max_blocks and cap defaulting to what the
+        timelines can hold: (io, plan, nblocks, the arrays io points into, to be kept alive until the call returns)"""
         ch = self.channels
         if fmt == PCM_F32_PLANAR:
             pcm = np.ascontiguousarray(pcm, np.float32)
@@ -472,16 +474,22 @@ class Context:
         plan = np.zeros((ns, max_blocks), abi.STREAM_BLOCK_DTYPE)
         nb = np.zeros(ns, np.int32)
         io.plan, io.nblocks = plan.ctypes.data, nb.ctypes.data
+        io.cap[0], io.cap[1] = int(cap[0]), int(cap[1])
+        return io, plan, nb, (pcm, pcm_len, eofp)
+
+    def _encode_streams(self, pcm, pcm_len, eof, fmt, max_blocks, cap, blobno, curves):
+        ch = self.channels
+        io, plan, nb, keep = self._streams_io(pcm, pcm_len, eof, fmt, max_blocks, cap)
         out = {}
         lead = () if curves is None else (curves,)
         for w in range(2):
-            n = self.bs[w] // 2
-            io.cap[w] = int(cap[w])
-            out[w] = {"posts": np.zeros(lead + (cap[w], ch, abi.FLOOR1_STRIDE), np.int32),
-                      "nonzero": np.zeros(lead + (cap[w], ch), np.int32),
-                      "iwork": np.zeros(lead + (cap[w], ch, n), np.int32), "ampmax_out": np.zeros(cap[w], np.float32)}
+            n, cw = self.bs[w] // 2, io.cap[w]
+            out[w] = {"posts": np.zeros(lead + (cw, ch, abi.FLOOR1_STRIDE), np.int32),
+                      "nonzero": np.zeros(lead + (cw, ch), np.int32),
+                      "iwork": np.zeros(lead + (cw, ch, n), np.int32), "ampmax_out": np.zeros(cw, np.float32)}
             io.posts[w], io.nonzero[w] = out[w]["posts"].ctypes.data, out[w]["nonzero"].ctypes.data
             io.iwork[w], io.ampmax_out[w] = out[w]["iwork"].ctypes.data, out[w]["ampmax_out"].ctypes.data
+        ns = plan.shape[0]
         if curves is None:
             self._chk(self.L.vb200_encode_streams(self.h, ns, blobno, C.byref(io)))
         else:
@@ -492,13 +500,10 @@ class Context:
         return {"plan": plan, "nblocks": nb, "count": [io.count[0], io.count[1]], 0: out[0], 1: out[1]}
 
     # ---- whole per-block encode DSP (Phase A -> floor1 -> Phase B) in one call ---------------
-    def encode_dsp(self, W, pcm, desc, nstreams=None, fmt=0, hop=0, ampmax0=None, independent=None, blobno=7,
-                   floats=False, iwork_s16=False, classes=False):
-        """Host buffers.  fmt 0: pcm [nblocks][ch][N] float; PCM_F32_PLANAR: [streams][ch][stride] float;
-        PCM_S16_INTERLEAVED: [streams][stride][ch] int16.  nstreams None = every block its own stream.
-        independent None = True when the blocks are not grouped in streams."""
+    def _encode_io(self, W, pcm, desc, nstreams, fmt, hop, ampmax0, independent):
+        """the inputs of the block-level encode calls as an abi.EncodeIO: (io, nstreams, blocks per stream, the arrays
+        io points into, to be kept alive until the call returns)"""
         ch, N = self.channels, self.bs[W]
-        n = N // 2
         desc = np.ascontiguousarray(desc, abi.BLOCKDESC_DTYPE)
         nb = desc.shape[0]
         if nstreams is None:
@@ -524,6 +529,16 @@ class Context:
         if ampmax0 is not None:
             ampmax0 = np.ascontiguousarray(ampmax0, np.float32)
             io.ampmax0 = ampmax0.ctypes.data
+        return io, nstreams, bps, (pcm, desc, ampmax0)
+
+    def encode_dsp(self, W, pcm, desc, nstreams=None, fmt=0, hop=0, ampmax0=None, independent=None, blobno=7,
+                   floats=False, iwork_s16=False, classes=False):
+        """Host buffers.  fmt 0: pcm [nblocks][ch][N] float; PCM_F32_PLANAR: [streams][ch][stride] float;
+        PCM_S16_INTERLEAVED: [streams][stride][ch] int16.  nstreams None = every block its own stream.
+        independent None = True when the blocks are not grouped in streams."""
+        ch, n = self.channels, self.bs[W] // 2
+        io, nstreams, bps, keep = self._encode_io(W, pcm, desc, nstreams, fmt, hop, ampmax0, independent)
+        nb = nstreams * bps
         out = {"posts": np.zeros((nb, ch, abi.FLOOR1_STRIDE), np.int32), "nonzero": np.zeros((nb, ch), np.int32),
                "iwork": np.zeros((nb, ch, n), np.int16 if iwork_s16 else np.int32),
                "ampmax_out": np.zeros(nb, np.float32)}
@@ -544,33 +559,9 @@ class Context:
     def encode_dsp_managed(self, W, pcm, desc, nstreams=None, fmt=0, hop=0, ampmax0=None, independent=None):
         """Bitrate-managed mode (vb200_encode_dsp_managed): the 15 curves of every block.  Inputs as encode_dsp;
         returns posts [15][nb][ch][FLOOR1_STRIDE], nonzero [15][nb][ch], iwork [15][nb][ch][n], ampmax_out [nb]."""
-        ch, N = self.channels, self.bs[W]
-        n = N // 2
-        desc = np.ascontiguousarray(desc, abi.BLOCKDESC_DTYPE)
-        nb = desc.shape[0]
-        if nstreams is None:
-            nstreams = nb
-            if independent is None:
-                independent = True
-        bps = nb // nstreams
-        assert bps * nstreams == nb
-        io = abi.EncodeIO()
-        if fmt == 0:
-            pcm = np.ascontiguousarray(pcm, np.float32).reshape(nb, ch, N)
-        elif fmt == PCM_F32_PLANAR:
-            pcm = np.ascontiguousarray(pcm, np.float32)
-            assert pcm.shape[:2] == (nstreams, ch)
-            io.stream_stride = pcm.shape[2]
-        else:
-            pcm = np.ascontiguousarray(pcm, np.int16)
-            assert pcm.shape[0] == nstreams and pcm.shape[2] == ch
-            io.stream_stride = pcm.shape[1]
-        io.pcm, io.pcm_fmt, io.hop = pcm.ctypes.data, fmt, hop
-        io.desc = desc.ctypes.data
-        io.independent = 1 if independent else 0
-        if ampmax0 is not None:
-            ampmax0 = np.ascontiguousarray(ampmax0, np.float32)
-            io.ampmax0 = ampmax0.ctypes.data
+        ch, n = self.channels, self.bs[W] // 2
+        io, nstreams, bps, keep = self._encode_io(W, pcm, desc, nstreams, fmt, hop, ampmax0, independent)
+        nb = nstreams * bps
         NB = abi.PACKETBLOBS
         out = {"posts": np.full((NB, nb, ch, abi.FLOOR1_STRIDE), -1, np.int32), "nonzero": np.full((NB, nb, ch), -1, np.int32),
                "iwork": np.full((NB, nb, ch, n), -1, np.int32), "ampmax_out": np.zeros(nb, np.float32)}
@@ -860,33 +851,14 @@ class Context:
                        data_cap=None):
         """vb200_encode_packets: PCM as for encode_dsp in, {"packets", "pkt_bits", "pkt_off", "data", "ampmax_out"}
         out"""
-        ch, N = self.channels, self.bs[W]
-        desc = np.ascontiguousarray(desc, abi.BLOCKDESC_DTYPE)
-        nb = desc.shape[0]
-        if nstreams is None:
-            nstreams = nb
-            if independent is None:
-                independent = True
-        io = abi.EncodeIO()
-        if fmt == 0:
-            pcm = np.ascontiguousarray(pcm, np.float32).reshape(nb, ch, N)
-        elif fmt == PCM_F32_PLANAR:
-            pcm = np.ascontiguousarray(pcm, np.float32)
-            io.stream_stride = pcm.shape[2]
-        else:
-            pcm = np.ascontiguousarray(pcm, np.int16)
-            io.stream_stride = pcm.shape[1]
-        io.pcm, io.pcm_fmt, io.hop, io.desc = pcm.ctypes.data, fmt, hop, desc.ctypes.data
-        io.independent = 1 if independent else 0
-        if ampmax0 is not None:
-            ampmax0 = np.ascontiguousarray(ampmax0, np.float32)
-            io.ampmax0 = ampmax0.ctypes.data
+        io, nstreams, bps, keep = self._encode_io(W, pcm, desc, nstreams, fmt, hop, ampmax0, independent)
+        nb = nstreams * bps
         cap = nb * self.packet_bound(W) if data_cap is None else data_cap
         out = {"pkt_off": np.zeros(nb, np.int64), "pkt_bits": np.zeros(nb, np.int32),
                "data": np.zeros(max(cap, 1), np.uint8), "ampmax_out": np.zeros(nb, np.float32)}
         io.ampmax_out = out["ampmax_out"].ctypes.data
-        self._chk(self.L.vb200_encode_packets(self.h, W, nstreams, nb // nstreams, blobno, C.byref(io),
-                                              _ptr(out["pkt_off"]), _ptr(out["pkt_bits"]), _ptr(out["data"]), cap))
+        self._chk(self.L.vb200_encode_packets(self.h, W, nstreams, bps, blobno, C.byref(io), _ptr(out["pkt_off"]),
+                                              _ptr(out["pkt_bits"]), _ptr(out["data"]), cap))
         return self._packets(out, nb)
 
     def encode_entropy_managed_dev(self, W, nblocks, blob_blocks, d_desc, d_posts, d_nonzero, d_iwork, pkt_stride,
@@ -905,33 +877,14 @@ class Context:
         """vb200_encode_packets_managed: PCM as for encode_dsp_managed in; {"packets": [15][nb] bytes, "pkt_bits"
         [15][nb], "pkt_off" [15][nb], "data", "ampmax_out"} out (and "rc" when check is False, in which case an error
         does not raise and "packets" is absent)"""
-        ch, N = self.channels, self.bs[W]
         NB = abi.PACKETBLOBS
-        desc = np.ascontiguousarray(desc, abi.BLOCKDESC_DTYPE)
-        nb = desc.shape[0]
-        if nstreams is None:
-            nstreams = nb
-            if independent is None:
-                independent = True
-        io = abi.EncodeIO()
-        if fmt == 0:
-            pcm = np.ascontiguousarray(pcm, np.float32).reshape(nb, ch, N)
-        elif fmt == PCM_F32_PLANAR:
-            pcm = np.ascontiguousarray(pcm, np.float32)
-            io.stream_stride = pcm.shape[2]
-        else:
-            pcm = np.ascontiguousarray(pcm, np.int16)
-            io.stream_stride = pcm.shape[1]
-        io.pcm, io.pcm_fmt, io.hop, io.desc = pcm.ctypes.data, fmt, hop, desc.ctypes.data
-        io.independent = 1 if independent else 0
-        if ampmax0 is not None:
-            ampmax0 = np.ascontiguousarray(ampmax0, np.float32)
-            io.ampmax0 = ampmax0.ctypes.data
+        io, nstreams, bps, keep = self._encode_io(W, pcm, desc, nstreams, fmt, hop, ampmax0, independent)
+        nb = nstreams * bps
         cap = NB * nb * self.packet_bound(W) if data_cap is None else data_cap
         out = {"pkt_off": np.zeros((NB, nb), np.int64), "pkt_bits": np.zeros((NB, nb), np.int32),
                "data": np.zeros(max(cap, 1), np.uint8), "ampmax_out": np.zeros(nb, np.float32)}
         io.ampmax_out = out["ampmax_out"].ctypes.data
-        rc = self.L.vb200_encode_packets_managed(self.h, W, nstreams, nb // nstreams, C.byref(io), _ptr(out["pkt_off"]),
+        rc = self.L.vb200_encode_packets_managed(self.h, W, nstreams, bps, C.byref(io), _ptr(out["pkt_off"]),
                                                  _ptr(out["pkt_bits"]), _ptr(out["data"]), cap)
         if not check:
             out["rc"] = rc
@@ -1005,29 +958,8 @@ class Context:
         """vb200_encode_streams_packets[_managed] on timeline buffers as for encode_streams: {"plan", "nblocks",
         "count", "info" (PACKET_INFO_DTYPE [ns][max_blocks]), "data", "packets": per stream [bytes]} (and "rc" when
         check is False, in which case an error does not raise and "packets" is absent).  carry: the _resume forms"""
-        ch = self.channels
-        if fmt == PCM_F32_PLANAR:
-            pcm = np.ascontiguousarray(pcm, np.float32)
-            ns, stride = pcm.shape[0], pcm.shape[2]
-            assert pcm.shape[1] == ch
-        else:
-            pcm = np.ascontiguousarray(pcm, np.int16)
-            ns, stride = pcm.shape[0], pcm.shape[1]
-            assert pcm.shape[2] == ch
-        pcm_len = np.ascontiguousarray(pcm_len, np.int64)
-        eofp = None if eof is None else np.ascontiguousarray(eof, np.int64)
-        if max_blocks is None:
-            max_blocks = stride // (self.bs[0] // 2) + 8
-        if cap is None:
-            cap = [ns * max_blocks, ns * (stride // (self.bs[1] // 2) + 8)]
-        io = abi.StreamsIO()
-        io.pcm, io.pcm_fmt, io.max_blocks, io.stream_stride = pcm.ctypes.data, fmt, max_blocks, stride
-        io.pcm_len = pcm_len.ctypes.data
-        io.eof = None if eofp is None else eofp.ctypes.data
-        plan = np.zeros((ns, max_blocks), abi.STREAM_BLOCK_DTYPE)
-        nb = np.zeros(ns, np.int32)
-        io.plan, io.nblocks = plan.ctypes.data, nb.ctypes.data
-        io.cap[0], io.cap[1] = int(cap[0]), int(cap[1])
+        io, plan, nb, keep = self._streams_io(pcm, pcm_len, eof, fmt, max_blocks, cap)
+        ns, max_blocks = plan.shape
         info = np.zeros((ns, max_blocks), abi.PACKET_INFO_DTYPE)
         if data_cap is None:
             data_cap = ns * max_blocks * max(self.packet_bound(0), self.packet_bound(1))
@@ -1044,13 +976,18 @@ class Context:
             rc = self.L.vb200_encode_streams_packets_managed(self.h, ns, C.byref(io), _ptr(info), _ptr(data), data_cap)
         else:
             rc = self.L.vb200_encode_streams_packets(self.h, ns, blobno, C.byref(io), _ptr(info), _ptr(data), data_cap)
+        return self._stream_packets(rc, check, io, plan, nb, info, data)
+
+    def _stream_packets(self, rc, check, io, plan, nb, info, data):
+        """the result of the calls that write stream-ordered packets: stream i's packets split out of data by its
+        first nb[i] info records ("rc" in place of "packets" when check is False)"""
         out = {"plan": plan, "nblocks": nb, "count": [io.count[0], io.count[1]], "info": info, "data": data}
         if not check:
             out["rc"] = rc
             return out
         self._chk(rc)
         out["packets"] = [[bytes(data[r["offset"]:r["offset"] + r["bytes"]]) for r in info[i, :nb[i]]]
-                          for i in range(ns)]
+                          for i in range(len(nb))]
         return out
 
     def encode_pcm_carry_init(self, nstreams, mark_steps=0):
@@ -1109,14 +1046,7 @@ class Context:
         else:
             rc = self.L.vb200_encode_pcm_packets(self.h, ns, blobno, C.byref(io), _ptr(carry), _ptr(info), _ptr(data),
                                                  data_cap)
-        out = {"plan": plan, "nblocks": nb, "count": [io.count[0], io.count[1]], "info": info, "data": data}
-        if not check:
-            out["rc"] = rc
-            return out
-        self._chk(rc)
-        out["packets"] = [[bytes(data[r["offset"]:r["offset"] + r["bytes"]]) for r in info[i, :nb[i]]]
-                          for i in range(ns)]
-        return out
+        return self._stream_packets(rc, check, io, plan, nb, info, data)
 
     def lpc_extrapolate(self, data, n, order, count, check=True):
         """vb200_lpc_extrapolate: data float32 [rows][stride], n [rows]; returns (coeff float32 [rows][order], out
