@@ -1,12 +1,12 @@
-"""The bitrate manager and whole streams' packets for the tests: build recipes and ctypes loaders of
+"""The bitrate manager and whole streams' packets for the tests: ctypes loaders of
   oracle/libvb_oracle_bitrate.so             the CPU oracle's restatement of vorbis_bitrate_addblock
                                              (vb_oracle_bitrate.c); builds anywhere gcc exists
   oracle/_ref/libvorbis_ref_bitrate.so       ref_bitrate.c + the stock reference objects: ref_bitrate_info,
                                              ref_bitrate_replay and ref_stream_capture
   oracle/_ref/libvorbis_dropin_bitrate.so    the same file + the managed multi-stream driver: a device context with
                                              the setup and entropy setup of a managed encoder
-The two reference libraries link the objects oracle/Makefile compiles from the unmodified reference sources and are
-only built where those exist; like the rest of oracle/_ref they travel.
+oracle/Makefile builds all three; the two reference libraries only where the reference sources exist, and like the
+rest of oracle/_ref they travel.
 
 TEST INFRASTRUCTURE ONLY: imported by tests/, tools/ and tests/golden/make_golden_bitrate.py, never by the product.
 """
@@ -16,44 +16,14 @@ import subprocess
 
 import numpy as np
 
-from oracle.halfrate import DROPIN_OBJS, OBJ, PARITY, REF_OBJS, REF_SRC, _stale
 from vorbis_b200 import abi
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 ORACLE_LIB = os.path.join(HERE, "libvb_oracle_bitrate.so")
 REF_LIB = os.path.join(HERE, "_ref", "libvorbis_ref_bitrate.so")
 DROPIN_LIB = os.path.join(HERE, "_ref", "libvorbis_dropin_bitrate.so")
 NB = abi.PACKETBLOBS
 BRANCHES = ("slew down", "slew up", "min loop", "max loop", "truncation", "padding")
-
-
-def build(cc="gcc"):
-    """the oracle library always; the two reference libraries where oracle/Makefile's objects exist"""
-    inc = os.path.join(ROOT, "include")
-    osrc = os.path.join(HERE, "vb_oracle_bitrate.c")
-    if _stale(ORACLE_LIB, [osrc, os.path.join(inc, "vorbis_b200.h")]):
-        subprocess.check_call([cc] + PARITY + ["-std=gnu99", "-Wall", "-I" + inc, "-shared", "-o", ORACLE_LIB, osrc,
-                                               "-lm"])
-    if not os.path.exists(os.path.join(REF_SRC, "lib", "mdct.c")):
-        return
-    refinc = ["-I" + os.path.join(HERE, "shim"), "-I" + os.path.join(REF_SRC, "include"),
-              "-I" + os.path.join(REF_SRC, "lib"), "-I" + inc]
-    src = os.path.join(HERE, "ref_bitrate.c")
-    for lib, objs, extra, tail in (
-            (REF_LIB, REF_OBJS, [], ["-lm"]),
-            (DROPIN_LIB, DROPIN_OBJS, ["-DVB200_DROPIN"],
-             ["-fopenmp", "-L" + os.path.join(ROOT, "vorbis_b200"), "-lvorbis_b200",
-              "-Wl,-rpath,$ORIGIN/../../vorbis_b200", "-lm"])):
-        paths = [os.path.join(OBJ, o) for o in objs]
-        if not all(os.path.exists(p) for p in paths):
-            continue
-        if not _stale(lib, paths + [src, os.path.join(inc, "vorbis_b200.h")]):
-            continue
-        obj = lib[:-3] + ".o"
-        subprocess.check_call([cc] + PARITY + ["-Wall"] + refinc + extra + ["-c", src, "-o", obj])
-        subprocess.check_call([cc, "-shared", "-Wl,-Bsymbolic", "-o", lib, obj] + paths + tail)
-        os.remove(obj)
 
 
 def ref_available(dropin=False):
@@ -132,7 +102,7 @@ _olib = None
 def _oracle_lib():
     global _olib
     if _olib is None:
-        build()
+        subprocess.check_call(["make", "-s", "-C", HERE, os.path.basename(ORACLE_LIB), "CC=gcc"])
         L = C.CDLL(ORACLE_LIB)
         L.vbo_bitrate_run.argtypes = [C.POINTER(abi.BitrateInfo), C.c_long, C.c_int, C.c_int, C.c_int, C.c_void_p,
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]

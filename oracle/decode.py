@@ -1,54 +1,20 @@
-"""Decode runs for the tests and tools/decode_throughput.py: build recipes and ctypes loaders of
+"""Decode runs for the tests and tools/decode_throughput.py: ctypes loaders of
   oracle/_ref/libvorbis_ref_decode.so     the stock reference encoder and decoder (ref_decode_streams.c)
   oracle/_ref/libvorbis_dropin_decode.so  many decoders through the multi-stream decode driver
                                           (vorbis_b200/host/vb200_decode.c, vb200md_*)
-Both link the objects oracle/Makefile compiles from the unmodified reference sources (targets `ref` and `dropin`)
-and are only built where those exist; like the rest of oracle/_ref they travel.
+oracle/Makefile builds both where the reference sources exist; like the rest of oracle/_ref they travel.
 
 TEST INFRASTRUCTURE ONLY: imported by tests/ and tools/, never by the product.
 """
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 
-from oracle.halfrate import DROPIN_OBJS, OBJ, PARITY, REF_OBJS, REF_SRC, _stale
-
 HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 REF_LIB = os.path.join(HERE, "_ref", "libvorbis_ref_decode.so")
 DROPIN_LIB = os.path.join(HERE, "_ref", "libvorbis_dropin_decode.so")
-DRIVER = os.path.join(ROOT, "vorbis_b200", "host", "vb200_decode.c")
 META = 5                       # offset, bytes, granulepos, e_o_s, packetno
-
-
-def build(cc="gcc"):
-    """the two libraries where oracle/Makefile's objects exist"""
-    if not os.path.exists(os.path.join(REF_SRC, "lib", "mdct.c")):
-        return
-    inc = os.path.join(ROOT, "include")
-    refinc = ["-I" + os.path.join(HERE, "shim"), "-I" + os.path.join(REF_SRC, "include"),
-              "-I" + os.path.join(REF_SRC, "lib"), "-I" + inc]
-    src = os.path.join(HERE, "ref_decode_streams.c")
-    for lib, objs, srcs, extra, tail in (
-            (REF_LIB, REF_OBJS, [src], ["-fopenmp"], ["-fopenmp", "-lm"]),
-            (DROPIN_LIB, DROPIN_OBJS, [src, DRIVER], ["-DVB200_DROPIN", "-fopenmp"],
-             ["-fopenmp", "-L" + os.path.join(ROOT, "vorbis_b200"), "-lvorbis_b200",
-              "-Wl,-rpath,$ORIGIN/../../vorbis_b200", "-lm"])):
-        paths = [os.path.join(OBJ, o) for o in objs]
-        if not all(os.path.exists(p) for p in paths):
-            continue
-        if not _stale(lib, paths + srcs + [os.path.join(inc, "vorbis_b200.h")]):
-            continue
-        own = []
-        for i, s in enumerate(srcs):
-            obj = lib[:-3] + ".%d.o" % i
-            subprocess.check_call([cc] + PARITY + ["-Wall"] + refinc + extra + ["-c", s, "-o", obj])
-            own.append(obj)
-        subprocess.check_call([cc, "-shared", "-Wl,-Bsymbolic", "-o", lib] + own + paths + tail)
-        for obj in own:
-            os.remove(obj)
 
 
 def available():

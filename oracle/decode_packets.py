@@ -1,53 +1,23 @@
-"""Checkers of the device entropy decode: build recipe and ctypes loader of
+"""Checkers of the device entropy decode: ctypes loader of
   oracle/_ref/libvorbis_ref_packets.so      ref_decode_packets.c + the stock reference objects: the managed
                                             encoder and the reference's staging
   oracle/_ref/libvorbis_dropin_packets.so   the same + the multi-stream decode driver
                                             (vorbis_b200/host/vb200_decode.c) + the drop-in reference objects
-Built only where oracle/Makefile's objects exist; like the rest of oracle/_ref it travels.
+oracle/Makefile builds both where the reference sources exist; like the rest of oracle/_ref they travel.
 
 TEST INFRASTRUCTURE ONLY: imported by tests/ and tools/, never by the product.
 """
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 
-from oracle.decode import DRIVER, META, Packets
-from oracle.halfrate import DROPIN_OBJS, OBJ, PARITY, REF_OBJS, REF_SRC, _stale
+from oracle.decode import META, Packets
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 LIB = os.path.join(HERE, "_ref", "libvorbis_dropin_packets.so")
 REF_LIB = os.path.join(HERE, "_ref", "libvorbis_ref_packets.so")
 FLOOR1_STRIDE = 65
-
-
-def build(cc="gcc"):
-    if not os.path.exists(os.path.join(REF_SRC, "lib", "mdct.c")):
-        return
-    inc = os.path.join(ROOT, "include")
-    refinc = ["-I" + os.path.join(HERE, "shim"), "-I" + os.path.join(REF_SRC, "include"),
-              "-I" + os.path.join(REF_SRC, "lib"), "-I" + inc]
-    src = os.path.join(HERE, "ref_decode_packets.c")
-    for lib, objs, srcs, extra, tail in (
-            (REF_LIB, REF_OBJS, [src], [], ["-lm"]),
-            (LIB, DROPIN_OBJS, [src, DRIVER], ["-DVB200_DROPIN", "-fopenmp"],
-             ["-fopenmp", "-L" + os.path.join(ROOT, "vorbis_b200"), "-lvorbis_b200",
-              "-Wl,-rpath,$ORIGIN/../../vorbis_b200", "-lm"])):
-        paths = [os.path.join(OBJ, o) for o in objs]
-        if not all(os.path.exists(p) for p in paths):
-            continue
-        if not _stale(lib, paths + srcs + [os.path.join(inc, "vorbis_b200.h")]):
-            continue
-        own = []
-        for i, s in enumerate(srcs):
-            obj = lib[:-3] + ".%d.o" % i
-            subprocess.check_call([cc] + PARITY + ["-Wall"] + refinc + extra + ["-c", s, "-o", obj])
-            own.append(obj)
-        subprocess.check_call([cc, "-shared", "-Wl,-Bsymbolic", "-o", lib] + own + paths + tail)
-        for obj in own:
-            os.remove(obj)
 
 
 def available():

@@ -1,10 +1,10 @@
-"""Checkers of vb200_decode_streams_packets: build recipe and ctypes loaders of
+"""Checkers of vb200_decode_streams_packets: ctypes loaders of
   oracle/libvb_oracle_decode_streams.so   the plain-C restatement of its per-stream plan (vb_oracle_decode_streams.c);
                                           builds anywhere gcc exists
   oracle/_ref/libvorbis_ref_plan.so       ref_decode_plan.c + the stock reference objects: the stock decoder's PCM and
                                           its state after every vorbis_synthesis_blockin, at full and half rate
-The second links the objects oracle/Makefile compiles from the unmodified reference sources and is only built where
-those exist; like the rest of oracle/_ref it travels.
+oracle/Makefile builds both; the second only where the reference sources exist, and like the rest of oracle/_ref it
+travels.
 
 TEST INFRASTRUCTURE ONLY: imported by tests/ and tools/, never by the product.
 """
@@ -15,35 +15,13 @@ import subprocess
 import numpy as np
 
 from oracle.decode import META
-from oracle.halfrate import OBJ, PARITY, REF_OBJS, REF_SRC, _stale
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 ORACLE_LIB = os.path.join(HERE, "libvb_oracle_decode_streams.so")
 REF_LIB = os.path.join(HERE, "_ref", "libvorbis_ref_plan.so")
 REF_REC = 8                    # status, W, samples, granulepos, pcm_returned, pcm_current, sequence, sample_count
 ORACLE_REC = 11                # the same, then lo, hi, fin
 STATE_WORDS = 6                # sizeof(vbo_ds_state) / 8
-
-
-def build(cc="gcc"):
-    src = os.path.join(HERE, "vb_oracle_decode_streams.c")
-    if _stale(ORACLE_LIB, [src]):
-        subprocess.check_call([cc] + PARITY + ["-std=gnu99", "-Wall", "-shared", "-o", ORACLE_LIB, src])
-    if not os.path.exists(os.path.join(REF_SRC, "lib", "mdct.c")):
-        return
-    paths = [os.path.join(OBJ, o) for o in REF_OBJS]
-    if not all(os.path.exists(p) for p in paths):
-        return
-    rsrc = os.path.join(HERE, "ref_decode_plan.c")
-    if not _stale(REF_LIB, paths + [rsrc]):
-        return
-    refinc = ["-I" + os.path.join(HERE, "shim"), "-I" + os.path.join(REF_SRC, "include"),
-              "-I" + os.path.join(REF_SRC, "lib"), "-I" + os.path.join(ROOT, "include")]
-    obj = REF_LIB[:-3] + ".o"
-    subprocess.check_call([cc] + PARITY + ["-Wall"] + refinc + ["-c", rsrc, "-o", obj])
-    subprocess.check_call([cc, "-shared", "-Wl,-Bsymbolic", "-o", REF_LIB, obj] + paths + ["-lm"])
-    os.remove(obj)
 
 
 def ref_available():
@@ -62,8 +40,7 @@ def _lib(ref):
             L.rdsp_decode.argtypes = [C.c_void_p, _lp, _lp, C.c_long, C.c_int, C.c_void_p, C.c_long, _lp,
                                       C.POINTER(C.c_int)]
         else:
-            if not os.path.exists(ORACLE_LIB):
-                build()
+            subprocess.check_call(["make", "-s", "-C", HERE, os.path.basename(ORACLE_LIB), "CC=gcc"])
             L = C.CDLL(ORACLE_LIB)
             L.vbo_ds_init.argtypes = [_lp, C.c_void_p, C.c_int]
             L.vbo_ds_run.argtypes = [_lp, C.c_void_p, _lp, C.c_long, C.c_int, C.c_void_p, C.c_int, _lp]

@@ -1,39 +1,17 @@
-"""Checker of the managed multi-stream driver's entropy path: build recipe and ctypes loader of
+"""Checker of the managed multi-stream driver's entropy path: ctypes loader of
   oracle/_ref/libvorbis_dropin_encmanaged.so   ref_encode_managed.c + the multi-stream encode driver
                                                (vorbis_b200/host/vb200_mapping0.c) + the drop-in reference objects
-Built only where oracle/Makefile's objects exist; like the rest of oracle/_ref it travels.
+oracle/Makefile builds it where the reference sources exist; like the rest of oracle/_ref it travels.
 
 TEST INFRASTRUCTURE ONLY: imported by tests/ and tools/, never by the product.
 """
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 
-from oracle.halfrate import DROPIN_OBJS, OBJ, PARITY, REF_SRC, _stale
-
 HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 LIB = os.path.join(HERE, "_ref", "libvorbis_dropin_encmanaged.so")
-
-
-def build(cc="gcc"):
-    if not os.path.exists(os.path.join(REF_SRC, "lib", "mdct.c")):
-        return
-    inc = os.path.join(ROOT, "include")
-    refinc = ["-I" + os.path.join(HERE, "shim"), "-I" + os.path.join(REF_SRC, "include"),
-              "-I" + os.path.join(REF_SRC, "lib"), "-I" + inc]
-    src = os.path.join(HERE, "ref_encode_managed.c")
-    paths = [os.path.join(OBJ, o) for o in DROPIN_OBJS]
-    if not all(os.path.exists(p) for p in paths) or not _stale(LIB, paths + [src]):
-        return
-    obj = LIB[:-3] + ".o"
-    subprocess.check_call([cc] + PARITY + ["-Wall"] + refinc + ["-DVB200_DROPIN", "-c", src, "-o", obj])
-    subprocess.check_call([cc, "-shared", "-Wl,-Bsymbolic", "-o", LIB, obj] + paths +
-                          ["-fopenmp", "-L" + os.path.join(ROOT, "vorbis_b200"), "-lvorbis_b200",
-                           "-Wl,-rpath,$ORIGIN/../../vorbis_b200", "-lm"])
-    os.remove(obj)
 
 
 def available():

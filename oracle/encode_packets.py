@@ -1,48 +1,21 @@
-"""Checkers of the device entropy coder: build recipe and ctypes loader of
+"""Checkers of the device entropy coder: ctypes loader of
   oracle/_ref/libvorbis_ref_encpackets.so      ref_encode_packets.c + the stock reference objects: the reference's own
                                                floor1_encode and residue class / forward on given posts and residue
   oracle/_ref/libvorbis_dropin_encpackets.so   the same file + the multi-stream encode driver
                                                (vorbis_b200/host/vb200_mapping0.c) + the drop-in reference objects
-Built only where oracle/Makefile's objects exist; like the rest of oracle/_ref it travels.
+oracle/Makefile builds both where the reference sources exist; like the rest of oracle/_ref they travel.
 
 TEST INFRASTRUCTURE ONLY: imported by tests/ and tools/, never by the product.
 """
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 
-from oracle.halfrate import DROPIN_OBJS, OBJ, PARITY, REF_OBJS, REF_SRC, _stale
-
 HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 LIB = os.path.join(HERE, "_ref", "libvorbis_dropin_encpackets.so")
 REF_LIB = os.path.join(HERE, "_ref", "libvorbis_ref_encpackets.so")
 FLOOR1_STRIDE = 65
-
-
-def build(cc="gcc"):
-    if not os.path.exists(os.path.join(REF_SRC, "lib", "mdct.c")):
-        return
-    inc = os.path.join(ROOT, "include")
-    refinc = ["-I" + os.path.join(HERE, "shim"), "-I" + os.path.join(REF_SRC, "include"),
-              "-I" + os.path.join(REF_SRC, "lib"), "-I" + inc]
-    src = os.path.join(HERE, "ref_encode_packets.c")
-    for lib, objs, extra, tail in (
-            (REF_LIB, REF_OBJS, [], ["-lm"]),
-            (LIB, DROPIN_OBJS, ["-DVB200_DROPIN", "-fopenmp"],
-             ["-fopenmp", "-L" + os.path.join(ROOT, "vorbis_b200"), "-lvorbis_b200",
-              "-Wl,-rpath,$ORIGIN/../../vorbis_b200", "-lm"])):
-        paths = [os.path.join(OBJ, o) for o in objs]
-        if not all(os.path.exists(p) for p in paths):
-            continue
-        if not _stale(lib, paths + [src, os.path.join(inc, "vorbis_b200.h")]):
-            continue
-        obj = lib[:-3] + ".o"
-        subprocess.check_call([cc] + PARITY + ["-Wall"] + refinc + extra + ["-c", src, "-o", obj])
-        subprocess.check_call([cc, "-shared", "-Wl,-Bsymbolic", "-o", lib, obj] + paths + tail)
-        os.remove(obj)
 
 
 def available():

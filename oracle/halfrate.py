@@ -1,9 +1,9 @@
-"""Half-rate decode (vorbis_synthesis_halfrate) for the tests: build recipes and ctypes loaders of
+"""Half-rate decode (vorbis_synthesis_halfrate) for the tests: ctypes loaders of
   oracle/libvb_oracle_halfrate.so          the CPU oracle's half-rate synthesis (vb_oracle_halfrate.c)
   oracle/_ref/libvorbis_ref_halfrate.so    the reference's own encoder / half-rate decoder (ref_halfrate.c)
   oracle/_ref/libvorbis_dropin_halfrate.so the same decoder with mdct_backward bound to the CUDA shim
-The two reference libraries link the objects oracle/Makefile compiles from the unmodified reference sources
-(targets `ref` and `dropin`) and are only built where those exist; like the rest of oracle/_ref they travel.
+oracle/Makefile builds all three; the two reference libraries only where the reference sources exist, and like the
+rest of oracle/_ref they travel.
 
 TEST INFRASTRUCTURE ONLY: imported by tests/ and tests/golden/make_golden_halfrate.py, never by the product.
 """
@@ -17,55 +17,13 @@ from vorbis_b200 import abi
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REF_DIR = os.path.join(HERE, "_ref")
-OBJ = os.path.join(REF_DIR, "obj")
 ORACLE_LIB = os.path.join(HERE, "libvb_oracle_halfrate.so")
 REF_LIB = os.path.join(REF_DIR, "libvorbis_ref_halfrate.so")
 DROPIN_LIB = os.path.join(REF_DIR, "libvorbis_dropin_halfrate.so")
-REF_SRC = os.environ.get("REF", "/root/reference")
-
-# oracle/Makefile: PARITY flags, REFSRC, REFINC, and the object sets of libvorbis_ref.so / libvorbis_dropin.so
-PARITY = ["-O2", "-fno-fast-math", "-ffp-contract=off", "-fPIC", "-fvisibility=default"]
-REFSRC = ["mdct", "window", "smallft", "psy", "block", "analysis", "synthesis", "envelope", "floor1", "floor0",
-          "res0", "codebook", "sharedbook", "info", "registry", "bitrate", "lpc", "lsp", "lookup", "vorbisenc"]
-REF_OBJS = [s + ".o" for s in REFSRC] + ["mapping0.o", "ref_driver.o", "bitpack.o"]
-DROPIN_OBJS = ([s + ".o" for s in REFSRC if s != "block"] +
-               ["block_shim.o", "mapping0_shim.o", "vb200_ref_shim.o", "vb200_mapping0.o", "bitpack.o"])
 
 f32p = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
 i32p = np.ctypeslib.ndpointer(np.int32, flags="C_CONTIGUOUS")
 i64p = np.ctypeslib.ndpointer(np.int64, flags="C_CONTIGUOUS")
-
-
-def _stale(target, sources):
-    return not os.path.exists(target) or any(os.path.getmtime(s) > os.path.getmtime(target) for s in sources)
-
-
-def build(cc="gcc"):
-    """the oracle library always; the two reference libraries where oracle/Makefile's objects exist"""
-    inc = os.path.join(os.path.dirname(HERE), "include")
-    deps = [os.path.join(HERE, f) for f in os.listdir(HERE) if f.startswith("vb_oracle") or f == "floor1_db_table.h"]
-    if _stale(ORACLE_LIB, deps):
-        subprocess.check_call([cc] + PARITY + ["-std=gnu99", "-Wall", "-I" + inc, "-I" + HERE, "-shared", "-o",
-                                               ORACLE_LIB, os.path.join(HERE, "vb_oracle_halfrate.c"), "-lm"])
-    if not os.path.exists(os.path.join(REF_SRC, "lib", "mdct.c")):
-        return
-    refinc = ["-I" + os.path.join(HERE, "shim"), "-I" + os.path.join(REF_SRC, "include"),
-              "-I" + os.path.join(REF_SRC, "lib"), "-I" + inc]
-    src = os.path.join(HERE, "ref_halfrate.c")
-    for lib, objs, extra, tail in (
-            (REF_LIB, REF_OBJS, [], ["-lm"]),
-            (DROPIN_LIB, DROPIN_OBJS, ["-DVB200_DROPIN"],
-             ["-fopenmp", "-L" + os.path.join(os.path.dirname(HERE), "vorbis_b200"), "-lvorbis_b200",
-              "-Wl,-rpath,$ORIGIN/../../vorbis_b200", "-lm"])):
-        paths = [os.path.join(OBJ, o) for o in objs]
-        if not all(os.path.exists(p) for p in paths):
-            continue
-        if not _stale(lib, paths + [src]):
-            continue
-        obj = lib[:-3] + ".o"
-        subprocess.check_call([cc] + PARITY + ["-Wall"] + refinc + extra + ["-c", src, "-o", obj])
-        subprocess.check_call([cc, "-shared", "-Wl,-Bsymbolic", "-o", lib, obj] + paths + tail)
-        os.remove(obj)
 
 
 # ---- the oracle ---------------------------------------------------------------------------------------
@@ -75,7 +33,7 @@ _olib = None
 def _oracle_lib():
     global _olib
     if _olib is None:
-        build()
+        subprocess.check_call(["make", "-s", "-C", HERE, os.path.basename(ORACLE_LIB), "CC=gcc"])
         L = C.CDLL(ORACLE_LIB)
         L.vbohs_create.restype = C.c_void_p
         L.vbohs_create.argtypes = [C.POINTER(abi.Setup), C.c_void_p]

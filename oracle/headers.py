@@ -1,51 +1,23 @@
-"""The reference's reading of three header packets: build recipe and ctypes loader of
+"""The reference's reading of three header packets: ctypes loader of
   oracle/_ref/libvorbis_ref_headers.so   ref_headers.c + the stock reference objects + the decode driver
                                          (vorbis_b200/host/vb200_decode.c, for vb200md_entropy_new)
-Built only where oracle/Makefile's objects exist; like the rest of oracle/_ref it travels.  Also `describe`, the
-comparable form of a (vb200_setup, vb200_entropy_setup, modebits) that both the reference's and the product's parse
-are reduced to.
+oracle/Makefile builds it where the reference sources exist; like the rest of oracle/_ref it travels.  Also
+`describe`, the comparable form of a (vb200_setup, vb200_entropy_setup, modebits) that both the reference's and the
+product's parse are reduced to.
 
 TEST INFRASTRUCTURE ONLY: imported by tests/ and tools/, never by the product.
 """
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 
-from oracle.decode import DRIVER
-from oracle.halfrate import OBJ, PARITY, REF_OBJS, REF_SRC, _stale
 from vorbis_b200 import abi
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 LIB = os.path.join(HERE, "_ref", "libvorbis_ref_headers.so")
 HANGS = -1000          # rh_open: vorbis_synthesis_init would not return (maptype 1, dimension 0)
 EIMPL_WHY = {1: "modes", 2: "floor0", 4: "submaps", 8: "dim", 16: "tables past the caps"}
-
-
-def build(cc="gcc"):
-    if not os.path.exists(os.path.join(REF_SRC, "lib", "mdct.c")):
-        return
-    inc = os.path.join(ROOT, "include")
-    refinc = ["-I" + os.path.join(HERE, "shim"), "-I" + os.path.join(REF_SRC, "include"),
-              "-I" + os.path.join(REF_SRC, "lib"), "-I" + inc]
-    srcs = [os.path.join(HERE, "ref_headers.c"), DRIVER]
-    paths = [os.path.join(OBJ, o) for o in REF_OBJS]
-    if not all(os.path.exists(p) for p in paths):
-        return
-    if not _stale(LIB, paths + srcs + [os.path.join(inc, "vorbis_b200.h")]):
-        return
-    own = []
-    for i, s in enumerate(srcs):
-        obj = LIB[:-3] + ".%d.o" % i
-        subprocess.check_call([cc] + PARITY + ["-Wall", "-fopenmp"] + refinc + ["-c", s, "-o", obj])
-        own.append(obj)
-    subprocess.check_call([cc, "-shared", "-Wl,-Bsymbolic", "-o", LIB] + own + paths +
-                          ["-fopenmp", "-L" + os.path.join(ROOT, "vorbis_b200"), "-lvorbis_b200",
-                           "-Wl,-rpath,$ORIGIN/../../vorbis_b200", "-lm"])
-    for obj in own:
-        os.remove(obj)
 
 
 def available():

@@ -1,20 +1,17 @@
-"""The LPC extrapolation of vorbis_analysis_wrote for the tests: build recipe and ctypes loaders of
+"""The LPC extrapolation of vorbis_analysis_wrote for the tests: ctypes loaders of
   oracle/libvb_oracle_lpc.so   vb_oracle_lpc.c: the plain-C restatement of the filter fit and the predictor
   oracle/_ref/libvorbis_ref.so the reference's own vorbis_lpc_from_data / vorbis_lpc_predict (compiled unmodified by
                                oracle/Makefile, lpc is in REFSRC; built only where the reference sources exist)
 and timeline(), which builds the v->pcm a stock encoder sees from its input and write schedule: the preamble from the
 write that crossed blocksizes[1] samples, the input, and the tail from the drained planner's base at the end write,
-which the carried planner of oracle/resume.py supplies.
+which the carried planner of oracle/resume.py supplies.  oracle/Makefile builds both libraries.
 
 TEST INFRASTRUCTURE ONLY: imported by tests/ and tools/, never by the product.
 """
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
-
-from oracle.halfrate import PARITY, _stale
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 ORACLE_LIB = os.path.join(HERE, "libvb_oracle_lpc.so")
@@ -22,12 +19,6 @@ REF_LIB = os.path.join(HERE, "_ref", "libvorbis_ref.so")
 PRE, TAIL = 16, 32
 
 f32p = np.ctypeslib.ndpointer(np.float32, flags="C_CONTIGUOUS")
-
-
-def build(cc="gcc"):
-    src = os.path.join(HERE, "vb_oracle_lpc.c")
-    if _stale(ORACLE_LIB, [src]):
-        subprocess.check_call([cc] + PARITY + ["-std=gnu99", "-Wall", "-shared", "-o", ORACLE_LIB, src])
 
 
 _libs = {}

@@ -1,47 +1,19 @@
-"""Bitrate-managed encoder runs for the tests: build recipes and ctypes loaders of
+"""Bitrate-managed encoder runs for the tests: ctypes loaders of
   oracle/_ref/libvorbis_ref_managed.so     the stock reference encoder from vorbis_encode_init (ref_managed.c)
   oracle/_ref/libvorbis_dropin_managed.so  N such encoders through the managed multi-stream driver
                                            (vorbis_b200/host/vb200_mapping0.c, vb200ms_open_managed)
-Both link the objects oracle/Makefile compiles from the unmodified reference sources (targets `ref` and `dropin`)
-and are only built where those exist; like the rest of oracle/_ref they travel.
+oracle/Makefile builds both where the reference sources exist; like the rest of oracle/_ref they travel.
 
 TEST INFRASTRUCTURE ONLY: imported by tests/, never by the product.
 """
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
-
-from oracle.halfrate import DROPIN_OBJS, OBJ, PARITY, REF_OBJS, REF_SRC, _stale
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REF_LIB = os.path.join(HERE, "_ref", "libvorbis_ref_managed.so")
 DROPIN_LIB = os.path.join(HERE, "_ref", "libvorbis_dropin_managed.so")
-
-
-def build(cc="gcc"):
-    """the two libraries where oracle/Makefile's objects exist"""
-    if not os.path.exists(os.path.join(REF_SRC, "lib", "mdct.c")):
-        return
-    inc = os.path.join(os.path.dirname(HERE), "include")
-    refinc = ["-I" + os.path.join(HERE, "shim"), "-I" + os.path.join(REF_SRC, "include"),
-              "-I" + os.path.join(REF_SRC, "lib"), "-I" + inc]
-    src = os.path.join(HERE, "ref_managed.c")
-    for lib, objs, extra, tail in (
-            (REF_LIB, REF_OBJS, [], ["-lm"]),
-            (DROPIN_LIB, DROPIN_OBJS, ["-DVB200_DROPIN"],
-             ["-fopenmp", "-L" + os.path.join(os.path.dirname(HERE), "vorbis_b200"), "-lvorbis_b200",
-              "-Wl,-rpath,$ORIGIN/../../vorbis_b200", "-lm"])):
-        paths = [os.path.join(OBJ, o) for o in objs]
-        if not all(os.path.exists(p) for p in paths):
-            continue
-        if not _stale(lib, paths + [src]):
-            continue
-        obj = lib[:-3] + ".o"
-        subprocess.check_call([cc] + PARITY + ["-Wall"] + refinc + extra + ["-c", src, "-o", obj])
-        subprocess.check_call([cc, "-shared", "-Wl,-Bsymbolic", "-o", lib, obj] + paths + tail)
-        os.remove(obj)
 
 
 def available():

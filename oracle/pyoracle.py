@@ -21,11 +21,7 @@ u8p = np.ctypeslib.ndpointer(np.uint8, flags="C_CONTIGUOUS")
 
 
 def build(force=False):
-    src = [os.path.join(HERE, f) for f in ("vb_oracle.c", "vb_oracle.h", "vb_oracle_b.inc", "vb_oracle_floor.inc")]
-    if (not force and os.path.exists(LIB_PATH)
-            and all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(s) for s in src)):
-        return
-    subprocess.check_call(["make", "-s", "-C", HERE, "libvb_oracle.so", "CC=gcc"])
+    subprocess.check_call(["make", "-s"] + (["-B"] if force else []) + ["-C", HERE, "libvb_oracle.so", "CC=gcc"])
 
 
 _lib = None

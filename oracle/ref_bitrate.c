@@ -13,7 +13,7 @@
  *   rbr_open_managed / rbr_ctx / rbr_close   a vb200ms_open_managed'd driver, whose context carries the setup and the
  *                                            entropy setup of the managed encoder
  *
- * oracle/bitrate.py links this file with the stock reference objects, and once more with the driver and the drop-in
+ * oracle/Makefile links this file with the stock reference objects, and once more with the driver and the drop-in
  * objects.
  */
 #include <stdint.h>

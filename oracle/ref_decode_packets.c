@@ -11,7 +11,7 @@
  *   rdp_md_run           rds_md_run with the host entropy path forced or not, reporting the path taken
  *
  * Packets live back to back in one byte buffer; meta[i] = {offset, bytes, granulepos, e_o_s, packetno}.
- * oracle/decode_packets.py links this file with the stock reference objects, and once more with the driver and the
+ * oracle/Makefile links this file with the stock reference objects, and once more with the driver and the
  * drop-in objects.
  */
 #include <stdint.h>

@@ -9,7 +9,7 @@
  *                 and the PCM in pcmout order, float [ch][cap].  modebits: private_state.modebits.
  *
  * Packets live back to back in one byte buffer; meta rows are {offset, bytes, granulepos, e_o_s, packetno}.
- * oracle/decode_streams.py links this file with the objects oracle/Makefile compiles from the unmodified reference.
+ * oracle/Makefile links this file with the objects it compiles from the unmodified reference.
  */
 #include <stdint.h>
 #include <stdlib.h>

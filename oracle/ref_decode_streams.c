@@ -9,7 +9,7 @@
  *                       (vorbis_b200/host/vb200_decode.c), fed in a given per-round schedule
  *
  * Packets live back to back in one byte buffer; meta[i] = {offset, bytes, granulepos, e_o_s, packetno}.
- * oracle/decode.py links this file with the objects oracle/Makefile compiles from the unmodified reference sources.
+ * oracle/Makefile links this file with the objects it compiles from the unmodified reference sources.
  */
 #include <math.h>
 #include <stdint.h>

@@ -4,7 +4,7 @@
  *                           (host_entropy = 1), or left as the driver chooses it (0); reports the path it took, as
  *                           ref_encode_packets.c's rep_ms_encode does
  *
- * oracle/encode_managed.py links this file with the managed multi-stream driver and the drop-in objects.
+ * oracle/Makefile links this file with the managed multi-stream driver and the drop-in objects.
  */
 #include <stdint.h>
 #include <stdlib.h>

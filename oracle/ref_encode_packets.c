@@ -10,7 +10,7 @@
  *   rep_setup_new / rep_setup_free                   the driver's struct vb200_encode_entropy_setup, for editing
  *   rep_ms_encode                                    ref_ms_encode with the host entropy path forced or not
  *
- * oracle/encode_packets.py links this file with the stock reference objects, and once more with the driver and the
+ * oracle/Makefile links this file with the stock reference objects, and once more with the driver and the
  * drop-in objects.
  */
 #include <stdint.h>

@@ -1,7 +1,7 @@
 /* ref_halfrate.c — half-rate decode through the UNMODIFIED reference sources.
  *
  * TEST INFRASTRUCTURE ONLY.  Compiled against the reference's headers and linked with the reference objects
- * oracle/Makefile builds (oracle/halfrate.py has the recipe):
+ * oracle/Makefile builds:
  *   _ref/libvorbis_ref_halfrate.so     the stock reference (target `ref`'s objects)
  *   _ref/libvorbis_dropin_halfrate.so  the drop-in build, mapping0_inverse's mdct_backward bound to the CUDA
  *                                      shim (target `dropin`'s objects); compiled with -DVB200_DROPIN

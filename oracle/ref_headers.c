@@ -9,7 +9,7 @@
  *               dimension is outside 1..127; bit 4: more codewords or value rows than VB200_HEADERS_MAX_*), and
  *               where that is 0 the handle carries md_setup's vb200_setup and vb200md_entropy_new's vb200_entropy_setup (vorbis_b200/host/vb200_decode.c) of the decoder.
  *   rh_setup / rh_entropy / rh_modebits / rh_info / rh_close
- * oracle/headers.py links this file with the stock reference objects and the driver.
+ * oracle/Makefile links this file with the stock reference objects and the driver.
  */
 #include <stdint.h>
 #include <stdlib.h>

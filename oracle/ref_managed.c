@@ -7,7 +7,7 @@
  *   ref_ms_encode_managed      (-DVB200_DROPIN) N encoders of that configuration through the managed multi-stream
  *                              driver of vorbis_b200/host/vb200_mapping0.c (vb200ms_open_managed), fed in lockstep
  *
- * Both feed 1024-sample writes.  oracle/managed.py links this file with the objects oracle/Makefile compiles from
+ * Both feed 1024-sample writes.  oracle/Makefile links this file with the objects it compiles from
  * the unmodified reference sources.
  */
 #include <stdint.h>

@@ -1,5 +1,5 @@
 /* ref_resume.c — the unmodified reference's planner state after every vorbis_analysis_blockout.  TEST INFRASTRUCTURE
- * ONLY (oracle/resume.py links it with the stock reference objects that oracle/Makefile compiles).
+ * ONLY (oracle/Makefile links it with the stock reference objects it compiles).
  *
  *   ref_resume_capture  a stock VBR encoder on one stream, written in chunks of `chunk` samples then
  *                       vorbis_analysis_wrote(v, 0), with the blockout loop of examples/encoder_example.c after every

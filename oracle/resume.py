@@ -1,46 +1,24 @@
-"""The carried block planner for the tests: build recipes and ctypes loaders of
+"""The carried block planner for the tests: ctypes loaders of
   oracle/libvb_oracle_resume.so        vb_oracle_resume.c: the plain-C restatement of the planner that
                                        vb200_encode_streams_packets[_managed]_resume carry from call to call
   oracle/_ref/libvorbis_ref_resume.so  ref_resume.c + the stock reference objects: the reference's planner state
                                        after every vorbis_analysis_blockout of a stream written in chunks
-The reference library links the objects oracle/Makefile compiles from the unmodified reference sources and is only
-built where those exist; like the rest of oracle/_ref it travels.
+oracle/Makefile builds both; the reference library only where the reference sources exist, and like the rest of
+oracle/_ref it travels.
 
 TEST INFRASTRUCTURE ONLY: imported by tests/, never by the product.
 """
 import ctypes as C
 import os
-import subprocess
 
 import numpy as np
 
-from oracle.halfrate import OBJ, PARITY, REF_OBJS, REF_SRC, _stale
 from vorbis_b200 import abi
 
 HERE = os.path.dirname(os.path.abspath(__file__))
-ROOT = os.path.dirname(HERE)
 ORACLE_LIB = os.path.join(HERE, "libvb_oracle_resume.so")
 REF_LIB = os.path.join(HERE, "_ref", "libvorbis_ref_resume.so")
 REC_FIELDS = ("write", "base", "current", "cursor", "curmark", "kept", "centerW", "W", "lW", "nW", "blocktype")
-
-
-def build(cc="gcc"):
-    inc = os.path.join(ROOT, "include")
-    osrc = os.path.join(HERE, "vb_oracle_resume.c")
-    if _stale(ORACLE_LIB, [osrc, os.path.join(inc, "vorbis_b200.h")]):
-        subprocess.check_call([cc] + PARITY + ["-std=gnu99", "-Wall", "-I" + inc, "-shared", "-o", ORACLE_LIB, osrc])
-    if not os.path.exists(os.path.join(REF_SRC, "lib", "mdct.c")):
-        return
-    paths = [os.path.join(OBJ, o) for o in REF_OBJS]
-    src = os.path.join(HERE, "ref_resume.c")
-    if not all(os.path.exists(p) for p in paths) or not _stale(REF_LIB, paths + [src]):
-        return
-    refinc = ["-I" + os.path.join(HERE, "shim"), "-I" + os.path.join(REF_SRC, "include"),
-              "-I" + os.path.join(REF_SRC, "lib"), "-I" + inc]
-    obj = REF_LIB[:-3] + ".o"
-    subprocess.check_call([cc] + PARITY + ["-Wall"] + refinc + ["-c", src, "-o", obj])
-    subprocess.check_call([cc, "-shared", "-Wl,-Bsymbolic", "-o", REF_LIB, obj] + paths + ["-lm"])
-    os.remove(obj)
 
 
 class Carry(C.Structure):

@@ -4,7 +4,7 @@
  * packet lengths alone: the 15 packets of a block are given as bit counts, and the result is the packet kept and its
  * final length in bytes (cut to maxsize, or padded with zero bytes up to minsize).  It is written from the reference's
  * description, not shared with the device code (vorbis_b200/csrc/vb200_bitrate.cuh), so that each checks the other.
- * Built into oracle/libvb_oracle_bitrate.so by oracle/bitrate.py, anywhere gcc exists.
+ * Built into oracle/libvb_oracle_bitrate.so by oracle/Makefile, anywhere gcc exists.
  */
 #include <math.h>
 #include <string.h>

@@ -10,7 +10,7 @@
  *   - de-coupling and the floor multiply still cover all n lines (lib/mapping0.c:754-790).
  * The overlap-add of vb_oracle_b.inc is written against a context's two transforms, so a second context
  * whose transforms are those of the halved sizes gives exactly the half-rate overlap-add.
- * Built by oracle/halfrate.py with the flags of oracle/Makefile's libvb_oracle.so.
+ * Built by oracle/Makefile with the flags of its libvb_oracle.so.
  */
 #include "vb_oracle.c"
 

@@ -1,5 +1,5 @@
 /* vb_oracle_lpc.c — the LPC extrapolation of vorbis_analysis_wrote restated in plain C.  TEST INFRASTRUCTURE ONLY
- * (oracle/lpc.py builds and binds it; it is the CPU counterpart of vorbis_b200/csrc/vb200_lpc.cuh).
+ * (oracle/Makefile builds it and oracle/lpc.py binds it; it is the CPU counterpart of vorbis_b200/csrc/vb200_lpc.cuh).
  *
  *   vbo_lpc_filter   the coefficients of an order-m linear predictor fitted to x[0 .. n): the lag-k autocorrelations
  *                    as sequential double sums over ascending i, the Levinson-Durbin recursion in double with a

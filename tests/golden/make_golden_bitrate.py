@@ -14,11 +14,12 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, ROOT)
 
+import __graft_entry__  # noqa: E402
 from oracle import bitrate as B  # noqa: E402
 
 
 def main():
-    B.build()
+    __graft_entry__.build()
     assert B.ref_available(), "oracle/_ref/libvorbis_ref_bitrate.so not built"
     rng = np.random.default_rng(31)
     out = {"names": np.array(list(B.CONFIGS))}

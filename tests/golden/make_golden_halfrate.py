@@ -2,7 +2,7 @@
 """Record the reference's half-rate decode (vorbis_synthesis_halfrate(vi, 1)) for tests/test_halfrate_oracle.py
 and tests/test_gpu_halfrate.py into tests/golden/ref/halfrate/halfrate.npz, keys "<cfg>__<name>".  For every decode
 fixture tests/golden/decode_<cfg>.npz: the block flags of its window, the half-rate PCM those blocks finish and
-the two half windows of the halved block sizes.  Needs oracle/_ref/libvorbis_ref_halfrate.so (oracle/halfrate.py
+the two half windows of the halved block sizes.  Needs oracle/_ref/libvorbis_ref_halfrate.so (oracle/Makefile
 builds it from the unmodified reference sources).  Writes no other file.
 
 usage:  python tests/golden/make_golden_halfrate.py
@@ -16,15 +16,16 @@ HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
+import __graft_entry__  # noqa: E402
 from conftest import CONFIG_NAMES  # noqa: E402
 from oracle import halfrate  # noqa: E402
 from test_halfrate_oracle import FIXTURE, reference_halfrate  # noqa: E402
 
 
 def main():
-    halfrate.build()
+    __graft_entry__.build()
     if not halfrate.ref_available():
-        sys.exit("oracle/_ref/libvorbis_ref_halfrate.so is missing: it needs oracle/Makefile's `ref` objects")
+        sys.exit("oracle/_ref/libvorbis_ref_halfrate.so is missing: it needs the reference sources")
     out = {}
     for name in CONFIG_NAMES:
         rec = reference_halfrate(name)

@@ -22,7 +22,7 @@
  * vb200shim_attach, whose decoder bindings carry only what the function-level mdct_backward shim needs.
  * Limits: floor type 1 only (OV_EIMPL otherwise), two modes with blockflag 0 and 1, full-rate decode; the device
  * path also needs residue types 1 and 2 (type 0 keeps the host path).
- * Compiled like any libvorbis-internal backend against lib/codec_internal.h (oracle/decode.py builds it).
+ * Compiled like any libvorbis-internal backend against lib/codec_internal.h (oracle/Makefile builds it).
  */
 #include <stdint.h>
 #include <stdio.h>
