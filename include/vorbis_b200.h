@@ -929,6 +929,66 @@ int vb200_ogg_group    (int nfiles, const uint8_t *data, int64_t data_bytes, con
                         int32_t *order, int32_t *npkt_out, struct vb200_packet_info *info_out,
                         vb200_file_group *groups, int32_t *ngroups);
 
+/* ---- Ogg Vorbis files out: the page mux of libogg on the device, for many streams in one call, whole or in pieces.
+ * No context.  The pages are those libogg 1.3.x (framing.c) makes when driven as examples/encoder_example.c drives it:
+ * ogg_stream_packetin of the three header packets, then ogg_stream_flush until it returns 0; for every audio packet
+ * ogg_stream_packetin, then ogg_stream_pageout until it returns 0.  The rules below restate framing.c as it behaves;
+ * they have not been run against libogg, and where they differ from libogg, libogg is right.
+ *   State per stream: a FIFO of lacing values (each marked as the first of its packet or not, each with a granule),
+ *     b_o_s (a page has been written), e_o_s (an e_o_s packet went in), pageno (from 0).
+ *   packetin of b bytes: b/255 values of 255, then one of b % 255 (0 bytes: one value 0; 255 bytes: 255, 0); the last
+ *     value takes the packet's granulepos, the first is marked; an e_o_s packet sets e_o_s.
+ *   flush_i(force): maxvals = min(fill, 255); none: no page.  !b_o_s: the page is the values up to and including the
+ *     first one below 255 (maxvals if none), granulepos 0.  Otherwise acc = done = just = 0, granulepos -1, and for
+ *     vals = 0 .. maxvals-1: if acc > 4096 and just >= 4, force and stop; acc += value; a value below 255 sets the
+ *     granulepos to its granule and just = ++done, a value of 255 sets just = 0.  vals == 255 forces.  No force: no
+ *     page.  The page: "OggS", version 0, flags (0x01 when value 0 is not the first of its packet, 0x02 when !b_o_s,
+ *     0x04 when e_o_s and fill == vals), granulepos int64 LE, serial, pageno++ and the CRC as u32 LE (the demux's
+ *     CRC, bytes 22..25 taken as zero), nseg = vals, the lacing values, the body; then b_o_s = 1 and the values go.
+ *   pageout = flush_i(fill && (e_o_s || !b_o_s)); flush = flush_i(1).
+ * A page is decided once the 4096/4 rule holds at a packet boundary with a packet after it, at 255 values, or at the
+ * end of an e_o_s packet, so the pages are a function of the packet sequence alone: a call writes every decided page
+ * and leaves the rest (fewer than 255 lacing values: at most 254 packets, 64 770 bytes) to the next call, where the
+ * caller passes those packets again.
+ * Inputs:
+ *   data [data_bytes]  packet bytes; never read outside [0, data_bytes)
+ *   hdr [nstreams][3]  the three header packets' rows (offset, bytes, granulepos) into data; streams may share rows.
+ *                      Read only for fresh carries; may be NULL when no carry is fresh.
+ *   npkt [nstreams], info [nstreams][max_packets]  this call's audio packets of each stream, the encoder's and the
+ *                      demux's table layout: offset absolute into data, bytes, granulepos and e_o_s are read;
+ *                      packetno and choice are not (Ogg does not store them).  The carry's kept packets come first.
+ *   carry [nstreams]   read and written: a fresh carry is all zero but for its serial.
+ * Outputs:
+ *   out_off [nstreams+1]  stream s's pages of this call are out[out_off[s] .. out_off[s+1]); so a call with fresh
+ *                      carries and every stream ending in e_o_s gives the (bytes, file_off) vb200_ogg_demux takes.
+ *   status [nstreams]  0 or VB200_EINVAL, when npkt is outside [kept, max_packets], a row has bytes < 0 or lies
+ *                      outside [0, data_bytes), an e_o_s row is not the last row passed, a done carry gets packets, a
+ *                      fresh carry has no header rows, or the carry is not one this call writes (state outside 0..2,
+ *                      negative kept or kept_segs, kept_segs without kept or with fewer segments in the first packet).
+ *                      Such a stream writes no bytes (its range is empty) and its carry stays as it was.
+ *   If out_off[nstreams] > out_cap, no page and no carry is written; out_off and status are, so out_cap = 0 (out NULL)
+ *   sizes a call.
+ * Three kernel launches whatever nstreams is (count, offsets, write; one warp per stream); no device scratch.
+ * _dev: device pointers, asynchronous on `stream`; checks its pointers and sizes only.  Host form: host buffers on the
+ * current CUDA device; returns VB200_EINVAL also when out_cap is too small or any status is nonzero, and writes the
+ * carries back only when it returns 0 (out, out_off and status whenever the pages fit).                       */
+typedef struct vb200_ogg_mux_carry {
+  uint32_t serial;     /* ogg_stream_init's serial; the caller sets it in a fresh (otherwise all-zero) carry */
+  uint32_t pageno;     /* the next page's sequence number */
+  int32_t  state;      /* 0 fresh (headers not yet written), 1 writing, 2 done (the EOS page is written) */
+  int32_t  kept;       /* audio packets at the end of the last call's input not yet wholly on pages:
+                          the next call passes them again, first, with the same bytes */
+  int32_t  kept_segs;  /* lacing values of the first kept packet already on pages */
+  int32_t  pad;
+} vb200_ogg_mux_carry;
+int vb200_ogg_mux_dev(int nstreams, const uint8_t *d_data, int64_t data_bytes, const struct vb200_packet_info *d_hdr,
+                      int max_packets, const int32_t *d_npkt, const struct vb200_packet_info *d_info,
+                      vb200_ogg_mux_carry *d_carry, uint8_t *d_out, int64_t out_cap, int64_t *d_out_off,
+                      int32_t *d_status, void *stream);
+int vb200_ogg_mux    (int nstreams, const uint8_t *data, int64_t data_bytes, const struct vb200_packet_info *hdr,
+                      int max_packets, const int32_t *npkt, const struct vb200_packet_info *info,
+                      vb200_ogg_mux_carry *carry, uint8_t *out, int64_t out_cap, int64_t *out_off, int32_t *status);
+
 /* ---- encode: the entropy coding of mapping0_forward (lib/mapping0.c:596-687) on the device, un-managed bitrate.
  * What floor1_encode (lib/floor1.c:753-921) and the residue class / forward of types 1 and 2 (lib/res0.c:534-648,
  * 725-809) read, registered on a context with vb200_encode_entropy_setup.

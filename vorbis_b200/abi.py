@@ -302,6 +302,10 @@ assert VorbisHeaders.setup.offset == 32 and VorbisHeaders.entropy.offset == 32 +
 # vb200_file_group: one group of vb200_ogg_group
 FILE_GROUP_DTYPE = np.dtype([("first", "<i4"), ("files", "<i4"), ("rep", "<i4")])
 assert FILE_GROUP_DTYPE.itemsize == 12
+# vb200_ogg_mux_carry: one stream's page state between vb200_ogg_mux calls
+OGG_MUX_CARRY_DTYPE = np.dtype([("serial", "<u4"), ("pageno", "<u4"), ("state", "<i4"), ("kept", "<i4"),
+                                ("kept_segs", "<i4"), ("pad", "<i4")])
+assert OGG_MUX_CARRY_DTYPE.itemsize == 24 and OGG_MUX_CARRY_DTYPE.fields["kept_segs"][1] == 16
 
 
 class EncCodebook(C.Structure):

@@ -32,6 +32,7 @@
 #include "vb200_ogg.cuh"
 #include "vb200_headers.h"
 #include "vb200_ogg_group.cuh"
+#include "vb200_ogg_mux.cuh"
 #include "floor1_db_table.h"
 
 using namespace vb200;
@@ -4702,6 +4703,73 @@ extern "C" int vb200_ogg_group(int nfiles, const uint8_t *data, int64_t data_byt
   for (int p = 0; p < nfiles; p++)                        // rows past npkt_out[p] are not written
     memcpy(info_out + (size_t)p * max_packets, rows.data() + (size_t)p * max_packets,
            sizeof(vb200_packet_info) * npkt_out[p]);
+  return 0;
+}
+
+// ======================================================================== //
+// Ogg files out: the page mux (vb200_ogg_mux.cuh)
+static_assert(sizeof(vb200_ogg_mux_carry) == 24 && offsetof(vb200_ogg_mux_carry, kept_segs) == 16,
+              "vb200_ogg_mux_carry layout (OGG_MUX_CARRY_DTYPE in abi.py)");
+extern "C" int vb200_ogg_mux_dev(int nstreams, const uint8_t *d_data, int64_t data_bytes, const vb200_packet_info *d_hdr,
+                                 int max_packets, const int32_t *d_npkt, const vb200_packet_info *d_info,
+                                 vb200_ogg_mux_carry *d_carry, uint8_t *d_out, int64_t out_cap, int64_t *d_out_off,
+                                 int32_t *d_status, void *stream) {
+  if (nstreams < 0 || max_packets < 1 || data_bytes < 0 || out_cap < 0)
+    return fail(VB200_EINVAL, "ogg_mux: nstreams < 0, max_packets < 1 or a negative size");
+  if (!d_out_off) return fail(VB200_EINVAL, "ogg_mux: null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (nstreams == 0) { CU(cudaMemsetAsync(d_out_off, 0, sizeof(int64_t), st)); return 0; }
+  if (!d_npkt || !d_info || !d_carry || !d_status || (data_bytes && !d_data) || (out_cap && !d_out))
+    return fail(VB200_EINVAL, "ogg_mux: null pointer");
+  OggMuxArgs A{nstreams, d_data, data_bytes, d_hdr, max_packets, d_npkt, d_info, d_carry, d_out, out_cap,
+               (long long *)d_out_off, d_status};
+  const int grid = (nstreams + OGG_MUX_WARPS - 1) / OGG_MUX_WARPS;
+  k_ogg_mux_count<<<grid, 32 * OGG_MUX_WARPS, 0, st>>>(A);
+  k_ds_scan<<<1, 1024, 0, st>>>(nstreams, A.out_off);
+  k_ogg_mux_write<<<grid, 32 * OGG_MUX_WARPS, 0, st>>>(A);
+  CU(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int vb200_ogg_mux(int nstreams, const uint8_t *data, int64_t data_bytes, const vb200_packet_info *hdr,
+                             int max_packets, const int32_t *npkt, const vb200_packet_info *info,
+                             vb200_ogg_mux_carry *carry, uint8_t *out, int64_t out_cap, int64_t *out_off,
+                             int32_t *status) {
+  if (nstreams < 0 || max_packets < 1 || data_bytes < 0 || out_cap < 0)
+    return fail(VB200_EINVAL, "ogg_mux: nstreams < 0, max_packets < 1 or a negative size");
+  if (!out_off) return fail(VB200_EINVAL, "ogg_mux: null pointer");
+  out_off[0] = 0;
+  if (nstreams == 0) return 0;
+  if (!npkt || !info || !carry || !status || (data_bytes && !data) || (out_cap && !out))
+    return fail(VB200_EINVAL, "ogg_mux: null pointer");
+  const size_t n_info = (size_t)nstreams * max_packets;
+  DevBuf buf;                                             // freed on return
+  uint8_t *dd, *dout;
+  vb200_packet_info *dh, *di;
+  int32_t *dn, *dst;
+  vb200_ogg_mux_carry *dc;
+  int64_t *doff;
+  int rc = carve(buf, [&](Carve &c) {
+    dd = c.take<uint8_t>((size_t)data_bytes); dh = c.take<vb200_packet_info>(hdr ? (size_t)nstreams * 3 : 0);
+    dn = c.take<int32_t>(nstreams); di = c.take<vb200_packet_info>(n_info); dc = c.take<vb200_ogg_mux_carry>(nstreams);
+    dout = c.take<uint8_t>((size_t)out_cap); doff = c.take<int64_t>(nstreams + 1); dst = c.take<int32_t>(nstreams);
+  });
+  if (rc) return rc;
+  if (data_bytes) CU(cudaMemcpy(dd, data, (size_t)data_bytes, cudaMemcpyHostToDevice));
+  if (hdr) CU(cudaMemcpy(dh, hdr, sizeof(vb200_packet_info) * nstreams * 3, cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(dn, npkt, sizeof(int32_t) * nstreams, cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(di, info, sizeof(vb200_packet_info) * n_info, cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(dc, carry, sizeof(vb200_ogg_mux_carry) * nstreams, cudaMemcpyHostToDevice));
+  if ((rc = vb200_ogg_mux_dev(nstreams, dd, data_bytes, hdr ? dh : nullptr, max_packets, dn, di, dc,
+                              out_cap ? dout : nullptr, out_cap, doff, dst, nullptr)))
+    return rc;
+  CU(cudaMemcpy(out_off, doff, sizeof(int64_t) * (nstreams + 1), cudaMemcpyDeviceToHost));
+  CU(cudaMemcpy(status, dst, sizeof(int32_t) * nstreams, cudaMemcpyDeviceToHost));
+  if (out_off[nstreams] > out_cap) return fail(VB200_EINVAL, "ogg_mux: out_cap below the pages' bytes");
+  if (out_off[nstreams]) CU(cudaMemcpy(out, dout, (size_t)out_off[nstreams], cudaMemcpyDeviceToHost));
+  for (int s = 0; s < nstreams; s++)
+    if (status[s]) return fail(VB200_EINVAL, "ogg_mux: a stream's rows or carry are invalid (see status)");
+  CU(cudaMemcpy(carry, dc, sizeof(vb200_ogg_mux_carry) * nstreams, cudaMemcpyDeviceToHost));
   return 0;
 }
 

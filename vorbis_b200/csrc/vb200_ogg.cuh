@@ -35,13 +35,8 @@ __device__ __forceinline__ uint32_t ogg_le32(const uint8_t *p) {
   return (uint32_t)p[0] | ((uint32_t)p[1] << 8) | ((uint32_t)p[2] << 16) | ((uint32_t)p[3] << 24);
 }
 
-__global__ void __launch_bounds__(32 * OGG_WARPS)
-k_ogg_demux(int nfiles, const uint8_t *__restrict__ bytes, const int64_t *__restrict__ file_off, int max_packets,
-            vb200_packet_info *__restrict__ info, int32_t *__restrict__ npkt_out, uint8_t *__restrict__ data,
-            vb200_ogg_stream *__restrict__ streams) {
-  __shared__ uint32_t crc_tab[256];
-  __shared__ uint32_t xpw[OGG_XPOW];
-  __shared__ uint8_t lace_all[OGG_WARPS][256];
+// the byte table of the CRC and xpw[k] = x^(8 * 2^k) mod P in shared memory, built by the whole block
+__device__ __forceinline__ void ogg_crc_setup(uint32_t *crc_tab, uint32_t *xpw) {
   for (int i = threadIdx.x; i < 256; i += blockDim.x) {
     uint32_t r = (uint32_t)i << 24;
     for (int k = 0; k < 8; k++) r = (r << 1) ^ ((r & 0x80000000u) ? OGG_POLY : 0u);
@@ -52,6 +47,37 @@ k_ogg_demux(int nfiles, const uint8_t *__restrict__ bytes, const int64_t *__rest
     for (int k = 1; k < OGG_XPOW; k++) xpw[k] = ogg_mulmod(xpw[k - 1], xpw[k - 1]);
   }
   __syncthreads();
+}
+
+// the CRC of pg[0 .. len) with bytes 22..25 taken as zero, by one converged warp: lane i runs the table over its
+// chunk from 0 and shifts the result by x^(8 * bytes after the chunk); every lane returns the xor of the chunks
+__device__ __forceinline__ uint32_t ogg_page_crc(const uint8_t *pg, int len, int lane, const uint32_t *crc_tab,
+                                                 const uint32_t *xpw) {
+  const int chunk = (len + 31) / 32;
+  const int a = min(lane * chunk, len), e = min(a + chunk, len);
+  uint32_t c = 0;
+  for (int i = a; i < e; i++) {
+    const uint32_t v = (i >= 22 && i < 26) ? 0u : pg[i];
+    c = (c << 8) ^ crc_tab[(c >> 24) ^ v];
+  }
+  if (c) {
+    uint32_t m = 1u;
+    for (int k = 0, n = len - e; n; k++, n >>= 1)
+      if (n & 1) m = ogg_mulmod(m, xpw[k]);
+    c = ogg_mulmod(c, m);
+  }
+  for (int o = 16; o; o >>= 1) c ^= __shfl_xor_sync(0xffffffffu, c, o);
+  return c;
+}
+
+__global__ void __launch_bounds__(32 * OGG_WARPS)
+k_ogg_demux(int nfiles, const uint8_t *__restrict__ bytes, const int64_t *__restrict__ file_off, int max_packets,
+            vb200_packet_info *__restrict__ info, int32_t *__restrict__ npkt_out, uint8_t *__restrict__ data,
+            vb200_ogg_stream *__restrict__ streams) {
+  __shared__ uint32_t crc_tab[256];
+  __shared__ uint32_t xpw[OGG_XPOW];
+  __shared__ uint8_t lace_all[OGG_WARPS][256];
+  ogg_crc_setup(crc_tab, xpw);
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
   const int f = blockIdx.x * OGG_WARPS + wib;
   if (f >= nfiles) return;
@@ -84,22 +110,7 @@ k_ogg_demux(int nfiles, const uint8_t *__restrict__ bytes, const int64_t *__rest
       }
       for (int o = 16; o; o >>= 1) body += __shfl_xor_sync(0xffffffffu, body, o);
       if (end - p < 27 + nseg + body) break;
-      const int len = 27 + nseg + body;
-      const int chunk = (len + 31) / 32;
-      const int a = min(lane * chunk, len), e = min(a + chunk, len);
-      uint32_t c = 0;
-      for (int i = a; i < e; i++) {
-        const uint32_t v = (i >= 22 && i < 26) ? 0u : pg[i];
-        c = (c << 8) ^ crc_tab[(c >> 24) ^ v];
-      }
-      if (c) {
-        uint32_t m = 1u;
-        for (int k = 0, n = len - e; n; k++, n >>= 1)
-          if (n & 1) m = ogg_mulmod(m, xpw[k]);
-        c = ogg_mulmod(c, m);
-      }
-      for (int o = 16; o; o >>= 1) c ^= __shfl_xor_sync(0xffffffffu, c, o);
-      ok = c == ogg_le32(pg + 22);
+      ok = ogg_page_crc(pg, 27 + nseg + body, lane, crc_tab, xpw) == ogg_le32(pg + 22);
     }
     if (!ok) {                                            // lose sync: resume at the next 'O'
       dropped++;

@@ -54,6 +54,7 @@ EXPORTS = [
     "vb200_ogg_demux_dev", "vb200_ogg_demux", "vb200_vorbis_window",
     "vb200_vorbis_headers_parse", "vb200_vorbis_headers_free",
     "vb200_ogg_group_scratch_bytes", "vb200_ogg_group_dev", "vb200_ogg_group",
+    "vb200_ogg_mux_dev", "vb200_ogg_mux",
     "vb200_malloc_device", "vb200_free_device", "vb200_memcpy_h2d", "vb200_memcpy_d2h", "vb200_synchronize",
 ]
 
@@ -196,6 +197,8 @@ def load():
     L.vb200_ogg_group_scratch_bytes.restype = C.c_size_t
     L.vb200_ogg_group_dev.argtypes = [C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp, vp, C.c_size_t, vp]
     L.vb200_ogg_group.argtypes = [C.c_int, vp, C.c_int64, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp]
+    L.vb200_ogg_mux_dev.argtypes = [C.c_int, vp, C.c_int64, vp, C.c_int, vp, vp, vp, vp, C.c_int64, vp, vp, vp]
+    L.vb200_ogg_mux.argtypes = [C.c_int, vp, C.c_int64, vp, C.c_int, vp, vp, vp, vp, C.c_int64, vp, vp]
     L.vb200_malloc_device.argtypes = [vp, C.c_size_t, C.POINTER(vp)]
     L.vb200_free_device.argtypes = [vp, vp]
     L.vb200_memcpy_h2d.argtypes = [vp, vp, vp, C.c_size_t]
@@ -1312,3 +1315,63 @@ def ogg_group_dev(nfiles, d_data, d_streams, max_packets, d_npkt, d_info, d_stat
     _check(L, L.vb200_ogg_group_dev(nfiles, _ptr(d_data), _ptr(d_streams), max_packets, _ptr(d_npkt), _ptr(d_info),
                                     _ptr(d_status), _ptr(d_order), _ptr(d_npkt_out), _ptr(d_info_out),
                                     _ptr(d_groups), _ptr(d_ngroups), _ptr(d_scratch), scratch_bytes, _ptr(stream)))
+
+
+# ---- Ogg Vorbis files out -----------------------------------------------------------------------------------
+def ogg_mux(packets, granules, eos=None, headers=None, serials=None, carries=None, hdr_granules=(0, 0, 0),
+            out_cap=None, check=True):
+    """vb200_ogg_mux on host lists, on the current CUDA device.  Per stream s: packets[s] (bytes; the carry's kept
+    packets first), granules[s] and eos[s] (default: e_o_s on the last packet), headers[s] (the three header packets,
+    needed for fresh carries), and either carries (OGG_MUX_CARRY_DTYPE [n], not modified) or serials (fresh carries).
+    Returns {"pages": per stream the bytes of this call's pages (the whole file for a fresh carry and an e_o_s packet),
+    "carry" (the new carries; the same as given unless rc is 0), "status", "out_off", "rc"}.  out_cap defaults to
+    what the pages need (a sizing call first)."""
+    L = load()
+    n = len(packets)
+    if carries is None:
+        carries = np.zeros(n, abi.OGG_MUX_CARRY_DTYPE)
+        carries["serial"] = serials
+    carry = np.ascontiguousarray(carries, abi.OGG_MUX_CARRY_DTYPE).copy()
+    if eos is None:
+        eos = [[k == len(p) - 1 for k in range(len(p))] for p in packets]
+    max_packets = max([1] + [len(p) for p in packets])
+    npkt = np.array([len(p) for p in packets], np.int32)
+    info = np.zeros((n, max_packets), abi.PACKET_INFO_DTYPE)
+    hdr = np.zeros((n, 3), abi.PACKET_INFO_DTYPE) if headers is not None else None
+    blobs, at = [], 0
+    for s in range(n):
+        if headers is not None:
+            for k, h in enumerate(headers[s]):
+                hdr[s, k] = (at, hdr_granules[k], len(h), 0, k, 0)
+                blobs.append(bytes(h))
+                at += len(h)
+        for k, p in enumerate(packets[s]):
+            info[s, k] = (at, granules[s][k], len(p), 1 if eos[s][k] else 0, 0, 0)
+            blobs.append(bytes(p))
+            at += len(p)
+    data = np.frombuffer(b"".join(blobs) + b"\0", np.uint8)
+    out_off = np.zeros(n + 1, np.int64)
+    status = np.zeros(max(n, 1), np.int32)
+
+    def call(out, cap, c):
+        return L.vb200_ogg_mux(n, _ptr(data), at, _ptr(hdr), max_packets, _ptr(npkt), _ptr(info), _ptr(c), _ptr(out),
+                               cap, _ptr(out_off), _ptr(status))
+    if out_cap is None:
+        call(None, 0, carry.copy())
+        out_cap = int(out_off[n])
+    out = np.zeros(max(out_cap, 1), np.uint8)
+    rc = call(out, out_cap, carry)
+    if check:
+        _check(L, rc)
+    fits = int(out_off[n]) <= out_cap
+    pages = [out[out_off[s]:out_off[s + 1]].tobytes() if fits else b"" for s in range(n)]
+    return {"pages": pages, "carry": carry, "status": status[:n], "out_off": out_off, "rc": rc}
+
+
+def ogg_mux_dev(nstreams, d_data, data_bytes, d_hdr, max_packets, d_npkt, d_info, d_carry, d_out, out_cap, d_out_off,
+                d_status, stream=None):
+    """vb200_ogg_mux_dev: device pointers (ints, e.g. torch tensors' data_ptr()), asynchronous on `stream`"""
+    L = load()
+    _check(L, L.vb200_ogg_mux_dev(nstreams, _ptr(d_data), data_bytes, _ptr(d_hdr), max_packets, _ptr(d_npkt),
+                                  _ptr(d_info), _ptr(d_carry), _ptr(d_out), out_cap, _ptr(d_out_off), _ptr(d_status),
+                                  _ptr(stream)))
