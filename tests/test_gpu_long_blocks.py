@@ -194,12 +194,12 @@ def test_encode_dsp_streams(cfg, W, fmt, monkeypatch):
 
 
 def test_encode_dsp_pipeline_forms(cfg, monkeypatch):
-    """the many-chunk host pipeline, device pointers and their errors, two concurrent half batches, int16 residue and
-    partition classes"""
-    for ramp in ("1", "0"):
-        P.test_encode_dsp_many_chunks(cfg, ramp, monkeypatch)
+    """the many-chunk host pipeline (ramped and flat chunk schedules), device pointers and their errors, two concurrent
+    half batches, int16 residue and partition classes"""
+    for ns in (30, 20):
+        P.test_encode_dsp_many_chunks(cfg, ns, monkeypatch)
     P.test_encode_dsp_device_pointers_and_errors(cfg)
-    P.test_encode_dsp_dev_split_half_batches(cfg, monkeypatch)
+    P.test_encode_dsp_dev_split_half_batches(cfg)
     for W in (0, 1):
         P.test_encode_dsp_int16_residue(cfg, W, monkeypatch)
     P.test_encode_dsp_with_classes(cfg, monkeypatch)

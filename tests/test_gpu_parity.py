@@ -4,7 +4,6 @@
 Bit-exact for every stage: the kernels execute the reference's arithmetic DAG with
 FMA contraction off (tolerance stated by north_star is 1e-4 relative; we hold 0)."""
 import ctypes as C
-import os
 
 import numpy as np
 import pytest
@@ -233,7 +232,8 @@ def test_decode_vs_oracle_random_streams(cfg):
 
 
 def test_phaseA_host_path_multichunk(cfg, monkeypatch):
-    """the pipelined two-lane host path (chunks alternate between two streams) == single chunk"""
+    """the pipelined two-lane host path (chunks alternate between two streams), without taps and with every tap
+    copied back chunk by chunk"""
     name, setup, ctx, o, enc, _ = cfg
     W = 0
     N, ch = setup.blocksize(W), setup.channels
@@ -245,10 +245,13 @@ def test_phaseA_host_path_multichunk(cfg, monkeypatch):
     desc["ampmax"] = -12.0
     monkeypatch.setenv("VB200_CHUNK_BLOCKS", "7")
     a = ctx.phaseA(W, pcm, desc)
+    at = ctx.phaseA(W, pcm, desc, taps=True)
     monkeypatch.delenv("VB200_CHUNK_BLOCKS")
-    b = o.phaseA(W, pcm, desc)
+    b = o.phaseA(W, pcm, desc, taps=True)
     for k in ("mdct", "logmdct", "logmask", "ampmax_out"):
         assert_bits_equal(a[k], b[k], "chunked " + k)
+    for k in ("mdct_raw", "logfft", "noise", "tone", "logmdct", "logmask", "mdct", "ampmax_out"):
+        assert_bits_equal(at[k], b[k], "chunked with taps " + k)
 
 
 def test_decouple_vs_oracle(cfg):
@@ -579,16 +582,16 @@ def test_encode_dsp_streams_vs_oracle(cfg, W, fmt, monkeypatch):
     assert not got["nonzero"][2 * bps:3 * bps].any(), "silent stream must come back all-zero"
 
 
-@pytest.mark.parametrize("ramp", ["1", "0"])
-def test_encode_dsp_many_chunks(cfg, ramp, monkeypatch):
+@pytest.mark.parametrize("ns", [30, 20])
+def test_encode_dsp_many_chunks(cfg, ns, monkeypatch):
     """the host-buffer pipeline of vb200_encode_dsp with more chunks than buffer sets (the event chain
-    H2D(k) -> kernels(k) -> D2H(k) -> H2D(k+4) is exercised) and the ramped chunk schedule on and off"""
+    H2D(k) -> kernels(k) -> D2H(k) -> H2D(k+4) is exercised), at 4 streams per chunk: 30 streams take the ramped
+    chunk schedule (10 chunks), 20 streams the flat one (5 chunks)"""
     name, setup, ctx, o, _, _ = cfg
     monkeypatch.setenv("VB200_CHUNK_BLOCKS", "12")
-    monkeypatch.setenv("VB200_CHUNK_RAMP", ramp)
     W = 1
     N, ch = setup.blocksize(W), setup.channels
-    hop, ns, bps = N // 2, 30, 3
+    hop, bps = N // 2, 3
     stride = (bps - 1) * hop + N
     rng = np.random.default_rng(4242)
     s16 = np.clip(6000 * rng.standard_normal((ns, stride, ch)) * rng.uniform(0.05, 1.2, (ns, 1, 1)), -32768, 32767).astype(np.int16)
@@ -602,7 +605,7 @@ def test_encode_dsp_many_chunks(cfg, ramp, monkeypatch):
     for rep in range(2):                                             # the second call reuses the buffer sets
         got = ctx.encode_dsp(W, s16, desc, nstreams=ns, fmt=vlib.PCM_S16_INTERLEAVED, hop=hop, ampmax0=amp0,
                              independent=False)
-        _enc_compare(got, want, "many chunks ramp=%s rep=%d" % (ramp, rep))
+        _enc_compare(got, want, "many chunks ns=%d rep=%d" % (ns, rep))
 
 
 @pytest.mark.parametrize("fmt", ["s16", "blocks"])
@@ -877,15 +880,14 @@ def test_encode_dsp_with_classes(cfg, monkeypatch):
         assert np.array_equal(got["classes"], wcls)
 
 
-def test_encode_dsp_dev_split_half_batches(cfg, monkeypatch):
-    """vb200_encode_dsp_dev run as two concurrent half-batches (VB200_SPLIT=2): same results"""
+def test_encode_dsp_dev_split_half_batches(cfg):
+    """vb200_encode_dsp_dev from 2048 blocks up runs as two concurrent half-batches of whole streams (here 341 and
+    342 streams of 3 blocks): int16 stream PCM in, the partition classes out, same results"""
     import torch
     name, setup, ctx, o, _, _ = cfg
-    monkeypatch.setenv("VB200_SPLIT", os.environ.get("VB200_TEST_SPLIT", "2"))
-    monkeypatch.setenv("VB200_SPLIT_MIN", "1")
     W = 1
     N, ch = setup.blocksize(W), setup.channels
-    n, hop, ns, bps = N // 2, N // 2, 5, 3
+    n, hop, ns, bps = N // 2, N // 2, 683, 3
     stride = (bps - 1) * hop + N
     rng = np.random.default_rng(31)
     s16 = np.clip(7000 * rng.standard_normal((ns, stride, ch)), -32768, 32767).astype(np.int16)

@@ -91,7 +91,8 @@ struct vb200_ctx {
   //   stage[]   HostIO: the device copies of a host form's inputs and outputs; nothing else uses it
   //   cycles    the debug cycle counters (VB200_PHASE_TIMING, VB200_FLOOR1_TIMING), kept between calls
   //   phaseA    phaseA_dev_common: log spectrum, row and block maxima
-  //   lane[]    the pipelined host vb200_analysis_phaseA, one per lane
+  //   lane[]    the host vb200_analysis_phaseA, one per lane: a chunk's copies, its intermediates and the taps
+  //             the caller asks for
   //   enc       the encode chain of vb200_encode_dsp_dev and vb200_encode_packets
   //   set[]     the pipelined host vb200_encode_dsp, one per buffer set: a chunk's copies and its chain
   //   mgd       vb200_encode_dsp_managed_dev
@@ -125,8 +126,7 @@ struct vb200_ctx {
   cudaStream_t s_enc[3] = {nullptr, nullptr, nullptr};   // compute 0, compute 1, host->device
   cudaStream_t s_d2h = nullptr;
   cudaEvent_t ev_h2d[ENC_SETS] = {}, ev_cmp[ENC_SETS] = {}, ev_d2h[ENC_SETS] = {};
-  int psy_ctas_per_sm = 5;
-  int psy_carveout_ctas = -1;        // CTAs/SM the generic psy kernel's shared-memory carve-out was last set for (per device)
+  bool psy_carveout_set = false;     // the generic psy kernel's shared-memory carve-out is set for this context
   // The *_dev entry points keep their intermediates in per-context scratch: two calls in flight on different
   // user streams would share it.  Every such call waits for the previous one's event and records its own.
   cudaEvent_t ev_scratch = nullptr;
@@ -1080,9 +1080,7 @@ k_decouple(int n, int ch, int steps, const int *__restrict__ mag, const int *__r
 // ======================================================================== //
 // launch helpers
 static int threads_for(int N) {
-  int div = 8;
-  { const char *e = getenv("VB200_XF_DIV"); if (e && atoi(e) > 0) div = atoi(e); }
-  int t = N / div;
+  int t = N / 8;
   if (t < 64) t = 64;
   if (t > 256) t = 256;
   return t;
@@ -1352,6 +1350,8 @@ static int phaseA_transform_launch(vb200_ctx *c, int W, int nblocks, const vb200
   return 0;
 }
 
+constexpr int PSY_CTAS_PER_SM = 5;   // the generic psy kernel's grid, and the CTAs its carve-out leaves room for
+
 // stage 3: noise / tone masks + mix of `nblocks` blocks of size W, given every block's global ampmax
 static int phaseA_psy_launch(vb200_ctx *c, int W, int nblocks, const vb200_phaseA_io *io, cudaStream_t st,
                              float *d_logfft, float *d_lmax, float *d_gmax) {
@@ -1361,21 +1361,15 @@ static int phaseA_psy_launch(vb200_ctx *c, int W, int nblocks, const vb200_phase
   const int total = P0.total > P1.total ? P0.total : P1.total;
   const int nruns = P0.nruns > P1.nruns ? P0.nruns : P1.nruns;
   const int ngrp = P0.ngrp > P1.ngrp ? P0.ngrp : P1.ngrp;
-  const char *ectas = getenv("VB200_PSY_CTAS");
   const size_t smem = psy_smem_bytes(P0, P1);
   int rc = set_smem(k_phaseA_psy, smem); if (rc) return rc;
-  {
+  if (!c->psy_carveout_set) {
     // leave the rest of the 256 KB unified array to L1: the static psy tables (~60 KB per look)
     // are read through it on every row
-    int &tuned = c->psy_carveout_ctas;
-    const int ctas = ectas ? atoi(ectas) : c->psy_ctas_per_sm;
-    if (tuned != ctas) {
-      int pct = (int)((ctas * (smem + 1024) * 100 + 228 * 1024 - 1) / (228 * 1024));
-      if (pct > 100) pct = 100;
-      CU(cudaFuncSetAttribute(k_phaseA_psy, cudaFuncAttributePreferredSharedMemoryCarveout, pct));
-      tuned = ctas;
-    }
-    c->psy_ctas_per_sm = ctas;
+    int pct = (int)((PSY_CTAS_PER_SM * (smem + 1024) * 100 + 228 * 1024 - 1) / (228 * 1024));
+    if (pct > 100) pct = 100;
+    CU(cudaFuncSetAttribute(k_phaseA_psy, cudaFuncAttributePreferredSharedMemoryCarveout, pct));
+    c->psy_carveout_set = true;
   }
   PsyArgs A;
   A.mdct_in = io->tap_mdct_raw ? io->tap_mdct_raw : io->mdct;
@@ -1396,7 +1390,6 @@ static int phaseA_psy_launch(vb200_ctx *c, int W, int nblocks, const vb200_phase
     int ctas = (int)((227 * 1024) / (smem3 + 1024));
     if (ctas > PSY3_MINB / R) ctas = PSY3_MINB / R;
     if (ctas < 1) ctas = 1;
-    if (ectas) ctas = atoi(ectas);
     const bool dbg3 = A.dbg_cycles || A.tap_noise || A.tap_tone;   // clock marks / taps: the debug instance
 #define LAUNCH_PSY3D(KK, DD)                                                                       \
     do {                                                                                           \
@@ -1414,7 +1407,7 @@ static int phaseA_psy_launch(vb200_ctx *c, int W, int nblocks, const vb200_phase
 #undef LAUNCH_PSY3D
 #undef LAUNCH_PSY3
   } else {
-    k_phaseA_psy<<<grid_for(c, rows, c->psy_ctas_per_sm), PSY_THREADS, smem, st>>>(P0, P1, ch, rows, A);
+    k_phaseA_psy<<<grid_for(c, rows, PSY_CTAS_PER_SM), PSY_THREADS, smem, st>>>(P0, P1, ch, rows, A);
   }
   return post_launch(c);
 }
@@ -1493,20 +1486,27 @@ extern "C" int vb200_analysis_phaseA_streams_dev(vb200_ctx *c, int W, int nstrea
   return phaseA_dev_common(c, W, nstreams * bps, io, nstreams, bps, d_amp0, stream);
 }
 
-// Host-buffer Phase A.  Without taps the batch is cut into chunks that alternate between two
-// lanes (stream + device buffers each): while one lane computes, the other lane's H2D / D2H
-// copies run on the copy engines.  Pinned host memory is needed for the copies to be truly
-// asynchronous (pageable memory still works, staged by the driver).
-static int phaseA_host_pipelined(vb200_ctx *c, int W, int nblocks, const vb200_phaseA_io *h) {
+// Host-buffer Phase A.  The batch is cut into chunks that alternate between two lanes (stream + device buffers
+// each): while one lane computes, the other lane's H2D / D2H copies run on the copy engines.  Pinned host memory is
+// needed for the copies to be truly asynchronous (pageable memory still works, staged by the driver).  With
+// profiling on, the whole batch is one chunk, so that vb200_phaseA_kernel_ms brackets the whole call.
+extern "C" int vb200_analysis_phaseA(vb200_ctx *c, int W, int nblocks, const vb200_phaseA_io *h) {
+  CHECK_CTX(c); CHECK_W(W);
+  if (!h) return fail(VB200_EINVAL, "null io");
+  if (c->n_psy != 4) return fail(VB200_EIMPL, "context has no psy lookups");
+  if (!h->pcm || !h->desc || !h->mdct || !h->logmdct || !h->logmask || !h->ampmax_out)
+    return fail(VB200_EINVAL, "phase A io pointers");
+  if (nblocks <= 0) return 0;
+  std::lock_guard<std::mutex> lk(c->mu);
   const int ch = c->setup.channels, N = c->dx[W].N, n = N / 2;
   int chunk = 4096;
   { const char *e = getenv("VB200_CHUNK_BLOCKS"); if (e && atoi(e) > 0) chunk = atoi(e); }
-  if (chunk > nblocks) chunk = nblocks;
+  if (chunk > nblocks || c->profiling) chunk = nblocks;
   const size_t crow = (size_t)chunk * ch;
   int rc;
   vb200_phaseA_io lane[2];
   float *logfft[2], *lmax[2], *gmax[2];
-  for (int L = 0; L < 2; L++) {
+  for (int L = 0; L < (chunk < nblocks ? 2 : 1); L++) {
     vb200_phaseA_io &d = lane[L];
     memset(&d, 0, sizeof(d));
     if ((rc = carve(c->lane[L], [&](Carve &k) {
@@ -1514,6 +1514,9 @@ static int phaseA_host_pipelined(vb200_ctx *c, int W, int nblocks, const vb200_p
            d.mdct = k.take<float>(crow * n); d.logmdct = k.take<float>(crow * n); d.logmask = k.take<float>(crow * n);
            d.ampmax_out = k.take<float>(chunk);
            logfft[L] = k.take<float>(crow * n); lmax[L] = k.take<float>(crow); gmax[L] = k.take<float>(chunk);
+           d.tap_noise = h->tap_noise ? k.take<float>(crow * n) : nullptr;
+           d.tap_tone = h->tap_tone ? k.take<float>(crow * n) : nullptr;
+           d.tap_mdct_raw = h->tap_mdct_raw ? k.take<float>(crow * n) : nullptr;
          }))) return rc;
   }
   for (int b0 = 0, it = 0; b0 < nblocks; b0 += chunk, it++) {
@@ -1524,52 +1527,17 @@ static int phaseA_host_pipelined(vb200_ctx *c, int W, int nblocks, const vb200_p
     CU(cudaMemcpyAsync((void *)d.pcm, h->pcm + r0 * N, sizeof(float) * rows * N, cudaMemcpyHostToDevice, st));
     CU(cudaMemcpyAsync((void *)d.desc, h->desc + b0, sizeof(vb200_block_desc) * nb, cudaMemcpyHostToDevice, st));
     if ((rc = phaseA_launch(c, W, nb, &d, 0, 0, nullptr, st, logfft[L], lmax[L], gmax[L]))) return rc;
-    CU(cudaMemcpyAsync(h->mdct + r0 * n, d.mdct, sizeof(float) * rows * n, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(h->logmdct + r0 * n, d.logmdct, sizeof(float) * rows * n, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(h->logmask + r0 * n, d.logmask, sizeof(float) * rows * n, cudaMemcpyDeviceToHost, st));
+    // the spectra and the taps asked for; the lane's logfft is the logfft tap
+    const std::pair<float *, const float *> spectra[] = {
+        {h->mdct, d.mdct}, {h->logmdct, d.logmdct}, {h->logmask, d.logmask}, {h->tap_noise, d.tap_noise},
+        {h->tap_tone, d.tap_tone}, {h->tap_logfft, logfft[L]}, {h->tap_mdct_raw, d.tap_mdct_raw}};
+    for (const auto &s : spectra)
+      if (s.first) CU(cudaMemcpyAsync(s.first + r0 * n, s.second, sizeof(float) * rows * n, cudaMemcpyDeviceToHost, st));
     CU(cudaMemcpyAsync(h->ampmax_out + b0, d.ampmax_out, sizeof(float) * nb, cudaMemcpyDeviceToHost, st));
   }
   CU(cudaStreamSynchronize(c->s_pipe[0]));
   CU(cudaStreamSynchronize(c->s_pipe[1]));
   return 0;
-}
-
-extern "C" int vb200_analysis_phaseA(vb200_ctx *c, int W, int nblocks, const vb200_phaseA_io *h) {
-  CHECK_CTX(c); CHECK_W(W);
-  if (!h) return fail(VB200_EINVAL, "null io");
-  if (c->n_psy != 4) return fail(VB200_EIMPL, "context has no psy lookups");
-  if (!h->pcm || !h->desc || !h->mdct || !h->logmdct || !h->logmask || !h->ampmax_out)
-    return fail(VB200_EINVAL, "phase A io pointers");
-  if (nblocks <= 0) return 0;
-  std::lock_guard<std::mutex> lk(c->mu);
-  if (!h->tap_noise && !h->tap_tone && !h->tap_logfft && !h->tap_mdct_raw && !c->profiling)
-    return phaseA_host_pipelined(c, W, nblocks, h);
-  const int ch = c->setup.channels, N = c->dx[W].N, n = N / 2;
-  const size_t rows = (size_t)nblocks * ch;
-  HostIO io{c};
-  vb200_phaseA_io d;
-  memset(&d, 0, sizeof(d));
-  void *p; int rc;
-  if ((rc = io.h2d(h->pcm, sizeof(float) * rows * N, &p))) return rc; d.pcm = (const float *)p;
-  if ((rc = io.h2d(h->desc, sizeof(vb200_block_desc) * nblocks, &p))) return rc; d.desc = (const vb200_block_desc *)p;
-  if ((rc = io.h2d(nullptr, sizeof(float) * rows * n, &p))) return rc; d.mdct = (float *)p;
-  if ((rc = io.h2d(nullptr, sizeof(float) * rows * n, &p))) return rc; d.logmdct = (float *)p;
-  if ((rc = io.h2d(nullptr, sizeof(float) * rows * n, &p))) return rc; d.logmask = (float *)p;
-  if ((rc = io.h2d(nullptr, sizeof(float) * nblocks, &p))) return rc; d.ampmax_out = (float *)p;
-  if (h->tap_noise) { if ((rc = io.h2d(nullptr, sizeof(float) * rows * n, &p))) return rc; d.tap_noise = (float *)p; }
-  if (h->tap_tone) { if ((rc = io.h2d(nullptr, sizeof(float) * rows * n, &p))) return rc; d.tap_tone = (float *)p; }
-  if (h->tap_logfft) { if ((rc = io.h2d(nullptr, sizeof(float) * rows * n, &p))) return rc; d.tap_logfft = (float *)p; }
-  if (h->tap_mdct_raw) { if ((rc = io.h2d(nullptr, sizeof(float) * rows * n, &p))) return rc; d.tap_mdct_raw = (float *)p; }
-  if ((rc = phaseA_dev_common(c, W, nblocks, &d, 0, 0, nullptr, c->s_main))) return rc;
-  if ((rc = io.d2h(h->mdct, d.mdct, sizeof(float) * rows * n))) return rc;
-  if ((rc = io.d2h(h->logmdct, d.logmdct, sizeof(float) * rows * n))) return rc;
-  if ((rc = io.d2h(h->logmask, d.logmask, sizeof(float) * rows * n))) return rc;
-  if ((rc = io.d2h(h->ampmax_out, d.ampmax_out, sizeof(float) * nblocks))) return rc;
-  if (h->tap_noise && (rc = io.d2h(h->tap_noise, d.tap_noise, sizeof(float) * rows * n))) return rc;
-  if (h->tap_tone && (rc = io.d2h(h->tap_tone, d.tap_tone, sizeof(float) * rows * n))) return rc;
-  if (h->tap_logfft && (rc = io.d2h(h->tap_logfft, d.tap_logfft, sizeof(float) * rows * n))) return rc;
-  if (h->tap_mdct_raw && (rc = io.d2h(h->tap_mdct_raw, d.tap_mdct_raw, sizeof(float) * rows * n))) return rc;
-  return io.sync();
 }
 
 // ======================================================================== //
@@ -2100,29 +2068,17 @@ extern "C" int vb200_encode_dsp_dev(vb200_ctx *c, int W, int nstreams, int bps, 
   // Two half-batches (whole streams each) on two internal streams, every kernel launched with half its
   // grid: the halves drift apart, so CTAs of different kernels (shared-memory bound transform, issue bound
   // psy, latency bound floor fit) share the SMs instead of one kernel type owning the machine at a time.
-  int split = 2;                      // H100 80GB HBM3 at a 400 W limit: 1 and 2 within noise (5.45 / 5.47 M blocks/s)
-  { const char *e = getenv("VB200_SPLIT"); if (e) split = atoi(e); }
-  size_t split_min = 2048;
-  { const char *e = getenv("VB200_SPLIT_MIN"); if (e && atoi(e) > 0) split_min = (size_t)atoi(e); }
+  // H100 80GB HBM3 at a 700 W limit, 100 000 blocks: 6.27-6.28 M blocks/s split, 6.17-6.18 M in one piece.
   if ((rc = scratch_begin(c, (cudaStream_t)stream))) return rc;
-  if (split < 2 || nstreams < 2 || c->profiling || nblocks < split_min) {
+  if (nstreams < 2 || c->profiling || nblocks < 2048) {
     if ((rc = encode_launch(c, W, nstreams, bps, blobno, d, S, (cudaStream_t)stream))) return rc;
     return scratch_end(c, (cudaStream_t)stream);
   }
   cudaStream_t user = (cudaStream_t)stream;
   CU(cudaEventRecord(c->ev_fork, user));
-  // pieces: (internal stream, share of the streams).  split 2: two halves.  split 4: four pieces on the
-  // two streams, 20/30 % then 30/20 %, so that the two streams are always at different kernels.
-  int npieces = 2, pst[4] = {0, 1, 0, 1}, share[4] = {50, 50, 0, 0};
-  if (split >= 4 && nstreams >= 8) { npieces = 4; share[0] = 20; share[1] = 30; share[2] = 30; share[3] = 20; }
-  { const char *e = getenv("VB200_SPLIT_SKEW"); if (e && atoi(e) > 0 && atoi(e) < 50 && npieces == 4) {
-      share[0] = atoi(e); share[1] = 50 - share[0]; share[2] = share[1]; share[3] = share[0]; } }
   c->grid_div = 2;
-  int s0 = 0;
-  for (int pc = 0; pc < npieces; pc++) {
-    int ns = pc == npieces - 1 ? nstreams - s0 : (int)((long)nstreams * share[pc] / 100);
-    if (ns < 1) ns = 1;
-    if (s0 + ns > nstreams - (npieces - 1 - pc)) ns = nstreams - (npieces - 1 - pc) - s0;
+  for (int k = 0, s0 = 0; k < 2; k++) {
+    const int ns = k ? nstreams - s0 : nstreams / 2;
     const size_t b0 = (size_t)s0 * bps, r0 = b0 * ch;
     vb200_encode_io h = *d;
     EncScratch T = S;
@@ -2136,9 +2092,8 @@ extern "C" int vb200_encode_dsp_dev(vb200_ctx *c, int W, int nstreams, int bps, 
     T.mdct += r0 * n; T.logmdct += r0 * n; T.logmask += r0 * n; T.logfft += r0 * n;
     T.lmax += r0; T.gmax += b0; T.fitnz += r0;
     if (T.iw32) T.iw32 += r0 * n;
-    cudaStream_t st = c->s_split[pst[pc]];
-    cudaError_t e = pc < 2 ? cudaStreamWaitEvent(st, c->ev_fork, 0) : cudaSuccess;
-    if (e == cudaSuccess) rc = encode_launch(c, W, ns, bps, blobno, &h, T, st);
+    cudaError_t e = cudaStreamWaitEvent(c->s_split[k], c->ev_fork, 0);
+    if (e == cudaSuccess) rc = encode_launch(c, W, ns, bps, blobno, &h, T, c->s_split[k]);
     if (rc || e != cudaSuccess) { c->grid_div = 1; return rc ? rc : fail(VB200_EFAULT, "encode split", e); }
     s0 += ns;
   }
@@ -2213,13 +2168,11 @@ extern "C" int vb200_encode_dsp(vb200_ctx *c, int W, int nstreams, int bps, int 
   const size_t pcm_per_stream = enc_pcm_bytes(h, ch, N, 1, bps);
   // Chunk schedule: the pipeline's fill (first H2D + first kernels before anything overlaps) and drain (last kernels
   // + last D2H) are exposed, so the first and the last chunks are small (cs/4, cs/2) and the middle ones full size.
-  int ramp = 1;
-  { const char *e = getenv("VB200_CHUNK_RAMP"); if (e) ramp = atoi(e); }
   std::vector<int> sched;
   {
     int left = nstreams;
     const int q = cs / 4 > 0 ? cs / 4 : 1, hlf = cs / 2 > 0 ? cs / 2 : 1;
-    if (ramp && nstreams >= 6 * cs) {
+    if (nstreams >= 6 * cs) {
       const int head[2] = {q, hlf};
       for (int k = 0; k < 2; k++) { sched.push_back(head[k]); left -= head[k]; }
       const int tail = q + hlf;
