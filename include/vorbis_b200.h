@@ -803,7 +803,8 @@ int vb200_decode_ranges    (vb200_ctx*, int nstreams, int max_packets, const int
  *   Stream.  The first captured page with the BOS flag, version 0 and a first packet that begins "\x01vorbis" fixes
  *     `serial`.  Before it, and after it for pages of other serials or a version other than 0, pages are skipped and
  *     counted in `foreign`.  The walk ends after that serial's EOS page; `chained` = 1 when the next captured page has
- *     the BOS flag.  Links after the first are not read.
+ *     the BOS flag.  Links after the first are not read: vb200_ogg_links[_dev] below finds every link, and its link_off
+ *     passed here as file_off demuxes one link per row.
  *   Packets.  Lacing value 255 continues a packet.  A page sequence number other than the previous page's plus one
  *     drops the pending partial packet and leaves one hole: packetno advances by one with no packet.  A continued page
  *     with nothing pending skips its leading fragment.  A page without the continued flag while a partial packet is
@@ -844,6 +845,47 @@ int vb200_ogg_demux_dev(int nfiles, const uint8_t *d_bytes, const int64_t *d_fil
                         void *stream);
 int vb200_ogg_demux    (int nfiles, const uint8_t *bytes, const int64_t *file_off, int max_packets,
                         struct vb200_packet_info *info, int32_t *npkt, uint8_t *data, vb200_ogg_stream *streams);
+
+/* ---- chained Ogg files: the links of many files on the device, in one call.  No context.  A chained file is complete
+ * Ogg Vorbis streams ("links") one after another: a radio capture with a link per track, `cat a.ogg b.ogg`.
+ * Input: bytes and file_off as vb200_ogg_demux takes them.
+ * Rule, per file: walk the captured pages exactly as vb200_ogg_demux does (capture pattern, CRC, resync at the next
+ * 'O', the end-of-file rules).  A link starts at the file's first byte, and at every captured page that has the BOS
+ * flag and follows a captured page without it.  Link k is the bytes from its start to the start of link k+1, or to the
+ * end of the file.  So:
+ *   - every file has at least one link; a file with no captured page is one link, which the demux reports
+ *     VB200_ENOTVORBIS;
+ *   - the BOS pages of a multiplexed link all come first (RFC 3533), so a Vorbis + Theora link is one link and the
+ *     demux takes its first Vorbis BOS page;
+ *   - any BOS page after a data page starts a new link, as in vorbisfile's streaming read, even when the link before
+ *     has no EOS page (a truncated track); failed captures and foreign pages between an EOS page and the next BOS page
+ *     belong to the earlier link;
+ *   - a BOS page with the same serial as the link before also starts a new link.  This departs from vorbisfile on
+ *     purpose: its streaming read feeds such a page to the running stream as a hole, and its seekable open reads the
+ *     whole file as one link; both hand the second copy's header packets to vorbis_synthesis.  RFC 3533 says a BOS page
+ *     begins a new logical stream, and `cat` of two files from an encoder with a fixed serial is the case users meet;
+ *   - a failed capture can end a link's demux early: where a failed capture's claimed extent (header, lacing table
+ *     and lacing sum) crosses the next link's start, the demux of the earlier link takes it as a page cut short by the
+ *     end of the file and its walk ends there, where the walk of the whole file fails the CRC, resyncs and still finds
+ *     any valid pages before the boundary.  Only damaged bytes just before a boundary do this.
+ * Output:
+ *   link_first [nfiles+1]  always written: file f's links are rows link_first[f] .. link_first[f+1]; link_first[nfiles]
+ *                      is the total.
+ *   link_off [total+1]     written only when total <= link_cap (so link_cap = 0, link_off NULL, sizes a call):
+ *                      link_off[link_first[f]] = file_off[f], link_off[total] = file_off[nfiles], every other entry the
+ *                      byte offset of a link's first page.  It is a file_off: vb200_ogg_demux[_dev](total, bytes,
+ *                      link_off, ..) gives one row per link, which vb200_ogg_group and the decode calls take unchanged
+ *                      (links of one setup form one group whatever their comment headers; a chain whose setup changes
+ *                      gives a group per setup).  File f's PCM is its links' outputs in row order.
+ * Three kernel launches whatever nfiles is (count, offsets, write; one warp per file walks its pages with the demux's
+ * lane split of the lacing sum and CRC, and copies no body); no device scratch.
+ * _dev: device pointers, asynchronous on `stream`; checks its pointers, nfiles >= 0 and link_cap >= 0 only.  Host form:
+ * host buffers, on the current CUDA device; also checks file_off (non-decreasing from >= 0), and returns VB200_EINVAL
+ * when link_cap is below the total (link_first is written, link_off is not).                                        */
+int vb200_ogg_links_dev(int nfiles, const uint8_t *d_bytes, const int64_t *d_file_off, int64_t *d_link_first,
+                        int64_t *d_link_off, int64_t link_cap, void *stream);
+int vb200_ogg_links    (int nfiles, const uint8_t *bytes, const int64_t *file_off, int64_t *link_first,
+                        int64_t *link_off, int64_t link_cap);
 
 /* The rising half window of an n-sample block as the reference tabulates it (lib/window.c vwin64 .. vwin8192): out[i] =
  * sin(.5*pi*sin^2((i+.5)/n*pi)) evaluated in double, printed with "%.10f" and read back with strtof, for i < n/2.

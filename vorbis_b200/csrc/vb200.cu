@@ -4547,6 +4547,61 @@ extern "C" int vb200_ogg_demux(int nfiles, const uint8_t *bytes, const int64_t *
   return 0;
 }
 
+// the links of chained files (k_ogg_links_* in vb200_ogg.cuh)
+extern "C" int vb200_ogg_links_dev(int nfiles, const uint8_t *d_bytes, const int64_t *d_file_off, int64_t *d_link_first,
+                                   int64_t *d_link_off, int64_t link_cap, void *stream) {
+  if (nfiles < 0 || link_cap < 0) return fail(VB200_EINVAL, "ogg_links: nfiles < 0 or link_cap < 0");
+  if (!d_file_off || !d_link_first || (link_cap && !d_link_off)) return fail(VB200_EINVAL, "ogg_links: null pointer");
+  cudaStream_t st = (cudaStream_t)stream;
+  if (nfiles == 0) {
+    CU(cudaMemsetAsync(d_link_first, 0, sizeof(int64_t), st));
+    if (d_link_off) CU(cudaMemcpyAsync(d_link_off, d_file_off, sizeof(int64_t), cudaMemcpyDeviceToDevice, st));
+    return 0;
+  }
+  if (!d_bytes) return fail(VB200_EINVAL, "ogg_links: null pointer");
+  long long *first = (long long *)d_link_first;
+  const int grid = (nfiles + OGG_WARPS - 1) / OGG_WARPS;
+  k_ogg_links_count<<<grid, 32 * OGG_WARPS, 0, st>>>(nfiles, d_bytes, d_file_off, first);
+  k_ds_scan<<<1, 1024, 0, st>>>(nfiles, first);
+  k_ogg_links_write<<<grid, 32 * OGG_WARPS, 0, st>>>(nfiles, d_bytes, d_file_off, first, d_link_off, link_cap);
+  CU(cudaGetLastError());
+  return 0;
+}
+
+extern "C" int vb200_ogg_links(int nfiles, const uint8_t *bytes, const int64_t *file_off, int64_t *link_first,
+                               int64_t *link_off, int64_t link_cap) {
+  if (nfiles < 0 || link_cap < 0) return fail(VB200_EINVAL, "ogg_links: nfiles < 0 or link_cap < 0");
+  if (!file_off || !link_first || (link_cap && !link_off)) return fail(VB200_EINVAL, "ogg_links: null pointer");
+  if (file_off[0] < 0) return fail(VB200_EINVAL, "ogg_links: file_off[0] < 0");
+  for (int f = 0; f < nfiles; f++)
+    if (file_off[f + 1] < file_off[f]) return fail(VB200_EINVAL, "ogg_links: file_off decreases");
+  const size_t total = (size_t)file_off[nfiles];
+  if (total && !bytes) return fail(VB200_EINVAL, "ogg_links: null pointer");
+  link_first[0] = 0;
+  if (nfiles == 0) {
+    if (link_off) link_off[0] = file_off[0];
+    return 0;
+  }
+  // every link after a file's first starts at a captured page of 27 bytes or more: the device table needs no more rows
+  const int64_t cap = std::min<int64_t>(link_cap, nfiles + (int64_t)(total / 27));
+  DevBuf buf;                                             // freed on return
+  uint8_t *db;
+  int64_t *doff, *dfirst, *dlinks;
+  int rc = carve(buf, [&](Carve &c) {
+    db = c.take<uint8_t>(total); doff = c.take<int64_t>(nfiles + 1); dfirst = c.take<int64_t>(nfiles + 1);
+    dlinks = c.take<int64_t>((size_t)cap + 1);
+  });
+  if (rc) return rc;
+  if (total) CU(cudaMemcpy(db, bytes, total, cudaMemcpyHostToDevice));
+  CU(cudaMemcpy(doff, file_off, sizeof(int64_t) * (nfiles + 1), cudaMemcpyHostToDevice));
+  if ((rc = vb200_ogg_links_dev(nfiles, db, doff, dfirst, dlinks, cap, nullptr))) return rc;
+  CU(cudaMemcpy(link_first, dfirst, sizeof(int64_t) * (nfiles + 1), cudaMemcpyDeviceToHost));
+  const int64_t links = link_first[nfiles];
+  if (links > link_cap) return fail(VB200_EINVAL, "ogg_links: link_cap below the link count");
+  CU(cudaMemcpy(link_off, dlinks, sizeof(int64_t) * (links + 1), cudaMemcpyDeviceToHost));
+  return 0;
+}
+
 extern "C" int vb200_vorbis_window(int n, float *out) {
   if (n < 64 || n > 8192 || !pow2(n) || !out) return fail(VB200_EINVAL, "vorbis_window: n must be 64, 128, .. 8192");
   vbh::window(n, out);

@@ -12,6 +12,12 @@
 //                 their loads one after another.  A failed capture looks for the next 'O' 32 bytes at a time with a ballot.  An accepted
 //                 page of the stream has its kept body copied by all lanes; the packet walk over the lacing values is
 //                 done by every lane alike and lane 0 writes the records.
+// and the link table of vb200_ogg_links[_dev]: three launches whatever nfiles is, one warp per file in the walks.
+//   k_ogg_links_count  walks the file's captured pages as k_ogg_demux does (ogg_capture: capture pattern, the lanes'
+//                      lacing sum and CRC split, the ballot resync) and counts the link starts into link_first[f + 1];
+//                      k_ds_scan (vb200_decode_streams.cuh) turns the counts into offsets.
+//   k_ogg_links_write  once the total fits link_cap, walks again and writes the file's link offsets from
+//                      link_first[f] on.  Neither copies a page body.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -68,6 +74,39 @@ __device__ __forceinline__ uint32_t ogg_page_crc(const uint8_t *pg, int len, int
   }
   for (int o = 16; o; o >>= 1) c ^= __shfl_xor_sync(0xffffffffu, c, o);
   return c;
+}
+
+// ogg_sync_pageseek at byte p of a file that ends at `end`, by one converged warp, as k_ogg_demux captures.  Returns
+// the captured page's length, 0 when the capture failed (p then moved to the next 'O' after it, or to end), or -1 when
+// fewer than 27 bytes are left or the page is cut short by the end of the file.  k_ogg_demux keeps this step written
+// out in its loop, because it stages the lacing table on the way: called from there, this function changes that
+// kernel's register allocation, so its SASS would not stay as it was.  The tests hold this step to oracle/ogg_links.py
+// and the demux's copy to oracle/ogg.py, which capture pages alike.
+__device__ __forceinline__ int ogg_capture(const uint8_t *bytes, int64_t &p, int64_t end, int lane,
+                                           const uint32_t *crc_tab, const uint32_t *xpw) {
+  if (end - p < 27) return -1;
+  const uint8_t *pg = bytes + p;
+  bool ok = pg[0] == 'O' && pg[1] == 'g' && pg[2] == 'g' && pg[3] == 'S';
+  int len = 0;
+  if (ok) {
+    const int nseg = pg[26];
+    if (end - p < 27 + nseg) return -1;
+    int body = 0;
+    for (int i = lane; i < nseg; i += 32) body += pg[27 + i];
+    for (int o = 16; o; o >>= 1) body += __shfl_xor_sync(0xffffffffu, body, o);
+    len = 27 + nseg + body;
+    if (end - p < len) return -1;
+    ok = ogg_page_crc(pg, len, lane, crc_tab, xpw) == ogg_le32(pg + 22);
+  }
+  if (ok) return len;
+  int64_t q = end;                                        // lose sync: resume at the next 'O'
+  for (int64_t b = p + 1; b < end; b += 32) {
+    const int64_t i = b + lane;
+    const unsigned m = __ballot_sync(0xffffffffu, i < end && bytes[i] == 'O');
+    if (m) { q = b + __ffs(m) - 1; break; }
+  }
+  p = q;
+  return 0;
 }
 
 __global__ void __launch_bounds__(32 * OGG_WARPS)
@@ -214,4 +253,62 @@ k_ogg_demux(int nfiles, const uint8_t *__restrict__ bytes, const int64_t *__rest
     streams[f] = o;
     npkt_out[f] = status == VB200_EBADHEADER ? 0 : np;
   }
+}
+
+// The link starts of one file after its first byte, by one converged warp: at(offset) for every captured page with
+// the BOS flag that follows a captured page without it (rule in include/vorbis_b200.h, vb200_ogg_links).
+template <class At>
+__device__ __forceinline__ void ogg_links_walk(const uint8_t *bytes, int64_t beg, int64_t end, int lane,
+                                               const uint32_t *crc_tab, const uint32_t *xpw, At &at) {
+  bool after_data = false;                                // the last captured page has no BOS flag
+  int64_t p = beg;
+  for (;;) {
+    const int len = ogg_capture(bytes, p, end, lane, crc_tab, xpw);
+    if (len < 0) break;
+    if (len == 0) continue;
+    const bool bos = (bytes[p + 5] & 2) != 0;
+    if (bos && after_data) at(p);
+    after_data = !bos;
+    p += len;
+  }
+}
+
+// link_first[f + 1] = file f's link count; k_ds_scan then turns the counts into offsets
+__global__ void __launch_bounds__(32 * OGG_WARPS)
+k_ogg_links_count(int nfiles, const uint8_t *__restrict__ bytes, const int64_t *__restrict__ file_off,
+                  long long *__restrict__ link_first) {
+  __shared__ uint32_t crc_tab[256];
+  __shared__ uint32_t xpw[OGG_XPOW];
+  ogg_crc_setup(crc_tab, xpw);
+  const int lane = threadIdx.x & 31;
+  const int f = blockIdx.x * OGG_WARPS + (threadIdx.x >> 5);
+  if (f >= nfiles) return;
+  long long n = 1;
+  auto at = [&](int64_t) { n++; };
+  ogg_links_walk(bytes, file_off[f], file_off[f + 1], lane, crc_tab, xpw, at);
+  if (lane == 0) link_first[f + 1] = n;
+}
+
+// link_off[link_first[f] ..] = file_off[f], then the offsets of the file's later links' first pages; the last file's
+// warp also writes link_off[total] = file_off[nfiles].  Nothing is written when total > link_cap.
+__global__ void __launch_bounds__(32 * OGG_WARPS)
+k_ogg_links_write(int nfiles, const uint8_t *__restrict__ bytes, const int64_t *__restrict__ file_off,
+                  const long long *__restrict__ link_first, int64_t *__restrict__ link_off, long long link_cap) {
+  __shared__ uint32_t crc_tab[256];
+  __shared__ uint32_t xpw[OGG_XPOW];
+  if (link_first[nfiles] > link_cap) return;              // the sizing call (or too small a table): nothing written
+  ogg_crc_setup(crc_tab, xpw);
+  const int lane = threadIdx.x & 31;
+  const int f = blockIdx.x * OGG_WARPS + (threadIdx.x >> 5);
+  if (f >= nfiles) return;
+  long long row = link_first[f];
+  if (lane == 0) {
+    link_off[row] = file_off[f];
+    if (f == nfiles - 1) link_off[link_first[nfiles]] = file_off[nfiles];
+  }
+  auto at = [&](int64_t p) {
+    row++;
+    if (lane == 0) link_off[row] = p;
+  };
+  ogg_links_walk(bytes, file_off[f], file_off[f + 1], lane, crc_tab, xpw, at);
 }

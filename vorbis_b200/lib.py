@@ -51,7 +51,7 @@ EXPORTS = [
     "vb200_encode_streams_packets_managed_resume",
     "vb200_encode_pcm_carry_bytes", "vb200_encode_pcm_carry_init", "vb200_encode_pcm_packets",
     "vb200_encode_pcm_packets_managed", "vb200_lpc_extrapolate",
-    "vb200_ogg_demux_dev", "vb200_ogg_demux", "vb200_vorbis_window",
+    "vb200_ogg_demux_dev", "vb200_ogg_demux", "vb200_ogg_links_dev", "vb200_ogg_links", "vb200_vorbis_window",
     "vb200_vorbis_headers_parse", "vb200_vorbis_headers_free",
     "vb200_ogg_group_scratch_bytes", "vb200_ogg_group_dev", "vb200_ogg_group",
     "vb200_ogg_mux_dev", "vb200_ogg_mux",
@@ -188,6 +188,8 @@ def load():
     L.vb200_lpc_extrapolate.argtypes = [vp, C.c_int, C.c_int, vp, C.c_int64, vp, C.c_int32, vp, vp, C.c_int64]
     L.vb200_ogg_demux_dev.argtypes = [C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, vp]
     L.vb200_ogg_demux.argtypes = [C.c_int, vp, vp, C.c_int, vp, vp, vp, vp]
+    L.vb200_ogg_links_dev.argtypes = [C.c_int, vp, vp, vp, vp, C.c_int64, vp]
+    L.vb200_ogg_links.argtypes = [C.c_int, vp, vp, vp, vp, C.c_int64]
     L.vb200_vorbis_window.argtypes = [C.c_int, vp]
     L.vb200_vorbis_headers_parse.argtypes = [vp, C.c_int32, vp, C.c_int32, vp, C.c_int32,
                                              C.POINTER(C.POINTER(abi.VorbisHeaders))]
@@ -1227,6 +1229,39 @@ def ogg_demux_dev(nfiles, d_bytes, d_file_off, max_packets, d_info, d_npkt, d_da
     L = load()
     _check(L, L.vb200_ogg_demux_dev(nfiles, _ptr(d_bytes), _ptr(d_file_off), max_packets, _ptr(d_info), _ptr(d_npkt),
                                     _ptr(d_data), _ptr(d_streams), _ptr(stream)))
+
+
+def ogg_links(files, link_cap=None, check=True):
+    """vb200_ogg_links on a list of Ogg files (bytes or uint8 arrays), on the current CUDA device.  Returns {"file_off"
+    int64 [n+1] (the files back to back), "link_first" int64 [n+1], "link_off" int64 [total+1] (zeros when link_cap
+    is below the total), "rc"}.  link_cap defaults to what the table needs (a sizing call first).  link_off with
+    link_first[n] is the file_off and nfiles of ogg_demux's rows: ogg_demux([bytes of each link]) is the same call."""
+    L = load()
+    arrs = [np.frombuffer(bytes(f), np.uint8) for f in files]
+    n = len(arrs)
+    file_off = np.zeros(n + 1, np.int64)
+    file_off[1:] = np.cumsum([len(a) for a in arrs])
+    buf = np.ascontiguousarray(np.concatenate(arrs) if n else np.zeros(1, np.uint8))
+    link_first = np.zeros(n + 1, np.int64)
+    if link_cap is None:
+        rc = L.vb200_ogg_links(n, _ptr(buf), _ptr(file_off), _ptr(link_first), None, 0)
+        link_cap = int(link_first[n]) if n else 0
+        if rc != 0 and link_cap == 0:
+            _check(L, rc)
+    link_off = np.zeros(link_cap + 1, np.int64)
+    rc = L.vb200_ogg_links(n, _ptr(buf), _ptr(file_off), _ptr(link_first), _ptr(link_off), link_cap)
+    if check:
+        _check(L, rc)
+    total = int(link_first[n])
+    return {"file_off": file_off, "link_first": link_first,
+            "link_off": link_off[:total + 1] if total <= link_cap else np.zeros(total + 1, np.int64), "rc": rc}
+
+
+def ogg_links_dev(nfiles, d_bytes, d_file_off, d_link_first, d_link_off, link_cap, stream=None):
+    """vb200_ogg_links_dev: device pointers (ints, e.g. torch tensors' data_ptr()), asynchronous on `stream`"""
+    L = load()
+    _check(L, L.vb200_ogg_links_dev(nfiles, _ptr(d_bytes), _ptr(d_file_off), _ptr(d_link_first), _ptr(d_link_off),
+                                    link_cap, _ptr(stream)))
 
 
 def vorbis_window(n):
