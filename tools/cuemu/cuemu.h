@@ -216,6 +216,8 @@ static inline int atomicAnd(int *p, int v) { return __atomic_fetch_and(p, v, __A
 static inline unsigned atomicOr(unsigned *p, unsigned v) { return __atomic_fetch_or(p, v, __ATOMIC_RELAXED); }
 static inline int atomicOr(int *p, int v) { return __atomic_fetch_or(p, v, __ATOMIC_RELAXED); }
 static inline int atomicMax(int *p, int v) { int o = __atomic_load_n(p, __ATOMIC_RELAXED); while (o < v && !__atomic_compare_exchange_n(p, &o, v, true, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {} return o; }
+static inline int atomicMin(int *p, int v) { int o = __atomic_load_n(p, __ATOMIC_RELAXED); while (o > v && !__atomic_compare_exchange_n(p, &o, v, true, __ATOMIC_RELAXED, __ATOMIC_RELAXED)) {} return o; }
+static inline unsigned long long atomicCAS(unsigned long long *p, unsigned long long cmp, unsigned long long v) { __atomic_compare_exchange_n(p, &cmp, v, false, __ATOMIC_RELAXED, __ATOMIC_RELAXED); return cmp; }
 static inline long long clock64() { return 0; }
 
 // ---- arithmetic intrinsics ----------------------------------------------------------------

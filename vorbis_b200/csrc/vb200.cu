@@ -1161,28 +1161,51 @@ extern "C" int vb200_mdct_backward_dev(vb200_ctx *c, int W, int nvec, const floa
   return post_launch(c);
 }
 
-// generic "copy in, run, copy out" for the host-buffer variants: every device buffer a host form stages, input
-// (src != nullptr: copied in on s_main) or output, takes the next buffer of the context's staging pool
+// "Copy in, run, copy out" for the host-buffer variants.  Every device buffer a host form stages, input or output,
+// takes the next buffer of the context's staging pool.  Sizes count elements of T, or bytes for T = void, where the
+// C ABI passes void * (the PCM, vb200_encode_io's iwork).  The first failure is kept in rc, and every later call does
+// nothing and returns nullptr, so a form stages everything, checks rc once, runs, queues its copies back and returns
+// sync().  The copies on s_main read and write the caller's memory, which may be pinned: a form that returns before
+// sync(), on any path, waits for them in the destructor, while its lock guard (declared first) still holds the context.
 struct HostIO {
   vb200_ctx *c;
-  int slot = 0;
-  int h2d(const void *src, size_t bytes, void **d) {
-    if (slot == STAGE_SLOTS) return fail(VB200_EFAULT, "host call stages more buffers than the staging pool holds");
-    int rc = ensure_buf(c->stage[slot++], bytes, d); if (rc) return rc;
-    if (src) CU(cudaMemcpyAsync(*d, src, bytes, cudaMemcpyHostToDevice, c->s_main));
-    return 0;
+  int slot = 0, rc = 0;
+  bool queued = false;               // copies queued on s_main since the last sync()
+  ~HostIO() { if (queued) cudaStreamSynchronize(c->s_main); }   // the error being returned holds the reason
+  // n elements, src copied in unless it is null
+  template <class T> T *in(const T *src, size_t n) {
+    if (!rc && slot == STAGE_SLOTS) rc = fail(VB200_EFAULT, "host call stages more buffers than the staging pool holds");
+    if (rc) return nullptr;
+    void *d;
+    if ((rc = ensure_buf(c->stage[slot++], bytes<T>(n), &d))) return nullptr;
+    if (src && (rc = copy(d, src, bytes<T>(n), cudaMemcpyHostToDevice))) return nullptr;
+    return (T *)d;
   }
+  template <class T> T *out(size_t n) { return in<T>(nullptr, n); }
   // packet bytes: the buffer is one byte longer, so that it exists when there are none
-  int h2d_packets(const uint8_t *src, int64_t bytes, void **d) {
-    int rc = h2d(nullptr, (size_t)bytes + 1, d); if (rc) return rc;
-    if (bytes) CU(cudaMemcpyAsync(*d, src, (size_t)bytes, cudaMemcpyHostToDevice, c->s_main));
+  uint8_t *packets(const uint8_t *src, int64_t n) {
+    uint8_t *d = out<uint8_t>((size_t)n + 1);
+    if (rc || (n && (rc = copy(d, src, (size_t)n, cudaMemcpyHostToDevice)))) return nullptr;
+    return d;
+  }
+  template <class T> void back(T *dst, const T *d, size_t n) {
+    if (!rc) rc = copy(dst, d, bytes<T>(n), cudaMemcpyDeviceToHost);
+  }
+  int sync() {
+    if (!rc) { queued = false; rc = wait(); }
+    return rc;
+  }
+
+ private:
+  template <class T> static size_t bytes(size_t n) {
+    if constexpr (std::is_void_v<T>) return n; else return sizeof(T) * n;
+  }
+  int copy(void *dst, const void *src, size_t n, cudaMemcpyKind kind) {
+    CU(cudaMemcpyAsync(dst, src, n, kind, c->s_main));
+    queued = true;
     return 0;
   }
-  int d2h(void *dst, const void *d, size_t bytes) {
-    CU(cudaMemcpyAsync(dst, d, bytes, cudaMemcpyDeviceToHost, c->s_main));
-    return 0;
-  }
-  int sync() { CU(cudaStreamSynchronize(c->s_main)); return 0; }
+  int wait() { CU(cudaStreamSynchronize(c->s_main)); return 0; }
 };
 
 extern "C" int vb200_mdct_forward(vb200_ctx *c, int W, int nvec, const float *in, float *out) {
@@ -1191,11 +1214,12 @@ extern "C" int vb200_mdct_forward(vb200_ctx *c, int W, int nvec, const float *in
   std::lock_guard<std::mutex> lk(c->mu);
   const int N = c->dx[W].N;
   HostIO io{c};
-  void *di, *dout; int rc;
-  if ((rc = io.h2d(in, sizeof(float) * (size_t)nvec * N, &di))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(float) * (size_t)nvec * N / 2, &dout))) return rc;
-  if ((rc = vb200_mdct_forward_dev(c, W, nvec, (const float *)di, (float *)dout, c->s_main))) return rc;
-  if ((rc = io.d2h(out, dout, sizeof(float) * (size_t)nvec * N / 2))) return rc;
+  const float *di = io.in(in, (size_t)nvec * N);
+  float *dout = io.out<float>((size_t)nvec * N / 2);
+  if (io.rc) return io.rc;
+  int rc;
+  if ((rc = vb200_mdct_forward_dev(c, W, nvec, di, dout, c->s_main))) return rc;
+  io.back(out, dout, (size_t)nvec * N / 2);
   return io.sync();
 }
 
@@ -1205,11 +1229,12 @@ extern "C" int vb200_mdct_backward(vb200_ctx *c, int W, int nvec, const float *i
   std::lock_guard<std::mutex> lk(c->mu);
   const int N = (c->halfrate ? c->dx_hs[W] : c->dx[W]).N;
   HostIO io{c};
-  void *di, *dout; int rc;
-  if ((rc = io.h2d(in, sizeof(float) * (size_t)nvec * N / 2, &di))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(float) * (size_t)nvec * N, &dout))) return rc;
-  if ((rc = vb200_mdct_backward_dev(c, W, nvec, (const float *)di, (float *)dout, c->s_main))) return rc;
-  if ((rc = io.d2h(out, dout, sizeof(float) * (size_t)nvec * N))) return rc;
+  const float *di = io.in(in, (size_t)nvec * N / 2);
+  float *dout = io.out<float>((size_t)nvec * N);
+  if (io.rc) return io.rc;
+  int rc;
+  if ((rc = vb200_mdct_backward_dev(c, W, nvec, di, dout, c->s_main))) return rc;
+  io.back(out, dout, (size_t)nvec * N);
   return io.sync();
 }
 
@@ -1219,13 +1244,13 @@ extern "C" int vb200_apply_window(vb200_ctx *c, int W, int nvec, const int32_t *
   std::lock_guard<std::mutex> lk(c->mu);
   const int N = c->dx[W].N;
   HostIO io{c};
-  void *dd, *dl = nullptr, *dn = nullptr; int rc;
-  if ((rc = io.h2d(data, sizeof(float) * (size_t)nvec * N, &dd))) return rc;
-  if (lW && (rc = io.h2d(lW, sizeof(int32_t) * nvec, &dl))) return rc;
-  if (nW && (rc = io.h2d(nW, sizeof(int32_t) * nvec, &dn))) return rc;
-  k_apply_window<<<grid_for(c, nvec, 8), 256, 0, c->s_main>>>(c->dwin, W, nvec, (const int *)dl, (const int *)dn, (float *)dd);
+  float *dd = io.in(data, (size_t)nvec * N);
+  const int32_t *dl = lW ? io.in(lW, nvec) : nullptr, *dn = nW ? io.in(nW, nvec) : nullptr;
+  if (io.rc) return io.rc;
+  k_apply_window<<<grid_for(c, nvec, 8), 256, 0, c->s_main>>>(c->dwin, W, nvec, dl, dn, dd);
+  int rc;
   if ((rc = post_launch(c))) return rc;
-  if ((rc = io.d2h(data, dd, sizeof(float) * (size_t)nvec * N))) return rc;
+  io.back(data, dd, (size_t)nvec * N);
   return io.sync();
 }
 
@@ -1235,13 +1260,14 @@ extern "C" int vb200_drft_forward(vb200_ctx *c, int W, int nvec, float *data) {
   std::lock_guard<std::mutex> lk(c->mu);
   const XformDev &X = c->dx[W];
   HostIO io{c};
-  void *dd; int rc;
-  if ((rc = io.h2d(data, sizeof(float) * (size_t)nvec * X.N, &dd))) return rc;
+  float *dd = io.in(data, (size_t)nvec * X.N);
+  if (io.rc) return io.rc;
   const size_t smem = sizeof(float) * 2 * fft_buf_floats(X.N);
+  int rc;
   if ((rc = set_smem(k_drft_forward, smem))) return rc;
-  k_drft_forward<<<grid_for(c, nvec, 8), threads_for(X.N), smem, c->s_main>>>(X, nvec, (float *)dd);
+  k_drft_forward<<<grid_for(c, nvec, 8), threads_for(X.N), smem, c->s_main>>>(X, nvec, dd);
   if ((rc = post_launch(c))) return rc;
-  if ((rc = io.d2h(data, dd, sizeof(float) * (size_t)nvec * X.N))) return rc;
+  io.back(data, dd, (size_t)nvec * X.N);
   return io.sync();
 }
 
@@ -1261,15 +1287,16 @@ extern "C" int vb200_noisemask(vb200_ctx *c, int look, int nvec, const float *lo
   std::lock_guard<std::mutex> lk(c->mu);
   const PsyDev &P = c->dpsy[look];
   HostIO io{c};
-  void *di, *dout; int rc;
-  const size_t bytes = sizeof(float) * (size_t)nvec * P.n;
-  if ((rc = io.h2d(logmdct, bytes, &di))) return rc;
-  if ((rc = io.h2d(nullptr, bytes, &dout))) return rc;
+  const size_t len = (size_t)nvec * P.n;
+  const float *di = io.in(logmdct, len);
+  float *dout = io.out<float>(len);
+  if (io.rc) return io.rc;
   const size_t smem = psy_smem_bytes(P, P);
+  int rc;
   if ((rc = set_smem(k_noisemask, smem))) return rc;
-  k_noisemask<<<grid_for(c, nvec, 4), PSY_THREADS, smem, c->s_main>>>(P, nvec, (const float *)di, (float *)dout);
+  k_noisemask<<<grid_for(c, nvec, 4), PSY_THREADS, smem, c->s_main>>>(P, nvec, di, dout);
   if ((rc = post_launch(c))) return rc;
-  if ((rc = io.d2h(noise, dout, bytes))) return rc;
+  io.back(noise, dout, len);
   return io.sync();
 }
 
@@ -1280,18 +1307,16 @@ extern "C" int vb200_tonemask(vb200_ctx *c, int look, int nvec, const float *log
   std::lock_guard<std::mutex> lk(c->mu);
   const PsyDev &P = c->dpsy[look];
   HostIO io{c};
-  void *di, *dg, *dl, *dout; int rc;
-  const size_t bytes = sizeof(float) * (size_t)nvec * P.n;
-  if ((rc = io.h2d(logfft, bytes, &di))) return rc;
-  if ((rc = io.h2d(gmax, sizeof(float) * nvec, &dg))) return rc;
-  if ((rc = io.h2d(lmax, sizeof(float) * nvec, &dl))) return rc;
-  if ((rc = io.h2d(nullptr, bytes, &dout))) return rc;
+  const size_t len = (size_t)nvec * P.n;
+  const float *di = io.in(logfft, len), *dg = io.in(gmax, nvec), *dl = io.in(lmax, nvec);
+  float *dout = io.out<float>(len);
+  if (io.rc) return io.rc;
   const size_t smem = psy_smem_bytes(P, P);
+  int rc;
   if ((rc = set_smem(k_tonemask, smem))) return rc;
-  k_tonemask<<<grid_for(c, nvec, 4), PSY_THREADS, smem, c->s_main>>>(P, nvec, (const float *)di, (const float *)dg,
-                                                             (const float *)dl, (float *)dout);
+  k_tonemask<<<grid_for(c, nvec, 4), PSY_THREADS, smem, c->s_main>>>(P, nvec, di, dg, dl, dout);
   if ((rc = post_launch(c))) return rc;
-  if ((rc = io.d2h(tone, dout, bytes))) return rc;
+  io.back(tone, dout, len);
   return io.sync();
 }
 
@@ -1303,18 +1328,17 @@ extern "C" int vb200_offset_and_mix(vb200_ctx *c, int look, int nvec, int sel, c
   std::lock_guard<std::mutex> lk(c->mu);
   const PsyDev &P = c->dpsy[look];
   HostIO io{c};
-  void *dn, *dt, *dm, *dl, *dk; int rc;
-  const size_t bytes = sizeof(float) * (size_t)nvec * P.n;
-  if ((rc = io.h2d(noise, bytes, &dn))) return rc;
-  if ((rc = io.h2d(tone, bytes, &dt))) return rc;
-  if ((rc = io.h2d(mdct, bytes, &dm))) return rc;
-  if ((rc = io.h2d(logmdct, bytes, &dl))) return rc;
-  if ((rc = io.h2d(nullptr, bytes, &dk))) return rc;
-  k_offset_and_mix<<<grid_for(c, (int)(((size_t)nvec * P.n + 255) / 256), 8), 256, 0, c->s_main>>>(
-      P, nvec, sel, (const float *)dn, (const float *)dt, (float *)dm, (const float *)dl, (float *)dk);
+  const size_t len = (size_t)nvec * P.n;
+  const float *dn = io.in(noise, len), *dt = io.in(tone, len);
+  float *dm = io.in(mdct, len);
+  const float *dl = io.in(logmdct, len);
+  float *dk = io.out<float>(len);
+  if (io.rc) return io.rc;
+  k_offset_and_mix<<<grid_for(c, (int)((len + 255) / 256), 8), 256, 0, c->s_main>>>(P, nvec, sel, dn, dt, dm, dl, dk);
+  int rc;
   if ((rc = post_launch(c))) return rc;
-  if ((rc = io.d2h(logmask, dk, bytes))) return rc;
-  if ((rc = io.d2h(mdct, dm, bytes))) return rc;
+  io.back(logmask, dk, len);
+  io.back(mdct, dm, len);
   return io.sync();
 }
 
@@ -1653,15 +1677,15 @@ extern "C" int vb200_couple_quantize_normalize(vb200_ctx *c, int W, int blocktyp
   if (nblocks <= 0) return 0;
   std::lock_guard<std::mutex> lk(c->mu);
   const int ch = c->setup.channels, n = c->dx[W].N / 2;
+  const size_t rows = (size_t)nblocks * ch;
   HostIO io{c};
-  void *dm, *di, *dz; int rc;
-  if ((rc = io.h2d(mdct, sizeof(float) * (size_t)nblocks * ch * n, &dm))) return rc;
-  if ((rc = io.h2d(iwork, sizeof(int32_t) * (size_t)nblocks * ch * n, &di))) return rc;
-  if ((rc = io.h2d(nonzero, sizeof(int32_t) * (size_t)nblocks * ch, &dz))) return rc;
-  if ((rc = vb200_couple_quantize_normalize_dev(c, W, blocktype, blobno, nblocks, (const float *)dm,
-                                                (int32_t *)di, (int32_t *)dz, c->s_main))) return rc;
-  if ((rc = io.d2h(iwork, di, sizeof(int32_t) * (size_t)nblocks * ch * n))) return rc;
-  if ((rc = io.d2h(nonzero, dz, sizeof(int32_t) * (size_t)nblocks * ch))) return rc;
+  const float *dm = io.in(mdct, rows * n);
+  int32_t *di = io.in(iwork, rows * n), *dz = io.in(nonzero, rows);
+  if (io.rc) return io.rc;
+  int rc;
+  if ((rc = vb200_couple_quantize_normalize_dev(c, W, blocktype, blobno, nblocks, dm, di, dz, c->s_main))) return rc;
+  io.back(iwork, di, rows * n);
+  io.back(nonzero, dz, rows);
   return io.sync();
 }
 
@@ -1736,17 +1760,17 @@ extern "C" int vb200_synthesis(vb200_ctx *c, int nstreams, int nblk, const int32
   const size_t nb = (size_t)nstreams * nblk;
   for (size_t i = 0; i < nb; i++) if (Wseq[i] < 0 || Wseq[i] > 1) return fail(VB200_EINVAL, "Wseq values must be 0/1");
   HostIO io{c};
-  void *dW, *dco, *dc, *dpo, *dp; int rc;
-  if ((rc = io.h2d(Wseq, sizeof(int32_t) * nb, &dW))) return rc;
-  if ((rc = io.h2d(coef_off, sizeof(int64_t) * nb, &dco))) return rc;
-  if ((rc = io.h2d(coef, sizeof(float) * (size_t)coef_len, &dc))) return rc;
-  if ((rc = io.h2d(pcm_off, sizeof(int64_t) * nb, &dpo))) return rc;
-  const size_t pbytes = sizeof(float) * (size_t)nstreams * ch * (size_t)pcm_stride;
-  if ((rc = io.h2d(nullptr, pbytes, &dp))) return rc;
-  CU(cudaMemsetAsync(dp, 0, pbytes, c->s_main));
-  if ((rc = vb200_synthesis_dev(c, nstreams, nblk, (const int32_t *)dW, (const int64_t *)dco, (const float *)dc,
-                                (const int64_t *)dpo, (float *)dp, pcm_stride, c->s_main))) return rc;
-  if ((rc = io.d2h(pcm, dp, pbytes))) return rc;
+  const int32_t *dW = io.in(Wseq, nb);
+  const int64_t *dco = io.in(coef_off, nb);
+  const float *dc = io.in(coef, (size_t)coef_len);
+  const int64_t *dpo = io.in(pcm_off, nb);
+  const size_t plen = (size_t)nstreams * ch * (size_t)pcm_stride;
+  float *dp = io.out<float>(plen);
+  if (io.rc) return io.rc;
+  CU(cudaMemsetAsync(dp, 0, sizeof(float) * plen, c->s_main));
+  int rc;
+  if ((rc = vb200_synthesis_dev(c, nstreams, nblk, dW, dco, dc, dpo, dp, pcm_stride, c->s_main))) return rc;
+  io.back(pcm, dp, plen);
   return io.sync();
 }
 
@@ -1764,12 +1788,13 @@ extern "C" int vb200_decouple(vb200_ctx *c, int W, int nblocks, float *res) {
   CHECK_CTX(c); CHECK_W(W);
   if (nblocks <= 0) return 0;
   std::lock_guard<std::mutex> lk(c->mu);
-  const size_t bytes = sizeof(float) * (size_t)nblocks * c->setup.channels * (c->dx[W].N / 2);
+  const size_t len = (size_t)nblocks * c->setup.channels * (c->dx[W].N / 2);
   HostIO io{c};
-  void *d; int rc;
-  if ((rc = io.h2d(res, bytes, &d))) return rc;
-  if ((rc = vb200_decouple_dev(c, W, nblocks, (float *)d, c->s_main))) return rc;
-  if ((rc = io.d2h(res, d, bytes))) return rc;
+  float *d = io.in(res, len);
+  if (io.rc) return io.rc;
+  int rc;
+  if ((rc = vb200_decouple_dev(c, W, nblocks, d, c->s_main))) return rc;
+  io.back(res, d, len);
   return io.sync();
 }
 
@@ -1844,15 +1869,13 @@ extern "C" int vb200_floor1_fit(vb200_ctx *c, int W, int floor_sel, int nrows, c
   std::lock_guard<std::mutex> lk(c->mu);
   const size_t n = c->dx[W].N / 2;
   HostIO io{c};
-  void *da, *db, *dp, *dz; int rc;
-  if ((rc = io.h2d(logmdct, sizeof(float) * nrows * n, &da))) return rc;
-  if ((rc = io.h2d(logmask, sizeof(float) * nrows * n, &db))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(int32_t) * (size_t)nrows * VB200_FLOOR1_STRIDE, &dp))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(int32_t) * (size_t)nrows, &dz))) return rc;
-  if ((rc = vb200_floor1_fit_dev(c, W, floor_sel, nrows, (const float *)da, (const float *)db, (int32_t *)dp,
-                                 (int32_t *)dz, c->s_main))) return rc;
-  if ((rc = io.d2h(posts, dp, sizeof(int32_t) * (size_t)nrows * VB200_FLOOR1_STRIDE))) return rc;
-  if ((rc = io.d2h(fit_nonzero, dz, sizeof(int32_t) * (size_t)nrows))) return rc;
+  const float *da = io.in(logmdct, nrows * n), *db = io.in(logmask, nrows * n);
+  int32_t *dp = io.out<int32_t>((size_t)nrows * VB200_FLOOR1_STRIDE), *dz = io.out<int32_t>(nrows);
+  if (io.rc) return io.rc;
+  int rc;
+  if ((rc = vb200_floor1_fit_dev(c, W, floor_sel, nrows, da, db, dp, dz, c->s_main))) return rc;
+  io.back(posts, dp, (size_t)nrows * VB200_FLOOR1_STRIDE);
+  io.back(fit_nonzero, dz, nrows);
   return io.sync();
 }
 
@@ -1863,16 +1886,15 @@ extern "C" int vb200_floor1_render(vb200_ctx *c, int W, int floor_sel, int nrows
   std::lock_guard<std::mutex> lk(c->mu);
   const size_t n = c->dx[W].N / 2;
   HostIO io{c};
-  void *dp, *dz, *di, *dn; int rc;
-  if ((rc = io.h2d(posts, sizeof(int32_t) * (size_t)nrows * VB200_FLOOR1_STRIDE, &dp))) return rc;
-  if ((rc = io.h2d(fit_nonzero, sizeof(int32_t) * (size_t)nrows, &dz))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(int32_t) * nrows * n, &di))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(int32_t) * (size_t)nrows, &dn))) return rc;
-  if ((rc = vb200_floor1_render_dev(c, W, floor_sel, nrows, (int32_t *)dp, (const int32_t *)dz, (int32_t *)di,
-                                    (int32_t *)dn, c->s_main))) return rc;
-  if ((rc = io.d2h(posts, dp, sizeof(int32_t) * (size_t)nrows * VB200_FLOOR1_STRIDE))) return rc;
-  if ((rc = io.d2h(ilogmask, di, sizeof(int32_t) * nrows * n))) return rc;
-  if ((rc = io.d2h(nonzero, dn, sizeof(int32_t) * (size_t)nrows))) return rc;
+  int32_t *dp = io.in(posts, (size_t)nrows * VB200_FLOOR1_STRIDE);
+  const int32_t *dz = io.in(fit_nonzero, nrows);
+  int32_t *di = io.out<int32_t>(nrows * n), *dn = io.out<int32_t>(nrows);
+  if (io.rc) return io.rc;
+  int rc;
+  if ((rc = vb200_floor1_render_dev(c, W, floor_sel, nrows, dp, dz, di, dn, c->s_main))) return rc;
+  io.back(posts, dp, (size_t)nrows * VB200_FLOOR1_STRIDE);
+  io.back(ilogmask, di, nrows * n);
+  io.back(nonzero, dn, nrows);
   return io.sync();
 }
 
@@ -1910,18 +1932,17 @@ static size_t enc_pcm_bytes(const vb200_encode_io *io, int ch, int N, int nstrea
 }
 
 // host forms of the chain: the inputs copied in, and int32 outputs of `curves` curves staged, in d
-static int enc_stage(HostIO &io, const vb200_encode_io *h, vb200_encode_io *d, int ch, int N, int nstreams, int bps,
-                     int curves) {
+static void enc_stage(HostIO &io, const vb200_encode_io *h, vb200_encode_io *d, int ch, int N, int nstreams, int bps,
+                      int curves) {
   const size_t nb = (size_t)nstreams * bps, rows = curves * nb * ch;
-  void *p; int rc;
-  if ((rc = io.h2d(h->pcm, enc_pcm_bytes(h, ch, N, nstreams, bps), &p))) return rc; d->pcm = p;
-  if ((rc = io.h2d(h->desc, sizeof(vb200_block_desc) * nb, &p))) return rc; d->desc = (const vb200_block_desc *)p;
-  if ((rc = io.h2d(h->ampmax0, sizeof(float) * nstreams, &p))) return rc; d->ampmax0 = h->ampmax0 ? (const float *)p : nullptr;
-  if ((rc = io.h2d(nullptr, sizeof(int32_t) * rows * VB200_FLOOR1_STRIDE, &p))) return rc; d->posts = (int32_t *)p;
-  if ((rc = io.h2d(nullptr, sizeof(int32_t) * rows, &p))) return rc; d->nonzero = (int32_t *)p;
-  if ((rc = io.h2d(nullptr, sizeof(int32_t) * rows * (N / 2), &p))) return rc; d->iwork = p;
-  if ((rc = io.h2d(nullptr, sizeof(float) * nb, &p))) return rc; d->ampmax_out = (float *)p;
-  return 0;
+  d->pcm = io.in(h->pcm, enc_pcm_bytes(h, ch, N, nstreams, bps));
+  d->desc = io.in(h->desc, nb);
+  const float *a0 = io.in(h->ampmax0, nstreams);     // staged even when there is none
+  d->ampmax0 = h->ampmax0 ? a0 : nullptr;
+  d->posts = io.out<int32_t>(rows * VB200_FLOOR1_STRIDE);
+  d->nonzero = io.out<int32_t>(rows);
+  d->iwork = io.out<int32_t>(rows * (N / 2));
+  d->ampmax_out = io.out<float>(nb);
 }
 
 // own_outputs: the call stages posts / nonzero / iwork itself, so the io need not give them
@@ -2145,12 +2166,13 @@ extern "C" int vb200_encode_dsp_managed(vb200_ctx *c, int W, int nstreams, int b
   HostIO io{c};
   vb200_encode_io d = *h;
   d.mdct = d.logmdct = d.logmask = nullptr;
-  if ((rc = enc_stage(io, h, &d, ch, N, nstreams, bps, NB))) return rc;
+  enc_stage(io, h, &d, ch, N, nstreams, bps, NB);
+  if (io.rc) return io.rc;
   if ((rc = vb200_encode_dsp_managed_dev(c, W, nstreams, bps, &d, c->s_main))) return rc;
-  if ((rc = io.d2h(h->posts, d.posts, sizeof(int32_t) * NB * rows * VB200_FLOOR1_STRIDE))) return rc;
-  if ((rc = io.d2h(h->nonzero, d.nonzero, sizeof(int32_t) * NB * rows))) return rc;
-  if ((rc = io.d2h(h->iwork, d.iwork, sizeof(int32_t) * NB * rows * n))) return rc;
-  if ((rc = io.d2h(h->ampmax_out, d.ampmax_out, sizeof(float) * nb))) return rc;
+  io.back(h->posts, d.posts, NB * rows * VB200_FLOOR1_STRIDE);
+  io.back(h->nonzero, d.nonzero, NB * rows);
+  io.back(h->iwork, d.iwork, sizeof(int32_t) * NB * rows * n);
+  io.back(h->ampmax_out, d.ampmax_out, nb);
   return io.sync();
 }
 
@@ -2285,12 +2307,11 @@ extern "C" int vb200_plan_blocks(vb200_ctx *c, int nstreams, const int32_t *mark
   cudaStream_t st = c->s_main;
   const size_t cap = (size_t)nstreams * max_blocks;
   HostIO io{c};
-  void *dm, *dl, *de = nullptr, *dp, *dn;
-  if ((rc = io.h2d(mark, sizeof(int32_t) * (size_t)nstreams * mark_stride, &dm))) return rc;
-  if ((rc = io.h2d(pcm_len, sizeof(int64_t) * nstreams, &dl))) return rc;
-  if (eof && (rc = io.h2d(eof, sizeof(int64_t) * nstreams, &de))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(vb200_stream_block) * cap, &dp))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(int32_t) * nstreams, &dn))) return rc;
+  const int32_t *dm = io.in(mark, (size_t)nstreams * mark_stride);
+  const int64_t *dl = io.in(pcm_len, nstreams), *de = eof ? io.in(eof, nstreams) : nullptr;
+  vb200_stream_block *dp = io.out<vb200_stream_block>(cap);
+  int32_t *dn = io.out<int32_t>(nstreams);
+  if (io.rc) return io.rc;
   int32_t *d_tot, *d_work; int2 *d_src[2]; vb200_block_desc *d_desc[2];
   if ((rc = carve(c->plan, [&](Carve &k) {
          d_tot = k.take<int32_t>(2); d_work = k.take<int32_t>(4 * (size_t)nstreams);
@@ -2298,12 +2319,12 @@ extern "C" int vb200_plan_blocks(vb200_ctx *c, int nstreams, const int32_t *mark
        }))) return rc;
   const int caps[2] = {(int)cap, (int)cap};
   if ((rc = scratch_begin(c, st))) return rc;
-  if ((rc = plan_launch(c, nstreams, (const int32_t *)dm, mark_stride, nsteps, (const int64_t *)dl, (const int64_t *)de,
-                        max_blocks, (vb200_stream_block *)dp, (int32_t *)dn, caps, d_src, d_desc, d_tot, d_work, st)))
+  if ((rc = plan_launch(c, nstreams, dm, mark_stride, nsteps, dl, de, max_blocks, dp, dn, caps, d_src, d_desc, d_tot,
+                        d_work, st)))
     return rc;
   if ((rc = scratch_end(c, st))) return rc;
-  if ((rc = io.d2h(plan, dp, sizeof(vb200_stream_block) * cap))) return rc;
-  if ((rc = io.d2h(nblocks, dn, sizeof(int32_t) * nstreams))) return rc;
+  io.back(plan, dp, cap);
+  io.back(nblocks, dn, nstreams);
   return io.sync();
 }
 
@@ -2475,27 +2496,24 @@ extern "C" int vb200_encode_streams_managed_dev(vb200_ctx *c, int nstreams, vb20
 // A host vb200_streams_io staged through io into the device copy d: the inputs copied in (the pcm only when
 // stage_pcm, else h->pcm is already on the device), the plan and nblocks, and for each size with cap[w] > 0 the
 // outputs of cap[w] blocks, of every curve for managed.
-static int streams_stage(vb200_ctx *c, HostIO &io, int nstreams, bool managed, bool stage_pcm,
-                         const vb200_streams_io *h, vb200_streams_io *d) {
+static void streams_stage(vb200_ctx *c, HostIO &io, int nstreams, bool managed, bool stage_pcm,
+                          const vb200_streams_io *h, vb200_streams_io *d) {
   const size_t ch = c->setup.channels, curves = managed ? VB200_PACKETBLOBS : 1;
   const size_t pcm_bytes = (size_t)nstreams * ch * (size_t)h->stream_stride * (h->pcm_fmt == VB200_PCM_S16_INTERLEAVED ? 2 : 4);
-  void *p;
-  int rc;
   *d = *h;
-  if (stage_pcm) { if ((rc = io.h2d(h->pcm, pcm_bytes, &p))) return rc; d->pcm = p; }
-  if ((rc = io.h2d(h->pcm_len, sizeof(int64_t) * nstreams, &p))) return rc; d->pcm_len = (const int64_t *)p;
-  if (h->eof) { if ((rc = io.h2d(h->eof, sizeof(int64_t) * nstreams, &p))) return rc; d->eof = (const int64_t *)p; }
-  if ((rc = io.h2d(nullptr, sizeof(vb200_stream_block) * nstreams * h->max_blocks, &p))) return rc; d->plan = (vb200_stream_block *)p;
-  if ((rc = io.h2d(nullptr, sizeof(int32_t) * nstreams, &p))) return rc; d->nblocks = (int32_t *)p;
+  if (stage_pcm) d->pcm = io.in(h->pcm, pcm_bytes);
+  d->pcm_len = io.in(h->pcm_len, nstreams);
+  if (h->eof) d->eof = io.in(h->eof, nstreams);
+  d->plan = io.out<vb200_stream_block>((size_t)nstreams * h->max_blocks);
+  d->nblocks = io.out<int32_t>(nstreams);
   for (int w = 0; w < 2; w++) {
     if (h->cap[w] <= 0) continue;
-    const size_t cw = h->cap[w], n = c->dx[w].N / 2;
-    if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * cw * ch * VB200_FLOOR1_STRIDE, &p))) return rc; d->posts[w] = (int32_t *)p;
-    if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * cw * ch, &p))) return rc; d->nonzero[w] = (int32_t *)p;
-    if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * cw * ch * n, &p))) return rc; d->iwork[w] = (int32_t *)p;
-    if ((rc = io.h2d(nullptr, sizeof(float) * cw, &p))) return rc; d->ampmax_out[w] = (float *)p;
+    const size_t rows = curves * h->cap[w] * ch, n = c->dx[w].N / 2;
+    d->posts[w] = io.out<int32_t>(rows * VB200_FLOOR1_STRIDE);
+    d->nonzero[w] = io.out<int32_t>(rows);
+    d->iwork[w] = io.out<int32_t>(rows * n);
+    d->ampmax_out[w] = io.out<float>(h->cap[w]);
   }
-  return 0;
 }
 
 // host buffers of both streams calls: one synchronous H2D - compute - D2H round trip.  managed: every output but
@@ -2506,31 +2524,29 @@ static int streams_host(vb200_ctx *c, int nstreams, int blobno, bool managed, vb
   if ((rc = streams_open(c, h)) || nstreams <= 0) return rc;
   if ((rc = streams_inputs(h, "encode_streams"))) return rc;
   std::lock_guard<std::mutex> lk(c->mu);
-  cudaStream_t st = c->s_main;
   const size_t ch = c->setup.channels, pcap = (size_t)nstreams * h->max_blocks;
   const int curves = managed ? VB200_PACKETBLOBS : 1;
   HostIO io{c};
   vb200_streams_io d;
-  if ((rc = streams_stage(c, io, nstreams, managed, true, h, &d))) return rc;
-  rc = encode_streams_launch(c, nstreams, blobno, managed, &d, st, nullptr);
+  streams_stage(c, io, nstreams, managed, true, h, &d);
+  if (io.rc) return io.rc;
+  rc = encode_streams_launch(c, nstreams, blobno, managed, &d, c->s_main, nullptr);
   h->count[0] = d.count[0]; h->count[1] = d.count[1];
   if (rc) return rc;
-  CU(cudaMemcpyAsync(h->plan, d.plan, sizeof(vb200_stream_block) * pcap, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(h->nblocks, d.nblocks, sizeof(int32_t) * nstreams, cudaMemcpyDeviceToHost, st));
+  io.back(h->plan, d.plan, pcap);
+  io.back(h->nblocks, d.nblocks, nstreams);
   for (int w = 0; w < 2; w++) {
     const size_t nb = d.count[w], n = c->dx[w].N / 2, cw = h->cap[w];
     if (!nb) continue;
     for (int k = 0; k < curves; k++) {
-      const size_t r0 = k * cw * ch;
-      CU(cudaMemcpyAsync(h->posts[w] + r0 * VB200_FLOOR1_STRIDE, d.posts[w] + r0 * VB200_FLOOR1_STRIDE,
-                         sizeof(int32_t) * nb * ch * VB200_FLOOR1_STRIDE, cudaMemcpyDeviceToHost, st));
-      CU(cudaMemcpyAsync(h->nonzero[w] + r0, d.nonzero[w] + r0, sizeof(int32_t) * nb * ch, cudaMemcpyDeviceToHost, st));
-      CU(cudaMemcpyAsync(h->iwork[w] + r0 * n, d.iwork[w] + r0 * n, sizeof(int32_t) * nb * ch * n, cudaMemcpyDeviceToHost, st));
+      const size_t r0 = k * cw * ch, p0 = r0 * VB200_FLOOR1_STRIDE;
+      io.back(h->posts[w] + p0, d.posts[w] + p0, nb * ch * VB200_FLOOR1_STRIDE);
+      io.back(h->nonzero[w] + r0, d.nonzero[w] + r0, nb * ch);
+      io.back(h->iwork[w] + r0 * n, d.iwork[w] + r0 * n, nb * ch * n);
     }
-    CU(cudaMemcpyAsync(h->ampmax_out[w], d.ampmax_out[w], sizeof(float) * nb, cudaMemcpyDeviceToHost, st));
+    io.back(h->ampmax_out[w], d.ampmax_out[w], nb);
   }
-  CU(cudaStreamSynchronize(st));
-  return 0;
+  return io.sync();
 }
 
 extern "C" int vb200_encode_streams(vb200_ctx *c, int nstreams, int blobno, vb200_streams_io *h) {
@@ -2592,14 +2608,14 @@ extern "C" int vb200_residue_classify(vb200_ctx *c, int W, int nblocks, const in
   if (nblocks <= 0) return 0;
   std::lock_guard<std::mutex> lk(c->mu);
   const size_t ch = c->setup.channels, n = c->dx[W].N / 2;
+  const size_t rows = nblocks * ch;
   HostIO io{c};
-  void *di, *dz, *dc; int rc;
-  if ((rc = io.h2d(iwork, sizeof(int32_t) * nblocks * ch * n, &di))) return rc;
-  if ((rc = io.h2d(nonzero, sizeof(int32_t) * nblocks * ch, &dz))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(int32_t) * nblocks * ch * (size_t)(class_stride > 0 ? class_stride : 1), &dc))) return rc;
-  if ((rc = vb200_residue_classify_dev(c, W, nblocks, (const int32_t *)di, (const int32_t *)dz, (int32_t *)dc,
-                                       class_stride, c->s_main))) return rc;
-  if ((rc = io.d2h(classes, dc, sizeof(int32_t) * nblocks * ch * (size_t)class_stride))) return rc;
+  const int32_t *di = io.in(iwork, rows * n), *dz = io.in(nonzero, rows);
+  int32_t *dc = io.out<int32_t>(rows * (size_t)(class_stride > 0 ? class_stride : 1));
+  if (io.rc) return io.rc;
+  int rc;
+  if ((rc = vb200_residue_classify_dev(c, W, nblocks, di, dz, dc, class_stride, c->s_main))) return rc;
+  io.back(classes, dc, rows * (size_t)class_stride);
   return io.sync();
 }
 
@@ -2624,12 +2640,12 @@ extern "C" int vb200_floor1_inverse2(vb200_ctx *c, int W, int floor_sel, int nro
   std::lock_guard<std::mutex> lk(c->mu);
   const size_t n = c->dx[W].N / 2;
   HostIO io{c};
-  void *dp, *dz, *dd; int rc;
-  if ((rc = io.h2d(posts, sizeof(int32_t) * (size_t)nrows * VB200_FLOOR1_STRIDE, &dp))) return rc;
-  if ((rc = io.h2d(present, sizeof(int32_t) * (size_t)nrows, &dz))) return rc;
-  if ((rc = io.h2d(data, sizeof(float) * nrows * n, &dd))) return rc;
-  if ((rc = vb200_floor1_inverse2_dev(c, W, floor_sel, nrows, (const int32_t *)dp, (const int32_t *)dz, (float *)dd, c->s_main))) return rc;
-  if ((rc = io.d2h(data, dd, sizeof(float) * nrows * n))) return rc;
+  const int32_t *dp = io.in(posts, (size_t)nrows * VB200_FLOOR1_STRIDE), *dz = io.in(present, nrows);
+  float *dd = io.in(data, nrows * n);
+  if (io.rc) return io.rc;
+  int rc;
+  if ((rc = vb200_floor1_inverse2_dev(c, W, floor_sel, nrows, dp, dz, dd, c->s_main))) return rc;
+  io.back(data, dd, nrows * n);
   return io.sync();
 }
 
@@ -2706,20 +2722,19 @@ extern "C" int vb200_decode_dsp(vb200_ctx *c, int nstreams, int nblk, const int3
   const size_t nb = (size_t)nstreams * nblk;
   for (size_t i = 0; i < nb; i++) if (Wseq[i] < 0 || Wseq[i] > 1) return fail(VB200_EINVAL, "Wseq values must be 0/1");
   HostIO io{c};
-  void *dW, *dco, *dc, *dpo, *dp, *dps, *dpr; int rc;
-  if ((rc = io.h2d(Wseq, sizeof(int32_t) * nb, &dW))) return rc;
-  if ((rc = io.h2d(coef_off, sizeof(int64_t) * nb, &dco))) return rc;
-  if ((rc = io.h2d(res, sizeof(float) * (size_t)res_len, &dc))) return rc;
-  if ((rc = io.h2d(pcm_off, sizeof(int64_t) * nb, &dpo))) return rc;
+  const int32_t *dW = io.in(Wseq, nb);
+  const int64_t *dco = io.in(coef_off, nb);
+  float *dc = io.in(res, (size_t)res_len);
+  const int64_t *dpo = io.in(pcm_off, nb);
   const size_t pbytes = (pcm_s16 ? sizeof(int16_t) : sizeof(float)) * (size_t)nstreams * ch * (size_t)pcm_stride;
-  if ((rc = io.h2d(nullptr, pbytes, &dp))) return rc;
-  if ((rc = io.h2d(posts, sizeof(int32_t) * nb * ch * VB200_FLOOR1_STRIDE, &dps))) return rc;
-  if ((rc = io.h2d(present, sizeof(int32_t) * nb * ch, &dpr))) return rc;
+  void *dp = io.out<void>(pbytes);
+  const int32_t *dps = io.in(posts, nb * ch * VB200_FLOOR1_STRIDE), *dpr = io.in(present, nb * ch);
+  if (io.rc) return io.rc;
   CU(cudaMemsetAsync(dp, 0, pbytes, c->s_main));
-  if ((rc = vb200_decode_dsp_dev(c, nstreams, nblk, (const int32_t *)dW, (const int64_t *)dco, (float *)dc,
-                                 (const int32_t *)dps, (const int32_t *)dpr, (const int64_t *)dpo, dp, pcm_s16,
-                                 pcm_stride, c->s_main))) return rc;
-  if ((rc = io.d2h(pcm, dp, pbytes))) return rc;
+  int rc;
+  if ((rc = vb200_decode_dsp_dev(c, nstreams, nblk, dW, dco, dc, dps, dpr, dpo, dp, pcm_s16, pcm_stride, c->s_main)))
+    return rc;
+  io.back(pcm, dp, pbytes);
   return io.sync();
 }
 
@@ -2751,27 +2766,22 @@ static int blocks_check(const vb200_ctx *c, int nstreams, int nblk, const int32_
 // after its PCM
 struct HostCarry {
   vb200_decode_carry *h;
-  size_t ntask, tbytes;
+  size_t ntask, tlen;
   vb200_decode_carry d{};
   HostCarry(const vb200_ctx *c, int nstreams, vb200_decode_carry *carry)
-      : h(carry), ntask((size_t)nstreams * c->setup.channels),
-        tbytes(sizeof(float) * ntask * (size_t)(c->setup.blocksizes[1] / 2)) {}
+      : h(carry), ntask((size_t)nstreams * c->setup.channels), tlen(ntask * (size_t)(c->setup.blocksizes[1] / 2)) {}
   int check() const {
     for (size_t i = 0; i < ntask; i++)
       if (h->W[i] < -1 || h->W[i] > 1) return fail(VB200_EINVAL, "carried W must be -1, 0 or 1");
     return 0;
   }
-  int stage(HostIO &io) {
-    void *t, *w; int rc;
-    if ((rc = io.h2d(h->tail, tbytes, &t))) return rc;
-    if ((rc = io.h2d(h->W, sizeof(int32_t) * ntask, &w))) return rc;
-    d = vb200_decode_carry{(float *)t, (int32_t *)w};
-    return 0;
+  void stage(HostIO &io) {
+    d.tail = io.in(h->tail, tlen);
+    d.W = io.in(h->W, ntask);
   }
-  int write_back(HostIO &io) const {
-    int rc;
-    if ((rc = io.d2h(h->tail, d.tail, tbytes))) return rc;
-    return io.d2h(h->W, d.W, sizeof(int32_t) * ntask);
+  void write_back(HostIO &io) const {
+    io.back(h->tail, d.tail, tlen);
+    io.back(h->W, d.W, ntask);
   }
 };
 
@@ -2809,23 +2819,21 @@ extern "C" int vb200_decode_dsp_resume(vb200_ctx *c, int nstreams, int nblk, con
   if ((rc = k.check())) return rc;
   std::lock_guard<std::mutex> lk(c->mu);
   HostIO io{c};
-  void *dW, *dco, *dc, *dpo, *dp, *dps, *dpr, *dn = nullptr;
-  if ((rc = io.h2d(Wseq, sizeof(int32_t) * nb, &dW))) return rc;
-  if ((rc = io.h2d(coef_off, sizeof(int64_t) * nb, &dco))) return rc;
-  if ((rc = io.h2d(res, sizeof(float) * (size_t)res_len, &dc))) return rc;
-  if ((rc = io.h2d(pcm_off, sizeof(int64_t) * nb, &dpo))) return rc;
+  const int32_t *dW = io.in(Wseq, nb);
+  const int64_t *dco = io.in(coef_off, nb);
+  float *dc = io.in(res, (size_t)res_len);
+  const int64_t *dpo = io.in(pcm_off, nb);
   const size_t pbytes = (pcm_s16 ? sizeof(int16_t) : sizeof(float)) * (size_t)nstreams * ch * (size_t)pcm_stride;
-  if ((rc = io.h2d(nullptr, pbytes, &dp))) return rc;
-  if ((rc = io.h2d(posts, sizeof(int32_t) * nb * ch * VB200_FLOOR1_STRIDE, &dps))) return rc;
-  if ((rc = io.h2d(present, sizeof(int32_t) * nb * ch, &dpr))) return rc;
-  if (count && (rc = io.h2d(count, sizeof(int32_t) * nstreams, &dn))) return rc;
-  if ((rc = k.stage(io))) return rc;
+  void *dp = io.out<void>(pbytes);
+  const int32_t *dps = io.in(posts, nb * ch * VB200_FLOOR1_STRIDE), *dpr = io.in(present, nb * ch);
+  const int32_t *dn = count ? io.in(count, nstreams) : nullptr;
+  k.stage(io);
+  if (io.rc) return io.rc;
   CU(cudaMemsetAsync(dp, 0, pbytes, c->s_main));
-  if ((rc = vb200_decode_dsp_resume_dev(c, nstreams, nblk, (const int32_t *)dn, (const int32_t *)dW,
-                                        (const int64_t *)dco, (float *)dc, (const int32_t *)dps, (const int32_t *)dpr,
-                                        (const int64_t *)dpo, dp, pcm_s16, pcm_stride, &k.d, c->s_main))) return rc;
-  if ((rc = io.d2h(pcm, dp, pbytes))) return rc;
-  if ((rc = k.write_back(io))) return rc;
+  if ((rc = vb200_decode_dsp_resume_dev(c, nstreams, nblk, dn, dW, dco, dc, dps, dpr, dpo, dp, pcm_s16, pcm_stride,
+                                        &k.d, c->s_main))) return rc;
+  io.back(pcm, dp, pbytes);
+  k.write_back(io);
   return io.sync();
 }
 
@@ -3064,21 +3072,18 @@ extern "C" int vb200_decode_entropy(vb200_ctx *c, int nblocks, const int32_t *Ws
   std::lock_guard<std::mutex> lk(c->mu);
   const size_t nb = (size_t)nblocks;
   HostIO io{c};
-  void *dW, *dpo, *dpb, *dd, *dco, *dr, *dps, *dpr;
-  if ((rc = io.h2d(Wseq, sizeof(int32_t) * nb, &dW))) return rc;
-  if ((rc = io.h2d(pkt_off, sizeof(int64_t) * nb, &dpo))) return rc;
-  if ((rc = io.h2d(pkt_bytes, sizeof(int32_t) * nb, &dpb))) return rc;
-  if ((rc = io.h2d_packets(data, data_bytes, &dd))) return rc;
-  if ((rc = io.h2d(coef_off, sizeof(int64_t) * nb, &dco))) return rc;
-  if ((rc = io.h2d(res, sizeof(float) * (size_t)res_len, &dr))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(int32_t) * nb * ch * VB200_FLOOR1_STRIDE, &dps))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(int32_t) * nb * ch, &dpr))) return rc;
-  if ((rc = vb200_decode_entropy_dev(c, nblocks, (const int32_t *)dW, (const int64_t *)dpo, (const int32_t *)dpb,
-                                     (const uint8_t *)dd, (const int64_t *)dco, (float *)dr, (int32_t *)dps,
-                                     (int32_t *)dpr, c->s_main))) return rc;
-  if ((rc = io.d2h(res, dr, sizeof(float) * (size_t)res_len))) return rc;
-  if ((rc = io.d2h(posts, dps, sizeof(int32_t) * nb * ch * VB200_FLOOR1_STRIDE))) return rc;
-  if ((rc = io.d2h(present, dpr, sizeof(int32_t) * nb * ch))) return rc;
+  const int32_t *dW = io.in(Wseq, nb);
+  const int64_t *dpo = io.in(pkt_off, nb);
+  const int32_t *dpb = io.in(pkt_bytes, nb);
+  const uint8_t *dd = io.packets(data, data_bytes);
+  const int64_t *dco = io.in(coef_off, nb);
+  float *dr = io.in(res, (size_t)res_len);
+  int32_t *dps = io.out<int32_t>(nb * ch * VB200_FLOOR1_STRIDE), *dpr = io.out<int32_t>(nb * ch);
+  if (io.rc) return io.rc;
+  if ((rc = vb200_decode_entropy_dev(c, nblocks, dW, dpo, dpb, dd, dco, dr, dps, dpr, c->s_main))) return rc;
+  io.back(res, dr, (size_t)res_len);
+  io.back(posts, dps, nb * ch * VB200_FLOOR1_STRIDE);
+  io.back(present, dpr, nb * ch);
   return io.sync();
 }
 
@@ -3121,25 +3126,23 @@ extern "C" int vb200_decode_packets_resume(vb200_ctx *c, int nstreams, int nblk,
   if ((rc = k.check())) return rc;
   std::lock_guard<std::mutex> lk(c->mu);
   HostIO io{c};
-  void *dW, *dco, *dc, *dpo, *dp, *dko, *dkb, *dd, *dn = nullptr;
-  if ((rc = io.h2d(Wseq, sizeof(int32_t) * nb, &dW))) return rc;
-  if ((rc = io.h2d(coef_off, sizeof(int64_t) * nb, &dco))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(float) * (size_t)(res_len ? res_len : 1), &dc))) return rc;
-  if ((rc = io.h2d(pcm_off, sizeof(int64_t) * nb, &dpo))) return rc;
+  const int32_t *dW = io.in(Wseq, nb);
+  const int64_t *dco = io.in(coef_off, nb);
+  float *dc = io.out<float>((size_t)(res_len ? res_len : 1));
+  const int64_t *dpo = io.in(pcm_off, nb);
   const size_t pbytes = (pcm_s16 ? sizeof(int16_t) : sizeof(float)) * (size_t)nstreams * ch * (size_t)pcm_stride;
-  if ((rc = io.h2d(nullptr, pbytes, &dp))) return rc;
-  if ((rc = io.h2d(pkt_off, sizeof(int64_t) * nb, &dko))) return rc;
-  if ((rc = io.h2d(pkt_bytes, sizeof(int32_t) * nb, &dkb))) return rc;
-  if ((rc = io.h2d_packets(data, data_bytes, &dd))) return rc;
-  if (count && (rc = io.h2d(count, sizeof(int32_t) * nstreams, &dn))) return rc;
-  if ((rc = k.stage(io))) return rc;
+  void *dp = io.out<void>(pbytes);
+  const int64_t *dko = io.in(pkt_off, nb);
+  const int32_t *dkb = io.in(pkt_bytes, nb);
+  const uint8_t *dd = io.packets(data, data_bytes);
+  const int32_t *dn = count ? io.in(count, nstreams) : nullptr;
+  k.stage(io);
+  if (io.rc) return io.rc;
   CU(cudaMemsetAsync(dp, 0, pbytes, c->s_main));
-  if ((rc = vb200_decode_packets_resume_dev(c, nstreams, nblk, (const int32_t *)dn, (const int32_t *)dW,
-                                            (const int64_t *)dco, (float *)dc, (const int64_t *)dko,
-                                            (const int32_t *)dkb, (const uint8_t *)dd, (const int64_t *)dpo, dp,
-                                            pcm_s16, pcm_stride, &k.d, c->s_main))) return rc;
-  if ((rc = io.d2h(pcm, dp, pbytes))) return rc;
-  if ((rc = k.write_back(io))) return rc;
+  if ((rc = vb200_decode_packets_resume_dev(c, nstreams, nblk, dn, dW, dco, dc, dko, dkb, dd, dpo, dp, pcm_s16,
+                                            pcm_stride, &k.d, c->s_main))) return rc;
+  io.back(pcm, dp, pbytes);
+  k.write_back(io);
   return io.sync();
 }
 
@@ -3277,23 +3280,22 @@ extern "C" int vb200_decode_streams_packets(vb200_ctx *c, int nstreams, int max_
   const int ch = c->setup.channels;
   const size_t el = pcm_s16 ? sizeof(int16_t) : sizeof(float);
   HostIO io{c};
-  void *dn, *di, *dd, *dp, *db, *dout;
-  if ((rc = io.h2d(npkt, sizeof(int32_t) * nstreams, &dn))) return rc;
-  if ((rc = io.h2d(info, sizeof(vb200_packet_info) * n, &di))) return rc;
-  if ((rc = io.h2d_packets(data, data_bytes, &dd))) return rc;
-  if ((rc = io.h2d(nullptr, el * (size_t)std::max<int64_t>(pcm_cap, 1), &dp))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(int64_t) * (nstreams + 1), &db))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(vb200_decoded_packet) * n, &dout))) return rc;
-  if ((rc = vb200_decode_streams_packets_dev(c, nstreams, max_packets, (const int32_t *)dn,
-                                             (const vb200_packet_info *)di, (const uint8_t *)dd, d_carry, pcm_s16, dp,
-                                             pcm_cap, (int64_t *)db, (vb200_decoded_packet *)dout, c->s_main)))
+  const int32_t *dn = io.in(npkt, nstreams);
+  const vb200_packet_info *di = io.in(info, n);
+  const uint8_t *dd = io.packets(data, data_bytes);
+  void *dp = io.out<void>(el * (size_t)std::max<int64_t>(pcm_cap, 1));
+  int64_t *db = io.out<int64_t>(nstreams + 1);
+  vb200_decoded_packet *dout = io.out<vb200_decoded_packet>(n);
+  if (io.rc) return io.rc;
+  if ((rc = vb200_decode_streams_packets_dev(c, nstreams, max_packets, dn, di, dd, d_carry, pcm_s16, dp, pcm_cap, db,
+                                             dout, c->s_main)))
     return rc;
-  if ((rc = io.d2h(pcm_base, db, sizeof(int64_t) * (nstreams + 1)))) return rc;
-  if ((rc = io.d2h(out, dout, sizeof(vb200_decoded_packet) * n))) return rc;
+  io.back(pcm_base, db, nstreams + 1);
+  io.back(out, dout, n);
   if ((rc = io.sync())) return rc;
   const int64_t total = pcm_base[nstreams] * ch;
   if (total > pcm_cap) return fail(VB200_EINVAL, "the PCM does not fit pcm_cap (pcm_base is filled)");
-  if (total && (rc = io.d2h(pcm, dp, el * (size_t)total))) return rc;
+  if (total) io.back(pcm, dp, el * (size_t)total);
   return io.sync();
 }
 
@@ -3331,17 +3333,15 @@ extern "C" int vb200_decode_streams_index(vb200_ctx *c, int nstreams, int max_pa
   std::lock_guard<std::mutex> lk(c->mu);
   const size_t n = (size_t)nstreams * max_packets;
   HostIO io{c};
-  void *dn, *di, *dd, *dl, *dout;
-  if ((rc = io.h2d(npkt, sizeof(int32_t) * nstreams, &dn))) return rc;
-  if ((rc = io.h2d(info, sizeof(vb200_packet_info) * n, &di))) return rc;
-  if ((rc = io.h2d_packets(data, data_bytes, &dd))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(int64_t) * nstreams, &dl))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(vb200_decoded_packet) * n, &dout))) return rc;
-  if ((rc = vb200_decode_streams_index_dev(c, nstreams, max_packets, (const int32_t *)dn, (const vb200_packet_info *)di,
-                                           (const uint8_t *)dd, (int64_t *)dl, (vb200_decoded_packet *)dout,
-                                           c->s_main))) return rc;
-  if ((rc = io.d2h(length, dl, sizeof(int64_t) * nstreams))) return rc;
-  if ((rc = io.d2h(out, dout, sizeof(vb200_decoded_packet) * n))) return rc;
+  const int32_t *dn = io.in(npkt, nstreams);
+  const vb200_packet_info *di = io.in(info, n);
+  const uint8_t *dd = io.packets(data, data_bytes);
+  int64_t *dl = io.out<int64_t>(nstreams);
+  vb200_decoded_packet *dout = io.out<vb200_decoded_packet>(n);
+  if (io.rc) return io.rc;
+  if ((rc = vb200_decode_streams_index_dev(c, nstreams, max_packets, dn, di, dd, dl, dout, c->s_main))) return rc;
+  io.back(length, dl, nstreams);
+  io.back(out, dout, n);
   return io.sync();
 }
 
@@ -3424,18 +3424,17 @@ extern "C" int vb200_decode_ranges(vb200_ctx *c, int nstreams, int max_packets, 
   const size_t n = (size_t)nstreams * max_packets;      // nstreams >= 1: a request names a stream
   const size_t pbytes = (pcm_s16 ? sizeof(int16_t) : sizeof(float)) * (size_t)nreq * c->setup.channels * out_stride;
   HostIO io{c};
-  void *dn, *di, *dd, *dq, *dp, *dg;
-  if ((rc = io.h2d(npkt, sizeof(int32_t) * nstreams, &dn))) return rc;
-  if ((rc = io.h2d(info, sizeof(vb200_packet_info) * n, &di))) return rc;
-  if ((rc = io.h2d_packets(data, data_bytes, &dd))) return rc;
-  if ((rc = io.h2d(req, sizeof(vb200_pcm_range) * nreq, &dq))) return rc;
-  if ((rc = io.h2d(nullptr, std::max<size_t>(pbytes, 1), &dp))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(int32_t) * nreq, &dg))) return rc;
-  if ((rc = vb200_decode_ranges_dev(c, nstreams, max_packets, (const int32_t *)dn, (const vb200_packet_info *)di,
-                                    (const uint8_t *)dd, nreq, (const vb200_pcm_range *)dq, pcm_s16, dp, out_stride,
-                                    (int32_t *)dg, c->s_main))) return rc;
-  if (pbytes && (rc = io.d2h(pcm, dp, pbytes))) return rc;
-  if ((rc = io.d2h(got, dg, sizeof(int32_t) * nreq))) return rc;
+  const int32_t *dn = io.in(npkt, nstreams);
+  const vb200_packet_info *di = io.in(info, n);
+  const uint8_t *dd = io.packets(data, data_bytes);
+  const vb200_pcm_range *dq = io.in(req, nreq);
+  void *dp = io.out<void>(std::max<size_t>(pbytes, 1));
+  int32_t *dg = io.out<int32_t>(nreq);
+  if (io.rc) return io.rc;
+  if ((rc = vb200_decode_ranges_dev(c, nstreams, max_packets, dn, di, dd, nreq, dq, pcm_s16, dp, out_stride, dg,
+                                    c->s_main))) return rc;
+  if (pbytes) io.back(pcm, dp, pbytes);
+  io.back(got, dg, nreq);
   return io.sync();
 }
 
@@ -3672,9 +3671,11 @@ extern "C" int vb200_encode_entropy_dev(vb200_ctx *c, int W, int nblocks, const 
 }
 
 // host forms: packets of the strided device buffer packed back to back, then the counts, offsets and bytes copied
-// back (the bytes only when they fit data_cap).  Synchronises.
-static int packets_pack_d2h(vb200_ctx *c, int nblocks, const uint8_t *d_strided, int64_t stride, const int32_t *d_bits,
-                            int64_t *pkt_off, int32_t *pkt_bits, uint8_t *data, int64_t data_cap, cudaStream_t st) {
+// back through io (the bytes only when they fit data_cap).  Synchronises.
+static int packets_pack_d2h(HostIO &io, int nblocks, const uint8_t *d_strided, int64_t stride, const int32_t *d_bits,
+                            int64_t *pkt_off, int32_t *pkt_bits, uint8_t *data, int64_t data_cap) {
+  vb200_ctx *c = io.c;
+  cudaStream_t st = c->s_main;
   long long *doff;
   uint8_t *dpk;
   int rc;
@@ -3686,15 +3687,14 @@ static int packets_pack_d2h(vb200_ctx *c, int nblocks, const uint8_t *d_strided,
   if ((rc = post_launch(c))) return rc;
   k_packet_gather<<<grid_for(c, nblocks, 8), 256, 0, st>>>(d_strided, stride, d_bits, doff, nblocks, data_cap, dpk);
   if ((rc = post_launch(c))) return rc;
-  int64_t total = 0;
-  CU(cudaMemcpyAsync(pkt_bits, d_bits, sizeof(int32_t) * nblocks, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(pkt_off, doff, sizeof(int64_t) * nblocks, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(&total, (int64_t *)doff + nblocks, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
+  long long total = 0;
+  io.back(pkt_bits, d_bits, nblocks);
+  io.back(pkt_off, (const int64_t *)doff, nblocks);
+  io.back(&total, doff + nblocks, 1);
+  if ((rc = io.sync())) return rc;
   if (total > data_cap) return fail(VB200_EINVAL, "packets exceed data_cap (pkt_bits filled)");
-  if (total) CU(cudaMemcpyAsync(data, dpk, (size_t)total, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
-  return 0;
+  if (total) io.back(data, dpk, total);
+  return io.sync();
 }
 
 extern "C" int vb200_encode_entropy(vb200_ctx *c, int W, int nblocks, const vb200_block_desc *desc, const int32_t *posts,
@@ -3710,18 +3710,14 @@ extern "C" int vb200_encode_entropy(vb200_ctx *c, int W, int nblocks, const vb20
   const size_t nb = (size_t)nblocks, ch = c->setup.channels, n = c->dx[W].N / 2;
   const int64_t stride = c->eent.bound[W];
   HostIO io{c};
-  void *dd, *dp, *dz, *di, *db, *ds;
-  if ((rc = io.h2d(desc, sizeof(vb200_block_desc) * nb, &dd))) return rc;
-  if ((rc = io.h2d(posts, sizeof(int32_t) * nb * ch * VB200_FLOOR1_STRIDE, &dp))) return rc;
-  if ((rc = io.h2d(nonzero, sizeof(int32_t) * nb * ch, &dz))) return rc;
-  if ((rc = io.h2d(iwork, sizeof(int32_t) * nb * ch * n, &di))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(int32_t) * nb, &db))) return rc;
-  if ((rc = io.h2d(nullptr, (size_t)stride * nb, &ds))) return rc;
-  if ((rc = vb200_encode_entropy_dev(c, W, nblocks, (const vb200_block_desc *)dd, (const int32_t *)dp,
-                                     (const int32_t *)dz, (const int32_t *)di, stride, (int32_t *)db, (uint8_t *)ds,
-                                     c->s_main))) return rc;
-  return packets_pack_d2h(c, nblocks, (const uint8_t *)ds, stride, (const int32_t *)db, pkt_off, pkt_bits, data,
-                          data_cap, c->s_main);
+  const vb200_block_desc *dd = io.in(desc, nb);
+  const int32_t *dp = io.in(posts, nb * ch * VB200_FLOOR1_STRIDE), *dz = io.in(nonzero, nb * ch),
+                *di = io.in(iwork, nb * ch * n);
+  int32_t *db = io.out<int32_t>(nb);
+  uint8_t *ds = io.out<uint8_t>((size_t)stride * nb);
+  if (io.rc) return io.rc;
+  if ((rc = vb200_encode_entropy_dev(c, W, nblocks, dd, dp, dz, di, stride, db, ds, c->s_main))) return rc;
+  return packets_pack_d2h(io, nblocks, ds, stride, db, pkt_off, pkt_bits, data, data_cap);
 }
 
 // Both block packet calls: the chain into staged outputs, the entropy coder, the packets packed back to back.
@@ -3749,10 +3745,10 @@ static int encode_packets(vb200_ctx *c, int W, int nstreams, int bps, int blobno
   cudaStream_t st = c->s_main;
   HostIO io{c};
   vb200_encode_io d = *h;
-  void *dbits, *dstr;
-  if ((rc = enc_stage(io, h, &d, ch, N, nstreams, bps, curves))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(int32_t) * curves * nb, &dbits))) return rc;
-  if ((rc = io.h2d(nullptr, (size_t)stride * curves * nb, &dstr))) return rc;
+  enc_stage(io, h, &d, ch, N, nstreams, bps, curves);
+  int32_t *dbits = io.out<int32_t>(curves * nb);
+  uint8_t *dstr = io.out<uint8_t>((size_t)stride * curves * nb);
+  if (io.rc) return io.rc;
   EncScratch S;
   MgdScratch M;
   if ((rc = carve(managed ? c->mgd : c->enc, [&](Carve &k) {
@@ -3761,12 +3757,11 @@ static int encode_packets(vb200_ctx *c, int W, int nstreams, int bps, int blobno
        }))) return rc;
   if ((rc = scratch_begin(c, st))) return rc;
   if ((rc = encode_launch(c, W, nstreams, bps, blobno, &d, S, st, managed ? &M : nullptr))) return rc;
-  if ((rc = encode_entropy_launch(c, W, (int)nb, d.desc, d.posts, d.nonzero, (const int32_t *)d.iwork, stride,
-                                  (int32_t *)dbits, (uint8_t *)dstr, st, managed, managed ? (long long)nb : 0))) return rc;
+  if ((rc = encode_entropy_launch(c, W, (int)nb, d.desc, d.posts, d.nonzero, (const int32_t *)d.iwork, stride, dbits,
+                                  dstr, st, managed, managed ? (long long)nb : 0))) return rc;
   if ((rc = scratch_end(c, st))) return rc;
-  if ((rc = io.d2h(h->ampmax_out, d.ampmax_out, sizeof(float) * nb))) return rc;
-  return packets_pack_d2h(c, curves * (int)nb, (const uint8_t *)dstr, stride, (const int32_t *)dbits, pkt_off, pkt_bits,
-                          data, data_cap, st);
+  io.back(h->ampmax_out, d.ampmax_out, nb);
+  return packets_pack_d2h(io, curves * (int)nb, dstr, stride, dbits, pkt_off, pkt_bits, data, data_cap);
 }
 
 extern "C" int vb200_encode_packets(vb200_ctx *c, int W, int nstreams, int bps, int blobno, const vb200_encode_io *h,
@@ -3868,20 +3863,15 @@ extern "C" int vb200_bitrate_addblocks(vb200_ctx *c, int nstreams, int max_block
   std::lock_guard<std::mutex> lk(c->mu);
   const size_t n = (size_t)nstreams * max_blocks;
   HostIO io{c};
-  void *dc, *dw, *db, *ds, *dch, *dby;
+  const int32_t *dc = io.in(count, nstreams), *dw = io.in(W, n), *db = io.in(pkt_bits, n * VB200_PACKETBLOBS);
+  vb200_bitrate_state *ds = io.in(state, nstreams);
   // choice and bytes go in as well: entries past count[s] come back as the caller left them
-  if ((rc = io.h2d(count, sizeof(int32_t) * nstreams, &dc))) return rc;
-  if ((rc = io.h2d(W, sizeof(int32_t) * n, &dw))) return rc;
-  if ((rc = io.h2d(pkt_bits, sizeof(int32_t) * n * VB200_PACKETBLOBS, &db))) return rc;
-  if ((rc = io.h2d(state, sizeof(vb200_bitrate_state) * nstreams, &ds))) return rc;
-  if ((rc = io.h2d(choice, sizeof(int32_t) * n, &dch))) return rc;
-  if ((rc = io.h2d(bytes, sizeof(int32_t) * n, &dby))) return rc;
-  if ((rc = vb200_bitrate_addblocks_dev(c, nstreams, max_blocks, (const int32_t *)dc, (const int32_t *)dw,
-                                        (const int32_t *)db, (vb200_bitrate_state *)ds, (int32_t *)dch, (int32_t *)dby,
-                                        c->s_main))) return rc;
-  if ((rc = io.d2h(state, ds, sizeof(vb200_bitrate_state) * nstreams))) return rc;
-  if ((rc = io.d2h(choice, dch, sizeof(int32_t) * n))) return rc;
-  if ((rc = io.d2h(bytes, dby, sizeof(int32_t) * n))) return rc;
+  int32_t *dch = io.in(choice, n), *dby = io.in(bytes, n);
+  if (io.rc) return io.rc;
+  if ((rc = vb200_bitrate_addblocks_dev(c, nstreams, max_blocks, dc, dw, db, ds, dch, dby, c->s_main))) return rc;
+  io.back(state, ds, nstreams);
+  io.back(choice, dch, n);
+  io.back(bytes, dby, n);
   return io.sync();
 }
 
@@ -4040,14 +4030,12 @@ static int streams_packets(vb200_ctx *c, int nstreams, int blobno, bool managed,
   const size_t n = (size_t)nstreams * h->max_blocks;
   HostIO own{c};
   HostIO &io = staged ? *staged : own;
-  void *p;
   vb200_streams_io d;
-  if ((rc = streams_stage(c, io, nstreams, managed, !staged, h, &d))) return rc;
+  streams_stage(c, io, nstreams, managed, !staged, h, &d);
+  char *dblob = carry ? io.in(cblob.data(), cblob.size()) : nullptr;
+  if (io.rc) return io.rc;
   CarryDev K{}, *Kp = nullptr;
-  char *dblob = nullptr;
   if (carry) {
-    if ((rc = io.h2d(cblob.data(), cblob.size(), &p))) return rc;
-    dblob = (char *)p;
     auto dev = [&](auto *hp) { return (decltype(hp))(dblob + ((char *)hp - cblob.data())); };
     K.pc = dev(hb.pc); K.marks = dev(hb.marks); K.cap = ccap; K.env = dev(hb.env); K.br = dev(hb.br);
     K.first = dev(hb.first); K.count = dev(hb.count); K.overflow = dev(hb.overflow);
@@ -4102,16 +4090,16 @@ static int streams_packets(vb200_ctx *c, int nstreams, int blobno, bool managed,
   else
     k_stream_gather<<<grid_for(c, (int)n, 8), 256, 0, st>>>(A);
   if ((rc = post_launch(c))) return rc;
-  int64_t total = 0;
-  if (carry) CU(cudaMemcpyAsync(cblob.data(), dblob, cblob.size(), cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(h->plan, d.plan, sizeof(vb200_stream_block) * n, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(h->nblocks, d.nblocks, sizeof(int32_t) * nstreams, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(info, dinfo, sizeof(vb200_packet_info) * n, cudaMemcpyDeviceToHost, st));
-  CU(cudaMemcpyAsync(&total, off + n, sizeof(int64_t), cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
+  long long total = 0;
+  if (carry) io.back(cblob.data(), dblob, cblob.size());
+  io.back(h->plan, d.plan, n);
+  io.back(h->nblocks, d.nblocks, nstreams);
+  io.back(info, dinfo, n);
+  io.back(&total, off + n, 1);
+  if ((rc = io.sync())) return rc;
   if (total > data_cap) return fail(VB200_EINVAL, "packets exceed data_cap (info filled)");
-  if (total) CU(cudaMemcpyAsync(data, dpk, (size_t)total, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
+  if (total) io.back(data, dpk, total);
+  if ((rc = io.sync())) return rc;
   if (carry) carry_unpack(c, nstreams, ccap, hb, carry);
   return 0;
 }
@@ -4248,12 +4236,8 @@ static int pcm_packets(vb200_ctx *c, int nstreams, int blobno, bool managed, vb2
   cudaStream_t st = c->s_main;
   const bool s16 = h->pcm_fmt == VB200_PCM_S16_INTERLEAVED;
   HostIO io{c};
-  void *din, *dblob;
   const size_t in_bytes = (size_t)nstreams * ch * (size_t)h->stream_stride * (s16 ? 2 : 4);
-  if ((rc = io.h2d(in_bytes ? h->pcm : nullptr, std::max<size_t>(in_bytes, 1), &din))) return rc;
-  float *dtl;
-  if ((rc = carve(c->ptl, [&](Carve &k) { dtl = k.take<float>((size_t)nstreams * ch * tstride); }))) return rc;
-  CU(cudaMemsetAsync(dtl, 0, sizeof(float) * nstreams * ch * tstride, st));   // columns past a stream's len read as 0
+  const void *din = io.in(in_bytes ? h->pcm : nullptr, std::max<size_t>(in_bytes, 1));
   // one staged buffer: the streams, the jobs (preamble jobs first) and the filters of every (stream, channel)
   PcmStream *bs; LpcJob *bj; float *bf;
   auto layout = [&](Carve &k) {
@@ -4265,8 +4249,12 @@ static int pcm_packets(vb200_ctx *c, int nstreams, int blobno, bool managed, vb2
   std::vector<char> blob(sz.off);
   Carve at{blob.data(), 0};
   layout(at);
-  if ((rc = io.h2d(nullptr, blob.size(), &dblob))) return rc;
-  auto dev = [&](auto *hp) { return (decltype(hp))((char *)dblob + ((char *)hp - blob.data())); };
+  char *dblob = io.out<char>(blob.size());
+  if (io.rc) return io.rc;
+  float *dtl;
+  if ((rc = carve(c->ptl, [&](Carve &k) { dtl = k.take<float>((size_t)nstreams * ch * tstride); }))) return rc;
+  CU(cudaMemsetAsync(dtl, 0, sizeof(float) * nstreams * ch * tstride, st));   // columns past a stream's len read as 0
+  auto dev = [&](auto *hp) { return (decltype(hp))(dblob + ((char *)hp - blob.data())); };
   const long long stride = h->stream_stride;
   int npre = 0, nj = 0;
   for (int pass = 0; pass < 2; pass++)
@@ -4317,8 +4305,8 @@ static int pcm_packets(vb200_ctx *c, int nstreams, int blobno, bool managed, vb2
   rc = streams_packets(c, nstreams, blobno, managed, &d, info, data, data_cap, enc.data(), &io);
   h->count[0] = d.count[0]; h->count[1] = d.count[1];
   if (rc) return rc;
-  CU(cudaMemcpyAsync(bf, dev(bf), (size_t)nstreams * fb, cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));
+  io.back(bf, dev(bf), (size_t)nstreams * ch * LPC_FILTER_FLOATS);
+  if ((rc = io.sync())) return rc;
   for (int s = 0; s < nstreams; s++) {
     char *cs = (char *)carry + (size_t)s * pb;
     PcmCarry &p = pc[s];
@@ -4355,36 +4343,33 @@ extern "C" int vb200_lpc_extrapolate(vb200_ctx *c, int nrows, int order, const f
   std::lock_guard<std::mutex> lk(c->mu);
   cudaStream_t st = c->s_main;
   HostIO io{c};
-  void *dd, *dj, *dc, *dp, *dout = nullptr;
-  int rc;
-  if ((rc = io.h2d(data, sizeof(float) * (size_t)nrows * data_stride, &dd))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(float) * (size_t)nrows * order, &dc))) return rc;
-  if ((rc = io.h2d(nullptr, sizeof(float) * (size_t)nrows * order, &dp))) return rc;
-  if (count > 0 && (rc = io.h2d(nullptr, sizeof(float) * (size_t)nrows * out_stride, &dout))) return rc;
+  const float *dd = io.in(data, (size_t)nrows * data_stride);
+  float *dc = io.out<float>((size_t)nrows * order), *dp = io.out<float>((size_t)nrows * order);
+  float *dout = count > 0 ? io.out<float>((size_t)nrows * out_stride) : nullptr;
   std::vector<LpcJob> jobs(nrows);
   for (int r = 0; r < nrows; r++) {
     LpcJob &J = jobs[r];
     J = LpcJob{};
     J.src = dd; J.off = (long long)r * data_stride; J.step = 1; J.n = n[r];
-    J.coef = (float *)dc + (size_t)r * order; J.prime = (float *)dp + (size_t)r * order;
+    J.coef = dc + (size_t)r * order; J.prime = dp + (size_t)r * order;
   }
-  if ((rc = io.h2d(jobs.data(), sizeof(LpcJob) * nrows, &dj))) return rc;
+  const LpcJob *dj = io.in(jobs.data(), nrows);
+  if (io.rc) return io.rc;
   const int grid = grid_for(c, (nrows + LPC_WARPS - 1) / LPC_WARPS, 8);
-  if (order == LPC_PRE) k_lpc_filter<LPC_PRE><<<grid, 32 * LPC_WARPS, 0, st>>>((const LpcJob *)dj, nrows, 0);
-  else k_lpc_filter<LPC_TAIL><<<grid, 32 * LPC_WARPS, 0, st>>>((const LpcJob *)dj, nrows, 0);
+  if (order == LPC_PRE) k_lpc_filter<LPC_PRE><<<grid, 32 * LPC_WARPS, 0, st>>>(dj, nrows, 0);
+  else k_lpc_filter<LPC_TAIL><<<grid, 32 * LPC_WARPS, 0, st>>>(dj, nrows, 0);
+  int rc;
   if ((rc = post_launch(c))) return rc;
   if (count > 0) {
     if (order == LPC_PRE)
-      k_lpc_predict<LPC_PRE><<<(nrows + 127) / 128, 128, 0, st>>>(nrows, (const float *)dc, (const float *)dp, count,
-                                                                  (float *)dout, out_stride);
+      k_lpc_predict<LPC_PRE><<<(nrows + 127) / 128, 128, 0, st>>>(nrows, dc, dp, count, dout, out_stride);
     else
-      k_lpc_predict<LPC_TAIL><<<(nrows + 127) / 128, 128, 0, st>>>(nrows, (const float *)dc, (const float *)dp, count,
-                                                                   (float *)dout, out_stride);
+      k_lpc_predict<LPC_TAIL><<<(nrows + 127) / 128, 128, 0, st>>>(nrows, dc, dp, count, dout, out_stride);
     if ((rc = post_launch(c))) return rc;
     CU(cudaMemcpy2DAsync(out, sizeof(float) * out_stride, dout, sizeof(float) * out_stride, sizeof(float) * count,
                          nrows, cudaMemcpyDeviceToHost, st));
   }
-  if ((rc = io.d2h(coeff, dc, sizeof(float) * (size_t)nrows * order))) return rc;
+  io.back(coeff, dc, (size_t)nrows * order);
   return io.sync();
 }
 
@@ -4456,17 +4441,17 @@ static int envelope_search_host(vb200_ctx *c, int nstreams, const void *pcm, int
   std::lock_guard<std::mutex> lk(c->mu);
   const int ch = c->setup.channels;
   const size_t pcm_bytes = (fmt == VB200_PCM_S16_INTERLEAVED ? sizeof(int16_t) : sizeof(float)) * (size_t)nstreams * ch * (size_t)stride;
-  const size_t st_bytes = sizeof(int32_t) * (size_t)nstreams * VB200_VE_STATE_WORDS(ch);
+  const size_t st_len = (size_t)nstreams * VB200_VE_STATE_WORDS(ch);
   HostIO io{c};
-  void *dn = nullptr, *dp, *ds, *dr;
-  if (steps_per_stream && (rc = io.h2d(steps_per_stream, sizeof(int32_t) * (size_t)nstreams, &dn))) return rc;
-  if ((rc = io.h2d(pcm, pcm_bytes, &dp))) return rc;
-  if ((rc = io.h2d(state, st_bytes, &ds))) return rc;
-  if ((rc = io.h2d(nullptr, (size_t)nstreams * nsteps, &dr))) return rc;
-  if ((rc = envelope_search_launch(c, nstreams, dp, fmt, stride, first_step, nsteps, (int32_t *)ds, (uint8_t *)dr,
-                                   c->s_main, (const int32_t *)dn, nullptr))) return rc;
-  if ((rc = io.d2h(state, ds, st_bytes))) return rc;
-  if ((rc = io.d2h(ret, dr, (size_t)nstreams * nsteps))) return rc;
+  const int32_t *dn = steps_per_stream ? io.in(steps_per_stream, nstreams) : nullptr;
+  const void *dp = io.in(pcm, pcm_bytes);
+  int32_t *ds = io.in(state, st_len);
+  uint8_t *dr = io.out<uint8_t>((size_t)nstreams * nsteps);
+  if (io.rc) return io.rc;
+  if ((rc = envelope_search_launch(c, nstreams, dp, fmt, stride, first_step, nsteps, ds, dr, c->s_main, dn, nullptr)))
+    return rc;
+  io.back(state, ds, st_len);
+  io.back(ret, dr, (size_t)nstreams * nsteps);
   return io.sync();
 }
 
