@@ -236,6 +236,7 @@ typedef struct vb200_phaseA_io {
   float *tap_mdct_raw;
 } vb200_phaseA_io;
 int vb200_analysis_phaseA_dev(vb200_ctx*, int W, int nblocks, const vb200_phaseA_io *d_io, void *stream);
+/* host buffers: the blocks are pipelined in chunks over the device buffer sets, as by vb200_encode_dsp */
 int vb200_analysis_phaseA    (vb200_ctx*, int W, int nblocks, const vb200_phaseA_io *io);
 
 /* Stream mode: `nstreams` streams of `blocks_per_stream` consecutive blocks

@@ -27,6 +27,20 @@ CASES = [(2, 44100, 0.5), (1, 22050, 0.3), (6, 48000, 0.2), (2, 44100, -0.1)]
 PAGINGS = [dict(max_segs=255), dict(max_segs=4), dict(max_segs=255, headers_alone=False)]
 
 
+def launched_kernels(call):
+    """names of the kernels call() launches (it synchronises), from torch.profiler.  A profiler session can lose the
+    record of the first kernel it sees, so a torch kernel (at::native, which the library never launches) runs first
+    and is left out of the list."""
+    import torch
+    from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]) as prof:
+        torch.ones(1, device="cuda").add_(1)
+        torch.cuda.synchronize()
+        call()
+    return [e.name for e in prof.events() if e.device_type.name == "CUDA" and
+            not e.name.startswith(("Memcpy", "Memset")) and "at::native" not in e.name]
+
+
 def _need():
     if not (decode.available() and dp.available() and ds.ref_available()):
         pytest.skip("oracle/_ref not built (needs the reference sources at build time)")
@@ -211,7 +225,6 @@ def test_damaged_files(cuda_ok, drivers):  # noqa: F811
 def test_dev_form_and_launches(cuda_ok):
     _need()
     import torch
-    from torch.profiler import ProfilerActivity, profile
     p = _stock(*CASES[0])
     base = [b for _, b in _damaged(p)] + _files(p, seed=9)
     for nfiles in (1, 1000):
@@ -226,12 +239,12 @@ def test_dev_form_and_launches(cuda_ok):
         d_data = torch.zeros_like(d_bytes)
         d_st = torch.zeros((nfiles, abi.OGG_STREAM_DTYPE.itemsize), dtype=torch.uint8, device=dev)
         torch.cuda.synchronize()
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
+
+        def call():
             lib.ogg_demux_dev(nfiles, d_bytes.data_ptr(), d_off.data_ptr(), mp, d_info.data_ptr(), d_npkt.data_ptr(),
                               d_data.data_ptr(), d_st.data_ptr())
             torch.cuda.synchronize()
-        kernels = [e.name for e in prof.events() if e.device_type.name == "CUDA" and
-                   not e.name.startswith(("Memcpy", "Memset"))]
+        kernels = launched_kernels(call)
         assert kernels == ["k_ogg_demux"] or (len(kernels) == 1 and "k_ogg_demux" in kernels[0]), kernels
         npkt = d_npkt.cpu().numpy()
         assert (npkt == host["npkt"]).all()

@@ -21,7 +21,7 @@ from oracle import decode
 from oracle import decode_packets as dp
 from oracle import decode_streams as ds
 from oracle import ogg
-from test_gpu_ogg import CASES, PAGINGS, _decode_as_stock, _stock
+from test_gpu_ogg import CASES, PAGINGS, _decode_as_stock, _stock, launched_kernels
 from vorbis_b200 import abi, lib
 
 pytestmark = pytest.mark.gpu
@@ -196,7 +196,6 @@ def test_group_against_reference(cuda_ok):
 def _dev_call(files, mp, profiled=False):
     """vb200_ogg_group_dev on the demux of files: (host form's result, device outputs, kernel names or None)"""
     import torch
-    from torch.profiler import ProfilerActivity, profile
     dev = torch.device("cuda", 0)
     nfiles = len(files)
     res = lib.ogg_demux(files, max_packets=mp)
@@ -214,15 +213,14 @@ def _dev_call(files, mp, profiled=False):
             d_scr.data_ptr(), sb)
     torch.cuda.synchronize()
     kernels = None
-    if profiled:
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            lib.ogg_group_dev(*args)
-            torch.cuda.synchronize()
-        kernels = [e.name for e in prof.events() if e.device_type.name == "CUDA" and
-                   not e.name.startswith(("Memcpy", "Memset"))]
-    else:
+
+    def call():
         lib.ogg_group_dev(*args)
         torch.cuda.synchronize()
+    if profiled:
+        kernels = launched_kernels(call)
+    else:
+        call()
     ng = int(d_ng.item())
     out = {"status": d_status.cpu().numpy(), "order": d_order.cpu().numpy(), "npkt": d_npkt_out.cpu().numpy(),
            "groups": d_groups.cpu().numpy()[:ng * abi.FILE_GROUP_DTYPE.itemsize].view(abi.FILE_GROUP_DTYPE),

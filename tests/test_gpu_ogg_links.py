@@ -20,7 +20,7 @@ from conftest import probe_signal
 from oracle import decode
 from oracle import ogg
 from oracle import ogg_links
-from test_gpu_ogg import _decode_as_stock, _need
+from test_gpu_ogg import _decode_as_stock, _need, launched_kernels
 from test_gpu_ogg_edges import FIELDS, _demux_at, _header_pages, _mutate
 from test_ogg_links_oracle import CASES, literal_table, table
 from vorbis_b200 import lib
@@ -232,7 +232,6 @@ def test_device_encode_and_mux_round_trip(cuda_ok):
 def _dev_call(files, link_cap, pad=0, profiled=False):
     """vb200_ogg_links_dev on files after `pad` bytes of 'O': (link_first, link_off (filled with -7 first), kernels)"""
     import torch
-    from torch.profiler import ProfilerActivity, profile
     dev = torch.device("cuda", 0)
     buf = np.frombuffer(b"".join(files), np.uint8)
     off = pad + np.concatenate([[0], np.cumsum([len(f) for f in files])]).astype(np.int64)
@@ -250,10 +249,7 @@ def _dev_call(files, link_cap, pad=0, profiled=False):
     kernels = None
     try:
         if profiled:
-            with profile(activities=[ProfilerActivity.CUDA]) as prof:
-                call()
-            kernels = [e.name for e in prof.events() if e.device_type.name == "CUDA" and
-                       not e.name.startswith(("Memcpy", "Memset"))]
+            kernels = launched_kernels(call)
         else:
             call()
         return d_first.cpu().numpy(), d_links.cpu().numpy(), kernels

@@ -22,6 +22,7 @@ from oracle import decode_packets as dp
 from oracle import decode_streams as ds
 from oracle import ogg
 from oracle import ogg_mux
+from test_gpu_ogg import launched_kernels
 from test_ogg_mux_oracle import CASES as HAND, SERIAL, hand_case, seeded_cuts, seeded_stream
 from vorbis_b200 import abi, lib
 
@@ -351,7 +352,6 @@ def _dev_call(ns, profiled=False):
     """vb200_ogg_mux_dev on ns seeded streams with fresh carries: (host form's result, device outputs, kernel names or
     None)"""
     import torch
-    from torch.profiler import ProfilerActivity, profile
     dev = torch.device("cuda", 0)
     base = _seeded(60, 4)
     S = [base[i % len(base)] for i in range(ns)]
@@ -389,10 +389,7 @@ def _dev_call(ns, profiled=False):
     torch.cuda.synchronize()
     kernels = None
     if profiled:
-        with profile(activities=[ProfilerActivity.CUDA]) as prof:
-            call()
-        kernels = [e.name for e in prof.events() if e.device_type.name == "CUDA" and
-                   not e.name.startswith(("Memcpy", "Memset"))]
+        kernels = launched_kernels(call)
     else:
         call()
     out = {"out_off": d_off.cpu().numpy(), "status": d_st.cpu().numpy(), "out": d_out.cpu().numpy(),

@@ -232,8 +232,8 @@ def test_decode_vs_oracle_random_streams(cfg):
 
 
 def test_phaseA_host_path_multichunk(cfg, monkeypatch):
-    """the pipelined two-lane host path (chunks alternate between two streams), without taps and with every tap
-    copied back chunk by chunk"""
+    """the pipelined host path (as vb200_encode_dsp's: 7 blocks per chunk give 10 ramped chunks over the four buffer
+    sets), without taps and with every tap copied back chunk by chunk"""
     name, setup, ctx, o, enc, _ = cfg
     W = 0
     N, ch = setup.blocksize(W), setup.channels
@@ -878,6 +878,39 @@ def test_encode_dsp_with_classes(cfg, monkeypatch):
     if not (setup.channels & (setup.channels - 1)):
         got = ctx.encode_dsp(1, enc["L_pcm"], desc, classes=True, iwork_s16=True)
         assert np.array_equal(got["classes"], wcls)
+
+
+def test_encode_dsp_class_stride_refused(cfg, monkeypatch):
+    """the pipelined host form refuses a class_stride below partvals inside the first chunk's chain, after that
+    chunk's copies in are queued; the same call on the same context with the right stride then gives what a fresh
+    context gives"""
+    name, setup, ctx, o, enc, _ = cfg
+    monkeypatch.setenv("VB200_CHUNK_BLOCKS", "1")                      # one block per chunk: 2 to 5 chunks
+    W, ch = 1, setup.channels
+    n = setup.blocksize(W) // 2
+    desc = make_desc(enc, "L")
+    fresh = vlib.Context(setup)
+    try:
+        want = fresh.encode_dsp(W, enc["L_pcm"], desc, classes=True)
+    finally:
+        fresh.close()
+    pv = ctx.residue_partvals(W)
+    assert pv > 1
+    io, ns, bps, keep = ctx._encode_io(W, enc["L_pcm"], desc, None, 0, 0, None, None)
+    nb = ns * bps
+    got = {"posts": np.zeros((nb, ch, abi.FLOOR1_STRIDE), np.int32), "nonzero": np.zeros((nb, ch), np.int32),
+           "iwork": np.zeros((nb, ch, n), np.int32), "ampmax_out": np.zeros(nb, np.float32),
+           "classes": np.full((nb, ch, pv), -1, np.int32)}
+    for k, v in got.items():
+        setattr(io, k, v.ctypes.data)
+    io.class_stride = pv - 1
+    assert ctx.L.vb200_encode_dsp(ctx.h, W, ns, bps, 7, C.byref(io)) == -131          # VB200_EINVAL
+    assert "class_stride < partvals" in (ctx.L.vb200_last_error() or b"").decode()
+    io.class_stride = pv
+    assert ctx.L.vb200_encode_dsp(ctx.h, W, ns, bps, 7, C.byref(io)) == 0
+    for k in ("posts", "nonzero", "iwork", "classes"):
+        assert np.array_equal(got[k], want[k]), k
+    assert_bits_equal(got["ampmax_out"], want["ampmax_out"], "ampmax_out")
 
 
 def test_encode_dsp_dev_split_half_batches(cfg):

@@ -66,7 +66,7 @@ struct DevBuf {
 };
 
 constexpr int STAGE_SLOTS = 16;      // device buffers one host form may stage (HostIO)
-constexpr int ENC_SETS = 4;          // buffer sets of the pipelined vb200_encode_dsp
+constexpr int ENC_SETS = 4;          // buffer sets of the pipelined host forms (HostPipe)
 
 struct vb200_ctx {
   int device = 0;
@@ -91,10 +91,9 @@ struct vb200_ctx {
   //   stage[]   HostIO: the device copies of a host form's inputs and outputs; nothing else uses it
   //   cycles    the debug cycle counters (VB200_PHASE_TIMING, VB200_FLOOR1_TIMING), kept between calls
   //   phaseA    phaseA_dev_common: log spectrum, row and block maxima
-  //   lane[]    the host vb200_analysis_phaseA, one per lane: a chunk's copies, its intermediates and the taps
-  //             the caller asks for
   //   enc       the encode chain of vb200_encode_dsp_dev and vb200_encode_packets
-  //   set[]     the pipelined host vb200_encode_dsp, one per buffer set: a chunk's copies and its chain
+  //   set[]     HostPipe, one per buffer set, for both pipelined host forms: a chunk's copies and its intermediates
+  //             (vb200_encode_dsp: its chain; vb200_analysis_phaseA: its maxima and the taps the caller asks for)
   //   mgd       vb200_encode_dsp_managed_dev
   //   plan      block planning: vb200_plan_blocks, and the envelope state, marks and plan tables of
   //             vb200_encode_streams[_managed]_dev
@@ -112,17 +111,15 @@ struct vb200_ctx {
   //   drg       vb200_decode_streams_index[_dev]: the packet headers, the per-stream plan tables and fresh heads,
   //             sized by nstreams x max_packets; vb200_decode_ranges[_dev]: the per-request block tables and residue
   //             scratch, sized by nreq and out_stride
-  DevBuf stage[STAGE_SLOTS], cycles, phaseA, lane[2], enc, set[ENC_SETS], mgd, plan, chain, env_scratch, coder, pack,
+  DevBuf stage[STAGE_SLOTS], cycles, phaseA, enc, set[ENC_SETS], mgd, plan, chain, env_scratch, coder, pack,
       spk, brc, dsk, ptl, drg;
-  cudaStream_t s_pipe[2] = {nullptr, nullptr};
   const ResDev *d_res[2] = {nullptr, nullptr};        // [VB200_MAX_SUBMAPS] residue class parameters per block size
   int res_partvals[2] = {0, 0};
   EnvDev env;                        // envelope detector tables (N = 128 transform, windows, thresholds)
   int grid_div = 1;                  // see grid_for
   cudaStream_t s_split[2] = {nullptr, nullptr};       // vb200_encode_dsp_dev: two concurrent half-batches
   cudaEvent_t ev_fork = nullptr, ev_join[2] = {nullptr, nullptr};
-  // vb200_encode_dsp (host buffers): chunks rotate over the ENC_SETS buffer sets; one stream per copy direction and
-  // two compute streams, ordered by events (see there)
+  // HostPipe: two compute streams and one stream per copy direction, ordered by events per buffer set (see there)
   cudaStream_t s_enc[3] = {nullptr, nullptr, nullptr};   // compute 0, compute 1, host->device
   cudaStream_t s_d2h = nullptr;
   cudaEvent_t ev_h2d[ENC_SETS] = {}, ev_cmp[ENC_SETS] = {}, ev_d2h[ENC_SETS] = {};
@@ -238,7 +235,6 @@ static int ctx_build(vb200_ctx *c, const vb200_setup *s, int device) {
   CU(cudaGetDeviceProperties(&prop, device));
   c->sm_count = prop.multiProcessorCount;
   CU(cudaStreamCreateWithFlags(&c->s_main, cudaStreamNonBlocking));
-  for (auto &st : c->s_pipe) CU(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
   for (auto &st : c->s_enc) CU(cudaStreamCreateWithFlags(&st, cudaStreamNonBlocking));
   CU(cudaStreamCreateWithFlags(&c->s_d2h, cudaStreamNonBlocking));
   for (auto &e : c->ev_h2d) CU(cudaEventCreateWithFlags(&e, cudaEventDisableTiming));
@@ -467,7 +463,6 @@ extern "C" void vb200_ctx_destroy(vb200_ctx *c) {
   if (!c) return;
   cudaSetDevice(c->device);
   for (void *p : c->owned) cudaFree(p);
-  for (auto &st : c->s_pipe) if (st) cudaStreamDestroy(st);
   for (auto &st : c->s_split) if (st) cudaStreamDestroy(st);
   if (c->ev_fork) cudaEventDestroy(c->ev_fork);
   for (auto &e : c->ev_join) if (e) cudaEventDestroy(e);
@@ -1161,6 +1156,11 @@ extern "C" int vb200_mdct_backward_dev(vb200_ctx *c, int W, int nvec, const floa
   return post_launch(c);
 }
 
+// bytes of n elements of T, or n bytes for T = void
+template <class T> static size_t elem_bytes(size_t n) {
+  if constexpr (std::is_void_v<T>) return n; else return sizeof(T) * n;
+}
+
 // "Copy in, run, copy out" for the host-buffer variants.  Every device buffer a host form stages, input or output,
 // takes the next buffer of the context's staging pool.  Sizes count elements of T, or bytes for T = void, where the
 // C ABI passes void * (the PCM, vb200_encode_io's iwork).  The first failure is kept in rc, and every later call does
@@ -1177,8 +1177,8 @@ struct HostIO {
     if (!rc && slot == STAGE_SLOTS) rc = fail(VB200_EFAULT, "host call stages more buffers than the staging pool holds");
     if (rc) return nullptr;
     void *d;
-    if ((rc = ensure_buf(c->stage[slot++], bytes<T>(n), &d))) return nullptr;
-    if (src && (rc = copy(d, src, bytes<T>(n), cudaMemcpyHostToDevice))) return nullptr;
+    if ((rc = ensure_buf(c->stage[slot++], elem_bytes<T>(n), &d))) return nullptr;
+    if (src && (rc = copy(d, src, elem_bytes<T>(n), cudaMemcpyHostToDevice))) return nullptr;
     return (T *)d;
   }
   template <class T> T *out(size_t n) { return in<T>(nullptr, n); }
@@ -1189,7 +1189,7 @@ struct HostIO {
     return d;
   }
   template <class T> void back(T *dst, const T *d, size_t n) {
-    if (!rc) rc = copy(dst, d, bytes<T>(n), cudaMemcpyDeviceToHost);
+    if (!rc) rc = copy(dst, d, elem_bytes<T>(n), cudaMemcpyDeviceToHost);
   }
   int sync() {
     if (!rc) { queued = false; rc = wait(); }
@@ -1197,15 +1197,80 @@ struct HostIO {
   }
 
  private:
-  template <class T> static size_t bytes(size_t n) {
-    if constexpr (std::is_void_v<T>) return n; else return sizeof(T) * n;
-  }
   int copy(void *dst, const void *src, size_t n, cudaMemcpyKind kind) {
     CU(cudaMemcpyAsync(dst, src, n, kind, c->s_main));
     queued = true;
     return 0;
   }
   int wait() { CU(cudaStreamSynchronize(c->s_main)); return 0; }
+};
+
+// "Copy in, run, copy out" chunk by chunk, for the host forms that stream a batch through the device.  The batch of
+// `units` (streams of unit_blocks blocks, or blocks) is cut into chunks that rotate over the ENC_SETS buffer sets
+// c->set[]: all host->device copies on one stream, all device->host copies on another (one DMA engine per direction
+// anyway), the kernels of consecutive chunks alternately on two compute streams (a chunk's kernel tails overlap the
+// next chunk's).  Events carry the order H2D(k) -> kernels(k) -> D2H(k) -> H2D(k + ENC_SETS) and nothing else, so the
+// copy engines run ahead of / behind the kernels.  Per chunk a form calls in(), run() and back(), and after the last
+// chunk returns sync().  Sizes count elements of the device pointer's type; the first failure is kept and the
+// destructor waits, as in HostIO.
+struct HostPipe {
+  vb200_ctx *c;
+  int full;                          // units of a full chunk: every set holds this many
+  std::vector<int> sched;            // units of each chunk
+  int rc = 0;
+  bool queued = false;               // copies queued since the last sync()
+  // chunk_blocks: blocks per full chunk unless VB200_CHUNK_BLOCKS sets it; one_chunk: the whole batch in one chunk
+  HostPipe(vb200_ctx *c, int units, int unit_blocks, int chunk_blocks, bool one_chunk = false) : c(c) {
+    { const char *e = getenv("VB200_CHUNK_BLOCKS"); if (e && atoi(e) > 0) chunk_blocks = atoi(e); }
+    full = one_chunk ? units : std::clamp(chunk_blocks / unit_blocks, 1, units);
+    // The pipeline's fill (first H2D + first kernels before anything overlaps) and drain (last kernels + last D2H)
+    // are exposed, so from 6 full chunks up the first and the last two are small (full/4, full/2), the rest full size.
+    const int q = std::max(full / 4, 1), hlf = std::max(full / 2, 1);
+    const bool ramp = units >= 6 * full;
+    if (ramp) sched = {q, hlf};
+    for (int left = units - (ramp ? 2 * (q + hlf) : 0); left > 0; left -= sched.back())
+      sched.push_back(std::min(left, full));
+    if (ramp) sched.insert(sched.end(), {hlf, q});
+  }
+  ~HostPipe() {
+    if (queued) for (cudaStream_t st : {c->s_enc[0], c->s_enc[1], c->s_enc[2], c->s_d2h}) cudaStreamSynchronize(st);
+  }
+  template <class T> void in(const T *d, const std::remove_cv_t<T> *src, size_t n) {
+    if (!rc) rc = copy((void *)d, src, elem_bytes<T>(n), cudaMemcpyHostToDevice, c->s_enc[2]);
+  }
+  template <class T> void back(std::remove_cv_t<T> *dst, const T *d, size_t n) {
+    if (!rc) rc = copy(dst, d, elem_bytes<T>(n), cudaMemcpyDeviceToHost, c->s_d2h);
+  }
+  // chunk k's kernels: launch(st) on its compute stream, after its copies in and before its copies back
+  template <class F> int run(int k, F &&launch) { return rc ? rc : (rc = chunk(k, launch)); }
+  int sync() {
+    if (!rc) { queued = false; rc = wait(); }
+    return rc;
+  }
+
+ private:
+  int copy(void *dst, const void *src, size_t n, cudaMemcpyKind kind, cudaStream_t st) {
+    CU(cudaMemcpyAsync(dst, src, n, kind, st));
+    queued = true;
+    return 0;
+  }
+  template <class F> int chunk(int k, F &launch) {
+    const int L = k % ENC_SETS;
+    cudaStream_t st = c->s_enc[k & 1];
+    if (k > 0) CU(cudaEventRecord(c->ev_d2h[(k - 1) % ENC_SETS], c->s_d2h));   // chunk k-1's copies back end here
+    CU(cudaEventRecord(c->ev_h2d[L], c->s_enc[2]));
+    CU(cudaStreamWaitEvent(st, c->ev_h2d[L], 0));
+    if (int r = launch(st)) return r;
+    CU(cudaEventRecord(c->ev_cmp[L], st));
+    CU(cudaStreamWaitEvent(c->s_d2h, c->ev_cmp[L], 0));
+    if (k + 1 >= ENC_SETS && k + 1 < (int)sched.size())   // the next chunk's copies in: its set's previous chunk is back
+      CU(cudaStreamWaitEvent(c->s_enc[2], c->ev_d2h[(k + 1) % ENC_SETS], 0));
+    return 0;
+  }
+  int wait() {
+    for (cudaStream_t st : {c->s_enc[0], c->s_enc[1], c->s_enc[2], c->s_d2h}) CU(cudaStreamSynchronize(st));
+    return 0;
+  }
 };
 
 extern "C" int vb200_mdct_forward(vb200_ctx *c, int W, int nvec, const float *in, float *out) {
@@ -1510,10 +1575,10 @@ extern "C" int vb200_analysis_phaseA_streams_dev(vb200_ctx *c, int W, int nstrea
   return phaseA_dev_common(c, W, nstreams * bps, io, nstreams, bps, d_amp0, stream);
 }
 
-// Host-buffer Phase A.  The batch is cut into chunks that alternate between two lanes (stream + device buffers
-// each): while one lane computes, the other lane's H2D / D2H copies run on the copy engines.  Pinned host memory is
-// needed for the copies to be truly asynchronous (pageable memory still works, staged by the driver).  With
-// profiling on, the whole batch is one chunk, so that vb200_phaseA_kernel_ms brackets the whole call.
+// Host-buffer Phase A: the blocks go through HostPipe in chunks of 4096; they are independent (desc[].ampmax is each
+// block's ampmax on entry), so any chunking gives the same outputs.  Pinned host memory is needed for the copies to be
+// truly asynchronous (pageable memory still works, staged by the driver).  With profiling on, the whole batch is one
+// chunk, so that vb200_phaseA_kernel_ms brackets the whole call.
 extern "C" int vb200_analysis_phaseA(vb200_ctx *c, int W, int nblocks, const vb200_phaseA_io *h) {
   CHECK_CTX(c); CHECK_W(W);
   if (!h) return fail(VB200_EINVAL, "null io");
@@ -1523,45 +1588,41 @@ extern "C" int vb200_analysis_phaseA(vb200_ctx *c, int W, int nblocks, const vb2
   if (nblocks <= 0) return 0;
   std::lock_guard<std::mutex> lk(c->mu);
   const int ch = c->setup.channels, N = c->dx[W].N, n = N / 2;
-  int chunk = 4096;
-  { const char *e = getenv("VB200_CHUNK_BLOCKS"); if (e && atoi(e) > 0) chunk = atoi(e); }
-  if (chunk > nblocks || c->profiling) chunk = nblocks;
-  const size_t crow = (size_t)chunk * ch;
+  HostPipe pipe(c, nblocks, 1, 4096, c->profiling);
+  const size_t cb = pipe.full, crow = cb * ch;
   int rc;
-  vb200_phaseA_io lane[2];
-  float *logfft[2], *lmax[2], *gmax[2];
-  for (int L = 0; L < (chunk < nblocks ? 2 : 1); L++) {
-    vb200_phaseA_io &d = lane[L];
-    memset(&d, 0, sizeof(d));
-    if ((rc = carve(c->lane[L], [&](Carve &k) {
-           d.pcm = k.take<float>(crow * N); d.desc = k.take<vb200_block_desc>(chunk);
-           d.mdct = k.take<float>(crow * n); d.logmdct = k.take<float>(crow * n); d.logmask = k.take<float>(crow * n);
-           d.ampmax_out = k.take<float>(chunk);
-           logfft[L] = k.take<float>(crow * n); lmax[L] = k.take<float>(crow); gmax[L] = k.take<float>(chunk);
-           d.tap_noise = h->tap_noise ? k.take<float>(crow * n) : nullptr;
-           d.tap_tone = h->tap_tone ? k.take<float>(crow * n) : nullptr;
-           d.tap_mdct_raw = h->tap_mdct_raw ? k.take<float>(crow * n) : nullptr;
-         }))) return rc;
-  }
-  for (int b0 = 0, it = 0; b0 < nblocks; b0 += chunk, it++) {
-    const int L = it & 1, nb = nblocks - b0 < chunk ? nblocks - b0 : chunk;
+  vb200_phaseA_io dset[ENC_SETS];
+  float *logfft[ENC_SETS], *lmax[ENC_SETS], *gmax[ENC_SETS];
+  for (int b0 = 0, it = 0; it < (int)pipe.sched.size(); b0 += pipe.sched[it], it++) {
+    const int L = it % ENC_SETS, nb = pipe.sched[it];
     const size_t rows = (size_t)nb * ch, r0 = (size_t)b0 * ch;
-    cudaStream_t st = c->s_pipe[L];
-    const vb200_phaseA_io &d = lane[L];
-    CU(cudaMemcpyAsync((void *)d.pcm, h->pcm + r0 * N, sizeof(float) * rows * N, cudaMemcpyHostToDevice, st));
-    CU(cudaMemcpyAsync((void *)d.desc, h->desc + b0, sizeof(vb200_block_desc) * nb, cudaMemcpyHostToDevice, st));
-    if ((rc = phaseA_launch(c, W, nb, &d, 0, 0, nullptr, st, logfft[L], lmax[L], gmax[L]))) return rc;
-    // the spectra and the taps asked for; the lane's logfft is the logfft tap
+    vb200_phaseA_io &d = dset[L];
+    if (it < ENC_SETS) {                             // the set's first chunk: every chunk fits cb blocks
+      memset(&d, 0, sizeof(d));
+      if ((rc = carve(c->set[L], [&](Carve &k) {
+             d.pcm = k.take<float>(crow * N); d.desc = k.take<vb200_block_desc>(cb);
+             d.mdct = k.take<float>(crow * n); d.logmdct = k.take<float>(crow * n); d.logmask = k.take<float>(crow * n);
+             d.ampmax_out = k.take<float>(cb);
+             logfft[L] = k.take<float>(crow * n); lmax[L] = k.take<float>(crow); gmax[L] = k.take<float>(cb);
+             d.tap_noise = h->tap_noise ? k.take<float>(crow * n) : nullptr;
+             d.tap_tone = h->tap_tone ? k.take<float>(crow * n) : nullptr;
+             d.tap_mdct_raw = h->tap_mdct_raw ? k.take<float>(crow * n) : nullptr;
+           }))) return rc;
+    }
+    pipe.in(d.pcm, h->pcm + r0 * N, rows * N);
+    pipe.in(d.desc, h->desc + b0, nb);
+    if ((rc = pipe.run(it, [&](cudaStream_t st) {
+           return phaseA_launch(c, W, nb, &d, 0, 0, nullptr, st, logfft[L], lmax[L], gmax[L]);
+         }))) return rc;
+    // the spectra and the taps asked for; the set's logfft is the logfft tap
     const std::pair<float *, const float *> spectra[] = {
         {h->mdct, d.mdct}, {h->logmdct, d.logmdct}, {h->logmask, d.logmask}, {h->tap_noise, d.tap_noise},
         {h->tap_tone, d.tap_tone}, {h->tap_logfft, logfft[L]}, {h->tap_mdct_raw, d.tap_mdct_raw}};
     for (const auto &s : spectra)
-      if (s.first) CU(cudaMemcpyAsync(s.first + r0 * n, s.second, sizeof(float) * rows * n, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(h->ampmax_out + b0, d.ampmax_out, sizeof(float) * nb, cudaMemcpyDeviceToHost, st));
+      if (s.first) pipe.back(s.first + r0 * n, s.second, rows * n);
+    pipe.back(h->ampmax_out + b0, d.ampmax_out, nb);
   }
-  CU(cudaStreamSynchronize(c->s_pipe[0]));
-  CU(cudaStreamSynchronize(c->s_pipe[1]));
-  return 0;
+  return pipe.sync();
 }
 
 // ======================================================================== //
@@ -2182,43 +2243,16 @@ extern "C" int vb200_encode_dsp(vb200_ctx *c, int W, int nstreams, int bps, int 
   if ((rc = enc_check(c, W, nstreams, bps, blobno, h))) return rc;
   std::lock_guard<std::mutex> lk(c->mu);
   const int ch = c->setup.channels, N = c->dx[W].N, n = N / 2;
-  int chunk_blocks = 8192;                           // H100 80GB HBM3 at a 400 W limit (ramped schedule): 4096 -> 5.34, 8192 -> 5.36, 16384 -> 5.21 M blocks/s end to end
-  { const char *e = getenv("VB200_CHUNK_BLOCKS"); if (e && atoi(e) > 0) chunk_blocks = atoi(e); }
-  int cs = chunk_blocks / bps;                       // whole streams per chunk
-  if (cs < 1) cs = 1;
-  if (cs > nstreams) cs = nstreams;
+  HostPipe pipe(c, nstreams, bps, 8192);             // H100 80GB HBM3 at a 400 W limit (ramped schedule): 4096 -> 5.34, 8192 -> 5.36, 16384 -> 5.21 M blocks/s end to end
+  const int cs = pipe.full;                          // whole streams per chunk
   const size_t pcm_per_stream = enc_pcm_bytes(h, ch, N, 1, bps);
-  // Chunk schedule: the pipeline's fill (first H2D + first kernels before anything overlaps) and drain (last kernels
-  // + last D2H) are exposed, so the first and the last chunks are small (cs/4, cs/2) and the middle ones full size.
-  std::vector<int> sched;
-  {
-    int left = nstreams;
-    const int q = cs / 4 > 0 ? cs / 4 : 1, hlf = cs / 2 > 0 ? cs / 2 : 1;
-    if (nstreams >= 6 * cs) {
-      const int head[2] = {q, hlf};
-      for (int k = 0; k < 2; k++) { sched.push_back(head[k]); left -= head[k]; }
-      const int tail = q + hlf;
-      while (left - tail >= cs) { sched.push_back(cs); left -= cs; }
-      if (left - tail > 0) { sched.push_back(left - tail); left = tail; }
-      sched.push_back(hlf); sched.push_back(left - hlf);
-    } else {
-      while (left > 0) { const int t = left < cs ? left : cs; sched.push_back(t); left -= t; }
-    }
-  }
-  // Three-stage pipeline over ENC_SETS buffer sets: all host->device copies on one stream, all device->host
-  // copies on another (one DMA engine per direction anyway), the kernels of consecutive chunks alternately on two
-  // compute streams (a chunk's kernel tails overlap the next chunk's kernels).  Events carry the order
-  // H2D(k) -> kernels(k) -> D2H(k) -> H2D(k + ENC_SETS); nothing else is ordered, so the copy engines run ahead
-  // of / behind the kernels instead of every lane alternating copy and compute on its own stream.
-  cudaStream_t s_h2d = c->s_enc[2], s_d2h = c->s_d2h;
   const bool s16 = h->iwork_fmt == VB200_IWORK_S16;
   const size_t isz = s16 ? sizeof(int16_t) : sizeof(int32_t), cb = (size_t)cs * bps, crow = cb * ch;
   vb200_encode_io dset[ENC_SETS];
   EncScratch sset[ENC_SETS];
-  for (int s0 = 0, it = 0; it < (int)sched.size(); s0 += sched[it], it++) {
-    const int L = it % ENC_SETS, ns = sched[it];
+  for (int s0 = 0, it = 0; it < (int)pipe.sched.size(); s0 += pipe.sched[it], it++) {
+    const int L = it % ENC_SETS, ns = pipe.sched[it];
     const size_t nb = (size_t)ns * bps, b0 = (size_t)s0 * bps, rows = nb * ch, r0 = b0 * ch;
-    cudaStream_t st = c->s_enc[it & 1];
     vb200_encode_io &d = dset[L];
     EncScratch &S = sset[L];
     if (it < ENC_SETS) {                             // the set's first chunk: every chunk fits cs streams
@@ -2235,31 +2269,22 @@ extern "C" int vb200_encode_dsp(vb200_ctx *c, int W, int nstreams, int bps, int 
              enc_layout(k, crow, cb, n, nullptr, s16, &S);
            }))) return rc;
     }
-    if (it >= ENC_SETS) CU(cudaStreamWaitEvent(s_h2d, c->ev_d2h[L], 0));   // this set's previous chunk is back on the host
-    CU(cudaMemcpyAsync((void *)d.pcm, (const char *)h->pcm + pcm_per_stream * s0, pcm_per_stream * ns, cudaMemcpyHostToDevice, s_h2d));
-    CU(cudaMemcpyAsync((void *)d.desc, h->desc + b0, sizeof(vb200_block_desc) * nb, cudaMemcpyHostToDevice, s_h2d));
-    if (h->ampmax0) CU(cudaMemcpyAsync((void *)d.ampmax0, h->ampmax0 + s0, sizeof(float) * ns, cudaMemcpyHostToDevice, s_h2d));
-    CU(cudaEventRecord(c->ev_h2d[L], s_h2d));
-    CU(cudaStreamWaitEvent(st, c->ev_h2d[L], 0));
-    if ((rc = encode_launch(c, W, ns, bps, blobno, &d, S, st))) return rc;
-    CU(cudaEventRecord(c->ev_cmp[L], st));
-    CU(cudaStreamWaitEvent(s_d2h, c->ev_cmp[L], 0));
-    st = s_d2h;
-    CU(cudaMemcpyAsync(h->posts + r0 * VB200_FLOOR1_STRIDE, d.posts, sizeof(int32_t) * rows * VB200_FLOOR1_STRIDE, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(h->nonzero + r0, d.nonzero, sizeof(int32_t) * rows, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync((char *)h->iwork + isz * r0 * n, d.iwork, isz * rows * n, cudaMemcpyDeviceToHost, st));
-    if (s16) CU(cudaMemcpyAsync(h->overflow + b0, d.overflow, sizeof(int32_t) * nb, cudaMemcpyDeviceToHost, st));
-    if (h->classes) CU(cudaMemcpyAsync(h->classes + r0 * (size_t)h->class_stride, d.classes,
-                                       sizeof(int32_t) * rows * (size_t)h->class_stride, cudaMemcpyDeviceToHost, st));
-    CU(cudaMemcpyAsync(h->ampmax_out + b0, d.ampmax_out, sizeof(float) * nb, cudaMemcpyDeviceToHost, st));
-    if (h->mdct) CU(cudaMemcpyAsync(h->mdct + r0 * n, S.mdct, sizeof(float) * rows * n, cudaMemcpyDeviceToHost, st));
-    if (h->logmdct) CU(cudaMemcpyAsync(h->logmdct + r0 * n, S.logmdct, sizeof(float) * rows * n, cudaMemcpyDeviceToHost, st));
-    if (h->logmask) CU(cudaMemcpyAsync(h->logmask + r0 * n, S.logmask, sizeof(float) * rows * n, cudaMemcpyDeviceToHost, st));
-    CU(cudaEventRecord(c->ev_d2h[L], s_d2h));
+    pipe.in(d.pcm, (const char *)h->pcm + pcm_per_stream * s0, pcm_per_stream * ns);
+    pipe.in(d.desc, h->desc + b0, nb);
+    if (h->ampmax0) pipe.in(d.ampmax0, h->ampmax0 + s0, ns);
+    if ((rc = pipe.run(it, [&](cudaStream_t st) { return encode_launch(c, W, ns, bps, blobno, &d, S, st); })))
+      return rc;
+    pipe.back(h->posts + r0 * VB200_FLOOR1_STRIDE, d.posts, rows * VB200_FLOOR1_STRIDE);
+    pipe.back(h->nonzero + r0, d.nonzero, rows);
+    pipe.back((char *)h->iwork + isz * r0 * n, d.iwork, isz * rows * n);
+    if (s16) pipe.back(h->overflow + b0, d.overflow, nb);
+    if (h->classes) pipe.back(h->classes + r0 * (size_t)h->class_stride, d.classes, rows * (size_t)h->class_stride);
+    pipe.back(h->ampmax_out + b0, d.ampmax_out, nb);
+    if (h->mdct) pipe.back(h->mdct + r0 * n, S.mdct, rows * n);
+    if (h->logmdct) pipe.back(h->logmdct + r0 * n, S.logmdct, rows * n);
+    if (h->logmask) pipe.back(h->logmask + r0 * n, S.logmask, rows * n);
   }
-  for (auto &st : c->s_enc) CU(cudaStreamSynchronize(st));
-  CU(cudaStreamSynchronize(c->s_d2h));
-  return 0;
+  return pipe.sync();
 }
 
 // ======================================================================== //
