@@ -142,6 +142,29 @@ def make_book(rng, dim, entries, maptype=1, ordered=False, sparse=0.0, none_used
     return book
 
 
+def balanced_lengths(rng, n):
+    """codeword lengths of a complete prefix code with n >= 2 leaves at two adjacent depths, shuffled (fast for the
+    large lattice books, where complete_lengths' random splits are slow)"""
+    L = ilog(n - 1)
+    ls = [L - 1] * ((1 << L) - n) + [L] * (2 * n - (1 << L))
+    return [int(x) for x in rng.permutation(ls)]
+
+
+def lattice_book(rng, dim, quantvals, delta, sparse=0.0):
+    """a map-type-1 book on the full centred integer lattice an encoder's residue search assumes: quantvals (odd) ^ dim
+    entries, minval -(quantvals >> 1) * delta, an integer delta, and each digit's value list in the order of
+    local_book_besterror's index (0, -delta, +delta, -2 delta, ...), so that the decoder reads back the vector the
+    encoder subtracted.  sparse: the share of entries left without a codeword"""
+    entries, ze = quantvals ** dim, quantvals >> 1
+    used = entries if not sparse else max(2, entries - int(sparse * entries))
+    ls = balanced_lengths(rng, used) if used > 1 else [1]
+    lengths = [int(x) for x in rng.permutation(ls + [0] * (entries - used))]
+    quant = [ze - (m + 1) // 2 if m & 1 else ze + m // 2 for m in range(quantvals)]
+    return {"dim": dim, "entries": entries, "lengths": lengths, "ordered": False, "sparse": used < entries,
+            "maptype": 1, "min": (1, ze * delta, 788) if ze else (0, 0, 0), "delta": (0, delta, 788),
+            "qbits": max(1, ilog(quantvals - 1)), "seqp": 0, "quant": quant}
+
+
 def _float32(w, sign, mant, exp):
     w.write(mant | (exp << 21) | (sign << 31), 32)
 
@@ -399,6 +422,10 @@ class Gen:
 
     def book(self, *a, **k):
         self.d["books"].append(make_book(self.rng, *a, **k))
+        return len(self.d["books"]) - 1
+
+    def lattice(self, *a, **k):
+        self.d["books"].append(lattice_book(self.rng, *a, **k))
         return len(self.d["books"]) - 1
 
     def floor(self, n, mult=None, partitions=None, dims=None, subs=None, minus_one=False, pclass=None):
