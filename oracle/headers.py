@@ -72,7 +72,7 @@ def _arr(p, n, dt):
 
 
 def describe(s, es):
-    """a plain dict of every field md_setup and vb200md_entropy_new give (abi.Setup, abi.EntropySetup); books as
+    """a plain dict of every field vb200md_setup and vb200md_entropy_new give (abi.Setup, abi.EntropySetup); books as
     sorted lists of (entry, length, bits, value row as uint32 bytes)"""
     ch = s.channels
     d = {"channels": ch, "rate": s.rate, "blocksizes": list(s.blocksizes), "n_psy": s.n_psy,

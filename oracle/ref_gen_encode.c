@@ -194,7 +194,7 @@ static int rge_refusal(rge *h){
   return why;
 }
 
-/* md_setup's fields (as ref_headers.c writes them) plus the encoder fields and the classification setup */
+/* vb200md_setup's fields (as ref_headers.c takes them) plus the encoder fields and the classification setup */
 static void rge_setup(rge *h){
   codec_setup_info *ci = (codec_setup_info*)h->vi.codec_setup;
   private_state *b = (private_state*)h->vd.backend_state;

@@ -7,7 +7,7 @@
  *               the vb200 structs cannot describe (bit 0: not two modes of block flags 0 and 1; bit 1: a submap of
  *               either mode on a floor of type 0; bit 2: more than VB200_MAX_SUBMAPS submaps; bit 3: a book whose
  *               dimension is outside 1..127; bit 4: more codewords or value rows than VB200_HEADERS_MAX_*), and
- *               where that is 0 the handle carries md_setup's vb200_setup and vb200md_entropy_new's vb200_entropy_setup (vorbis_b200/host/vb200_decode.c) of the decoder.
+ *               where that is 0 the handle carries vb200md_setup's vb200_setup and vb200md_entropy_new's vb200_entropy_setup (vorbis_b200/host/vb200_decode.c) of the decoder.
  *   rh_setup / rh_entropy / rh_modebits / rh_info / rh_close
  * oracle/Makefile links this file with the stock reference objects and the driver.
  */
@@ -20,12 +20,12 @@
 #include "backends.h"
 #include "registry.h"
 #include "misc.h"
-#include "window.h"
 
 #include "vorbis_b200.h"
 
 #define RH_HANGS (-1000)
 
+int vb200md_setup(vorbis_info *vi, vorbis_dsp_state *vd, vb200_setup *s);
 vb200_entropy_setup *vb200md_entropy_new(vorbis_info *vi, vorbis_dsp_state *vd, int *err);
 void vb200md_entropy_free(vb200_entropy_setup *es);
 
@@ -43,40 +43,6 @@ void rh_close(rh *h){
   vorbis_comment_clear(&h->vc);
   vorbis_info_clear(&h->vi);
   free(h);
-}
-
-/* md_setup of vb200_decode.c: the fields it reads from the decoder */
-static void rh_md_setup(rh *h){
-  codec_setup_info *ci = (codec_setup_info*)h->vi.codec_setup;
-  private_state *b = (private_state*)h->vd.backend_state;
-  vb200_setup *s = &h->s;
-  int w, j, k;
-  memset(s, 0, sizeof(*s));
-  s->channels = h->vi.channels;
-  s->rate = (int32_t)h->vi.rate;
-  s->blocksizes[0] = (int32_t)ci->blocksizes[0];
-  s->blocksizes[1] = (int32_t)ci->blocksizes[1];
-  s->window[0] = _vorbis_window_get(b->window[0]);
-  s->window[1] = _vorbis_window_get(b->window[1]);
-  for(w = 0; w < 2; w++){
-    vorbis_info_mapping0 *mp = (vorbis_info_mapping0*)ci->map_param[ci->mode_param[w]->mapping];
-    s->coupling_steps[w] = mp->coupling_steps;
-    for(k = 0; k < mp->coupling_steps; k++){ s->coupling_mag[w][k] = mp->coupling_mag[k]; s->coupling_ang[w][k] = mp->coupling_ang[k]; }
-    s->submaps[w] = mp->submaps;
-    for(k = 0; k < h->vi.channels; k++) s->chmux[w][k] = (uint8_t)mp->chmuxlist[k];
-    for(j = 0; j < VB200_MAX_SUBMAPS; j++) s->residue[w][j].type = -1;
-    for(j = 0; j < mp->submaps; j++){
-      int fl = mp->floorsubmap[j];
-      vorbis_info_floor1 *fi = (vorbis_info_floor1*)ci->floor_param[fl];
-      vorbis_look_floor1 *lk = (vorbis_look_floor1*)b->flr[fl];
-      vb200_floor1_setup *o = &s->floor1[w][j];
-      o->posts = lk->posts;
-      for(k = 0; k < lk->posts; k++) o->postlist[k] = fi->postlist[k];
-      o->mult = fi->mult; o->n = lk->n;
-      o->maxover = fi->maxover; o->maxunder = fi->maxunder; o->maxerr = fi->maxerr;
-      o->twofitweight = fi->twofitweight; o->twofitatten = fi->twofitatten;
-    }
-  }
 }
 
 static int rh_eimpl(rh *h){
@@ -127,7 +93,7 @@ rh *rh_open(const unsigned char *id, long id_bytes, const unsigned char *cm, lon
   h->init = 1;
   *rc = 0;
   if((*eimpl = rh_eimpl(h)) != 0) return h;
-  rh_md_setup(h);
+  if((e = vb200md_setup(&h->vi, &h->vd, &h->s)) != 0){ *rc = e; rh_close(h); return NULL; }
   h->es = vb200md_entropy_new(&h->vi, &h->vd, &e);
   if(!h->es){ *rc = e ? e : -1; rh_close(h); return NULL; }
   return h;

@@ -1,5 +1,5 @@
 """vb200_vorbis_headers_parse (vorbis_b200/csrc/vb200_headers.h) against the reference's own reading of the same three
-header packets (oracle/ref_headers.c: vorbis_synthesis_headerin x3, vorbis_synthesis_init, then the fields md_setup
+header packets (oracle/ref_headers.c: vorbis_synthesis_headerin x3, vorbis_synthesis_init, then the fields vb200md_setup
 reads and the struct vb200md_entropy_new builds):
 - stock setups: every one the suite pins (GRID, HIGH and MULTI of tests/test_oracle_vs_ref.py, the 512/4096 setups
   below q0, the four of the Ogg tests) and the managed 128 kbit/s stereo and 64 kbit/s mono encoders.  The parse

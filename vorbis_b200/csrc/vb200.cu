@@ -158,12 +158,13 @@ static int scratch_end(vb200_ctx *c, cudaStream_t st) {
   return 0;
 }
 
+// a device copy of src[count] in *dst, freed with the tables of `owned`
 template <class T>
-static int upload(vb200_ctx *c, const T *src, size_t count, const T **dst) {
+static int upload(std::vector<void *> &owned, const T *src, size_t count, const T **dst) {
   void *d = nullptr;
   size_t bytes = sizeof(T) * (count ? count : 1);
   CU(cudaMalloc(&d, bytes));
-  c->owned.push_back(d);
+  owned.push_back(d);
   if (count) CU(cudaMemcpy(d, src, sizeof(T) * count, cudaMemcpyHostToDevice));
   *dst = reinterpret_cast<const T *>(d);
   return 0;
@@ -219,13 +220,13 @@ static int xform_upload(vb200_ctx *c, int N, const float *window, HostXform &h, 
   for (int i = 0; i < h.nf && i < 8; i++) d.fac[i] = h.fac[i];
   for (size_t i = 0; i < h.stage_off.size() && i < 8; i++) d.stage_off[i] = h.stage_off[i];
   int rc;
-  if ((rc = upload(c, h.trig.data(), h.trig.size(), &d.trig))) return rc;
-  if ((rc = upload(c, h.bitrev.data(), h.bitrev.size(), &d.bitrev))) return rc;
+  if ((rc = upload(c->owned, h.trig.data(), h.trig.size(), &d.trig))) return rc;
+  if ((rc = upload(c->owned, h.bitrev.data(), h.bitrev.size(), &d.bitrev))) return rc;
   const float *tw = nullptr;
-  if ((rc = upload(c, h.stage_tw.data(), h.stage_tw.size(), &tw))) return rc;
+  if ((rc = upload(c->owned, h.stage_tw.data(), h.stage_tw.size(), &tw))) return rc;
   d.stage_tw = reinterpret_cast<const float2 *>(tw);
-  if ((rc = upload(c, h.win.data(), h.win.size(), &d.win))) return rc;
-  return upload(c, h.wa.data(), h.wa.size(), &d.wa);
+  if ((rc = upload(c->owned, h.win.data(), h.win.size(), &d.win))) return rc;
+  return upload(c->owned, h.wa.data(), h.wa.size(), &d.wa);
 }
 
 extern "C" void vb200_ctx_destroy(vb200_ctx *c);
@@ -268,7 +269,7 @@ static int ctx_build(vb200_ctx *c, const vb200_setup *s, int device) {
       if (d.partvals > c->res_partvals[w]) c->res_partvals[w] = d.partvals;
     }
     int rc;
-    if ((rc = upload(c, hr, (size_t)VB200_MAX_SUBMAPS, &c->d_res[w]))) return rc;
+    if ((rc = upload(c->owned, hr, (size_t)VB200_MAX_SUBMAPS, &c->d_res[w]))) return rc;
   }
   {
     // envelope detector lookups, _ve_envelope_init (lib/envelope.c:31-74)
@@ -280,17 +281,17 @@ static int ctx_build(vb200_ctx *c, const vb200_setup *s, int device) {
     d.N = h.N; d.log2n = h.log2n; d.nst = h.log2n - 6; d.nf = h.nf; d.scale = h.scale;
     for (size_t i = 0; i < h.stage_off.size() && i < 8; i++) d.stage_off[i] = h.stage_off[i];
     int rc;
-    if ((rc = upload(c, h.trig.data(), h.trig.size(), &d.trig))) return rc;
-    if ((rc = upload(c, h.bitrev.data(), h.bitrev.size(), &d.bitrev))) return rc;
+    if ((rc = upload(c->owned, h.trig.data(), h.trig.size(), &d.trig))) return rc;
+    if ((rc = upload(c->owned, h.bitrev.data(), h.bitrev.size(), &d.bitrev))) return rc;
     const float *tw = nullptr;
-    if ((rc = upload(c, h.stage_tw.data(), h.stage_tw.size(), &tw))) return rc;
+    if ((rc = upload(c->owned, h.stage_tw.data(), h.stage_tw.size(), &tw))) return rc;
     d.stage_tw = reinterpret_cast<const float2 *>(tw);
     float win[ENV_N];
     for (int i = 0; i < ENV_N; i++) {
       win[i] = (float)std::sin(i / (ENV_N - 1.) * M_PI);
       win[i] = win[i] * win[i];
     }
-    if ((rc = upload(c, win, (size_t)ENV_N, &E.win))) return rc;
+    if ((rc = upload(c->owned, win, (size_t)ENV_N, &E.win))) return rc;
     static const int B[VB200_VE_BANDS] = {2, 4, 6, 9, 13, 17, 22}, En[VB200_VE_BANDS] = {4, 5, 6, 8, 8, 8, 8};
     float bwin[VB200_VE_BANDS * 8] = {0};
     for (int j = 0; j < VB200_VE_BANDS; j++) {
@@ -303,16 +304,16 @@ static int ctx_build(vb200_ctx *c, const vb200_setup *s, int device) {
       E.begin[j] = B[j]; E.end[j] = En[j];
       E.preecho[j] = s->preecho_thresh[j]; E.postecho[j] = s->postecho_thresh[j];
     }
-    if ((rc = upload(c, bwin, (size_t)VB200_VE_BANDS * 8, &E.bwin))) return rc;
+    if ((rc = upload(c->owned, bwin, (size_t)VB200_VE_BANDS * 8, &E.bwin))) return rc;
     E.stretch_penalty = s->stretch_penalty; E.minenergy = s->preecho_minenergy;
   }
   {
     int rc;
-    if ((rc = upload(c, VB_FLOOR1_FROMDB, (size_t)256, &c->d_fromdB))) return rc;
+    if ((rc = upload(c->owned, VB_FLOOR1_FROMDB, (size_t)256, &c->d_fromdB))) return rc;
     for (int w = 0; w < 2; w++) {
       if (s->coupling_steps[w] < 0 || s->coupling_steps[w] > VB200_MAX_COUPLING) return fail(VB200_EINVAL, "coupling_steps");
-      if ((rc = upload(c, (const int *)s->coupling_mag[w], (size_t)s->coupling_steps[w], &c->d_mag[w]))) return rc;
-      if ((rc = upload(c, (const int *)s->coupling_ang[w], (size_t)s->coupling_steps[w], &c->d_ang[w]))) return rc;
+      if ((rc = upload(c->owned, (const int *)s->coupling_mag[w], (size_t)s->coupling_steps[w], &c->d_mag[w]))) return rc;
+      if ((rc = upload(c->owned, (const int *)s->coupling_ang[w], (size_t)s->coupling_steps[w], &c->d_ang[w]))) return rc;
     }
   }
   c->n_psy = s->n_psy;
@@ -334,33 +335,33 @@ static int ctx_build(vb200_ctx *c, const vb200_setup *s, int device) {
     d.noisemaxsupp = p.noisemaxsupp; d.max_curve_dB = p.max_curve_dB; d.m_val = p.m_val;
     for (int j = 0; j < 3; j++) d.tone_masteratt[j] = p.tone_masteratt[j];
     int rc;
-    if ((rc = upload(c, p.ath, p.n, &d.ath))) return rc;
-    if ((rc = upload(c, p.octave, p.n, &d.octave))) return rc;
-    if ((rc = upload(c, p.bark, p.n, &d.bark))) return rc;
-    if ((rc = upload(c, p.tonecurves, (size_t)VB200_P_BANDS * VB200_P_LEVELS * (VB200_EHMER_MAX + 2),
+    if ((rc = upload(c->owned, p.ath, p.n, &d.ath))) return rc;
+    if ((rc = upload(c->owned, p.octave, p.n, &d.octave))) return rc;
+    if ((rc = upload(c->owned, p.bark, p.n, &d.bark))) return rc;
+    if ((rc = upload(c->owned, p.tonecurves, (size_t)VB200_P_BANDS * VB200_P_LEVELS * (VB200_EHMER_MAX + 2),
                      &d.tonecurves))) return rc;
-    if ((rc = upload(c, p.noiseoffset, (size_t)VB200_P_NOISECURVES * p.n, &d.noiseoffset))) return rc;
-    if ((rc = upload(c, p.noisecompand, (size_t)VB200_COMPAND_LEVELS, &d.noisecompand))) return rc;
+    if ((rc = upload(c->owned, p.noiseoffset, (size_t)VB200_P_NOISECURVES * p.n, &d.noiseoffset))) return rc;
+    if ((rc = upload(c->owned, p.noisecompand, (size_t)VB200_COMPAND_LEVELS, &d.noisecompand))) return rc;
     if ((1 << f.linesper_log2) != p.eighth_octave_lines)
       return fail(VB200_EIMPL, "eighth_octave_lines must be a power of two (lib/psy.h:108)");
     const int *dr = nullptr, *dg = nullptr, *dc = nullptr, *ds = nullptr;
-    if ((rc = upload(c, f.runinfo.data(), f.runinfo.size(), &dr))) return rc;
-    if ((rc = upload(c, f.grp.data(), f.grp.size(), &dg))) return rc;
-    if ((rc = upload(c, f.cls_run.data(), f.cls_run.size(), &dc))) return rc;
-    if ((rc = upload(c, f.slot_rng.data(), f.slot_rng.size(), &ds))) return rc;
+    if ((rc = upload(c->owned, f.runinfo.data(), f.runinfo.size(), &dr))) return rc;
+    if ((rc = upload(c->owned, f.grp.data(), f.grp.size(), &dg))) return rc;
+    if ((rc = upload(c->owned, f.cls_run.data(), f.cls_run.size(), &dc))) return rc;
+    if ((rc = upload(c->owned, f.slot_rng.data(), f.slot_rng.size(), &ds))) return rc;
     d.runinfo = reinterpret_cast<const int4 *>(dr);
     d.grps = reinterpret_cast<const int4 *>(dg);
     d.cls_run = reinterpret_cast<const int2 *>(dc);
     d.slot_rng = reinterpret_cast<const int2 *>(ds);
     d.linesper_log2 = f.linesper_log2;
     { const int *drr = nullptr, *dlg = nullptr;
-      if ((rc = upload(c, f.runrec.data(), f.runrec.size(), &drr))) return rc;
-      if ((rc = upload(c, f.long_grp.data(), f.long_grp.size(), &dlg))) return rc;
+      if ((rc = upload(c->owned, f.runrec.data(), f.runrec.size(), &drr))) return rc;
+      if ((rc = upload(c->owned, f.long_grp.data(), f.long_grp.size(), &dlg))) return rc;
       d.runrec = reinterpret_cast<const int4 *>(drr); d.long_grp = dlg; d.nlong = (int)f.long_grp.size(); }
-    { const short *db = nullptr; if ((rc = upload(c, f.bin_grp.data(), f.bin_grp.size(), &db))) return rc; d.bin_grp = db; }
+    { const short *db = nullptr; if ((rc = upload(c->owned, f.bin_grp.data(), f.bin_grp.size(), &db))) return rc; d.bin_grp = db; }
     if (p.eighth_octave_lines > 32) return fail(VB200_EIMPL, "eighth_octave_lines > 32");
     if (p.total_octave_lines >= 2048) return fail(VB200_EIMPL, "total_octave_lines >= 2048");
-    { const int *dco = nullptr; if ((rc = upload(c, f.cls_off.data(), f.cls_off.size(), &dco))) return rc; d.cls_off = dco; }
+    { const int *dco = nullptr; if ((rc = upload(c->owned, f.cls_off.data(), f.cls_off.size(), &dco))) return rc; d.cls_off = dco; }
     d.max_cls_len = 0;
     for (size_t k = 0; k + 1 < f.cls_off.size(); k++) d.max_cls_len = std::max(d.max_cls_len, f.cls_off[k + 1] - f.cls_off[k]);
   }
@@ -431,8 +432,8 @@ static int ctx_build(vb200_ctx *c, const vb200_setup *s, int device) {
       if (sm >= VB200_MAX_SUBMAPS) return fail(VB200_EINVAL, "chmux");
     }
     int rc;
-    if ((rc = upload(c, hf, (size_t)VB200_MAX_SUBMAPS, &c->d_floor[w]))) return rc;
-    if ((rc = upload(c, (const unsigned char *)s->chmux[w], (size_t)VB200_MAX_CHANNELS + 1, &c->d_chmux[w]))) return rc;
+    if ((rc = upload(c->owned, hf, (size_t)VB200_MAX_SUBMAPS, &c->d_floor[w]))) return rc;
+    if ((rc = upload(c->owned, (const unsigned char *)s->chmux[w], (size_t)VB200_MAX_CHANNELS + 1, &c->d_chmux[w]))) return rc;
   }
   return 0;
 }
@@ -2937,6 +2938,100 @@ static int ent_book(const vb200_codebook &b, EntBook &d, std::vector<uint32_t> &
   return 0;
 }
 
+// the channels of submap sm in block size w (*bundle) and the samples its residue spans: n, or for type 2 the
+// bundle's n lines interleaved
+static long res_limit(const vb200_setup &S, int w, int sm, int type, int *bundle) {
+  const long n = S.blocksizes[w] / 2;
+  *bundle = 0;
+  for (int k = 0; k < S.channels; k++) *bundle += S.chmux[w][k] == sm;
+  return type == 2 ? *bundle * n : n;
+}
+
+// The floor and residue tables of both entropy coders: es->floor / es->residue of every submap of both block sizes
+// checked against the context setup and the books' dims, into hf / hr (residue type -1 past a size's submaps).
+// verb ("decode" / "encode") names the coder in the VB200_EIMPL messages.  EntRes::partvals is left to the caller.
+template <class ES>
+static int ent_tables(const vb200_setup &S, const ES *es, const char *verb, EntFloor (&hf)[2][VB200_MAX_SUBMAPS],
+                      EntRes (&hr)[2][VB200_MAX_SUBMAPS]) {
+  const int nb = es->nbooks;
+  auto book_ok = [&](int b) { return b >= 0 && b < nb; };
+  memset(hf, 0, sizeof(hf));
+  memset(hr, 0, sizeof(hr));
+  for (int w = 0; w < 2; w++) {
+    const int subs = S.submaps[w];
+    if (subs < 1) return fail(VB200_EINVAL, "no submaps in the context setup");
+    for (int k = 0; k < S.channels; k++)
+      if (S.chmux[w][k] >= subs) return fail(VB200_EINVAL, "chmux past submaps");
+    for (int sm = 0; sm < VB200_MAX_SUBMAPS; sm++) hr[w][sm].type = -1;
+    for (int sm = 0; sm < subs; sm++) {
+      const vb200_floor_decode &f = es->floor[w][sm];
+      const vb200_floor1_setup &f1 = S.floor1[w][sm];
+      EntFloor &F = hf[w][sm];
+      if (f.type != 1) return fail(VB200_EIMPL, (std::string("only floor type 1 ") + verb + "s on the device").c_str());
+      if (f1.posts <= 0) return fail(VB200_EINVAL, "no floor1 setup for a submap");
+      if (f.partitions < 0 || f.partitions > 31) return fail(VB200_EINVAL, "floor partitions");
+      int posts = 2;
+      for (int i = 0; i < f.partitions; i++) {
+        const int cl = f.partitionclass[i];
+        if (cl < 0 || cl > 15) return fail(VB200_EINVAL, "floor partition class");
+        if (f.class_dim[cl] < 1 || f.class_dim[cl] > 8 || f.class_subs[cl] < 0 || f.class_subs[cl] > 3)
+          return fail(VB200_EINVAL, "floor class dim / subs");
+        posts += f.class_dim[cl];
+      }
+      if (posts != f1.posts) return fail(VB200_EINVAL, "floor partitions do not give the floor's posts");
+      static const int quant_q[4] = {256, 128, 86, 64};
+      F.partitions = f.partitions; F.posts = f1.posts;
+      F.quant_q = quant_q[f1.mult - 1]; F.qbits = ilog_u((unsigned)F.quant_q - 1);
+      for (int cl = 0; cl < 16; cl++) for (int j = 0; j < 8; j++) F.subbook[cl][j] = -1;
+      for (int i = 0; i < f.partitions; i++) {
+        const int cl = f.partitionclass[i];
+        F.pclass[i] = (unsigned char)cl;
+        F.cdim[cl] = (unsigned char)f.class_dim[cl]; F.csubs[cl] = (unsigned char)f.class_subs[cl];
+        if (f.class_subs[cl] && !book_ok(f.class_book[cl])) return fail(VB200_EINVAL, "floor class book");
+        F.cbook[cl] = (short)(f.class_subs[cl] ? f.class_book[cl] : 0);
+        for (int j = 0; j < (1 << f.class_subs[cl]); j++) {
+          const int b = f.class_subbook[cl][j];
+          if (b != -1 && !book_ok(b)) return fail(VB200_EINVAL, "floor subclass book");
+          F.subbook[cl][j] = (short)b;
+        }
+      }
+      const vb200_residue_decode &r = es->residue[w][sm];
+      EntRes &R = hr[w][sm];
+      if (r.type == 0)
+        return fail(VB200_EIMPL, (std::string("residue type 0 does not ") + verb + " on the device").c_str());
+      if (r.type != 1 && r.type != 2) return fail(VB200_EINVAL, "residue type");
+      int bundle;
+      if (r.grouping < 1 || r.begin < 0 || r.end < r.begin || r.begin > res_limit(S, w, sm, r.type, &bundle))
+        return fail(VB200_EINVAL, "residue begin / end / grouping do not fit the block");
+      if (r.partitions < 1 || r.partitions > 64 || !book_ok(r.groupbook)) return fail(VB200_EINVAL, "residue partitions / groupbook");
+      const int ppw = es->books[r.groupbook].dim;
+      long long pv = 1;
+      for (int j = 0; j < ppw && pv <= (1ll << 31); j++) pv *= r.partitions;
+      if (pv != r.partvals) return fail(VB200_EINVAL, "residue partvals != partitions ^ dim(groupbook)");
+      R.type = r.type; R.begin = r.begin; R.end = r.end; R.grouping = r.grouping;
+      R.groupbook = r.groupbook; R.ppw = ppw; R.partitions = r.partitions; R.stages = 0;
+      for (int cl = 0; cl < 64; cl++)
+        for (int st = 0; st < 8; st++) {
+          const int b = cl < r.partitions ? r.stagebook[cl][st] : -1;
+          if (b != -1 && !book_ok(b)) return fail(VB200_EINVAL, "residue stage book");
+          R.stagebook[cl][st] = (short)b;
+          if (b >= 0) R.stages = std::max(R.stages, st + 1);
+        }
+    }
+  }
+  return 0;
+}
+
+// Frees the registered tables of `owned` once no kernel may still read them: the context's stream, then the device
+// (the _dev forms run on the caller's streams).  With c->mu held.
+static int release_tables(vb200_ctx *c, std::vector<void *> &owned) {
+  CU(cudaStreamSynchronize(c->s_main));
+  CU(cudaDeviceSynchronize());
+  for (void *p : owned) cudaFree(p);
+  owned.clear();
+  return 0;
+}
+
 extern "C" int vb200_decode_entropy_setup(vb200_ctx *c, const vb200_entropy_setup *es) {
   CHECK_CTX(c);
   if (!es || es->nbooks < 0 || (es->nbooks > 0 && !es->books)) return fail(VB200_EINVAL, "entropy setup");
@@ -2950,112 +3045,37 @@ extern "C" int vb200_decode_entropy_setup(vb200_ctx *c, const vb200_entropy_setu
   int rc;
   for (int i = 0; i < nb; i++)
     if ((rc = ent_book(es->books[i], books[i], tab, vec, ent))) return rc;
-  auto book_ok = [&](int b) { return b >= 0 && b < nb; };
   EntFloor hf[2][VB200_MAX_SUBMAPS];
   EntRes hr[2][VB200_MAX_SUBMAPS];
-  memset(hf, 0, sizeof(hf));
-  memset(hr, 0, sizeof(hr));
+  if ((rc = ent_tables(S, es, "decode", hf, hr))) return rc;
   size_t cls_cap = 1;
-  for (int w = 0; w < 2; w++) {
-    const int n = S.blocksizes[w] / 2, subs = S.submaps[w];
-    if (subs < 1) return fail(VB200_EINVAL, "no submaps in the context setup");
-    for (int k = 0; k < ch; k++)
-      if (S.chmux[w][k] >= subs) return fail(VB200_EINVAL, "chmux past submaps");
-    for (int sm = 0; sm < VB200_MAX_SUBMAPS; sm++) hr[w][sm].type = -1;
-    for (int sm = 0; sm < subs; sm++) {
-      const vb200_floor_decode &f = es->floor[w][sm];
-      const vb200_floor1_setup &f1 = S.floor1[w][sm];
-      EntFloor &F = hf[w][sm];
-      if (f.type != 1) return fail(VB200_EIMPL, "only floor type 1 decodes on the device");
-      if (f1.posts <= 0) return fail(VB200_EINVAL, "no floor1 setup for a submap");
-      if (f.partitions < 0 || f.partitions > 31) return fail(VB200_EINVAL, "floor partitions");
-      int posts = 2;
-      for (int i = 0; i < f.partitions; i++) {
-        const int cl = f.partitionclass[i];
-        if (cl < 0 || cl > 15) return fail(VB200_EINVAL, "floor partition class");
-        posts += f.class_dim[cl];
-      }
-      if (posts != f1.posts) return fail(VB200_EINVAL, "floor partitions do not give the floor's posts");
-      F.partitions = f.partitions; F.posts = f1.posts;
-      static const int quant_q[4] = {256, 128, 86, 64};
-      F.quant_q = quant_q[f1.mult - 1]; F.qbits = ilog_u((unsigned)F.quant_q - 1);
-      for (int i = 0; i < f.partitions; i++) F.pclass[i] = (unsigned char)f.partitionclass[i];
-      for (int cl = 0; cl < 16; cl++) {
-        for (int j = 0; j < 8; j++) F.subbook[cl][j] = -1;
-        bool used = false;
-        for (int i = 0; i < f.partitions; i++) used |= f.partitionclass[i] == cl;
-        if (!used) continue;
-        if (f.class_dim[cl] < 1 || f.class_dim[cl] > 8 || f.class_subs[cl] < 0 || f.class_subs[cl] > 3)
-          return fail(VB200_EINVAL, "floor class dim / subs");
-        if (f.class_subs[cl] && !book_ok(f.class_book[cl])) return fail(VB200_EINVAL, "floor class book");
-        F.cdim[cl] = (unsigned char)f.class_dim[cl]; F.csubs[cl] = (unsigned char)f.class_subs[cl];
-        F.cbook[cl] = (short)(f.class_subs[cl] ? f.class_book[cl] : 0);
-        for (int j = 0; j < (1 << f.class_subs[cl]); j++) {
-          const int b = f.class_subbook[cl][j];
-          if (b != -1 && !book_ok(b)) return fail(VB200_EINVAL, "floor subclass book");
-          F.subbook[cl][j] = (short)b;
-        }
-      }
-      const vb200_residue_decode &r = es->residue[w][sm];
+  for (int w = 0; w < 2; w++)
+    for (int sm = 0; sm < S.submaps[w]; sm++) {
       EntRes &R = hr[w][sm];
-      if (r.type == 0) return fail(VB200_EIMPL, "residue type 0 does not decode on the device");
-      if (r.type != 1 && r.type != 2) return fail(VB200_EINVAL, "residue type");
-      int bundle = 0;
-      for (int k = 0; k < ch; k++) bundle += S.chmux[w][k] == sm;
-      const long limit = r.type == 2 ? (long)bundle * n : n;
-      if (r.grouping < 1 || r.begin < 0 || r.end < r.begin || r.begin > limit)
-        return fail(VB200_EINVAL, "residue begin / end / grouping do not fit the block");
-      if (r.partitions < 1 || r.partitions > 64 || !book_ok(r.groupbook)) return fail(VB200_EINVAL, "residue partitions / groupbook");
-      const int ppw = es->books[r.groupbook].dim;
-      long long pv = 1;
-      for (int j = 0; j < ppw && pv <= (1ll << 31); j++) pv *= r.partitions;
-      if (pv != r.partvals) return fail(VB200_EINVAL, "residue partvals != partitions ^ dim(groupbook)");
-      R.type = r.type; R.begin = r.begin; R.end = r.end; R.grouping = r.grouping; R.partvals = r.partvals;
-      R.groupbook = r.groupbook; R.ppw = ppw; R.partitions = r.partitions; R.stages = 0;
-      for (int cl = 0; cl < 64; cl++)
-        for (int st = 0; st < 8; st++) {
-          const int b = cl < r.partitions ? r.stagebook[cl][st] : -1;
-          if (b != -1 && !book_ok(b)) return fail(VB200_EINVAL, "residue stage book");
+      R.partvals = es->residue[w][sm].partvals;
+      for (int cl = 0; cl < R.partitions; cl++)
+        for (int st = 0; st < R.stages; st++) {
+          const int b = R.stagebook[cl][st];
           if (b >= 0 && es->books[b].used > 0 && !es->books[b].value)
             return fail(VB200_EINVAL, "residue stage book without values");
-          R.stagebook[cl][st] = (short)b;
-          if (b >= 0) R.stages = std::max(R.stages, st + 1);
         }
-      const long end = std::min((long)r.end, limit);
-      const size_t need = (size_t)((end - r.begin) / r.grouping) * (r.type == 2 ? 1 : bundle);
-      cls_cap = std::max(cls_cap, need);
+      int bundle;
+      const long end = std::min((long)R.end, res_limit(S, w, sm, R.type, &bundle));
+      cls_cap = std::max(cls_cap, (size_t)((end - R.begin) / R.grouping) * (R.type == 2 ? 1 : bundle));
     }
-  }
   const size_t smem = sizeof(int32_t) * (size_t)ch * (VB200_FLOOR1_STRIDE + 1) + 2 * (size_t)ch + cls_cap;
   if (smem > ENT_SMEM_MAX) return fail(VB200_EIMPL, "partition classes of a block exceed the shared memory");
   std::lock_guard<std::mutex> lk(c->mu);
-  CU(cudaStreamSynchronize(c->s_main));
-  for (void *p : c->ent_owned) cudaFree(p);
-  c->ent_owned.clear();
+  if ((rc = release_tables(c, c->ent_owned))) return rc;
   c->ent = EntDev{};
-  auto up = [&](const void *src, size_t bytes, const void **dst) -> int {
-    void *d = nullptr;
-    CU(cudaMalloc(&d, bytes ? bytes : 4));
-    c->ent_owned.push_back(d);
-    if (bytes) CU(cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice));
-    *dst = d;
-    return 0;
-  };
   EntDev E{};
-  const void *p;
-  if ((rc = up(books.data(), sizeof(EntBook) * books.size(), &p))) return rc;
-  E.books = (const EntBook *)p;
-  if ((rc = up(tab.data(), sizeof(uint32_t) * tab.size(), &p))) return rc;
-  E.tab = (const uint32_t *)p;
-  if ((rc = up(vec.data(), sizeof(float) * vec.size(), &p))) return rc;
-  E.vec = (const float *)p;
-  if ((rc = up(ent.data(), sizeof(int) * ent.size(), &p))) return rc;
-  E.ent = (const int *)p;
+  if ((rc = upload(c->ent_owned, books.data(), books.size(), &E.books))) return rc;
+  if ((rc = upload(c->ent_owned, tab.data(), tab.size(), &E.tab))) return rc;
+  if ((rc = upload(c->ent_owned, vec.data(), vec.size(), &E.vec))) return rc;
+  if ((rc = upload(c->ent_owned, ent.data(), ent.size(), &E.ent))) return rc;
   for (int w = 0; w < 2; w++) {
-    if ((rc = up(hf[w], sizeof(hf[w]), &p))) return rc;
-    E.floor[w] = (const EntFloor *)p;
-    if ((rc = up(hr[w], sizeof(hr[w]), &p))) return rc;
-    E.res[w] = (const EntRes *)p;
+    if ((rc = upload(c->ent_owned, hf[w], (size_t)VB200_MAX_SUBMAPS, &E.floor[w]))) return rc;
+    if ((rc = upload(c->ent_owned, hr[w], (size_t)VB200_MAX_SUBMAPS, &E.res[w]))) return rc;
     E.chmux[w] = c->d_chmux[w]; E.mag[w] = c->d_mag[w]; E.ang[w] = c->d_ang[w];
     E.steps[w] = S.coupling_steps[w]; E.submaps[w] = S.submaps[w]; E.n[w] = S.blocksizes[w] / 2;
   }
@@ -3490,94 +3510,48 @@ extern "C" int vb200_encode_entropy_setup(vb200_ctx *c, const struct vb200_encod
     len.insert(len.end(), b.length, b.length + b.entries);
     cw.insert(cw.end(), b.codeword, b.codeword + b.entries);
   }
-  auto book_ok = [&](int b) { return b >= 0 && b < nb; };
   EntFloor hf[2][VB200_MAX_SUBMAPS];
   EntRes hr[2][VB200_MAX_SUBMAPS];
-  memset(hf, 0, sizeof(hf));
-  memset(hr, 0, sizeof(hr));
+  int rc;
+  if ((rc = ent_tables(S, es, "encode", hf, hr))) return rc;
   int slots[2] = {0, 0}, bound[2] = {0, 0};
   for (int w = 0; w < 2; w++) {
-    const int n = S.blocksizes[w] / 2, subs = S.submaps[w];
-    if (subs < 1) return fail(VB200_EINVAL, "no submaps in the context setup");
-    for (int k = 0; k < ch; k++)
-      if (S.chmux[w][k] >= subs) return fail(VB200_EINVAL, "chmux past submaps");
-    for (int sm = 0; sm < VB200_MAX_SUBMAPS; sm++) hr[w][sm].type = -1;
     long long nslot = 1 + ch, bits = 1 + es->modebits + (w ? 2 : 0);
-    for (int sm = 0; sm < subs; sm++) {
-      const vb200_floor_decode &f = es->floor[w][sm];
-      const vb200_floor1_setup &f1 = S.floor1[w][sm];
-      EntFloor &F = hf[w][sm];
-      if (f.type != 1) return fail(VB200_EIMPL, "only floor type 1 encodes on the device");
-      if (f1.posts <= 0) return fail(VB200_EINVAL, "no floor1 setup for a submap");
-      if (f.partitions < 0 || f.partitions > 31) return fail(VB200_EINVAL, "floor partitions");
-      int posts = 2;
-      for (int i = 0; i < f.partitions; i++) {
-        const int cl = f.partitionclass[i];
-        if (cl < 0 || cl > 15) return fail(VB200_EINVAL, "floor partition class");
-        if (f.class_dim[cl] < 1 || f.class_dim[cl] > 8 || f.class_subs[cl] < 0 || f.class_subs[cl] > 3)
-          return fail(VB200_EINVAL, "floor class dim / subs");
-        posts += f.class_dim[cl];
-      }
-      if (posts != f1.posts) return fail(VB200_EINVAL, "floor partitions do not give the floor's posts");
-      static const int quant_q[4] = {256, 128, 86, 64};
-      F.partitions = f.partitions; F.posts = f1.posts;
-      F.quant_q = quant_q[f1.mult - 1]; F.qbits = ilog_u((unsigned)F.quant_q - 1);
-      long long fbits = 1 + 2 * F.qbits;
-      for (int cl = 0; cl < 16; cl++) for (int j = 0; j < 8; j++) F.subbook[cl][j] = -1;
-      for (int i = 0; i < f.partitions; i++) {
-        const int cl = f.partitionclass[i];
-        F.pclass[i] = (unsigned char)cl;
-        F.cdim[cl] = (unsigned char)f.class_dim[cl]; F.csubs[cl] = (unsigned char)f.class_subs[cl];
-        if (f.class_subs[cl] && !book_ok(f.class_book[cl])) return fail(VB200_EINVAL, "floor class book");
-        F.cbook[cl] = (short)(f.class_subs[cl] ? f.class_book[cl] : 0);
-        int sub_longest = 0;
-        for (int j = 0; j < (1 << f.class_subs[cl]); j++) {
-          const int b = f.class_subbook[cl][j];
-          if (b != -1 && !book_ok(b)) return fail(VB200_EINVAL, "floor subclass book");
-          F.subbook[cl][j] = (short)b;
-          if (b >= 0) sub_longest = std::max(sub_longest, longest[b]);
-        }
-        fbits += (f.class_subs[cl] ? longest[f.class_book[cl]] : 0) + (long long)f.class_dim[cl] * sub_longest;
-      }
-      for (int k = 0; k < ch; k++) bits += S.chmux[w][k] == sm ? fbits : 0;
-      const vb200_residue_decode &r = es->residue[w][sm];
-      const vb200_residue_setup &rc = S.residue[w][sm];
+    for (int sm = 0; sm < S.submaps[w]; sm++) {
+      const EntFloor &F = hf[w][sm];
       EntRes &R = hr[w][sm];
-      if (r.type == 0) return fail(VB200_EIMPL, "residue type 0 does not encode on the device");
-      if (r.type != 1 && r.type != 2) return fail(VB200_EINVAL, "residue type");
-      int bundle = 0;
-      for (int k = 0; k < ch; k++) bundle += S.chmux[w][k] == sm;
-      const long limit = r.type == 2 ? (long)bundle * n : n;
-      if (r.grouping < 1 || r.begin < 0 || r.end < r.begin || r.end > limit)
+      const vb200_residue_setup &rs = S.residue[w][sm];
+      int bundle;
+      if (R.end > res_limit(S, w, sm, R.type, &bundle))
         return fail(VB200_EINVAL, "residue begin / end / grouping do not fit the block");
-      if (rc.type != r.type || rc.begin != r.begin || rc.end != r.end || rc.grouping != r.grouping ||
-          rc.partitions != r.partitions)
+      if (rs.type != R.type || rs.begin != R.begin || rs.end != R.end || rs.grouping != R.grouping ||
+          rs.partitions != R.partitions)
         return fail(VB200_EINVAL, "residue differs from the context's classification setup");
-      if (r.partitions < 1 || r.partitions > 64 || !book_ok(r.groupbook)) return fail(VB200_EINVAL, "residue partitions / groupbook");
-      const int ppw = es->books[r.groupbook].dim;
-      long long pv = 1;
-      for (int j = 0; j < ppw && pv <= (1ll << 31); j++) pv *= r.partitions;
-      if (pv != r.partvals) return fail(VB200_EINVAL, "residue partvals != partitions ^ dim(groupbook)");
-      R.type = r.type; R.begin = r.begin; R.end = r.end; R.grouping = r.grouping; R.partvals = (r.end - r.begin) / r.grouping;
-      R.groupbook = r.groupbook; R.ppw = ppw; R.partitions = r.partitions; R.stages = 0;
+      R.partvals = (R.end - R.begin) / R.grouping;
       int stage_longest[8] = {0, 0, 0, 0, 0, 0, 0, 0};
-      for (int cl = 0; cl < 64; cl++)
-        for (int st = 0; st < 8; st++) {
-          const int b = cl < r.partitions ? r.stagebook[cl][st] : -1;
-          if (b != -1 && !book_ok(b)) return fail(VB200_EINVAL, "residue stage book");
-          R.stagebook[cl][st] = (short)b;
+      for (int cl = 0; cl < R.partitions; cl++)
+        for (int st = 0; st < R.stages; st++) {
+          const int b = R.stagebook[cl][st];
           if (b < 0) continue;
           const vb200_enc_codebook &B = es->books[b];
           long long lattice = 1;
           for (int j = 0; j < B.dim && lattice <= B.entries; j++) lattice *= B.quantvals;
           if (B.dim > 8 || B.quantvals <= 0 || lattice > B.entries)
             return fail(VB200_EINVAL, "residue stage book: dim > 8 or a lattice that does not fit its entries");
-          R.stages = std::max(R.stages, st + 1);
-          stage_longest[st] = std::max(stage_longest[st], (r.grouping / B.dim) * longest[b]);
+          stage_longest[st] = std::max(stage_longest[st], (R.grouping / B.dim) * longest[b]);
         }
-      const long long nvec = r.type == 2 ? 1 : bundle, groups = (R.partvals + ppw - 1) / ppw;
+      long long fbits = 1 + 2 * F.qbits;
+      for (int i = 0; i < F.partitions; i++) {
+        const int cl = F.pclass[i];
+        int sub_longest = 0;
+        for (int j = 0; j < (1 << F.csubs[cl]); j++)
+          if (F.subbook[cl][j] >= 0) sub_longest = std::max(sub_longest, longest[F.subbook[cl][j]]);
+        fbits += (F.csubs[cl] ? longest[F.cbook[cl]] : 0) + (long long)F.cdim[cl] * sub_longest;
+      }
+      bits += bundle * fbits;
+      const long long nvec = R.type == 2 ? 1 : bundle, groups = (R.partvals + R.ppw - 1) / R.ppw;
       nslot += groups * nvec + (long long)R.stages * R.partvals * nvec;
-      bits += nvec * groups * longest[r.groupbook];
+      bits += nvec * groups * longest[R.groupbook];
       for (int st = 0; st < R.stages; st++) bits += nvec * R.partvals * stage_longest[st];
     }
     if (sizeof(int) * (size_t)nslot > EENT_SMEM_MAX) return fail(VB200_EIMPL, "pieces of one packet exceed the shared memory");
@@ -3586,33 +3560,15 @@ extern "C" int vb200_encode_entropy_setup(vb200_ctx *c, const struct vb200_encod
     bound[w] = (int)(((bits + 7) / 8 + 3) & ~3ll);
   }
   std::lock_guard<std::mutex> lk(c->mu);
-  CU(cudaStreamSynchronize(c->s_main));
-  CU(cudaDeviceSynchronize());                       // no kernel may still read the tables being replaced
-  for (void *p : c->eent_owned) cudaFree(p);
-  c->eent_owned.clear();
+  if ((rc = release_tables(c, c->eent_owned))) return rc;
   c->eent = EncEntDev{};
-  auto up = [&](const void *src, size_t bytes, const void **dst) -> int {
-    void *d = nullptr;
-    CU(cudaMalloc(&d, bytes ? bytes : 4));
-    c->eent_owned.push_back(d);
-    if (bytes) CU(cudaMemcpy(d, src, bytes, cudaMemcpyHostToDevice));
-    *dst = d;
-    return 0;
-  };
   EncEntDev E{};
-  const void *p;
-  int rc;
-  if ((rc = up(books.data(), sizeof(EncBook) * books.size(), &p))) return rc;
-  E.books = (const EncBook *)p;
-  if ((rc = up(len.data(), len.size(), &p))) return rc;
-  E.len = (const unsigned char *)p;
-  if ((rc = up(cw.data(), sizeof(uint32_t) * cw.size(), &p))) return rc;
-  E.cw = (const uint32_t *)p;
+  if ((rc = upload(c->eent_owned, books.data(), books.size(), &E.books))) return rc;
+  if ((rc = upload(c->eent_owned, len.data(), len.size(), &E.len))) return rc;
+  if ((rc = upload(c->eent_owned, cw.data(), cw.size(), &E.cw))) return rc;
   for (int w = 0; w < 2; w++) {
-    if ((rc = up(hf[w], sizeof(hf[w]), &p))) return rc;
-    E.floor[w] = (const EntFloor *)p;
-    if ((rc = up(hr[w], sizeof(hr[w]), &p))) return rc;
-    E.res[w] = (const EntRes *)p;
+    if ((rc = upload(c->eent_owned, hf[w], (size_t)VB200_MAX_SUBMAPS, &E.floor[w]))) return rc;
+    if ((rc = upload(c->eent_owned, hr[w], (size_t)VB200_MAX_SUBMAPS, &E.res[w]))) return rc;
     E.submaps[w] = S.submaps[w]; E.slots[w] = slots[w]; E.bound[w] = bound[w];
   }
   E.ch = ch; E.modebits = es->modebits;

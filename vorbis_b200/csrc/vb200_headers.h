@@ -4,7 +4,7 @@
 // It restates the reference decoder's acceptance and tables: vorbis_synthesis_headerin ×3 (lib/info.c:211-450,
 // the book unpack of lib/codebook.c:147-285, floor1_unpack, floor0_unpack, res0_unpack, mapping0_unpack) and the
 // failure points of vorbis_synthesis_init, which are those of vorbis_book_init_decode (lib/sharedbook.c:393-519).
-// Its output is what vorbis_b200/host/vb200_decode.c derives from a live decoder after those calls: md_setup's
+// Its output is what vorbis_b200/host/vb200_decode.c derives from a live decoder after those calls: vb200md_setup's
 // vb200_setup and vb200md_entropy_new's vb200_entropy_setup.
 #pragma once
 #include <cmath>
@@ -537,7 +537,7 @@ inline int parse(const uint8_t *id, int32_t id_bytes, const uint8_t *comment, in
   }
   first[books.size()] = o.length.size();
   vfirst[books.size()] = o.value.size();
-  // md_setup's vb200_setup
+  // vb200md_setup's vb200_setup
   vb200_setup *s = &h->setup;
   s->channels = h->channels;
   s->rate = h->rate;

@@ -38,6 +38,7 @@
 #include "window.h"
 
 #include "vorbis_b200.h"
+#include "vb200_vorbis_setup.h"
 
 #ifdef _OPENMP
 #include <omp.h>
@@ -118,49 +119,38 @@ void vb200md_close(vb200md *m){
   free(m);
 }
 
-/* the device setup of this decoder: transforms, windows, coupling and the floor-1 curve of every submap per
- * block size (lib/mapping0.c:714-795 reads nothing else) */
-static int md_setup(vb200md *m, vb200_setup *s){
-  codec_setup_info *ci = (codec_setup_info*)m->vi.codec_setup;
-  private_state *b = (private_state*)m->vd.backend_state;
+/* the device setup of a decoder after vorbis_synthesis_init: transforms, windows, coupling and the floor-1 curve of
+ * every submap per block size (lib/mapping0.c:714-795 reads nothing else).  0, or OV_EIMPL for a layout the device
+ * decoder does not take. */
+int vb200md_setup(vorbis_info *vi, vorbis_dsp_state *vd, vb200_setup *s){
+  codec_setup_info *ci = (codec_setup_info*)vi->codec_setup;
+  private_state *b = (private_state*)vd->backend_state;
   int w, j, k;
   memset(s, 0, sizeof(*s));
-  s->channels = m->vi.channels;
-  s->rate = (int32_t)m->vi.rate;
+  s->channels = vi->channels;
+  s->rate = (int32_t)vi->rate;
   s->blocksizes[0] = (int32_t)ci->blocksizes[0];
   s->blocksizes[1] = (int32_t)ci->blocksizes[1];
   s->window[0] = _vorbis_window_get(b->window[0]);
   s->window[1] = _vorbis_window_get(b->window[1]);
-  if(ci->modes != 2 || m->vi.channels > VB200_MAX_CHANNELS) return OV_EIMPL;
+  if(vi->channels > VB200_MAX_CHANNELS) return OV_EIMPL;
   for(w = 0; w < 2; w++){
-    vorbis_info_mapping0 *mp;
-    if(ci->mode_param[w]->blockflag != w || ci->map_type[ci->mode_param[w]->mapping] != 0) return OV_EIMPL;
-    mp = (vorbis_info_mapping0*)ci->map_param[ci->mode_param[w]->mapping];
-    if(mp->submaps > VB200_MAX_SUBMAPS || mp->coupling_steps > VB200_MAX_COUPLING) return OV_EIMPL;
+    vorbis_info_mapping0 *mp = vb200vs_mapping(ci, w);
+    if(!mp || mp->coupling_steps > VB200_MAX_COUPLING) return OV_EIMPL;
     s->coupling_steps[w] = mp->coupling_steps;
     for(k = 0; k < mp->coupling_steps; k++){ s->coupling_mag[w][k] = mp->coupling_mag[k]; s->coupling_ang[w][k] = mp->coupling_ang[k]; }
     s->submaps[w] = mp->submaps;
-    for(k = 0; k < m->vi.channels; k++) s->chmux[w][k] = (uint8_t)mp->chmuxlist[k];
+    for(k = 0; k < vi->channels; k++) s->chmux[w][k] = (uint8_t)mp->chmuxlist[k];
     for(j = 0; j < VB200_MAX_SUBMAPS; j++) s->residue[w][j].type = -1;
     for(j = 0; j < mp->submaps; j++){
-      int fl = mp->floorsubmap[j];
-      vorbis_info_floor1 *fi;
-      vorbis_look_floor1 *lk;
-      vb200_floor1_setup *o = &s->floor1[w][j];
-      if(ci->floor_type[fl] != 1) return OV_EIMPL;
-      fi = (vorbis_info_floor1*)ci->floor_param[fl];
-      lk = (vorbis_look_floor1*)b->flr[fl];
-      if(lk->posts > VB200_FLOOR1_STRIDE) return OV_EIMPL;
-      o->posts = lk->posts;
-      for(k = 0; k < lk->posts; k++) o->postlist[k] = fi->postlist[k];
-      o->mult = fi->mult; o->n = lk->n;
-      o->maxover = fi->maxover; o->maxunder = fi->maxunder; o->maxerr = fi->maxerr;
-      o->twofitweight = fi->twofitweight; o->twofitatten = fi->twofitatten;
+      const int fl = mp->floorsubmap[j];
+      const vorbis_look_floor1 *lk = (const vorbis_look_floor1*)b->flr[fl];
+      if(ci->floor_type[fl] != 1 || lk->posts > VB200_FLOOR1_STRIDE) return OV_EIMPL;
+      vb200vs_floor1(&s->floor1[w][j], (const vorbis_info_floor1*)ci->floor_param[fl], lk);
     }
   }
   return 0;
 }
-
 
 /* ---- the entropy setup of the device decoder, derived from the decoder's own tables ---------------------------- */
 typedef struct {
@@ -178,8 +168,6 @@ static uint32_t md_bitrev(uint32_t x){
   x = ((x >>  2) & 0x33333333U) | ((x <<  2) & 0xccccccccU);
   return ((x >> 1) & 0x55555555U) | ((x << 1) & 0xaaaaaaaaU);
 }
-
-static int md_ilog(unsigned v){ int r = 0; while(v){ r++; v >>= 1; } return r; }
 
 /* the codewords of one decode book (NULL arrays: count only), for both layouts of lib/codebook.h:73-110
  * (lib/sharedbook.c:393-519).  Unordered: codelist holds each codeword left-aligned, codelengths its length and
@@ -234,7 +222,7 @@ vb200_entropy_setup *vb200md_entropy_new(vorbis_info *vi, vorbis_dsp_state *vd, 
   private_state *b = (private_state*)vd->backend_state;
   md_entropy_tables *t = (md_entropy_tables*)calloc(1, sizeof(*t));
   long total = 0, at = 0;
-  int i, w, j, k, rc = OV_EFAULT;
+  int i, k, rc = OV_EFAULT;
   oggpack_buffer opb;
   if(!t) goto fail;
   for(i = 0; i < ci->books; i++) total += md_book_codewords(ci->decbooks + i, NULL, NULL, NULL);
@@ -265,42 +253,7 @@ vb200_entropy_setup *vb200md_entropy_new(vorbis_info *vi, vorbis_dsp_state *vd, 
     at += n;
   }
   oggpack_writeclear(&opb);
-  rc = OV_EIMPL;
-  if(ci->modes != 2) goto fail;
-  for(w = 0; w < 2; w++){
-    vorbis_info_mapping0 *mp;
-    if(ci->mode_param[w]->blockflag != w || ci->map_type[ci->mode_param[w]->mapping] != 0) goto fail;
-    mp = (vorbis_info_mapping0*)ci->map_param[ci->mode_param[w]->mapping];
-    if(mp->submaps > VB200_MAX_SUBMAPS) goto fail;
-    for(j = 0; j < mp->submaps; j++){
-      const int fl = mp->floorsubmap[j], rs = mp->residuesubmap[j];
-      vb200_floor_decode *f = &t->es.floor[w][j];
-      vb200_residue_decode *r = &t->es.residue[w][j];
-      f->type = ci->floor_type[fl];
-      if(f->type == 1){
-        const vorbis_info_floor1 *fi = (const vorbis_info_floor1*)ci->floor_param[fl];
-        f->partitions = fi->partitions;
-        for(k = 0; k < fi->partitions && k < 31; k++) f->partitionclass[k] = fi->partitionclass[k];
-        for(k = 0; k < 16; k++){
-          int s;
-          f->class_dim[k] = fi->class_dim[k]; f->class_subs[k] = fi->class_subs[k]; f->class_book[k] = fi->class_book[k];
-          for(s = 0; s < 8; s++) f->class_subbook[k][s] = fi->class_subbook[k][s];
-        }
-      }
-      r->type = ci->residue_type[rs];
-      {
-        const vorbis_info_residue0 *ri = (const vorbis_info_residue0*)ci->residue_param[rs];
-        int acc = 0, c;
-        r->begin = (int32_t)ri->begin; r->end = (int32_t)ri->end; r->grouping = ri->grouping;
-        r->partitions = ri->partitions; r->partvals = ri->partvals; r->groupbook = ri->groupbook;
-        for(c = 0; c < 64; c++){                  /* as res0_look lays them out, lib/res0.c:274-292 */
-          const int stages = c < ri->partitions ? md_ilog((unsigned)ri->secondstages[c]) : 0;
-          for(k = 0; k < 8; k++)
-            r->stagebook[c][k] = k < stages && (ri->secondstages[c] & (1 << k)) ? ri->booklist[acc++] : -1;
-        }
-      }
-    }
-  }
+  if((rc = vb200vs_entropy(ci, &t->books[0].dim, sizeof(*t->books), t->es.floor, t->es.residue)) != 0) goto fail;
   if(err) *err = 0;
   return &t->es;
 fail:
@@ -328,7 +281,7 @@ vb200md *vb200md_open_err(int nstreams, ogg_packet hdr[3], int pcm_s16, int devi
   m->ch = m->vi.channels;
   m->bs[0] = vorbis_info_blocksize(&m->vi, 0);
   m->bs[1] = vorbis_info_blocksize(&m->vi, 1);
-  if((rc = md_setup(m, &s)) != 0) goto fail;
+  if((rc = vb200md_setup(&m->vi, &m->vd, &s)) != 0) goto fail;
 #ifdef _OPENMP
   m->threads = omp_get_max_threads();
 #else

@@ -41,6 +41,7 @@
 #include "bitrate.h"
 
 #include "vorbis_b200.h"
+#include "vb200_vorbis_setup.h"
 
 #ifdef _OPENMP
 #include <omp.h>
@@ -220,8 +221,6 @@ static int forward_batch(vb200_binding *bind, ms_batch *B, vorbis_block **blocks
 }
 
 /* ---- the device entropy coder ------------------------------------------------------------------------------------ */
-static int ms_ilog(unsigned v){ int r = 0; while(v){ r++; v >>= 1; } return r; }
-
 /* The struct vb200_encode_entropy_setup of an encoder after vorbis_analysis_init: every book of ci->fullbooks (its
  * lengthlist, codelist and integer lattice), the floor-1 and residue fields of both modes' submaps with the stage
  * books laid out as res0_look lays out partbooks (lib/res0.c:274-292), modebits.  The codeword arrays point into the
@@ -231,9 +230,9 @@ int vb200ms_entropy_setup_build(vorbis_dsp_state *vd, struct vb200_encode_entrop
   codec_setup_info *ci = (codec_setup_info*)vd->vi->codec_setup;
   private_state *b = (private_state*)vd->backend_state;
   vb200_enc_codebook *books;
-  int i, w, j, k;
+  int i;
   memset(es, 0, sizeof(*es));
-  if(ci->modes != 2 || !ci->fullbooks) return OV_EIMPL;
+  if(!ci->fullbooks) return OV_EIMPL;
   books = (vb200_enc_codebook*)calloc(ci->books > 0 ? ci->books : 1, sizeof(*books));
   if(!books) return OV_EFAULT;
   for(i = 0; i < ci->books; i++){
@@ -243,46 +242,12 @@ int vb200ms_entropy_setup_build(vorbis_dsp_state *vd, struct vb200_encode_entrop
     books[i].minval = cb->minval; books[i].delta = cb->delta; books[i].quantvals = cb->quantvals;
   }
   es->nbooks = ci->books; es->books = books; es->modebits = b->modebits;
-  for(w = 0; w < 2; w++){
-    vorbis_info_mapping0 *mp;
-    if(ci->mode_param[w]->blockflag != w || ci->map_type[ci->mode_param[w]->mapping] != 0) goto impl;
-    mp = (vorbis_info_mapping0*)ci->map_param[ci->mode_param[w]->mapping];
-    if(mp->submaps > VB200_MAX_SUBMAPS) goto impl;
-    for(j = 0; j < VB200_MAX_SUBMAPS; j++) es->residue[w][j].type = -1;
-    for(j = 0; j < mp->submaps; j++){
-      const int fl = mp->floorsubmap[j], rs = mp->residuesubmap[j];
-      vb200_floor_decode *f = &es->floor[w][j];
-      vb200_residue_decode *r = &es->residue[w][j];
-      const vorbis_info_residue0 *ri = (const vorbis_info_residue0*)ci->residue_param[rs];
-      int acc = 0, c;
-      f->type = ci->floor_type[fl];
-      if(f->type == 1){
-        const vorbis_info_floor1 *fi = (const vorbis_info_floor1*)ci->floor_param[fl];
-        f->partitions = fi->partitions;
-        for(k = 0; k < fi->partitions && k < 31; k++) f->partitionclass[k] = fi->partitionclass[k];
-        for(k = 0; k < 16; k++){
-          int s;
-          f->class_dim[k] = fi->class_dim[k]; f->class_subs[k] = fi->class_subs[k]; f->class_book[k] = fi->class_book[k];
-          for(s = 0; s < 8; s++) f->class_subbook[k][s] = fi->class_subbook[k][s];
-        }
-      }
-      r->type = ci->residue_type[rs];
-      r->begin = (int32_t)ri->begin; r->end = (int32_t)ri->end; r->grouping = ri->grouping;
-      r->partitions = ri->partitions; r->groupbook = ri->groupbook;
-      r->partvals = 1;                                     /* look->partvals of res0_look (lib/res0.c:296) */
-      for(k = 0; k < ci->fullbooks[ri->groupbook].dim; k++) r->partvals *= ri->partitions;
-      for(c = 0; c < 64; c++){
-        const int stages = c < ri->partitions ? ms_ilog((unsigned)ri->secondstages[c]) : 0;
-        for(k = 0; k < 8; k++)
-          r->stagebook[c][k] = k < stages && (ri->secondstages[c] & (1 << k)) ? ri->booklist[acc++] : -1;
-      }
-    }
+  if(vb200vs_entropy(ci, &books[0].dim, sizeof(*books), es->floor, es->residue)){
+    free(books);
+    es->books = NULL;
+    return OV_EIMPL;
   }
   return 0;
-impl:
-  free(books);
-  es->books = NULL;
-  return OV_EIMPL;
 }
 
 /* bits bits of a device packet (bit k of the packet is bit k%8 of byte k/8) onto opb, in pieces of up to 32 bits

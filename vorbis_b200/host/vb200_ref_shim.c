@@ -36,6 +36,7 @@
 #include "envelope.h"
 
 #include "vorbis_b200.h"
+#include "vb200_vorbis_setup.h"
 
 int vb200shim_attach_new(vorbis_dsp_state *vd, int device);
 /* Bindings: one device context per codec setup (vorbis_info.codec_setup), shared by every vorbis_dsp_state
@@ -199,16 +200,8 @@ int vb200shim_attach_new(vorbis_dsp_state *vd, int device){
         o->grouping = ri->grouping; o->partitions = ri->partitions;
         for(i = 0; i < 64; i++){ o->classmetric1[i] = ri->classmetric1[i]; o->classmetric2[i] = ri->classmetric2[i]; }
       }
-      if(ci->floor_type[fl] == 1){
-        vorbis_info_floor1 *fi = (vorbis_info_floor1*)ci->floor_param[fl];
-        vorbis_look_floor1 *lk = (vorbis_look_floor1*)b->flr[fl];
-        vb200_floor1_setup *o = &s.floor1[w][j];
-        o->posts = lk->posts;
-        for(i = 0; i < lk->posts; i++) o->postlist[i] = fi->postlist[i];
-        o->mult = fi->mult; o->n = lk->n;
-        o->maxover = fi->maxover; o->maxunder = fi->maxunder; o->maxerr = fi->maxerr;
-        o->twofitweight = fi->twofitweight; o->twofitatten = fi->twofitatten;
-      }
+      if(ci->floor_type[fl] == 1)
+        vb200vs_floor1(&s.floor1[w][j], (vorbis_info_floor1*)ci->floor_param[fl], (vorbis_look_floor1*)b->flr[fl]);
     }
   }
   rc = vb200_ctx_create(&s, device, &g.ctx);
