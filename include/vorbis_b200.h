@@ -972,6 +972,65 @@ int vb200_ogg_group    (int nfiles, const uint8_t *data, int64_t data_bytes, con
                         int32_t *order, int32_t *npkt_out, struct vb200_packet_info *info_out,
                         vb200_file_group *groups, int32_t *ngroups);
 
+/* ---- sample ranges straight from Ogg files: what vorbisfile's ov_pcm_seek + ov_read give one file, for many rows in
+ * one call, without demuxing them whole (vorbis_b200/csrc/vb200_ogg_ranges.cuh).  Needs a registered
+ * vb200_decode_entropy_setup (else VB200_EINVAL); full rate, and half rate after vb200_synthesis_halfrate.
+ *   rows   row f is bytes[row_off[f] .. row_off[f+1]), what vb200_ogg_demux takes as file_off: whole files, or the
+ *          link_off of vb200_ogg_links, one row per link.  The row's stream is the one the demux picks (the serial of
+ *          its first Vorbis BOS page), read with the demux's capture, pagein and packetout rules; pages of other
+ *          serials are skipped.  Every row belongs to the context's setup (a group of vb200_ogg_group, or known).  A
+ *          row whose later link repeats the first link's serial is passed by links: the seek reads that serial's
+ *          granulepos across the row.
+ *   req    vb200_pcm_range with stream = row.  pcm, out_stride, pcm_s16 and got as in vb200_decode_ranges; got[r] is
+ *          also VB200_ENOTVORBIS or VB200_EBADHEADER where the demux gives the row that status.  Every error leaves
+ *          the row zero.
+ * Positions are granule-based, as in ov_pcm_seek.  g1 is the granulepos of the row's first accepted audio packet that
+ * carries one, c1 the samples a fresh decode returns up to and including it (vb200_decode_ranges' counting), and
+ * G0 = g1 - (c1 << halfrate).  Sample t of the row is granule G0 + (t << halfrate); a position is (g - G0) >> halfrate.
+ * Seek, per request with start t:
+ *   T = G0 + (t << halfrate) - blocksizes[1]/2.  Pages qualify when they are the row's serial, version 0, granulepos
+ *   != -1, and start at or after page A1 (the page that ends g1's packet); a BOS page of the serial ends the search
+ *   (a later link).  When g1 > T, or the row has no
+ *   g1, the request walks from the row's first audio packet: vb200_decode_ranges' plan exactly.  Otherwise P is found
+ *   by bisection over byte offsets [end of A1, end of row): while the window is longer than 8192 bytes, the first
+ *   qualifying page captured from its middle moves the low end past it when its granulepos is <= T, else the high
+ *   end to the middle; then pages are scanned forward from the low end while they qualify with granulepos <= T,
+ *   stopping after an EOS page.  P is the last page so found (A1 when none).
+ *   The walk then takes the packets that begin after P's last finished packet.  Its first accepted packet (block 1)
+ *   only primes.  The anchor is the first accepted packet of the walk with a granulepos g; with rel the sum of
+ *   blocksizes[lW]/4 + blocksizes[W]/4 over the accepted packets after block 1 up to the anchor, block 1 ends at
+ *   granule g - rel and position ((g - G0) >> halfrate) - (rel >> halfrate).  From there blockin's bookkeeping runs
+ *   as in vb200_decode_ranges (ds_blockin: block 1 as the first block of a fresh decode with granulepos g - rel), so
+ *   trims, holes and drops after P count as a fresh decode counts them.
+ *   When P is the EOS page, got = 0.  When the walk from P finds no anchor, or the anchor is the e_o_s packet (its
+ *   granulepos is the end after the trim, which cannot be counted back), P is sought once more with T = gP - 1; if
+ *   that finds no page, is the EOS page, or again gives no anchor or the e_o_s one, the request walks from the row's
+ *   first audio packet.
+ * Contract: on every row with no lost packet (sequence hole, failed capture that took packets, dropped packet) before
+ * the range's end, got and the samples equal vb200_decode_ranges on the vb200_ogg_demux tables of the same rows, bit
+ * for bit, float and int16, full and half rate.  That covers the files a stock encoder or vb200_ogg_mux writes, rows
+ * whose first granulepos is far above zero, rows with other serials interleaved and the links of chained files.  On
+ * rows with lost packets the result is the rule above (oracle/ogg_ranges.py restates it).
+ * Packet scratch: packets spanning pages are not contiguous in the file, so each request gathers the packets it keeps
+ * into pkt_cap bytes of its own: the priming block and the blocks that meet the range, plus, while the range is not
+ * met, the packet being read after the priming candidate.  pkt_cap >= the bytes of the kept packets plus the largest
+ * packet walked before the range suffices; a request that needs more gives got[r] = VB200_EINVAL, row zero.
+ * Device scratch (the arena of vb200_decode_ranges, carved once per call): nreq*(blocks*40 + 12 bytes + residue
+ * floats*4 bytes + pkt_cap bytes) + 1 byte, blocks and residue floats as in vb200_decode_ranges.
+ * Launches: a memset of the output rows, then three kernels whatever nreq and nrows are: the plan (one warp per
+ * request: the first pages, a bisection of O(log(row bytes / 8192)) page captures, and the pages from P to the
+ * range's end, each captured with its CRC), entropy decode + DSP, synthesis.  A request's cost does not grow with the
+ * row's length past the range, or with other rows.
+ * _dev: every pointer is device memory; asynchronous; checks its pointers, nreq >= 0, out_stride >= 0 and pkt_cap >= 0
+ * only.  Host form: host buffers; also checks row_off (non-decreasing from >= 0), and returns VB200_EINVAL for a
+ * request's row outside [0, nrows), start < 0 or length outside [0, out_stride].                                     */
+int vb200_ogg_ranges_dev(vb200_ctx*, int nrows, const uint8_t *d_bytes, const int64_t *d_row_off,
+                         int nreq, const vb200_pcm_range *d_req, int pcm_s16, void *d_pcm, int32_t out_stride,
+                         int64_t pkt_cap, int32_t *d_got, void *stream);
+int vb200_ogg_ranges    (vb200_ctx*, int nrows, const uint8_t *bytes, const int64_t *row_off,
+                         int nreq, const vb200_pcm_range *req, int pcm_s16, void *pcm, int32_t out_stride,
+                         int64_t pkt_cap, int32_t *got);
+
 /* ---- Ogg Vorbis files out: the page mux of libogg on the device, for many streams in one call, whole or in pieces.
  * No context.  The pages are those libogg 1.3.x (framing.c) makes when driven as examples/encoder_example.c drives it:
  * ogg_stream_packetin of the three header packets, then ogg_stream_flush until it returns 0; for every audio packet

@@ -30,6 +30,7 @@
 #include "vb200_decode_ranges.cuh"
 #include "vb200_lpc.cuh"
 #include "vb200_ogg.cuh"
+#include "vb200_ogg_ranges.cuh"
 #include "vb200_headers.h"
 #include "vb200_ogg_group.cuh"
 #include "vb200_ogg_mux.cuh"
@@ -110,7 +111,8 @@ struct vb200_ctx {
   //             that the LPC kernels build and the streams packets path reads
   //   drg       vb200_decode_streams_index[_dev]: the packet headers, the per-stream plan tables and fresh heads,
   //             sized by nstreams x max_packets; vb200_decode_ranges[_dev]: the per-request block tables and residue
-  //             scratch, sized by nreq and out_stride
+  //             scratch, sized by nreq and out_stride; vb200_ogg_ranges[_dev]: the same and the per-request packet
+  //             scratch, sized by nreq and pkt_cap
   DevBuf stage[STAGE_SLOTS], cycles, phaseA, enc, set[ENC_SETS], mgd, plan, chain, env_scratch, coder, pack,
       spk, brc, dsk, ptl, drg;
   const ResDev *d_res[2] = {nullptr, nullptr};        // [VB200_MAX_SUBMAPS] residue class parameters per block size
@@ -3478,6 +3480,89 @@ extern "C" int vb200_decode_ranges(vb200_ctx *c, int nstreams, int max_packets, 
   if (io.rc) return io.rc;
   if ((rc = vb200_decode_ranges_dev(c, nstreams, max_packets, dn, di, dd, nreq, dq, pcm_s16, dp, out_stride, dg,
                                     c->s_main))) return rc;
+  if (pbytes) io.back(pcm, dp, pbytes);
+  io.back(got, dg, nreq);
+  return io.sync();
+}
+
+// ---- sample ranges straight from Ogg files (vb200_ogg_ranges.cuh): k_or_plan in place of k_dr_plan, then the same
+// k_decode_packets<true> and k_synthesis<*, *, SYN_RANGE> over the gathered packets
+extern "C" int vb200_ogg_ranges_dev(vb200_ctx *c, int nrows, const uint8_t *d_bytes, const int64_t *d_row_off,
+                                    int nreq, const vb200_pcm_range *d_req, int pcm_s16, void *d_pcm,
+                                    int32_t out_stride, int64_t pkt_cap, int32_t *d_got, void *stream) {
+  CHECK_CTX(c);
+  if (nreq < 0) return fail(VB200_EINVAL, "nreq must be >= 0");
+  if (nreq == 0) return 0;
+  if (out_stride < 0) return fail(VB200_EINVAL, "out_stride must be >= 0");
+  if (pkt_cap < 0) return fail(VB200_EINVAL, "pkt_cap must be >= 0");
+  if (nrows < 0 || (nrows > 0 && (!d_bytes || !d_row_off)) || !d_req || !d_pcm || !d_got)
+    return fail(VB200_EINVAL, "ogg ranges pointers");
+  int rc;
+  if ((rc = ent_check(c))) return rc;
+  const long long nblk = dr_blocks(c, out_stride), rescap = dr_residue(c, out_stride);
+  if ((long long)nreq * nblk > INT32_MAX) return fail(VB200_EINVAL, "nreq * block slots must fit an int");
+  const int ch = c->setup.channels;
+  const cudaStream_t st = (cudaStream_t)stream;
+  const size_t nb = (size_t)nreq * nblk;
+  OrPlanArgs P;
+  float *res;
+  if ((rc = carve(c->drg, [&](Carve &k) {
+         P.Wseq = k.take<int>(nb); P.pkt_bytes = k.take<int>(nb); P.pkt_off = k.take<long long>(nb);
+         P.coef_off = k.take<long long>(nb); P.pcm_off = k.take<long long>(nb); P.win = k.take<int2>(nb);
+         P.count = k.take<int>(nreq); P.base = k.take<long long>(nreq + 1);
+         res = k.take<float>((size_t)nreq * rescap);
+         P.pkt = k.take<uint8_t>((size_t)nreq * pkt_cap + 1);
+       }))) return rc;
+  P.nrows = nrows; P.nreq = nreq; P.ch = ch; P.hs = c->halfrate ? 1 : 0;
+  P.modebits = c->ent.modebits;
+  P.bs[0] = c->setup.blocksizes[0]; P.bs[1] = c->setup.blocksizes[1];
+  P.out_stride = out_stride; P.nblk = (int)nblk; P.res_cap = rescap; P.pkt_cap = pkt_cap;
+  P.bytes = d_bytes; P.row_off = d_row_off; P.req = d_req; P.got = d_got;
+  if ((rc = scratch_begin(c, st))) return rc;
+  const size_t el = pcm_s16 ? sizeof(int16_t) : sizeof(float);
+  CU(cudaMemsetAsync(d_pcm, 0, el * (size_t)nreq * ch * (size_t)out_stride, st));
+  k_or_plan<<<(unsigned)((nreq + OR_WARPS - 1) / OR_WARPS), 32 * OR_WARPS, 0, st>>>(P);
+  if ((rc = post_launch(c))) return rc;
+  const DecodePackets DP{P.pkt_off, P.pkt_bytes, P.pkt};
+  if ((rc = decode_front(c, nreq, (int)nblk, P.count, P.Wseq, (const int64_t *)P.coef_off, res, nullptr, nullptr, &DP,
+                         st))) return rc;
+  DsTrim T{};
+  T.win = P.win; T.base = P.base;
+  if ((rc = synthesis_launch<SYN_RANGE>(c, pcm_s16, nreq, (int)nblk, P.count, P.Wseq, (const int64_t *)P.coef_off, res,
+                                        (const int64_t *)P.pcm_off, d_pcm, 0, nullptr, T, st))) return rc;
+  return scratch_end(c, st);
+}
+
+extern "C" int vb200_ogg_ranges(vb200_ctx *c, int nrows, const uint8_t *bytes, const int64_t *row_off,
+                                int nreq, const vb200_pcm_range *req, int pcm_s16, void *pcm, int32_t out_stride,
+                                int64_t pkt_cap, int32_t *got) {
+  CHECK_CTX(c);
+  if (nreq < 0) return fail(VB200_EINVAL, "nreq must be >= 0");
+  if (nrows < 0 || !row_off || !req || !pcm || !got || out_stride < 0 || pkt_cap < 0)
+    return fail(VB200_EINVAL, "ogg ranges pointers");
+  int rc;
+  if ((rc = ent_check(c))) return rc;
+  if (row_off[0] < 0) return fail(VB200_EINVAL, "ogg_ranges: row_off[0] < 0");
+  for (int f = 0; f < nrows; f++)
+    if (row_off[f + 1] < row_off[f]) return fail(VB200_EINVAL, "ogg_ranges: row_off decreases");
+  const int64_t total = row_off[nrows];
+  if (total && !bytes) return fail(VB200_EINVAL, "ogg ranges pointers");
+  for (int r = 0; r < nreq; r++)
+    if (req[r].stream < 0 || req[r].stream >= nrows || req[r].start < 0 || req[r].length < 0 ||
+        req[r].length > out_stride)
+      return fail(VB200_EINVAL, "a request's row, start or length is out of range");
+  if (nreq == 0) return 0;
+  std::lock_guard<std::mutex> lk(c->mu);
+  const size_t pbytes = (pcm_s16 ? sizeof(int16_t) : sizeof(float)) * (size_t)nreq * c->setup.channels * out_stride;
+  HostIO io{c};
+  const uint8_t *db = io.packets(bytes, total);
+  const int64_t *doff = io.in(row_off, (size_t)nrows + 1);
+  const vb200_pcm_range *dq = io.in(req, nreq);
+  void *dp = io.out<void>(std::max<size_t>(pbytes, 1));
+  int32_t *dg = io.out<int32_t>(nreq);
+  if (io.rc) return io.rc;
+  if ((rc = vb200_ogg_ranges_dev(c, nrows, db, doff, nreq, dq, pcm_s16, dp, out_stride, pkt_cap, dg, c->s_main)))
+    return rc;
   if (pbytes) io.back(pcm, dp, pbytes);
   io.back(got, dg, nreq);
   return io.sync();

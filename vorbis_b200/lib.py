@@ -54,7 +54,7 @@ EXPORTS = [
     "vb200_ogg_demux_dev", "vb200_ogg_demux", "vb200_ogg_links_dev", "vb200_ogg_links", "vb200_vorbis_window",
     "vb200_vorbis_headers_parse", "vb200_vorbis_headers_free",
     "vb200_ogg_group_scratch_bytes", "vb200_ogg_group_dev", "vb200_ogg_group",
-    "vb200_ogg_mux_dev", "vb200_ogg_mux",
+    "vb200_ogg_mux_dev", "vb200_ogg_mux", "vb200_ogg_ranges_dev", "vb200_ogg_ranges",
     "vb200_malloc_device", "vb200_free_device", "vb200_memcpy_h2d", "vb200_memcpy_d2h", "vb200_synchronize",
 ]
 
@@ -201,6 +201,8 @@ def load():
     L.vb200_ogg_group.argtypes = [C.c_int, vp, C.c_int64, vp, C.c_int, vp, vp, vp, vp, vp, vp, vp, vp]
     L.vb200_ogg_mux_dev.argtypes = [C.c_int, vp, C.c_int64, vp, C.c_int, vp, vp, vp, vp, C.c_int64, vp, vp, vp]
     L.vb200_ogg_mux.argtypes = [C.c_int, vp, C.c_int64, vp, C.c_int, vp, vp, vp, vp, C.c_int64, vp, vp]
+    L.vb200_ogg_ranges_dev.argtypes = [vp, C.c_int, vp, vp, C.c_int, vp, C.c_int, vp, C.c_int32, C.c_int64, vp, vp]
+    L.vb200_ogg_ranges.argtypes = [vp, C.c_int, vp, vp, C.c_int, vp, C.c_int, vp, C.c_int32, C.c_int64, vp]
     L.vb200_malloc_device.argtypes = [vp, C.c_size_t, C.POINTER(vp)]
     L.vb200_free_device.argtypes = [vp, vp]
     L.vb200_memcpy_h2d.argtypes = [vp, vp, vp, C.c_size_t]
@@ -806,6 +808,31 @@ class Context:
         self._chk(self.L.vb200_decode_ranges_dev(self.h, nstreams, max_packets, _ptr(d_npkt), _ptr(d_info),
                                                  _ptr(d_data), nreq, _ptr(d_req), pcm_s16, _ptr(d_pcm), out_stride,
                                                  _ptr(d_got), _ptr(stream)))
+
+    def ogg_ranges(self, files, req, out_stride, pkt_cap, s16=False, check=True):
+        """vb200_ogg_ranges on a list of Ogg rows (bytes or uint8 arrays) laid back to back: req PCM_RANGE_DTYPE [nreq]
+        (or (start, row, length) rows).  Returns {"pcm": float [nreq][ch][out_stride] or int16
+        [nreq][out_stride][ch], "got" int32 [nreq], "row_off" int64 [nrows+1], "rc"}"""
+        arrs = [np.frombuffer(bytes(f), np.uint8) for f in files]
+        row_off = np.zeros(len(arrs) + 1, np.int64)
+        row_off[1:] = np.cumsum([len(a) for a in arrs])
+        buf = np.ascontiguousarray(np.concatenate(arrs) if arrs else np.zeros(1, np.uint8))
+        if not (isinstance(req, np.ndarray) and req.dtype == abi.PCM_RANGE_DTYPE):
+            req = np.array([tuple(r) for r in req], abi.PCM_RANGE_DTYPE)
+        req = np.ascontiguousarray(req)
+        nreq, ch = len(req), self.channels
+        pcm = np.zeros((nreq, out_stride, ch) if s16 else (nreq, ch, out_stride), np.int16 if s16 else np.float32)
+        got = np.zeros(nreq, np.int32)
+        rc = self.L.vb200_ogg_ranges(self.h, len(arrs), _ptr(buf), _ptr(row_off), nreq, _ptr(req), 1 if s16 else 0,
+                                     _ptr(pcm), out_stride, pkt_cap, _ptr(got))
+        if check:
+            self._chk(rc)
+        return {"pcm": pcm, "got": got, "row_off": row_off, "rc": rc}
+
+    def ogg_ranges_dev(self, nrows, d_bytes, d_row_off, nreq, d_req, pcm_s16, d_pcm, out_stride, pkt_cap, d_got,
+                       stream=None):
+        self._chk(self.L.vb200_ogg_ranges_dev(self.h, nrows, _ptr(d_bytes), _ptr(d_row_off), nreq, _ptr(d_req),
+                                              pcm_s16, _ptr(d_pcm), out_stride, pkt_cap, _ptr(d_got), _ptr(stream)))
 
     # ---- encode: the entropy coding of mapping0_forward on the device -----------------------------
     def encode_entropy_setup(self, es):
