@@ -9,8 +9,9 @@ s16 staging of the transform, the k_cqn fallback, interleaved int16 output at od
 (vorbisenc divides the requested rate by the channel count) and every buffer sized by the channel count run at
 counts no other test reaches.
 
-- The stages against the oracle, which tests/test_oracle_vs_ref.py pins to the reference at these setups (MULTI), fed
-  the blocks the reference encoder cut from its chain stream (tests/golden/ref).
+- The setup-family suite of tests/setup_families.py on the rows of FAMILY: the stages against the oracle, which
+  tests/test_oracle_vs_ref.py pins to the reference at these setups (MULTI), fed the blocks the reference encoder cut
+  from its chain stream (tests/golden/ref), and packets and PCM against the stock encoder and decoder.
 - Content built so that the reference itself exercises the compaction: a silent channel between used ones, a channel
   that starts late, a copied channel, a full-scale int16 square wave, a 40 Hz sine and a stretch where every channel
   is silent.  The tests assert that the reference's capture holds those cases, then compare residue, classes, packets
@@ -26,27 +27,23 @@ import refgold as G
 import test_gpu_decode_packets as DP
 import test_gpu_decode_ranges as DR
 import test_gpu_decode_streams as DS
-import test_gpu_dropin as DI
 import test_gpu_encode_packets as EP
-import test_gpu_long_blocks as LB
-import test_gpu_parity as P
 import test_gpu_pcm_packets as PC
 import test_gpu_stream_packets as SP
-import test_gpu_stream_resume as SR
 import test_oracle_vs_ref as T
 from conftest import assert_bits_equal, probe_signal
 from oracle import bitrate as B
-from oracle import decode, halfrate, pyoracle, pyref
+from oracle import decode, pyoracle, pyref
 from oracle import decode_packets as dp
 from oracle import decode_streams as ds
+from setup_families import *  # noqa: F401,F403  (the suite's tests and fixtures, among them drivers)
+from setup_families import Family
 from test_decode_streams_oracle import make_streams
-from test_gpu_decode_streams import drivers  # noqa: F401  (a fixture)
 from vorbis_b200 import abi, lib as vlib
 
 pytestmark = pytest.mark.gpu
 
 MULTI = T.MULTI
-CAPTURE = {args: ("chain", T.chain_signal) for args in MULTI}
 # per setup: block sizes and (type, begin, end, grouping, partitions) of the residue for W = 0 and 1, read from the
 # stored setups; every one has no coupling steps and one submap holding every channel
 FEATURES = {
@@ -66,8 +63,8 @@ def _residue(setup, W):
 
 
 def check_features(setup, args):
-    """the setup has the structure this file is about, so that a vorbisenc change cannot turn the tests into a repeat
-    of the mono ones"""
+    """the setup has the structure this family is about, so that a vorbisenc change cannot turn the tests into a
+    repeat of the mono ones"""
     bs, res = FEATURES[args]
     ch = args[0]
     assert setup.channels == ch
@@ -80,109 +77,17 @@ def check_features(setup, args):
         assert got == res[W], "W=%d residue %s" % (W, got)
 
 
-@pytest.fixture(scope="module", params=MULTI, ids=lambda a: G.case_id(*a))
-def cfg(request, oracle_lib, cuda_ok):
-    """(name, setup, context, oracle, encoder blocks, None): the shape of test_gpu_parity.py's fixture"""
-    args = request.param
-    setup = G.load_setup(*args)
-    check_features(setup, args)
-    o = oracle_lib.Oracle(setup)
-    ctx = vlib.Context(setup)
-    yield G.case_id(*args), setup, ctx, o, LB._encoder_blocks(args, o, CAPTURE), None
-    ctx.close()
-
-
-# ---- stages against the oracle --------------------------------------------------------------------------------------
-def test_tables(cfg):
-    P.test_tables_match_oracle(cfg)
-
-
-@pytest.mark.parametrize("W", [0, 1])
-def test_transforms_vs_oracle(cfg, W):
-    name, setup, ctx, o, _, _ = cfg
-    LB._check_transforms(ctx, o, W, 133, 100 * W + 133)
-
-
-@pytest.mark.parametrize("look", [0, 1, 2, 3])
-def test_psy_stages(cfg, look):
-    P.test_psy_stages_vs_oracle_random(cfg, look)
-
-
-@pytest.mark.parametrize("kernel", ["fast", "generic"])
-@pytest.mark.parametrize("W", [0, 1])
-def test_phaseA(cfg, W, kernel, monkeypatch):
-    LB.test_phaseA(cfg, W, kernel, monkeypatch)
-
-
-def test_phaseA_host_multichunk_and_streams(cfg, monkeypatch):
-    """stream mode, float planar and int16 interleaved ingest (the s16 staging takes its stereo path only at two
-    channels), and the host path in many chunks"""
-    LB.test_phaseA_host_multichunk_and_streams(cfg, monkeypatch)
-
-
-@pytest.mark.parametrize("W", [0, 1])
-def test_floor1(cfg, W):
-    LB.test_floor1(cfg, W)
-
-
-@pytest.mark.parametrize("W", [0, 1])
-def test_couple_quantize_normalize(cfg, W):
-    """k_cqn, the fallback every count above two takes"""
-    P.test_couple_quantize_normalize_vs_oracle_random(cfg, W)
-
-
-@pytest.mark.parametrize("W", [0, 1])
-def test_residue_and_inverse_floor(cfg, W):
-    P.test_residue_classify_vs_oracle(cfg, W)
-    P.test_floor1_inverse2_vs_oracle(cfg, W)
-
-
-def test_synthesis_and_decode(cfg):
-    LB.test_synthesis_and_decode(cfg)
-
-
-@pytest.mark.parametrize("fmt", ["blocks", "f32", "s16"])
-@pytest.mark.parametrize("W", [0, 1])
-def test_encode_dsp_streams(cfg, W, fmt, monkeypatch):
-    P.test_encode_dsp_streams_vs_oracle(cfg, W, fmt, monkeypatch)
-
-
-def test_encode_dsp_pipeline_forms(cfg, monkeypatch):
-    LB.test_encode_dsp_pipeline_forms(cfg, monkeypatch)
-
-
-@pytest.mark.parametrize("fmt", ["s16", "blocks"])
-@pytest.mark.parametrize("W", [0, 1])
-def test_encode_dsp_managed(cfg, W, fmt):
-    P.test_encode_dsp_managed_vs_oracle(cfg, W, fmt)
-
-
-def test_envelope_and_plan(cfg):
-    LB.test_envelope_and_plan(cfg)
-
-
-def test_envelope_search_vs_reference(cuda_ok):
-    """the device's envelope search on the reference's own stream buffers gives its marks and filter state"""
-    for args in MULTI:
-        LB.test_envelope_search_vs_reference(cuda_ok, args)
-
-
-def test_encode_streams_mixed_block_sizes(cfg):
-    for fmt in ("f32", "s16"):
-        LB.test_encode_streams_mixed_block_sizes(cfg, fmt)
-
-
-@pytest.fixture(scope="module")
-def halfrate_cfg(cfg):
-    name, setup, _, _, enc, _ = cfg
-    ctx = vlib.Context(setup)
-    ctx.synthesis_halfrate(1)
-    yield name, setup, ctx, halfrate.Oracle.create(setup), enc, None
-    ctx.close()
-
-
-def test_halfrate(halfrate_cfg):
-    LB.test_halfrate(halfrate_cfg)
+# name, channels, rate, max, nominal and min bitrate, the small-reservoir settings, and the VBR quality whose template
+# vorbisenc picks for the nominal rate per channel (64 and 96 kbit/s on rate_mapping_44_un)
+MANAGED = [("abr512_71", 8, 48000, -1, 512000, -1, None, 0.14),
+           ("cbr384_quad", 4, 44100, 384000, 384000, 384000, None, 0.5)]
+FAMILY = Family(
+    name="multi", setups=MULTI, capture={}, check=check_features, blocksizes=lambda args: FEATURES[args][0],
+    nvec=[[133]], fmts=[["f32", "s16"]], envelope=[MULTI],
+    rows={"test_stock_encoder_packets": MULTI, "test_stock_decoder": MULTI, "test_stock_halfrate_decoder": MULTI,
+          "test_function_level_dropin": MULTI,
+          "test_stock_managed_encoder": [pytest.param(*m[:7], id="-".join(map(str, m))) for m in MANAGED]},
+    uncoupled_q={m[0]: m[7] for m in MANAGED})
 
 
 # ---- the classes layout ---------------------------------------------------------------------------------------------
@@ -359,42 +264,7 @@ def test_content_vs_stock_decoder(cuda_ok, drivers, args):  # noqa: F811
         DS._check(got, want, ch, s16, "content s16=%s" % s16)
 
 
-# ---- against the stock encoder and decoder (oracle/_ref) ------------------------------------------------------------
-@pytest.mark.parametrize("ch,rate,q", MULTI)
-def test_stock_encoder_packets(cuda_ok, ch, rate, q):
-    """captured blocks through encode_dsp + encode_entropy and encode_packets; whole streams in one call, through a
-    fresh carry and cut into pieces; raw float and int16 PCM one call per stock write"""
-    EP.test_stage_parity_captured_blocks(cuda_ok, ch, rate, q)
-    SP.test_unmanaged_whole_streams(cuda_ok, ch, rate, q)
-    SR.test_fresh_carry_one_call_equals_packets_call(cuda_ok, ch, rate, q)
-    SR.test_cuts_equal_one_call_unmanaged(cuda_ok, ch, rate, q)
-    PC.test_one_call_per_stock_write(cuda_ok, ch, rate, q)
-
-
-@pytest.mark.parametrize("ch,rate,q", MULTI)
-def test_stock_decoder(cuda_ok, drivers, ch, rate, q):  # noqa: F811
-    """the entropy decode's staging, the fused decode, the vb200md driver, and decode_streams_packets and
-    decode_ranges on the seven kinds of stream of tests/test_decode_streams_oracle.py"""
-    if not (decode.available() and dp.available()):
-        pytest.skip("oracle/_ref not built (needs the reference sources at build time)")
-    made = []
-
-    def driver(p):
-        made.append(dp.Driver(p))
-        return made[-1]
-    try:
-        DP.test_stage_parity(cuda_ok, driver, ch, rate, q)
-        DP.test_fused_equals_entropy_then_dsp(cuda_ok, driver, ch, rate, q, "two")
-    finally:
-        for d in made:
-            d.close()
-    for s16 in (False, True):
-        DP.test_driver_device_and_host_paths_equal_stock(cuda_ok, ch, rate, q, s16)
-    for page_final in (False, True):
-        DS.test_streams_equal_stock_decoder(cuda_ok, drivers, ch, rate, q, page_final)
-        DR.test_index_and_ranges_equal_stock_decoder(cuda_ok, drivers, ch, rate, q, page_final)
-
-
+# ---- odd channel counts ---------------------------------------------------------------------------------------------
 @pytest.mark.parametrize("out_stride", [4097, 11025])
 @pytest.mark.parametrize("args", [(3, 44100, 0.4), (5, 44100, 0.9), (3, 22050, 0.3)], ids=lambda a: G.case_id(*a))
 def test_odd_channels_and_odd_out_stride(cuda_ok, drivers, args, out_stride):  # noqa: F811
@@ -411,60 +281,6 @@ def test_odd_channels_and_odd_out_stride(cuda_ok, drivers, args, out_stride):  #
     for s16 in (False, True):
         DR._check_ranges(ctx.decode_ranges(npkt, info, buf, req, out_stride, s16=s16), req, whole, s16,
                          "%d channels, out_stride %d s16=%s" % (ch, out_stride, s16))
-
-
-@pytest.mark.parametrize("ch,rate,q", MULTI)
-def test_stock_halfrate_decoder(cuda_ok, drivers, ch, rate, q):  # noqa: F811
-    """half rate: decode_streams_packets and decode_ranges against the stock half-rate decoder, and the reference
-    decoder with mdct_backward on the device at half and full rate"""
-    DS.test_halfrate_equals_stock_halfrate_decoder(cuda_ok, drivers, ch, rate, q)
-    DR.test_halfrate_equals_stock_halfrate_decoder(cuda_ok, drivers, ch, rate, q)
-    if not (halfrate.ref_available() and halfrate.ref_available(dropin=True)):
-        pytest.skip("oracle/_ref not built (needs the reference sources at build time)")
-    pcm = probe_signal(ch, rate, 0.6, seed=5)
-    packets = halfrate.ref_encode(ch, rate, q, pcm)
-    bs = FEATURES[(ch, rate, q)][0]
-    for half in (True, False):
-        want = halfrate.ref_decode(packets, bs, ch, pcm.shape[1] + 8192, halfrate=half)
-        got = halfrate.ref_decode(packets, bs, ch, pcm.shape[1] + 8192, halfrate=half, dropin=True)
-        assert set(want["W"].tolist()) == {0, 1}
-        assert np.array_equal(got["W"], want["W"]) and got["pcm"].shape == want["pcm"].shape
-        assert np.array_equal(got["pcm"].view(np.uint32), want["pcm"].view(np.uint32)), "half rate %s" % half
-
-
-@pytest.mark.parametrize("ch,rate,q", MULTI)
-def test_function_level_dropin(cuda_ok, ch, rate, q):
-    """the reference's encoder and decoder with their hot callees bound to the device: byte-identical packets and
-    bit-identical PCM"""
-    DI.test_encoder_packets_identical(cuda_ok, ch, rate, q)
-
-
-# name, channels, rate, max, nominal and min bitrate, the small-reservoir settings, and the VBR quality whose template
-# vorbisenc picks for the nominal rate per channel (64 and 96 kbit/s on rate_mapping_44_un)
-MANAGED = [("abr512_71", 8, 48000, -1, 512000, -1, None, 0.14),
-           ("cbr384_quad", 4, 44100, 384000, 384000, 384000, None, 0.5)]
-
-
-@pytest.mark.parametrize("name,ch,rate,max_br,nominal,min_br,rm2,q", MANAGED)
-def test_stock_managed_encoder(cuda_ok, name, ch, rate, max_br, nominal, min_br, rm2, q):
-    """the managed encoder takes the uncoupled template of the rate per channel; whole streams in one call, in pieces
-    and from raw PCM"""
-    SP._need_ref()
-    if not B.ref_available(True):
-        pytest.skip("oracle/_ref not built (needs the reference sources at build time)")
-    d = B.ManagedDriver(ch, rate, max_br, nominal, min_br)       # refuses a host entropy path
-    bs, partvals = list(d.ctx.bs), [d.ctx.residue_partvals(W) for W in (0, 1)]
-    d.close()
-    r = pyref.Ref(ch, rate, q)
-    s = r.setup()
-    r.close()
-    assert list(s.c.coupling_steps) == [0, 0] and list(s.c.submaps) == [1, 1]
-    assert bs == [s.blocksize(0), s.blocksize(1)] == [256, 2048], name
-    assert partvals == [(s.c.residue[W][0].end - s.c.residue[W][0].begin) // s.c.residue[W][0].grouping
-                        for W in (0, 1)], "%s: %s partitions" % (name, partvals)
-    SP.test_managed_whole_streams(cuda_ok, name, ch, rate, max_br, nominal, min_br, rm2)
-    SR.test_cuts_equal_one_call_managed(cuda_ok, name, ch, rate, max_br, nominal, min_br, rm2)
-    PC.test_managed_one_call_per_stock_write(cuda_ok, name, ch, rate, max_br, nominal, min_br, rm2)
 
 
 # ---- many channels --------------------------------------------------------------------------------------------------

@@ -11,12 +11,14 @@ from conftest import assert_bits_equal, probe_signal
 from vorbis_b200 import abi, lib as vlib
 
 # the setups vorbisenc picks above q = 0.5: full-band residue with the _residue_44_high / _hi_un / _44p_hi books,
-# uncoupled 5.1 (no coupling steps, two submaps), 96 kHz and coupled 22.05 kHz stereo (tests/test_gpu_high_quality.py)
+# uncoupled 5.1 (no coupling steps, two submaps), 96 kHz and coupled 22.05 kHz stereo (tests/test_gpu_high_quality.py,
+# the family "high" of tests/setup_families.py)
 HIGH = [(2, 44100, 0.6), (2, 44100, 1.0), (1, 44100, 0.9), (6, 48000, 0.5), (6, 48000, 0.9), (2, 96000, 0.7),
         (2, 22050, 0.9)]
 HIGH_NEW = [a for a in HIGH if a != (2, 96000, 0.7)]          # the lists that already hold (2, 96000, 0.7)
 # the uncoupled setups vorbisenc picks for channel counts other than 1, 2 and 6: one submap over every channel, no
-# coupling steps, type-1 residue over several channels (tests/test_gpu_multichannel.py)
+# coupling steps, type-1 residue over several channels (tests/test_gpu_multichannel.py, the family
+# "multi" of tests/setup_families.py)
 MULTI = [(3, 44100, 0.4), (4, 48000, 0.1), (5, 44100, 0.9), (8, 48000, 0.3), (8, 44100, -0.1), (4, 32000, 0.2),
          (3, 22050, 0.3)]
 GRID = [(2, 44100, 0.5), (1, 44100, 0.4), (2, 44100, 0.1), (2, 44100, 0.3), (1, 44100, 0.2),

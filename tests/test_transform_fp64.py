@@ -7,7 +7,8 @@ mdct_backward and drft_forward (float32, the reference's own arithmetic) are com
 evaluated in float64.  The error bound is calibrated at N = 2048, where the oracle is pinned to the reference bit for
 bit: the float32 rounding error measured there, times a small factor, grows with log2 N.  An indexing or twiddle mistake
 at any size gives errors of the order of the signal and fails by many orders of magnitude.
-tests/test_gpu_long_blocks.py holds the device's transforms to the same bound."""
+tests/test_gpu_long_blocks.py holds the device's transforms to the same bound (with the checks of
+tests/setup_families.py)."""
 import numpy as np
 import pytest
 
