@@ -177,9 +177,10 @@ def test_odd_channels_and_odd_out_stride(cuda_ok, drivers, out_stride):  # noqa:
 
 @pytest.mark.parametrize("seed", range(4))
 def test_fuzzed_bookkeeping_equals_streams(cuda_ok, drivers, seed):  # noqa: F811
-    """k_dr_plan runs blockin's bookkeeping as its own copy of k_ds_plan's step: on seeded packet metadata (granulepos
-    on random packets, some behind the count, packetno gaps, e_o_s flags, dropped and empty packets) the ranges of a
-    stream equal the matching slices of a fresh-carry vb200_decode_streams_packets call, and got follows its lengths"""
+    """k_dr_plan walks the packets its own way and takes k_ds_plan's blockin step (ds_blockin) on them: on seeded
+    packet metadata (granulepos on random packets, some behind the count, packetno gaps, e_o_s flags, dropped and empty
+    packets) the ranges of a stream equal the matching slices of a fresh-carry vb200_decode_streams_packets call, and
+    got follows its lengths"""
     _need()
     ch, rate, q = CASES[0]
     buf, hdr, audios = make_streams(ch, rate, q)

@@ -30,9 +30,13 @@ PAGINGS = [dict(max_segs=255), dict(max_segs=4), dict(max_segs=255, headers_alon
 def launched_kernels(call):
     """names of the kernels call() launches (it synchronises), from torch.profiler.  A profiler session can lose the
     record of the first kernel it sees, so a torch kernel (at::native, which the library never launches) runs first
-    and is left out of the list."""
+    and is left out of the list.  The first session of a process (CUPTI starting up) can lose every record, so a
+    session with only that torch kernel runs before the one that is read."""
     import torch
     from torch.profiler import ProfilerActivity, profile
+    with profile(activities=[ProfilerActivity.CUDA]):
+        torch.ones(1, device="cuda").add_(1)
+        torch.cuda.synchronize()
     with profile(activities=[ProfilerActivity.CUDA]) as prof:
         torch.ones(1, device="cuda").add_(1)
         torch.cuda.synchronize()

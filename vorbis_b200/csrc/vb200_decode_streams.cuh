@@ -85,9 +85,7 @@ k_ds_header(int nstreams, int max_packets, int modebits, const int *__restrict__
 
 // blockin's bookkeeping for one packet that vorbis_synthesis accepted (block flag W): h advances, and [lo, hi) is
 // the window of the block's finished samples that pcmout returns (lib/block.c:741-751, 835-941, >> hs at half rate).
-// bs: blocksizes.  k_ds_plan runs the same step written out in its loop: called from there, this function changes
-// that kernel's register allocation, so its SASS would not stay as it was; the index and ranges tests check that the
-// two give the same windows.
+// bs: blocksizes.  k_ds_plan, k_dr_plan and k_or_plan all take this step.
 __device__ __forceinline__ void ds_blockin(DsHead &h, int W, const vb200_packet_info &p, const int *bs, int hs,
                                            long long &lo_, long long &hi_) {
   const int lW = h.W;
@@ -170,45 +168,10 @@ k_ds_plan(DsPlanArgs A) {
       continue;
     }
     const vb200_packet_info p = A.info[slot];
-    const int lW = h.W, W = v;
-    const long long fin = lW >= 0 ? (long long)((A.bs[lW] / 4 + A.bs[W] / 4) >> hs) : 0;
-    if (h.sequence == -1 || h.sequence + 1 != (long long)p.packetno) { h.granulepos = -1; h.sample_count = -1; }
-    h.sequence = p.packetno;
-    long long lo = 0, hi = fin;                            // pcm_returned, pcm_current past prevCenter
-    if (h.sample_count == -1) h.sample_count = 0;
-    else h.sample_count += A.bs[lW] / 4 + A.bs[W] / 4;
-    if (h.granulepos == -1) {
-      if (p.granulepos != -1) {
-        h.granulepos = p.granulepos;
-        if (h.sample_count > h.granulepos) {
-          long long extra = h.sample_count - p.granulepos;
-          if (extra < 0) extra = 0;
-          if (p.e_o_s) {                                   // trim the end
-            if (extra > (hi - lo) << hs) extra = (hi - lo) << hs;
-            hi -= extra >> hs;
-          } else {                                         // trim the beginning
-            lo += extra >> hs;
-            if (lo > hi) lo = hi;
-          }
-        }
-      }
-    } else {
-      h.granulepos += A.bs[lW] / 4 + A.bs[W] / 4;
-      if (p.granulepos != -1 && h.granulepos != p.granulepos) {
-        if (h.granulepos > p.granulepos) {
-          long long extra = h.granulepos - p.granulepos;
-          if (extra && p.e_o_s) {                          // partial last frame
-            if (extra > (hi - lo) << hs) extra = (hi - lo) << hs;
-            if (extra < 0) extra = 0;
-            hi -= extra >> hs;
-          }
-        }
-        h.granulepos = p.granulepos;
-      }
-    }
-    h.W = W;
+    long long lo, hi;
+    ds_blockin(h, v, p, A.bs, hs, lo, hi);
     const size_t b = (size_t)st * A.max_packets + j;
-    A.Wseq[b] = W;
+    A.Wseq[b] = v;
     A.pkt_off[b] = p.offset;
     A.pkt_bytes[b] = p.bytes;
     A.coef_off[b] = (long long)b * rows;

@@ -78,10 +78,11 @@ __device__ __forceinline__ uint32_t ogg_page_crc(const uint8_t *pg, int len, int
 
 // ogg_sync_pageseek at byte p of a file that ends at `end`, by one converged warp, as k_ogg_demux captures.  Returns
 // the captured page's length, 0 when the capture failed (p then moved to the next 'O' after it, or to end), or -1 when
-// fewer than 27 bytes are left or the page is cut short by the end of the file.  k_ogg_demux keeps this step written
-// out in its loop, because it stages the lacing table on the way: called from there, this function changes that
-// kernel's register allocation, so its SASS would not stay as it was.  The tests hold this step to oracle/ogg_links.py
-// and the demux's copy to oracle/ogg.py, which capture pages alike.
+// fewer than 27 bytes are left or the page is cut short by the end of the file.  k_ogg_demux keeps this step and its
+// packet walk written out in its loop, with one copy of each page body: the demux on this function and k_or_plan's
+// walk (or_walk, which copies packet by packet so that its visitors can move and drop packets) measured slower on an
+// H100 once many files share the GPU (INTEGRATION §2g).  The tests hold this step to oracle/ogg_links.py and the
+// demux's copy to oracle/ogg.py, which capture pages alike.
 __device__ __forceinline__ int ogg_capture(const uint8_t *bytes, int64_t &p, int64_t end, int lane,
                                            const uint32_t *crc_tab, const uint32_t *xpw) {
   if (end - p < 27) return -1;
