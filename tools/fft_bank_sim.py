@@ -7,6 +7,9 @@ request costs max over banks of the number of distinct words; a 64-bit request i
 128-bit one per quarter-warp.  Lanes of a warp that take different branches issue separate instructions.
 Compare with the shared-memory bank conflicts by source line of a profile of k_phaseA_transform.
 
+The templated sizes run two levels per pass (dev_fft_pass44 / dev_fft_pass42): sim_fused() models those passes with
+the kernel's item order and reports them beside the one-level schedule, on the padding the kernel uses.
+
 usage: tools/fft_bank_sim.py [N] [threads]
 """
 import sys
@@ -120,6 +123,83 @@ PADS = {
     "2 per 32 + 4 per 256": lambda a: a + 2 * (a >> 5) + 4 * (a >> 8),
 }
 
+def _count(items, gen):
+    """items in thread order; gen(v) -> (branch, [(slot, width, addr) loads], [(slot, width, addr) stores])"""
+    loads = stores = 0
+    for w0 in range(0, items, 32):
+        ins_l, ins_s = defaultdict(list), defaultdict(list)
+        for lane in range(32):
+            v = w0 + lane
+            if v >= items:
+                continue
+            br, ls, ss = gen(v)
+            for s, w, a in ls:
+                ins_l[(br, s, w)].append((lane, a))
+            for s, w, a in ss:
+                ins_s[(br, s, w)].append((lane, a))
+        loads += sum(wavefronts(a, key[2]) for key, a in ins_l.items())
+        stores += sum(wavefronts(a, key[2]) for key, a in ins_s.items())
+    return loads, stores
+
+
+def sim_fused(pad):
+    """the two-levels-per-pass schedule of the templated kernels: {pass name: (loads, stores)} for one row"""
+    wr = lambda e: pad(e + 1)
+    single = sim(pad)
+    ps = passes(N)
+    res, k1 = {}, 0
+    while k1 < len(ps):
+        ip, l1, ido, first = ps[k1]
+        if ip != 4 or k1 + 1 == len(ps):
+            res["radix %d ido=%d" % (ip, ido)] = single[(ip, l1, ido)]
+            k1 += 1
+            continue
+        ipb = ps[k1 + 1][0]
+        a, L, t0, ib = ido, l1, l1 * ido, 4 * ido
+        nj = 4 if ipb == 4 else 2
+        Ls = L // nj                                       # k step between the level-A blocks of one item
+        rd = (lambda e: e) if first else wr
+
+        def tw_stores(o, ip_):
+            if ipb == 4:
+                return [o + ip_ - 1, o + 2 * ib - ip_ - 1, o + 2 * ib + ip_ - 1, o + 4 * ib - ip_ - 1]
+            return [o + ip_ - 1, o + 2 * ib - ip_ - 1]
+
+        if a == 1:
+            def gen(kp):
+                ls = [((j, s), 1, rd(kp + Ls * j + s * t0)) for j in range(4) for s in range(4)]
+                o = 16 * kp
+                ss = [("0", 1, wr(o)), ("15", 1, wr(o + 15)), ("7", 2, wr(o + 7)), ("3", 2, wr(o + 3)),
+                      ("11", 2, wr(o + 11))] + [(("t", n), 2, wr(e)) for n, e in enumerate(tw_stores(o, 2))]
+                return "a", ls, ss
+            items = Ls
+        else:
+            hm1 = a // 2 - 1
+
+            def gen(v):
+                o = nj * (v if v < Ls else (v - Ls) // hm1) * ib
+                if v < Ls:
+                    ls = [((c, j, s), 1, wr((v + Ls * j) * a + c + s * t0)) for c in (0, a - 1) for j in range(nj)
+                          for s in range(4)]
+                    ss = [("0", 1, wr(o)), ("e", 1, wr(o + nj * ib - 1)), ("m", 2, wr(o + (2 if nj == 4 else 1) * ib - 1))]
+                    if nj == 4:
+                        ss += [("1", 2, wr(o + ib - 1)), ("3", 2, wr(o + 3 * ib - 1))]
+                    for m in (1, 2, 3):
+                        ss += [(("t", m, n), 2, wr(e)) for n, e in enumerate(tw_stores(o, m * a))]
+                    return "s", ls, ss
+                g = v - Ls
+                kp, i = g // hm1, 2 * (1 + g % hm1)
+                ls = [((j, s), 2, wr((kp + Ls * j) * a + i - 1 + s * t0)) for j in range(nj) for s in range(4)]
+                ss = []
+                for m, ip_ in enumerate((i, 2 * a - i, 2 * a + i, 4 * a - i)):
+                    ss += [(("t", m, n), 2, wr(e)) for n, e in enumerate(tw_stores(o, ip_))]
+                return "t", ls, ss
+            items = Ls * (a // 2)
+        res["radix 4+%d ido=%d,%d" % (ipb, a, ib)] = _count(items, gen)
+        k1 += 2
+    return res
+
+
 if __name__ == "__main__":
     print("real FFT of N=%d, wavefronts per row (loads + stores); the ideal is one per 32 lanes x 4 B" % N)
     for name, pad in PADS.items():
@@ -131,3 +211,9 @@ if __name__ == "__main__":
         if name in ("none", "2 per 32"):
             for (ip, l1, ido), (l, s) in r.items():
                 print("      radix %d  l1=%4d ido=%4d   loads %5d stores %5d" % (ip, l1, ido, l, s))
+    kernel_pad = PADS["2 per 32"]
+    r = sim_fused(kernel_pad)
+    print("two levels per pass (templated sizes), padding 2 per 32: loads %5d stores %5d total %5d"
+          % (sum(v[0] for v in r.values()), sum(v[1] for v in r.values()), sum(sum(v) for v in r.values())))
+    for name, (l, s) in r.items():
+        print("      %-22s loads %5d stores %5d" % (name, l, s))

@@ -736,7 +736,7 @@ k_phaseA_transform(XformDev X, WinDev Wd, int W, int ch, int nrows,
     }
     __syncthreads();
     mode = row + gridDim.x < nrows ? stage(row + gridDim.x) : 0;
-    dev_mdct_forward<NC>(X, sx, sw, mdct + (size_t)row * n, tid, nt, mdct_pad_buffer(sf));
+    dev_mdct_forward<NC, (NC > 0)>(X, sx, sw, mdct + (size_t)row * n, tid, nt, mdct_pad_buffer(sf));
     const float *f = dev_drft_forward<NC>(X, sx, sf, tid, nt);
     // log spectrum + local maximum (lib/mapping0.c:310-345)
     float mx = -1e30f;

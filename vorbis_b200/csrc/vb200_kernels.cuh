@@ -179,13 +179,87 @@ __device__ __forceinline__ void dev_fly8(const float4 v0, const float4 v1, float
   o1.w = s73 + s51;  o1.y = s73 - s51;
 }
 
+// one radix-2 butterfly of mdct_butterfly_generic / _first (lib/mdct.c:216-314): hi <- hi + lo, lo <- (hi - lo) * t
+__device__ __forceinline__ void fly_bf(float2 &hi, float2 &lo, float2 t) {
+  const float r0 = hi.x - lo.x, r1 = hi.y - lo.y;
+  hi = make_float2(hi.x + lo.x, hi.y + lo.y);
+  lo = make_float2(r1 * t.y + r0 * t.x, r1 * t.x - r0 * t.y);
+}
+
+// The item of the 32-point fly's first level (lib/mdct.c:152-209; see the loop in dev_butterflies, which keeps its
+// own copy so that the kernels without paired levels compile as before) on registers: hi = (30-2q), lo = (14-2q).
+__device__ __forceinline__ void fly32_bf(float2 &hi, float2 &lo, int q) {
+  const float dxp = hi.x - lo.x, dxn = lo.x - hi.x, dyp = hi.y - lo.y, dyn = lo.y - hi.y;
+  const float r0 = q >= 5 ? dxn : dxp;
+  const float r1 = q >= 4 ? dyn : dyp;
+  // odd q: o0 = r0*k00 + r1*k01, o1 = r0*k10 + r1*k11
+  const bool q15 = (q == 1) | (q == 7);                // k00 = k11 = C1 there, C3 for q = 3, 5
+  const float k00 = q15 ? VB_C1 : VB_C3;
+  const float k3 = q15 ? VB_C3 : VB_C1;                // the other constant, sign by case
+  const float k01 = q < 4 ? -k3 : k3;
+  const float k10 = q < 4 ? k3 : -k3;
+  const float A0 = r0 * k00 + r1 * k01;
+  const float A1 = r0 * k10 + r1 * k00;
+  // q = 2: (r0 - r1)*C2, (r0 + r1)*C2;  q = 6: (r1 + r0)*C2, (r1 - r0)*C2
+  const float B0 = (q == 2 ? r0 - r1 : r1 + r0) * VB_C2;
+  const float B1 = (q == 2 ? r0 + r1 : r1 - r0) * VB_C2;
+  // q = 0: r0, r1;  q = 4: r1, r0
+  const float T0 = q == 0 ? r0 : r1, T1 = q == 0 ? r1 : r0;
+  const bool odd = q & 1, triv = (q & 3) == 0;
+  const float o0 = odd ? A0 : (triv ? T0 : B0);
+  const float o1 = odd ? A1 : (triv ? T1 : B1);
+  hi = make_float2(hi.x + lo.x, hi.y + lo.y);
+  lo = make_float2(o0, o1);
+}
+
+// Levels s and s+1 of the butterflies in one shared-memory pass (NC > 0; level nst is the 32-point fly's first
+// level).  Level s pairs (P-2-2q, P/2-2-2q) in a block of P values; level s+1 does the same in each half.  Level-s
+// items q and q + P/8 touch exactly the four pairs that level s+1 item q touches in the two halves, so one thread
+// takes those four pairs through both levels in registers.
 template <int NC>
+__device__ __forceinline__ void dev_fly_pair(const XformDev &X, float *x, int s, int tid, int nt) {
+  constexpr int log2n = XLog2<NC>::v, nst = log2n - 6, n2 = NC >> 1;
+  const int P = n2 >> s, e = P >> 3;
+  const int sh = log2n - 4 - s;                  // log2(P/8)
+  const float2 *tw = X.stage_tw + X.stage_off[s];
+  for (int u = tid; u < (n2 >> 3); u += nt) {
+    const int blk = u >> sh, q = u & (e - 1);
+    float *xb = x + P * blk;
+    float2 *pu1 = reinterpret_cast<float2 *>(xb + P - 2 - 2 * q);
+    float2 *pl1 = reinterpret_cast<float2 *>(xb + (P >> 1) - 2 - 2 * q);
+    float2 *pu2 = reinterpret_cast<float2 *>(xb + 3 * (P >> 2) - 2 - 2 * q);
+    float2 *pl2 = reinterpret_cast<float2 *>(xb + (P >> 2) - 2 - 2 * q);
+    float2 u1 = *pu1, l1 = *pl1, u2 = *pu2, l2 = *pl2;
+    fly_bf(u1, l1, __ldg(tw + q));
+    fly_bf(u2, l2, __ldg(tw + q + e));
+    if (s + 1 < nst) {
+      const float2 t = __ldg(X.stage_tw + X.stage_off[s + 1] + q);
+      fly_bf(u1, u2, t);
+      fly_bf(l1, l2, t);
+    } else {
+      fly32_bf(u1, u2, q);
+      fly32_bf(l1, l2, q);
+    }
+    *pu1 = u1; *pl1 = l1; *pu2 = u2; *pl2 = l2;
+  }
+}
+
+// PAIRED (NC > 0 only): the generic levels and the 32-point fly's first level two per pass (dev_fly_pair)
+template <int NC, bool PAIRED = false>
 __device__ __forceinline__ void dev_butterflies(const XformDev &X, float *x, int tid, int nt, float *padbuf = nullptr) {
   const int N = NC ? NC : X.N;
   const int log2n = NC ? XLog2<NC>::v : X.log2n;
   const int nst = log2n - 6;
   const int n2 = N >> 1;
   const int items = n2 >> 2;
+  if constexpr (PAIRED) {
+    static_assert(NC > 0, "paired butterflies need the block size at compile time");
+#pragma unroll
+    for (int s = 0; s + 1 <= nst; s += 2) {
+      dev_fly_pair<NC>(X, x, s, tid, nt);
+      __syncthreads();
+    }
+  } else {
 #pragma unroll
   for (int s = 0; s < nst; s++) {
     const int P = n2 >> s;
@@ -205,6 +279,8 @@ __device__ __forceinline__ void dev_butterflies(const XformDev &X, float *x, int
     }
     __syncthreads();
   }
+  }
+  if (!PAIRED || ((nst + 1) & 1)) {   // paired: an odd level count leaves the 32-point level on its own
   // 32-point fly, first level (lib/mdct.c:152-209): item q pairs (30-2q) with (14-2q).  The eight cases of
   // the reference differ in which difference they take (a-b or b-a: both are computed, x-x is +0 either way,
   // so one is not the negation of the other) and in the rotation: none (q=0,4), (r0 -/+ r1)*C2 (q=2,6), or
@@ -239,6 +315,7 @@ __device__ __forceinline__ void dev_butterflies(const XformDev &X, float *x, int
     *reinterpret_cast<float2 *>(xc + b) = make_float2(o0, o1);
   }
   __syncthreads();
+  }
   // 16-point fly (lib/mdct.c:117-147) with its two 8-point flies (:93-115): one item per 16 values, all in
   // registers - one shared-memory round trip and one barrier instead of two, and no per-lane case split
   for (int u = tid; u < (n2 >> 4); u += nt) {
@@ -311,7 +388,8 @@ __device__ __forceinline__ void dev_bitreverse(const XformDev &X, float *w, int 
 // mdct_forward, lib/mdct.c:492-562.
 // padbuf: optional n2 + n2/16 + n2/256 + 8 floats of scratch (16-byte aligned) for the padded hand-over
 // between the butterflies and the bit-reverse stage
-template <int NC>
+// PAIRED: the butterflies two levels per pass (dev_butterflies), for the templated transform kernel
+template <int NC, bool PAIRED = false>
 __device__ __forceinline__ void dev_mdct_forward(const XformDev &X, const float *in, float *w,
                                                  float *out, int tid, int nt, float *padbuf = nullptr) {
   const int N = NC ? NC : X.N, n2 = N >> 1, n4 = N >> 2, n16 = N >> 4;
@@ -340,7 +418,7 @@ __device__ __forceinline__ void dev_mdct_forward(const XformDev &X, const float 
     *reinterpret_cast<float2 *>(w2 + 2 * p) = make_float2(r1 * t.y + r0 * t.x, r1 * t.x - r0 * t.y);
   }
   __syncthreads();
-  dev_butterflies<NC>(X, w2, tid, nt, padbuf);
+  dev_butterflies<NC, PAIRED>(X, w2, tid, nt, padbuf);
   dev_bitreverse<NC>(X, w, tid, nt, padbuf);
   const float2 *Tp = reinterpret_cast<const float2 *>(X.trig + n2);
   const float scale = X.scale;
@@ -556,12 +634,259 @@ __device__ __forceinline__ void dev_fft_pass2(int ido, int l1, const float *cc, 
   }
 }
 
+// ---- Two FFT levels per shared-memory pass (the power-of-two sizes with NC known at compile time).
+// Level A is a dradf4 pass (ido = a, l1 = L); level B the pass after it (ido = 4a, l1 = L/4 for radix 4,
+// L/2 for radix 2).  Level B reads element i' + 4a*k' + t0*j' (t0 = L*a = N/4), which level A writes as
+// element i' of its output block k = k' + (L/4)*j' (radix-2 B: k = k' + (L/2)*j', j' < 2).  So the level-A
+// items of one column i at those 4 (2) values of k produce exactly the inputs of 4 level-B items, which one
+// thread runs from registers: one load and one store of every element per two levels, and one barrier.
+// The butterflies below are those of dev_fft_pass4 / dev_fft_pass2, expression for expression.
+
+// dradf4, column 0 (and the whole butterfly when ido = 1): o[0], (o[2ido-1], o[2ido]), o[4ido-1]
+__device__ __forceinline__ void r4_col0(float a0, float a1, float a2, float a3, float &y0, float2 &y2, float &y4) {
+  const float tr1 = a1 + a3;
+  const float tr2 = a0 + a2;
+  y0 = tr1 + tr2;
+  y2 = make_float2(a0 - a2, a3 - a1);
+  y4 = tr2 - tr1;
+}
+// dradf4, column ido-1: (o[ido-1], o[ido]), (o[3ido-1], o[3ido])
+__device__ __forceinline__ void r4_colL(float a0, float a1, float a2, float a3, float2 &y1, float2 &y3) {
+  const float hsqt2 = .70710678118654752f;
+  const float ti1 = -hsqt2 * (a1 + a3);
+  const float tr1 =  hsqt2 * (a1 - a3);
+  y1 = make_float2(tr1 + a0, ti1 - a2);
+  y3 = make_float2(a0 - tr1, ti1 + a2);
+}
+// dradf4, twiddled pair i (input pairs (i-1, i) of the four l1 blocks): the output pairs ending at
+// i, 2ido-i, 2ido+i and 4ido-i
+__device__ __forceinline__ void r4_tw(float2 a0, float2 a1, float2 a2, float2 a3, const float *w1, const float *w2,
+                                      const float *w3, int i, float2 &y0, float2 &y1, float2 &y2, float2 &y3) {
+  const float wa1r = __ldg(w1 + i - 2), wa1i = __ldg(w1 + i - 1);
+  const float wa2r = __ldg(w2 + i - 2), wa2i = __ldg(w2 + i - 1);
+  const float wa3r = __ldg(w3 + i - 2), wa3i = __ldg(w3 + i - 1);
+  const float cr2 = wa1r * a1.x + wa1i * a1.y;
+  const float ci2 = wa1r * a1.y - wa1i * a1.x;
+  const float cr3 = wa2r * a2.x + wa2i * a2.y;
+  const float ci3 = wa2r * a2.y - wa2i * a2.x;
+  const float cr4 = wa3r * a3.x + wa3i * a3.y;
+  const float ci4 = wa3r * a3.y - wa3i * a3.x;
+  const float tr1 = cr2 + cr4, tr4 = cr4 - cr2;
+  const float ti1 = ci2 + ci4, ti4 = ci2 - ci4;
+  const float ti2 = a0.y + ci3, ti3 = a0.y - ci3;
+  const float tr2 = a0.x + cr3, tr3 = a0.x - cr3;
+  y0 = make_float2(tr1 + tr2, ti1 + ti2);
+  y1 = make_float2(tr3 - ti4, tr4 - ti3);
+  y2 = make_float2(ti4 + tr3, tr4 + ti3);
+  y3 = make_float2(tr2 - tr1, ti1 - ti2);
+}
+// dradf2, twiddled pair i: the output pairs ending at i and 2ido-i
+__device__ __forceinline__ void r2_tw(float2 a0, float2 a1, const float *w1, int i, float2 &y0, float2 &y1) {
+  const float wr = __ldg(w1 + i - 2), wi = __ldg(w1 + i - 1);
+  const float tr2 = wr * a1.x + wi * a1.y;
+  const float ti2 = wr * a1.y - wi * a1.x;
+  y0 = make_float2(a0.x + tr2, a0.y + ti2);
+  y1 = make_float2(a0.x - tr2, ti2 - a0.y);
+}
+__device__ __forceinline__ void st_f2(float *p, int e, float2 v) { *reinterpret_cast<float2 *>(p + fft_idx(e)) = v; }
+// padded index of e + D from r = fft_idx(e): one add when 32 | D (D is a compile-time constant in the fused passes),
+// so the loads of an item share one index computation
+__device__ __forceinline__ int fft_idx_add(int r, int e, int D) { return (D & 31) == 0 ? r + D + (D >> 4) : fft_idx(e + D); }
+__device__ __forceinline__ float2 ld_f2(const float *p) { return *reinterpret_cast<const float2 *>(p); }
+
+// level-B dradf4 (ido = ib) twiddled item i' of block k' from its four input pairs, stored
+__device__ __forceinline__ void r4_tw_store(const float2 (&p)[4], const float *w1, const float *w2, const float *w3,
+                                            int ip, int ib, int o, float *ch) {
+  float2 y0, y1, y2, y3;
+  r4_tw(p[0], p[1], p[2], p[3], w1, w2, w3, ip, y0, y1, y2, y3);
+  const int e0 = o + ip - 1, e1 = o + 2 * ib - ip - 1;
+  const int r0 = fft_idx(e0), r1 = fft_idx(e1);
+  *reinterpret_cast<float2 *>(ch + r0) = y0;
+  *reinterpret_cast<float2 *>(ch + r1) = y1;
+  *reinterpret_cast<float2 *>(ch + fft_idx_add(r0, e0, 2 * ib)) = y2;
+  *reinterpret_cast<float2 *>(ch + fft_idx_add(r1, e1, 2 * ib)) = y3;
+}
+
+// dradf4 (ido = a, l1 = L) then dradf4 (ido = 4a, l1 = L/4).  FIRST: level A reads the plain input (a = 1 only).
+template <bool FIRST>
+__device__ __forceinline__ void dev_fft_pass44(int a, int L, const float *cc, float *ch,
+                                               const float *wa1, const float *wa2, const float *wa3,
+                                               const float *wb1, const float *wb2, const float *wb3, int tid, int nt) {
+  const int t0 = L * a, Lq = L >> 2, ib = 4 * a;
+  if (a == 1) {
+    // item k': the four one-column level-A butterflies of k = k' + Lq*j' give the 16 elements of level-B block k'
+    for (int kp = tid; kp < Lq; kp += nt) {
+      float y0[4], y3[4];
+      float2 y12[4];
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        const int k = kp + Lq * j;
+        r4_col0(cc[fft_rd<FIRST>(k)], cc[fft_rd<FIRST>(k + t0)], cc[fft_rd<FIRST>(k + 2 * t0)],
+                cc[fft_rd<FIRST>(k + 3 * t0)], y0[j], y12[j], y3[j]);
+      }
+      const int o = 16 * kp;
+      float z0, z15;
+      float2 z7, z3, z11;
+      r4_col0(y0[0], y0[1], y0[2], y0[3], z0, z7, z15);
+      ch[fft_idx(o)] = z0;
+      st_f2(ch, o + 7, z7);
+      ch[fft_idx(o + 15)] = z15;
+      r4_colL(y3[0], y3[1], y3[2], y3[3], z3, z11);
+      st_f2(ch, o + 3, z3);
+      st_f2(ch, o + 11, z11);
+      r4_tw_store(y12, wb1, wb2, wb3, 2, 4, o, ch);
+    }
+    return;
+  }
+  // a >= 4: Lq*a/2 items of 32 elements.  The first Lq are the two un-twiddled level-A columns of block k'
+  // (giving level B's un-twiddled columns and its pairs i' = a, 2a, 3a), the others one twiddled level-A
+  // column i (giving level B's pairs i' = i, 2a-i, 2a+i, 4a-i).
+  const int hm1 = (a >> 1) - 1;
+  const int items = Lq * (a >> 1);
+  for (int v = tid; v < items; v += nt) {
+    if (v < Lq) {
+      const int kp = v;
+      float s0[4], s1[4];
+      float2 pa[3][4];                                     // [i' = a, 2a, 3a][j']
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        const int c0 = kp * a, e = c0 + a - 1, D = Lq * a * j;
+        const int r = fft_idx(c0), q = fft_idx(e);
+        r4_col0(cc[fft_idx_add(r, c0, D)], cc[fft_idx_add(r, c0, D + t0)], cc[fft_idx_add(r, c0, D + 2 * t0)],
+                cc[fft_idx_add(r, c0, D + 3 * t0)], s0[j], pa[1][j], s1[j]);
+        r4_colL(cc[fft_idx_add(q, e, D)], cc[fft_idx_add(q, e, D + t0)], cc[fft_idx_add(q, e, D + 2 * t0)],
+                cc[fft_idx_add(q, e, D + 3 * t0)], pa[0][j], pa[2][j]);
+      }
+      const int o = 4 * kp * ib;
+      float z0, zl;
+      float2 zm, z1, z3;
+      r4_col0(s0[0], s0[1], s0[2], s0[3], z0, zm, zl);
+      ch[fft_idx(o)] = z0;
+      st_f2(ch, o + 2 * ib - 1, zm);
+      ch[fft_idx(o + 4 * ib - 1)] = zl;
+      r4_colL(s1[0], s1[1], s1[2], s1[3], z1, z3);
+      st_f2(ch, o + ib - 1, z1);
+      st_f2(ch, o + 3 * ib - 1, z3);
+#pragma unroll
+      for (int m = 0; m < 3; m++) r4_tw_store(pa[m], wb1, wb2, wb3, (m + 1) * a, ib, o, ch);
+    } else {
+      const int g = v - Lq;
+      const int kp = g / hm1, i = 2 * (1 + g - kp * hm1);
+      const int e = kp * a + i - 1, r = fft_idx(e);
+      float2 y[4][4];                                      // [i' = i, 2a-i, 2a+i, 4a-i][j']
+#pragma unroll
+      for (int j = 0; j < 4; j++) {
+        const int D = Lq * a * j;
+        r4_tw(ld_f2(cc + fft_idx_add(r, e, D)), ld_f2(cc + fft_idx_add(r, e, D + t0)),
+              ld_f2(cc + fft_idx_add(r, e, D + 2 * t0)), ld_f2(cc + fft_idx_add(r, e, D + 3 * t0)), wa1, wa2, wa3, i,
+              y[0][j], y[1][j], y[2][j], y[3][j]);
+      }
+      const int o = 4 * kp * ib;
+      r4_tw_store(y[0], wb1, wb2, wb3, i, ib, o, ch);
+      r4_tw_store(y[1], wb1, wb2, wb3, 2 * a - i, ib, o, ch);
+      r4_tw_store(y[2], wb1, wb2, wb3, 2 * a + i, ib, o, ch);
+      r4_tw_store(y[3], wb1, wb2, wb3, 4 * a - i, ib, o, ch);
+    }
+  }
+}
+
+// dradf4 (ido = a >= 4, l1 = L) then dradf2 (ido = 4a, l1 = L/2): items of 16 elements, as in dev_fft_pass44
+__device__ __forceinline__ void dev_fft_pass42(int a, int L, const float *cc, float *ch,
+                                               const float *wa1, const float *wa2, const float *wa3,
+                                               const float *wb1, int tid, int nt) {
+  const int t0 = L * a, Lh = L >> 1, ib = 4 * a;
+  const int hm1 = (a >> 1) - 1;
+  const int items = Lh * (a >> 1);
+  for (int v = tid; v < items; v += nt) {
+    if (v < Lh) {
+      const int kp = v;
+      float s0[2], s1[2];
+      float2 pa[3][2];                                     // [i' = a, 2a, 3a][j']
+#pragma unroll
+      for (int j = 0; j < 2; j++) {
+        const int c0 = kp * a, e = c0 + a - 1, D = Lh * a * j;
+        const int r = fft_idx(c0), q = fft_idx(e);
+        r4_col0(cc[fft_idx_add(r, c0, D)], cc[fft_idx_add(r, c0, D + t0)], cc[fft_idx_add(r, c0, D + 2 * t0)],
+                cc[fft_idx_add(r, c0, D + 3 * t0)], s0[j], pa[1][j], s1[j]);
+        r4_colL(cc[fft_idx_add(q, e, D)], cc[fft_idx_add(q, e, D + t0)], cc[fft_idx_add(q, e, D + 2 * t0)],
+                cc[fft_idx_add(q, e, D + 3 * t0)], pa[0][j], pa[2][j]);
+      }
+      const int o = 2 * kp * ib;
+      ch[fft_idx(o)]              = s0[0] + s0[1];
+      ch[fft_idx(o + 2 * ib - 1)] = s0[0] - s0[1];
+      st_f2(ch, o + ib - 1, make_float2(s1[0], -s1[1]));
+#pragma unroll
+      for (int m = 0; m < 3; m++) {
+        const int ip = (m + 1) * a;
+        float2 y0, y1;
+        r2_tw(pa[m][0], pa[m][1], wb1, ip, y0, y1);
+        st_f2(ch, o + ip - 1, y0);
+        st_f2(ch, o + 2 * ib - ip - 1, y1);
+      }
+    } else {
+      const int g = v - Lh;
+      const int kp = g / hm1, i = 2 * (1 + g - kp * hm1);
+      const int e = kp * a + i - 1, r = fft_idx(e);
+      float2 y[4][2];                                      // [i' = i, 2a-i, 2a+i, 4a-i][j']
+#pragma unroll
+      for (int j = 0; j < 2; j++) {
+        const int D = Lh * a * j;
+        r4_tw(ld_f2(cc + fft_idx_add(r, e, D)), ld_f2(cc + fft_idx_add(r, e, D + t0)),
+              ld_f2(cc + fft_idx_add(r, e, D + 2 * t0)), ld_f2(cc + fft_idx_add(r, e, D + 3 * t0)), wa1, wa2, wa3, i,
+              y[0][j], y[1][j], y[2][j], y[3][j]);
+      }
+      const int o = 2 * kp * ib;
+      const int ips[4] = {i, 2 * a - i, 2 * a + i, 4 * a - i};
+#pragma unroll
+      for (int m = 0; m < 4; m++) {
+        float2 y0, y1;
+        r2_tw(y[m][0], y[m][1], wb1, ips[m], y0, y1);
+        st_f2(ch, o + ips[m] - 1, y0);
+        st_f2(ch, o + 2 * ib - ips[m] - 1, y1);
+      }
+    }
+  }
+}
+
+// the factor of pass k1 of a power-of-two N (see dev_drft_forward)
+__host__ __device__ constexpr int fft_factor(int log2n, int k1) { return (k1 == ((log2n + 1) >> 1) - 1 && (log2n & 1)) ? 2 : 4; }
+
+// dev_drft_forward for NC > 0: the passes from K1 on, two levels per pass where both exist and the first is radix 4
+template <int NC, int K1, int L2, int IW>
+__device__ __forceinline__ float *dev_drft_passes(const XformDev &X, float *src, float *dst, int tid, int nt) {
+  constexpr int log2n = XLog2<NC>::v, nf = (log2n + 1) >> 1;
+  if constexpr (K1 >= nf) {
+    return src;
+  } else {
+    constexpr int ipA = fft_factor(log2n, K1), l1A = L2 / ipA, idoA = NC / L2, iwA = IW - (ipA - 1) * idoA;
+    const float *wa = X.wa + iwA - 1;
+    if constexpr (ipA == 4 && K1 + 1 < nf) {
+      constexpr int ipB = fft_factor(log2n, K1 + 1), l1B = l1A / ipB, idoB = NC / l1A, iwB = iwA - (ipB - 1) * idoB;
+      const float *wb = X.wa + iwB - 1;
+      if constexpr (ipB == 4) {
+        dev_fft_pass44<K1 == 0>(idoA, l1A, src, dst, wa, wa + idoA, wa + 2 * idoA, wb, wb + idoB, wb + 2 * idoB, tid, nt);
+      } else {
+        static_assert(K1 > 0, "the radix-2 pass is never second");
+        dev_fft_pass42(idoA, l1A, src, dst, wa, wa + idoA, wa + 2 * idoA, wb, tid, nt);
+      }
+      __syncthreads();
+      return dev_drft_passes<NC, K1 + 2, l1B, iwB>(X, dst, src, tid, nt);
+    } else {
+      if constexpr (ipA == 4) dev_fft_pass4<K1 == 0>(idoA, l1A, src, dst, wa, wa + idoA, wa + 2 * idoA, tid, nt);
+      else dev_fft_pass2<K1 == 0>(idoA, l1A, src, dst, wa, tid, nt);
+      __syncthreads();
+      return dev_drft_passes<NC, K1 + 1, l1A, iwA>(X, dst, src, tid, nt);
+    }
+  }
+}
+
 // a: N plain input floats (16-byte aligned).  a and b must each have room for fft_buf_floats(N) floats:
 // after the first pass `a` is reused as a padded ping-pong buffer.  Returns the buffer that holds the
 // result; logical element e of it is at [fft_idx(e)].
 template <int NC>
 __device__ __forceinline__ float *dev_drft_forward(const XformDev &X, float *a, float *b,
                                                    int tid, int nt) {
+  if constexpr (NC > 0) return dev_drft_passes<NC, 0, NC, NC>(X, a, b, tid, nt);
   const int N = NC ? NC : X.N;
   // power-of-two N: drfti1 stores 4,..,4 with a single 2 (odd log2) moved to the front, and the
   // passes run last factor first: radix 4 throughout, the radix-2 pass (if any) comes last
