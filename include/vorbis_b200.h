@@ -22,7 +22,8 @@
  *     the host-pointer entry points serialise on a per-context mutex.  _dev calls
  *     that use that scratch (Phase A, encode_dsp, encode_dsp_managed,
  *     encode_streams, encode_streams_managed, envelope_search, encode_entropy,
- *     encode_entropy_managed) may be issued on different CUDA streams: each waits
+ *     encode_entropy_managed, encode_pcm_packets, encode_pcm_packets_managed)
+ *     may be issued on different CUDA streams: each waits
  *     (on the device, via an event) for the previous such call of the same
  *     context, so they never share
  *     the scratch in time.  Growing the scratch re-allocates (cudaFree/cudaMalloc
@@ -1327,7 +1328,9 @@ int vb200_encode_streams_packets_managed_resume(vb200_ctx*, int nstreams, vb200_
  * pcm_len[s] below the kept samples or above stream_stride, an end call with new samples, an end on an undrained
  * carry, a second end, and samples after the end.  Launches: four (the preamble filters, the timelines up to eof, the
  * tail filters, the tails) plus those of the _resume call, whatever the stream count.  Device scratch: that of the
- * _resume calls plus the input and nstreams x channels x (the longest timeline passed) floats.  Host pointers only. */
+ * _resume calls plus the input and nstreams x channels x tl_stride floats of timeline, tl_stride = stream_stride +
+ * blocksizes[1]/2 + 3*blocksizes[1] rounded up to a multiple of 4.  Host pointers; the _dev forms below take device
+ * memory. */
 typedef struct vb200_pcm_carry {
   vb200_encode_carry enc;  /* the encode carry's head (base in timeline samples, granulepos, packetno, done) */
   int64_t raw_base;        /* input sample where the next call's buffer starts: max(0, enc.base - blocksizes[1]/2) */
@@ -1353,6 +1356,49 @@ int vb200_encode_pcm_packets        (vb200_ctx*, int nstreams, int blobno, vb200
                                      vb200_packet_info *info, uint8_t *data, int64_t data_cap);
 int vb200_encode_pcm_packets_managed(vb200_ctx*, int nstreams, vb200_pcm_io *io, void *carry,
                                      vb200_packet_info *info, uint8_t *data, int64_t data_cap);
+/* The same calls on device memory, for PCM that is already on the GPU (a model's output, a batch just decoded) and
+ * packets that stay there (vb200_decode_streams_packets_dev, vb200_ogg_mux_dev).  Per-stream bookkeeping, the carry
+ * checks and the carry update run on the device, and the carries stay there.
+ *   d_io     a host struct: pcm, pcm_len, end, plan and nblocks point to device memory; pcm_fmt, max_blocks,
+ *            stream_stride and cap[] are read on the host; count[] is not written (see d_result).
+ *   mark_steps  the value given to vb200_encode_pcm_carry_init, so that the carry stride is known on the host.
+ *   d_first  [nstreams] or NULL: row s of pcm starts at input sample first[s] (NULL: the carry's raw_base), and
+ *            pcm_len[s] counts samples from there.  A row needs first[s] <= raw_base and first[s] + pcm_len[s] >=
+ *            written; its new samples are those past written.  So a whole clip can stay in one buffer passed with
+ *            first = 0 on every call, and no carry has to be read back to lay out the next call's rows.
+ *   d_carry  [nstreams][vb200_encode_pcm_carry_bytes(ctx, mark_steps)]: the bytes of the host form's carries, so a
+ *            carry moves between the forms at any call boundary (vb200_encode_pcm_carry_init on the host, then copy).
+ *   d_info, d_data, data_cap, d_status [nstreams], d_result: device outputs.
+ * Returns VB200_EINVAL at once only for what the host sees: a null context or pointer, pcm_fmt, max_blocks < 1,
+ * cap < 0, blobno, nstreams x max_blocks, no encode entropy setup, (managed) no managed bitrate setup.  Everything
+ * else is reported on the device: status[s] = VB200_EINVAL for a carry of another setup or mark capacity, a managed
+ * carry made before the bitrate setup, pcm_len below the kept samples or above stream_stride, first out of range, an
+ * end call with new samples, a second end, an end on an undrained carry, samples after the end; result->rc =
+ * VB200_EINVAL for any such stream, count > cap, bytes > data_cap or a mark window overflow.  With rc != 0 no packet
+ * byte is written and every carry stays byte for byte; status, count and bytes (when the plan fits cap) say what the
+ * call needs.  With rc == 0 the packets, info, plan, nblocks, counts and carries are the host form's, bit for bit.
+ * Asynchronous on `stream`: no launch waits for the plan, so every launch and carve after it is sized by cap[w]
+ * (every slot up to cap[w] is transformed and coded; the ones the plan leaves empty hold a copy of a valid block that
+ * nothing reads), and the counts, the refusals and the bytes stay on the device.  So cap[] near the need (e.g. the
+ * last call's count plus a margin) keeps the work near the host form's.  Scratch: the context's (the interlock of
+ * the _dev calls above): nstreams x ch x tl_stride floats of timeline (tl_stride from stream_stride, as above: a whole
+ * clip passed on every call costs its length in timeline each call), and per size w the chain of cap[w] blocks (the
+ * transforms, masks, posts, nonzero and iwork of cap[w] x ch rows, x VB200_PACKETBLOBS curves for managed) and the
+ * strided packets of cap[w] blocks.  Launches: a fixed number per call, whatever the stream count. */
+typedef struct vb200_encode_result {   /* device memory, written by every _dev packet call */
+  int64_t bytes;      /* bytes of this call's packets, whether or not they fit data_cap (0 when count > cap) */
+  int32_t count[2];   /* blocks of each size the call planned, whether or not they fit cap[] */
+  int32_t rc;         /* 0, or VB200_EINVAL */
+  int32_t pad;
+} vb200_encode_result;
+int vb200_encode_pcm_packets_dev        (vb200_ctx*, int nstreams, int blobno, int mark_steps, const vb200_pcm_io *d_io,
+                                         const int64_t *d_first, void *d_carry, vb200_packet_info *d_info,
+                                         uint8_t *d_data, int64_t data_cap, int32_t *d_status,
+                                         vb200_encode_result *d_result, void *stream);
+int vb200_encode_pcm_packets_managed_dev(vb200_ctx*, int nstreams, int mark_steps, const vb200_pcm_io *d_io,
+                                         const int64_t *d_first, void *d_carry, vb200_packet_info *d_info,
+                                         uint8_t *d_data, int64_t data_cap, int32_t *d_status,
+                                         vb200_encode_result *d_result, void *stream);
 /* The stage call of those kernels: per row r, vorbis_lpc_from_data(data[r][0 .. n[r]), order) (lib/lpc.c:60-130), then
  * vorbis_lpc_predict of `count` samples continuing the window, primed with its last `order` samples (:132-159).
  * order 16 or 32; order <= n[r] <= data_stride; out_stride >= count.  coeff [nrows][order] and out [nrows][out_stride]

@@ -225,6 +225,9 @@ assert ENCODE_CARRY_HEAD_DTYPE.itemsize == 24
 PCM_CARRY_HEAD_DTYPE = np.dtype([("enc", ENCODE_CARRY_HEAD_DTYPE), ("raw_base", "<i8"), ("written", "<i8"),
                                  ("ended", "<i4"), ("drained", "<i4")])
 assert PCM_CARRY_HEAD_DTYPE.itemsize == 48
+# vb200_encode_result: what a _dev packet call reports on the device
+ENCODE_RESULT_DTYPE = np.dtype([("bytes", "<i8"), ("count", "<i4", (2,)), ("rc", "<i4"), ("pad", "<i4")])
+assert ENCODE_RESULT_DTYPE.itemsize == 24
 # vb200_decoded_packet: what vb200_decode_streams_packets reports for every packet it was given
 DECODED_PACKET_DTYPE = np.dtype([("pcm_offset", "<i8"), ("granulepos", "<i8"), ("samples", "<i4"), ("status", "<i4")])
 assert DECODED_PACKET_DTYPE.itemsize == 24

@@ -29,6 +29,7 @@
 #include "vb200_decode_streams.cuh"
 #include "vb200_decode_ranges.cuh"
 #include "vb200_lpc.cuh"
+#include "vb200_pcm.cuh"
 #include "vb200_ogg.cuh"
 #include "vb200_ogg_ranges.cuh"
 #include "vb200_headers.h"
@@ -107,8 +108,9 @@ struct vb200_ctx {
   //   brc       the host form of vb200_bitrate_addblocks
   //   dsk       vb200_decode_streams_packets[_dev]: the packet headers, the block tables, the per-stream plan and the
   //             residue scratch, sized by nstreams x max_packets
-  //   ptl       vb200_encode_pcm_packets[_managed]: the planar float timelines [nstreams][ch][longest this call passes]
-  //             that the LPC kernels build and the streams packets path reads
+  //   ptl       vb200_encode_pcm_packets[_managed][_dev]: the planar float timelines [nstreams][ch][tl_stride], the
+  //             carries unpacked, the LPC jobs, and the posts / nonzero / iwork of cap[] blocks that the streams
+  //             packets path writes
   //   drg       vb200_decode_streams_index[_dev]: the packet headers, the per-stream plan tables and fresh heads,
   //             sized by nstreams x max_packets; vb200_decode_ranges[_dev]: the per-request block tables and residue
   //             scratch, sized by nreq and out_stride; vb200_ogg_ranges[_dev]: the same and the per-request packet
@@ -2392,9 +2394,12 @@ static int streams_check(vb200_ctx *c, int nstreams, vb200_streams_io *d) {
 // the managed tail, which a[w] taps the noise and tone masks into.  Begins the call's use of the context scratch.
 // K: carried streams (the envelope state, marks, planner and ampmax chain start from the carries and go back to
 // them); K->count's largest entry is nsteps_env.
+// async_tot (the _dev raw-PCM calls): nothing waits for the plan.  The launches and carves after it are sized by
+// cap[] (count[] = cap[]), k_plan_pad fills the slots the plan leaves empty with a valid block, and *async_tot gets
+// the plan's device totals; a plan past cap[] or a mark window overflow is for the caller to report on the device.
 static int streams_front(vb200_ctx *c, int nstreams, vb200_streams_io *d, cudaStream_t st, EncScratch S[2],
                          vb200_phaseA_io a[2], vb200_block_desc *d_desc[2], MgdScratch *M = nullptr,
-                         const CarryDev *K = nullptr, int nsteps_env = 0) {
+                         const CarryDev *K = nullptr, int nsteps_env = 0, const int32_t **async_tot = nullptr) {
   int rc;
   const int ch = c->setup.channels;
   // 1. envelope search over the whole timeline (fresh detector state), 2. marks, 3. plan
@@ -2434,9 +2439,19 @@ static int streams_front(vb200_ctx *c, int nstreams, vb200_streams_io *d, cudaSt
   if ((rc = plan_launch(c, nstreams, d_mark, mark_stride, nsteps, d->pcm_len, d->eof, d->max_blocks, d->plan, d->nblocks,
                         d->cap, d_src, d_desc, d_tot, d_work, st, K))) return rc;
   int tot[2], overflow = 0;
-  CU(cudaMemcpyAsync(tot, d_tot, sizeof(tot), cudaMemcpyDeviceToHost, st));
-  if (K) CU(cudaMemcpyAsync(&overflow, K->overflow, sizeof(int), cudaMemcpyDeviceToHost, st));
-  CU(cudaStreamSynchronize(st));                       // the launches below are sized by the plan
+  if (async_tot) {
+    tot[0] = d->cap[0]; tot[1] = d->cap[1];
+    *async_tot = d_tot;
+    if (tot[0] > 0 || tot[1] > 0) {
+      k_plan_pad<<<dim3(grid_for(c, (std::max(tot[0], tot[1]) + 255) / 256, 8), 2), 256, 0, st>>>(
+          d_tot, tot[0], tot[1], d_src[0], d_src[1], d_desc[0], d_desc[1]);
+      if ((rc = post_launch(c))) return rc;
+    }
+  } else {
+    CU(cudaMemcpyAsync(tot, d_tot, sizeof(tot), cudaMemcpyDeviceToHost, st));
+    if (K) CU(cudaMemcpyAsync(&overflow, K->overflow, sizeof(int), cudaMemcpyDeviceToHost, st));
+    CU(cudaStreamSynchronize(st));                     // the launches below are sized by the plan
+  }
   d->count[0] = tot[0]; d->count[1] = tot[1];
   if (overflow) return fail(VB200_EINVAL, "encode carry: the mark window does not fit the carry's mark capacity");
   if (tot[0] > d->cap[0] || tot[1] > d->cap[1]) return fail(VB200_EINVAL, "encode_streams: more blocks than cap[] (count[] holds the need)");
@@ -2462,15 +2477,18 @@ static int streams_front(vb200_ctx *c, int nstreams, vb200_streams_io *d, cudaSt
   {
     float sa[2];
     for (int w = 0; w < 2; w++) sa[w] = ((float)(c->dx[w].N / 2) / (float)c->setup.rate) * c->setup.ampmax_att_per_sec;   // lib/psy.c:843
+    for (int w = 0; w < 2; w++)                        // the padded slots' ampmax, which nothing reads
+      if (async_tot && tot[w]) CU(cudaMemsetAsync(S[w].gmax, 0, sizeof(float) * tot[w], st));
     if (K)
       k_ampmax_plan_carry<<<(nstreams + 127) / 128, 128, 0, st>>>(nstreams, d->max_blocks, ch, d->plan, d->nblocks,
                                                                   tot[0] ? S[0].lmax : nullptr, tot[1] ? S[1].lmax : nullptr,
                                                                   sa[0], sa[1], tot[0] ? S[0].gmax : nullptr,
-                                                                  tot[1] ? S[1].gmax : nullptr, K->pc);
+                                                                  tot[1] ? S[1].gmax : nullptr, tot[0], tot[1], K->pc);
     else
       k_ampmax_plan<<<(nstreams + 127) / 128, 128, 0, st>>>(nstreams, d->max_blocks, ch, d->plan, d->nblocks,
                                                             tot[0] ? S[0].lmax : nullptr, tot[1] ? S[1].lmax : nullptr,
-                                                            sa[0], sa[1], tot[0] ? S[0].gmax : nullptr, tot[1] ? S[1].gmax : nullptr);
+                                                            sa[0], sa[1], tot[0] ? S[0].gmax : nullptr, tot[1] ? S[1].gmax : nullptr,
+                                                            tot[0], tot[1]);
     if ((rc = post_launch(c))) return rc;
   }
   return 0;
@@ -2480,7 +2498,7 @@ static int streams_front(vb200_ctx *c, int nstreams, vb200_streams_io *d, cudaSt
 // (optional): the two batches' block descriptors, which stay in the plan arena until its next carve
 static int encode_streams_launch(vb200_ctx *c, int nstreams, int blobno, bool managed, vb200_streams_io *d,
                                  cudaStream_t st, vb200_block_desc **desc_out, const CarryDev *K = nullptr,
-                                 int nsteps_env = 0) {
+                                 int nsteps_env = 0, const int32_t **async_tot = nullptr) {
   int rc;
   if ((rc = streams_check(c, nstreams, d)) || nstreams <= 0) return rc;
   if (!managed && (blobno < 0 || blobno >= VB200_PACKETBLOBS)) return fail(VB200_EINVAL, "blobno");
@@ -2489,7 +2507,7 @@ static int encode_streams_launch(vb200_ctx *c, int nstreams, int blobno, bool ma
   vb200_phaseA_io a[2];
   vb200_block_desc *d_desc[2];
   MgdScratch M[2];
-  if ((rc = streams_front(c, nstreams, d, st, S, a, d_desc, managed ? M : nullptr, K, nsteps_env))) return rc;
+  if ((rc = streams_front(c, nstreams, d, st, S, a, d_desc, managed ? M : nullptr, K, nsteps_env, async_tot))) return rc;
   // 6. the rest of the chain per size
   for (int w = 0; w < 2; w++) {
     if (!d->count[w]) continue;
@@ -4062,15 +4080,83 @@ static void carry_unpack(vb200_ctx *c, int nstreams, int cap, const CarryBlob &b
   }
 }
 
-// Both whole-stream packet calls: the streams chain into staged device buffers, the entropy coder per size, then
-// (k_stream_bits, [k_bitrate_choose], k_packet_offsets, k_stream_gather) on the spk arena, carved once when the
-// per-size block counts are known.  One synchronous round trip on s_main.  carry (host): the _resume forms, whose
-// carries are staged as one more buffer and written back only when the call succeeds.  staged (the raw-PCM calls):
-// the caller holds c->mu, h->pcm is a float planar timeline already on the device, and the call stages through the
-// caller's HostIO.
+// The device half of every streams packets call, on st: the streams chain into d's device buffers (Kp: carried
+// streams), the entropy coder per size, then (k_stream_bits, [k_bitrate_choose], k_packet_offsets, k_stream_gather)
+// on the spk arena, carved once when the per-size block counts are known.  dinfo / dpk: the caller's, or when null
+// carved here (dpk with data_cap bytes) and returned; *total: the device byte total.  R (the _dev raw-PCM calls): the
+// chain runs without waiting for its plan, sized by cap[] (streams_front), and the call's vb200_encode_result is
+// written before the gather, which writes bytes only when its rc is 0.
+struct SpkResult { vb200_encode_result *res; const int32_t *bad; };
+static int spk_chain(vb200_ctx *c, int nstreams, int blobno, bool managed, vb200_streams_io *d, cudaStream_t st,
+                     const CarryDev *Kp, int nsteps_env, vb200_packet_info *&dinfo, uint8_t *&dpk, int64_t data_cap,
+                     long long **total, const SpkResult *R = nullptr) {
+  int rc;
+  const int curves = managed ? VB200_PACKETBLOBS : 1;
+  const size_t n = (size_t)nstreams * d->max_blocks;
+  vb200_block_desc *desc[2] = {nullptr, nullptr};
+  const int32_t *d_tot = nullptr;
+  if ((rc = encode_streams_launch(c, nstreams, blobno, managed, d, st, desc, Kp, nsteps_env, R ? &d_tot : nullptr)))
+    return rc;
+  int32_t *bits[2] = {nullptr, nullptr}, *Wb, *sbits, *fbits, *choice = nullptr;
+  uint8_t *strided[2] = {nullptr, nullptr};
+  long long *off;
+  const bool own_info = !dinfo, own_data = !dpk;
+  if ((rc = carve(c->spk, [&](Carve &k) {
+         for (int w = 0; w < 2; w++) {
+           const size_t cnt = d->count[w];
+           if (!cnt) continue;
+           bits[w] = k.take<int32_t>(curves * cnt);
+           strided[w] = k.take<uint8_t>(curves * cnt * (size_t)c->eent.bound[w]);
+         }
+         Wb = k.take<int32_t>(n); sbits = k.take<int32_t>(n * curves); fbits = k.take<int32_t>(n);
+         if (managed) choice = k.take<int32_t>(n);
+         off = k.take<long long>(n + 1);
+         if (own_info) dinfo = k.take<vb200_packet_info>(n);
+         if (own_data) dpk = k.take<uint8_t>((size_t)std::max<int64_t>(data_cap, 1));
+       }))) return rc;
+  for (int w = 0; w < 2; w++) {
+    const int cnt = d->count[w];
+    if (!cnt) continue;
+    if ((rc = encode_entropy_dev(c, w, cnt, managed, managed ? d->cap[w] : 0, desc[w], d->posts[w], d->nonzero[w],
+                                 d->iwork[w], c->eent.bound[w], bits[w], strided[w], st))) return rc;
+  }
+  k_stream_bits<<<grid_for(c, (int)((n + 255) / 256), 8), 256, 0, st>>>(nstreams, d->max_blocks, d->plan, d->nblocks,
+                                                                        curves, bits[0], bits[1], d->count[0],
+                                                                        d->count[1], Wb, sbits, fbits);
+  if ((rc = post_launch(c))) return rc;
+  if (managed) {
+    k_bitrate_choose<<<(nstreams + 127) / 128, 128, 0, st>>>(c->br, nstreams, d->max_blocks, d->nblocks, Wb, sbits,
+                                                             Kp ? Kp->br : nullptr, choice, fbits, 8);
+    if ((rc = post_launch(c))) return rc;
+  }
+  k_packet_offsets<<<1, 1024, 0, st>>>(fbits, (int)n, off);
+  if ((rc = post_launch(c))) return rc;
+  if (R) {
+    k_pcm_result<<<1, 32, 0, st>>>(R->res, off + n, data_cap, d_tot, d->cap[0], d->cap[1], Kp->overflow, R->bad);
+    if ((rc = post_launch(c))) return rc;
+  }
+  GatherArgs A;
+  A.plan = d->plan; A.nblocks = d->nblocks; A.eof = d->eof; A.nstreams = nstreams; A.max_blocks = d->max_blocks;
+  A.curves = curves;
+  for (int w = 0; w < 2; w++) {
+    A.bs[w] = c->setup.blocksizes[w]; A.count[w] = d->count[w]; A.stride[w] = c->eent.bound[w]; A.data[w] = strided[w];
+  }
+  A.sbits = sbits; A.choice = choice; A.fbits = fbits; A.off = off; A.cap = data_cap; A.info = dinfo; A.dst = dpk;
+  A.rc = R ? &R->res->rc : nullptr;
+  if (Kp)
+    k_stream_gather_carry<<<grid_for(c, (int)n, 8), 256, 0, st>>>(A, Kp->pc);
+  else
+    k_stream_gather<<<grid_for(c, (int)n, 8), 256, 0, st>>>(A);
+  if ((rc = post_launch(c))) return rc;
+  *total = off + n;
+  return 0;
+}
+
+// Both whole-stream packet calls: the streams chain on staged device buffers (spk_chain).  One synchronous round
+// trip on s_main.  carry (host): the _resume forms, whose carries are staged as one more buffer and written back only
+// when the call succeeds.
 static int streams_packets(vb200_ctx *c, int nstreams, int blobno, bool managed, vb200_streams_io *h,
-                           vb200_packet_info *info, uint8_t *data, int64_t data_cap, void *carry = nullptr,
-                           HostIO *staged = nullptr) {
+                           vb200_packet_info *info, uint8_t *data, int64_t data_cap, void *carry = nullptr) {
   int rc;
   if ((rc = streams_open(c, h))) return rc;
   if (!c->eent.books) return fail(VB200_EINVAL, "no vb200_encode_entropy_setup registered");
@@ -4089,15 +4175,11 @@ static int streams_packets(vb200_ctx *c, int nstreams, int blobno, bool managed,
   CarryBlob hb{};
   int ccap = 0, nsteps_env = 0;
   if (carry && (rc = carry_pack(c, nstreams, managed, h, carry, cblob, hb, &ccap, &nsteps_env))) return rc;
-  std::unique_lock<std::mutex> lk(c->mu, std::defer_lock);
-  if (!staged) lk.lock();
-  cudaStream_t st = c->s_main;
-  const int curves = managed ? VB200_PACKETBLOBS : 1;
+  std::lock_guard<std::mutex> lk(c->mu);
   const size_t n = (size_t)nstreams * h->max_blocks;
-  HostIO own{c};
-  HostIO &io = staged ? *staged : own;
+  HostIO io{c};
   vb200_streams_io d;
-  streams_stage(c, io, nstreams, managed, !staged, h, &d);
+  streams_stage(c, io, nstreams, managed, true, h, &d);
   char *dblob = carry ? io.in(cblob.data(), cblob.size()) : nullptr;
   if (io.rc) return io.rc;
   CarryDev K{}, *Kp = nullptr;
@@ -4107,61 +4189,18 @@ static int streams_packets(vb200_ctx *c, int nstreams, int blobno, bool managed,
     K.first = dev(hb.first); K.count = dev(hb.count); K.overflow = dev(hb.overflow);
     Kp = &K;
   }
-  vb200_block_desc *desc[2] = {nullptr, nullptr};
-  rc = encode_streams_launch(c, nstreams, blobno, managed, &d, st, desc, Kp, nsteps_env);
+  vb200_packet_info *dinfo = nullptr;
+  uint8_t *dpk = nullptr;
+  long long *dtotal;
+  rc = spk_chain(c, nstreams, blobno, managed, &d, c->s_main, Kp, nsteps_env, dinfo, dpk, data_cap, &dtotal);
   h->count[0] = d.count[0]; h->count[1] = d.count[1];
   if (rc) return rc;
-  int32_t *bits[2] = {nullptr, nullptr}, *Wb, *sbits, *fbits, *choice = nullptr;
-  uint8_t *strided[2] = {nullptr, nullptr}, *dpk;
-  long long *off;
-  vb200_packet_info *dinfo;
-  if ((rc = carve(c->spk, [&](Carve &k) {
-         for (int w = 0; w < 2; w++) {
-           const size_t cnt = d.count[w];
-           if (!cnt) continue;
-           bits[w] = k.take<int32_t>(curves * cnt);
-           strided[w] = k.take<uint8_t>(curves * cnt * (size_t)c->eent.bound[w]);
-         }
-         Wb = k.take<int32_t>(n); sbits = k.take<int32_t>(n * curves); fbits = k.take<int32_t>(n);
-         if (managed) choice = k.take<int32_t>(n);
-         off = k.take<long long>(n + 1); dinfo = k.take<vb200_packet_info>(n);
-         dpk = k.take<uint8_t>((size_t)std::max<int64_t>(data_cap, 1));
-       }))) return rc;
-  for (int w = 0; w < 2; w++) {
-    const int cnt = d.count[w];
-    if (!cnt) continue;
-    if ((rc = encode_entropy_dev(c, w, cnt, managed, managed ? d.cap[w] : 0, desc[w], d.posts[w], d.nonzero[w],
-                                 d.iwork[w], c->eent.bound[w], bits[w], strided[w], st))) return rc;
-  }
-  k_stream_bits<<<grid_for(c, (int)((n + 255) / 256), 8), 256, 0, st>>>(nstreams, h->max_blocks, d.plan, d.nblocks, curves,
-                                                                        bits[0], bits[1], d.count[0], d.count[1], Wb,
-                                                                        sbits, fbits);
-  if ((rc = post_launch(c))) return rc;
-  if (managed) {
-    k_bitrate_choose<<<(nstreams + 127) / 128, 128, 0, st>>>(c->br, nstreams, h->max_blocks, d.nblocks, Wb, sbits,
-                                                             Kp ? K.br : nullptr, choice, fbits, 8);
-    if ((rc = post_launch(c))) return rc;
-  }
-  k_packet_offsets<<<1, 1024, 0, st>>>(fbits, (int)n, off);
-  if ((rc = post_launch(c))) return rc;
-  GatherArgs A;
-  A.plan = d.plan; A.nblocks = d.nblocks; A.eof = d.eof; A.nstreams = nstreams; A.max_blocks = h->max_blocks;
-  A.curves = curves;
-  for (int w = 0; w < 2; w++) {
-    A.bs[w] = c->setup.blocksizes[w]; A.count[w] = d.count[w]; A.stride[w] = c->eent.bound[w]; A.data[w] = strided[w];
-  }
-  A.sbits = sbits; A.choice = choice; A.fbits = fbits; A.off = off; A.cap = data_cap; A.info = dinfo; A.dst = dpk;
-  if (Kp)
-    k_stream_gather_carry<<<grid_for(c, (int)n, 8), 256, 0, st>>>(A, K.pc);
-  else
-    k_stream_gather<<<grid_for(c, (int)n, 8), 256, 0, st>>>(A);
-  if ((rc = post_launch(c))) return rc;
   long long total = 0;
   if (carry) io.back(cblob.data(), dblob, cblob.size());
   io.back(h->plan, d.plan, n);
   io.back(h->nblocks, d.nblocks, nstreams);
   io.back(info, dinfo, n);
-  io.back(&total, off + n, 1);
+  io.back(&total, dtotal, 1);
   if ((rc = io.sync())) return rc;
   if (total > data_cap) return fail(VB200_EINVAL, "packets exceed data_cap (info filled)");
   if (total) io.back(data, dpk, total);
@@ -4202,13 +4241,6 @@ extern "C" int vb200_encode_streams_packets_managed_resume(vb200_ctx *c, int nst
 // packets path.  The host carry of a stream is a PcmCarry, then the encode carry (carry_parts bytes), then the filters
 // of every channel (LPC_FILTER_FLOATS floats: the order-16 preamble coefficients and prime, the order-32 tail
 // coefficients and prime), each part 8-byte aligned.
-struct PcmCarry {
-  vb200_encode_carry enc;            // a copy of the encode carry's head, refreshed by every call (vb200_pcm_carry)
-  long long raw_base, written;
-  int ended, drained;
-  int pre_done;                      // v->preextrapolate: the preamble filter has been made
-  int ch, bs1, pad;
-};
 static_assert(offsetof(PcmCarry, raw_base) == offsetof(vb200_pcm_carry, raw_base) &&
               offsetof(PcmCarry, written) == offsetof(vb200_pcm_carry, written) &&
               offsetof(PcmCarry, ended) == offsetof(vb200_pcm_carry, ended) &&
@@ -4241,9 +4273,112 @@ extern "C" int vb200_encode_pcm_carry_init(vb200_ctx *c, int nstreams, int mark_
   return 0;
 }
 
-// Launches: k_lpc_filter<16> (the preamble filters due this call), k_pcm_timeline<false> (the timelines up to eof),
-// k_lpc_filter<32> (the tail filters due, which read those timelines), k_pcm_timeline<true> (the tails), then the
-// launches of the streams packets call on the timelines: four more than that call, whatever the stream count.
+// The device buffers of one raw-PCM call, and what the chain gives back
+struct PcmCall {
+  const void *pcm;
+  int s16, max_blocks, mark_cap, cap[2];
+  int64_t stride;
+  const int64_t *pcm_len, *first;        // first: null for the carries' raw_base
+  const int32_t *end;
+  unsigned char *carry;                  // [nstreams][vb200_encode_pcm_carry_bytes]
+  vb200_stream_block *plan;
+  int32_t *nblocks, *status;
+  vb200_packet_info *info;               // info and data: the caller's, or null for the spk arena's (returned)
+  uint8_t *data;
+  int64_t data_cap;
+  vb200_encode_result *res;              // the _dev forms: the result and the refusals on the device
+  int count[2];                          // out: the plan's totals
+  long long *total;                      // out: the byte total (device)
+  int32_t *bad;                          // out: some stream was refused (device)
+};
+
+// The raw-PCM chain of both forms on st.  Launches: k_pcm_pack, k_lpc_filter<16> (the preamble filters due this
+// call), k_pcm_timeline<false> (the timelines up to eof), k_lpc_filter<32> (the tail filters due, which read those
+// timelines), k_pcm_timeline<true> (the tails), the streams packets chain on the timelines ([k_pcm_result] for the
+// _dev forms), then k_pcm_unpack: six more than the _resume calls, whatever the stream count.  The timeline stride is
+// known from the input stride, so nothing here waits for the host; the streams chain waits once for its plan.
+static int pcm_chain(vb200_ctx *c, int nstreams, int blobno, bool managed, PcmCall &P, cudaStream_t st) {
+  int rc;
+  const int ch = c->setup.channels, bs1 = c->setup.blocksizes[1], half = bs1 / 2;
+  const CarryParts q = carry_parts(c, P.mark_cap);
+  const size_t sw = VB200_VE_STATE_WORDS(ch), curves = managed ? VB200_PACKETBLOBS : 1;
+  const long long tstride = (P.stride + half + 3LL * bs1 + 3) & ~3LL;     // the longest timeline a stream passes
+  const int nsteps = (int)(tstride / PLAN_STEP) - PLAN_VE_WIN;
+  PcmPackArgs A{};
+  vb200_streams_io d{};
+  float *dtl;
+  int32_t *flags;                        // the mark window overflow, then bad
+  if ((rc = carve(c->ptl, [&](Carve &k) {
+         dtl = k.take<float>((size_t)nstreams * ch * tstride);
+         A.ps = k.take<PcmStream>(nstreams); A.tl_len = k.take<int64_t>(nstreams); A.eof = k.take<int64_t>(nstreams);
+         A.jobs = k.take<LpcJob>(2 * (size_t)nstreams * ch);
+         A.filt = k.take<float>((size_t)nstreams * ch * LPC_FILTER_FLOATS);
+         A.head = k.take<PcmCarry>(nstreams); A.pc = k.take<PlanCarry>(nstreams);
+         A.mk = k.take<uint8_t>((size_t)nstreams * P.mark_cap); A.envs = k.take<int32_t>(nstreams * sw);
+         A.brs = k.take<vb200_bitrate_state>(nstreams);
+         A.first_step = k.take<int32_t>(nstreams); A.count = k.take<int32_t>(nstreams);
+         flags = k.take<int32_t>(2);
+         for (int w = 0; w < 2; w++) {
+           if (P.cap[w] <= 0) continue;
+           const size_t rows = curves * P.cap[w] * ch, n = c->dx[w].N / 2;
+           d.posts[w] = k.take<int32_t>(rows * VB200_FLOOR1_STRIDE); d.nonzero[w] = k.take<int32_t>(rows);
+           d.iwork[w] = k.take<int32_t>(rows * n); d.ampmax_out[w] = k.take<float>(P.cap[w]);
+         }
+       }))) return rc;
+  if ((rc = scratch_begin(c, st))) return rc;
+  CU(cudaMemsetAsync(dtl, 0, sizeof(float) * nstreams * ch * tstride, st));   // columns past a stream's len read as 0
+  CU(cudaMemsetAsync(flags, 0, 2 * sizeof(int32_t), st));
+  A.carry = P.carry; A.pb = (long long)(sizeof(PcmCarry) + q.bytes + pcm_filt_bytes(c));
+  A.marks = q.marks; A.env = q.env; A.br = q.br;
+  A.nstreams = nstreams; A.ch = ch; A.bs0 = c->setup.blocksizes[0]; A.bs1 = bs1; A.cap = P.mark_cap;
+  A.managed = managed; A.env_words = (int)sw;
+  A.pcm_len = P.pcm_len; A.first = P.first; A.end = P.end; A.in_stride = P.stride; A.tl_stride = tstride;
+  A.nsteps = nsteps; A.in = P.pcm; A.s16 = P.s16; A.tl = dtl; A.status = P.status; A.bad = flags + 1;
+  k_pcm_pack<<<(nstreams + 127) / 128, 128, 0, st>>>(A);
+  if ((rc = post_launch(c))) return rc;
+  PcmTimelineArgs T;
+  T.in = P.pcm; T.s16 = P.s16; T.ch = ch; T.half = half; T.in_stride = P.stride; T.tl_stride = tstride;
+  T.st = A.ps; T.filt = A.filt; T.tl = dtl; T.nstreams = nstreams;
+  const int pairs = nstreams * ch, lg = grid_for(c, (pairs + LPC_WARPS - 1) / LPC_WARPS, 8);
+  k_lpc_filter<LPC_PRE><<<lg, 32 * LPC_WARPS, 0, st>>>(A.jobs, pairs, 1);
+  if ((rc = post_launch(c))) return rc;
+  k_pcm_timeline<false><<<grid_for(c, pairs, 8), 256, 0, st>>>(T);
+  if ((rc = post_launch(c))) return rc;
+  k_lpc_filter<LPC_TAIL><<<lg, 32 * LPC_WARPS, 0, st>>>(A.jobs + pairs, pairs, 1);
+  if ((rc = post_launch(c))) return rc;
+  k_pcm_timeline<true><<<(pairs + 255) / 256, 256, 0, st>>>(T);
+  if ((rc = post_launch(c))) return rc;
+  d.pcm = dtl; d.pcm_fmt = VB200_PCM_F32_PLANAR; d.max_blocks = P.max_blocks; d.stream_stride = tstride;
+  d.pcm_len = A.tl_len; d.eof = A.eof; d.plan = P.plan; d.nblocks = P.nblocks;
+  d.cap[0] = P.cap[0]; d.cap[1] = P.cap[1];
+  CarryDev K;
+  K.pc = A.pc; K.marks = A.mk; K.cap = P.mark_cap; K.env = A.envs; K.br = A.brs; K.first = A.first_step;
+  K.count = A.count; K.overflow = flags;
+  const SpkResult R{P.res, A.bad};
+  P.bad = A.bad;
+  rc = spk_chain(c, nstreams, blobno, managed, &d, st, &K, nsteps, P.info, P.data, P.data_cap, &P.total,
+                 P.res ? &R : nullptr);
+  P.count[0] = d.count[0]; P.count[1] = d.count[1];
+  if (rc) return rc;
+  k_pcm_unpack<<<(nstreams + 127) / 128, 128, 0, st>>>(A, P.nblocks, P.max_blocks, P.res ? &P.res->rc : nullptr);
+  return post_launch(c);
+}
+
+// the checks both forms make on the host, in the host form's order after its own first ones
+static int pcm_call_check(vb200_ctx *c, int nstreams, int blobno, bool managed, const vb200_pcm_io *h,
+                          const void *info, const uint8_t *data, int64_t data_cap) {
+  int rc;
+  if ((rc = plan_check(c))) return rc;
+  if (!c->eent.books) return fail(VB200_EINVAL, "no vb200_encode_entropy_setup registered");
+  if (managed && (rc = bitrate_check(c))) return rc;
+  if (!managed && (blobno < 0 || blobno >= VB200_PACKETBLOBS)) return fail(VB200_EINVAL, "blobno");
+  if (!h->plan || !h->nblocks) return fail(VB200_EINVAL, "encode_streams_packets: pcm, pcm_len, plan, nblocks");
+  if (h->cap[0] < 0 || h->cap[1] < 0) return fail(VB200_EINVAL, "cap");
+  if (!info || (!data && data_cap > 0) || data_cap < 0) return fail(VB200_EINVAL, "encode_streams_packets outputs");
+  if ((int64_t)nstreams * h->max_blocks > INT32_MAX / VB200_PACKETBLOBS) return fail(VB200_EINVAL, "nstreams x max_blocks");
+  return cqn_channels_check(c);
+}
+
 static int pcm_packets(vb200_ctx *c, int nstreams, int blobno, bool managed, vb200_pcm_io *h, void *carry,
                        vb200_packet_info *info, uint8_t *data, int64_t data_cap) {
   int rc;
@@ -4253,27 +4388,17 @@ static int pcm_packets(vb200_ctx *c, int nstreams, int blobno, bool managed, vb2
   if (nstreams <= 0) return 0;
   if (!carry) return fail(VB200_EINVAL, "null carry");
   if (!h->pcm || !h->pcm_len || h->stream_stride < 0 || h->max_blocks < 1) return fail(VB200_EINVAL, "encode_pcm_packets: pcm, pcm_len, stride, max_blocks");
-  const int ch = c->setup.channels, bs1 = c->setup.blocksizes[1], half = bs1 / 2;
+  const int ch = c->setup.channels, bs1 = c->setup.blocksizes[1];
   PcmCarry p0;
   memcpy(&p0, carry, sizeof(p0));
   if (p0.ch != ch || p0.bs1 != bs1) return fail(VB200_EINVAL, "pcm carry of another setup");
   const int mark_cap = ((const PlanCarry *)((const char *)carry + sizeof(PcmCarry)))->mark_cap;
-  const size_t eb = carry_parts(c, mark_cap).bytes, fb = pcm_filt_bytes(c), pb = sizeof(PcmCarry) + eb + fb;
-  // the write of every stream, as vorbis_analysis_wrote would take it
-  std::vector<PcmCarry> pc(nstreams);
-  std::vector<PcmStream> ps(nstreams);
-  std::vector<int64_t> tl_len(nstreams), eof(nstreams);
-  std::vector<char> enc((size_t)nstreams * eb);
-  std::vector<int> pre_due(nstreams), tail_due(nstreams);
-  // the streams path wants a stride of at least blocksizes[1], a multiple of 4 for float PCM
-  long long tstride = bs1, njobs = 0;
+  const size_t pb = sizeof(PcmCarry) + carry_parts(c, mark_cap).bytes + pcm_filt_bytes(c);
+  // the refusals k_pcm_pack reports on the device, here with their messages (keep the two in step)
   for (int s = 0; s < nstreams; s++) {
     const char *cs = (const char *)carry + (size_t)s * pb;
-    PcmCarry &p = pc[s];
+    PcmCarry p;
     memcpy(&p, cs, sizeof(p));
-    memcpy(enc.data() + (size_t)s * eb, cs + sizeof(PcmCarry), eb);
-    PlanCarry q;
-    memcpy(&q, cs + sizeof(PcmCarry), sizeof(q));
     if (p.ch != ch || p.bs1 != bs1) return fail(VB200_EINVAL, "pcm carries of different setups");
     const int64_t kept = p.written - p.raw_base, fresh = h->pcm_len[s] - kept;
     const bool end = h->end && h->end[s];
@@ -4283,107 +4408,48 @@ static int pcm_packets(vb200_ctx *c, int nstreams, int blobno, bool managed, vb2
     if (end && p.ended) return fail(VB200_EINVAL, "a second end");
     if (end && fresh) return fail(VB200_EINVAL, "an end call with new samples (end is vorbis_analysis_wrote(v, 0))");
     if (end && !p.drained) return fail(VB200_EINVAL, "an end call on a carry max_blocks left undrained");
-    p.written += fresh;
-    // lib/block.c:525 and :480 (pcm_current - centerW is the samples written until the preamble exists)
-    pre_due[s] = !p.pre_done && (p.written > bs1 || end);
-    tail_due[s] = end;
-    p.pre_done |= pre_due[s];
-    p.ended |= end;
-    PcmStream &t = ps[s];
-    t.base = q.base; t.raw_base = p.raw_base;
-    t.eof = p.ended ? half + p.written : 0;
-    t.len = q.done || !p.pre_done ? 0 : (p.ended ? t.eof + 3LL * bs1 : half + p.written) - q.base;
-    tl_len[s] = t.len; eof[s] = t.eof;
-    tstride = std::max(tstride, t.len);
-    njobs += (pre_due[s] + tail_due[s]) * ch;
   }
-  tstride = (tstride + 3) & ~3LL;
+  if ((rc = pcm_call_check(c, nstreams, blobno, managed, h, info, data, data_cap))) return rc;
+  for (int s = 0; s < nstreams; s++) {
+    PlanCarry q;
+    memcpy(&q, (const char *)carry + (size_t)s * pb + sizeof(PcmCarry), sizeof(q));
+    if (q.ch != ch || q.bs0 != c->setup.blocksizes[0] || q.bs1 != bs1 || q.mark_cap != mark_cap || mark_cap < 1)
+      return fail(VB200_EINVAL, "encode carries of different setups or mark capacities");
+    if (managed && !q.br_ready)
+      return fail(VB200_EINVAL, "encode carry made before a managed vb200_bitrate_setup (no bitrate state)");
+  }
   std::lock_guard<std::mutex> lk(c->mu);
-  cudaStream_t st = c->s_main;
-  const bool s16 = h->pcm_fmt == VB200_PCM_S16_INTERLEAVED;
+  const size_t n = (size_t)nstreams * h->max_blocks;
   HostIO io{c};
-  const size_t in_bytes = (size_t)nstreams * ch * (size_t)h->stream_stride * (s16 ? 2 : 4);
-  const void *din = io.in(in_bytes ? h->pcm : nullptr, std::max<size_t>(in_bytes, 1));
-  // one staged buffer: the streams, the jobs (preamble jobs first) and the filters of every (stream, channel)
-  PcmStream *bs; LpcJob *bj; float *bf;
-  auto layout = [&](Carve &k) {
-    bs = k.take<PcmStream>(nstreams); bj = k.take<LpcJob>((size_t)std::max(njobs, 1LL));
-    bf = k.take<float>((size_t)nstreams * ch * LPC_FILTER_FLOATS);
-  };
-  Carve sz{nullptr, 0};
-  layout(sz);
-  std::vector<char> blob(sz.off);
-  Carve at{blob.data(), 0};
-  layout(at);
-  char *dblob = io.out<char>(blob.size());
+  PcmCall P{};
+  P.s16 = h->pcm_fmt == VB200_PCM_S16_INTERLEAVED;
+  const size_t in_bytes = (size_t)nstreams * ch * (size_t)h->stream_stride * (P.s16 ? 2 : 4);
+  P.pcm = io.in(in_bytes ? h->pcm : nullptr, std::max<size_t>(in_bytes, 1));
+  P.max_blocks = h->max_blocks; P.mark_cap = mark_cap; P.cap[0] = h->cap[0]; P.cap[1] = h->cap[1];
+  P.stride = h->stream_stride;
+  P.pcm_len = io.in(h->pcm_len, nstreams);
+  P.end = h->end ? io.in(h->end, nstreams) : nullptr;
+  P.carry = (unsigned char *)io.in((const char *)carry, nstreams * pb);
+  P.plan = io.out<vb200_stream_block>(n); P.nblocks = io.out<int32_t>(nstreams); P.status = io.out<int32_t>(nstreams);
+  P.data_cap = data_cap;
   if (io.rc) return io.rc;
-  float *dtl;
-  if ((rc = carve(c->ptl, [&](Carve &k) { dtl = k.take<float>((size_t)nstreams * ch * tstride); }))) return rc;
-  CU(cudaMemsetAsync(dtl, 0, sizeof(float) * nstreams * ch * tstride, st));   // columns past a stream's len read as 0
-  auto dev = [&](auto *hp) { return (decltype(hp))(dblob + ((char *)hp - blob.data())); };
-  const long long stride = h->stream_stride;
-  int npre = 0, nj = 0;
-  for (int pass = 0; pass < 2; pass++)
-    for (int s = 0; s < nstreams; s++) {
-      if (!(pass ? tail_due[s] : pre_due[s])) continue;
-      const PcmStream &t = ps[s];
-      for (int k = 0; k < ch; k++) {
-        LpcJob &J = bj[nj++];
-        const long long q = (long long)s * ch + k;
-        float *f = dev(bf) + q * LPC_FILTER_FLOATS + (pass ? 2 * LPC_PRE : 0);
-        J.coef = f; J.prime = f + (pass ? LPC_TAIL : LPC_PRE);
-        if (!pass) {
-          // _preextrapolate_helper: the input [0, P) time-reversed (raw_base is 0 before the preamble exists)
-          const long long P = pc[s].written;
-          J.src = din; J.s16 = s16; J.n = P;
-          J.off = s16 ? ((long long)s * stride + P - 1) * ch + k : q * stride + P - 1;
-          J.step = s16 ? -ch : -1;
-        } else {
-          // vorbis_analysis_wrote(v, 0): timeline [eof - n, eof), n = min(eof - base, blocksizes[1])
-          const long long n = std::min<long long>(t.eof - t.base, bs1);
-          J.src = dtl; J.s16 = 0; J.n = n; J.off = q * tstride + t.eof - n - t.base; J.step = 1;
-        }
-      }
-      if (!pass) npre = nj;
-    }
-  for (int s = 0; s < nstreams; s++) {
-    bs[s] = ps[s];
-    memcpy(bf + (size_t)s * ch * LPC_FILTER_FLOATS, (const char *)carry + (size_t)s * pb + sizeof(PcmCarry) + eb, fb);
-  }
-  CU(cudaMemcpyAsync(dblob, blob.data(), blob.size(), cudaMemcpyHostToDevice, st));
-  PcmTimelineArgs A;
-  A.in = din; A.s16 = s16; A.ch = ch; A.half = half; A.in_stride = stride; A.tl_stride = tstride;
-  A.st = dev(bs); A.filt = dev(bf); A.tl = dtl; A.nstreams = nstreams;
-  const int pairs = nstreams * ch;
-  k_lpc_filter<LPC_PRE><<<grid_for(c, (npre + LPC_WARPS - 1) / LPC_WARPS, 8), 32 * LPC_WARPS, 0, st>>>(dev(bj), npre, 1);
-  if ((rc = post_launch(c))) return rc;
-  k_pcm_timeline<false><<<grid_for(c, pairs, 8), 256, 0, st>>>(A);
-  if ((rc = post_launch(c))) return rc;
-  k_lpc_filter<LPC_TAIL><<<grid_for(c, (nj - npre + LPC_WARPS - 1) / LPC_WARPS, 8), 32 * LPC_WARPS, 0, st>>>(
-      dev(bj) + npre, nj - npre, 1);
-  if ((rc = post_launch(c))) return rc;
-  k_pcm_timeline<true><<<(pairs + 255) / 256, 256, 0, st>>>(A);
-  if ((rc = post_launch(c))) return rc;
-  vb200_streams_io d{};
-  d.pcm = dtl; d.pcm_fmt = VB200_PCM_F32_PLANAR; d.max_blocks = h->max_blocks; d.stream_stride = tstride;
-  d.pcm_len = tl_len.data(); d.eof = eof.data(); d.plan = h->plan; d.nblocks = h->nblocks;
-  d.cap[0] = h->cap[0]; d.cap[1] = h->cap[1];
-  rc = streams_packets(c, nstreams, blobno, managed, &d, info, data, data_cap, enc.data(), &io);
-  h->count[0] = d.count[0]; h->count[1] = d.count[1];
+  rc = pcm_chain(c, nstreams, blobno, managed, P, c->s_main);
+  h->count[0] = P.count[0]; h->count[1] = P.count[1];
   if (rc) return rc;
-  io.back(bf, dev(bf), (size_t)nstreams * ch * LPC_FILTER_FLOATS);
+  if ((rc = scratch_end(c, c->s_main))) return rc;
+  long long total = 0;
+  int bad = 0;
+  io.back(h->plan, P.plan, n);
+  io.back(h->nblocks, P.nblocks, nstreams);
+  io.back(info, P.info, n);
+  io.back(&total, P.total, 1);
+  io.back(&bad, P.bad, 1);
   if ((rc = io.sync())) return rc;
-  for (int s = 0; s < nstreams; s++) {
-    char *cs = (char *)carry + (size_t)s * pb;
-    PcmCarry &p = pc[s];
-    memcpy(&p.enc, enc.data() + (size_t)s * eb, sizeof(p.enc));
-    p.raw_base = std::max<long long>(0, p.enc.base - half);
-    p.drained = h->nblocks[s] < h->max_blocks;
-    memcpy(cs, &p, sizeof(p));
-    memcpy(cs + sizeof(PcmCarry), enc.data() + (size_t)s * eb, eb);
-    memcpy(cs + sizeof(PcmCarry) + eb, bf + (size_t)s * ch * LPC_FILTER_FLOATS, fb);
-  }
-  return 0;
+  if (bad) return fail(VB200_EINVAL, "pcm carry inconsistent with its encode carry");
+  if (total > data_cap) return fail(VB200_EINVAL, "packets exceed data_cap (info filled)");
+  if (total) io.back(data, P.data, total);
+  io.back((char *)carry, (const char *)P.carry, nstreams * pb);
+  return io.sync();
 }
 
 extern "C" int vb200_encode_pcm_packets(vb200_ctx *c, int nstreams, int blobno, vb200_pcm_io *io, void *carry,
@@ -4396,6 +4462,45 @@ extern "C" int vb200_encode_pcm_packets_managed(vb200_ctx *c, int nstreams, vb20
                                                 vb200_packet_info *info, uint8_t *data, int64_t data_cap) {
   CHECK_CTX(c);
   return pcm_packets(c, nstreams, 0, true, io, carry, info, data, data_cap);
+}
+
+static int pcm_packets_dev(vb200_ctx *c, int nstreams, int blobno, bool managed, int mark_steps, const vb200_pcm_io *h,
+                           const int64_t *d_first, void *d_carry, vb200_packet_info *d_info, uint8_t *d_data,
+                           int64_t data_cap, int32_t *d_status, vb200_encode_result *d_result, void *stream) {
+  int rc;
+  if (!h) return fail(VB200_EINVAL, "null io");
+  if (h->pcm_fmt != VB200_PCM_F32_PLANAR && h->pcm_fmt != VB200_PCM_S16_INTERLEAVED) return fail(VB200_EINVAL, "pcm format");
+  if (nstreams <= 0) return 0;
+  if (!h->pcm || !h->pcm_len || h->stream_stride < 0 || h->max_blocks < 1) return fail(VB200_EINVAL, "encode_pcm_packets: pcm, pcm_len, stride, max_blocks");
+  if (!d_carry || !d_status || !d_result) return fail(VB200_EINVAL, "encode_pcm_packets_dev: carry, status, result");
+  if ((rc = pcm_call_check(c, nstreams, blobno, managed, h, d_info, d_data, data_cap))) return rc;
+  const cudaStream_t st = (cudaStream_t)stream;
+  PcmCall P{};
+  P.pcm = h->pcm; P.s16 = h->pcm_fmt == VB200_PCM_S16_INTERLEAVED; P.max_blocks = h->max_blocks;
+  P.mark_cap = carry_cap(c, mark_steps); P.cap[0] = h->cap[0]; P.cap[1] = h->cap[1]; P.stride = h->stream_stride;
+  P.pcm_len = h->pcm_len; P.first = d_first; P.end = h->end; P.carry = (unsigned char *)d_carry;
+  P.plan = h->plan; P.nblocks = h->nblocks; P.status = d_status; P.info = d_info; P.data = d_data;
+  P.data_cap = data_cap; P.res = d_result;
+  if ((rc = pcm_chain(c, nstreams, blobno, managed, P, st))) return rc;
+  return scratch_end(c, st);
+}
+
+extern "C" int vb200_encode_pcm_packets_dev(vb200_ctx *c, int nstreams, int blobno, int mark_steps,
+                                            const vb200_pcm_io *d_io, const int64_t *d_first, void *d_carry,
+                                            vb200_packet_info *d_info, uint8_t *d_data, int64_t data_cap,
+                                            int32_t *d_status, vb200_encode_result *d_result, void *stream) {
+  CHECK_CTX(c);
+  return pcm_packets_dev(c, nstreams, blobno, false, mark_steps, d_io, d_first, d_carry, d_info, d_data, data_cap,
+                         d_status, d_result, stream);
+}
+
+extern "C" int vb200_encode_pcm_packets_managed_dev(vb200_ctx *c, int nstreams, int mark_steps,
+                                                    const vb200_pcm_io *d_io, const int64_t *d_first, void *d_carry,
+                                                    vb200_packet_info *d_info, uint8_t *d_data, int64_t data_cap,
+                                                    int32_t *d_status, vb200_encode_result *d_result, void *stream) {
+  CHECK_CTX(c);
+  return pcm_packets_dev(c, nstreams, 0, true, mark_steps, d_io, d_first, d_carry, d_info, d_data, data_cap, d_status,
+                         d_result, stream);
 }
 
 extern "C" int vb200_lpc_extrapolate(vb200_ctx *c, int nrows, int order, const float *data, int64_t data_stride,

@@ -148,7 +148,7 @@ k_bitrate_choose(BitrateDev B, int nstreams, int max_blocks, const int32_t *__re
 
 // Block k of stream s (entry t = s*max_blocks + k): W[t] and, for every curve c, sbits[t*curves + c] =
 // bits_W[c*count[W] + slot].  fbits[t] = 0 past nblocks[s]; with one curve (un-managed) fbits[t] is that packet's
-// bit count, with VB200_PACKETBLOBS the chooser fills it.
+// bit count, with VB200_PACKETBLOBS the chooser fills it.  A slot at or past count[W] reads as 0 bits.
 __global__ void __launch_bounds__(256)
 k_stream_bits(int nstreams, int max_blocks, const vb200_stream_block *__restrict__ plan,
               const int32_t *__restrict__ nblocks, int curves, const int32_t *__restrict__ bits0,
@@ -162,6 +162,11 @@ k_stream_bits(int nstreams, int max_blocks, const vb200_stream_block *__restrict
     const int32_t *b = W ? bits1 : bits0;
     const long long cnt = W ? count1 : count0;
     Wb[t] = W;
+    if (slot >= cnt) {                  // a _dev call whose plan outgrew cap[] (refused): no bits to read
+      for (int c = 0; c < curves; c++) sbits[t * curves + c] = 0;
+      fbits[t] = 0;
+      continue;
+    }
     for (int c = 0; c < curves; c++) sbits[t * curves + c] = b[c * cnt + slot];
     if (curves == 1) fbits[t] = b[slot];
   }
@@ -182,6 +187,7 @@ struct GatherArgs {
   long long cap;
   vb200_packet_info *info;
   uint8_t *dst;
+  const int32_t *rc;                // or nullptr: the bytes are written only when *rc is 0 (the _dev raw-PCM calls)
 };
 
 // one CTA per block in a grid-stride loop; info is always written, the bytes only when all of them fit cap.
@@ -190,7 +196,7 @@ struct GatherArgs {
 template <bool CARRY>
 __device__ __forceinline__ void stream_gather_body(const GatherArgs &A, PlanCarry *pc) {
   const long long total = (long long)A.nstreams * A.max_blocks;
-  const bool fits = A.off[total] <= A.cap;
+  const bool fits = A.off[total] <= A.cap && !(A.rc && *A.rc);
   for (long long t = blockIdx.x; t < total; t += gridDim.x) {
     const int s = (int)(t / A.max_blocks), k = (int)(t - (long long)s * A.max_blocks);
     const long long o = A.off[t];

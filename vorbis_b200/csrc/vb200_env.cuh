@@ -57,6 +57,9 @@ __device__ __forceinline__ void env_spectrum_body(const EnvDev &E, const EnvSrc 
       store = valid && first_step + j < count_ps[sst];
       s0 = store ? (long)ENV_STEP * (first_ps[sst] + first_step + j) : 0;
     }
+    // a stride-bounded step range (the raw-PCM calls): a CTA whose warps all lie past their streams' counts has
+    // nothing to compute
+    if (VAR && !__syncthreads_or(store)) continue;
     if (src.fmt == VB200_PCM_S16_INTERLEAVED) {
       const long st = sc / src.ch; const int c = (int)(sc - st * src.ch);
       const short *p = reinterpret_cast<const short *>(src.base) + ((long long)st * src.stride + s0) * src.ch + c;

@@ -46,6 +46,7 @@ __global__ void __launch_bounds__(32 * LPC_WARPS) k_lpc_filter(const LpcJob *__r
   for (int j = blockIdx.x * LPC_WARPS + wid; j < njobs; j += gridDim.x * LPC_WARPS) {
     const LpcJob J = jobs[j];
     const long long n = J.n;
+    if (n < 0) continue;                                  // a slot with no job this call
     if (guard && n <= 2 * M) {
       if (lane < M) { J.coef[lane] = 0.f; J.prime[lane] = 0.f; }
       continue;

@@ -259,15 +259,32 @@ k_plan_fill(int nstreams, int max_blocks, vb200_stream_block *__restrict__ plan,
   }
 }
 
+// The _dev raw-PCM calls size every launch after the plan by cap[W] without waiting for the totals: the slots the
+// plan leaves empty, [totals[W], cap[W]), become a valid block (stream 0 at position 0, a plain long or impulse block)
+// whose results nothing reads.  blockIdx.y = W.
+__global__ void __launch_bounds__(256)
+k_plan_pad(const int32_t *__restrict__ totals, int cap0, int cap1, int2 *__restrict__ src0, int2 *__restrict__ src1,
+           vb200_block_desc *__restrict__ desc0, vb200_block_desc *__restrict__ desc1) {
+  const int W = blockIdx.y, cap = W ? cap1 : cap0;
+  for (int slot = totals[W] + blockIdx.x * blockDim.x + threadIdx.x; slot < cap; slot += gridDim.x * blockDim.x) {
+    vb200_block_desc d;
+    d.lW = W; d.nW = W; d.blocktype = W; d.ampmax = 0.f;
+    (W ? src1 : src0)[slot] = make_int2(0, 0);
+    (W ? desc1 : desc0)[slot] = d;
+  }
+}
+
 // every block's global_ampmax: the decay chain of vorbis_analysis_blockout along the stream
 // (lib/block.c:626-628: g = max(g, previous block's ampmax on exit); g = _vp_ampmax_decay(g) with the CURRENT
-// block's size, lib/psy.c:837-848), then the block's own local maxima (lib/mapping0.c:244,346)
+// block's size, lib/psy.c:837-848), then the block's own local maxima (lib/mapping0.c:244,346).  Slots at or past
+// cap[W] (a _dev call whose plan outgrew cap[], refused later) are not read or written.
 template <bool CARRY>
 __device__ __forceinline__ void ampmax_plan_body(int nstreams, int max_blocks, int ch,
                                                  const vb200_stream_block *__restrict__ plan,
                                                  const int32_t *__restrict__ nblocks, const float *__restrict__ lmax0,
                                                  const float *__restrict__ lmax1, float secs_att0, float secs_att1,
-                                                 float *__restrict__ gmax0, float *__restrict__ gmax1, PlanCarry *pc) {
+                                                 float *__restrict__ gmax0, float *__restrict__ gmax1, int cap0,
+                                                 int cap1, PlanCarry *pc) {
   const int st = blockIdx.x * blockDim.x + threadIdx.x;
   if (st >= nstreams) return;
   const vb200_stream_block *p = plan + (size_t)st * max_blocks;
@@ -280,9 +297,11 @@ __device__ __forceinline__ void ampmax_plan_body(int nstreams, int max_blocks, i
     g = g + (W ? secs_att1 : secs_att0);
     if (g < -9999.f) g = -9999.f;
     float o = g;
-    const float *lm = (W ? lmax1 : lmax0) + (size_t)slot * ch;
-    for (int c = 0; c < ch; c++) o = fmaxf(o, lm[c]);
-    (W ? gmax1 : gmax0)[slot] = o;
+    if (slot < (W ? cap1 : cap0)) {
+      const float *lm = (W ? lmax1 : lmax0) + (size_t)slot * ch;
+      for (int c = 0; c < ch; c++) o = fmaxf(o, lm[c]);
+      (W ? gmax1 : gmax0)[slot] = o;
+    }
     prev = o;
   }
   if (CARRY) { pc[st].gmax = g; pc[st].prev = prev; }
@@ -291,9 +310,10 @@ __device__ __forceinline__ void ampmax_plan_body(int nstreams, int max_blocks, i
 __global__ void __launch_bounds__(128)
 k_ampmax_plan(int nstreams, int max_blocks, int ch, const vb200_stream_block *__restrict__ plan,
               const int32_t *__restrict__ nblocks, const float *__restrict__ lmax0, const float *__restrict__ lmax1,
-              float secs_att0, float secs_att1, float *__restrict__ gmax0, float *__restrict__ gmax1) {
+              float secs_att0, float secs_att1, float *__restrict__ gmax0, float *__restrict__ gmax1, int cap0,
+              int cap1) {
   ampmax_plan_body<false>(nstreams, max_blocks, ch, plan, nblocks, lmax0, lmax1, secs_att0, secs_att1, gmax0, gmax1,
-                          nullptr);
+                          cap0, cap1, nullptr);
 }
 
 // g and prev start from the carry and go back to it
@@ -301,8 +321,9 @@ __global__ void __launch_bounds__(128)
 k_ampmax_plan_carry(int nstreams, int max_blocks, int ch, const vb200_stream_block *__restrict__ plan,
                     const int32_t *__restrict__ nblocks, const float *__restrict__ lmax0, const float *__restrict__ lmax1,
                     float secs_att0, float secs_att1, float *__restrict__ gmax0, float *__restrict__ gmax1,
-                    PlanCarry *__restrict__ pc) {
-  ampmax_plan_body<true>(nstreams, max_blocks, ch, plan, nblocks, lmax0, lmax1, secs_att0, secs_att1, gmax0, gmax1, pc);
+                    int cap0, int cap1, PlanCarry *__restrict__ pc) {
+  ampmax_plan_body<true>(nstreams, max_blocks, ch, plan, nblocks, lmax0, lmax1, secs_att0, secs_att1, gmax0, gmax1,
+                         cap0, cap1, pc);
 }
 
 }  // namespace vb200

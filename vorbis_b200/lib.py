@@ -50,7 +50,8 @@ EXPORTS = [
     "vb200_encode_carry_bytes", "vb200_encode_carry_init", "vb200_encode_streams_packets_resume",
     "vb200_encode_streams_packets_managed_resume",
     "vb200_encode_pcm_carry_bytes", "vb200_encode_pcm_carry_init", "vb200_encode_pcm_packets",
-    "vb200_encode_pcm_packets_managed", "vb200_lpc_extrapolate",
+    "vb200_encode_pcm_packets_managed", "vb200_encode_pcm_packets_dev", "vb200_encode_pcm_packets_managed_dev",
+    "vb200_lpc_extrapolate",
     "vb200_ogg_demux_dev", "vb200_ogg_demux", "vb200_ogg_links_dev", "vb200_ogg_links", "vb200_vorbis_window",
     "vb200_vorbis_headers_parse", "vb200_vorbis_headers_free",
     "vb200_ogg_group_scratch_bytes", "vb200_ogg_group_dev", "vb200_ogg_group",
@@ -185,6 +186,10 @@ def load():
     L.vb200_encode_pcm_carry_init.argtypes = [vp, C.c_int, C.c_int, vp]
     L.vb200_encode_pcm_packets.argtypes = [vp, C.c_int, C.c_int, C.POINTER(abi.PcmIO), vp, vp, vp, C.c_int64]
     L.vb200_encode_pcm_packets_managed.argtypes = [vp, C.c_int, C.POINTER(abi.PcmIO), vp, vp, vp, C.c_int64]
+    L.vb200_encode_pcm_packets_dev.argtypes = [vp, C.c_int, C.c_int, C.c_int, C.POINTER(abi.PcmIO), vp, vp, vp, vp,
+                                               C.c_int64, vp, vp, vp]
+    L.vb200_encode_pcm_packets_managed_dev.argtypes = [vp, C.c_int, C.c_int, C.POINTER(abi.PcmIO), vp, vp, vp, vp,
+                                                       C.c_int64, vp, vp, vp]
     L.vb200_lpc_extrapolate.argtypes = [vp, C.c_int, C.c_int, vp, C.c_int64, vp, C.c_int32, vp, vp, C.c_int64]
     L.vb200_ogg_demux_dev.argtypes = [C.c_int, vp, vp, C.c_int, vp, vp, vp, vp, vp]
     L.vb200_ogg_demux.argtypes = [C.c_int, vp, vp, C.c_int, vp, vp, vp, vp]
@@ -1079,6 +1084,25 @@ class Context:
             rc = self.L.vb200_encode_pcm_packets(self.h, ns, blobno, C.byref(io), _ptr(carry), _ptr(info), _ptr(data),
                                                  data_cap)
         return self._stream_packets(rc, check, io, plan, nb, info, data)
+
+    def encode_pcm_packets_dev(self, nstreams, d_pcm, pcm_fmt, stream_stride, d_pcm_len, d_carry, d_plan, d_nblocks,
+                               max_blocks, cap, d_info, d_data, data_cap, d_status, d_result, d_end=None, d_first=None,
+                               mark_steps=0, managed=False, blobno=7, stream=None, check=True):
+        """vb200_encode_pcm_packets[_managed]_dev: d_ arguments are device addresses (ints, e.g. data_ptr());
+        the call's outcome is in d_status and d_result (abi.ENCODE_RESULT_DTYPE).  Returns the synchronous status."""
+        io = abi.PcmIO()
+        io.pcm, io.pcm_fmt, io.max_blocks, io.stream_stride = _ptr(d_pcm), pcm_fmt, max_blocks, stream_stride
+        io.pcm_len, io.end, io.plan, io.nblocks = _ptr(d_pcm_len), _ptr(d_end), _ptr(d_plan), _ptr(d_nblocks)
+        io.cap[0], io.cap[1] = int(cap[0]), int(cap[1])
+        args = (_ptr(d_first), _ptr(d_carry), _ptr(d_info), _ptr(d_data), data_cap, _ptr(d_status), _ptr(d_result),
+                _ptr(stream))
+        if managed:
+            rc = self.L.vb200_encode_pcm_packets_managed_dev(self.h, nstreams, mark_steps, C.byref(io), *args)
+        else:
+            rc = self.L.vb200_encode_pcm_packets_dev(self.h, nstreams, blobno, mark_steps, C.byref(io), *args)
+        if check:
+            self._chk(rc)
+        return rc
 
     def lpc_extrapolate(self, data, n, order, count, check=True):
         """vb200_lpc_extrapolate: data float32 [rows][stride], n [rows]; returns (coeff float32 [rows][order], out
