@@ -126,7 +126,9 @@ typedef struct vb200_setup {
   int32_t coupling_prepointamp[VB200_PACKETBLOBS];
   int32_t coupling_postpointamp[VB200_PACKETBLOBS];
   int32_t sliding_lowpass[2][VB200_PACKETBLOBS];
-  /* vorbis_info_mapping0 coupling (lib/backends.h:127-141), per W           */
+  /* vorbis_info_mapping0 coupling (lib/backends.h:127-141), per W.  vb200_ctx_create refuses with
+   * VB200_EINVAL the maps mapping0_unpack refuses (lib/mapping0.c:110-118): an index outside
+   * [0, channels), or mag == ang                                            */
   int32_t coupling_steps[2];
   int32_t coupling_mag[2][VB200_MAX_COUPLING];
   int32_t coupling_ang[2][VB200_MAX_COUPLING];

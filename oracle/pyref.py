@@ -26,6 +26,12 @@ def available():
     return os.path.exists(LIB_PATH)
 
 
+def coupling_hooks_available():
+    """whether the built library has ref_set_coupling and ref_get_headers (Ref.set_coupling, Ref.headers); a library
+    built from an older ref_driver.c has neither, and every other entry point still works"""
+    return available() and all(hasattr(lib(), k) for k in ("ref_set_coupling", "ref_get_headers"))
+
+
 class Capture(C.Structure):
     _fields_ = [
         ("maxblocks", C.c_int), ("Nmax", C.c_int), ("nblocks", C.c_int),
@@ -73,6 +79,8 @@ def _declare(L):
     L.ref_vd.argtypes = [C.c_void_p]
     L.ref_blocksize.argtypes = [C.c_void_p, C.c_int]
     L.ref_get_packets.argtypes = [C.c_void_p, C.c_void_p, C.c_long, C.c_void_p, C.c_int]
+    if hasattr(L, "ref_get_headers"):
+        L.ref_get_headers.argtypes = [C.c_void_p, C.c_void_p, C.c_long, C.c_void_p]
     L.ref_encode_capture.argtypes = [C.c_void_p, f32p, C.c_long, C.POINTER(Capture), C.POINTER(C.c_long)]
     L.ref_decode_capture.restype = C.c_long
     L.ref_decode_capture.argtypes = [C.c_void_p, C.POINTER(Capture), f32p, C.c_long, C.c_void_p]
@@ -90,6 +98,8 @@ def lib():
         L.ref_close.argtypes = [C.c_void_p]
         L.ref_blocksize.argtypes = [C.c_void_p, C.c_int]
         L.ref_get_setup.argtypes = [C.c_void_p, C.POINTER(abi.Setup)]
+        if hasattr(L, "ref_set_coupling"):
+            L.ref_set_coupling.argtypes = [C.c_void_p, C.c_int, C.c_int, i32p, i32p]
         L.ref_get_table.argtypes = [C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_int]
         L.ref_mdct_forward.argtypes = [C.c_void_p, C.c_int, C.c_int, f32p, f32p]
         L.ref_mdct_backward.argtypes = [C.c_void_p, C.c_int, C.c_int, f32p, f32p]
@@ -158,6 +168,19 @@ class Ref:
             off += sizes[i]
         return out
 
+    def headers(self):
+        """the identification, comment and setup header packets encode_capture wrote (list of 3 bytes objects)"""
+        cap = 1 << 20
+        buf = (C.c_ubyte * cap)()
+        sizes = (C.c_long * 3)()
+        if self.L.ref_get_headers(self.h, buf, cap, sizes) != 3:
+            raise RuntimeError("no headers: run encode_capture first")
+        raw, off, out = bytes(buf), 0, []
+        for n in sizes:
+            out.append(raw[off:off + n])
+            off += n
+        return out
+
     def close(self):
         if self.h and getattr(self, "dropin", False):
             self.L.vb200shim_detach()
@@ -176,6 +199,14 @@ class Ref:
         if self.L.ref_get_setup(self.h, C.byref(s)):
             raise RuntimeError("ref_get_setup failed")
         return abi.SetupHolder.from_struct(s)
+
+    def set_coupling(self, W, steps):
+        """replace the coupling map of mode W by steps = [(mag, ang), ...] (ref_set_coupling): setup(), the stage
+        calls, the batched chains and the headers of encode_capture then use it.  The map is not checked."""
+        mag = np.ascontiguousarray([m for m, _ in steps] or [0], np.int32)
+        ang = np.ascontiguousarray([a for _, a in steps] or [0], np.int32)
+        if self.L.ref_set_coupling(self.h, W, len(steps), mag, ang):
+            raise RuntimeError("ref_set_coupling refused W=%d with %d steps" % (W, len(steps)))
 
     def table(self, W, which):
         N = self.bs[W]

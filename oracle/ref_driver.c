@@ -123,6 +123,21 @@ int ref_get_packets(void *hv, unsigned char *buf, long cap, long *sizes, int max
   return i;
 }
 
+/* the three header packets ref_encode_capture wrote, back to back; returns 3, or -1 before the capture or when they do
+ * not fit in cap bytes */
+int ref_get_headers(void *hv, unsigned char *buf, long cap, long *sizes){
+  ref_handle *h = (ref_handle*)hv;
+  long off = 0; int i;
+  if(!h->hdrcopy[0]) return -1;
+  for(i = 0; i < 3; i++){
+    if(off + h->hdr[i].bytes > cap) return -1;
+    memcpy(buf + off, h->hdr[i].packet, h->hdr[i].bytes);
+    sizes[i] = h->hdr[i].bytes;
+    off += h->hdr[i].bytes;
+  }
+  return 3;
+}
+
 int ref_blocksize(void *hv, int W){
   ref_handle *h = (ref_handle*)hv;
   codec_setup_info *ci = (codec_setup_info*)h->vi.codec_setup;
@@ -240,6 +255,23 @@ int ref_get_setup(void *hv, vb200_setup *s){
       }
     }
   }
+  return 0;
+}
+
+/* rewrite the coupling map of the mapping mode W uses (vorbisenc writes one mapping per mode): every later call on the
+ * handle - the stage calls, the batched chains, ref_get_setup and the setup header ref_encode_capture writes - sees
+ * the new map.  The map is not checked: the caller passes one mapping0_unpack accepts.  Returns 0, or -1 when the
+ * two modes share a mapping or steps is out of range.                                                              */
+int ref_set_coupling(void *hv, int W, int steps, const int32_t *mag, const int32_t *ang){
+  ref_handle *h = (ref_handle*)hv;
+  codec_setup_info *ci = (codec_setup_info*)h->vi.codec_setup;
+  vorbis_info_mapping0 *m;
+  int k;
+  if(W < 0 || W > 1 || ci->modes < 2 || ci->mode_param[0]->mapping == ci->mode_param[1]->mapping) return -1;
+  m = (vorbis_info_mapping0*)ci->map_param[ci->mode_param[W]->mapping];
+  if(steps < 0 || steps > (int)(sizeof(m->coupling_mag)/sizeof(m->coupling_mag[0]))) return -1;
+  m->coupling_steps = steps;
+  for(k = 0; k < steps; k++){ m->coupling_mag[k] = mag[k]; m->coupling_ang[k] = ang[k]; }
   return 0;
 }
 

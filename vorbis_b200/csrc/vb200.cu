@@ -314,8 +314,7 @@ static int ctx_build(vb200_ctx *c, const vb200_setup *s, int device) {
   {
     int rc;
     if ((rc = upload(c->owned, VB_FLOOR1_FROMDB, (size_t)256, &c->d_fromdB))) return rc;
-    for (int w = 0; w < 2; w++) {
-      if (s->coupling_steps[w] < 0 || s->coupling_steps[w] > VB200_MAX_COUPLING) return fail(VB200_EINVAL, "coupling_steps");
+    for (int w = 0; w < 2; w++) {                      // the map was checked by vb200_ctx_create
       if ((rc = upload(c->owned, (const int *)s->coupling_mag[w], (size_t)s->coupling_steps[w], &c->d_mag[w]))) return rc;
       if ((rc = upload(c->owned, (const int *)s->coupling_ang[w], (size_t)s->coupling_steps[w], &c->d_ang[w]))) return rc;
     }
@@ -451,6 +450,15 @@ extern "C" int vb200_ctx_create(const vb200_setup *s, int device, vb200_ctx **ou
   if (s->blocksizes[0] > s->blocksizes[1]) return fail(VB200_EINVAL, "blocksizes[0] > blocksizes[1]");
   if (s->n_psy != 0 && s->n_psy != 4) return fail(VB200_EIMPL, "n_psy must be 0 or 4");
   if (s->channels < 1 || s->channels > VB200_MAX_CHANNELS) return fail(VB200_EINVAL, "channels");
+  // mapping0_unpack's checks (lib/mapping0.c:110-118): every kernel that couples or decouples indexes the block's
+  // channel rows with these, so a map the stock decoder refuses gets no context
+  for (int w = 0; w < 2; w++) {
+    if (s->coupling_steps[w] < 0 || s->coupling_steps[w] > VB200_MAX_COUPLING) return fail(VB200_EINVAL, "coupling_steps");
+    for (int k = 0; k < s->coupling_steps[w]; k++) {
+      const int m = s->coupling_mag[w][k], a = s->coupling_ang[w][k];
+      if (m < 0 || a < 0 || m == a || m >= s->channels || a >= s->channels) return fail(VB200_EINVAL, "coupling map");
+    }
+  }
   int ndev = 0;
   CU(cudaGetDeviceCount(&ndev));
   if (device < 0 || device >= ndev) return fail(VB200_EINVAL, "no such CUDA device");
